@@ -2,7 +2,7 @@
 
 There is no CPU fallback: if the shared library is missing or no CUDA device is
 visible, the first use raises.  `build()` compiles the library in-tree with nvcc
-(sm_100a); `load()` dlopens it and declares every prototype.
+(sm_90a); `load()` dlopens it and declares every prototype.
 """
 import ctypes as C
 import os
@@ -99,7 +99,7 @@ _lib = None
 
 
 def build(verbose=False):
-    """Compile libkge_b200.so in-tree for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile libkge_b200.so in-tree for sm_90a (nvcc cross-compiles without a GPU)."""
     cmd = ["make", "-C", CSRC, "-j8"]
     out = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if verbose or out.returncode != 0:

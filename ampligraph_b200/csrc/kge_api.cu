@@ -109,8 +109,8 @@ extern "C" int kge_create(const kge_config *cfg, kge_handle **out)
     if (guard_.err != cudaSuccess) return cuda_fail(guard_.err, "cudaSetDevice");
     cudaDeviceProp prop;
     KGE_CUDA(cudaGetDeviceProperties(&prop, cfg->device), "cudaGetDeviceProperties");
-    if (prop.major < 10)
-        return fail(KGE_ERR_UNSUPPORTED, "kge_create: device is sm_%d%d; libkge_b200 is built for sm_100a only",
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(KGE_ERR_UNSUPPORTED, "kge_create: device is sm_%d%d; libkge_b200 is built for sm_90a only",
                     prop.major, prop.minor);
 
     kge_handle *h = new (std::nothrow) kge_handle();
@@ -146,7 +146,7 @@ extern "C" int kge_create(const kge_config *cfg, kge_handle **out)
     // tuning aids (scripts/kbench.py): cap the warps per CTA, choose the buffering of non-resident slots
     if (const char *ev = getenv("KGE_B200_TRAIN_WARPS")) { const int w = atoi(ev); if (w >= 1 && w < max_warps) max_warps = w; }
     if (const char *ev = getenv("KGE_B200_TRAIN_NBUF")) nbuf = atoi(ev) == 1 ? 1 : 2;
-    // Residency policy, tuned on B200 (scripts/kbench.py sweep, profiles/): keep all eta corruptions resident
+    // Residency policy (scripts/kbench.py sweeps run before the H100 port; not re-run): keep all eta corruptions resident
     // (one gather per row) while >= KGE_MIN_RESIDENT_WARPS warps still fit; otherwise shrink G until
     // min(max_warps, KGE_TARGET_WARPS) warps fit -- the gradient pass then re-gathers the other groups, which
     // costs less than running with few warps.
@@ -441,10 +441,9 @@ static int train_step_impl(kge_handle *h, int32_t mode, const kge_shard_map *map
     // trilinear instantiations); default: the specialised kernel of kge_train_res.cu where it applies
     const char *force = getenv("KGE_B200_TRAIN_KERNEL");
     const bool fast = h->res_warps > 0 && p.shard_world <= 1 && p.stash == nullptr && !(force && strcmp(force, "general") == 0);
-    // Dynamic assignment of positives to warps (kge_train_common.cuh) where it was measured to pay: the resident fast path on
-    // tables that live in L2 with enough positives per warp for the imbalance to matter -- cfg2 145 -> 137 us.  On an
-    // HBM-resident table it LOSES (`big`, 3.2 GB: 668 -> 905 us, reproducibly; the general kernel on cfg4 / cfg5w: +-1 %),
-    // so those keep the static stride (profiles/r2o_kbench_{static,dynamic}.log).  KGE_B200_TRAIN_SCHED=static|dynamic forces.
+    // Dynamic assignment of positives to warps (kge_train_common.cuh) where it was measured to pay before the H100 port: the resident fast path on
+    // tables that live in L2 with enough positives per warp for the imbalance to matter (cfg2).  On an HBM-resident table it
+    // LOSES (and the general kernel on cfg4 / cfg5w gains nothing), so those keep the static stride.  KGE_B200_TRAIN_SCHED=static|dynamic forces.
     {
         const char *ev = getenv("KGE_B200_TRAIN_SCHED");
         const long long n_warps = (long long)h->sm_count * (fast ? h->res_warps : h->warps);
@@ -453,9 +452,8 @@ static int train_step_impl(kge_handle *h, int32_t mode, const kge_shard_map *map
         if (ev && strcmp(ev, "dynamic") == 0) dyn = true;
         p.sched = (dyn && B < (1ll << 24)) ? h->done_counter + 1 : nullptr;  // float counter: exact below 2^24
         // The hot-entity privatisation (kge_set_hot_entities) was a remedy for the same imbalance -- warps that drew many
-        // positives of a hot entity fell behind on its serialised atomics -- and with the dynamic assignment it only costs:
-        // bench.py's process 148.5 us with the hint, 138.3 us without (profiles/r2t_bench_probes*.log).  It stays in effect for
-        // the static stride (153.8 vs 168 us there, profiles/r2h_*).
+        // positives of a hot entity fell behind on its serialised atomics -- and with the dynamic assignment it only costs
+        // time in bench.py's workload.  It stays in effect for the static stride, where it pays.
         if (p.sched) p.hot_ent[0] = p.hot_ent[1] = -1;
     }
     if (h->rot_warps > 0 && p.shard_world <= 1 && p.stash == nullptr && !(force && strcmp(force, "general") == 0)) {
@@ -826,7 +824,7 @@ static int rank_impl(kge_handle *h, const kge_shard_map *map, int64_t filt_base,
     else
         KGE_CUDA(launch_rank_count(p, cnt, st), "kge_rank: count");
     if (filt_off_dev && n_filt > 0)
-        KGE_CUDA(launch_rank_filter_n(p, (const long long *)filt_off_dev, filt_idx_dev, n_filt, cnt, st), "kge_rank: filter");
+        KGE_CUDA(launch_rank_filter_n(p, (const long long *)filt_off_dev, filt_idx_dev, n_filt, cnt, h->sm_count, st), "kge_rank: filter");
     if (counts_dev) KGE_CUDA(launch_rank_accumulate(cnt, b, counts_dev, st), "kge_rank: accumulate");
     else if (ranks_dev) KGE_CUDA(launch_rank_finalize(cnt, b, strategy, ranks_dev, st), "kge_rank: finalize");
     return KGE_OK;

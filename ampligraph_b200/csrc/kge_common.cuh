@@ -1,12 +1,12 @@
-// kge_common.cuh -- shared device helpers for libkge_b200 (sm_100a only).
+// kge_common.cuh -- shared device helpers for libkge_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include "../../include/kge_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libkge_b200 targets sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900 || !defined(__CUDA_ARCH_FEAT_SM90_ALL))
+#error "libkge_b200 targets sm_90a (H100) only"
 #endif
 
 namespace kge {

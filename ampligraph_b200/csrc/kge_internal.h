@@ -4,12 +4,12 @@
 
 // per-lane register state grows with NIT (float4 chunks per lane): trade threads for registers
 // (RotatE carries 11 float4 vectors of per-positive state per chunk -- cos, sin, o, y = R s, four Z sums, d/dphi: give it more registers)
-// (RotatE with 12 warps at 168 registers was measured against 8 warps at 229: 273 us vs 267 us on cfg4, profiles/r2m_kbench_cfg4_sweep.log)
+// (RotatE with 12 warps at 168 registers was measured no faster than 8 warps at 229 on cfg4 before the H100 port)
 #define KGE_TRAIN_THREADS(model, nit) ((nit) <= 1 ? 512 : (nit) == 2 ? ((model) == KGE_ROTATE ? 256 : 384) : 256)
 #define KGE_MAX_PEERS 8
-#define KGE_MIN_RESIDENT_WARPS 8  // tuned on B200: fewer warps/SM than this costs more than re-gathering
+#define KGE_MIN_RESIDENT_WARPS 8  // fewer warps/SM than this costs more than re-gathering
 #define KGE_TARGET_WARPS 10
-#define KGE_MIN_RESIDENT_WARPS_WIDE 6  // the fast path on DistMult rows of 257..512 floats (NIT = 4): cfg3 113.6 us with 6 resident warps against 133 us for the grouped general kernel with 8 (profiles/r2l_*)
+#define KGE_MIN_RESIDENT_WARPS_WIDE 6  // the fast path on DistMult rows of 257..512 floats (NIT = 4): 6 resident warps beat the grouped general kernel with 8 on cfg3 (measured before the H100 port)
 
 namespace kge {
 
@@ -138,13 +138,13 @@ cudaError_t launch_rank_prepare(const Layout &L, const ShardView &sv, const floa
 // cnt = [b,3] int32 workspace: #(qpos < qc), #(qpos == qc), #filtered
 cudaError_t launch_rank_count(const RankParams &p, int32_t *cnt, cudaStream_t st);
 cudaError_t launch_rank_filter_n(const RankParams &p, const long long *filt_off, const int32_t *filt_idx,
-                                 long long n_pairs, int32_t *cnt, cudaStream_t st);
+                                 long long n_pairs, int32_t *cnt, int sm_count, cudaStream_t st);
 cudaError_t launch_rank_finalize(const int32_t *cnt, long long b, int strategy, int32_t *ranks, cudaStream_t st);
 cudaError_t launch_rank_accumulate(const int32_t *cnt, long long b, int32_t *counts, cudaStream_t st);  // counts += cnt
 
 // kge_rank_tc.cu: tensor-core filter + exact refine for the bilinear models
 struct RankTcLayout {  // carve-up of the tensor-core part of the caller's workspace
-    int nkb, ksteps, n_qb, n_ct;
+    int nkb, n_qb, n_ct;
     unsigned pair_cap;
     size_t off_a, off_b, off_thr, off_tnorm, off_count, off_pairs, bytes;
 };

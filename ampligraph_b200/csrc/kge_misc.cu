@@ -1,4 +1,4 @@
-// kge_misc.cu -- predict-path scoring, layout packing, Glorot initialisation (sm_100a).
+// kge_misc.cu -- predict-path scoring, layout packing, Glorot initialisation (sm_90a).
 #include <math.h>
 
 #include "kge_internal.h"

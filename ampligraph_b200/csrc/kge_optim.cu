@@ -1,4 +1,4 @@
-// kge_optim.cu -- optimizer update of the embedding tables (sm_100a).
+// kge_optim.cu -- optimizer update of the embedding tables (sm_90a).
 //
 // Replaces OptimizerWrapper.minimize -> tf.keras.optimizers.legacy.*.apply_gradients
 // (optimizers.py:136-168) and the regularisers attached to the tables
@@ -415,8 +415,8 @@ __global__ void __launch_bounds__(256) kge_optim_exchange_kernel(const ExchangeA
 // One instantiation of the exchange kernel, on a grid that is CO-RESIDENT: no CTA waits for another CTA of the grid, so a
 // second wave would be correct -- but it starts only when first-wave CTAs retire, i.e. after their system-scope fence, and
 // then runs its share of the exchange alone.  With the grid fixed at 4 CTAs per SM the 70-register variants (3 resident
-// CTAs per SM: world 2) ran a quarter of the shard in such a second wave: "wait for the last CTA" 25 us of a 66 us kernel
-// at N=2 (profiles/r2w_bench_n2.json), 5 us at N=8 where 4 CTAs fit.  The loops are grid-stride, so fewer CTAs only
+// CTAs per SM: world 2) ran a quarter of the shard in such a second wave, and waiting for the last CTA took a large part of
+// the kernel (measured before the H100 port).  The loops are grid-stride, so fewer CTAs only
 // means more trips per thread.
 template <int KIND, bool REG, int WORLD, bool MC>
 static cudaError_t launch_exchange_variant(const ExchangeArgs &a, const OptimParams &o, long long want, int sm_count,
@@ -459,7 +459,7 @@ cudaError_t launch_optimizer_exchange(const OptimParams &o, const ExchangeParams
     // no CTA ever waits for another CTA of this grid (phase 1 is per CTA, phase 3 is the last finisher alone), so the
     // grid need not be co-resident; a few CTAs per SM are enough to keep the NVLink loads in flight
     // grid: up to 4 CTAs per SM; the NVLS variant is software-pipelined, so it wants a few trips per thread rather than
-    // every load of the shard in flight at once (KGE_B200_EXCHANGE_TRIPS, default 1 = one trip; measured values in DESIGN.md)
+    // every load of the shard in flight at once (KGE_B200_EXCHANGE_TRIPS, default 1 = one trip)
     int trips = 1;
     if (const char *e = getenv("KGE_B200_EXCHANGE_TRIPS")) trips = atoi(e) > 0 ? atoi(e) : 1;
     const int U = xp.world <= 4 ? 4 : 2;

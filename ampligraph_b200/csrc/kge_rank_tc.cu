@@ -1,4 +1,4 @@
-// kge_rank_tc.cu -- tensor-core FILTER pass of the all-entity ranking for the bilinear models (sm_100a: tcgen05 + TMEM).
+// kge_rank_tc.cu -- tensor-core FILTER pass of the all-entity ranking for the bilinear models (sm_90a: wgmma).
 //
 // For DistMult / ComplEx / HolE the corruption scores of a batch of queries are a contraction
 // S[b, E] = Q[b, ld] . T[E, ld]^T (DistMult.py:51-99, ComplEx.py:65-151, HolE.py:47-89 compute it by broadcasting to
@@ -7,12 +7,11 @@
 // per (query, candidate) pair, on which side of the positive's quantisation bin the candidate's score falls:
 //
 //   1. split      every fp32 operand x into two bf16 numbers, x ~ hi + lo (|x - hi - lo| <= 2^-16 |x|), laid out in HBM
-//                 as ready-made UMMA operand tiles (8x8 "core matrices", K-major, no swizzle);
-//   2. filter     (this kernel) approximate scores a = Qhi.Thi + Qhi.Tlo + Qlo.Thi on the 5th-generation tensor cores:
-//                 tcgen05.mma kind::f16 (bf16 x bf16 -> fp32), accumulators in TMEM, operand tiles staged by the copy
-//                 engine (cp.async.bulk + mbarrier), one issuing thread, double-buffered accumulators so that the epilogue
-//                 of one tile overlaps the MMAs of the next.  The epilogue (tcgen05.ld) compares a with the two edges
-//                 U, L of the positive's bin: |a - s_canonical| <= delta is proven below, so a >= U + delta means
+//                 as ready-made wgmma operand tiles (8x8 "core matrices", K-major, no swizzle);
+//   2. filter     (this kernel) approximate scores a = Qhi.Thi + Qhi.Tlo + Qlo.Thi on the tensor cores: wgmma.mma_async
+//                 m64n256k16 (bf16 x bf16 -> fp32), accumulators in the registers of two consumer warpgroups, operand
+//                 tiles staged by the copy engine (cp.async.bulk + mbarrier ring, one producer thread).  The epilogue
+//                 compares a with the two edges U, L of the positive's bin: |a - s_canonical| <= delta is proven below, so a >= U + delta means
 //                 "greater", L + delta <= a <= U - delta means "equal", a <= L - delta means "smaller";
 //   3. refine     the few pairs inside a +-delta band around an edge are appended to a list and re-scored with the exact
 //                 canonical chain (kge_rank_refine_kernel) -- same arithmetic as the FP32 kernel, same counters.
@@ -37,8 +36,8 @@ namespace kge {
 // ---------------------------------------------------------------------------------------------------------------------
 // geometry
 // ---------------------------------------------------------------------------------------------------------------------
-constexpr int TC_MQ = 128;                         // queries per A tile    (UMMA M, one TMEM lane per query)
-constexpr int TC_NC = 256;                         // candidates per B tile (UMMA N, one TMEM column per candidate)
+constexpr int TC_MQ = 128;                         // queries per A tile    (two wgmma M = 64 halves, one per consumer warpgroup)
+constexpr int TC_NC = 256;                         // candidates per B tile (wgmma N)
 constexpr int TC_KB = 32;                          // columns per k-block (2 MMA k-steps of 16)
 constexpr int TC_KC = TC_KB / 8;                   // 8-column chunks (core-matrix columns) per k-block
 constexpr int TC_KSTEPS = TC_KB / 16;              // MMA k-steps per k-block
@@ -47,17 +46,16 @@ constexpr int TC_B_ELEMS = TC_NC * TC_KB;
 constexpr int TC_A_BYTES = 2 * TC_A_ELEMS * 2;     // hi + lo, contiguous in HBM and in shared memory: 16 KB
 constexpr int TC_B_BYTES = 2 * TC_B_ELEMS * 2;     // 32 KB
 constexpr int TC_STAGE_BYTES = TC_A_BYTES + TC_B_BYTES;  // 48 KB per pipeline stage
-constexpr int TC_STAGES = 4;                       // operand ring depth: the loop is bound by the latency of the bulk copies (a 96 KB
-                                                   // stage x 2 measured 15 us per 7-k-block tile against 4.9 us of MMAs), so more,
-                                                   // smaller stages in flight beat fewer, larger ones
-constexpr int TC_THREADS = 192;                    // warp 0 producer, warp 1 MMA issuer, warps 2..5 epilogue
-constexpr int TC_TMEM_COLS = 512;                  // two accumulator stages of 256 fp32 columns
+constexpr int TC_STAGES = 4;                       // operand ring depth: 192 KB of the 227 KB a block may use; the loop is bound by
+                                                   // the latency of the bulk copies, so several smaller stages in flight beat
+                                                   // fewer, larger ones
+constexpr int TC_THREADS = 384;                    // warpgroup 0 producer, warpgroups 1-2 wgmma + epilogue
 
 // ---------------------------------------------------------------------------------------------------------------------
 // 1. split: fp32 rows -> blocked bf16 hi/lo operand tiles.
 //    tile (rb, kb) of a matrix with RB rows per block: [hi: RB x TC_KB][lo: RB x TC_KB]; inside a part, element (r, c) lives
 //    at ((r/8 * TC_KC + c/8) * 8 + r%8) * 8 + c%8: 8x8 core matrices of 128 contiguous bytes, TC_KC of them (one k-block)
-//    per 8-row group -> the canonical K-major SWIZZLE_NONE layout with LBO = 128 B (next k-chunk), SBO = TC_KC*128 B
+//    per 8-row group -> the canonical K-major no-swizzle layout with LBO = 128 B (next k-chunk), SBO = TC_KC*128 B
 //    (next 8-row group), so a whole tile is ONE contiguous bulk copy and needs no tensor map.
 // ---------------------------------------------------------------------------------------------------------------------
 // One WARP per row: lanes stride over the row's 8-column chunks (coalesced 32-byte reads), write the hi / lo core-matrix
@@ -122,73 +120,73 @@ __global__ void __launch_bounds__(256) kge_rank_split_kernel(const float *__rest
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// PTX wrappers: tcgen05 (MMA, TMEM alloc / load / fences, commit)
+// PTX wrappers: wgmma (warpgroup MMA, operands from shared memory, accumulators in registers)
 // ---------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t *smem_dst, uint32_t ncols)
-{
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols)
-{
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem desc] . B[smem desc]^T, bf16 x bf16 -> fp32, issued by ONE thread for the CTA
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on an mbarrier when every MMA issued so far by this thread has completed (implies fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t *bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
 __device__ __forceinline__ void mbar_arrive(uint64_t *bar)
 {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-// 32 lanes x 32 consecutive fp32 columns of this warp's TMEM lane quarter
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32])
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait()
 {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// pins the accumulators after a wait: no use of them may move above it
+__device__ __forceinline__ void acc_fence(float (&d)[128])
+{
 #pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+    for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// D[64 x 256] (+)= A[64 x 16] . B[256 x 16]^T, bf16 x bf16 -> fp32, both operands K-major in shared memory; issued by the
+// whole warpgroup.  Thread t of the warpgroup holds d[i] = D[16*(t/32) + (t%32)/4 + 8*((i/2)%2)][8*(i/4) + 2*(t%4) + i%2].
+__device__ __forceinline__ void wgmma_m64n256k16_bf16(float (&d)[128], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate)
+{
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+        "%128, %129, p, 1, 1, 0, 0;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+          "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+          "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+          "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate));
 }
 
-// shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout, mma_sm100_desc.hpp): K-major, SWIZZLE_NONE,
-// leading byte offset (next 8-column chunk along K) 128 B, stride byte offset (next 8-row group) TC_KC*128 B, version 1 (sm_100)
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t smem_addr)
+// shared-memory matrix descriptor (sm_90 wgmma): K-major, no swizzle (layout type 0), leading byte offset (next 8-column
+// chunk along K) 128 B, stride byte offset (next 8-row group) TC_KC*128 B, base offset 0
+__device__ __forceinline__ uint64_t wgmma_smem_desc(uint32_t smem_addr)
 {
-    return (uint64_t)((smem_addr >> 4) & 0x3fffu) | ((uint64_t)(128u >> 4) << 16) | ((uint64_t)((TC_KC * 128u) >> 4) << 32) |
-           ((uint64_t)1 << 46);
+    return (uint64_t)((smem_addr >> 4) & 0x3fffu) | ((uint64_t)(128u >> 4) << 16) | ((uint64_t)((TC_KC * 128u) >> 4) << 32);
 }
-// instruction descriptor (cute::UMMA::InstrDescriptor): D fp32, A/B bf16, both K-major, N = 256, M = 128, dense
-constexpr uint32_t TC_IDESC = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TC_NC >> 3) << 17) | ((uint32_t)(TC_MQ >> 4) << 24);
 
 struct TcParams {
-    const __nv_bfloat16 *a_split;  // [n_qb][nkb][hi|lo][128 x 64] query tiles
-    const __nv_bfloat16 *b_split;  // [n_ct][nkb][hi|lo][256 x 64] candidate tiles
+    const __nv_bfloat16 *a_split;  // [n_qb][nkb][hi|lo][128 x 32] query tiles
+    const __nv_bfloat16 *b_split;  // [n_ct][nkb][hi|lo][256 x 32] candidate tiles
     const float4 *thr;             // [n_qb*128] {U, L, eps_rel*|q|, slack}
     const float *tile_norm;        // [n_ct] max |e| of the tile
     int32_t *cnt;                  // [b,3]
@@ -196,15 +194,17 @@ struct TcParams {
     unsigned *pair_count;
     unsigned pair_cap;
     long long b, n_cand;
-    int nkb, ksteps, n_qb, n_ct, ctas_per_qb;
+    int nkb, n_qb, n_ct, ctas_per_qb;
     float *probe_a, *probe_d;      // diagnostic outputs (PROBE instantiation only)
     float scale;
 };
 
 // ---------------------------------------------------------------------------------------------------------------------
 // 2. the filter kernel.  CTA (qb, j): query block qb, candidate tiles j, j + ctas_per_qb, ...; one CTA per SM.
-//    Per tile: nkb trips of a TC_STAGES-deep ring {cp.async.bulk A tile + B tile -> 3 MMAs per k-step}, then 128x256 accumulators are
-//    read back by four warps (one query per thread) while the next tile's MMAs fill the other accumulator stage.
+//    Warpgroup 0: one thread feeds a TC_STAGES-deep ring of {A tile + B tile} with bulk copies.  Warpgroups 1 and 2: query
+//    rows 0-63 / 64-127 of the A tile against all 256 candidates of the B tile, 3 wgmma per k-step into 128 fp32 registers
+//    per thread; one k-block stays in flight while the previous stage is released.  After the tile's last k-block each
+//    thread compares its 128 accumulators (2 queries x 64 candidates) with the bin edges of its two queries.
 // ---------------------------------------------------------------------------------------------------------------------
 template <bool PROBE>
 __global__ void __launch_bounds__(TC_THREADS, 1) kge_rank_tc_kernel(const TcParams p)
@@ -213,27 +213,19 @@ __global__ void __launch_bounds__(TC_THREADS, 1) kge_rank_tc_kernel(const TcPara
     unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~(uintptr_t)1023);
     uint64_t *full = reinterpret_cast<uint64_t *>(smem + TC_STAGES * TC_STAGE_BYTES);  // [TC_STAGES] operands landed
     uint64_t *empty = full + TC_STAGES;                                        // [TC_STAGES] operands consumed
-    uint64_t *tfull = empty + TC_STAGES;                                       // [2] accumulator stage complete
-    uint64_t *tempty = tfull + 2;                                              // [2] accumulator stage drained
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(tempty + 2);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
     const int qb = blockIdx.x % p.n_qb, first = blockIdx.x / p.n_qb;
     const int n_items = first < p.n_ct ? (p.n_ct - first + p.ctas_per_qb - 1) / p.ctas_per_qb : 0;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < TC_STAGES; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, 1); }
-        for (int s = 0; s < 2; ++s) { mbar_init(tfull + s, 1); mbar_init(tempty + s, 4); }
+        for (int s = 0; s < TC_STAGES; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, 8); }  // empty: every consumer warp
         fence_mbar_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, TC_TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
-        // ---------------- producer: one thread feeds the two-stage operand ring with bulk copies ----------------
-        if (lane == 0) {
+    if (wg == 0) {
+        // ---------------- producer: one thread feeds the operand ring with bulk copies ----------------
+        if (threadIdx.x == 0) {
             uint32_t it = 0;
             for (int i = 0; i < n_items; ++i) {
                 const int ct = first + i * p.ctas_per_qb;
@@ -247,88 +239,92 @@ __global__ void __launch_bounds__(TC_THREADS, 1) kge_rank_tc_kernel(const TcPara
                 }
             }
         }
-    } else if (warp == 1) {
-        // ---------------- MMA issuer: lane 0 issues every tcgen05.mma of the CTA ----------------
-        uint32_t it = 0;
-        for (int i = 0; i < n_items; ++i) {
-            const int acc = i & 1;
-            mbar_wait(tempty + acc, ((i >> 1) & 1u) ^ 1u);  // the epilogue has drained this accumulator stage
-            tc_fence_after();
-            const uint32_t d_tmem = tmem_base + (uint32_t)(acc * TC_NC);
-            for (int kb = 0; kb < p.nkb; ++kb, ++it) {
-                const int s = it % TC_STAGES;
-                mbar_wait(full + s, (it / TC_STAGES) & 1u);
-                tc_fence_after();
-                if (lane == 0) {
-                    const uint32_t a_hi = smem_u32(smem + (size_t)s * TC_STAGE_BYTES), a_lo = a_hi + TC_A_ELEMS * 2;
-                    const uint32_t b_hi = a_hi + TC_A_BYTES, b_lo = b_hi + TC_B_ELEMS * 2;
-                    const int ks_n = min(TC_KSTEPS, p.ksteps - kb * TC_KSTEPS);
-                    for (int ks = 0; ks < ks_n; ++ks) {
-                        const uint32_t o = (uint32_t)ks * 256u;  // two 128-byte k-chunks per k-step of 16
-                        const uint64_t da_hi = umma_smem_desc(a_hi + o), da_lo = umma_smem_desc(a_lo + o);
-                        const uint64_t db_hi = umma_smem_desc(b_hi + o), db_lo = umma_smem_desc(b_lo + o);
-                        umma_bf16(d_tmem, da_hi, db_hi, TC_IDESC, (kb | ks) != 0);
-                        umma_bf16(d_tmem, da_hi, db_lo, TC_IDESC, 1u);
-                        umma_bf16(d_tmem, da_lo, db_hi, TC_IDESC, 1u);
-                    }
-                    umma_commit(empty + s);                       // operands of this stage may be overwritten
-                    if (kb == p.nkb - 1) umma_commit(tfull + acc);  // accumulators of this tile are final
-                }
-                __syncwarp();
-            }
-        }
-    } else {
-        // ---------------- epilogue: thread = one query (TMEM lane), loop over the tile's 256 candidate columns ----------------
-        const int lg = warp & 3;  // a warp may only touch TMEM lanes [32*(warp%4), +32)
-        const int ql = lg * 32 + lane;
-        const long long q = (long long)qb * TC_MQ + ql;
-        const float4 thr = p.thr[q];
-        const float U = thr.x, L = thr.y;
-        int gt = 0, ge = 0;
-        for (int i = 0; i < n_items; ++i) {
-            const int acc = i & 1;
-            const int ct = first + i * p.ctas_per_qb;
-            const long long c0 = (long long)ct * TC_NC;
-            const int nvalid = (int)min((long long)TC_NC, p.n_cand - c0);
-            const float delta = __fmaf_ru(__fmul_ru(thr.z, p.tile_norm[ct]), 1.0001f, thr.w);
-            mbar_wait(tfull + acc, (i >> 1) & 1u);
-            tc_fence_after();
-            for (int ch = 0; ch < TC_NC / 32; ++ch) {
-                if (ch * 32 >= nvalid) break;  // warp-uniform
-                float v[32];
-                tmem_ld32(tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)(acc * TC_NC + ch * 32), v);
+        return;
+    }
+
+    // ---------------- consumers: warpgroup cw owns query rows [64*cw, 64*cw + 64) of the tile ----------------
+    const int cw = wg - 1;
+    const int r0 = 64 * cw + 16 * warp + (lane >> 2);  // this thread's two queries: r0 and r0 + 8
+    const long long q0 = (long long)qb * TC_MQ + r0, q1 = q0 + 8;
+    const float4 thr0 = p.thr[q0], thr1 = p.thr[q1];
+    const uint32_t a_row_off = (uint32_t)(64 * cw / 8) * (TC_KC * 128u);  // 8-row groups of the A tile before row 64*cw
+    int gt0 = 0, ge0 = 0, gt1 = 0, ge1 = 0;
+    uint32_t it = 0;
+    float d[128];
+    for (int i = 0; i < n_items; ++i) {
+        const int ct = first + i * p.ctas_per_qb;
+        int prev = -1;
+        for (int kb = 0; kb < p.nkb; ++kb, ++it) {
+            const int s = it % TC_STAGES;
+            mbar_wait(full + s, (it / TC_STAGES) & 1u);
+            const uint32_t a_hi = smem_u32(smem + (size_t)s * TC_STAGE_BYTES) + a_row_off, a_lo = a_hi + TC_A_ELEMS * 2;
+            const uint32_t b_hi = smem_u32(smem + (size_t)s * TC_STAGE_BYTES) + TC_A_BYTES, b_lo = b_hi + TC_B_ELEMS * 2;
+            wgmma_fence();
+            // always TC_KSTEPS k-steps: the split kernel zero-fills every k-block past ld, and a trip count known at compile
+            // time keeps the MMAs of one k-block in flight (a run-time bound makes ptxas serialise every wgmma)
 #pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const float a = v[j];
-                    const bool ok = ch * 32 + j < nvalid;
-                    if (PROBE) {
-                        if (ok && q < p.b) {
-                            p.probe_a[(size_t)q * p.n_cand + c0 + ch * 32 + j] = a * p.scale;
-                            p.probe_d[(size_t)q * p.n_cand + c0 + ch * 32 + j] = delta * p.scale;
-                        }
-                        continue;
-                    }
-                    const bool undecided = fminf(fabsf(a - U), fabsf(a - L)) < delta;
-                    gt += (ok && !undecided && a >= U) ? 1 : 0;
-                    ge += (ok && !undecided && a >= L) ? 1 : 0;
-                    if (ok && undecided) {
-                        const unsigned slot = atomicAdd(p.pair_count, 1u);
-                        if (slot < p.pair_cap) p.pairs[slot] = make_int2((int)q, (int)(c0 + ch * 32 + j));
-                    }
-                }
+            for (int ks = 0; ks < TC_KSTEPS; ++ks) {
+                const uint32_t o = (uint32_t)ks * 256u;  // two 128-byte k-chunks per k-step of 16
+                const uint64_t da_hi = wgmma_smem_desc(a_hi + o), da_lo = wgmma_smem_desc(a_lo + o);
+                const uint64_t db_hi = wgmma_smem_desc(b_hi + o), db_lo = wgmma_smem_desc(b_lo + o);
+                wgmma_m64n256k16_bf16(d, da_hi, db_hi, (kb | ks) != 0);
+                wgmma_m64n256k16_bf16(d, da_hi, db_lo, 1u);
+                wgmma_m64n256k16_bf16(d, da_lo, db_hi, 1u);
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tempty + acc);
+            wgmma_commit();
+            wgmma_wait<1>();  // the k-block before this one has completed: its stage may be overwritten
+            if (prev >= 0 && lane == 0) mbar_arrive(empty + prev);
+            prev = s;
         }
-        if (q < p.b) {
-            if (gt) atomicAdd(p.cnt + 3 * q + 0, gt);
-            if (ge - gt) atomicAdd(p.cnt + 3 * q + 1, ge - gt);
+        wgmma_wait<0>();
+        acc_fence(d);
+        if (lane == 0) mbar_arrive(empty + prev);
+
+        const long long c0 = (long long)ct * TC_NC;
+        const int nvalid = (int)min((long long)TC_NC, p.n_cand - c0);
+        const float tn = p.tile_norm[ct];
+        const float delta0 = __fmaf_ru(__fmul_ru(thr0.z, tn), 1.0001f, thr0.w);
+        const float delta1 = __fmaf_ru(__fmul_ru(thr1.z, tn), 1.0001f, thr1.w);
+#pragma unroll
+        for (int j = 0; j < 128; ++j) {
+            const bool second = (j >> 1) & 1;
+            const int col = 8 * (j >> 2) + 2 * (lane & 3) + (j & 1);
+            const float a = d[j];
+            const bool ok = col < nvalid;
+            const float U = second ? thr1.x : thr0.x, L = second ? thr1.y : thr0.y, delta = second ? delta1 : delta0;
+            const long long q = second ? q1 : q0;
+            if (PROBE) {
+                if (ok && q < p.b) {
+                    p.probe_a[(size_t)q * p.n_cand + c0 + col] = a * p.scale;
+                    p.probe_d[(size_t)q * p.n_cand + c0 + col] = delta * p.scale;
+                }
+                continue;
+            }
+            const bool undecided = fminf(fabsf(a - U), fabsf(a - L)) < delta;
+            const int g = (ok && !undecided && a >= U) ? 1 : 0, e = (ok && !undecided && a >= L) ? 1 : 0;
+            if (second) { gt1 += g; ge1 += e; } else { gt0 += g; ge0 += e; }
+            if (ok && undecided) {
+                const unsigned slot = atomicAdd(p.pair_count, 1u);
+                if (slot < p.pair_cap) p.pairs[slot] = make_int2((int)q, (int)(c0 + col));
+            }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, TC_TMEM_COLS);
+    // the four threads of a quad share their two queries
+#pragma unroll
+    for (int o = 1; o <= 2; o <<= 1) {
+        gt0 += __shfl_xor_sync(0xffffffffu, gt0, o); ge0 += __shfl_xor_sync(0xffffffffu, ge0, o);
+        gt1 += __shfl_xor_sync(0xffffffffu, gt1, o); ge1 += __shfl_xor_sync(0xffffffffu, ge1, o);
+    }
+    if ((lane & 3) == 0) {
+        if (q0 < p.b) {
+            if (gt0) atomicAdd(p.cnt + 3 * q0 + 0, gt0);
+            if (ge0 - gt0) atomicAdd(p.cnt + 3 * q0 + 1, ge0 - gt0);
+        }
+        if (q1 < p.b) {
+            if (gt1) atomicAdd(p.cnt + 3 * q1 + 0, gt1);
+            if (ge1 - gt1) atomicAdd(p.cnt + 3 * q1 + 1, ge1 - gt1);
+        }
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -380,7 +376,6 @@ RankTcLayout rank_tc_layout(const Layout &L, long long b, long long n_cand, int 
 {
     RankTcLayout w;
     w.nkb = (L.ld + TC_KB - 1) / TC_KB;
-    w.ksteps = (L.ld + 15) / 16;
     w.n_qb = (int)((b + TC_MQ - 1) / TC_MQ);
     w.n_ct = (int)((n_cand + TC_NC - 1) / TC_NC);
     long long cap = b * n_cand / 16;
@@ -427,13 +422,13 @@ cudaError_t launch_rank_count_tc(const RankParams &p, const RankTcLayout &w, voi
     TcParams t;
     t.a_split = a_split; t.b_split = b_split; t.thr = thr; t.tile_norm = tnorm; t.cnt = cnt;
     t.pairs = pairs; t.pair_count = count; t.pair_cap = w.pair_cap;
-    t.b = p.b; t.n_cand = p.n_cand; t.nkb = w.nkb; t.ksteps = w.ksteps; t.n_qb = w.n_qb; t.n_ct = w.n_ct;
+    t.b = p.b; t.n_cand = p.n_cand; t.nkb = w.nkb; t.n_qb = w.n_qb; t.n_ct = w.n_ct;
     int per = sm_count / w.n_qb;
     if (per < 1) per = 1;
     if (per > w.n_ct) per = w.n_ct;
     t.ctas_per_qb = per;
     t.probe_a = probe_a; t.probe_d = probe_d; t.scale = p.scale;
-    const size_t smem = (size_t)TC_STAGES * TC_STAGE_BYTES + 1024 /*alignment*/ + 128 /*barriers + TMEM slot*/;
+    const size_t smem = (size_t)TC_STAGES * TC_STAGE_BYTES + 1024 /*alignment*/ + 128 /*barriers*/;
     if (probe_a) {
         if ((e = cudaFuncSetAttribute(kge_rank_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return e;
         kge_rank_tc_kernel<true><<<(unsigned)(w.n_qb * per), TC_THREADS, smem, st>>>(t);

@@ -1,4 +1,4 @@
-// kge_train.cu -- fused forward+backward of one training batch (sm_100a).
+// kge_train.cu -- fused forward+backward of one training batch (sm_90a).
 //
 // Replaces, in ONE kernel: EmbeddingLookupLayer.call (layers/encoding/
 // EmbeddingLookupLayer.py:307-342) for positives and corruptions,
@@ -14,10 +14,9 @@
 // row, completion on a per-warp mbarrier); scores, loss and dL/dscore are
 // computed from shared memory, which stays read-only after the gather; gradient
 // float4s go straight from registers to the gradient tables with
-// red.global.add.v4.f32.  (Round 1 also carried a copy-engine scatter --
-// cp.reduce.async.bulk of whole rows staged in shared memory -- and a
-// two-warps-per-positive variant; both measured slower on B200, 195 vs 165 us and
-// +10 % on cfg2, profiles/r1a_*, and were removed.)  The reference re-gathers
+// red.global.add.v4.f32.  (A copy-engine scatter -- cp.reduce.async.bulk of whole
+// rows staged in shared memory -- and a two-warps-per-positive variant were both
+// measured slower on cfg2 before the H100 port and removed.)  The reference re-gathers
 // s,p,o for every corruption (3(1+eta) rows per positive); here each needed row
 // moves once: (3+eta) rows in, (3+eta) gradient rows out = 2(3+eta)*ld*4 bytes
 // per positive.
@@ -343,10 +342,9 @@ struct Scorer<KGE_TRANSE, NIT> {
 //   df/do = (a,b); df/ds = -R(-phi)(a,b); df/dphi = a*y_im - b*y_re, y = R(phi) s.
 // The reference's gradient is NaN at an exactly-zero residual; here it is 0.
 //
-// The kernel is FP32-issue bound on this model (profiles/r2a_train_cfg4_ncu_full_summary.json), so the
-// scorer is written to a per-element instruction budget: every float4 operation is two packed f32x2
-// instructions (negations and subtractions are operand modifiers of FADD2 / FFMA2, never separate
-// instructions), a residual is two dependent packed fmas per component, the modulus is one MUFU.SQRT, the unit vector one MUFU.RSQ
+// The kernel is FP32-issue bound on this model, so the scorer is written to a per-element instruction budget:
+// every float4 operation is four fp32 instructions (negations and subtractions are operand modifiers of FADD /
+// FFMA, never separate instructions), a residual is two dependent fmas per component, the modulus is one MUFU.SQRT, the unit vector one MUFU.RSQ
 // on max(x, tiny) (an exactly-zero residual gives 0 * finite = 0), and lanes past the end of the window are
 // masked arithmetically (they read the window's last chunk; only their stores are predicated) so the row
 // loops carry no divergence bookkeeping.
@@ -561,8 +559,7 @@ __global__ void __launch_bounds__(KGE_TRAIN_THREADS(MODEL, NIT)) kge_train_kerne
     const int lw = p.slot_floats;              // slot stride (>= HALVES*wk)
     const int n_cb = RESIDENT ? 1 : p.n_cb;    // column windows per row
     const int n_groups = RESIDENT ? 1 : (eta + G - 1) / G;
-    // (making these loop invariants opaque to the front end, as kge_train_res.cu does, changes nothing here:
-    // cfg3 131 -> 133 us, cfg4 / cfg5w unchanged, profiles/r2f_kbench_general_keep.log)
+    // (making these loop invariants opaque to the front end, as kge_train_res.cu does, was measured to change nothing here before the H100 port)
     constexpr bool resident = RESIDENT;
     // slot: s, p, o windows, then group buffer 0 and (non-resident, p.nbuf == 2) group buffer 1: the next group is
     // gathered while the current one is being processed, which hides the gather latency inside the warp (NVLink

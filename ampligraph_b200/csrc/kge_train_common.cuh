@@ -1,5 +1,5 @@
 // kge_train_common.cuh -- device helpers shared by the training kernels (kge_train.cu: the general kernel;
-// kge_train_res.cu: the resident trilinear fast path): packed-fp32 float4 arithmetic, the gradient sink, warp
+// kge_train_res.cu: the resident trilinear fast path): fp32-pair float4 arithmetic, the gradient sink, warp
 // reductions, and the per-positive loss + dL/dscore of the five reference losses.
 #pragma once
 #include <math.h>
@@ -14,8 +14,8 @@ namespace kge {
 __device__ __forceinline__ float4 f4zero() { return make_float4(0.f, 0.f, 0.f, 0.f); }
 __device__ __forceinline__ float4 f4ld(const float *p) { return *reinterpret_cast<const float4 *>(p); }
 __device__ __forceinline__ void f4st(float *p, float4 v) { *reinterpret_cast<float4 *>(p) = v; }
-// Blackwell packed fp32: fma/mul/add.rn.f32x2 (SASS FFMA2/FMUL2/FADD2) do two IEEE fp32 operations per
-// issue slot on a 64-bit register pair.  The kernel is issue-bound, so every float4 op is two f32x2 ops.
+// fp32 pairs: two values in a 64-bit register pair.  Hopper has no packed fp32 instruction, so a pair operation is two
+// IEEE fp32 operations (FFMA / FMUL / FADD, round to nearest), one per half; pk2 / upk2 are register renames.
 typedef unsigned long long f32x2_t;
 __device__ __forceinline__ f32x2_t pk2(float lo, float hi)
 {
@@ -26,21 +26,21 @@ __device__ __forceinline__ f32x2_t pk2(float lo, float hi)
 __device__ __forceinline__ void upk2(f32x2_t v, float &lo, float &hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
 __device__ __forceinline__ f32x2_t fma2(f32x2_t a, f32x2_t b, f32x2_t c)
 {
-    f32x2_t d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-    return d;
+    float a0, a1, b0, b1, c0, c1;
+    upk2(a, a0, a1); upk2(b, b0, b1); upk2(c, c0, c1);
+    return pk2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 __device__ __forceinline__ f32x2_t mul2(f32x2_t a, f32x2_t b)
 {
-    f32x2_t d;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
+    float a0, a1, b0, b1;
+    upk2(a, a0, a1); upk2(b, b0, b1);
+    return pk2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 __device__ __forceinline__ f32x2_t add2(f32x2_t a, f32x2_t b)
 {
-    f32x2_t d;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
+    float a0, a1, b0, b1;
+    upk2(a, a0, a1); upk2(b, b0, b1);
+    return pk2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 __device__ __forceinline__ float4 f4from(f32x2_t lo, f32x2_t hi)
 {
@@ -87,7 +87,8 @@ __device__ __forceinline__ void red_add_v4(float *g, float4 v)
                  : "memory");
 }
 // -DKGE_PROFILE_NOSCATTER builds a profiling variant that drops the gradient scatter (how much of the kernel the atomics
-// cost).  The product never tests a run-time flag here: a branch around every RED cost 3.5 % (cfg2) to 11 % (cfg3).
+// cost).  The product never tests a run-time flag here: a branch around every RED was measured to cost several percent
+// before the H100 port (not re-measured).
 struct SinkRed {
     static __device__ __forceinline__ void put(float *, float *grow, int, int goff, float4 v) { red_add_v4(grow + goff, v); }
 };
@@ -223,7 +224,7 @@ __device__ __forceinline__ void red4(char *row, uint32_t byte_off, float4 v) { r
 // (a FLOAT counter on purpose: the compiler -- nvcc for atomicAdd(), ptxas for atom.add / atom.inc in inline PTX, u32 and u64,
 // even with a laundered addend -- aggregates a warp's integer atomic adds (VOTE + POPC, one ATOMG) and reads the result back
 // with a shuffle right after it, which puts the whole L2 round trip, microseconds when HBM is saturated, at the top of every
-// positive: measured +35 % on the HBM-resident `big` shape, profiles/r2n_kbench_dynamic.log.  atom.add.f32 is left alone;
+// positive: measured markedly slower on an HBM-resident table before the H100 port.  atom.add.f32 is left alone;
 // counts are exact below 2^24, the host falls back to the static stride for larger batches.)
 #define KGE_SCHED_MAX_B (1ll << 24)
 __device__ __forceinline__ float sched_draw(unsigned *sched)  // the caller converts when it consumes the value, not here

@@ -1,22 +1,21 @@
-// kge_train_res.cu -- the RESIDENT TRILINEAR fast path of the fused training step (sm_100a).
+// kge_train_res.cu -- the RESIDENT TRILINEAR fast path of the fused training step (sm_90a).
 //
 // Same contract as kge_train_kernel (kge_train.cu; reference: train_step ScoringBasedEmbeddingModel.py:370-429 ->
 // EmbeddingLookupLayer.call, CorruptionGenerationLayerTrain.call, DistMult/ComplEx/HolE _compute_scores, the five
 // losses, tape.gradient), specialised for the shape the headline workload has: DistMult / ComplEx / HolE, every row of
 // a positive resident in the warp's shared-memory slot (one column window, one group), eta <= 32 (one corruption per
-// lane), a single (not row-sharded) table.  What the specialisation buys (ncu source page of the general kernel,
-// profiles/r2b_train_cfg2_general_kernel_source_hot.txt: 2,344 instructions per positive, 135 per pair of the gradient loop of which
-// 56 are loads / FMAs / REDs): all shared-memory traffic goes through explicit 32-bit shared addresses (one IADD per
+// lane), a single (not row-sharded) table.  What the specialisation buys (in the general kernel fewer than half the
+// instructions of the gradient loop are loads / FMAs / REDs): all shared-memory traffic goes through explicit 32-bit shared addresses (one IADD per
 // 128-bit load instead of 64-bit generic pointer arithmetic re-derived every trip), gradient rows are addressed as
 // one 64-bit base per row plus the lane's byte offset, the shard/window/group machinery does not exist, and the
-// corruption sort is one ballot pair.  Arithmetic per element is identical to the general kernel's (same f32x2 FMAs in
+// corruption sort is one ballot pair.  Arithmetic per element is identical to the general kernel's (same fp32 FMAs in
 // the same order), so both produce the same scores; gradients differ only in the order of the fp32 atomics.
 #include "kge_train_common.cuh"
 
 namespace kge {
 
 #ifndef KGE_HOT
-#define KGE_HOT 1  // entities whose subject/object gradient rows are privatised per warp (1 or 2; measured on B200: 1 -> 150.8 us, 2 -> 153.2 us in bench.py, and 2 costs the uniform case 3 us: profiles/r2i_kbench_hot*.log)
+#define KGE_HOT 1  // entities whose subject/object gradient rows are privatised per warp (1 or 2; 2 measured no faster on cfg2 and slower on uniform triples before the H100 port)
 #endif
 
 // ---- the kernel ----------------------------------------------------------------------------------------------------------
@@ -27,11 +26,11 @@ namespace kge {
 //   [ s | o | eta replaced rows ] [ sc: eta_pad floats ] [ nid ] [ jorig ] [ mbarrier ]
 // The relation row is NOT staged: each lane loads its chunks of p straight into registers (ld.global.nc, issued before
 // the wait for the gather, so the latency hides behind it) and keeps them until the gradient rows of s, p, o are formed.
-// One row less per positive is what lets a 12th warp fit beside cfg2's 11 (12 x (12 x 1600 + 160) B = 226.9 KB).
+// One row less per positive is what lets a 12th warp fit beside cfg2's 11 (12 x (12 x 1600 + 160) B = 226.9 KB of the 227 KB a
+// block may use).
 // Gradient rows leave the SM as red.global.add.v4.f32 straight from registers.  Sending part of them down the copy
 // engine's road instead (g*Q staged over the gathered row with st.shared.v4, one cp.reduce.async.bulk per row) was
-// measured on B200 and is slower: cfg2 152 us -> 170 us with every second replaced row, 178 us with all of them
-// (profiles/r2d_kbench_scatter_split*.log); without any scatter the kernel takes 123 us (r2d_kbench_noscatter_fast.log).
+// measured slower on cfg2 before the H100 port, for every second replaced row and for all of them.
 template <int HALVES, int NIT, int THREADS>
 __global__ void __launch_bounds__(THREADS) kge_train_res_kernel(const TrainParams p)
 {
@@ -82,9 +81,8 @@ __global__ void __launch_bounds__(THREADS) kge_train_res_kernel(const TrainParam
     double loss_acc = 0.0;
     // Hot-entity privatisation.  On a skewed graph a few entities own a large share of all subject / object slots (Zipf(1)
     // over 14.5 k entities: the first holds 10 %, the first two 15 %), and every one of those positives adds 100 float4 to
-    // the SAME gradient row: ~42,000 atomics per 128-byte line per step, which the L2 serialises per address -- measured
-    // 170 us against 145 us for the same kernel on uniformly drawn triples, depending on which L2 slices the hot lines
-    // share (profiles/r2g_bench_probes.log).  The caller names up to KGE_HOT entities (kge_set_hot_entities; the facade
+    // the SAME gradient row: ~42,000 atomics per 128-byte line per step, which the L2 serialises per address -- measurably
+    // slower than the same kernel on uniformly drawn triples (measured before the H100 port).  The caller names up to KGE_HOT entities (kge_set_hot_entities; the facade
     // takes the most frequent ones of the training set); each warp sums their subject / object gradient rows in registers
     // over all the positives it processes and issues ONE set of REDs per hot row when it retires.
     int hot0 = p.hot_ent[0], hot1 = KGE_HOT > 1 ? p.hot_ent[1] : -1;
@@ -94,9 +92,8 @@ __global__ void __launch_bounds__(THREADS) kge_train_res_kernel(const TrainParam
     for (int it = 0; it < NIT; ++it) H0r[it] = H0i[it] = H1r[it] = H1i[it] = f4zero();
 
     const long long n_warps = (long long)gridDim.x * (blockDim.x >> 5);
-    // (measured and rejected: two or three positives per draw -- no gain / slower, profiles/r2p_kbench_chunk{2,3}.log; requesting the
-    // next positive's triple after the score pass, so that the top of a positive waits for nothing -- cfg2 unchanged, cfg3 +3 %,
-    // profiles/r2v_kbench_*triple_prefetch.log)
+    // (measured and rejected before the H100 port: two or three positives per draw -- no gain / slower; requesting the next positive's triple after
+    // the score pass, so that the top of a positive waits for nothing -- no gain on cfg2, slower on cfg3)
     float next_draw = 0.f;  // lane 0: this warp's draw from the positive counter (kge_train_common.cuh: dynamic assignment)
     for (long long i = (long long)blockIdx.x * (blockDim.x >> 5) + warp; i < p.B;
          i = p.sched ? n_warps + (long long)(unsigned)__shfl_sync(0xffffffffu, next_draw, 0) : i + n_warps) {

@@ -1,11 +1,11 @@
-// kge_train_rot.cu -- the RotatE fast path of the fused training step (sm_100a).
+// kge_train_rot.cu -- the RotatE fast path of the fused training step (sm_90a).
 //
 // Same contract as kge_train_kernel<KGE_ROTATE> (kge_train.cu; reference: train_step ScoringBasedEmbeddingModel.py:370-429 ->
 // EmbeddingLookupLayer.call, CorruptionGenerationLayerTrain.call, RotatE._compute_scores RotatE.py:62-104, the five losses,
 // tape.gradient), specialised the way kge_train_res.cu specialises the trilinear models, for the shape cfg4 has: one column
 // window (k <= 256), a single (not row-sharded) table, any eta.  After the scorer had been put on an instruction budget the
-// general kernel was latency-bound at 2 warps per scheduler with a third of every inner loop spent on addressing
-// (profiles/r2n_train_cfg4_ncu_full_summary.json, DESIGN.md 3.1); what this kernel does differently:
+// general kernel was (profiled before the H100 port) latency-bound at 2 warps per scheduler with a third of every inner loop spent on addressing
+// (DESIGN.md 3.1); what this kernel does differently:
 //   * s, o and the rotation row of the positive go STRAIGHT TO REGISTERS (ld.global.nc, coalesced 16 B per lane): everything
 //     the two passes need of them is y = R(phi) s, o, cos, sin, which live in registers anyway.  The shared-memory slot then
 //     holds only replaced rows, so the same 28 KB per warp take groups of 8 corruptions instead of 7 (cfg4: 4 groups
@@ -14,7 +14,7 @@
 //     into the buffer that has just been consumed (the general kernel re-gathers all but the last);
 //   * explicit 32-bit shared addresses, loop invariants kept in registers (KGE_KEEP*), one 64-bit gradient base per replaced
 //     row with the second chunk and the imaginary half as immediate / register offsets of the RED.
-// Arithmetic per element is the general kernel's (same packed f32x2 operations in the same order), so both produce the same
+// Arithmetic per element is the general kernel's (same fp32 operations in the same order), so both produce the same
 // scores bit for bit; gradients differ only in the order of the fp32 atomics
 // (tests/test_gpu_parity.py::test_resident_fast_path_equals_general_kernel).
 #include "kge_train_common.cuh"
@@ -125,8 +125,8 @@ __global__ void __launch_bounds__(256) kge_train_rot_kernel(const TrainParams p)
         if (lane < 3) tv = __ldg(p.triples + 3 * i + lane);
         const int s_id = __shfl_sync(0xffffffffu, tv, 0), p_id = __shfl_sync(0xffffffffu, tv, 1), o_id = __shfl_sync(0xffffffffu, tv, 2);
         // this lane's chunks of s, the rotation row [cos | sin] and o, straight to registers -- requested FIRST, so that their
-        // latency hides behind the corruption draws below (ncu: long-scoreboard was the top stall with the loads placed
-        // where they are consumed, profiles/r2t_train_cfg4_ncu_full_summary.json)
+        // latency hides behind the corruption draws below (long-scoreboard was the top stall with the loads placed
+        // where they are consumed, profiled before the H100 port)
         float4 sr[NIT], si[NIT], C[NIT], Sn[NIT], Or_[NIT], Oi[NIT];
         {
             const char *srow = reinterpret_cast<const char *>(p.ent + (size_t)s_id * ld);

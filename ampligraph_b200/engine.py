@@ -51,7 +51,7 @@ class KGEEngine:
         models) | 'exact' (FP32 canonical chain for every pair); env KGE_B200_RANK_MODE overrides the default."""
         self.lib = _lib.load()
         if not torch.cuda.is_available():
-            raise RuntimeError("ampligraph_b200 needs a CUDA device (B200, sm_100a); there is no CPU path")
+            raise RuntimeError("ampligraph_b200 needs a CUDA device (H100, sm_90a); there is no CPU path")
         if scoring_type not in _lib.SCORING:
             raise ValueError("Unknown scoring_type: %r" % (scoring_type,))
         if loss not in _lib.LOSSES:

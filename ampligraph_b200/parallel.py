@@ -53,7 +53,7 @@ def tables_close(got, ref, init, rtol=3e-4, atol_of_update=2e-3, outlier_of_upda
     the parameter, so the absolute tolerance is stated relative to how far the parameters MOVED (u = max|ref - init|):
       * all but a fraction `outlier_fraction` of the elements: |got - ref| <= atol_of_update*u + rtol*|ref|;
       * EVERY element: |got - ref| <= outlier_of_update*u + rtol*|ref| -- an element whose summed gradient cancels to ~0 has
-        its Adam direction decided by rounding noise (measured: up to 6e-3 u on cfg4 over 8 shards, loss equal to 1e-11),
+        its Adam direction decided by rounding noise (measured before the H100 port: up to 6e-3 u on cfg4 over 8 shards, loss equal to 1e-11),
         whereas a lost or doubled contribution moves a whole row by O(1) u and fails this bound.
     Returns (ok, max_abs_err / u)."""
     import numpy as np
@@ -103,8 +103,8 @@ class DataParallelTrainer:
                 self.eng = make_engine(self._symmetric_alloc)
                 reject_lazy("lazy_" if self.eng.lazy else "", self.world)
                 self._finish_p2p_setup()
-                # NVLS moves 2/N of a block per rank per step through the links instead of 2(N-1)/N: it wins from 4 GPUs up
-                # (measured, profiles/); at N = 2 the switch round trip of the local contribution makes it slower than p2p
+                # NVLS moves 2/N of a block per rank per step through the links instead of 2(N-1)/N: it wins from 4 GPUs up;
+                # at N = 2 the switch round trip of the local contribution makes it slower than p2p
                 want_nvls = mode == "nvls" or (mode == "auto" and self.world >= int(os.environ.get("KGE_B200_NVLS_MIN_WORLD", "4")))
                 mc = int(getattr(self.hdl, "multicast_ptr", 0) or 0) if want_nvls else 0
                 if mode == "nvls" and not mc:

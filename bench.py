@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- training throughput of the fused KGE step on B200 (driver contract).
+"""bench.py -- training throughput of the fused KGE step on H100.
 
     python bench.py --gpus 1 --steps 20 --warmup 5
+    python bench.py --gpus 1 --steps 20 --warmup 5 --dump-outputs DIR   # + the last timed step's results as DIR/*.npy
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
     python bench.py --impl reference ...      # the reference-semantics CPU path (oracle)
 
@@ -15,7 +16,7 @@ own batch; the whole tail of the step (cross-rank barrier, gradient reduce-scatt
 parameter all-gather, barrier) is ONE kernel over NVLink peer memory (parallel.DataParallelTrainer),
 with the NCCL all-reduce + full optimizer as fallback (KGE_B200_DP_MODE=nccl).
 
-Outside the headline timed region the same JSON line carries an `extra` block (VERDICT r1 #1): the other
+Outside the headline timed region the same JSON line carries an `extra` block: the other
 BASELINE configs measured at their stated sizes (cfg3, cfg4, cfg5; row-sharded when N>1), full-entity ranking,
 and -- at every N>1 -- self-checks that the data-parallel / row-sharded step equals the single-GPU step on the
 concatenated batch (`dp_parity`, `sharded_parity`).
@@ -85,13 +86,13 @@ def measured_hbm_peak():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "MEASURED_PEAKS.json"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "fallback: H100 SXM data-sheet HBM3 bandwidth (not measured)"
 
 
 class ClockSampler:
     """SM clock + throttle reasons sampled DURING the timed region.  NVML is polled from a thread
-    every ~2 ms (the nvidia-smi -lms loop of B200_PROFILING.md cannot deliver a sample inside a
-    timed region that lasts a few tens of milliseconds)."""
+    every ~2 ms (an nvidia-smi polling loop cannot deliver a sample inside a timed region that
+    lasts a few tens of milliseconds)."""
 
     def __init__(self, index):
         self.index, self.samples, self._stop, self.th, self.err = index, [], False, None, None
@@ -186,8 +187,8 @@ def run_cpu_reference(steps, warmup, batch, threads=None, budget_s=None):
 
     t_full = None
     if threads is None:
-        # "all the host threads it can use": torch-CPU oversubscribes on many-core hosts (128 threads were 4x
-        # slower than 8 on the first B200 box), so time one step per candidate count and keep the fastest
+        # "all the host threads it can use": torch-CPU oversubscribes on many-core hosts (128 threads can be several
+        # times slower than 8), so time one step per candidate count and keep the fastest
         best = None
         for th in sorted({os.cpu_count(), 64, 32, 16, 8} & set(range(1, os.cpu_count() + 1)), reverse=True):
             torch.set_num_threads(th)
@@ -501,6 +502,16 @@ def guarded(extra, key, fn):
         extra[key] = {"error": repr(e), "trace": traceback.format_exc()[-600:]}
 
 
+def dump_outputs(out_dir, eng, last_loss):
+    """What a caller of the timed train_step holds after its last step: both embedding tables (fp32, 23 MB for cfg2)
+    and that step's [batch loss, regulariser loss] (fp64)."""
+    os.makedirs(out_dir, exist_ok=True)
+    ent, rel = (x.cpu().numpy() for x in eng.get_embeddings())
+    np.save(os.path.join(out_dir, "ent_embeddings.npy"), np.ascontiguousarray(ent, dtype=np.float32))
+    np.save(os.path.join(out_dir, "rel_embeddings.npy"), np.ascontiguousarray(rel, dtype=np.float32))
+    np.save(os.path.join(out_dir, "last_step_loss.npy"), last_loss.cpu().numpy().astype(np.float64))
+
+
 # ---------------------------------------------------------------------------
 def main_ours(args):
     import torch
@@ -571,7 +582,11 @@ def main_ours(args):
     g0.record()
     for i in range(args.steps):
         if os.environ.get("KGE_BENCH_NOFLUSH") != "1":  # (diagnostic switch; the reported numbers always flush)
-            flush.fill_(i & 0xff)  # evict L2 (126 MB) outside the timed events
+            flush.fill_(i & 0xff)  # evict L2 (50 MB on H100) outside the timed events
+        if args.dump_outputs and i == args.steps - 1:
+            # 16-byte snapshot so the last step's own loss can be dumped: outside the step's events (`value` is untouched),
+            # inside the g0..g1 device timeline, which it lengthens by one tiny copy only when dumping
+            loss_before_last = eng.loss_acc.clone()
         step(args.warmup + i, evs[i])
     g1.record()
     cpu_enqueue_ms = 1e3 * (time.perf_counter() - c0) / args.steps  # host time to enqueue one step (flush included)
@@ -579,6 +594,8 @@ def main_ours(args):
     gpu_timeline_ms = g0.elapsed_time(g1) / args.steps                # device time per step, flush included
     launches = eng.launches - launches0
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:  # tables are replicated: rank 0's copy is every rank's
+        dump_outputs(args.dump_outputs, eng, eng.loss_acc - loss_before_last)
     if os.environ.get("KGE_BENCH_DEBUG") == "1" and rank == 0:
         print("per-step kernel us:", [round(1e3 * e[0].elapsed_time(e[1]), 1) for e in evs], file=sys.stderr)
         print("per-step tail us:", [round(1e3 * e[1].elapsed_time(e[2]), 1) for e in evs], file=sys.stderr)
@@ -728,12 +745,6 @@ def main_ours(args):
         row_bytes = eng.ld * 4
         alg_bytes = 2 * (3 + eta) * row_bytes * B  # SURVEY 8(d): (3+eta) rows in + (3+eta) gradient rows out
         achieved = alg_bytes / (t_kern / 1e3) / 1e9
-        traffic = None
-        try:
-            with open(os.path.join(ROOT, "profiles", "train_kernel_traffic.json")) as f:
-                traffic = json.load(f).get("dram_bytes_per_launch")
-        except Exception:
-            pass
         cpu_steps = 3
         cpu = run_cpu_reference(cpu_steps, 1, B) if world == 1 and not args.no_cpu else None
         line = {"metric": METRIC, "value": value, "unit": "triples/s", "n_gpus": world, "steps": args.steps,
@@ -753,7 +764,7 @@ def main_ours(args):
                                "per-step loss read one step late)", "last_loss": e2e_losses[-1] if e2e_losses else None},
                 "gpu_launches": launches,
                 "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                             "traffic": traffic, "kernel": CFG["kernel"],
+                             "kernel": CFG["kernel"],
                              "kernel_ms": t_kern, "algorithmic_bytes_per_launch": alg_bytes, "peak_source": peak_src,
                              "note": "cfg2's tables (23 MB) are L2-resident: this kernel is issue/latency bound, not HBM bound, "
                                      "and `achieved` can exceed the HBM peak; extra.cfg5* / extra.cfg4* are the HBM-resident cases"},
@@ -776,7 +787,11 @@ if __name__ == "__main__":
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg (profiling runs)")
     ap.add_argument("--no-extra", action="store_true", help="skip the extra block (profiling runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed (both tables, its loss) as DIR/<name>.npy")
     a = ap.parse_args()
+    if a.steps < 1:
+        ap.error("--steps must be at least 1")
     if a.impl == "reference":
         main_reference(a)
     else:

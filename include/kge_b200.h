@@ -1,5 +1,5 @@
 /*
- * kge_b200.h -- C-ABI of libkge_b200.so, the sm_100a replacement for AmpliGraph's
+ * kge_b200.h -- C-ABI of libkge_b200.so, the sm_90a replacement for AmpliGraph's
  * per-batch training step and all-entity ranking step.
  *
  * The reference has no FFI: its boundary is two Python registries and three
@@ -69,7 +69,7 @@ enum kge_optimizer { KGE_OPT_SGD = 0, KGE_OPT_ADAM = 1, KGE_OPT_ADAGRAD = 2 };
 enum kge_side { KGE_SIDE_S = 0, KGE_SIDE_O = 1 };
 enum kge_rank_strategy { KGE_RANK_WORST = 0, KGE_RANK_BEST = 1, KGE_RANK_MIDDLE = 2 };
 /* how kge_rank scores the candidates of DistMult / ComplEx / HolE (the bilinear models, a [b,K]x[K,E] contraction):
- * AUTO = tensor cores (tcgen05, split-bf16 operands) decide every (query, candidate) pair whose approximate score is
+ * AUTO = tensor cores (wgmma, split-bf16 operands) decide every (query, candidate) pair whose approximate score is
  * provably on one side of the positive's quantisation bin, the few remaining pairs are re-scored with the exact
  * canonical FP32 chain -- ranks are bit-identical to EXACT, which runs that chain for every pair. */
 enum kge_rank_mode { KGE_RANK_MODE_AUTO = 0, KGE_RANK_MODE_EXACT = 1 };

@@ -6,7 +6,7 @@
  * --impl reference leg may load this library; the product (ampligraph_b200/)
  * never does.
  *
- * What it restates (paths under /root/reference/ampligraph/latent_features/):
+ * What it restates (paths under ampligraph/latent_features/ of the reference):
  *   scoring  layers/scoring/TransE.py:37-114, DistMult.py:34-99,
  *            ComplEx.py:39-151, HolE.py:31-89, RotatE.py:62-217
  *   ranks    layers/scoring/AbstractScoringLayer.py:156-422

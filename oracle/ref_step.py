@@ -5,7 +5,7 @@ Torch-CPU fp32 restatement, op for op, of the reference's *training step*
 CUDA path has something to be checked against and timed beside.  TensorFlow is
 not installable in this image (python 3.12, no wheel), hence torch autograd
 stands in for tf.GradientTape; every function cites the reference lines it
-follows (paths under /root/reference/ampligraph/latent_features/).
+follows (paths under ampligraph/latent_features/ of the reference).
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline /
 --impl reference legs may import this module.

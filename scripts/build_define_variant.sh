@@ -12,6 +12,6 @@ mkdir -p "$wt/ampligraph_b200" "$root/_variants"
 cp -r "$root/include" "$wt/include"
 cp -r "$root/ampligraph_b200/csrc" "$wt/ampligraph_b200/csrc"
 rm -rf "$wt/ampligraph_b200/csrc/_build"
-make -C "$wt/ampligraph_b200/csrc" -j"$(nproc)" NVCCFLAGS="-O3 -std=c++17 -lineinfo -gencode arch=compute_100a,code=sm_100a -Xcompiler -fPIC -Xptxas -v --fmad=true $*" >/dev/null
+make -C "$wt/ampligraph_b200/csrc" -j"$(nproc)" NVCCFLAGS="-O3 -std=c++17 -lineinfo -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC -Xptxas -v --fmad=true $*" >/dev/null
 cp "$wt/ampligraph_b200/libkge_b200.so" "$root/_variants/libkge_$name.so"
 echo "built working tree with [$*] -> _variants/libkge_$name.so"

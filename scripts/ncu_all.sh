@@ -1,12 +1,12 @@
 #!/usr/bin/env bash
-# One GPU call that produces an ncu capture for every kernel family of libkge_b200 (north_star: "each kernel ships
-# with an ncu capture").  Run on the B200 box from the repo root, ONE GPU (ncu replays each kernel ~40x):
-#   gpurun --timeout 1200 -- 'bash scripts/ncu_all.sh r2'
-# Outputs (small CSV/JSON summaries, no .ncu-rep) land in gpurun_out/; copy what should be judged into profiles/.
+# One command that produces an ncu capture for every kernel family of libkge_b200.  Run from the repo root on ONE GPU
+# (ncu replays each kernel ~40x):
+#   bash scripts/ncu_all.sh <tag> [capture names]
+# Outputs (small CSV/JSON summaries, no .ncu-rep) land in $NCU_OUT (default ncu_out/, ignored by git).
 set -uo pipefail
 tag=${1:-rX}
 only=${2:-all}   # 'all', or a space-separated list of capture names to run (e.g. "train_cfg3 train_cfg4 rank_rotate")
-out=gpurun_out
+out=${NCU_OUT:-ncu_out}
 mkdir -p $out
 NCU="ncu --clock-control none"
 
@@ -42,7 +42,7 @@ cap train_cfg5w kge_train_kernel 2 1 python scripts/kbench.py one cfg5w 0
 # optimizers: lazy (touched rows only) and the one-launch exchange kernel (world = 1: a multi-rank command must not run under ncu)
 cap optim_lazy kge_optim_lazy_kernel 2 1 python -m pytest tests/test_gpu_parity.py -q -k "lazy_optimizer_matches_restatement and lazy_adam"
 cap optim_exchange kge_optim_exchange_kernel 1 1 python -m pytest tests/test_gpu_parity.py -q -k exchange_kernel_world1
-# ranking kernels: tensor-core filter + its helpers (ComplEx, auto mode), FFMA2 dot kernel (exact mode), packed pair kernel (TransE, RotatE)
+# ranking kernels: tensor-core filter + its helpers (ComplEx, auto mode), FP32 dot kernel (exact mode), pair kernel (TransE, RotatE)
 cap rank_tc 'kge_rank_tc_kernel|kge_rank_split_kernel|kge_rank_refine_kernel' 0 8 python scripts/rbench.py one ComplEx 200 14505 1024
 KGE_B200_RANK_MODE=exact cap rank_dot 'kge_rank_dot_kernel|kge_rank_q|kge_rank_finalize' 0 4 python scripts/rbench.py one ComplEx 200 14505 1024
 cap rank_transe kge_rank_pair_kernel 0 1 python scripts/rbench.py one TransE 400 14505 1024

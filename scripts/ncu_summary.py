@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""Turn ncu CSV exports into the small, reviewable artefacts kept under profiles/.
+"""Turn ncu CSV exports into small, reviewable summaries.
 
-  launch list : ncu --metrics gpu__time_duration.sum --clock-control none -c N --csv --log-file L.csv <cmd>
-                python scripts/ncu_summary.py launches L.csv profiles/<tag>_launch_list_summary.csv "<cmd>"
-  full set    : ncu --set full --clock-control none --import-source on -k regex:... -o R <cmd>
-                ncu -i R.ncu-rep --page raw --csv > R_raw.csv
-                python scripts/ncu_summary.py full R_raw.csv profiles/<tag>_ncu_full_summary.json "<cmd>"
+  launch list : ncu --metrics gpu__time_duration.sum --clock-control none -c N --csv --log-file ncu_out/L.csv <cmd>
+                python scripts/ncu_summary.py launches ncu_out/L.csv ncu_out/<tag>_launch_list_summary.csv "<cmd>"
+  full set    : ncu --set full --clock-control none --import-source on -k regex:... -o ncu_out/R <cmd>
+                ncu -i ncu_out/R.ncu-rep --page raw --csv > ncu_out/R_raw.csv
+                python scripts/ncu_summary.py full ncu_out/R_raw.csv ncu_out/<tag>_ncu_full_summary.json "<cmd>"
 
 Numbers printed by the profiled command itself are never bench values.
 """

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""SASS opcode histogram of libkge_b200.so, per kernel (static instruction counts), and the Blackwell-specific
-mnemonics that prove which engines a kernel uses (UBLKCP = cp.async.bulk, UTC*MMA = tcgen05.mma, LDTM = tcgen05.ld,
-REDG = red.global, FFMA2/FMUL2/FADD2 = packed fp32, SYNCS = mbarrier, LDGMC = multimem.ld_reduce).  Usage: python scripts/sass_histogram.py [so] > profiles/<tag>_sass_opcodes.txt"""
+"""SASS opcode histogram of libkge_b200.so, per kernel (static instruction counts), and the Hopper-specific
+mnemonics that prove which engines a kernel uses (UBLKCP = cp.async.bulk, HGMMA = wgmma, REDG = red.global,
+SYNCS = mbarrier, LDGMC = multimem.ld_reduce).  Usage: python scripts/sass_histogram.py [so] > ncu_out/<tag>_sass_opcodes.txt"""
 import collections
 import re
 import subprocess
@@ -20,7 +20,7 @@ for line in txt.splitlines():
     m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\d+\s+)?([A-Z][A-Z0-9_]*)", line)
     if m and kern:
         hist[kern][m.group(1)] += 1
-MARK = ("UBLKCP", "UBLKRED", "UTCHMMA", "UTCQMMA", "UTCIMMA", "UTCOMMA", "UTCBAR", "LDTM", "STTM", "UTMALDG", "REDG", "FFMA2", "FMUL2", "FADD2", "SYNCS", "HMMA", "LDGSTS", "LDGMC")
+MARK = ("UBLKCP", "UBLKRED", "HGMMA", "WARPGROUP", "UTMALDG", "REDG", "SYNCS", "HMMA", "LDGSTS", "LDGMC")
 print("# static SASS opcode counts per kernel of %s (cuobjdump -sass); marker mnemonics first, then the ten most frequent" % so)
 for k, h in hist.items():
     tot = sum(h.values())

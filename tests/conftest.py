@@ -9,7 +9,7 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 
-try:  # the oracle's torch-CPU ops oversubscribe badly on many-core shared hosts (seen on the B200 boxes)
+try:  # the oracle's torch-CPU ops oversubscribe badly on many-core shared hosts
     import torch
     torch.set_num_threads(min(8, os.cpu_count() or 1))
 except Exception:
@@ -17,7 +17,7 @@ except Exception:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; select with -m gpu)")
 
 
 @pytest.fixture(scope="session")

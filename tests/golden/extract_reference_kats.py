@@ -5,10 +5,10 @@ TensorFlow cannot be imported in the build image, so instead of *running* the
 reference this script parses the reference's test files with `ast` and lifts
 the literal inputs and expected outputs out of them (evaluating only numpy
 expressions; `tf.constant` / `tf.ragged.constant` are stubbed to numpy/lists).
-Run it HERE (where /root/reference exists); the JSON it writes is committed and
-is what travels to the GPU box.
+Run it against a checkout of the reference; the JSON it writes is committed, so
+the tests never need the reference itself.
 
-    python tests/golden/extract_reference_kats.py [/root/reference]
+    python tests/golden/extract_reference_kats.py <path to the reference checkout>
 
 Output: tests/golden/reference_kats.json
 """
@@ -20,7 +20,9 @@ import types
 
 import numpy as np
 
-REF = sys.argv[1] if len(sys.argv) > 1 else "/root/reference"
+if len(sys.argv) != 2:
+    sys.exit(__doc__)
+REF = sys.argv[1]
 TESTS = os.path.join(REF, "tests", "ampligraph", "latent_features")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "reference_kats.json")
 
@@ -219,7 +221,7 @@ def corruption_kat():
 def main():
     kats = {
         "generated_by": "tests/golden/extract_reference_kats.py",
-        "reference": "Accenture/AmpliGraph (mounted at /root/reference)",
+        "reference": "Accenture/AmpliGraph @ 260a732",
         "scoring": scoring_kats(),
         "ranks": rank_kats(),
         "losses": loss_kats(),

@@ -1,6 +1,6 @@
 """GPU parity tests: the CUDA path (through the C-ABI) against the oracle.
 
-Run on the B200 box with `pytest -m gpu`.  Tolerances: fp32 scores / gradients /
+Run on an H100 with `pytest -m gpu`.  Tolerances: fp32 scores / gradients /
 losses within 1e-4 relative (BASELINE.json north_star); ranks bit-exact.
 """
 import numpy as np
@@ -418,7 +418,7 @@ def _zipf_triples(E, R, n, rng):
     # BASELINE configs[1] and [2] at their FULL stated size (entities, batch), Zipf-distributed triples
     ("cfg2", "ComplEx", 200, 10, 14505, 237, 27212, "self_adversarial"),
     ("cfg3", "DistMult", 400, 20, 40943, 11, 8684, "pairwise"),
-    # configs[3] and [4]: exact (k, eta) and a table that does not fit the 126 MB L2 (197 MB / 800 MB); the batch is
+    # configs[3] and [4]: exact (k, eta) and a table that does not fit the H100's 50 MB L2 (197 MB / 800 MB); the batch is
     # bounded so that the CPU oracle (which materialises [B*eta, K] tensors) finishes in seconds
     ("cfg4", "RotatE", 200, 30, 123182, 37, 2048, "self_adversarial"),
     ("cfg5", "ComplEx", 1000, 50, 100000, 1000, 512, "self_adversarial"),
@@ -636,7 +636,7 @@ def test_single_buffered_groups_equal_prefetched_groups(model, k, eta, monkeypat
 
 @pytest.mark.parametrize("model,k", [("TransE", 50), ("TransE", 403), ("RotatE", 7), ("RotatE", 200)])
 def test_packed_pair_ranking_kernel_equals_scalar_tile_kernel(model, k, monkeypatch):
-    """kge_rank_pair_kernel (two canonical chains per packed f32x2 instruction) against kge_rank_tile_kernel (one chain per
+    """kge_rank_pair_kernel (two canonical chains per pair of fp32 registers) against kge_rank_tile_kernel (one chain per
     register, KGE_B200_RANK_KERNEL=tile): every corruption score bit for bit, ragged candidate / query counts, a window of
     candidates; both match the oracle elsewhere (test_corruption_scores_vs_oracle, the rank tests)."""
     rng = np.random.default_rng(97)
@@ -920,7 +920,7 @@ TC_MODELS = ["DistMult", "ComplEx", "HolE"]
                                                ("HolE", 37, 1500, 70, 0.5), ("ComplEx", 1000, 800, 257, 0.02),
                                                ("DistMult", 50, 5000, 64, 1.0)])
 def test_tc_filter_error_bound(model, k, E, b, scale):
-    """The tensor-core filter pass (tcgen05, split-bf16 operands) is sound iff its approximate score is within the bound it
+    """The tensor-core filter pass (wgmma, split-bf16 operands) is sound iff its approximate score is within the bound it
     assumes of the canonical FP32 score for EVERY (query, candidate) pair (kge_rank_tc.cu header).  Measured through
     kge_rank_filter_probe against kge_corruption_scores; the bound must also hold with a >= 4x margin, and the
     approximation must be genuinely fine (3 bf16 products, not 1)."""

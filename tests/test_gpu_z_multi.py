@@ -1,4 +1,4 @@
-"""2-GPU tests (run on a box with >= 2 B200s, e.g. `gpurun --gpus 2`): the data-parallel step --
+"""2-GPU tests (run on a machine with >= 2 H100s): the data-parallel step --
 fused peer-memory optimizer ("p2p") and NCCL all-reduce ("nccl") -- equals the single-GPU step on
 the concatenated global batch; sharded ranking equals full ranking."""
 import os

@@ -93,6 +93,11 @@ PROTOTYPES = {
     "kge_rank_filter_probe": (C.c_int, [_P, C.c_int32, _P, _P, _P, C.c_int64, _P, C.c_int64, C.c_int64, _P, _P, _P,
                                         C.c_int64, _P]),
     "kge_rank_workspace_bytes": (C.c_int64, [_P, C.c_int64, C.c_int64]),
+    "kge_topk": (C.c_int, [_P, C.c_int32, _P, _P, _P, C.c_int64, _P, C.c_int64, C.c_int64, _P, _P, C.c_int64, C.c_int32,
+                           _P, _P, _P, C.c_int64, _P]),
+    "kge_topk_workspace_bytes": (C.c_int64, [_P, C.c_int64, C.c_int64, C.c_int32]),
+    "kge_select_topk": (C.c_int, [_P, _P, C.c_int64, C.c_int64, C.c_int32, _P, _P, _P, C.c_int64, _P]),
+    "kge_select_topk_workspace_bytes": (C.c_int64, [_P, C.c_int64, C.c_int64, C.c_int32]),
 }
 
 _lib = None

@@ -30,6 +30,7 @@ struct kge_handle {
     long long stash_rows;
     int hot_ent[2];              // kge_set_hot_entities (-1: none)
     int l2_bytes;                // cudaDeviceProp::l2CacheSize
+    long long topk_chunk;        // KGE_B200_TOPK_CHUNK: candidates per kge_topk chunk (0: sized to L2)
 };
 
 // Make the handle's device current for the duration of an entry point (ADVICE r1: two handles on different GPUs
@@ -127,6 +128,8 @@ extern "C" int kge_create(const kge_config *cfg, kge_handle **out)
     h->sm_count = prop.multiProcessorCount;
     h->max_smem = (int)prop.sharedMemPerBlockOptin;
     h->l2_bytes = prop.l2CacheSize;
+    // development switch: force the kge_topk chunk (the tests use it to run many chunks over small tables)
+    if (const char *ev = getenv("KGE_B200_TOPK_CHUNK")) { const long long c = atoll(ev); if (c >= 1) h->topk_chunk = c; }
     h->score_scale = (cfg->scoring == KGE_HOLE) ? hole_scale(L.K) : 1.f;
     h->rot_div = (cfg->scoring == KGE_ROTATE) ? rotate_divisor(L.K, cfg->max_rel_size > 0 ? cfg->max_rel_size : cfg->n_rel) : 1.f;
 
@@ -726,7 +729,8 @@ struct RankWorkspace {
     size_t bytes;
 };
 static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-static RankWorkspace carve_rank_workspace(const kge_handle *h, void *base, int64_t b, int64_t n_cand)
+// tc_region = false: never carve the tensor-core region (kge_topk runs the exact chain only)
+static RankWorkspace carve_rank_workspace(const kge_handle *h, void *base, int64_t b, int64_t n_cand, bool tc_region = true)
 {
     RankWorkspace w;
     char *p = (char *)base;
@@ -737,7 +741,7 @@ static RankWorkspace carve_rank_workspace(const kge_handle *h, void *base, int64
     w.qaux = (float *)(p + off); off += qbytes;
     w.qpos = (int32_t *)(p + off); off += align256((size_t)b * sizeof(int32_t));
     w.cnt = (int32_t *)(p + off); off += align256((size_t)3 * b * sizeof(int32_t));
-    w.tc = h->cfg.rank_mode == KGE_RANK_MODE_AUTO && rank_tc_applicable(h->L, 0, b, n_cand);
+    w.tc = tc_region && h->cfg.rank_mode == KGE_RANK_MODE_AUTO && rank_tc_applicable(h->L, 0, b, n_cand);
     w.tc_base = nullptr;
     if (w.tc) {
         off = (off + 1023) & ~(size_t)1023;
@@ -887,4 +891,173 @@ extern "C" int kge_rank_filter_probe(kge_handle *h, int32_t side, const float *e
     if (!approx_dev || !delta_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_rank_filter_probe: null output");
     return rank_impl(h, nullptr, 0, side, KGE_RANK_WORST, ent_dev, rel_dev, triples_dev, b, cand_ids_dev, cand_begin, n_cand,
                      nullptr, nullptr, 0, nullptr, nullptr, approx_dev, workspace_dev, workspace_bytes, stream, delta_dev);
+}
+
+// ---- top-k link prediction ---------------------------------------------------------------------------------
+// the running lists of kge_topk_select_kernel: keys and raw scores [2, b, k] each, state [b]
+struct TopkLists {
+    unsigned long long *keys;
+    float *vals;
+    int2 *state;
+    size_t bytes;
+};
+static TopkLists carve_topk_lists(void *base, size_t off, int64_t b, int32_t k)
+{
+    TopkLists l;
+    char *p = (char *)base;
+    l.keys = (unsigned long long *)(p + off); off += align256((size_t)2 * b * k * sizeof(unsigned long long));
+    l.vals = (float *)(p + off); off += align256((size_t)2 * b * k * sizeof(float));
+    l.state = (int2 *)(p + off); off += align256((size_t)b * sizeof(int2));
+    l.bytes = off;
+    return l;
+}
+// Candidates per chunk: the [b, C] fp32 chunk the scoring kernel writes and the select kernel reads back is sized to the
+// L2 (50 MB on an H100), so it mostly stays there; multiple of 256 (the scoring tile).  Half the L2 was measured slower
+// (DESIGN.md 5): more, smaller scoring launches each end in a partly idle wave.
+static int64_t topk_chunk(const kge_handle *h, int64_t b, int64_t n_cand)
+{
+    int64_t c = h->topk_chunk;
+    if (c <= 0) {
+        c = (int64_t)h->l2_bytes / (4 * (b > 0 ? b : 1)) / 256 * 256;
+        if (c < 256) c = 256;
+        if (c < n_cand) {  // equal chunks: no small last chunk whose scoring launch leaves most SMs idle
+            const int64_t n_chunks = (n_cand + c - 1) / c;
+            c = ((n_cand + n_chunks - 1) / n_chunks + 255) / 256 * 256;
+        }
+    }
+    if (c > n_cand) c = n_cand;
+    return c < 1 ? 1 : c;
+}
+struct TopkWorkspace {
+    RankWorkspace r;  // query vectors and the (unused) rank counters of the scoring kernels
+    float *chunk;     // [b, C]
+    TopkLists l;
+};
+static TopkWorkspace carve_topk_workspace(const kge_handle *h, void *base, int64_t b, int64_t n_cand, int32_t k)
+{
+    TopkWorkspace w;
+    w.r = carve_rank_workspace(h, base, b, n_cand, false);
+    size_t off = w.r.bytes;
+    w.chunk = (float *)((char *)base + off);
+    off += align256((size_t)b * topk_chunk(h, b, n_cand) * sizeof(float));
+    w.l = carve_topk_lists(base, off, b, k);
+    return w;
+}
+
+extern "C" int64_t kge_topk_workspace_bytes(const kge_handle *h, int64_t b, int64_t n_cand, int32_t k)
+{
+    if (!h || b < 0 || n_cand < 0 || k < 1) return 0;
+    return (int64_t)carve_topk_workspace(h, nullptr, b, n_cand, k).l.bytes;
+}
+
+extern "C" int64_t kge_select_topk_workspace_bytes(const kge_handle *h, int64_t b, int64_t n, int32_t k)
+{
+    if (!h || b < 0 || n < 0 || k < 1) return 0;
+    return (int64_t)carve_topk_lists(nullptr, 0, b, k).bytes;
+}
+
+static int check_topk_workspace(void *ws, int64_t bytes, int64_t need, const char *fn)
+{
+    if (!ws || bytes < need)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "%s: workspace of %lld bytes needed (%s_workspace_bytes), got %lld", fn,
+                    (long long)need, fn, (long long)(ws ? bytes : 0));
+    if (((uintptr_t)ws & 1023u) != 0) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: workspace must be 1024-byte aligned", fn);
+    return KGE_OK;
+}
+
+extern "C" int kge_topk(kge_handle *h, int32_t side, const float *ent_dev, const float *rel_dev, const int32_t *triples_dev,
+                        int64_t b, const int32_t *cand_ids_dev, int64_t cand_begin, int64_t n_cand,
+                        const int64_t *filt_off_dev, const int32_t *filt_idx_dev, int64_t n_filt, int32_t k,
+                        int32_t *ids_dev, float *scores_dev, void *workspace_dev, int64_t workspace_bytes, void *stream)
+{
+    KGE_CHECK_HANDLE(h, "kge_topk");
+    if (side != KGE_SIDE_S && side != KGE_SIDE_O) return fail(KGE_ERR_INVALID_ARGUMENT, "Invalid value for corrupt_side");
+    if (k < 1) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_topk: k must be >= 1, got %d", k);
+    if (b < 0 || n_cand < 0 || cand_begin < 0 || n_filt < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_topk: negative size");
+    if (n_cand > 0x7fffffffLL) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_topk: n_cand must be < 2^31");
+    if (b == 0) return KGE_OK;
+    if (!ent_dev || !rel_dev || !triples_dev || !ids_dev || !scores_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_topk: null pointer");
+    if (cand_ids_dev && cand_begin != 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_topk: cand_begin must be 0 with cand_ids_dev");
+    if (!cand_ids_dev && cand_begin + n_cand > h->cfg.n_ent)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_topk: candidate range [%lld,%lld) exceeds n_ent %lld", (long long)cand_begin,
+                    (long long)(cand_begin + n_cand), (long long)h->cfg.n_ent);
+    if ((filt_off_dev == nullptr || filt_idx_dev == nullptr) && n_filt > 0)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_topk: filter offsets and indices must be given together");
+    if (int rc = check_topk_workspace(workspace_dev, workspace_bytes, kge_topk_workspace_bytes(h, b, n_cand, k), "kge_topk")) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    const TopkWorkspace w = carve_topk_workspace(h, workspace_dev, b, n_cand, k);
+    if (int rc = refresh_rotation(h, rel_dev, st)) return rc;
+    ShardView sv;
+    memset(&sv, 0, sizeof(sv));
+    KGE_CUDA(launch_rank_prepare(h->L, sv, ent_dev, rel_dev, h->rot, triples_dev, b, h->score_scale, w.r.qs, w.r.qo, w.r.qaux,
+                                 w.r.qpos, st),
+             "kge_topk: prepare");
+    KGE_CUDA(cudaMemsetAsync(w.l.state, 0, (size_t)b * sizeof(int2), st), "kge_topk: memset");
+    RankParams p;
+    memset(&p, 0, sizeof(p));
+    p.L = h->L;
+    p.side = side;
+    p.strategy = KGE_RANK_WORST;
+    p.ent = ent_dev;
+    p.qvec = side == KGE_SIDE_S ? w.r.qs : w.r.qo;
+    p.qaux = w.r.qaux;
+    p.qpos = w.r.qpos;
+    p.b = b;
+    p.scale = h->score_scale;
+    p.scores = w.chunk;
+    TopkSelectParams s;
+    memset(&s, 0, sizeof(s));
+    s.scores = w.chunk;
+    s.b = b;
+    s.k = k;
+    if (n_filt > 0) { s.filt_off = (const long long *)filt_off_dev; s.filt_idx = filt_idx_dev; }
+    s.filt_shift = cand_ids_dev ? 0 : cand_begin;
+    s.keys = w.l.keys;
+    s.vals = w.l.vals;
+    s.state = w.l.state;
+    const int64_t C = topk_chunk(h, b, n_cand);
+    for (int64_t c0 = 0; c0 < n_cand; c0 += C) {
+        const int64_t nc = n_cand - c0 < C ? n_cand - c0 : C;
+        // the exact FP32 chain in every rank_mode: scores bit-identical to kge_corruption_scores ([b, nc], row stride nc)
+        p.cand_ids = cand_ids_dev ? cand_ids_dev + c0 : nullptr;
+        p.cand_begin = cand_ids_dev ? 0 : cand_begin + c0;
+        p.n_cand = nc;
+        KGE_CUDA(launch_rank_count(p, w.r.cnt, st), "kge_topk: scores");
+        s.ld = nc;
+        s.n = nc;
+        s.base = c0;
+        KGE_CUDA(launch_topk_select(s, st), "kge_topk: select");
+    }
+    KGE_CUDA(launch_topk_write(w.l.state, w.l.keys, w.l.vals, b, k, cand_ids_dev, cand_begin, ids_dev, scores_dev, st),
+             "kge_topk: write");
+    return KGE_OK;
+}
+
+extern "C" int kge_select_topk(kge_handle *h, const float *scores_dev, int64_t b, int64_t n, int32_t k, int32_t *pos_dev,
+                               float *out_dev, void *workspace_dev, int64_t workspace_bytes, void *stream)
+{
+    KGE_CHECK_HANDLE(h, "kge_select_topk");
+    if (k < 1) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_select_topk: k must be >= 1, got %d", k);
+    if (b < 0 || n < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_select_topk: negative size");
+    if (n > 0x7fffffffLL) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_select_topk: n must be < 2^31");
+    if (b == 0) return KGE_OK;
+    if ((n > 0 && !scores_dev) || !pos_dev || !out_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_select_topk: null pointer");
+    if (int rc = check_topk_workspace(workspace_dev, workspace_bytes, kge_select_topk_workspace_bytes(h, b, n, k), "kge_select_topk"))
+        return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    const TopkLists l = carve_topk_lists(workspace_dev, 0, b, k);
+    KGE_CUDA(cudaMemsetAsync(l.state, 0, (size_t)b * sizeof(int2), st), "kge_select_topk: memset");
+    TopkSelectParams s;
+    memset(&s, 0, sizeof(s));
+    s.scores = scores_dev;
+    s.ld = n;
+    s.n = n;
+    s.b = b;
+    s.k = k;
+    s.keys = l.keys;
+    s.vals = l.vals;
+    s.state = l.state;
+    KGE_CUDA(launch_topk_select(s, st), "kge_select_topk: select");
+    KGE_CUDA(launch_topk_write(l.state, l.keys, l.vals, b, k, nullptr, 0, pos_dev, out_dev, st), "kge_select_topk: write");
+    return KGE_OK;
 }

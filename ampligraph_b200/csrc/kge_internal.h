@@ -142,6 +142,23 @@ cudaError_t launch_rank_filter_n(const RankParams &p, const long long *filt_off,
 cudaError_t launch_rank_finalize(const int32_t *cnt, long long b, int strategy, int32_t *ranks, cudaStream_t st);
 cudaError_t launch_rank_accumulate(const int32_t *cnt, long long b, int32_t *counts, cudaStream_t st);  // counts += cnt
 
+// kge_topk.cu: running top-k per query over chunks of candidate scores (ordering contract: see the file)
+struct TopkSelectParams {
+    const float *scores;                 // [b, ld]: this chunk's scores in columns [0, n)
+    long long ld, n, base;               // row stride, columns, candidate position of column 0
+    long long b;
+    int k;
+    const long long *filt_off;           // [b+1] CSR offsets or nullptr; filt_idx - filt_shift = candidate positions
+    const int32_t *filt_idx;             // to exclude (outside [0, n_cand): ignored)
+    long long filt_shift;
+    unsigned long long *keys;            // [2, b, k] sorted keys of the running lists (double-buffered)
+    float *vals;                         // [2, b, k] their raw scores
+    int2 *state;                         // [b] {entries, current buffer}; zero before the first chunk
+};
+cudaError_t launch_topk_select(const TopkSelectParams &p, cudaStream_t st);
+cudaError_t launch_topk_write(const int2 *state, const unsigned long long *keys, const float *vals, long long b, int k,
+                              const int32_t *cand_ids, long long cand_begin, int32_t *ids, float *out, cudaStream_t st);
+
 // kge_rank_tc.cu: tensor-core filter + exact refine for the bilinear models
 struct RankTcLayout {  // carve-up of the tensor-core part of the caller's workspace
     int nkb, n_qb, n_ct;

@@ -303,7 +303,10 @@ class KGEEngine:
     def rank_workspace(self, b, n_cand):
         """The caller-owned scratch kge_rank needs (kge_rank_workspace_bytes): one cached torch buffer, grown on demand.
         Growing frees the old buffer through torch's stream-ordered caching allocator, so no synchronisation is needed."""
-        need = int(self.lib.kge_rank_workspace_bytes(self.h, int(b), int(n_cand)))
+        return self._workspace(int(self.lib.kge_rank_workspace_bytes(self.h, int(b), int(n_cand))))
+
+    def _workspace(self, need):
+        """The cached 1024-byte aligned scratch of rank_workspace, at least `need` bytes; top-k shares it."""
         if self._rank_ws is None or self._rank_ws.numel() < need:
             raw = torch.empty(max(need, 1024) + 1024, dtype=torch.uint8, device=self.device)
             off = (-raw.data_ptr()) % 1024  # the library wants a 1024-byte aligned base (operand tiles of the tensor-core pass)
@@ -366,3 +369,40 @@ class KGEEngine:
                                                   self._stream()))
         self.launches += 3
         return out
+
+    @_traced("kge.topk")
+    def topk(self, triples, side, k, filt_off=None, filt_idx=None, cand_ids=None, cand_begin=0, n_cand=None):
+        """Link prediction (kge_topk): the k best candidates on `side` of each query -> (ids int32 [b,k], scores fp32 [b,k])
+        on the device, sorted by (score desc, candidate position asc), NaN first; scores bit-identical to
+        corruption_scores.  Candidates and filter (candidate positions to exclude) as in rank; rows with fewer than k
+        eligible candidates end in id -1 / score -inf."""
+        assert triples.dtype == torch.int32 and triples.is_cuda and triples.is_contiguous()
+        b = triples.shape[0]
+        if n_cand is None:
+            n_cand = cand_ids.numel() if cand_ids is not None else self.n_ent - cand_begin
+        n_filt = int(filt_idx.numel()) if filt_idx is not None else 0
+        ids = torch.empty((b, max(int(k), 0)), dtype=torch.int32, device=self.device)
+        scores = torch.empty((b, max(int(k), 0)), dtype=torch.float32, device=self.device)
+        ws, ws_bytes = self._topk_workspace(self.lib.kge_topk_workspace_bytes(self.h, b, int(n_cand), int(k)))
+        _lib.check(self.lib.kge_topk(self.h, _lib.SIDES[side], _ptr(self.ent), _ptr(self.rel), _ptr(triples), b,
+                                     _ptr(cand_ids), int(cand_begin), int(n_cand), _ptr(filt_off), _ptr(filt_idx), n_filt,
+                                     int(k), _ptr(ids), _ptr(scores), _ptr(ws), ws_bytes, self._stream()))
+        return ids, scores
+
+    @_traced("kge.select_topk")
+    def select_topk(self, scores, k):
+        """kge_select_topk on a [b, n] fp32 device matrix -> (positions int32 [b,k], values fp32 [b,k]), same order and
+        padding (-1 / -inf) as topk."""
+        assert scores.dtype == torch.float32 and scores.is_cuda and scores.is_contiguous() and scores.dim() == 2
+        b, n = scores.shape
+        pos = torch.empty((b, max(int(k), 0)), dtype=torch.int32, device=self.device)
+        out = torch.empty((b, max(int(k), 0)), dtype=torch.float32, device=self.device)
+        ws, ws_bytes = self._topk_workspace(self.lib.kge_select_topk_workspace_bytes(self.h, b, n, int(k)))
+        _lib.check(self.lib.kge_select_topk(self.h, _ptr(scores), b, n, int(k), _ptr(pos), _ptr(out), _ptr(ws), ws_bytes,
+                                            self._stream()))
+        return pos, out
+
+    def _topk_workspace(self, need):
+        # need == 0: invalid arguments (k < 1, ...) -- the call itself reports them
+        need = int(need)
+        return self._workspace(need) if need > 0 else (None, 0)

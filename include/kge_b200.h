@@ -386,6 +386,30 @@ int kge_rank_filter_probe(kge_handle *h, int32_t side, const float *ent_dev, con
  * the split-bf16 copies of the candidate rows and query vectors the tensor-core pass reads). */
 int64_t kge_rank_workspace_bytes(const kge_handle *h, int64_t b, int64_t n_cand);
 
+/* discovery.query_topn (discovery.py:985-1168), batched: the k best candidates on `side` for each of b queries.
+ * Candidates, cand_ids / cand_begin / n_cand and the filter CSR (candidate POSITIONS; those are excluded) follow
+ * kge_rank.  Every id in triples_dev must be valid; the column of `side` does not affect the result.
+ * ids_dev/scores_dev [b,k]: sorted by (score desc, position asc), NaN first; scores are kge_corruption_scores' bit
+ * for bit; rows with fewer than k eligible candidates are padded with id -1, score -inf.
+ * The reference scores every completed triple on the host and sorts them all (:1143-1168); here the candidates are
+ * scored in L2-sized chunks by the exact FP32 chain (in every rank_mode) and merged into a running top-k per query, so
+ * no [b, n_cand] matrix exists.  Any 1 <= k works; k > n_cand pads.  workspace_dev: at least
+ * kge_topk_workspace_bytes(h, b, n_cand, k) bytes, 1024-byte aligned, contents undefined afterwards. */
+int kge_topk(kge_handle *h, int32_t side, const float *ent_dev, const float *rel_dev, const int32_t *triples_dev,
+             int64_t b, const int32_t *cand_ids_dev, int64_t cand_begin, int64_t n_cand,
+             const int64_t *filt_off_dev, const int32_t *filt_idx_dev, int64_t n_filt, int32_t k,
+             int32_t *ids_dev, float *scores_dev, void *workspace_dev, int64_t workspace_bytes, void *stream);
+/* bytes of scratch kge_topk needs: query vectors, one [b, C] score chunk (C sized to half the L2, or
+ * KGE_B200_TOPK_CHUNK) and the double-buffered running lists (12 bytes per slot, 2 * b * k slots). */
+int64_t kge_topk_workspace_bytes(const kge_handle *h, int64_t b, int64_t n_cand, int32_t k);
+
+/* the same selection over a caller's [b, n] score matrix (positions out); relation completion uses it
+ * (discovery.py:1160-1166: argsort of the predicted scores of the R completed triples).  pos_dev/out_dev [b,k], same
+ * order and padding (position -1, -inf) as kge_topk; out_dev holds the input values bit for bit. */
+int kge_select_topk(kge_handle *h, const float *scores_dev, int64_t b, int64_t n, int32_t k,
+                    int32_t *pos_dev, float *out_dev, void *workspace_dev, int64_t workspace_bytes, void *stream);
+int64_t kge_select_topk_workspace_bytes(const kge_handle *h, int64_t b, int64_t n, int32_t k);
+
 #ifdef __cplusplus
 }
 #endif

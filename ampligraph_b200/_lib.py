@@ -74,6 +74,8 @@ PROTOTYPES = {
     "kge_set_row_stamps": (C.c_int, [_P, _P, _P]),
     "kge_set_row_stash": (C.c_int, [_P, _P, C.c_int64]),
     "kge_set_hot_entities": (C.c_int, [_P, _P, C.c_int32]),
+    "kge_train_workspace_bytes": (C.c_int64, [_P, C.c_int64]),
+    "kge_set_train_workspace": (C.c_int, [_P, _P, C.c_int64, _P]),
     "kge_rows_resident": (C.c_int, [_P]),
     "kge_step_stamp": (C.c_int32, [C.c_uint64]),
     "kge_optimizer_step_lazy": (C.c_int, [_P, C.POINTER(KgeOptimizerConfig), C.c_int64, _P, _P, _P, _P, C.c_int64, _P,

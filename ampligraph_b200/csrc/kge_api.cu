@@ -31,6 +31,8 @@ struct kge_handle {
     int hot_ent[2];              // kge_set_hot_entities (-1: none)
     int l2_bytes;                // cudaDeviceProp::l2CacheSize
     long long topk_chunk;        // KGE_B200_TOPK_CHUNK: candidates per kge_topk chunk (0: sized to L2)
+    void *train_ws;              // caller-owned training workspace (kge_set_train_workspace) or nullptr
+    long long train_ws_bytes;
 };
 
 // Make the handle's device current for the duration of an entry point (ADVICE r1: two handles on different GPUs
@@ -358,6 +360,56 @@ static int check_shard_map(const kge_handle *h, const kge_shard_map *map, const 
     return KGE_OK;
 }
 
+// Carve-up of the training workspace for a batch of B positives (the owner-computes path of the resident kernel,
+// kge_train_bucket.cu): the per-entity counts first, so that they stay where kge_set_train_workspace zeroed them whatever B is.
+static long long carve_train_workspace(const kge_handle *h, int64_t B, char *base, TrainParams::Buckets *bk)
+{
+    const long long E = h->cfg.n_ent, n = (long long)h->cfg.eta * B;
+    auto al = [](long long x) { return (x + 15) & ~15ll; };
+    long long at = 0;
+    auto take = [&](long long bytes) { char *q = base ? base + at : nullptr; at += al(bytes); return q; };
+    char *cnt = take(4 * E), *off = take(4 * (E + 1)), *tiles = take(4 * ((E + 8191) / 8192)), *pos = take(4 * n),
+         *eid = take(4 * n), *other = take(4 * n), *rel = take(4 * n), *g = take(4 * n);
+    if (bk) {
+        bk->cnt = reinterpret_cast<int *>(cnt); bk->off = reinterpret_cast<int *>(off); bk->tiles = reinterpret_cast<int *>(tiles);
+        bk->pos = reinterpret_cast<int *>(pos);
+        bk->eid = reinterpret_cast<int *>(eid); bk->other = reinterpret_cast<int *>(other); bk->rel = reinterpret_cast<int *>(rel);
+        bk->g = reinterpret_cast<float *>(g);
+    }
+    return at;
+}
+
+// Whether a fused step of B positives takes the owner-computes path (given a workspace): the resident kernel applies, the
+// step replaces every entity at least once on average (eta*B >= n_ent), and KGE_B200_TRAIN_REPL=scatter (A/B runs, the
+// tests that compare the two) does not keep the REDs.  The bucket sum reads one kept-side entity row per corruption; it
+// pays where replaced entities repeat within a step (measured on H100: cfg2, 19 corruptions per entity, and cfg3, 4.2,
+// gain) and loses where they do not ('big' in scripts/kbench.py: 2 M entities, 0.33 per entity, HBM-resident, 1.65 ->
+// 1.88 ms; DESIGN.md 5).
+static bool bucket_applies(const kge_handle *h, int64_t B)
+{
+    const char *rv = getenv("KGE_B200_TRAIN_REPL");
+    return h->res_warps > 0 && (long long)h->cfg.eta * B >= h->cfg.n_ent && !(rv && strcmp(rv, "scatter") == 0);
+}
+
+extern "C" int64_t kge_train_workspace_bytes(const kge_handle *h, int64_t B)
+{
+    if (!h || B < 0 || !bucket_applies(h, B)) return 0;
+    return carve_train_workspace(h, B, nullptr, nullptr);
+}
+
+extern "C" int kge_set_train_workspace(kge_handle *h, void *ws_dev, int64_t bytes, void *stream)
+{
+    KGE_CHECK_HANDLE(h, "kge_set_train_workspace");
+    if (bytes < 0 || (ws_dev && ((uintptr_t)ws_dev & 15)))
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_set_train_workspace: bytes < 0 or workspace not 16-byte aligned");
+    if (ws_dev && bytes < carve_train_workspace(h, 0, nullptr, nullptr))
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_set_train_workspace: %lld bytes do not hold the per-entity counts", (long long)bytes);
+    if (ws_dev) KGE_CUDA(cudaMemsetAsync(ws_dev, 0, 4 * (size_t)h->cfg.n_ent, (cudaStream_t)stream), "kge_set_train_workspace");
+    h->train_ws = ws_dev;
+    h->train_ws_bytes = ws_dev ? bytes : 0;
+    return KGE_OK;
+}
+
 static int train_step_impl(kge_handle *h, int32_t mode, const kge_shard_map *map, const float *ent_dev,
                            const float *rel_dev, float *grad_ent_dev, float *grad_rel_dev,
                            const int32_t *triples_dev, int64_t B, const int32_t *neg_ent_dev,
@@ -470,8 +522,17 @@ static int train_step_impl(kge_handle *h, int32_t mode, const kge_shard_map *map
     if (fast) {
         p.rows_bytes = h->res_rows_bytes;
         p.region_bytes = h->res_region_bytes;
+        // Owner-computes gradient of the replaced rows (kge_train_bucket.cu) where it applies (bucket_applies) and a workspace
+        // is set: on H100 the eta*B uniformly scattered row REDs it removes cost about half the kernel (DESIGN.md 3.2, 5).
+        const bool gather = mode != KGE_STEP_FORWARD_ONLY && h->train_ws != nullptr && bucket_applies(h, B) &&
+                            (long long)h->cfg.eta * B < (1ll << 31) && carve_train_workspace(h, B, nullptr, nullptr) <= h->train_ws_bytes;
+        if (gather) {
+            carve_train_workspace(h, B, static_cast<char *>(h->train_ws), &p.bk);
+            KGE_CUDA(launch_bucket_prepass(p, st), "kge_train_step (bucket pre-pass)");
+        }
         KGE_CUDA(launch_train_res(p, h->nit, h->sm_count, h->res_warps * 32, (size_t)h->res_warps * h->res_region_bytes, st),
                  "kge_train_step");
+        if (gather) KGE_CUDA(launch_bucket_sum(p, h->nit, st), "kge_train_step (bucket sum)");
         return KGE_OK;
     }
     KGE_CUDA(launch_train(p, h->nit, h->sm_count, h->warps * 32, (size_t)h->warps * h->region_bytes, st),

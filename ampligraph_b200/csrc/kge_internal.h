@@ -48,6 +48,18 @@ struct TrainParams {
     int hot_ent[2];  // entities whose subject/object gradient rows are summed per warp before they are scattered (-1: none); fast path only
     float *stash;  // [B, eta, ld] local copy of the replaced rows gathered by the score pass (sharded runs) or nullptr
     unsigned *sched;  // {next positive, retired warps}: dynamic assignment of positives to warps (see next_positive), or nullptr = static stride
+    // owner-computes gradient of the replaced rows (kge_train_bucket.cu; fast path only), carved from the caller's training
+    // workspace; bk.g == nullptr: the replaced rows' gradients are scattered with REDs instead
+    struct Buckets {
+        int *cnt;     // [n_ent] corruptions per replaced entity (zero between steps: the scan resets it)
+        int *off;     // [n_ent + 1] CSR offsets of each entity's entries
+        int *tiles;   // [ceil(n_ent / 8192)] entries per tile of the two-level scan
+        int *pos;     // [eta*B] rank of corruption r = j*B+i inside its entity's bucket
+        int *eid;     // [eta*B] entry -> replaced entity
+        int *other;   // [eta*B] entry -> the positive's entity on the side that was kept
+        int *rel;     // [eta*B] entry -> relation id | side << 31 (1: object replaced)
+        float *g;     // [eta*B] entry -> scale * dL/dscore of the corruption
+    } bk;
 };
 
 // grid = min(occupancy * sm_count, ceil(B / warps))
@@ -55,6 +67,11 @@ cudaError_t launch_train(const TrainParams &p, int nit, int sm_count, int thread
 // kge_train_res.cu: the resident trilinear fast path (DistMult / ComplEx / HolE, all rows of a positive resident, eta <= 32, one
 // table); p.rows_bytes / p.region_bytes carry ITS slot geometry (kge_create: res_*), threads = res_warps * 32
 cudaError_t launch_train_res(const TrainParams &p, int nit, int sm_count, int threads, size_t smem, cudaStream_t st);
+// kge_train_bucket.cu: the owner-computes sum of the replaced rows' gradients around launch_train_res (p.bk set):
+// before it, bucket the eta*B corruptions by replaced entity (count + scan); after it, one warp per run of entries
+// forms each entity's gradient row and adds it to p.grad_ent once
+cudaError_t launch_bucket_prepass(const TrainParams &p, cudaStream_t st);
+cudaError_t launch_bucket_sum(const TrainParams &p, int nit, cudaStream_t st);
 // kge_train_rot.cu: the RotatE fast path (one column window, single table, any eta in groups of p.G with two buffers -- or one
 // group when everything fits); p.G / p.rows_bytes / p.region_bytes carry ITS slot geometry (kge_create: rot_*), threads = rot_warps * 32
 cudaError_t launch_train_rot(const TrainParams &p, int nit, int sm_count, int threads, size_t smem, cudaStream_t st);

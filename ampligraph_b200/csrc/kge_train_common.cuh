@@ -212,6 +212,31 @@ __device__ __forceinline__ void bulk_load_s(uint32_t smem_dst, const void *gmem_
 #define KGE_KEEPF(x) asm volatile("" : "+f"(x))
 __device__ __forceinline__ void red4(char *row, uint32_t byte_off, float4 v) { red_add_v4(reinterpret_cast<float *>(row + byte_off), v); }
 
+// Query vectors of the trilinear models (DistMult: HALVES = 1; ComplEx / HolE: HALVES = 2, re / im halves), one float4
+// chunk: the score of a corruption is <row, Q>, and its replaced row's gradient is g * Q.  The fused kernel
+// (kge_train_res.cu) and the owner-computes gradient sum (kge_train_bucket.cu) both form Q here, so every g * Q term is
+// bit-identical between them.  Subject replaced: Q0(p, o); object replaced: Q1(s, p).
+template <int HALVES>
+__device__ __forceinline__ void query_subj(float4 pr, float4 pi, float4 orr, float4 oi, float4 &qr, float4 &qi)
+{
+    if constexpr (HALVES == 2) {
+        qr = f4fma(pi, oi, pr * orr);
+        qi = pr * oi - pi * orr;
+    } else {
+        qr = pr * orr;
+    }
+}
+template <int HALVES>
+__device__ __forceinline__ void query_obj(float4 sr, float4 si, float4 pr, float4 pi, float4 &qr, float4 &qi)
+{
+    if constexpr (HALVES == 2) {
+        qr = sr * pr - si * pi;
+        qi = f4fma(sr, pi, si * pr);
+    } else {
+        qr = sr * pr;
+    }
+}
+
 
 // --------------------------------------------------------------------------
 // Dynamic assignment of positives to warps.  A static stride (warp w takes w, w + n_warps, ...) quantises the launch to

@@ -18,6 +18,16 @@ namespace kge {
 #define KGE_HOT 1  // entities whose subject/object gradient rows are privatised per warp (1 or 2; 2 measured no faster on cfg2 and slower on uniform triples before the H100 port)
 #endif
 
+// RED of one chunk of a replaced entity's gradient row.  -DKGE_PROFILE_NOREPLRED builds a profiling variant that drops
+// only these (the s / p / o rows keep theirs): how much of the kernel the uniformly scattered replaced-row REDs cost.
+__device__ __forceinline__ void red_repl_v4(float *g, float4 v)
+{
+#ifdef KGE_PROFILE_NOREPLRED
+    if (v.x != 1.2345e38f) return;  // profiling build: the RED is dropped, v stays live
+#endif
+    red_add_v4(g, v);
+}
+
 // ---- the kernel ----------------------------------------------------------------------------------------------------------
 // HALVES = 1: DistMult (f = sum s p o, DistMult.py:48); HALVES = 2: ComplEx / HolE (ComplEx.py:52-62; HolE.py:45 scales by
 // 2/k, folded into the gradient scalars).  Lane l owns float4 chunks c = l + 32*it (it < NIT) of every half-row; lanes past
@@ -31,7 +41,10 @@ namespace kge {
 // Gradient rows leave the SM as red.global.add.v4.f32 straight from registers.  Sending part of them down the copy
 // engine's road instead (g*Q staged over the gathered row with st.shared.v4, one cp.reduce.async.bulk per row) was
 // measured slower on cfg2 before the H100 port, for every second replaced row and for all of them.
-template <int HALVES, int NIT, int THREADS>
+// GATHER: the owner-computes path (kge_train_bucket.cu) -- instead of scattering g * Q into each replaced row, every
+// corruption leaves (its entity, the kept-side entity, the relation and side, g) in its entity's bucket, at the slot the
+// pre-pass ranked it to; the bucket sum forms the rows afterwards.  Everything else is the same kernel.
+template <int HALVES, int NIT, int THREADS, bool GATHER>
 __global__ void __launch_bounds__(THREADS) kge_train_res_kernel(const TrainParams p)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -102,17 +115,20 @@ __global__ void __launch_bounds__(THREADS) kge_train_res_kernel(const TrainParam
         int tv = 0;
         if (lane < 3) tv = __ldg(p.triples + 3 * i + lane);
         const int s_id = __shfl_sync(0xffffffffu, tv, 0), p_id = __shfl_sync(0xffffffffu, tv, 1), o_id = __shfl_sync(0xffffffffu, tv, 2);
-        int keep = -1, repl = 0;
+        int keep = -1, repl = 0, bk_at = 0;
         if (lane < eta) {
             const unsigned long long r = (unsigned long long)lane * (unsigned long long)p.B + (unsigned long long)i;  // tile order j*B+i
             if (p.neg_ent) { repl = p.neg_ent[r]; keep = p.neg_keep[r] ? 1 : 0; }
             else draw_corruption(p.seed, p.step, r, p.n_ent, &keep, &repl);
+            if constexpr (GATHER) bk_at = p.bk.off[repl] + p.bk.pos[r];  // consumed after the loss: the loads are long done
         }
         // slots [0, n0) replaced the subject (keep_subj == 0), slots [n0, eta) the object; jorig[slot] = j
         const unsigned m0 = __ballot_sync(0xffffffffu, keep == 0), m1 = __ballot_sync(0xffffffffu, keep == 1);
         const int n0 = __popc(m0);
+        int slot = 0;  // this lane's corruption's slot
         if (lane < eta) {
             const int t = keep ? n0 + __popc(m1 & lt) : __popc(m0 & lt);
+            slot = t;
             sts_i(nid_s + 4u * (uint32_t)t, repl);
             sts_i(jor_s + 4u * (uint32_t)t, lane);
             if (stamping) p.stamp_ent[repl] = p.stamp;  // lazy optimizer: row touched
@@ -162,17 +178,15 @@ __global__ void __launch_bounds__(THREADS) kge_train_res_kernel(const TrainParam
                 if constexpr (HALVES == 2) {
                     const float4 sr = lds4(a), si = lds4(a + hsB);
                     const float4 orr = lds4(a + lwB), oi = lds4(a + lwB + hsB);
-                    Q0r[it] = f4fma(pi[it], oi, pr[it] * orr);
-                    Q0i[it] = pr[it] * oi - pi[it] * orr;
-                    Q1r[it] = sr * pr[it] - si * pi[it];
-                    Q1i[it] = f4fma(sr, pi[it], si * pr[it]);
+                    query_subj<2>(pr[it], pi[it], orr, oi, Q0r[it], Q0i[it]);
+                    query_obj<2>(sr, si, pr[it], pi[it], Q1r[it], Q1i[it]);
                     acc = f4fma(sr, Q0r[it], acc);
                     acc = f4fma(si, Q0i[it], acc);
                     W0i[it] = W1i[it] = f4zero();
                 } else {
                     const float4 vs = lds4(a), vo = lds4(a + lwB);
-                    Q0r[it] = pr[it] * vo;
-                    Q1r[it] = vs * pr[it];
+                    query_subj<1>(pr[it], pi[it], vo, vo, Q0r[it], Q0i[it]);
+                    query_obj<1>(vs, vs, pr[it], pi[it], Q1r[it], Q1i[it]);
                     acc = f4fma(vs, Q0r[it], acc);
                 }
                 W0r[it] = W1r[it] = f4zero();
@@ -248,6 +262,14 @@ __global__ void __launch_bounds__(THREADS) kge_train_res_kernel(const TrainParam
             dP = p.dpos[i];
         }
         __syncwarp();
+        if constexpr (GATHER) {
+            if (lane < eta) {  // the g of red_row below, handed to the bucket sum
+                p.bk.g[bk_at] = scale * lds_f(sc_s + 4u * (uint32_t)slot);
+                p.bk.eid[bk_at] = repl;
+                p.bk.other[bk_at] = keep ? s_id : o_id;
+                p.bk.rel[bk_at] = p_id | (keep ? (int)0x80000000u : 0);
+            }
+        }
 
         // ---- pass B: gradient rows of the replaced entities, two rows of one side per trip; W += g * row ----
         // gradient REDs of one replaced row: g * Q at the lane's chunks.  One 64-bit base per half; chunk it sits 512*it bytes
@@ -259,8 +281,8 @@ __global__ void __launch_bounds__(THREADS) kge_train_res_kernel(const TrainParam
 #pragma unroll
             for (int it = 0; it < NIT; ++it) {
                 if (!live[it]) break;
-                red_add_v4(reinterpret_cast<float *>(g0 + 512 * it), g * qr[it]);
-                if constexpr (HALVES == 2) red_add_v4(reinterpret_cast<float *>(g1 + 512 * it), g * qi[it]);
+                red_repl_v4(reinterpret_cast<float *>(g0 + 512 * it), g * qr[it]);
+                if constexpr (HALVES == 2) red_repl_v4(reinterpret_cast<float *>(g1 + 512 * it), g * qi[it]);
             }
         };
         auto grad_side = [&](int lo, int hi, const float4(&qr)[NIT], const float4(&qi)[NIT], float4(&Wr)[NIT], float4(&Wi)[NIT]) {
@@ -283,8 +305,10 @@ __global__ void __launch_bounds__(THREADS) kge_train_res_kernel(const TrainParam
                         Wi[it] = f4fma(gb, bi, Wi[it]);
                     }
                 }
-                red_row(ida, ga, qr, qi);
-                if (has_b) red_row(idb, gb, qr, qi);
+                if constexpr (!GATHER) {
+                    red_row(ida, ga, qr, qi);
+                    if (has_b) red_row(idb, gb, qr, qi);
+                }
             }
         };
         grad_side(0, n0, Q0r, Q0i, W0r, W0i);
@@ -352,7 +376,7 @@ template <int HALVES, int NIT>
 static cudaError_t launch_res(const TrainParams &p, int sm_count, int threads, size_t smem, cudaStream_t st)
 {
     constexpr int THREADS = KGE_TRAIN_THREADS(KGE_COMPLEX, NIT);
-    auto kern = kge_train_res_kernel<HALVES, NIT, THREADS>;
+    auto kern = p.bk.g ? kge_train_res_kernel<HALVES, NIT, THREADS, true> : kge_train_res_kernel<HALVES, NIT, THREADS, false>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     int occ = 0;

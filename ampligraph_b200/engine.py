@@ -165,6 +165,16 @@ class KGEEngine:
             _lib.check(self.lib.kge_set_row_stash(self.h, _ptr(self.row_stash), need))
         return self.row_stash
 
+    def ensure_train_workspace(self, B):
+        """The training workspace kge_train_step uses to sum the replaced entities' gradient rows per entity
+        (kge_set_train_workspace): one cached buffer, grown with B; nothing where the library's path does not apply.
+        Returns whether a fused step of B positives takes that path."""
+        need = int(self.lib.kge_train_workspace_bytes(self.h, int(B)))
+        if need > 0 and (getattr(self, "_train_ws", None) is None or self._train_ws.numel() < need):
+            self._train_ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+            _lib.check(self.lib.kge_set_train_workspace(self.h, _ptr(self._train_ws), need, self._stream()))
+        return need > 0
+
     def set_hot_entities(self, triples=None, ids=None):
         """Hot-entity hint (kge_set_hot_entities): the two most frequent subject/object ids of `triples` (numpy / torch
         [N,3] of indexed triples) or explicit `ids`; None/empty clears it."""
@@ -222,12 +232,14 @@ class KGEEngine:
             neg_ent, neg_keep = negatives
             assert neg_ent.dtype == torch.int32 and neg_keep.dtype == torch.uint8
             assert neg_ent.numel() == B * self.eta and neg_keep.numel() == B * self.eta
+        bucketed = mode != _lib.STEP_FORWARD_ONLY and self.ensure_train_workspace(B)
         _lib.check(self.lib.kge_train_step(
             self.h, mode, _ptr(self.ent), _ptr(self.rel), _ptr(self.g_ent), _ptr(self.g_rel), _ptr(triples), B,
             _ptr(neg_ent), _ptr(neg_keep), int(seed), int(step), _ptr(self.loss_acc), _ptr(scores_pos),
             _ptr(scores_neg), _ptr(dpos), _ptr(dneg), self._stream()))
         self._last_step = int(step)
-        self.launches += 2 if self.scoring_type == "RotatE" else 1
+        # RotatE: rotation table + kernel; bucketed: count, two scan launches, kernel, bucket sum
+        self.launches += 2 if self.scoring_type == "RotatE" else 5 if bucketed else 1
 
     def _one_block(self):
         """True when tables, gradients and slots still ARE the [ent | rel] blocks allocated here (callers may rebind them: the

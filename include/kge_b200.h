@@ -228,6 +228,18 @@ int kge_set_row_stash(kge_handle *h, float *stash_dev, int64_t rows);
  * 3.2) the imbalance the hint cures does not arise and it is ignored (measured: it would cost 7 %).  The reference has no
  * counterpart (TensorFlow's unsorted_segment_sum deduplicates all rows, optimizers.py:166 -> legacy apply_gradients). */
 int kge_set_hot_entities(kge_handle *h, const int32_t *ids_host, int32_t n);
+/* Optional training workspace for kge_train_step (results are unchanged up to fp32 summation order).  Where the
+ * resident trilinear kernel runs (DistMult / ComplEx / HolE, eta <= 32, one table), a step replaces every entity at least
+ * once on average (eta*B >= n_ent: the per-entity sum only pays where replaced entities repeat) and a workspace of at least
+ * kge_train_workspace_bytes(h, B) bytes is set, a fused step sums the gradient rows of the replaced entities per entity
+ * (bucket the eta*B corruptions by replaced entity, then one warp forms each entity's row and adds it once) instead of
+ * scattering every corruption's row with atomics; DESIGN.md 3.2.  kge_train_workspace_bytes returns 0 where the path
+ * does not apply.  kge_set_train_workspace zeroes the first bytes of the buffer on `stream`; afterwards the library keeps
+ * them zero between steps, so the buffer must not be used for anything else (ws_dev = NULL detaches it).  16-byte
+ * aligned.  The environment variable KGE_B200_TRAIN_REPL=scatter keeps the atomic scatter for A/B runs (and makes
+ * kge_train_workspace_bytes return 0). */
+int64_t kge_train_workspace_bytes(const kge_handle *h, int64_t B);
+int kge_set_train_workspace(kge_handle *h, void *ws_dev, int64_t bytes, void *stream);
 /* 1 when all 3+eta row windows of a positive stay in shared memory (single gather, the stash is never
  * used), 0 when the kernel works in negative groups / column windows, -1 for a NULL handle. */
 int kge_rows_resident(const kge_handle *h);

@@ -23,6 +23,7 @@ STRATEGIES = {"worst": 0, "best": 1, "middle": 2}
 STEP_FUSED, STEP_FORWARD_ONLY, STEP_BACKWARD_EXT = 0, 1, 2
 RANK_MODES = {"auto": 0, "exact": 1}
 INIT_KINDS = {"uniform": 0, "normal": 1, "truncated_normal": 2, "constant": 3}
+METRICS = {"euclidean": 0, "manhattan": 1}
 ABI_VERSION = 2
 
 
@@ -100,6 +101,12 @@ PROTOTYPES = {
     "kge_topk_workspace_bytes": (C.c_int64, [_P, C.c_int64, C.c_int64, C.c_int32]),
     "kge_select_topk": (C.c_int, [_P, _P, C.c_int64, C.c_int64, C.c_int32, _P, _P, _P, C.c_int64, _P]),
     "kge_select_topk_workspace_bytes": (C.c_int64, [_P, C.c_int64, C.c_int64, C.c_int32]),
+    "kge_knn": (C.c_int, [_P, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int64, _P, C.c_int64, C.c_int64, _P, _P,
+                          C.c_int64, C.c_int32, C.c_int32, _P, _P, _P, C.c_int64, _P]),
+    "kge_knn_workspace_bytes": (C.c_int64, [_P, C.c_int64, C.c_int64, C.c_int32, C.c_int32]),
+    "kge_radius_neighbors": (C.c_int, [_P, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int64, _P, C.c_int64, C.c_int64,
+                                       C.c_float, _P, _P, _P, C.c_int64, _P]),
+    "kge_radius_workspace_bytes": (C.c_int64, [_P, C.c_int64, C.c_int64, C.c_int32]),
 }
 
 _lib = None

@@ -7,6 +7,7 @@
 #include <new>
 
 #include "kge_internal.h"
+#include "kge_rank_common.cuh"  // the OP_* chains kge_knn / kge_radius_neighbors choose by metric
 
 using namespace kge;
 
@@ -1120,5 +1121,168 @@ extern "C" int kge_select_topk(kge_handle *h, const float *scores_dev, int64_t b
     s.state = l.state;
     KGE_CUDA(launch_topk_select(s, st), "kge_select_topk: select");
     KGE_CUDA(launch_topk_write(l.state, l.keys, l.vals, b, k, nullptr, 0, pos_dev, out_dev, st), "kge_select_topk: write");
+    return KGE_OK;
+}
+
+// ---- nearest-neighbour and radius search over a point matrix ----------------------------------------------------
+// Scratch of kge_knn / kge_radius_neighbors: the gathered query rows, the (unused) rank counters the scoring kernels
+// update, one [b, C] chunk of -d (C: the kge_topk rule), then the running lists (kge_knn) or the per-row cursors
+// (kge_radius_neighbors).
+struct KnnWorkspace {
+    float *qvec;     // [b, ld]
+    int32_t *cnt;    // [b, 4]: three counters + the zero "positive" of each query
+    float *chunk;    // [b, C]
+    TopkLists l;     // kge_knn
+    long long *cursor;  // [b] kge_radius_neighbors
+    size_t bytes;
+};
+static KnnWorkspace carve_knn_workspace(const kge_handle *h, void *base, int64_t b, int64_t n_cand, int32_t k, int32_t ld)
+{
+    KnnWorkspace w;
+    memset(&w, 0, sizeof(w));
+    char *p = (char *)base;
+    size_t off = 0;
+    w.qvec = (float *)(p + off); off += align256((size_t)b * ld * sizeof(float));
+    w.cnt = (int32_t *)(p + off); off += align256((size_t)4 * b * sizeof(int32_t));
+    w.chunk = (float *)(p + off); off += align256((size_t)b * topk_chunk(h, b, n_cand) * sizeof(float));
+    if (k > 0) {
+        w.l = carve_topk_lists(base, off, b, k);
+        off = w.l.bytes;
+    } else {
+        w.cursor = (long long *)(p + off); off += align256((size_t)b * sizeof(long long));
+    }
+    w.bytes = off;
+    return w;
+}
+
+extern "C" int64_t kge_knn_workspace_bytes(const kge_handle *h, int64_t b, int64_t n_cand, int32_t k, int32_t ld)
+{
+    if (!h || b < 0 || n_cand < 0 || k < 1 || ld < 4 || ld % 4) return 0;
+    return (int64_t)carve_knn_workspace(h, nullptr, b, n_cand, k, ld).bytes;
+}
+
+extern "C" int64_t kge_radius_workspace_bytes(const kge_handle *h, int64_t b, int64_t n_cand, int32_t ld)
+{
+    if (!h || b < 0 || n_cand < 0 || ld < 4 || ld % 4) return 0;
+    return (int64_t)carve_knn_workspace(h, nullptr, b, n_cand, 0, ld).bytes;
+}
+
+// the checks kge_knn and kge_radius_neighbors share (b > 0)
+static int check_points(const char *fn, int32_t metric, const float *points_dev, int64_t n_points, int32_t ld,
+                        const int32_t *query_ids_dev, const int32_t *cand_ids_dev, int64_t cand_begin, int64_t n_cand)
+{
+    if (metric != KGE_METRIC_EUCLIDEAN && metric != KGE_METRIC_MANHATTAN)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "%s: unknown metric %d", fn, metric);
+    if (ld < 4 || ld % 4) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: ld must be a positive multiple of 4, got %d", fn, ld);
+    if (n_points > 0x7fffffffLL) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: ids are int32 (n_points < 2^31)", fn);
+    if (!points_dev || !query_ids_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: null pointer", fn);
+    if (((uintptr_t)points_dev & 15u) != 0) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: points_dev must be 16-byte aligned", fn);
+    if (cand_ids_dev && cand_begin != 0) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: cand_begin must be 0 with cand_ids_dev", fn);
+    if (!cand_ids_dev && cand_begin + n_cand > n_points)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "%s: candidate range [%lld,%lld) exceeds n_points %lld", fn, (long long)cand_begin,
+                    (long long)(cand_begin + n_cand), (long long)n_points);
+    return KGE_OK;
+}
+
+static RankParams knn_rank_params(int32_t ld, const float *points_dev, const KnnWorkspace &w, int64_t b)
+{
+    RankParams p;
+    memset(&p, 0, sizeof(p));
+    p.L.model = KGE_TRANSE;  // not read: the op is explicit, and the non-RotatE kernels read only L.ld
+    p.L.k = p.L.kp = p.L.ld = p.L.K = ld;
+    p.L.halves = 1;
+    p.strategy = KGE_RANK_WORST;
+    p.ent = points_dev;
+    p.qvec = w.qvec;
+    p.qpos = w.cnt + 3 * b;
+    p.b = b;
+    p.scale = 1.f;
+    p.scores = w.chunk;
+    return p;
+}
+
+extern "C" int kge_knn(kge_handle *h, int32_t metric, const float *points_dev, int64_t n_points, int32_t ld,
+                       const int32_t *query_ids_dev, int64_t b, const int32_t *cand_ids_dev, int64_t cand_begin, int64_t n_cand,
+                       const int64_t *filt_off_dev, const int32_t *filt_idx_dev, int64_t n_filt, int32_t k, int32_t farthest,
+                       int32_t *ids_dev, float *dist_dev, void *workspace_dev, int64_t workspace_bytes, void *stream)
+{
+    KGE_CHECK_HANDLE(h, "kge_knn");
+    if (k < 1) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_knn: k must be >= 1, got %d", k);
+    if (b < 0 || n_points < 0 || n_cand < 0 || cand_begin < 0 || n_filt < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_knn: negative size");
+    if (n_cand > 0x7fffffffLL) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_knn: n_cand must be < 2^31");
+    if (b == 0) return KGE_OK;
+    if (int rc = check_points("kge_knn", metric, points_dev, n_points, ld, query_ids_dev, cand_ids_dev, cand_begin, n_cand)) return rc;
+    if (!ids_dev || !dist_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_knn: null pointer");
+    if ((filt_off_dev == nullptr || filt_idx_dev == nullptr) && n_filt > 0)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_knn: filter offsets and indices must be given together");
+    if (int rc = check_topk_workspace(workspace_dev, workspace_bytes, kge_knn_workspace_bytes(h, b, n_cand, k, ld), "kge_knn")) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    const KnnWorkspace w = carve_knn_workspace(h, workspace_dev, b, n_cand, k, ld);
+    KGE_CUDA(launch_knn_gather(points_dev, ld, query_ids_dev, b, w.qvec, st), "kge_knn: gather");
+    KGE_CUDA(cudaMemsetAsync(w.cnt, 0, (size_t)4 * b * sizeof(int32_t), st), "kge_knn: memset");
+    KGE_CUDA(cudaMemsetAsync(w.l.state, 0, (size_t)b * sizeof(int2), st), "kge_knn: memset");
+    RankParams p = knn_rank_params(ld, points_dev, w, b);
+    const int op = metric == KGE_METRIC_EUCLIDEAN ? OP_L2_SUB : OP_L1_SUB;
+    TopkSelectParams s;
+    memset(&s, 0, sizeof(s));
+    s.scores = w.chunk;
+    s.b = b;
+    s.k = k;
+    if (n_filt > 0) { s.filt_off = (const long long *)filt_off_dev; s.filt_idx = filt_idx_dev; }
+    s.filt_shift = cand_ids_dev ? 0 : cand_begin;
+    s.keys = w.l.keys;
+    s.vals = w.l.vals;
+    s.state = w.l.state;
+    const int64_t C = topk_chunk(h, b, n_cand);
+    for (int64_t c0 = 0; c0 < n_cand; c0 += C) {
+        const int64_t nc = n_cand - c0 < C ? n_cand - c0 : C;
+        p.cand_ids = cand_ids_dev ? cand_ids_dev + c0 : nullptr;
+        p.cand_begin = cand_ids_dev ? 0 : cand_begin + c0;
+        p.n_cand = nc;
+        KGE_CUDA(launch_rank_count_op(p, op, w.cnt, st), "kge_knn: distances");  // -d, [b, nc]
+        if (farthest) KGE_CUDA(launch_knn_negate(w.chunk, b * nc, st), "kge_knn: negate");
+        s.ld = nc;
+        s.n = nc;
+        s.base = c0;
+        KGE_CUDA(launch_topk_select(s, st), "kge_knn: select");
+    }
+    KGE_CUDA(launch_topk_write(w.l.state, w.l.keys, w.l.vals, b, k, cand_ids_dev, cand_begin, ids_dev, dist_dev, st, !farthest),
+             "kge_knn: write");
+    return KGE_OK;
+}
+
+extern "C" int kge_radius_neighbors(kge_handle *h, int32_t metric, const float *points_dev, int64_t n_points, int32_t ld,
+                                    const int32_t *query_ids_dev, int64_t b, const int32_t *cand_ids_dev, int64_t cand_begin,
+                                    int64_t n_cand, float radius, int64_t *offsets_dev, int32_t *nbr_dev,
+                                    void *workspace_dev, int64_t workspace_bytes, void *stream)
+{
+    KGE_CHECK_HANDLE(h, "kge_radius_neighbors");
+    if (b < 0 || n_points < 0 || n_cand < 0 || cand_begin < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_radius_neighbors: negative size");
+    if (n_cand > 0x7fffffffLL) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_radius_neighbors: n_cand must be < 2^31");
+    if (b == 0) return KGE_OK;
+    if (int rc = check_points("kge_radius_neighbors", metric, points_dev, n_points, ld, query_ids_dev, cand_ids_dev, cand_begin, n_cand))
+        return rc;
+    if (!offsets_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_radius_neighbors: null pointer");
+    if (int rc = check_topk_workspace(workspace_dev, workspace_bytes, kge_radius_workspace_bytes(h, b, n_cand, ld), "kge_radius"))
+        return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    const KnnWorkspace w = carve_knn_workspace(h, workspace_dev, b, n_cand, 0, ld);
+    KGE_CUDA(launch_knn_gather(points_dev, ld, query_ids_dev, b, w.qvec, st), "kge_radius_neighbors: gather");
+    KGE_CUDA(cudaMemsetAsync(w.cnt, 0, (size_t)4 * b * sizeof(int32_t), st), "kge_radius_neighbors: memset");
+    KGE_CUDA(cudaMemsetAsync(w.cursor, 0, (size_t)b * sizeof(long long), st), "kge_radius_neighbors: memset");
+    RankParams p = knn_rank_params(ld, points_dev, w, b);
+    const int op = metric == KGE_METRIC_EUCLIDEAN ? OP_L2_SUB : OP_L1_SUB;
+    const long long *off = nbr_dev ? (const long long *)offsets_dev : nullptr;
+    const int64_t C = topk_chunk(h, b, n_cand);
+    for (int64_t c0 = 0; c0 < n_cand; c0 += C) {
+        const int64_t nc = n_cand - c0 < C ? n_cand - c0 : C;
+        p.cand_ids = cand_ids_dev ? cand_ids_dev + c0 : nullptr;
+        p.cand_begin = cand_ids_dev ? 0 : cand_begin + c0;
+        p.n_cand = nc;
+        KGE_CUDA(launch_rank_count_op(p, op, w.cnt, st), "kge_radius_neighbors: distances");  // -d, [b, nc]
+        KGE_CUDA(launch_radius_chunk(w.chunk, nc, nc, c0, b, radius, cand_ids_dev, cand_begin, w.cursor, off, nbr_dev, st),
+                 nbr_dev ? "kge_radius_neighbors: emit" : "kge_radius_neighbors: count");
+    }
+    if (!nbr_dev) KGE_CUDA(launch_radius_counts(w.cursor, b, (long long *)offsets_dev, st), "kge_radius_neighbors: counts");
     return KGE_OK;
 }

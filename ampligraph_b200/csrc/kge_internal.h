@@ -154,6 +154,9 @@ cudaError_t launch_rank_prepare(const Layout &L, const ShardView &sv, const floa
                                 float *qaux, int32_t *qpos, cudaStream_t st);
 // cnt = [b,3] int32 workspace: #(qpos < qc), #(qpos == qc), #filtered
 cudaError_t launch_rank_count(const RankParams &p, int32_t *cnt, cudaStream_t st);
+// the same with the chain chosen by the caller (an OP_* of kge_rank_common.cuh) instead of by (model, side):
+// kge_knn / kge_radius_neighbors score points with OP_L2_SUB / OP_L1_SUB; only p.L.ld is read for the non-RotatE ops
+cudaError_t launch_rank_count_op(const RankParams &p, int op, int32_t *cnt, cudaStream_t st);
 cudaError_t launch_rank_filter_n(const RankParams &p, const long long *filt_off, const int32_t *filt_idx,
                                  long long n_pairs, int32_t *cnt, int sm_count, cudaStream_t st);
 cudaError_t launch_rank_finalize(const int32_t *cnt, long long b, int strategy, int32_t *ranks, cudaStream_t st);
@@ -173,8 +176,25 @@ struct TopkSelectParams {
     int2 *state;                         // [b] {entries, current buffer}; zero before the first chunk
 };
 cudaError_t launch_topk_select(const TopkSelectParams &p, cudaStream_t st);
+// negate: write -value (padding +inf) instead of the stored value (padding -inf)
 cudaError_t launch_topk_write(const int2 *state, const unsigned long long *keys, const float *vals, long long b, int k,
-                              const int32_t *cand_ids, long long cand_begin, int32_t *ids, float *out, cudaStream_t st);
+                              const int32_t *cand_ids, long long cand_begin, int32_t *ids, float *out, cudaStream_t st,
+                              bool negate = false);
+
+// kge_knn.cu: nearest-neighbour and radius search over the rows of a point matrix (scored by launch_rank_count_op)
+// qvec[i, :] = points[query_ids[i], :] for i < b (ld floats, ld % 4 == 0)
+cudaError_t launch_knn_gather(const float *points, int ld, const int32_t *query_ids, long long b, float *qvec, cudaStream_t st);
+// x = -x over n floats (farthest: turns the chunk's -d into +d, so the select keeps the largest distances)
+cudaError_t launch_knn_negate(float *x, long long n, cudaStream_t st);
+// one CTA per query row of a [b, ld] chunk of -d scores, columns [0, n) = candidate positions base + c:
+// off == nullptr (count): cursor[q] += #{c : d <= radius};
+// off != nullptr (emit): the positions' ids (cand_ids[pos] or cand_begin + pos) go to nbr[off[q] + cursor[q] ...] in
+// ascending position order and cursor[q] advances (writes beyond off[q + 1] are dropped)
+cudaError_t launch_radius_chunk(const float *chunk, long long ld, long long n, long long base, long long b, float radius,
+                                const int32_t *cand_ids, long long cand_begin, long long *cursor, const long long *off,
+                                int32_t *nbr, cudaStream_t st);
+// offsets[0] = 0, offsets[1 + q] = cursor[q]
+cudaError_t launch_radius_counts(const long long *cursor, long long b, long long *offsets, cudaStream_t st);
 
 // kge_rank_tc.cu: tensor-core filter + exact refine for the bilinear models
 struct RankTcLayout {  // carve-up of the tensor-core part of the caller's workspace

@@ -153,7 +153,9 @@ __global__ void __launch_bounds__(TK_THREADS) kge_topk_select_kernel(const TopkS
 }
 
 // [b, k] outputs of the running lists: ids (cand_ids[pos], or cand_begin + pos; pos itself for kge_select_topk) and raw
-// scores; rows with fewer than k eligible candidates are padded with id -1, score -inf.
+// scores; rows with fewer than k eligible candidates are padded with id -1, score -inf.  NEG: every value is written
+// negated, padding included (+inf) -- kge_knn stores -d to find the nearest points and reports d.
+template <bool NEG>
 __global__ void kge_topk_write_kernel(const int2 *__restrict__ state, const unsigned long long *__restrict__ keys,
                                       const float *__restrict__ vals, long long b, int k, const int32_t *__restrict__ cand_ids,
                                       long long cand_begin, int32_t *__restrict__ ids, float *__restrict__ out)
@@ -167,10 +169,10 @@ __global__ void kge_topk_write_kernel(const int2 *__restrict__ state, const unsi
         const size_t src = (size_t)st.y * b * k + i;
         const long long pos = topk_pos(keys[src]);
         ids[i] = cand_ids ? cand_ids[pos] : (int32_t)(cand_begin + pos);
-        out[i] = vals[src];
+        out[i] = NEG ? -vals[src] : vals[src];
     } else {
         ids[i] = -1;
-        out[i] = -INFINITY;
+        out[i] = NEG ? INFINITY : -INFINITY;
     }
 }
 
@@ -182,11 +184,13 @@ cudaError_t launch_topk_select(const TopkSelectParams &p, cudaStream_t st)
 }
 
 cudaError_t launch_topk_write(const int2 *state, const unsigned long long *keys, const float *vals, long long b, int k,
-                              const int32_t *cand_ids, long long cand_begin, int32_t *ids, float *out, cudaStream_t st)
+                              const int32_t *cand_ids, long long cand_begin, int32_t *ids, float *out, cudaStream_t st,
+                              bool negate)
 {
     const long long n = b * k;
     if (n == 0) return cudaSuccess;
-    kge_topk_write_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(state, keys, vals, b, k, cand_ids, cand_begin, ids, out);
+    auto kern = negate ? kge_topk_write_kernel<true> : kge_topk_write_kernel<false>;
+    kern<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(state, keys, vals, b, k, cand_ids, cand_begin, ids, out);
     return cudaGetLastError();
 }
 

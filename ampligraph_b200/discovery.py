@@ -7,9 +7,16 @@
   top_n leave it.  Relation completion scores the R completed triples with the kernel predict uses and orders them
   with kge_select_topk.
 * query_topn_batch  -- extension: many (s, p, ?) or (?, p, o) queries in one call, optionally filtered like evaluate.
+* find_nearest_neighbours -- discovery.find_nearest_neighbours (discovery.py:1171-1244): the n_neighbors nearest
+  entities of each given entity in embedding space, one kge_knn call per batch of queries instead of sklearn
+  NearestNeighbors on the host.
+* find_duplicates   -- discovery.find_duplicates (discovery.py:714-982): groups of entities, relations or triples whose
+  embeddings lie within a tolerance of each other.  tolerance='auto' runs the reference's bisection over the duplicate
+  fraction, evaluated on the host from one nearest-other-row kge_knn pass instead of one radius self-join per step.
 
-Order of the results (both functions): score descending; equal scores by candidate position ascending (the order of
-ents_to_consider / rels_to_consider, or of the entity / relation ids); NaN before +inf (DESIGN.md 3.6).
+Order of the link-prediction results: score descending; equal scores by candidate position ascending (the order of
+ents_to_consider / rels_to_consider, or of the entity / relation ids); NaN before +inf (DESIGN.md 3.6).  Distances are
+the canonical fp32 chains of kge_knn (DESIGN.md 3.7), equal distances again by candidate position.
 """
 import logging
 
@@ -17,6 +24,7 @@ import numpy as np
 import torch
 
 from .datasets import DataIndexer, FilterIndex, as_triple_array
+from .engine import fp32_floor
 
 logger = logging.getLogger(__name__)
 
@@ -199,3 +207,163 @@ def query_topn_batch(model, X, side="o", top_n=10, use_filter=False, ents_to_con
         labels[start:start + len(qb)] = _labels(model, ids.cpu().numpy(), "e")
         scores[start:start + len(qb)] = val.cpu().numpy()
     return labels, scores
+
+
+# sklearn metric names -> the two chains kge_knn implements ('minkowski' is sklearn's default, p = 2)
+_METRICS = {"euclidean": "euclidean", "l2": "euclidean", "minkowski": "euclidean",
+            "manhattan": "manhattan", "l1": "manhattan", "cityblock": "manhattan"}
+
+
+def _metric(metric):
+    if isinstance(metric, str) and metric in _METRICS:
+        return _METRICS[metric]
+    raise NotImplementedError("metric {!r} is not supported: the distances are computed on the GPU, which implements "
+                              "{}".format(metric, ", ".join(sorted(_METRICS))))
+
+
+def _check_finite(points):
+    if not bool(torch.isfinite(points).all()):
+        raise ValueError("Input contains NaN or infinity: the embeddings are not finite.")
+
+
+def _query_batches(n, k):
+    """[start, stop) ranges of queries per kge_knn call: as query_topn_batch, bounded by the running lists' share."""
+    chunk = max(1, min(_BATCH_QUERIES, _LIST_BYTES // (24 * max(int(k), 1))))
+    return [(s, min(s + chunk, n)) for s in range(0, n, chunk)]
+
+
+def find_nearest_neighbours(kge_model, entities, n_neighbors=10, entities_subset=None, metric="euclidean"):
+    """discovery.find_nearest_neighbours (discovery.py:1171-1244): the n_neighbors nearest entities of each of
+    `entities` in embedding space, among all entities (in id order) or among entities_subset (in its order).
+
+    Returns (neighbors [len(entities), n_neighbors] labels, distances [len(entities), n_neighbors] fp32), each row
+    distance ascending, equal distances in candidate order.  As with sklearn's kneighbors(X), an entity is not excluded
+    from its own neighbours.  metric: 'euclidean' / 'l2' / 'minkowski' or 'manhattan' / 'l1' / 'cityblock'; anything
+    else raises NotImplementedError.  Distances are the canonical fp32 chains (DESIGN.md 3.7)."""
+    if not kge_model.is_fitted:  # :1219-1225
+        raise AssertionError("KGE model is not fit!")
+    if not isinstance(entities, (list, np.ndarray)):
+        raise AssertionError("Invalid type for entities! Must be a list or np.array")
+    if entities_subset is not None and not isinstance(entities_subset, (list, np.ndarray)):
+        raise AssertionError("Invalid type for entities_subset! Must be a list or np.array")
+    eng = _check_fitted(kge_model)
+    cand, n_cand = None, _count(kge_model, "e")
+    if entities_subset is not None:
+        sub = _ids(kge_model, entities_subset, "e")
+        if (sub < 0).any():
+            raise _error("Entities in `entities_subset` have not been seen by the model.")
+        cand, n_cand = _dev(eng, sub, np.int32), len(sub)
+    if not n_neighbors < n_cand:  # :1233
+        raise AssertionError("n_neighbors must be less than the number of entities being fit!")
+    if int(n_neighbors) < 1:
+        raise ValueError("Expected n_neighbors > 0. Got {}".format(n_neighbors))
+    metric = _metric(metric)
+    q = _ids(kge_model, entities, "e")
+    if (q < 0).any():
+        raise _error("Entities in `entities` have not been seen by the model.")
+    qd = _dev(eng, q, np.int32)
+    _check_finite(eng.ent[qd.long()])
+    _check_finite(eng.ent[:n_cand] if cand is None else eng.ent[cand.long()])
+
+    k = int(n_neighbors)
+    labels = np.empty((len(q), k), dtype=object)
+    dist = np.empty((len(q), k), np.float32)
+    for start, stop in _query_batches(len(q), k):
+        ids, d = eng.knn(eng.ent, qd[start:stop], k, metric, cand_ids=cand, n_cand=n_cand)
+        labels[start:stop] = _labels(kge_model, ids.cpu().numpy(), "e")
+        dist[start:stop] = d.cpu().numpy()
+    return np.array(labels.tolist()).reshape(len(q), k), dist
+
+
+def duplicate_fraction(d1, keys):
+    """The duplicate fraction of find_duplicates as a function of the tolerance, from the nearest-other-row distances.
+
+    d1[i] = min over rows j != i of d(i, j) (fp32), keys[i] = the label of row i (hashable).  Row i has a radius
+    neighbour other than itself iff d1[i] <= tol, and d is symmetric, so the union of the reference's duplicate sets
+    (discovery.py:961) is the set of labels of the rows with d1 <= tol: fraction(tol) = that many labels / len(d1).
+    Returns fraction(tol), evaluated by a binary search over the per-label minimum of d1."""
+    d1 = np.asarray(d1, np.float64)
+    group = {}
+    g = np.fromiter((group.setdefault(key, len(group)) for key in keys), np.int64, len(d1))
+    per_label = np.full(len(group), np.inf)
+    np.minimum.at(per_label, g, d1)
+    per_label.sort()
+    n = len(d1)
+    return lambda tol: int(np.searchsorted(per_label, tol, side="right")) / n
+
+
+def find_duplicates(X, model, mode="e", metric="l2", tolerance="auto", expected_fraction_duplicates=0.1, verbose=False):
+    """discovery.find_duplicates (discovery.py:714-982): the groups of rows of X whose embeddings lie within
+    `tolerance` of each other -> (set of frozensets of labels (mode 't': of triples as tuples), tolerance).
+
+    mode 'e' / 'r': X is an array of entities / relations; 't': X is [n, 3] triples, embedded as the concatenation of
+    the subject, predicate and object rows.  metric as in find_nearest_neighbours.  tolerance='auto' searches it with
+    the reference's bisection (scipy.optimize.bisect over [0, largest pairwise euclidean distance], xtol 1e-3, 50
+    iterations) for expected_fraction_duplicates; each step is evaluated on the host from one kge_knn pass that finds
+    every row's nearest other row (duplicate_fraction).  The duplicates themselves come from one kge_radius_neighbors
+    self-join at the final tolerance: d <= tolerance, inclusive, with the same fp32 d as the bisection saw."""
+    from scipy import optimize
+
+    if getattr(model, "is_backward", False):
+        model = model.model
+    if not model.is_fitted:  # :891-894
+        raise _error("Model has not been fitted.")
+    modes = ("t", "e", "r")
+    if mode not in modes:
+        raise _error("Argument `mode` must be one of the following: {}.".format(", ".join(modes)))
+    X = np.asarray(X)
+    if mode == "t" and (len(X.shape) != 2 or X.shape[1] != 3):
+        raise _error("For 't' mode the input X must be a matrix with three columns.")
+    if mode in ("e", "r") and len(X.shape) != 1:
+        raise _error("For 'e' or 'r' mode the input X must be an array.")
+    metric = _metric(metric)
+    eng = _check_fitted(model)
+
+    def rows(values, kind):
+        ids = _ids(model, values, kind)
+        if (ids < 0).any():
+            raise _error("{} in X have not been seen by the model.".format("Entities" if kind == "e" else "Relations"))
+        return _dev(eng, ids, np.int64)
+
+    if mode == "t":
+        points = torch.cat([eng.ent[rows(X[:, 0], "e")], eng.rel[rows(X[:, 1], "r")], eng.ent[rows(X[:, 2], "e")]], 1)
+    else:
+        points = (eng.ent if mode == "e" else eng.rel)[rows(X, mode)]
+    points = points.contiguous()
+    _check_finite(points)
+    n = len(X)
+    every = torch.arange(n, dtype=torch.int32, device=eng.device)
+
+    if tolerance == "auto":
+        d1 = np.empty(n, np.float32)
+        max_distance = 0.0
+        for start, stop in _query_batches(n, 1):
+            q = every[start:stop]
+            # each row's own position is excluded: the nearest OTHER row (a repeated label counts at distance 0)
+            off = torch.arange(stop - start + 1, dtype=torch.int64, device=eng.device)
+            _, d = eng.knn(points, q, 1, metric, n_cand=n, filt_off=off, filt_idx=q)
+            d1[start:stop] = d[:, 0].cpu().numpy()
+            # the bracket of :972, spatial.distance_matrix: euclidean whatever the metric
+            _, far = eng.knn(points, q, 1, "euclidean", n_cand=n, farthest=True)
+            max_distance = max(max_distance, float(far.max()))
+        fraction = duplicate_fraction(d1, [tuple(r) for r in X] if mode == "t" else X.tolist())
+
+        def opt(tol, info):  # :953-969
+            fraction_duplicates = fraction(tol)
+            if verbose:
+                info["Nfeval"] += 1
+                logger.info("Eval {}: tol: {}, duplicate fraction: {}".format(info["Nfeval"], tol, fraction_duplicates))
+            return fraction_duplicates - expected_fraction_duplicates
+
+        tolerance = optimize.bisect(opt, 0.0, max_distance, xtol=1e-3, maxiter=50, args=({"Nfeval": 0},))
+
+    dups = set()
+    radius = fp32_floor(tolerance)
+    for start, stop in _query_batches(n, 1):
+        off, nbr = eng.radius_neighbors(points, every[start:stop], radius, metric, n_cand=n)
+        off, nbr = off.cpu().numpy(), nbr.cpu().numpy()
+        for i in range(stop - start):
+            row = nbr[off[i]:off[i + 1]]
+            if len(row) > 1:  # :942-950
+                dups.add(frozenset(tuple(X[j]) for j in row) if mode == "t" else frozenset(X[j] for j in row))
+    return dups, tolerance

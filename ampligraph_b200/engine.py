@@ -20,6 +20,21 @@ def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
+def _metric(metric):
+    if metric not in _lib.METRICS:
+        raise ValueError("unknown metric %r; supported: %s" % (metric, ", ".join(_lib.METRICS)))
+    return _lib.METRICS[metric]
+
+
+def fp32_floor(x):
+    """The largest fp32 value not above the Python number x: for every fp32 d, d <= fp32_floor(x) iff d <= x."""
+    with np.errstate(over="ignore"):  # beyond the fp32 range: +inf, stepped down to the largest finite value
+        r = np.float32(x)
+    if float(r) > float(x):
+        r = np.nextafter(r, np.float32(-np.inf))
+    return float(r)
+
+
 _NVTX = os.environ.get("KGE_B200_NVTX", "0") == "1"
 
 
@@ -413,6 +428,54 @@ class KGEEngine:
         _lib.check(self.lib.kge_select_topk(self.h, _ptr(scores), b, n, int(k), _ptr(pos), _ptr(out), _ptr(ws), ws_bytes,
                                             self._stream()))
         return pos, out
+
+    @_traced("kge.knn")
+    def knn(self, points, query_ids, k, metric, cand_ids=None, cand_begin=0, n_cand=None, filt_off=None, filt_idx=None,
+            farthest=False):
+        """Nearest-neighbour search (kge_knn) over the rows of `points`, any [n, ld] fp32 CUDA tensor with ld % 4 == 0
+        (self.ent, self.rel or a gathered matrix): the k nearest (farthest=True: farthest) candidate rows of each row
+        query_ids[i] -> (ids int32 [b,k], distances fp32 [b,k]) on the device, distance ascending (farthest:
+        descending), ties by candidate position ascending; rows with fewer than k eligible candidates end in id -1 /
+        distance +inf (farthest: -inf).  metric: 'euclidean' | 'manhattan'.  Candidates and filter (candidate positions to
+        exclude) as in topk."""
+        assert points.dtype == torch.float32 and points.is_cuda and points.is_contiguous() and points.dim() == 2
+        assert query_ids.dtype == torch.int32 and query_ids.is_cuda and query_ids.is_contiguous()
+        b, (n_points, ld) = query_ids.numel(), points.shape
+        if n_cand is None:
+            n_cand = cand_ids.numel() if cand_ids is not None else n_points - cand_begin
+        n_filt = int(filt_idx.numel()) if filt_idx is not None else 0
+        ids = torch.empty((b, max(int(k), 0)), dtype=torch.int32, device=self.device)
+        dist = torch.empty((b, max(int(k), 0)), dtype=torch.float32, device=self.device)
+        ws, ws_bytes = self._topk_workspace(self.lib.kge_knn_workspace_bytes(self.h, b, int(n_cand), int(k), ld))
+        _lib.check(self.lib.kge_knn(self.h, _metric(metric), _ptr(points), n_points, ld, _ptr(query_ids), b, _ptr(cand_ids),
+                                    int(cand_begin), int(n_cand), _ptr(filt_off), _ptr(filt_idx), n_filt, int(k),
+                                    int(bool(farthest)), _ptr(ids), _ptr(dist), _ptr(ws), ws_bytes, self._stream()))
+        return ids, dist
+
+    @_traced("kge.radius_neighbors")
+    def radius_neighbors(self, points, query_ids, radius, metric, cand_ids=None, cand_begin=0, n_cand=None):
+        """Radius search (kge_radius_neighbors): for each row query_ids[i] of `points`, every candidate row at distance
+        d <= radius -> (offsets int64 [b+1], ids int32 [offsets[-1]]) on the device, row i's ids in ascending candidate
+        position.  d is knn's fp32 distance; radius is taken as the largest fp32 not above it, so the test is exactly
+        d <= radius for the Python number.  Two passes (count, then emit into the CSR); synchronises once for the size."""
+        assert points.dtype == torch.float32 and points.is_cuda and points.is_contiguous() and points.dim() == 2
+        assert query_ids.dtype == torch.int32 and query_ids.is_cuda and query_ids.is_contiguous()
+        b, (n_points, ld) = query_ids.numel(), points.shape
+        if n_cand is None:
+            n_cand = cand_ids.numel() if cand_ids is not None else n_points - cand_begin
+        offsets = torch.zeros(b + 1, dtype=torch.int64, device=self.device)
+        ws, ws_bytes = self._topk_workspace(self.lib.kge_radius_workspace_bytes(self.h, b, int(n_cand), ld))
+
+        def call(nbr):
+            _lib.check(self.lib.kge_radius_neighbors(self.h, _metric(metric), _ptr(points), n_points, ld, _ptr(query_ids), b,
+                                                     _ptr(cand_ids), int(cand_begin), int(n_cand), fp32_floor(radius),
+                                                     _ptr(offsets), _ptr(nbr), _ptr(ws), ws_bytes, self._stream()))
+        call(None)
+        torch.cumsum(offsets, 0, out=offsets)
+        nbr = torch.empty(int(offsets[-1]), dtype=torch.int32, device=self.device)
+        if nbr.numel() > 0:  # an empty tensor's data pointer is NULL, which would ask for another count pass
+            call(nbr)
+        return offsets, nbr
 
     def _topk_workspace(self, need):
         # need == 0: invalid arguments (k < 1, ...) -- the call itself reports them

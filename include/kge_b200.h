@@ -422,6 +422,37 @@ int kge_select_topk(kge_handle *h, const float *scores_dev, int64_t b, int64_t n
                     int32_t *pos_dev, float *out_dev, void *workspace_dev, int64_t workspace_bytes, void *stream);
 int64_t kge_select_topk_workspace_bytes(const kge_handle *h, int64_t b, int64_t n, int32_t k);
 
+/* Distances of kge_knn / kge_radius_neighbors, each a fixed chain over the columns in ascending order with query row q
+ * and candidate row x, one correctly rounded fp32 operation at a time:
+ *   euclidean: acc = +0; for c: t = q_c - x_c; acc = fma(t, t, acc); d = sqrt(acc)
+ *   manhattan: acc = +0; for c: acc = acc + |q_c - x_c|;              d = acc
+ * Zero columns present in both rows change nothing, so d over a padded table row equals d over its dense
+ * get_embeddings row; d(i, j) == d(j, i) bit for bit. */
+enum kge_metric { KGE_METRIC_EUCLIDEAN = 0, KGE_METRIC_MANHATTAN = 1 };
+
+/* sklearn NearestNeighbors.kneighbors (discovery.py:1171-1244): the k nearest (farthest = 1: farthest) of the
+ * candidate rows of points_dev [n_points, ld] (ld % 4 == 0, 16-byte aligned) for each query row query_ids_dev[i].
+ * Candidates (cand_ids_dev or [cand_begin, cand_begin + n_cand)) and the filter CSR of excluded candidate POSITIONS
+ * follow kge_topk.  ids_dev/dist_dev [b, k]: distance ascending (farthest: descending), ties by position ascending;
+ * distances bit-identical to the canonical chain; short rows padded with id -1, distance +inf (farthest: -inf).
+ * Every id on the device must be valid.  The handle supplies the device and the chunk rule of kge_topk (its model
+ * plays no part).  workspace_dev: kge_knn_workspace_bytes bytes, 1024-byte aligned, contents undefined afterwards. */
+int kge_knn(kge_handle *h, int32_t metric, const float *points_dev, int64_t n_points, int32_t ld,
+            const int32_t *query_ids_dev, int64_t b, const int32_t *cand_ids_dev, int64_t cand_begin, int64_t n_cand,
+            const int64_t *filt_off_dev, const int32_t *filt_idx_dev, int64_t n_filt, int32_t k, int32_t farthest,
+            int32_t *ids_dev, float *dist_dev, void *workspace_dev, int64_t workspace_bytes, void *stream);
+int64_t kge_knn_workspace_bytes(const kge_handle *h, int64_t b, int64_t n_cand, int32_t k, int32_t ld);
+
+/* sklearn radius_neighbors: every candidate with d <= radius (inclusive; the same d as kge_knn, bit for bit).
+ * nbr_dev == NULL: count pass, writes offsets_dev[1..b] = per-row counts (offsets_dev[0] = 0); the caller turns them
+ * into CSR offsets.  nbr_dev != NULL: offsets_dev holds the CSR offsets, nbr_dev[off[i]..off[i+1]) receives row i's
+ * candidate ids in ascending position order (deterministic; ids beyond off[i+1] are dropped). */
+int kge_radius_neighbors(kge_handle *h, int32_t metric, const float *points_dev, int64_t n_points, int32_t ld,
+                         const int32_t *query_ids_dev, int64_t b, const int32_t *cand_ids_dev, int64_t cand_begin,
+                         int64_t n_cand, float radius, int64_t *offsets_dev, int32_t *nbr_dev,
+                         void *workspace_dev, int64_t workspace_bytes, void *stream);
+int64_t kge_radius_workspace_bytes(const kge_handle *h, int64_t b, int64_t n_cand, int32_t ld);
+
 #ifdef __cplusplus
 }
 #endif

@@ -483,15 +483,19 @@ static int train_step_impl(kge_handle *h, int32_t mode, const kge_shard_map *map
     p.hot_ent[0] = h->hot_ent[0];
     p.hot_ent[1] = h->hot_ent[1];
     p.stash = (h->stash && h->stash_rows >= B * (int64_t)h->cfg.eta) ? h->stash : nullptr;
+    if (map) {
+        // the map's stamps replace the handle's for any world (a one-rank map runs the unsharded kernels, which stamp
+        // p.stamp_ent directly); all or nothing
+        p.stamp_ent = map->stamp_ent[0];
+        for (int q = 0; q < map->world; ++q) {
+            p.stamp_ent_shard[q] = map->stamp_ent[q];
+            if (!map->stamp_ent[q]) p.stamp_ent = nullptr;
+        }
+    }
     if (map && map->world > 1) {
         p.shard_world = map->world;
         p.rows_per_shard = (int)map->rows_per_shard;
         for (int q = 0; q < map->world; ++q) { p.ent_shard[q] = map->ent[q]; p.grad_ent_shard[q] = map->grad_ent[q]; }
-        p.stamp_ent = map->stamp_ent[0];
-        for (int q = 0; q < map->world; ++q) {
-            p.stamp_ent_shard[q] = map->stamp_ent[q];
-            if (!map->stamp_ent[q]) p.stamp_ent = nullptr;  // all or nothing
-        }
     }
     // KGE_B200_TRAIN_KERNEL=general keeps every shape on the general kernel (A/B runs, and the tests that cover its resident
     // trilinear instantiations); default: the specialised kernel of kge_train_res.cu where it applies

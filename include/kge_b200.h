@@ -201,7 +201,8 @@ typedef struct kge_shard_map {
     int64_t rows_per_shard;
     const float *ent[8];
     float *grad_ent[8];
-    int32_t *stamp_ent[8]; /* optional lazy-optimizer row stamps of every shard (all NULL = off) */
+    int32_t *stamp_ent[8]; /* optional lazy-optimizer row stamps of every shard (all NULL = off); for any world,
+                              world 1 included, they replace the entity stamps of kge_set_row_stamps */
 } kge_shard_map;
 
 /* kge_train_step on a row-sharded entity table: the SAME fused kernel, its bulk row gathers and

@@ -350,14 +350,21 @@ def test_train_steps_vs_oracle(opt, params, reg):
     eng.close()
 
 
-@pytest.mark.parametrize("opt", ["lazy_adam", "lazy_adagrad", "lazy_sgd"])
-def test_lazy_optimizer_matches_restatement(opt):
+LAZY_OPTS = ["lazy_adam", "lazy_adagrad", "lazy_sgd"]
+# DistMult runs the resident trilinear kernel, RotatE the RotatE kernel, ComplEx with neg_group = 3 the general kernel: each
+# stamps the rows it touches itself (DistMult keeps its original test ids)
+LAZY_CASES = ([pytest.param(opt, "DistMult", 0, id=opt) for opt in LAZY_OPTS] +
+              [pytest.param(opt, m, g, id="%s-%s" % (m, opt)) for m, g in (("RotatE", 0), ("ComplEx", 3)) for opt in LAZY_OPTS])
+
+
+@pytest.mark.parametrize("opt,model,neg_group", LAZY_CASES)
+def test_lazy_optimizer_matches_restatement(opt, model, neg_group):
     """opt-in lazy optimizer (rows touched by the step only) vs the oracle's lazy restatement; untouched
     rows must not move at all."""
     rng = np.random.default_rng(43)
-    model, E, R, k, eta, B = "DistMult", 400, 6, 12, 3, 25   # few positives: most rows stay untouched
+    E, R, k, eta, B = 400, 6, 12, 3, 25   # few positives: most rows stay untouched
     ent, rel = _tables(model, E, R, k, rng, scale=0.5)
-    eng = _engine(model, k, eta, E, R, loss="nll", optimizer=opt, optimizer_params={"learning_rate": 0.01})
+    eng = _engine(model, k, eta, E, R, loss="nll", optimizer=opt, optimizer_params={"learning_rate": 0.01}, neg_group=neg_group)
     eng.set_embeddings(ent, rel)
     rs = _ref(model, k, ent, rel, eta, "nll", {}, optimizer=opt, optimizer_params={"learning_rate": 0.01})
     touched = np.zeros(E, bool)

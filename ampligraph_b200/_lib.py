@@ -107,6 +107,11 @@ PROTOTYPES = {
     "kge_radius_neighbors": (C.c_int, [_P, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int64, _P, C.c_int64, C.c_int64,
                                        C.c_float, _P, _P, _P, C.c_int64, _P]),
     "kge_radius_workspace_bytes": (C.c_int64, [_P, C.c_int64, C.c_int64, C.c_int32]),
+    "kge_radius_union": (C.c_int, [_P, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int64, _P, C.c_int64, C.c_int64,
+                                   C.c_float, _P, _P, C.c_int64, _P]),
+    "kge_radius_min_key": (C.c_int, [_P, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int64, _P, C.c_int64, C.c_int64,
+                                     C.c_float, _P, _P, _P, C.c_int64, _P]),
+    "kge_forest_flatten": (C.c_int, [_P, _P, C.c_int64, _P]),
 }
 
 _lib = None

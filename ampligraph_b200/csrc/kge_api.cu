@@ -1255,38 +1255,120 @@ extern "C" int kge_knn(kge_handle *h, int32_t metric, const float *points_dev, i
     return KGE_OK;
 }
 
-extern "C" int kge_radius_neighbors(kge_handle *h, int32_t metric, const float *points_dev, int64_t n_points, int32_t ld,
-                                    const int32_t *query_ids_dev, int64_t b, const int32_t *cand_ids_dev, int64_t cand_begin,
-                                    int64_t n_cand, float radius, int64_t *offsets_dev, int32_t *nbr_dev,
-                                    void *workspace_dev, int64_t workspace_bytes, void *stream)
+// The checks and the chunk loop kge_radius_neighbors, kge_radius_union and kge_radius_min_key share (b > 0 after the
+// call returns KGE_OK with *w set): gather the queries, then for every L2-sized candidate chunk score -d into w->chunk
+// ([b, nc], row stride nc) and run epilogue(nc, c0), whose errors are reported as "<fn>: <stage>".
+static int check_radius(kge_handle *h, const char *fn, int32_t metric, const float *points_dev, int64_t n_points,
+                        int32_t ld, const int32_t *query_ids_dev, int64_t b, const int32_t *cand_ids_dev, int64_t cand_begin,
+                        int64_t n_cand, void *workspace_dev, int64_t workspace_bytes, KnnWorkspace *w)
 {
-    KGE_CHECK_HANDLE(h, "kge_radius_neighbors");
-    if (b < 0 || n_points < 0 || n_cand < 0 || cand_begin < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_radius_neighbors: negative size");
-    if (n_cand > 0x7fffffffLL) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_radius_neighbors: n_cand must be < 2^31");
+    if (b < 0 || n_points < 0 || n_cand < 0 || cand_begin < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: negative size", fn);
+    if (n_cand > 0x7fffffffLL) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: n_cand must be < 2^31", fn);
     if (b == 0) return KGE_OK;
-    if (int rc = check_points("kge_radius_neighbors", metric, points_dev, n_points, ld, query_ids_dev, cand_ids_dev, cand_begin, n_cand))
-        return rc;
-    if (!offsets_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_radius_neighbors: null pointer");
+    if (int rc = check_points(fn, metric, points_dev, n_points, ld, query_ids_dev, cand_ids_dev, cand_begin, n_cand)) return rc;
     if (int rc = check_topk_workspace(workspace_dev, workspace_bytes, kge_radius_workspace_bytes(h, b, n_cand, ld), "kge_radius"))
         return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    const KnnWorkspace w = carve_knn_workspace(h, workspace_dev, b, n_cand, 0, ld);
-    KGE_CUDA(launch_knn_gather(points_dev, ld, query_ids_dev, b, w.qvec, st), "kge_radius_neighbors: gather");
-    KGE_CUDA(cudaMemsetAsync(w.cnt, 0, (size_t)4 * b * sizeof(int32_t), st), "kge_radius_neighbors: memset");
-    KGE_CUDA(cudaMemsetAsync(w.cursor, 0, (size_t)b * sizeof(long long), st), "kge_radius_neighbors: memset");
+    *w = carve_knn_workspace(h, workspace_dev, b, n_cand, 0, ld);
+    return KGE_OK;
+}
+
+template <class Epilogue>
+static int radius_sweep(const kge_handle *h, const char *fn, const char *stage, int32_t metric, const float *points_dev,
+                        int32_t ld, const int32_t *query_ids_dev, int64_t b, const int32_t *cand_ids_dev, int64_t cand_begin,
+                        int64_t n_cand, const KnnWorkspace &w, cudaStream_t st, Epilogue epilogue)
+{
+    char what[96];
+    cudaError_t e = launch_knn_gather(points_dev, ld, query_ids_dev, b, w.qvec, st);
+    if (e != cudaSuccess) return cuda_fail(e, (snprintf(what, sizeof(what), "%s: gather", fn), what));
+    e = cudaMemsetAsync(w.cnt, 0, (size_t)4 * b * sizeof(int32_t), st);
+    if (e != cudaSuccess) return cuda_fail(e, (snprintf(what, sizeof(what), "%s: memset", fn), what));
     RankParams p = knn_rank_params(ld, points_dev, w, b);
     const int op = metric == KGE_METRIC_EUCLIDEAN ? OP_L2_SUB : OP_L1_SUB;
-    const long long *off = nbr_dev ? (const long long *)offsets_dev : nullptr;
     const int64_t C = topk_chunk(h, b, n_cand);
     for (int64_t c0 = 0; c0 < n_cand; c0 += C) {
         const int64_t nc = n_cand - c0 < C ? n_cand - c0 : C;
         p.cand_ids = cand_ids_dev ? cand_ids_dev + c0 : nullptr;
         p.cand_begin = cand_ids_dev ? 0 : cand_begin + c0;
         p.n_cand = nc;
-        KGE_CUDA(launch_rank_count_op(p, op, w.cnt, st), "kge_radius_neighbors: distances");  // -d, [b, nc]
-        KGE_CUDA(launch_radius_chunk(w.chunk, nc, nc, c0, b, radius, cand_ids_dev, cand_begin, w.cursor, off, nbr_dev, st),
-                 nbr_dev ? "kge_radius_neighbors: emit" : "kge_radius_neighbors: count");
+        e = launch_rank_count_op(p, op, w.cnt, st);  // -d, [b, nc]
+        if (e != cudaSuccess) return cuda_fail(e, (snprintf(what, sizeof(what), "%s: distances", fn), what));
+        e = epilogue(nc, c0);
+        if (e != cudaSuccess) return cuda_fail(e, (snprintf(what, sizeof(what), "%s: %s", fn, stage), what));
     }
+    return KGE_OK;
+}
+
+extern "C" int kge_radius_neighbors(kge_handle *h, int32_t metric, const float *points_dev, int64_t n_points, int32_t ld,
+                                    const int32_t *query_ids_dev, int64_t b, const int32_t *cand_ids_dev, int64_t cand_begin,
+                                    int64_t n_cand, float radius, int64_t *offsets_dev, int32_t *nbr_dev,
+                                    void *workspace_dev, int64_t workspace_bytes, void *stream)
+{
+    KGE_CHECK_HANDLE(h, "kge_radius_neighbors");
+    KnnWorkspace w;
+    if (int rc = check_radius(h, "kge_radius_neighbors", metric, points_dev, n_points, ld, query_ids_dev, b, cand_ids_dev,
+                              cand_begin, n_cand, workspace_dev, workspace_bytes, &w))
+        return rc;
+    if (b == 0) return KGE_OK;
+    if (!offsets_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_radius_neighbors: null pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    KGE_CUDA(cudaMemsetAsync(w.cursor, 0, (size_t)b * sizeof(long long), st), "kge_radius_neighbors: memset");
+    const long long *off = nbr_dev ? (const long long *)offsets_dev : nullptr;
+    if (int rc = radius_sweep(h, "kge_radius_neighbors", nbr_dev ? "emit" : "count", metric, points_dev, ld, query_ids_dev, b,
+                              cand_ids_dev, cand_begin, n_cand, w, st, [&](int64_t nc, int64_t c0) {
+                                  return launch_radius_chunk(w.chunk, nc, nc, c0, b, radius, cand_ids_dev, cand_begin,
+                                                             w.cursor, off, nbr_dev, st);
+                              }))
+        return rc;
     if (!nbr_dev) KGE_CUDA(launch_radius_counts(w.cursor, b, (long long *)offsets_dev, st), "kge_radius_neighbors: counts");
+    return KGE_OK;
+}
+
+extern "C" int kge_radius_union(kge_handle *h, int32_t metric, const float *points_dev, int64_t n_points, int32_t ld,
+                                const int32_t *query_ids_dev, int64_t b, const int32_t *cand_ids_dev, int64_t cand_begin,
+                                int64_t n_cand, float radius, int32_t *parent_dev, void *workspace_dev,
+                                int64_t workspace_bytes, void *stream)
+{
+    KGE_CHECK_HANDLE(h, "kge_radius_union");
+    KnnWorkspace w;
+    if (int rc = check_radius(h, "kge_radius_union", metric, points_dev, n_points, ld, query_ids_dev, b, cand_ids_dev,
+                              cand_begin, n_cand, workspace_dev, workspace_bytes, &w))
+        return rc;
+    if (b == 0) return KGE_OK;
+    if (!parent_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_radius_union: null pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    return radius_sweep(h, "kge_radius_union", "union", metric, points_dev, ld, query_ids_dev, b, cand_ids_dev, cand_begin,
+                        n_cand, w, st, [&](int64_t nc, int64_t c0) {
+                            return launch_radius_union_chunk(w.chunk, nc, nc, c0, b, radius, query_ids_dev, cand_ids_dev,
+                                                             cand_begin, parent_dev, st);
+                        });
+}
+
+extern "C" int kge_radius_min_key(kge_handle *h, int32_t metric, const float *points_dev, int64_t n_points, int32_t ld,
+                                  const int32_t *query_ids_dev, int64_t b, const int32_t *cand_ids_dev, int64_t cand_begin,
+                                  int64_t n_cand, float radius, const int32_t *key_dev, int32_t *out_dev,
+                                  void *workspace_dev, int64_t workspace_bytes, void *stream)
+{
+    KGE_CHECK_HANDLE(h, "kge_radius_min_key");
+    KnnWorkspace w;
+    if (int rc = check_radius(h, "kge_radius_min_key", metric, points_dev, n_points, ld, query_ids_dev, b, cand_ids_dev,
+                              cand_begin, n_cand, workspace_dev, workspace_bytes, &w))
+        return rc;
+    if (b == 0) return KGE_OK;
+    if (!key_dev || !out_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_radius_min_key: null pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    KGE_CUDA(launch_min_key_init(out_dev, b, st), "kge_radius_min_key: init");
+    return radius_sweep(h, "kge_radius_min_key", "min", metric, points_dev, ld, query_ids_dev, b, cand_ids_dev, cand_begin,
+                        n_cand, w, st, [&](int64_t nc, int64_t c0) {
+                            return launch_radius_min_key_chunk(w.chunk, nc, nc, c0, b, radius, cand_ids_dev, cand_begin,
+                                                               key_dev, out_dev, st);
+                        });
+}
+
+extern "C" int kge_forest_flatten(kge_handle *h, int32_t *parent_dev, int64_t n, void *stream)
+{
+    KGE_CHECK_HANDLE(h, "kge_forest_flatten");
+    if (n < 0 || n > 0x7fffffffLL) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_forest_flatten: n must be in [0, 2^31)");
+    if (n > 0 && !parent_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_forest_flatten: null pointer");
+    KGE_CUDA(launch_forest_flatten(parent_dev, n, (cudaStream_t)stream), "kge_forest_flatten");
     return KGE_OK;
 }

@@ -196,6 +196,21 @@ cudaError_t launch_radius_chunk(const float *chunk, long long ld, long long n, l
 // offsets[0] = 0, offsets[1 + q] = cursor[q]
 cudaError_t launch_radius_counts(const long long *cursor, long long b, long long *offsets, cudaStream_t st);
 
+// kge_cluster.cu: the DBSCAN epilogues over the same [b, ld] chunks of -d (columns [0, n) = positions base + c) and
+// the union-find forest parent[] they build (invariants in the file's header)
+// union(query_ids[q], id(pos)) for every in-radius pair with different ids
+cudaError_t launch_radius_union_chunk(const float *chunk, long long ld, long long n, long long base, long long b,
+                                      float radius, const int32_t *query_ids, const int32_t *cand_ids,
+                                      long long cand_begin, int32_t *parent, cudaStream_t st);
+// out[0..b) = INT32_MAX, before the first chunk of launch_radius_min_key_chunk
+cudaError_t launch_min_key_init(int32_t *out, long long b, cudaStream_t st);
+// out[q] = min(out[q], key[id(pos)] over the in-radius positions)
+cudaError_t launch_radius_min_key_chunk(const float *chunk, long long ld, long long n, long long base, long long b,
+                                        float radius, const int32_t *cand_ids, long long cand_begin,
+                                        const int32_t *key, int32_t *out, cudaStream_t st);
+// parent[x] = root(x) for x < n
+cudaError_t launch_forest_flatten(int32_t *parent, long long n, cudaStream_t st);
+
 // kge_rank_tc.cu: tensor-core filter + exact refine for the bilinear models
 struct RankTcLayout {  // carve-up of the tensor-core part of the caller's workspace
     int nkb, n_qb, n_ct;

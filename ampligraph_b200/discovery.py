@@ -13,6 +13,10 @@
 * find_duplicates   -- discovery.find_duplicates (discovery.py:714-982): groups of entities, relations or triples whose
   embeddings lie within a tolerance of each other.  tolerance='auto' runs the reference's bisection over the duplicate
   fraction, evaluated on the host from one nearest-other-row kge_knn pass instead of one radius self-join per step.
+* find_clusters     -- discovery.find_clusters (discovery.py:546-711): cluster the embeddings of entities, relations or
+  triples.  sklearn's DBSCAN (the default) runs on the GPU with sklearn's labels (KGEEngine.dbscan: radius counts,
+  then a union-find over the in-radius core pairs, no neighbourhood list stored); any other algorithm runs its
+  fit_predict on the host, as in the reference.
 
 Order of the link-prediction results: score descending; equal scores by candidate position ascending (the order of
 ents_to_consider / rels_to_consider, or of the entity / relation ids); NaN before +inf (DESIGN.md 3.6).  Distances are
@@ -292,6 +296,41 @@ def duplicate_fraction(d1, keys):
     return lambda tol: int(np.searchsorted(per_label, tol, side="right")) / n
 
 
+def _check_mode(X, mode):
+    """The mode and shape checks of find_duplicates / find_clusters (discovery.py:896-908, :686-701) -> X as an array."""
+    modes = ("t", "e", "r")
+    if mode not in modes:
+        raise _error("Argument `mode` must be one of the following: {}.".format(", ".join(modes)))
+    X = np.asarray(X)
+    if mode == "t" and (len(X.shape) != 2 or X.shape[1] != 3):
+        raise _error("For 't' mode the input X must be a matrix with three columns.")
+    if mode in ("e", "r") and len(X.shape) != 1:
+        raise _error("For 'e' or 'r' mode the input X must be an array.")
+    return X
+
+
+def _row_ids(model, X, mode):
+    """[(ids, kind)] of the column blocks of X's embedding rows: (X, mode) for mode 'e' / 'r', the subject, predicate
+    and object columns for mode 't'.  Unseen labels raise ValueError."""
+    cols = ((X[:, 0], "e"), (X[:, 1], "r"), (X[:, 2], "e")) if mode == "t" else ((X, mode),)
+    out = []
+    for values, kind in cols:
+        ids = _ids(model, values, kind)
+        if (ids < 0).any():
+            raise _error("{} in X have not been seen by the model.".format("Entities" if kind == "e" else "Relations"))
+        out.append((ids, kind))
+    return out
+
+
+def _points(model, eng, X, mode):
+    """The embedding rows of X on the device, contiguous fp32: entity / relation table rows (mode 'e' / 'r') or the
+    concatenation [s | p | o] of each triple's rows (mode 't').  Unseen labels and non-finite values raise ValueError."""
+    blocks = [(eng.ent if kind == "e" else eng.rel)[_dev(eng, ids, np.int64)] for ids, kind in _row_ids(model, X, mode)]
+    points = (blocks[0] if len(blocks) == 1 else torch.cat(blocks, 1)).contiguous()
+    _check_finite(points)
+    return points
+
+
 def find_duplicates(X, model, mode="e", metric="l2", tolerance="auto", expected_fraction_duplicates=0.1, verbose=False):
     """discovery.find_duplicates (discovery.py:714-982): the groups of rows of X whose embeddings lie within
     `tolerance` of each other -> (set of frozensets of labels (mode 't': of triples as tuples), tolerance).
@@ -308,29 +347,10 @@ def find_duplicates(X, model, mode="e", metric="l2", tolerance="auto", expected_
         model = model.model
     if not model.is_fitted:  # :891-894
         raise _error("Model has not been fitted.")
-    modes = ("t", "e", "r")
-    if mode not in modes:
-        raise _error("Argument `mode` must be one of the following: {}.".format(", ".join(modes)))
-    X = np.asarray(X)
-    if mode == "t" and (len(X.shape) != 2 or X.shape[1] != 3):
-        raise _error("For 't' mode the input X must be a matrix with three columns.")
-    if mode in ("e", "r") and len(X.shape) != 1:
-        raise _error("For 'e' or 'r' mode the input X must be an array.")
+    X = _check_mode(X, mode)
     metric = _metric(metric)
     eng = _check_fitted(model)
-
-    def rows(values, kind):
-        ids = _ids(model, values, kind)
-        if (ids < 0).any():
-            raise _error("{} in X have not been seen by the model.".format("Entities" if kind == "e" else "Relations"))
-        return _dev(eng, ids, np.int64)
-
-    if mode == "t":
-        points = torch.cat([eng.ent[rows(X[:, 0], "e")], eng.rel[rows(X[:, 1], "r")], eng.ent[rows(X[:, 2], "e")]], 1)
-    else:
-        points = (eng.ent if mode == "e" else eng.rel)[rows(X, mode)]
-    points = points.contiguous()
-    _check_finite(points)
+    points = _points(model, eng, X, mode)
     n = len(X)
     every = torch.arange(n, dtype=torch.int32, device=eng.device)
 
@@ -367,3 +387,80 @@ def find_duplicates(X, model, mode="e", metric="l2", tolerance="auto", expected_
             if len(row) > 1:  # :942-950
                 dups.add(frozenset(tuple(X[j]) for j in row) if mode == "t" else frozenset(X[j] for j in row))
     return dups, tolerance
+
+
+def _dbscan_on_gpu(clustering_algorithm):
+    """(eps, min_samples, metric) when find_clusters runs the clustering on the GPU, None when it calls the
+    algorithm's own fit_predict on the host.
+
+    On the GPU: None (DBSCAN()'s defaults, without importing sklearn) and objects whose type is exactly
+    sklearn.cluster.DBSCAN with metric_params None and a metric of _METRICS; 'minkowski' only with p 2 (euclidean) or
+    1 (manhattan) -- sklearn itself rejects p None there, and other p are other metrics.  The other metrics ignore p.
+    algorithm, leaf_size and n_jobs do not change sklearn's labels.  A subclass may override fit, so it stays on the
+    host with everything else."""
+    if clustering_algorithm is None:
+        return 0.5, 5, "euclidean"
+    try:
+        from sklearn.cluster import DBSCAN
+    except ImportError:
+        return None
+    if type(clustering_algorithm) is not DBSCAN or clustering_algorithm.metric_params is not None:
+        return None
+    metric = clustering_algorithm.metric
+    if not isinstance(metric, str) or metric not in _METRICS:
+        return None
+    if metric == "minkowski":
+        p = clustering_algorithm.p
+        if p is None or p not in (1, 2):
+            return None
+        metric = "manhattan" if p == 1 else "euclidean"
+    return clustering_algorithm.eps, clustering_algorithm.min_samples, _METRICS[metric]
+
+
+def _embeddings(model, X, mode):
+    """get_embeddings of X as the reference builds them (discovery.py:703-709): dense rows, [s | p | o] for mode 't'."""
+    if mode == "t":
+        return np.hstack((model.get_embeddings(X[:, 0], embedding_type="e"),
+                          model.get_embeddings(X[:, 1], embedding_type="r"),
+                          model.get_embeddings(X[:, 2], embedding_type="e")))
+    return model.get_embeddings(X, embedding_type=mode)
+
+
+def find_clusters(X, model, clustering_algorithm=None, mode="e"):
+    """discovery.find_clusters (discovery.py:546-711): cluster the embeddings of X -> labels, int64 [len(X)].
+
+    mode 'e' / 'r': X is an array of entities / relations; 't': X is [n, 3] triples, embedded as the concatenation of
+    the subject, predicate and object rows.  clustering_algorithm: an object with fit_predict; None means sklearn's
+    DBSCAN() (eps 0.5, min_samples 5, euclidean), the reference's default.
+
+    DBSCAN (None, or exactly sklearn.cluster.DBSCAN with a euclidean or manhattan metric) runs on the GPU
+    (KGEEngine.dbscan) and returns sklearn's labels for knn's fp32 distances (DESIGN.md 3.8); the estimator then
+    carries labels_, core_sample_indices_, components_ (the dense embedding rows of the core samples) and
+    n_features_in_, as after its own fit.  Every other algorithm -- KMeans, a cosine DBSCAN, a DBSCAN subclass -- runs
+    its fit_predict on the host on the dense embeddings, exactly as the reference does."""
+    if getattr(model, "is_backward", False):
+        model = model.model
+    if not model.is_fitted:  # :676-679
+        raise _error("Model has not been fitted.")
+    if clustering_algorithm is not None and not hasattr(clustering_algorithm, "fit_predict"):  # :681-684
+        raise _error("Clustering algorithm does not have the `fit_predict` method.")
+    X = _check_mode(X, mode)
+    gpu = _dbscan_on_gpu(clustering_algorithm)
+    if gpu is None:
+        _row_ids(model, X, mode)  # get_embeddings would drop unseen labels
+        return clustering_algorithm.fit_predict(_embeddings(model, X, mode))
+    if clustering_algorithm is not None and hasattr(clustering_algorithm, "_validate_params"):
+        clustering_algorithm._validate_params()  # sklearn's own errors for eps <= 0, min_samples < 1, ...
+    eps, min_samples, metric = gpu
+    eng = _check_fitted(model)
+    points = _points(model, eng, X, mode)
+    labels, core = eng.dbscan(points, eps, min_samples, metric)
+    labels = labels.cpu().numpy()
+    if clustering_algorithm is not None:  # as DBSCAN.fit leaves them
+        core_idx = np.flatnonzero(core.cpu().numpy())
+        components = _embeddings(model, X[core_idx], mode)
+        clustering_algorithm.labels_ = labels
+        clustering_algorithm.core_sample_indices_ = core_idx
+        clustering_algorithm.components_ = components if len(core_idx) else np.empty((0, components.shape[1]))
+        clustering_algorithm.n_features_in_ = components.shape[1]
+    return labels

@@ -35,6 +35,31 @@ def fp32_floor(x):
     return float(r)
 
 
+INT32_MAX = 2 ** 31 - 1
+DBSCAN_BATCH = 1024  # queries per kge_radius_* call of KGEEngine.dbscan (discovery.find_duplicates' batch)
+
+
+def dbscan_labels(core, root, border_root):
+    """sklearn DBSCAN's labels from the union-find result, on any device (O(n) plumbing of KGEEngine.dbscan).
+
+    core: bool [n].  root: int [n], for every core row the smallest index of its component (the component's seed);
+    other entries are not read.  border_root: int [n], for every non-core row the smallest root among its core
+    neighbours, or a value outside [0, n) if it has none; core entries are not read.
+    Clusters are numbered 0, 1, ... in ascending seed order (an exclusive cumsum over the roots, the core rows with
+    root[x] == x).  A core row takes its component's number, a non-core row that of border_root, or -1 (noise).
+    -> int64 [n]."""
+    n = core.numel()
+    idx = torch.arange(n, device=core.device)
+    root, border_root = root.long(), border_root.long()
+    is_root = (core & (root == idx)).long()
+    number = torch.cumsum(is_root, 0) - is_root
+    labels = torch.full((n,), -1, dtype=torch.int64, device=core.device)
+    labels[core] = number[root[core]]
+    border = ~core & (border_root >= 0) & (border_root < n)
+    labels[border] = number[border_root[border]]
+    return labels
+
+
 _NVTX = os.environ.get("KGE_B200_NVTX", "0") == "1"
 
 
@@ -458,24 +483,98 @@ class KGEEngine:
         d <= radius -> (offsets int64 [b+1], ids int32 [offsets[-1]]) on the device, row i's ids in ascending candidate
         position.  d is knn's fp32 distance; radius is taken as the largest fp32 not above it, so the test is exactly
         d <= radius for the Python number.  Two passes (count, then emit into the CSR); synchronises once for the size."""
-        assert points.dtype == torch.float32 and points.is_cuda and points.is_contiguous() and points.dim() == 2
-        assert query_ids.dtype == torch.int32 and query_ids.is_cuda and query_ids.is_contiguous()
-        b, (n_points, ld) = query_ids.numel(), points.shape
-        if n_cand is None:
-            n_cand = cand_ids.numel() if cand_ids is not None else n_points - cand_begin
-        offsets = torch.zeros(b + 1, dtype=torch.int64, device=self.device)
-        ws, ws_bytes = self._topk_workspace(self.lib.kge_radius_workspace_bytes(self.h, b, int(n_cand), ld))
+        head, tail = self._radius_args(points, query_ids, radius, metric, cand_ids, cand_begin, n_cand)
+        offsets = torch.zeros(query_ids.numel() + 1, dtype=torch.int64, device=self.device)
 
         def call(nbr):
-            _lib.check(self.lib.kge_radius_neighbors(self.h, _metric(metric), _ptr(points), n_points, ld, _ptr(query_ids), b,
-                                                     _ptr(cand_ids), int(cand_begin), int(n_cand), fp32_floor(radius),
-                                                     _ptr(offsets), _ptr(nbr), _ptr(ws), ws_bytes, self._stream()))
+            _lib.check(self.lib.kge_radius_neighbors(*head, _ptr(offsets), _ptr(nbr), *tail))
         call(None)
         torch.cumsum(offsets, 0, out=offsets)
         nbr = torch.empty(int(offsets[-1]), dtype=torch.int32, device=self.device)
         if nbr.numel() > 0:  # an empty tensor's data pointer is NULL, which would ask for another count pass
             call(nbr)
         return offsets, nbr
+
+    def _radius_args(self, points, query_ids, radius, metric, cand_ids, cand_begin, n_cand):
+        """The leading arguments of the kge_radius_* calls (radius as the largest fp32 not above it) and the trailing
+        ones (their workspace, the stream)."""
+        assert points.dtype == torch.float32 and points.is_cuda and points.is_contiguous() and points.dim() == 2
+        assert query_ids.dtype == torch.int32 and query_ids.is_cuda and query_ids.is_contiguous()
+        b, (n_points, ld) = query_ids.numel(), points.shape
+        if n_cand is None:
+            n_cand = cand_ids.numel() if cand_ids is not None else n_points - cand_begin
+        ws, ws_bytes = self._topk_workspace(self.lib.kge_radius_workspace_bytes(self.h, b, int(n_cand), ld))
+        head = (self.h, _metric(metric), _ptr(points), n_points, ld, _ptr(query_ids), b, _ptr(cand_ids), int(cand_begin),
+                int(n_cand), fp32_floor(radius))
+        return head, (_ptr(ws), ws_bytes, self._stream())
+
+    def radius_counts(self, points, query_ids, radius, metric, cand_ids=None, cand_begin=0, n_cand=None):
+        """The count pass of radius_neighbors alone: #{candidates at d <= radius} of each query -> int64 [b] on the
+        device, without synchronising."""
+        head, tail = self._radius_args(points, query_ids, radius, metric, cand_ids, cand_begin, n_cand)
+        offsets = torch.zeros(query_ids.numel() + 1, dtype=torch.int64, device=self.device)
+        _lib.check(self.lib.kge_radius_neighbors(*head, _ptr(offsets), None, *tail))
+        return offsets[1:]
+
+    def radius_union(self, points, query_ids, radius, metric, parent, cand_ids=None, cand_begin=0, n_cand=None):
+        """kge_radius_union: joins each row query_ids[i] with every candidate row at d <= radius (radius_neighbors'
+        test) in the union-find forest `parent` (int32 [len(points)], parent[x] = x before the first call); a root
+        always hooks under the smaller root, so each tree's root is its smallest id."""
+        assert parent.dtype == torch.int32 and parent.is_cuda and parent.numel() == points.shape[0]
+        head, tail = self._radius_args(points, query_ids, radius, metric, cand_ids, cand_begin, n_cand)
+        _lib.check(self.lib.kge_radius_union(*head, _ptr(parent), *tail))
+
+    def radius_min_key(self, points, query_ids, radius, metric, key, cand_ids=None, cand_begin=0, n_cand=None):
+        """kge_radius_min_key: the smallest key[c] over the candidate ids c at d <= radius of each row query_ids[i] ->
+        int32 [b] on the device, 2^31 - 1 where there is none.  key: int32 [len(points)], indexed by id."""
+        assert key.dtype == torch.int32 and key.is_cuda and key.numel() == points.shape[0]
+        head, tail = self._radius_args(points, query_ids, radius, metric, cand_ids, cand_begin, n_cand)
+        out = torch.empty(query_ids.numel(), dtype=torch.int32, device=self.device)
+        _lib.check(self.lib.kge_radius_min_key(*head, _ptr(key), _ptr(out), *tail))
+        return out
+
+    def forest_flatten(self, parent):
+        """kge_forest_flatten: parent[x] = root(x) for every x, in place, after the unions."""
+        assert parent.dtype == torch.int32 and parent.is_cuda and parent.is_contiguous()
+        _lib.check(self.lib.kge_forest_flatten(self.h, _ptr(parent), parent.numel(), self._stream()))
+
+    @_traced("kge.dbscan")
+    def dbscan(self, points, eps, min_samples, metric, batch=DBSCAN_BATCH):
+        """sklearn DBSCAN(eps, min_samples, metric).fit_predict over the rows of `points` (any [n, ld] fp32 CUDA tensor
+        with ld % 4 == 0, as for knn), with knn's fp32 distances and the test d <= eps (eps taken as the largest fp32 not
+        above it) -> (labels int64 [n], core bool [n]) on the device.  Labels follow sklearn's: clusters numbered by
+        their smallest core row, noise -1 (DESIGN.md 3.8).
+
+        Four sweeps of `batch` queries each: the radius count of every row (core: count >= min_samples), the union of
+        the in-radius core pairs (queries core[s:e], candidates core[s:], so each pair is scored at most twice), the
+        flatten of the forest, and the smallest root among the core neighbours of every non-core row.  Synchronises
+        once, to compact the core ids."""
+        assert points.dtype == torch.float32 and points.is_cuda and points.is_contiguous() and points.dim() == 2
+        n = points.shape[0]
+        if not float(eps) > 0:
+            raise ValueError("eps must be > 0, got %r" % (eps,))
+        if int(min_samples) < 1:
+            raise ValueError("min_samples must be >= 1, got %r" % (min_samples,))
+        if n >= 2 ** 31:
+            raise ValueError("dbscan: ids are int32 (n < 2^31), got n = %d" % n)
+        radius, dev = fp32_floor(eps), self.device
+        every = torch.arange(n, dtype=torch.int32, device=dev)
+        counts = torch.empty(n, dtype=torch.int64, device=dev)
+        for s in range(0, n, batch):
+            counts[s:s + batch] = self.radius_counts(points, every[s:s + batch], radius, metric, n_cand=n)
+        core = counts >= int(min_samples)
+        core_ids = torch.nonzero(core).flatten().to(torch.int32)
+        parent = every.clone()
+        for s in range(0, core_ids.numel(), batch):
+            self.radius_union(points, core_ids[s:s + batch], radius, metric, parent, cand_ids=core_ids[s:])
+        self.forest_flatten(parent)
+        border = torch.full((n,), INT32_MAX, dtype=torch.int32, device=dev)
+        if core_ids.numel() > 0:
+            rest = torch.nonzero(~core).flatten().to(torch.int32)
+            for s in range(0, rest.numel(), batch):
+                q = rest[s:s + batch]
+                border[q.long()] = self.radius_min_key(points, q, radius, metric, parent, cand_ids=core_ids)
+        return dbscan_labels(core, parent, border), core
 
     def _topk_workspace(self, need):
         # need == 0: invalid arguments (k < 1, ...) -- the call itself reports them

@@ -454,6 +454,36 @@ int kge_radius_neighbors(kge_handle *h, int32_t metric, const float *points_dev,
                          void *workspace_dev, int64_t workspace_bytes, void *stream);
 int64_t kge_radius_workspace_bytes(const kge_handle *h, int64_t b, int64_t n_cand, int32_t ld);
 
+/* DBSCAN without neighbourhood lists: the device half of discovery.find_clusters (discovery.py:546-711) with sklearn's
+ * DBSCAN, whose fit runs a radius_neighbors self-join, keeps every neighbourhood and labels the rows in
+ * sklearn.cluster._dbscan_inner.dbscan_inner.  With A(i, j) = d(i, j) <= radius (kge_radius_neighbors' test, i = j
+ * included) and core(i) = #{j : A(i, j)} >= min_samples, sklearn's labels are: the connected components of the core
+ * rows under A, numbered by their smallest core index; a non-core row with a core neighbour takes the component with
+ * the smallest such index among its neighbours'; every other row is noise.  The count pass of kge_radius_neighbors
+ * gives the cores; the three calls below give the components and the border rows.  Arguments, candidates, the chunk
+ * rule and the workspace (kge_radius_workspace_bytes) are those of kge_radius_neighbors; none allocates or
+ * synchronises.
+ *
+ * kge_radius_union: for every in-radius pair (query_ids_dev[i], candidate id c) with different ids, unions the two in
+ * the caller's union-find forest parent_dev[n_points] (int32), which starts as parent[x] = x (or is the result of
+ * earlier kge_radius_union calls).  A root hooks under the smaller root, so whatever the order of the unions every
+ * tree's root is its smallest id: DBSCAN's component seed.  Concurrent calls may share the forest; parent[x] <= x
+ * always, and every x's path leads to its root. */
+int kge_radius_union(kge_handle *h, int32_t metric, const float *points_dev, int64_t n_points, int32_t ld,
+                     const int32_t *query_ids_dev, int64_t b, const int32_t *cand_ids_dev, int64_t cand_begin,
+                     int64_t n_cand, float radius, int32_t *parent_dev, void *workspace_dev, int64_t workspace_bytes,
+                     void *stream);
+/* out_dev[i] = the smallest key_dev[c] over the candidate ids c within the radius of query row query_ids_dev[i], or
+ * INT32_MAX if there is none.  key_dev is indexed by id (n_points entries).  DBSCAN's border rows
+ * (dbscan_inner's depth-first search reaches a border row first from the cluster with the smallest seed): queries the
+ * non-core rows, candidates the core rows, key the flattened forest. */
+int kge_radius_min_key(kge_handle *h, int32_t metric, const float *points_dev, int64_t n_points, int32_t ld,
+                       const int32_t *query_ids_dev, int64_t b, const int32_t *cand_ids_dev, int64_t cand_begin,
+                       int64_t n_cand, float radius, const int32_t *key_dev, int32_t *out_dev, void *workspace_dev,
+                       int64_t workspace_bytes, void *stream);
+/* parent_dev[x] = root(x) for every x < n (n < 2^31), after the unions (DBSCAN: the component seed of each core row). */
+int kge_forest_flatten(kge_handle *h, int32_t *parent_dev, int64_t n, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

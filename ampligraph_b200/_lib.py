@@ -112,6 +112,8 @@ PROTOTYPES = {
     "kge_radius_min_key": (C.c_int, [_P, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int64, _P, C.c_int64, C.c_int64,
                                      C.c_float, _P, _P, _P, C.c_int64, _P]),
     "kge_forest_flatten": (C.c_int, [_P, _P, C.c_int64, _P]),
+    "kge_graph_counts": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, _P, _P, C.c_int64, _P]),
+    "kge_graph_workspace_bytes": (C.c_int64, [C.c_int64]),
 }
 
 _lib = None

@@ -1372,3 +1372,30 @@ extern "C" int kge_forest_flatten(kge_handle *h, int32_t *parent_dev, int64_t n,
     KGE_CUDA(launch_forest_flatten(parent_dev, n, (cudaStream_t)stream), "kge_forest_flatten");
     return KGE_OK;
 }
+
+extern "C" int64_t kge_graph_workspace_bytes(int64_t n_nodes)
+{
+    if (n_nodes < 0 || n_nodes > 0x7fffffffLL) return 0;
+    return (int64_t)graph_workspace_bytes(n_nodes);
+}
+
+extern "C" int kge_graph_counts(const int64_t *offsets_dev, const int32_t *nbr_dev, const int32_t *order_dev,
+                                int64_t n_nodes, int64_t *tri2_dev, int64_t *sq_dev, int64_t *pot_dev,
+                                void *workspace_dev, int64_t workspace_bytes, void *stream)
+{
+    if (n_nodes < 0 || n_nodes > 0x7fffffffLL)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_graph_counts: n_nodes must be in [0, 2^31)");
+    if (n_nodes == 0) return KGE_OK;
+    if (!offsets_dev || !nbr_dev || !order_dev || !tri2_dev || !sq_dev || !pot_dev)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_graph_counts: null pointer");
+    const int64_t need = kge_graph_workspace_bytes(n_nodes);
+    if (need == 0) return fail(KGE_ERR_CUDA, "kge_graph_counts: device query failed");
+    if (!workspace_dev || workspace_bytes < need)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_graph_counts: workspace of %lld bytes, need %lld",
+                    (long long)workspace_bytes, (long long)need);
+    if ((uintptr_t)workspace_dev % 8) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_graph_counts: workspace not 8-byte aligned");
+    KGE_CUDA(launch_graph_counts((const long long *)offsets_dev, nbr_dev, order_dev, n_nodes, workspace_dev,
+                                 (long long *)tri2_dev, (long long *)sq_dev, (long long *)pot_dev, (cudaStream_t)stream),
+             "kge_graph_counts");
+    return KGE_OK;
+}

@@ -211,6 +211,13 @@ cudaError_t launch_radius_min_key_chunk(const float *chunk, long long ld, long l
 // parent[x] = root(x) for x < n
 cudaError_t launch_forest_flatten(int32_t *parent, long long n, cudaStream_t st);
 
+// kge_graph.cu: per-node wedge counts of an undirected simple graph in CSR (definitions in the file's header), on the
+// current device.  The workspace (8-byte aligned) holds the work counter and, when n int32 counters do not fit in
+// shared memory, one such slice per CTA; graph_workspace_bytes returns 0 for n < 0 or on a device query failure.
+long long graph_workspace_bytes(long long n);
+cudaError_t launch_graph_counts(const long long *off, const int32_t *nbr, const int32_t *order, long long n,
+                                void *workspace, long long *tri2, long long *sq, long long *pot, cudaStream_t st);
+
 // kge_rank_tc.cu: tensor-core filter + exact refine for the bilinear models
 struct RankTcLayout {  // carve-up of the tensor-core part of the caller's workspace
     int nkb, n_qb, n_ct;

@@ -17,6 +17,10 @@
   triples.  sklearn's DBSCAN (the default) runs on the GPU with sklearn's labels (KGEEngine.dbscan: radius counts,
   then a union-find over the in-radius core pairs, no neighbourhood list stored); any other algorithm runs its
   fit_predict on the host, as in the reference.
+* generate_candidates / discover_facts -- discovery.generate_candidates and discover_facts (discovery.py:21-543):
+  candidate statements sampled by entity weights, filtered against X, ranked by evaluate.  The networkx statistics of
+  the graph strategies come from per-node wedge counts on the GPU (engine.graph_counts, DESIGN.md 3.9); the
+  candidates are the reference's, row for row, for a given seed.
 
 Order of the link-prediction results: score descending; equal scores by candidate position ascending (the order of
 ents_to_consider / rels_to_consider, or of the entity / relation ids); NaN before +inf (DESIGN.md 3.6).  Distances are
@@ -464,3 +468,218 @@ def find_clusters(X, model, clustering_algorithm=None, mode="e"):
         clustering_algorithm.components_ = components if len(core_idx) else np.empty((0, components.shape[1]))
         clustering_algorithm.n_features_in_ = components.shape[1]
     return labels
+
+
+_CANDIDATE_STRATEGIES = ("random_uniform", "entity_frequency", "graph_degree", "cluster_coefficient",
+                         "cluster_triangles", "cluster_squares")
+
+
+def _first_known(cand, known):
+    """The rows _setdiff2d removes (discovery.py:522-543): those whose key is in `known` (sorted, unique) and that are
+    the first occurrence of their key within `cand`.  A later repeat of a known row is kept, as in the reference, whose
+    cumsum over the [|A|, |B|, 3] comparison marks only the first match of each row of B.  -> bool [len(cand)]."""
+    cand = np.asarray(cand, np.int64)
+    hit = np.zeros(len(cand), bool)
+    if len(known):
+        pos = np.minimum(np.searchsorted(known, cand), len(known) - 1)
+        hit = known[pos] == cand
+    first = np.zeros(len(cand), bool)
+    first[np.unique(cand, return_index=True)[1]] = True
+    return hit & first
+
+
+def _setdiff2d(A, B):
+    """discovery._setdiff2d (discovery.py:522-543) with sorted int64 row keys instead of the [|A|, |B|, m] comparison
+    array: the rows of A, less the first occurrence in A of every row that is also in B."""
+    if len(A.shape) != 2 or len(B.shape) != 2:
+        raise RuntimeError("Input arrays must be 2-dimensional.")
+    rows = np.concatenate([A, B]) if len(A) and len(B) else (A if len(A) else B)
+    if len(rows) == 0 or len(A) == 0:
+        return A
+    codes = np.stack([np.unique(rows[:, c], return_inverse=True)[1].ravel() for c in range(rows.shape[1])], 1)
+    key = np.unique(codes, axis=0, return_inverse=True)[1].ravel().astype(np.int64)
+    return A[~_first_known(key[:len(A)], np.unique(key[len(A):]))]
+
+
+def _graph_weights(strategy, s_node, o_node, n_nodes):
+    """The per-node statistic C of generate_candidates' graph strategies (discovery.py:457-471), float64 [n_nodes], for
+    the undirected graph with one edge {s_node[i], o_node[i]} per triple: nx.Graph.degree (numpy, a self-loop counting
+    twice), or nx.clustering / nx.triangles / nx.square_clustering from the GPU counts (engine.graph_counts).  Each
+    value is a float64 division of exact integers, so it is networkx's Python int / int bit for bit."""
+    if strategy == "graph_degree":
+        keys = np.unique(np.minimum(s_node, o_node) * n_nodes + np.maximum(s_node, o_node))
+        a, b = keys // n_nodes, keys % n_nodes
+        return (np.bincount(a, minlength=n_nodes) + np.bincount(b, minlength=n_nodes)).astype(np.float64)
+    from .engine import graph_counts
+    triples = np.stack([s_node, np.zeros_like(s_node), o_node], 1)  # the predicate column is not read
+    g = {k: v.cpu().numpy() for k, v in graph_counts(triples, n_nodes).items()}
+    tri2, d = g["tri2"], g["d"]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        if strategy == "cluster_triangles":
+            return (tri2 // 2).astype(np.float64)
+        if strategy == "cluster_coefficient":
+            return np.where(tri2 == 0, 0.0, tri2.astype(np.float64) / (d * (d - 1)).astype(np.float64))
+        sq, pot = g["sq"], g["pot"]
+        return np.where((d > 1) & (pot > 0), sq.astype(np.float64) / pot.astype(np.float64), 0.0)
+
+
+class _CandidateSource:
+    """What generate_candidates derives from X alone, computed once and shared by every relation of discover_facts:
+    the entity pools e_s / e_o, their sampling weights and the sorted int64 keys of X's triples.  Nodes are the
+    positions in np.unique of X's subject and object columns together."""
+
+    def __init__(self, X, strategy, consolidate_sides):
+        X = X[:, :3] if X.shape[1] > 3 else X  # :334-337
+        self.X, self.strategy = X, strategy
+        self.nodes = np.unique(np.concatenate((X[:, 0], X[:, 2])))
+        self.rels = np.unique(X[:, 1])
+        s_node, o_node = np.searchsorted(self.nodes, X[:, 0]), np.searchsorted(self.nodes, X[:, 2])
+        self.known = np.unique(self._key(s_node, np.searchsorted(self.rels, X[:, 1]), o_node))
+        if consolidate_sides:  # :382-387
+            self.e_s = self.e_o = self.nodes
+        else:
+            self.e_s, self.e_o = np.unique(X[:, 0]), np.unique(X[:, 2])
+        self.s_node, self.o_node = np.searchsorted(self.nodes, self.e_s), np.searchsorted(self.nodes, self.e_o)
+        self.p_s = self.p_o = None
+        if strategy == "entity_frequency":  # :433-449
+            if consolidate_sides:
+                c_s = c_o = np.unique(X[:, [0, 2]], return_counts=True)[1]
+            else:
+                c_s, c_o = np.unique(X[:, 0], return_counts=True)[1], np.unique(X[:, 2], return_counts=True)[1]
+            self.p_s = c_s.astype(np.float64) / np.sum(c_s.astype(np.float64))
+            self.p_o = c_o.astype(np.float64) / np.sum(c_o.astype(np.float64))
+        elif strategy != "random_uniform":  # :451-477
+            C = _graph_weights(strategy, s_node, o_node, len(self.nodes))
+            w_s, w_o = C[self.s_node], C[self.o_node]
+            self.p_s, self.p_o = w_s / np.sum(w_s), w_o / np.sum(w_o)
+
+    def _key(self, s, r, o):
+        n = len(self.nodes)
+        return (np.asarray(s, np.int64) * len(self.rels) + np.asarray(r, np.int64)) * n + np.asarray(o, np.int64)
+
+    def generate(self, target_rel, max_candidates, seed):
+        """The sampling loop of generate_candidates (:391-431, :479-519) for one target_rel (a label or a list of
+        labels, one meshgrid over them), with its own RandomState(seed); the arguments are checked by the caller."""
+        if isinstance(max_candidates, float):
+            max_candidates = int(max_candidates * len(self.X))
+        rel = np.asarray(target_rel).ravel()
+        r_pos = np.minimum(np.searchsorted(self.rels, rel), max(len(self.rels) - 1, 0))
+        r_id = np.where(self.rels[r_pos] == rel, r_pos, -1) if len(self.rels) else np.full(len(rel), -1)
+
+        rng = np.random.RandomState(seed)
+        uniform = self.strategy == "random_uniform"
+        sample_size = int(np.sqrt(max_candidates) + 10)
+        X_candidates = np.zeros([max_candidates, 3], dtype=object)
+        num_retries, max_retries = 0, 5
+        start_idx, end_idx = 0, 0
+        while end_idx <= max_candidates - 1:
+            # choice over positions draws exactly what choice over the labels does: the stream depends on the size
+            if uniform:
+                i_s = rng.choice(len(self.e_s), size=sample_size, replace=False)
+                i_o = rng.choice(len(self.e_o), size=sample_size, replace=False)
+            else:
+                i_s = rng.choice(len(self.e_s), size=sample_size, replace=True, p=self.p_s)
+                i_o = rng.choice(len(self.e_o), size=sample_size, replace=True, p=self.p_o)
+            gen = np.array(np.meshgrid(self.e_s[i_s], target_rel, self.e_o[i_o])).T.reshape(-1, 3)
+            ids = np.array(np.meshgrid(self.s_node[i_s], r_id, self.o_node[i_o])).T.reshape(-1, 3)
+            key = np.where(ids[:, 1] >= 0, self._key(ids[:, 0], ids[:, 1], ids[:, 2]), -1)
+            gen = gen[~_first_known(key, self.known)]
+            gen = gen[np.where(gen[:, 0] != gen[:, 2])]  # :371-374
+            select_idx = min(len(gen), len(X_candidates) - start_idx)
+            end_idx = start_idx + select_idx
+            X_candidates[start_idx:end_idx, :] = gen[0:select_idx, :]
+            start_idx = end_idx
+            num_retries += 1
+            if num_retries == max_retries:
+                break
+        return X_candidates[0:end_idx, :]
+
+
+def _check_candidate_args(rels, target_rel, max_candidates):
+    """The checks of generate_candidates after the strategy's (discovery.py:349-363); rels = np.unique(X[:, 1])."""
+    if target_rel not in rels:
+        logger.warning("Target relation is not found in triples.")  # no error: target_rel may be missing from X
+    if not isinstance(max_candidates, (float, int)):
+        raise ValueError("Parameter max_candidates must be a float or int.")
+    if max_candidates <= 0:
+        raise ValueError("Parameter max_candidates must be a positive integer or float in range (0,1].")
+
+
+def generate_candidates(X, strategy, target_rel, max_candidates, consolidate_sides=False, seed=0):
+    """discovery.generate_candidates (discovery.py:274-519): candidate statements (s, target_rel, o) sampled from the
+    entities of X by `strategy`, without the triples of X and without reflexive ones -> object array [n, 3],
+    n <= max_candidates.
+
+    For a given seed the result is the reference's, row for row.  The sampling is the reference's loop (the same
+    np.random.choice calls on a RandomState(seed), which draws the legacy stream np.random.seed(seed) gives, but leaves
+    the global RNG alone).  The filter of known triples has _setdiff2d's semantics on sorted int64 keys, without its
+    [|A|, |B|, 3] array.  The graph statistics of 'cluster_coefficient', 'cluster_triangles' and 'cluster_squares' are
+    computed on the GPU (engine.graph_counts, DESIGN.md 3.9) and equal networkx's bit for bit; 'graph_degree' and
+    'entity_frequency' are counted on the host."""
+    X = np.asarray(X)
+    if strategy not in _CANDIDATE_STRATEGIES:  # :338-347
+        raise ValueError("%s is not a valid candidate generation strategy." % strategy)
+    _check_candidate_args(np.unique(X[:, 1]), target_rel, max_candidates)  # before the weights, as in the reference
+    return _CandidateSource(X, strategy, consolidate_sides).generate(target_rel, max_candidates, seed)
+
+
+def discover_facts(X, model, top_n=10, strategy="random_uniform", max_candidates=100, target_rel=None, seed=0):
+    """discovery.discover_facts (discovery.py:21-271): candidate statements from generate_candidates, ranked by
+    model.evaluate against their subject and object corruptions (filtered by X); the candidates whose mean rank is
+    <= top_n -> (X_pred object array [n, 3], mean ranks float64 [n]).
+
+    target_rel: a relation label, a list of them (one meshgrid over the list, as in the reference), or None for every
+    relation the model knows, in the indexer's order, each sampled with the generator reset to `seed`.  A float
+    max_candidates is a fraction of len(X).  The weights and X's keys are computed once per call, and every candidate
+    is ranked in one evaluate call (the ranks do not depend on batching).  The 'exhaustive' strategy is rejected, as in
+    the reference.
+
+    Deliberate deviations from the reference (DESIGN.md 7):
+    * target_rel=None stacks the per-relation results with np.vstack, in relation order; the reference's np.hstack
+      raises as soon as two relations discover different numbers of facts.
+    * candidates with an entity (or relation) the model has not seen are dropped with a warning before ranking, as the
+      reference's docstring promises; its ranks would no longer line up with its candidates.
+    * the global numpy RNG is not reseeded."""
+    if getattr(model, "is_backward", False):
+        model = model.model
+    if not model.is_fitted:  # :175-178
+        raise _error("Model is not fitted.")
+    if strategy not in _CANDIDATE_STRATEGIES:  # :185-195
+        raise _error("%s is not a valid strategy." % strategy)
+    X = np.asarray(X)
+    if isinstance(max_candidates, float):  # :201-207
+        max_candidates = int(max_candidates * len(X))
+    if isinstance(target_rel, str):
+        target_rel = [target_rel]
+    known_rels = _labels(model, np.arange(_count(model, "r")), "r").tolist()
+    if target_rel is None:  # :212-229
+        logger.info("No target relation specified. Using all relations to generate candidate statements.")
+        rel_list = known_rels
+    else:
+        missing_rels = [rel for rel in target_rel if rel not in known_rels]
+        if len(missing_rels) > 0:
+            raise _error("Target relation(s) not found in model: {}".format(missing_rels))
+        rel_list = [target_rel]
+
+    if not isinstance(max_candidates, (float, int)) or max_candidates <= 0:  # before the weights
+        _check_candidate_args(np.unique(X[:, 1]), rel_list[0] if rel_list else None, max_candidates)
+    source = _CandidateSource(X, strategy, False)
+    parts = []
+    for relation in rel_list:
+        logger.info("Generating candidates for relation: %s" % relation)
+        _check_candidate_args(source.rels, relation, max_candidates)
+        parts.append(source.generate(relation, max_candidates, seed))
+    candidates = np.vstack(parts) if parts else np.empty((0, 3), dtype=object)
+    seen = (_ids(model, candidates[:, 0], "e") >= 0) & (_ids(model, candidates[:, 1], "r") >= 0) & \
+        (_ids(model, candidates[:, 2], "e") >= 0)
+    if not seen.all():
+        logger.warning("%d candidate statements contain entities not seen by the model and are dropped.",
+                       int((~seen).sum()))
+        candidates = candidates[seen]
+    if len(candidates) == 0:
+        return candidates, np.empty(0, np.float64)
+    ranks = model.evaluate(candidates, use_filter={"test": X}, corrupt_side="s,o", verbose=False)
+    avg_ranks = np.mean(ranks, axis=1)
+    preds = avg_ranks <= top_n
+    logger.info("Discovered %d facts" % int(preds.sum()))
+    return candidates[preds], avg_ranks[preds]

@@ -60,6 +60,76 @@ def dbscan_labels(core, root, border_root):
     return labels
 
 
+def graph_csr(triples, n_nodes, device=None):
+    """The CSR of graph_counts, built on the device with torch: (degree, d, offsets int64 [n + 1], nbr int32, order
+    int32 [n]) for the undirected simple graph of the edges {s, o} of indexed triples [n, 3] (a CUDA tensor or a host
+    array).  degree is nx.Graph.degree (a self-loop counts twice); d = |N(v)| leaves self-loops out; nbr lists both
+    directions of each unique non-loop edge, sorted; order is the heaviest-first processing order (descending sum of
+    the neighbours' d, the wedges through v).  device: default that of a CUDA `triples`, else the current one."""
+    if device is not None:
+        dev = torch.device(device)
+    elif torch.is_tensor(triples) and triples.is_cuda:
+        dev = triples.device
+    else:
+        dev = torch.device("cuda", torch.cuda.current_device())
+    n = int(n_nodes)
+    if not 0 <= n < 2 ** 31:
+        raise ValueError("graph_counts: n_nodes must be in [0, 2^31), got %d" % n)
+    t = (triples if torch.is_tensor(triples) else torch.as_tensor(np.ascontiguousarray(triples))).to(dev)
+    if t.dim() != 2 or t.shape[1] != 3:
+        raise ValueError("graph_counts: triples must be [n, 3]")
+    s, o = t[:, 0].long(), t[:, 2].long()
+    if s.numel() and (int(torch.minimum(s, o).min()) < 0 or int(torch.maximum(s, o).max()) >= n):
+        raise ValueError("graph_counts: node ids must be in [0, n_nodes)")
+    keys = torch.unique(torch.minimum(s, o) * n + torch.maximum(s, o))  # one key per undirected edge
+    a, b = keys // n, keys % n
+    degree = torch.bincount(a, minlength=n) + torch.bincount(b, minlength=n)  # a == b: a self-loop counts twice
+    a, b = a[a != b], b[a != b]
+    src, dst = torch.cat([a, b]), torch.cat([b, a])
+    perm = torch.argsort(src * n + dst)
+    src, nbr = src[perm], dst[perm].to(torch.int32).contiguous()
+    d = torch.bincount(src, minlength=n)
+    offsets = torch.zeros(n + 1, dtype=torch.int64, device=dev)
+    torch.cumsum(d, 0, out=offsets[1:])
+    work = torch.zeros(n, dtype=torch.int64, device=dev).index_add_(0, src, d[nbr.long()])
+    order = torch.argsort(work, descending=True).to(torch.int32).contiguous()
+    return degree, d, offsets, nbr, order
+
+
+def graph_counts_csr(offsets, nbr, order):
+    """kge_graph_counts on a CSR of graph_csr -> (tri2, sq, pot), int64 [n] on its device, stream-ordered."""
+    lib, dev, n = _lib.load(), offsets.device, offsets.numel() - 1
+    with torch.cuda.device(dev):
+        tri2, sq, pot = (torch.zeros(n, dtype=torch.int64, device=dev) for _ in range(3))
+        if nbr.numel() == 0:  # no edge: every count is 0 (and an empty tensor's data pointer is NULL)
+            return tri2, sq, pot
+        need = int(lib.kge_graph_workspace_bytes(n))
+        if n > 0 and need == 0:
+            raise RuntimeError("kge_graph_workspace_bytes failed for %d nodes" % n)
+        ws = torch.empty(max(need, 8), dtype=torch.uint8, device=dev)
+        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        _lib.check(lib.kge_graph_counts(_ptr(offsets), _ptr(nbr), _ptr(order), n, _ptr(tri2), _ptr(sq), _ptr(pot),
+                                        _ptr(ws), need, stream))
+    return tri2, sq, pot
+
+
+def graph_counts(triples, n_nodes, device=None):
+    """Per-node statistics of the undirected simple graph of indexed triples (kge_graph_counts, DESIGN.md 3.9).
+
+    triples: [n, 3] ints (a CUDA tensor or a host array); each triple (s, p, o) is an edge {s, o}, s and o in
+    [0, n_nodes).  Repeated edges and the two directions of one edge count once; self-loops are left out of the
+    adjacency.  device: the CUDA device to run on (default: that of a CUDA `triples`, else the current one).
+    Returns a dict of int64 [n_nodes] tensors on that device:
+      degree -- nx.Graph.degree (a self-loop counts twice),
+      d      -- |N(v)|, the degree without self-loops,
+      tri2, sq, pot -- the kernel's counts: nx.triangles = tri2 / 2, nx.clustering = tri2 / (d (d - 1)) (0 if tri2 = 0),
+      nx.square_clustering = sq / pot (0 if d < 2 or pot <= 0).
+    The CSR is built on the device (graph_csr), then one kge_graph_counts call counts the wedges."""
+    degree, d, offsets, nbr, order = graph_csr(triples, n_nodes, device)
+    tri2, sq, pot = graph_counts_csr(offsets, nbr, order)
+    return {"degree": degree, "d": d, "tri2": tri2, "sq": sq, "pot": pot}
+
+
 _NVTX = os.environ.get("KGE_B200_NVTX", "0") == "1"
 
 

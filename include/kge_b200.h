@@ -484,6 +484,29 @@ int kge_radius_min_key(kge_handle *h, int32_t metric, const float *points_dev, i
 /* parent_dev[x] = root(x) for every x < n (n < 2^31), after the unions (DBSCAN: the component seed of each core row). */
 int kge_forest_flatten(kge_handle *h, int32_t *parent_dev, int64_t n, void *stream);
 
+/* Per-node wedge counts of an undirected simple graph: the device half of discovery.generate_candidates' graph
+ * strategies (nx.triangles, nx.clustering and nx.square_clustering, discovery.py:457-471).  No handle: the call runs on
+ * the calling thread's current device, on `stream`; it neither allocates nor synchronises.
+ *
+ * The graph is a CSR over n_nodes < 2^31 nodes: offsets_dev int64 [n_nodes + 1], nbr_dev int32 [offsets[n_nodes]],
+ * N(v) = nbr[offsets[v], offsets[v + 1]) without repeats and without v itself (each undirected edge in both lists).
+ * order_dev int32 [n_nodes] is a permutation of the nodes, the order in which they are taken (heaviest first,
+ * e.g. by sum_{u in N(v)} d(u), balances the load; the results do not depend on it).  With d(v) = |N(v)| and
+ * P(v, y) = |N(v) & N(y)|, the call writes int64 [n_nodes]:
+ *   tri2_dev[v] = sum_{u in N(v)} P(v, u)                         (twice nx.triangles)
+ *   sq_dev[v]   = sum_{y != v} P(v, y) (P(v, y) - 1) / 2
+ *   pot_dev[v]  = (sum_{u in N(v)} d(u)) (d(v) - 1) - d(v) (d(v) - 1) - tri2[v] - sq[v]
+ * so that nx.clustering = tri2 / (d (d - 1)) (0 if tri2 = 0) and nx.square_clustering = sq / pot (0 if d < 2 or
+ * pot <= 0), exactly, in float64.  The results are integers and do not depend on scheduling.
+ *
+ * Workspace: kge_graph_workspace_bytes(n_nodes) bytes, 8-byte aligned, for the current device (a work counter, plus
+ * n_nodes int32 counters per CTA when they do not fit in shared memory: 2 CTAs per SM); 0 = invalid n_nodes or a
+ * failed device query.  The contents need no initialisation. */
+int kge_graph_counts(const int64_t *offsets_dev, const int32_t *nbr_dev, const int32_t *order_dev, int64_t n_nodes,
+                     int64_t *tri2_dev, int64_t *sq_dev, int64_t *pot_dev, void *workspace_dev, int64_t workspace_bytes,
+                     void *stream);
+int64_t kge_graph_workspace_bytes(int64_t n_nodes);
+
 #ifdef __cplusplus
 }
 #endif

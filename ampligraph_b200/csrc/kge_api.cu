@@ -11,6 +11,14 @@
 
 using namespace kge;
 
+// the training kernels, each with its own slot geometry (kge_handle::slot)
+enum TrainPath {
+    TRAIN_GENERAL,  // kge_train.cu: any shape
+    TRAIN_RES,      // kge_train_res.cu: the resident trilinear fast path
+    TRAIN_ROT,      // kge_train_rot.cu: the RotatE fast path
+    TRAIN_PATHS
+};
+
 struct kge_handle {
     kge_config cfg;
     Layout L;
@@ -22,10 +30,10 @@ struct kge_handle {
     float *rot;              // [n_rel, ld] rotation table (RotatE only)
     unsigned *done_counter;  // [0]: last-CTA counter of kge_optimizer_step_exchange; [1], [2]: the training kernels' positive counter and retired-warp counter (self-resetting)
     unsigned long long *exchange_trace;  // caller-owned 8 x uint64 phase stamps of the next exchange launches, or nullptr
-    // training launch geometry
-    int nit, G, nbuf, warps, eta_pad, rows_bytes, region_bytes, wk, n_cb, slot_floats, resident;
-    int res_warps, res_rows_bytes, res_region_bytes;  // slot geometry of the resident trilinear fast path (kge_train_res.cu); res_warps = 0: not applicable
-    int rot_warps, rot_G, rot_rows_bytes, rot_region_bytes;  // slot geometry of the RotatE fast path (kge_train_rot.cu); rot_warps = 0: not applicable
+    // training launch geometry: the row layout every kernel shares, then one slot per kernel
+    int nit, eta_pad, wk, n_cb, slot_floats;
+    int nbuf, resident;  // the general kernel's group buffers and residency (kge_rows_resident)
+    TrainSlot slot[TRAIN_PATHS];
     int *stamp_ent, *stamp_rel;  // lazy-optimizer row stamps (caller-owned) or nullptr
     float *stash;                // caller-owned row stash for sharded runs (kge_set_row_stash) or nullptr
     long long stash_rows;
@@ -172,36 +180,31 @@ extern "C" int kge_create(const kge_config *cfg, kge_handle **out)
         }
     }
     h->resident = res ? 1 : 0;
-    h->G = G;
     h->nbuf = nbuf;
-    h->rows_bytes = (res ? 3 + G : 3 + nbuf * G) * row_bytes;
-    h->region_bytes = h->rows_bytes + aux;
-    int warps = h->max_smem / h->region_bytes;
-    if (warps > max_warps) warps = max_warps;
-    h->warps = warps;  // 0 => even (3+1) windows do not fit (reported by kge_train_step)
+    {
+        const int rows = (res ? 3 + G : 3 + nbuf * G) * row_bytes, region = rows + aux;
+        const int warps = h->max_smem / region;  // 0 => even (3+1) windows do not fit (reported by kge_train_step)
+        h->slot[TRAIN_GENERAL] = {warps < max_warps ? warps : max_warps, G, rows, region};
+    }
     h->hot_ent[0] = h->hot_ent[1] = -1;
 
     // ---- the resident trilinear fast path (kge_train_res.cu): DistMult / ComplEx / HolE, one window, eta <= 32; its slot
     // holds s, o and the eta replaced rows (the relation row lives in registers) + sc | nid | jorig + one mbarrier.
     // Same residency rule as above, with its own (one row smaller) slot.
-    h->res_warps = 0;
     // DistMult rows of up to 512 floats (NIT = 4) qualify too: its per-lane state is a third of ComplEx's.
     if ((cfg->scoring == KGE_DISTMULT || cfg->scoring == KGE_COMPLEX || cfg->scoring == KGE_HOLE) && h->n_cb == 1 &&
         (h->nit <= 2 || cfg->scoring == KGE_DISTMULT) && cfg->eta <= 32 && cfg->neg_group <= 0) {
-        const int res_aux = (3 * h->eta_pad * 4 + 8 + 15) / 16 * 16;
-        h->res_rows_bytes = (2 + cfg->eta) * row_bytes;
-        h->res_region_bytes = h->res_rows_bytes + res_aux;
-        int rw = h->max_smem / h->res_region_bytes;
+        const int rows = (2 + cfg->eta) * row_bytes, region = rows + (3 * h->eta_pad * 4 + 8 + 15) / 16 * 16;
+        int rw = h->max_smem / region;
         if (rw > max_warps) rw = max_warps;
         int min_res = max_warps < KGE_MIN_RESIDENT_WARPS ? max_warps : KGE_MIN_RESIDENT_WARPS;
         if (h->nit == 4) min_res = KGE_MIN_RESIDENT_WARPS_WIDE;
         if (const char *ev = getenv("KGE_B200_RES_MIN_WARPS")) min_res = atoi(ev);  // tuning aid
-        if (rw >= min_res) h->res_warps = rw;
+        if (rw >= min_res) h->slot[TRAIN_RES] = {rw, cfg->eta, rows, region};
     }
 
     // ---- the RotatE fast path (kge_train_rot.cu): one window, rows of up to 256 floats per half; its slot holds ONLY replaced
     // rows (s, o and the rotation row live in registers): all eta of them when they fit beside 8 warps, else two buffers of G.
-    h->rot_warps = 0;
     if (cfg->scoring == KGE_ROTATE && h->n_cb == 1 && h->nit <= 2 && cfg->neg_group <= 0) {
         const int rot_aux = (4 * h->eta_pad * 4 + 16 + 15) / 16 * 16;  // sc | nid | jorig | side, two mbarriers
         const int rw = 8;                                                // 256 threads (launch bound of the kernel)
@@ -211,12 +214,8 @@ extern "C" int kge_create(const kge_config *cfg, kge_handle **out)
             const int g = atoi(ev);
             if (g >= 1 && g <= cap / 2 && g < cfg->eta) rG = g;
         }
-        if (rG >= 1) {
-            h->rot_warps = rw;
-            h->rot_G = rG;
-            h->rot_rows_bytes = (rG >= cfg->eta ? rG : 2 * rG) * row_bytes;
-            h->rot_region_bytes = h->rot_rows_bytes + rot_aux;
-        }
+        const int rows = (rG >= cfg->eta ? rG : 2 * rG) * row_bytes;
+        if (rG >= 1) h->slot[TRAIN_ROT] = {rw, rG, rows, rows + rot_aux};
     }
 
     if (cfg->scoring == KGE_ROTATE) {
@@ -361,41 +360,56 @@ static int check_shard_map(const kge_handle *h, const kge_shard_map *map, const 
     return KGE_OK;
 }
 
+// Bump allocation of a caller-owned workspace: each region starts at a multiple of its alignment and is padded to one;
+// `at` is the bytes taken so far.  base == nullptr only sizes the workspace (every region is then nullptr).
+struct Carve {
+    char *base;
+    size_t at = 0;
+    explicit Carve(void *ws) : base(static_cast<char *>(ws)) {}
+    template <class T> T *take(size_t bytes, size_t align)
+    {
+        at = (at + align - 1) / align * align;
+        T *q = base ? reinterpret_cast<T *>(base + at) : nullptr;
+        at += (bytes + align - 1) / align * align;
+        return q;
+    }
+};
+
 // Carve-up of the training workspace for a batch of B positives (the owner-computes path of the resident kernel,
 // kge_train_bucket.cu): the per-entity counts first, so that they stay where kge_set_train_workspace zeroed them whatever B is.
-static long long carve_train_workspace(const kge_handle *h, int64_t B, char *base, TrainParams::Buckets *bk)
+static TrainParams::Buckets carve_train_workspace(const kge_handle *h, int64_t B, Carve &c)
 {
-    const long long E = h->cfg.n_ent, n = (long long)h->cfg.eta * B;
-    auto al = [](long long x) { return (x + 15) & ~15ll; };
-    long long at = 0;
-    auto take = [&](long long bytes) { char *q = base ? base + at : nullptr; at += al(bytes); return q; };
-    char *cnt = take(4 * E), *off = take(4 * (E + 1)), *tiles = take(4 * ((E + 8191) / 8192)), *pos = take(4 * n),
-         *eid = take(4 * n), *other = take(4 * n), *rel = take(4 * n), *g = take(4 * n);
-    if (bk) {
-        bk->cnt = reinterpret_cast<int *>(cnt); bk->off = reinterpret_cast<int *>(off); bk->tiles = reinterpret_cast<int *>(tiles);
-        bk->pos = reinterpret_cast<int *>(pos);
-        bk->eid = reinterpret_cast<int *>(eid); bk->other = reinterpret_cast<int *>(other); bk->rel = reinterpret_cast<int *>(rel);
-        bk->g = reinterpret_cast<float *>(g);
-    }
-    return at;
+    const size_t E = h->cfg.n_ent, n = (size_t)h->cfg.eta * B;
+    TrainParams::Buckets bk;
+    bk.cnt = c.take<int>(4 * E, 16);
+    bk.off = c.take<int>(4 * (E + 1), 16);
+    bk.tiles = c.take<int>(4 * ((E + 8191) / 8192), 16);
+    bk.pos = c.take<int>(4 * n, 16);
+    bk.eid = c.take<int>(4 * n, 16);
+    bk.other = c.take<int>(4 * n, 16);
+    bk.rel = c.take<int>(4 * n, 16);
+    bk.g = c.take<float>(4 * n, 16);
+    return bk;
 }
 
-// Whether a fused step of B positives takes the owner-computes path (given a workspace): the resident kernel applies, the
-// step replaces every entity at least once on average (eta*B >= n_ent), and KGE_B200_TRAIN_REPL=scatter (A/B runs, the
-// tests that compare the two) does not keep the REDs.  The bucket sum reads one kept-side entity row per corruption; it
-// pays where replaced entities repeat within a step (measured on H100: cfg2, 19 corruptions per entity, and cfg3, 4.2,
-// gain) and loses where they do not ('big' in scripts/kbench.py: 2 M entities, 0.33 per entity, HBM-resident, 1.65 ->
-// 1.88 ms; DESIGN.md 5).
-static bool bucket_applies(const kge_handle *h, int64_t B)
+// Bytes of training workspace the owner-computes path needs for a step of B positives, or 0 where it does not apply: it
+// applies where the resident kernel does, the step replaces every entity at least once on average (eta*B >= n_ent), and
+// KGE_B200_TRAIN_REPL=scatter (A/B runs, the tests that compare the two) does not keep the REDs.  The bucket sum reads one
+// kept-side entity row per corruption; it pays where replaced entities repeat within a step (measured on H100: cfg2, 19
+// corruptions per entity, and cfg3, 4.2, gain) and loses where they do not ('big' in scripts/kbench.py: 2 M entities, 0.33
+// per entity, HBM-resident, 1.65 -> 1.88 ms; DESIGN.md 5).
+static int64_t bucket_workspace_bytes(const kge_handle *h, int64_t B)
 {
     const char *rv = getenv("KGE_B200_TRAIN_REPL");
-    return h->res_warps > 0 && (long long)h->cfg.eta * B >= h->cfg.n_ent && !(rv && strcmp(rv, "scatter") == 0);
+    if (h->slot[TRAIN_RES].warps == 0 || (long long)h->cfg.eta * B < h->cfg.n_ent || (rv && strcmp(rv, "scatter") == 0)) return 0;
+    Carve c(nullptr);
+    carve_train_workspace(h, B, c);
+    return (int64_t)c.at;
 }
 
 extern "C" int64_t kge_train_workspace_bytes(const kge_handle *h, int64_t B)
 {
-    if (!h || B < 0 || !bucket_applies(h, B)) return 0;
-    return carve_train_workspace(h, B, nullptr, nullptr);
+    return h && B >= 0 ? bucket_workspace_bytes(h, B) : 0;
 }
 
 extern "C" int kge_set_train_workspace(kge_handle *h, void *ws_dev, int64_t bytes, void *stream)
@@ -403,12 +417,26 @@ extern "C" int kge_set_train_workspace(kge_handle *h, void *ws_dev, int64_t byte
     KGE_CHECK_HANDLE(h, "kge_set_train_workspace");
     if (bytes < 0 || (ws_dev && ((uintptr_t)ws_dev & 15)))
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_set_train_workspace: bytes < 0 or workspace not 16-byte aligned");
-    if (ws_dev && bytes < carve_train_workspace(h, 0, nullptr, nullptr))
+    Carve counts(nullptr);
+    carve_train_workspace(h, 0, counts);
+    if (ws_dev && bytes < (int64_t)counts.at)
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_set_train_workspace: %lld bytes do not hold the per-entity counts", (long long)bytes);
     if (ws_dev) KGE_CUDA(cudaMemsetAsync(ws_dev, 0, 4 * (size_t)h->cfg.n_ent, (cudaStream_t)stream), "kge_set_train_workspace");
     h->train_ws = ws_dev;
     h->train_ws_bytes = ws_dev ? bytes : 0;
     return KGE_OK;
+}
+
+// The kernel a training step runs: a fast path where its slot applies, on one (not row-sharded) table and without a row
+// stash; the general kernel otherwise, and for every shape under KGE_B200_TRAIN_KERNEL=general (A/B runs, and the tests
+// that cover its resident trilinear instantiations).
+static TrainPath train_path(const kge_handle *h, const kge_shard_map *map, const float *stash)
+{
+    const char *force = getenv("KGE_B200_TRAIN_KERNEL");
+    if ((map && map->world > 1) || stash || (force && strcmp(force, "general") == 0)) return TRAIN_GENERAL;
+    if (h->slot[TRAIN_ROT].warps > 0) return TRAIN_ROT;
+    if (h->slot[TRAIN_RES].warps > 0) return TRAIN_RES;
+    return TRAIN_GENERAL;
 }
 
 static int train_step_impl(kge_handle *h, int32_t mode, const kge_shard_map *map, const float *ent_dev,
@@ -432,9 +460,9 @@ static int train_step_impl(kge_handle *h, int32_t mode, const kge_shard_map *map
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_train_step: BACKWARD_EXT needs dpos_dev and dneg_dev");
     if (mode == KGE_STEP_FORWARD_ONLY && (!scores_pos_dev || !scores_neg_dev))
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_train_step: FORWARD_ONLY needs both score outputs");
-    if (h->warps < 1)
+    if (h->slot[TRAIN_GENERAL].warps < 1)
         return fail(KGE_ERR_UNSUPPORTED, "kge_train_step: one positive's working set (%d B) exceeds shared memory (%d B)",
-                    h->region_bytes, h->max_smem);
+                    h->slot[TRAIN_GENERAL].region_bytes, h->max_smem);
     cudaStream_t st = (cudaStream_t)stream;
     if (int rc = refresh_rotation(h, rel_dev, st)) return rc;
 
@@ -456,15 +484,12 @@ static int train_step_impl(kge_handle *h, int32_t mode, const kge_shard_map *map
     p.kp = h->L.kp;
     p.ld = h->L.ld;
     p.nch = h->L.kp / 4;
-    p.G = h->G;
     p.nbuf = h->nbuf;
     p.wk = h->wk;
     p.n_cb = h->n_cb;
     p.slot_floats = h->slot_floats;
     p.resident = h->resident;
     p.eta_pad = h->eta_pad;
-    p.rows_bytes = h->rows_bytes;
-    p.region_bytes = h->region_bytes;
     p.loss = h->cfg.loss;
     p.reduction = h->cfg.reduction;
     p.mode = mode;
@@ -497,17 +522,18 @@ static int train_step_impl(kge_handle *h, int32_t mode, const kge_shard_map *map
         p.rows_per_shard = (int)map->rows_per_shard;
         for (int q = 0; q < map->world; ++q) { p.ent_shard[q] = map->ent[q]; p.grad_ent_shard[q] = map->grad_ent[q]; }
     }
-    // KGE_B200_TRAIN_KERNEL=general keeps every shape on the general kernel (A/B runs, and the tests that cover its resident
-    // trilinear instantiations); default: the specialised kernel of kge_train_res.cu where it applies
-    const char *force = getenv("KGE_B200_TRAIN_KERNEL");
-    const bool fast = h->res_warps > 0 && p.shard_world <= 1 && p.stash == nullptr && !(force && strcmp(force, "general") == 0);
+    const TrainPath path = train_path(h, map, p.stash);
+    const TrainSlot &slot = h->slot[path];
+    p.G = slot.G;
+    p.rows_bytes = slot.rows_bytes;
+    p.region_bytes = slot.region_bytes;
     // Dynamic assignment of positives to warps (kge_train_common.cuh) where it was measured to pay before the H100 port: the resident fast path on
     // tables that live in L2 with enough positives per warp for the imbalance to matter (cfg2).  On an HBM-resident table it
     // LOSES (and the general kernel on cfg4 / cfg5w gains nothing), so those keep the static stride.  KGE_B200_TRAIN_SCHED=static|dynamic forces.
     {
         const char *ev = getenv("KGE_B200_TRAIN_SCHED");
-        const long long n_warps = (long long)h->sm_count * (fast ? h->res_warps : h->warps);
-        bool dyn = fast && B >= 8 * n_warps && 2ll * h->cfg.n_ent * h->L.ld * 4 <= (long long)h->l2_bytes;
+        const long long n_warps = (long long)h->sm_count * slot.warps;
+        bool dyn = path == TRAIN_RES && B >= 8 * n_warps && 2ll * h->cfg.n_ent * h->L.ld * 4 <= (long long)h->l2_bytes;
         if (ev && strcmp(ev, "static") == 0) dyn = false;
         if (ev && strcmp(ev, "dynamic") == 0) dyn = true;
         p.sched = (dyn && B < (1ll << 24)) ? h->done_counter + 1 : nullptr;  // float counter: exact below 2^24
@@ -516,32 +542,26 @@ static int train_step_impl(kge_handle *h, int32_t mode, const kge_shard_map *map
         // time in bench.py's workload.  It stays in effect for the static stride, where it pays.
         if (p.sched) p.hot_ent[0] = p.hot_ent[1] = -1;
     }
-    if (h->rot_warps > 0 && p.shard_world <= 1 && p.stash == nullptr && !(force && strcmp(force, "general") == 0)) {
-        p.G = h->rot_G;
-        p.rows_bytes = h->rot_rows_bytes;
-        p.region_bytes = h->rot_region_bytes;
-        KGE_CUDA(launch_train_rot(p, h->nit, h->sm_count, h->rot_warps * 32, (size_t)h->rot_warps * h->rot_region_bytes, st),
-                 "kge_train_step");
+    if (path == TRAIN_ROT) {
+        KGE_CUDA(launch_train_rot(p, h->nit, slot, h->sm_count, st), "kge_train_step");
         return KGE_OK;
     }
-    if (fast) {
-        p.rows_bytes = h->res_rows_bytes;
-        p.region_bytes = h->res_region_bytes;
-        // Owner-computes gradient of the replaced rows (kge_train_bucket.cu) where it applies (bucket_applies) and a workspace
-        // is set: on H100 the eta*B uniformly scattered row REDs it removes cost about half the kernel (DESIGN.md 3.2, 5).
-        const bool gather = mode != KGE_STEP_FORWARD_ONLY && h->train_ws != nullptr && bucket_applies(h, B) &&
-                            (long long)h->cfg.eta * B < (1ll << 31) && carve_train_workspace(h, B, nullptr, nullptr) <= h->train_ws_bytes;
+    if (path == TRAIN_RES) {
+        // Owner-computes gradient of the replaced rows (kge_train_bucket.cu) where it applies and the workspace set holds it
+        // (train_ws_bytes is 0 without one): on H100 the eta*B uniformly scattered row REDs it removes cost about half the
+        // kernel (DESIGN.md 3.2, 5).
+        const int64_t need = mode != KGE_STEP_FORWARD_ONLY ? bucket_workspace_bytes(h, B) : 0;
+        const bool gather = need > 0 && need <= h->train_ws_bytes && (long long)h->cfg.eta * B < (1ll << 31);
         if (gather) {
-            carve_train_workspace(h, B, static_cast<char *>(h->train_ws), &p.bk);
+            Carve c(h->train_ws);
+            p.bk = carve_train_workspace(h, B, c);
             KGE_CUDA(launch_bucket_prepass(p, st), "kge_train_step (bucket pre-pass)");
         }
-        KGE_CUDA(launch_train_res(p, h->nit, h->sm_count, h->res_warps * 32, (size_t)h->res_warps * h->res_region_bytes, st),
-                 "kge_train_step");
+        KGE_CUDA(launch_train_res(p, h->nit, slot, h->sm_count, st), "kge_train_step");
         if (gather) KGE_CUDA(launch_bucket_sum(p, h->nit, st), "kge_train_step (bucket sum)");
         return KGE_OK;
     }
-    KGE_CUDA(launch_train(p, h->nit, h->sm_count, h->warps * 32, (size_t)h->warps * h->region_bytes, st),
-             "kge_train_step");
+    KGE_CUDA(launch_train(p, h->nit, slot, h->sm_count, st), "kge_train_step");
     return KGE_OK;
 }
 
@@ -792,37 +812,73 @@ struct RankWorkspace {
     bool tc;                 // tensor-core filter region present (KGE_RANK_MODE_AUTO, bilinear model, large enough call)
     RankTcLayout tcl;
     void *tc_base;
-    size_t bytes;
 };
-static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 // tc_region = false: never carve the tensor-core region (kge_topk runs the exact chain only)
-static RankWorkspace carve_rank_workspace(const kge_handle *h, void *base, int64_t b, int64_t n_cand, bool tc_region = true)
+static RankWorkspace carve_rank_workspace(const kge_handle *h, Carve &c, int64_t b, int64_t n_cand, bool tc_region)
 {
     RankWorkspace w;
-    char *p = (char *)base;
-    size_t off = 0;
-    const size_t qbytes = align256((size_t)b * h->L.ld * sizeof(float));
-    w.qs = (float *)(p + off); off += qbytes;
-    w.qo = (float *)(p + off); off += qbytes;
-    w.qaux = (float *)(p + off); off += qbytes;
-    w.qpos = (int32_t *)(p + off); off += align256((size_t)b * sizeof(int32_t));
-    w.cnt = (int32_t *)(p + off); off += align256((size_t)3 * b * sizeof(int32_t));
+    const size_t qbytes = (size_t)b * h->L.ld * sizeof(float);
+    w.qs = c.take<float>(qbytes, 256);
+    w.qo = c.take<float>(qbytes, 256);
+    w.qaux = c.take<float>(qbytes, 256);
+    w.qpos = c.take<int32_t>((size_t)b * sizeof(int32_t), 256);
+    w.cnt = c.take<int32_t>((size_t)3 * b * sizeof(int32_t), 256);
     w.tc = tc_region && h->cfg.rank_mode == KGE_RANK_MODE_AUTO && rank_tc_applicable(h->L, 0, b, n_cand);
     w.tc_base = nullptr;
     if (w.tc) {
-        off = (off + 1023) & ~(size_t)1023;
         w.tcl = rank_tc_layout(h->L, b, n_cand, h->cfg.rank_pair_cap);
-        w.tc_base = p + off;
-        off += w.tcl.bytes;
+        w.tc_base = c.take<char>(w.tcl.bytes, 1024);  // a multiple of 1024
     }
-    w.bytes = off;
     return w;
 }
 
 extern "C" int64_t kge_rank_workspace_bytes(const kge_handle *h, int64_t b, int64_t n_cand)
 {
     if (!h || b < 0 || n_cand < 0) return 0;
-    return (int64_t)carve_rank_workspace(h, nullptr, b, n_cand).bytes;
+    Carve c(nullptr);
+    carve_rank_workspace(h, c, b, n_cand, true);
+    return (int64_t)c.at;
+}
+
+// A caller-owned workspace of `need` bytes (fn_workspace_bytes), 1024-byte aligned
+static int check_workspace(void *ws, int64_t bytes, int64_t need, const char *fn)
+{
+    if (!ws || bytes < need)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "%s: workspace of %lld bytes needed (%s_workspace_bytes), got %lld", fn,
+                    (long long)need, fn, (long long)(ws ? bytes : 0));
+    if (((uintptr_t)ws & 1023u) != 0) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: workspace must be 1024-byte aligned", fn);
+    return KGE_OK;
+}
+
+// The candidate window of a call over n_rows rows (named `rows` in the message): explicit ids, or the range
+// [cand_begin, cand_begin + n_cand)
+static int check_candidates(const char *fn, const int32_t *cand_ids, int64_t cand_begin, int64_t n_cand, int64_t n_rows,
+                            const char *rows)
+{
+    if (cand_ids && cand_begin != 0) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: cand_begin must be 0 with cand_ids_dev", fn);
+    if (!cand_ids && cand_begin + n_cand > n_rows)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "%s: candidate range [%lld,%lld) exceeds %s %lld", fn, (long long)cand_begin,
+                    (long long)(cand_begin + n_cand), rows, (long long)n_rows);
+    return KGE_OK;
+}
+
+// The scoring parameters of b model queries prepared into w (launch_rank_prepare) against the entity rows ent; the
+// candidate window and the outputs are the caller's
+static RankParams query_rank_params(const kge_handle *h, const RankWorkspace &w, int32_t side, int32_t strategy,
+                                    const float *ent, int64_t b)
+{
+    RankParams p;
+    memset(&p, 0, sizeof(p));
+    p.L = h->L;
+    p.side = side;
+    p.strategy = strategy;
+    p.ent = ent;
+    p.qvec = side == KGE_SIDE_S ? w.qs : w.qo;
+    p.qaux = w.qaux;
+    p.qpos = w.qpos;
+    p.b = b;
+    p.scale = h->score_scale;
+    return p;
 }
 
 static int rank_impl(kge_handle *h, const kge_shard_map *map, int64_t filt_base, int32_t side, int32_t strategy,
@@ -840,19 +896,15 @@ static int rank_impl(kge_handle *h, const kge_shard_map *map, int64_t filt_base,
     if (b == 0) return KGE_OK;
     if (!ent_dev || !rel_dev || !triples_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_rank: null pointer");
     if (!ranks_dev && !counts_dev && !scores_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_rank: no output buffer");
-    if (cand_ids_dev && cand_begin != 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_rank: cand_begin must be 0 with cand_ids_dev");
-    if (!map && !cand_ids_dev && cand_begin + n_cand > h->cfg.n_ent)
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_rank: candidate range [%lld,%lld) exceeds n_ent %lld",
-                    (long long)cand_begin, (long long)(cand_begin + n_cand), (long long)h->cfg.n_ent);
+    // (a shard's window [0, n_local) always lies inside n_ent)
+    if (int rc = check_candidates("kge_rank", cand_ids_dev, cand_begin, n_cand, h->cfg.n_ent, "n_ent")) return rc;
+    // both filter pointers null with n_filt > 0: nothing is filtered (kge_topk / kge_knn reject that)
     if ((filt_off_dev == nullptr) != (filt_idx_dev == nullptr) && n_filt > 0)
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_rank: filter offsets and indices must be given together");
-    const int64_t need = kge_rank_workspace_bytes(h, b, n_cand);
-    if (!workspace_dev || workspace_bytes < need)
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_rank: workspace of %lld bytes needed (kge_rank_workspace_bytes), got %lld",
-                    (long long)need, (long long)(workspace_dev ? workspace_bytes : 0));
-    if (((uintptr_t)workspace_dev & 1023u) != 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_rank: workspace must be 1024-byte aligned");
+    if (int rc = check_workspace(workspace_dev, workspace_bytes, kge_rank_workspace_bytes(h, b, n_cand), "kge_rank")) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    const RankWorkspace w = carve_rank_workspace(h, workspace_dev, b, n_cand);
+    Carve c(workspace_dev);
+    const RankWorkspace w = carve_rank_workspace(h, c, b, n_cand, true);
     if (int rc = refresh_rotation(h, rel_dev, st)) return rc;
     ShardView sv;
     memset(&sv, 0, sizeof(sv));
@@ -867,20 +919,10 @@ static int rank_impl(kge_handle *h, const kge_shard_map *map, int64_t filt_base,
     // raw counters of THIS call in a zeroed scratch; added to the caller's accumulator or finalized into ranks_dev below
     int32_t *cnt = w.cnt;
     KGE_CUDA(cudaMemsetAsync(cnt, 0, (size_t)3 * b * sizeof(int32_t), st), "kge_rank: memset");
-    RankParams p;
-    memset(&p, 0, sizeof(p));
-    p.L = h->L;
-    p.side = side;
-    p.strategy = strategy;
-    p.ent = ent_dev;
-    p.qvec = side == KGE_SIDE_S ? w.qs : w.qo;
-    p.qaux = w.qaux;
-    p.qpos = w.qpos;
+    RankParams p = query_rank_params(h, w, side, strategy, ent_dev, b);
     p.cand_ids = cand_ids_dev;
     p.cand_begin = cand_begin;
     p.n_cand = n_cand;
-    p.b = b;
-    p.scale = h->score_scale;
     p.filt_base = filt_base;
     p.scores = scores_dev;
     if (probe_delta_dev) {  // kge_rank_filter_probe: approximate scores + assumed bound, nothing is counted
@@ -965,16 +1007,13 @@ struct TopkLists {
     unsigned long long *keys;
     float *vals;
     int2 *state;
-    size_t bytes;
 };
-static TopkLists carve_topk_lists(void *base, size_t off, int64_t b, int32_t k)
+static TopkLists carve_topk_lists(Carve &c, int64_t b, int32_t k)
 {
     TopkLists l;
-    char *p = (char *)base;
-    l.keys = (unsigned long long *)(p + off); off += align256((size_t)2 * b * k * sizeof(unsigned long long));
-    l.vals = (float *)(p + off); off += align256((size_t)2 * b * k * sizeof(float));
-    l.state = (int2 *)(p + off); off += align256((size_t)b * sizeof(int2));
-    l.bytes = off;
+    l.keys = c.take<unsigned long long>((size_t)2 * b * k * sizeof(unsigned long long), 256);
+    l.vals = c.take<float>((size_t)2 * b * k * sizeof(float), 256);
+    l.state = c.take<int2>((size_t)b * sizeof(int2), 256);
     return l;
 }
 // Candidates per chunk: the [b, C] fp32 chunk the scoring kernel writes and the select kernel reads back is sized to the
@@ -999,35 +1038,77 @@ struct TopkWorkspace {
     float *chunk;     // [b, C]
     TopkLists l;
 };
-static TopkWorkspace carve_topk_workspace(const kge_handle *h, void *base, int64_t b, int64_t n_cand, int32_t k)
+static TopkWorkspace carve_topk_workspace(const kge_handle *h, Carve &c, int64_t b, int64_t n_cand, int32_t k)
 {
     TopkWorkspace w;
-    w.r = carve_rank_workspace(h, base, b, n_cand, false);
-    size_t off = w.r.bytes;
-    w.chunk = (float *)((char *)base + off);
-    off += align256((size_t)b * topk_chunk(h, b, n_cand) * sizeof(float));
-    w.l = carve_topk_lists(base, off, b, k);
+    w.r = carve_rank_workspace(h, c, b, n_cand, false);
+    w.chunk = c.take<float>((size_t)b * topk_chunk(h, b, n_cand) * sizeof(float), 256);
+    w.l = carve_topk_lists(c, b, k);
     return w;
 }
 
 extern "C" int64_t kge_topk_workspace_bytes(const kge_handle *h, int64_t b, int64_t n_cand, int32_t k)
 {
     if (!h || b < 0 || n_cand < 0 || k < 1) return 0;
-    return (int64_t)carve_topk_workspace(h, nullptr, b, n_cand, k).l.bytes;
+    Carve c(nullptr);
+    carve_topk_workspace(h, c, b, n_cand, k);
+    return (int64_t)c.at;
 }
 
 extern "C" int64_t kge_select_topk_workspace_bytes(const kge_handle *h, int64_t b, int64_t n, int32_t k)
 {
     if (!h || b < 0 || n < 0 || k < 1) return 0;
-    return (int64_t)carve_topk_lists(nullptr, 0, b, k).bytes;
+    Carve c(nullptr);
+    carve_topk_lists(c, b, k);
+    return (int64_t)c.at;
 }
 
-static int check_topk_workspace(void *ws, int64_t bytes, int64_t need, const char *fn)
+// The select of b running top-k lists over chunks of scores; with n_filt > 0 the filter pairs exclude the candidate
+// positions filt_idx - filt_shift
+static TopkSelectParams topk_select_params(const float *scores, int64_t b, int32_t k, const TopkLists &l,
+                                           const int64_t *filt_off, const int32_t *filt_idx, int64_t n_filt, int64_t filt_shift)
 {
-    if (!ws || bytes < need)
-        return fail(KGE_ERR_INVALID_ARGUMENT, "%s: workspace of %lld bytes needed (%s_workspace_bytes), got %lld", fn,
-                    (long long)need, fn, (long long)(ws ? bytes : 0));
-    if (((uintptr_t)ws & 1023u) != 0) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: workspace must be 1024-byte aligned", fn);
+    TopkSelectParams s;
+    memset(&s, 0, sizeof(s));
+    s.scores = scores;
+    s.b = b;
+    s.k = k;
+    if (n_filt > 0) { s.filt_off = (const long long *)filt_off; s.filt_idx = filt_idx; }
+    s.filt_shift = filt_shift;
+    s.keys = l.keys;
+    s.vals = l.vals;
+    s.state = l.state;
+    return s;
+}
+// one chunk of nc columns (row stride nc), the candidate positions c0.., into the running lists
+static cudaError_t select_chunk(TopkSelectParams s, int64_t nc, int64_t c0, cudaStream_t st)
+{
+    s.ld = s.n = nc;
+    s.base = c0;
+    return launch_topk_select(s, st);
+}
+
+static int stage_fail(cudaError_t e, const char *fn, const char *stage)
+{
+    return fail(KGE_ERR_CUDA, "%s: %s: %s (%s)", fn, stage, cudaGetErrorName(e), cudaGetErrorString(e));
+}
+
+// The chunked candidate sweep of kge_topk, kge_knn and the radius calls, over the b queries the caller prepared for p:
+// for every chunk of topk_chunk candidates, score them with chain `op` into p.scores ([b, nc], row stride nc), then run
+// epilogue(nc, c0).  CUDA errors are reported as "<fn>: <stage>".
+template <class Epilogue>
+static int sweep(const kge_handle *h, const char *fn, const char *stage, RankParams p, int op, int32_t *cnt,
+                 const int32_t *cand_ids, int64_t cand_begin, int64_t n_cand, cudaStream_t st, Epilogue epilogue)
+{
+    const int64_t C = topk_chunk(h, p.b, n_cand);
+    for (int64_t c0 = 0; c0 < n_cand; c0 += C) {
+        const int64_t nc = n_cand - c0 < C ? n_cand - c0 : C;
+        p.cand_ids = cand_ids ? cand_ids + c0 : nullptr;
+        p.cand_begin = cand_ids ? 0 : cand_begin + c0;
+        p.n_cand = nc;
+        if (cudaError_t e = launch_rank_count_op(p, op, cnt, st)) return stage_fail(e, fn, "scores");
+        if (cudaError_t e = epilogue(nc, c0)) return stage_fail(e, fn, stage);
+    }
     return KGE_OK;
 }
 
@@ -1043,15 +1124,13 @@ extern "C" int kge_topk(kge_handle *h, int32_t side, const float *ent_dev, const
     if (n_cand > 0x7fffffffLL) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_topk: n_cand must be < 2^31");
     if (b == 0) return KGE_OK;
     if (!ent_dev || !rel_dev || !triples_dev || !ids_dev || !scores_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_topk: null pointer");
-    if (cand_ids_dev && cand_begin != 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_topk: cand_begin must be 0 with cand_ids_dev");
-    if (!cand_ids_dev && cand_begin + n_cand > h->cfg.n_ent)
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_topk: candidate range [%lld,%lld) exceeds n_ent %lld", (long long)cand_begin,
-                    (long long)(cand_begin + n_cand), (long long)h->cfg.n_ent);
+    if (int rc = check_candidates("kge_topk", cand_ids_dev, cand_begin, n_cand, h->cfg.n_ent, "n_ent")) return rc;
     if ((filt_off_dev == nullptr || filt_idx_dev == nullptr) && n_filt > 0)
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_topk: filter offsets and indices must be given together");
-    if (int rc = check_topk_workspace(workspace_dev, workspace_bytes, kge_topk_workspace_bytes(h, b, n_cand, k), "kge_topk")) return rc;
+    if (int rc = check_workspace(workspace_dev, workspace_bytes, kge_topk_workspace_bytes(h, b, n_cand, k), "kge_topk")) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    const TopkWorkspace w = carve_topk_workspace(h, workspace_dev, b, n_cand, k);
+    Carve c(workspace_dev);
+    const TopkWorkspace w = carve_topk_workspace(h, c, b, n_cand, k);
     if (int rc = refresh_rotation(h, rel_dev, st)) return rc;
     ShardView sv;
     memset(&sv, 0, sizeof(sv));
@@ -1059,41 +1138,13 @@ extern "C" int kge_topk(kge_handle *h, int32_t side, const float *ent_dev, const
                                  w.r.qpos, st),
              "kge_topk: prepare");
     KGE_CUDA(cudaMemsetAsync(w.l.state, 0, (size_t)b * sizeof(int2), st), "kge_topk: memset");
-    RankParams p;
-    memset(&p, 0, sizeof(p));
-    p.L = h->L;
-    p.side = side;
-    p.strategy = KGE_RANK_WORST;
-    p.ent = ent_dev;
-    p.qvec = side == KGE_SIDE_S ? w.r.qs : w.r.qo;
-    p.qaux = w.r.qaux;
-    p.qpos = w.r.qpos;
-    p.b = b;
-    p.scale = h->score_scale;
+    // the exact FP32 chain in every rank_mode: scores bit-identical to kge_corruption_scores
+    RankParams p = query_rank_params(h, w.r, side, KGE_RANK_WORST, ent_dev, b);
     p.scores = w.chunk;
-    TopkSelectParams s;
-    memset(&s, 0, sizeof(s));
-    s.scores = w.chunk;
-    s.b = b;
-    s.k = k;
-    if (n_filt > 0) { s.filt_off = (const long long *)filt_off_dev; s.filt_idx = filt_idx_dev; }
-    s.filt_shift = cand_ids_dev ? 0 : cand_begin;
-    s.keys = w.l.keys;
-    s.vals = w.l.vals;
-    s.state = w.l.state;
-    const int64_t C = topk_chunk(h, b, n_cand);
-    for (int64_t c0 = 0; c0 < n_cand; c0 += C) {
-        const int64_t nc = n_cand - c0 < C ? n_cand - c0 : C;
-        // the exact FP32 chain in every rank_mode: scores bit-identical to kge_corruption_scores ([b, nc], row stride nc)
-        p.cand_ids = cand_ids_dev ? cand_ids_dev + c0 : nullptr;
-        p.cand_begin = cand_ids_dev ? 0 : cand_begin + c0;
-        p.n_cand = nc;
-        KGE_CUDA(launch_rank_count(p, w.r.cnt, st), "kge_topk: scores");
-        s.ld = nc;
-        s.n = nc;
-        s.base = c0;
-        KGE_CUDA(launch_topk_select(s, st), "kge_topk: select");
-    }
+    const TopkSelectParams s = topk_select_params(w.chunk, b, k, w.l, filt_off_dev, filt_idx_dev, n_filt, cand_ids_dev ? 0 : cand_begin);
+    if (int rc = sweep(h, "kge_topk", "select", p, rank_op(h->L.model, side), w.r.cnt, cand_ids_dev, cand_begin, n_cand, st,
+                       [&](int64_t nc, int64_t c0) { return select_chunk(s, nc, c0, st); }))
+        return rc;
     KGE_CUDA(launch_topk_write(w.l.state, w.l.keys, w.l.vals, b, k, cand_ids_dev, cand_begin, ids_dev, scores_dev, st),
              "kge_topk: write");
     return KGE_OK;
@@ -1108,22 +1159,13 @@ extern "C" int kge_select_topk(kge_handle *h, const float *scores_dev, int64_t b
     if (n > 0x7fffffffLL) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_select_topk: n must be < 2^31");
     if (b == 0) return KGE_OK;
     if ((n > 0 && !scores_dev) || !pos_dev || !out_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_select_topk: null pointer");
-    if (int rc = check_topk_workspace(workspace_dev, workspace_bytes, kge_select_topk_workspace_bytes(h, b, n, k), "kge_select_topk"))
+    if (int rc = check_workspace(workspace_dev, workspace_bytes, kge_select_topk_workspace_bytes(h, b, n, k), "kge_select_topk"))
         return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    const TopkLists l = carve_topk_lists(workspace_dev, 0, b, k);
+    Carve c(workspace_dev);
+    const TopkLists l = carve_topk_lists(c, b, k);
     KGE_CUDA(cudaMemsetAsync(l.state, 0, (size_t)b * sizeof(int2), st), "kge_select_topk: memset");
-    TopkSelectParams s;
-    memset(&s, 0, sizeof(s));
-    s.scores = scores_dev;
-    s.ld = n;
-    s.n = n;
-    s.b = b;
-    s.k = k;
-    s.keys = l.keys;
-    s.vals = l.vals;
-    s.state = l.state;
-    KGE_CUDA(launch_topk_select(s, st), "kge_select_topk: select");
+    KGE_CUDA(select_chunk(topk_select_params(scores_dev, b, k, l, nullptr, nullptr, 0, 0), n, 0, st), "kge_select_topk: select");
     KGE_CUDA(launch_topk_write(l.state, l.keys, l.vals, b, k, nullptr, 0, pos_dev, out_dev, st), "kge_select_topk: write");
     return KGE_OK;
 }
@@ -1138,37 +1180,33 @@ struct KnnWorkspace {
     float *chunk;    // [b, C]
     TopkLists l;     // kge_knn
     long long *cursor;  // [b] kge_radius_neighbors
-    size_t bytes;
 };
-static KnnWorkspace carve_knn_workspace(const kge_handle *h, void *base, int64_t b, int64_t n_cand, int32_t k, int32_t ld)
+static KnnWorkspace carve_knn_workspace(const kge_handle *h, Carve &c, int64_t b, int64_t n_cand, int32_t k, int32_t ld)
 {
     KnnWorkspace w;
     memset(&w, 0, sizeof(w));
-    char *p = (char *)base;
-    size_t off = 0;
-    w.qvec = (float *)(p + off); off += align256((size_t)b * ld * sizeof(float));
-    w.cnt = (int32_t *)(p + off); off += align256((size_t)4 * b * sizeof(int32_t));
-    w.chunk = (float *)(p + off); off += align256((size_t)b * topk_chunk(h, b, n_cand) * sizeof(float));
-    if (k > 0) {
-        w.l = carve_topk_lists(base, off, b, k);
-        off = w.l.bytes;
-    } else {
-        w.cursor = (long long *)(p + off); off += align256((size_t)b * sizeof(long long));
-    }
-    w.bytes = off;
+    w.qvec = c.take<float>((size_t)b * ld * sizeof(float), 256);
+    w.cnt = c.take<int32_t>((size_t)4 * b * sizeof(int32_t), 256);
+    w.chunk = c.take<float>((size_t)b * topk_chunk(h, b, n_cand) * sizeof(float), 256);
+    if (k > 0) w.l = carve_topk_lists(c, b, k);
+    else w.cursor = c.take<long long>((size_t)b * sizeof(long long), 256);
     return w;
 }
 
 extern "C" int64_t kge_knn_workspace_bytes(const kge_handle *h, int64_t b, int64_t n_cand, int32_t k, int32_t ld)
 {
     if (!h || b < 0 || n_cand < 0 || k < 1 || ld < 4 || ld % 4) return 0;
-    return (int64_t)carve_knn_workspace(h, nullptr, b, n_cand, k, ld).bytes;
+    Carve c(nullptr);
+    carve_knn_workspace(h, c, b, n_cand, k, ld);
+    return (int64_t)c.at;
 }
 
 extern "C" int64_t kge_radius_workspace_bytes(const kge_handle *h, int64_t b, int64_t n_cand, int32_t ld)
 {
     if (!h || b < 0 || n_cand < 0 || ld < 4 || ld % 4) return 0;
-    return (int64_t)carve_knn_workspace(h, nullptr, b, n_cand, 0, ld).bytes;
+    Carve c(nullptr);
+    carve_knn_workspace(h, c, b, n_cand, 0, ld);
+    return (int64_t)c.at;
 }
 
 // the checks kge_knn and kge_radius_neighbors share (b > 0)
@@ -1181,11 +1219,7 @@ static int check_points(const char *fn, int32_t metric, const float *points_dev,
     if (n_points > 0x7fffffffLL) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: ids are int32 (n_points < 2^31)", fn);
     if (!points_dev || !query_ids_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: null pointer", fn);
     if (((uintptr_t)points_dev & 15u) != 0) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: points_dev must be 16-byte aligned", fn);
-    if (cand_ids_dev && cand_begin != 0) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: cand_begin must be 0 with cand_ids_dev", fn);
-    if (!cand_ids_dev && cand_begin + n_cand > n_points)
-        return fail(KGE_ERR_INVALID_ARGUMENT, "%s: candidate range [%lld,%lld) exceeds n_points %lld", fn, (long long)cand_begin,
-                    (long long)(cand_begin + n_cand), (long long)n_points);
-    return KGE_OK;
+    return check_candidates(fn, cand_ids_dev, cand_begin, n_cand, n_points, "n_points");
 }
 
 static RankParams knn_rank_params(int32_t ld, const float *points_dev, const KnnWorkspace &w, int64_t b)
@@ -1205,6 +1239,18 @@ static RankParams knn_rank_params(int32_t ld, const float *points_dev, const Knn
     return p;
 }
 
+// The sweep of kge_knn and the radius calls: gather the b query points, then sweep -d (the metric's chain) into w.chunk
+template <class Epilogue>
+static int point_sweep(const kge_handle *h, const char *fn, const char *stage, int32_t metric, const float *points_dev,
+                       int32_t ld, const int32_t *query_ids_dev, int64_t b, const int32_t *cand_ids_dev, int64_t cand_begin,
+                       int64_t n_cand, const KnnWorkspace &w, cudaStream_t st, Epilogue epilogue)
+{
+    if (cudaError_t e = launch_knn_gather(points_dev, ld, query_ids_dev, b, w.qvec, st)) return stage_fail(e, fn, "gather");
+    if (cudaError_t e = cudaMemsetAsync(w.cnt, 0, (size_t)4 * b * sizeof(int32_t), st)) return stage_fail(e, fn, "memset");
+    return sweep(h, fn, stage, knn_rank_params(ld, points_dev, w, b), metric == KGE_METRIC_EUCLIDEAN ? OP_L2_SUB : OP_L1_SUB,
+                 w.cnt, cand_ids_dev, cand_begin, n_cand, st, epilogue);
+}
+
 extern "C" int kge_knn(kge_handle *h, int32_t metric, const float *points_dev, int64_t n_points, int32_t ld,
                        const int32_t *query_ids_dev, int64_t b, const int32_t *cand_ids_dev, int64_t cand_begin, int64_t n_cand,
                        const int64_t *filt_off_dev, const int32_t *filt_idx_dev, int64_t n_filt, int32_t k, int32_t farthest,
@@ -1219,45 +1265,27 @@ extern "C" int kge_knn(kge_handle *h, int32_t metric, const float *points_dev, i
     if (!ids_dev || !dist_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_knn: null pointer");
     if ((filt_off_dev == nullptr || filt_idx_dev == nullptr) && n_filt > 0)
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_knn: filter offsets and indices must be given together");
-    if (int rc = check_topk_workspace(workspace_dev, workspace_bytes, kge_knn_workspace_bytes(h, b, n_cand, k, ld), "kge_knn")) return rc;
+    if (int rc = check_workspace(workspace_dev, workspace_bytes, kge_knn_workspace_bytes(h, b, n_cand, k, ld), "kge_knn")) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    const KnnWorkspace w = carve_knn_workspace(h, workspace_dev, b, n_cand, k, ld);
-    KGE_CUDA(launch_knn_gather(points_dev, ld, query_ids_dev, b, w.qvec, st), "kge_knn: gather");
-    KGE_CUDA(cudaMemsetAsync(w.cnt, 0, (size_t)4 * b * sizeof(int32_t), st), "kge_knn: memset");
+    Carve c(workspace_dev);
+    const KnnWorkspace w = carve_knn_workspace(h, c, b, n_cand, k, ld);
     KGE_CUDA(cudaMemsetAsync(w.l.state, 0, (size_t)b * sizeof(int2), st), "kge_knn: memset");
-    RankParams p = knn_rank_params(ld, points_dev, w, b);
-    const int op = metric == KGE_METRIC_EUCLIDEAN ? OP_L2_SUB : OP_L1_SUB;
-    TopkSelectParams s;
-    memset(&s, 0, sizeof(s));
-    s.scores = w.chunk;
-    s.b = b;
-    s.k = k;
-    if (n_filt > 0) { s.filt_off = (const long long *)filt_off_dev; s.filt_idx = filt_idx_dev; }
-    s.filt_shift = cand_ids_dev ? 0 : cand_begin;
-    s.keys = w.l.keys;
-    s.vals = w.l.vals;
-    s.state = w.l.state;
-    const int64_t C = topk_chunk(h, b, n_cand);
-    for (int64_t c0 = 0; c0 < n_cand; c0 += C) {
-        const int64_t nc = n_cand - c0 < C ? n_cand - c0 : C;
-        p.cand_ids = cand_ids_dev ? cand_ids_dev + c0 : nullptr;
-        p.cand_begin = cand_ids_dev ? 0 : cand_begin + c0;
-        p.n_cand = nc;
-        KGE_CUDA(launch_rank_count_op(p, op, w.cnt, st), "kge_knn: distances");  // -d, [b, nc]
-        if (farthest) KGE_CUDA(launch_knn_negate(w.chunk, b * nc, st), "kge_knn: negate");
-        s.ld = nc;
-        s.n = nc;
-        s.base = c0;
-        KGE_CUDA(launch_topk_select(s, st), "kge_knn: select");
-    }
+    const TopkSelectParams s = topk_select_params(w.chunk, b, k, w.l, filt_off_dev, filt_idx_dev, n_filt, cand_ids_dev ? 0 : cand_begin);
+    if (int rc = point_sweep(h, "kge_knn", "select", metric, points_dev, ld, query_ids_dev, b, cand_ids_dev, cand_begin, n_cand, w, st,
+                             [&](int64_t nc, int64_t c0) {
+                                 if (farthest) {  // +d: the select keeps the largest distances
+                                     const cudaError_t e = launch_knn_negate(w.chunk, b * nc, st);
+                                     if (e != cudaSuccess) return e;
+                                 }
+                                 return select_chunk(s, nc, c0, st);
+                             }))
+        return rc;
     KGE_CUDA(launch_topk_write(w.l.state, w.l.keys, w.l.vals, b, k, cand_ids_dev, cand_begin, ids_dev, dist_dev, st, !farthest),
              "kge_knn: write");
     return KGE_OK;
 }
 
-// The checks and the chunk loop kge_radius_neighbors, kge_radius_union and kge_radius_min_key share (b > 0 after the
-// call returns KGE_OK with *w set): gather the queries, then for every L2-sized candidate chunk score -d into w->chunk
-// ([b, nc], row stride nc) and run epilogue(nc, c0), whose errors are reported as "<fn>: <stage>".
+// The checks kge_radius_neighbors, kge_radius_union and kge_radius_min_key share; for b > 0, *w is carved on success
 static int check_radius(kge_handle *h, const char *fn, int32_t metric, const float *points_dev, int64_t n_points,
                         int32_t ld, const int32_t *query_ids_dev, int64_t b, const int32_t *cand_ids_dev, int64_t cand_begin,
                         int64_t n_cand, void *workspace_dev, int64_t workspace_bytes, KnnWorkspace *w)
@@ -1266,35 +1294,10 @@ static int check_radius(kge_handle *h, const char *fn, int32_t metric, const flo
     if (n_cand > 0x7fffffffLL) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: n_cand must be < 2^31", fn);
     if (b == 0) return KGE_OK;
     if (int rc = check_points(fn, metric, points_dev, n_points, ld, query_ids_dev, cand_ids_dev, cand_begin, n_cand)) return rc;
-    if (int rc = check_topk_workspace(workspace_dev, workspace_bytes, kge_radius_workspace_bytes(h, b, n_cand, ld), "kge_radius"))
+    if (int rc = check_workspace(workspace_dev, workspace_bytes, kge_radius_workspace_bytes(h, b, n_cand, ld), "kge_radius"))
         return rc;
-    *w = carve_knn_workspace(h, workspace_dev, b, n_cand, 0, ld);
-    return KGE_OK;
-}
-
-template <class Epilogue>
-static int radius_sweep(const kge_handle *h, const char *fn, const char *stage, int32_t metric, const float *points_dev,
-                        int32_t ld, const int32_t *query_ids_dev, int64_t b, const int32_t *cand_ids_dev, int64_t cand_begin,
-                        int64_t n_cand, const KnnWorkspace &w, cudaStream_t st, Epilogue epilogue)
-{
-    char what[96];
-    cudaError_t e = launch_knn_gather(points_dev, ld, query_ids_dev, b, w.qvec, st);
-    if (e != cudaSuccess) return cuda_fail(e, (snprintf(what, sizeof(what), "%s: gather", fn), what));
-    e = cudaMemsetAsync(w.cnt, 0, (size_t)4 * b * sizeof(int32_t), st);
-    if (e != cudaSuccess) return cuda_fail(e, (snprintf(what, sizeof(what), "%s: memset", fn), what));
-    RankParams p = knn_rank_params(ld, points_dev, w, b);
-    const int op = metric == KGE_METRIC_EUCLIDEAN ? OP_L2_SUB : OP_L1_SUB;
-    const int64_t C = topk_chunk(h, b, n_cand);
-    for (int64_t c0 = 0; c0 < n_cand; c0 += C) {
-        const int64_t nc = n_cand - c0 < C ? n_cand - c0 : C;
-        p.cand_ids = cand_ids_dev ? cand_ids_dev + c0 : nullptr;
-        p.cand_begin = cand_ids_dev ? 0 : cand_begin + c0;
-        p.n_cand = nc;
-        e = launch_rank_count_op(p, op, w.cnt, st);  // -d, [b, nc]
-        if (e != cudaSuccess) return cuda_fail(e, (snprintf(what, sizeof(what), "%s: distances", fn), what));
-        e = epilogue(nc, c0);
-        if (e != cudaSuccess) return cuda_fail(e, (snprintf(what, sizeof(what), "%s: %s", fn, stage), what));
-    }
+    Carve c(workspace_dev);
+    *w = carve_knn_workspace(h, c, b, n_cand, 0, ld);
     return KGE_OK;
 }
 
@@ -1313,11 +1316,11 @@ extern "C" int kge_radius_neighbors(kge_handle *h, int32_t metric, const float *
     cudaStream_t st = (cudaStream_t)stream;
     KGE_CUDA(cudaMemsetAsync(w.cursor, 0, (size_t)b * sizeof(long long), st), "kge_radius_neighbors: memset");
     const long long *off = nbr_dev ? (const long long *)offsets_dev : nullptr;
-    if (int rc = radius_sweep(h, "kge_radius_neighbors", nbr_dev ? "emit" : "count", metric, points_dev, ld, query_ids_dev, b,
-                              cand_ids_dev, cand_begin, n_cand, w, st, [&](int64_t nc, int64_t c0) {
-                                  return launch_radius_chunk(w.chunk, nc, nc, c0, b, radius, cand_ids_dev, cand_begin,
-                                                             w.cursor, off, nbr_dev, st);
-                              }))
+    if (int rc = point_sweep(h, "kge_radius_neighbors", nbr_dev ? "emit" : "count", metric, points_dev, ld, query_ids_dev, b,
+                             cand_ids_dev, cand_begin, n_cand, w, st, [&](int64_t nc, int64_t c0) {
+                                 return launch_radius_chunk(w.chunk, nc, nc, c0, b, radius, cand_ids_dev, cand_begin,
+                                                            w.cursor, off, nbr_dev, st);
+                             }))
         return rc;
     if (!nbr_dev) KGE_CUDA(launch_radius_counts(w.cursor, b, (long long *)offsets_dev, st), "kge_radius_neighbors: counts");
     return KGE_OK;
@@ -1336,11 +1339,11 @@ extern "C" int kge_radius_union(kge_handle *h, int32_t metric, const float *poin
     if (b == 0) return KGE_OK;
     if (!parent_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_radius_union: null pointer");
     cudaStream_t st = (cudaStream_t)stream;
-    return radius_sweep(h, "kge_radius_union", "union", metric, points_dev, ld, query_ids_dev, b, cand_ids_dev, cand_begin,
-                        n_cand, w, st, [&](int64_t nc, int64_t c0) {
-                            return launch_radius_union_chunk(w.chunk, nc, nc, c0, b, radius, query_ids_dev, cand_ids_dev,
-                                                             cand_begin, parent_dev, st);
-                        });
+    return point_sweep(h, "kge_radius_union", "union", metric, points_dev, ld, query_ids_dev, b, cand_ids_dev, cand_begin,
+                       n_cand, w, st, [&](int64_t nc, int64_t c0) {
+                           return launch_radius_union_chunk(w.chunk, nc, nc, c0, b, radius, query_ids_dev, cand_ids_dev,
+                                                            cand_begin, parent_dev, st);
+                       });
 }
 
 extern "C" int kge_radius_min_key(kge_handle *h, int32_t metric, const float *points_dev, int64_t n_points, int32_t ld,
@@ -1357,11 +1360,11 @@ extern "C" int kge_radius_min_key(kge_handle *h, int32_t metric, const float *po
     if (!key_dev || !out_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_radius_min_key: null pointer");
     cudaStream_t st = (cudaStream_t)stream;
     KGE_CUDA(launch_min_key_init(out_dev, b, st), "kge_radius_min_key: init");
-    return radius_sweep(h, "kge_radius_min_key", "min", metric, points_dev, ld, query_ids_dev, b, cand_ids_dev, cand_begin,
-                        n_cand, w, st, [&](int64_t nc, int64_t c0) {
-                            return launch_radius_min_key_chunk(w.chunk, nc, nc, c0, b, radius, cand_ids_dev, cand_begin,
-                                                               key_dev, out_dev, st);
-                        });
+    return point_sweep(h, "kge_radius_min_key", "min", metric, points_dev, ld, query_ids_dev, b, cand_ids_dev, cand_begin,
+                       n_cand, w, st, [&](int64_t nc, int64_t c0) {
+                           return launch_radius_min_key_chunk(w.chunk, nc, nc, c0, b, radius, cand_ids_dev, cand_begin,
+                                                              key_dev, out_dev, st);
+                       });
 }
 
 extern "C" int kge_forest_flatten(kge_handle *h, int32_t *parent_dev, int64_t n, void *stream)

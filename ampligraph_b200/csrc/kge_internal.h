@@ -62,19 +62,26 @@ struct TrainParams {
     } bk;
 };
 
-// grid = min(occupancy * sm_count, ceil(B / warps))
-cudaError_t launch_train(const TrainParams &p, int nit, int sm_count, int threads, size_t smem, cudaStream_t st);
+// Per-warp shared-memory slot of one training kernel (kge_create): warps per CTA, replaced rows per group, and the
+// slot's row windows and total bytes.  warps == 0: the kernel does not apply to the handle's shape.
+struct TrainSlot {
+    int warps, G, rows_bytes, region_bytes;
+};
+
+// Every training launcher runs slot.warps warps per CTA on grid = min(occupancy * sm_count, ceil(B / warps));
+// p.G / p.rows_bytes / p.region_bytes are the same slot's.
+cudaError_t launch_train(const TrainParams &p, int nit, const TrainSlot &slot, int sm_count, cudaStream_t st);
 // kge_train_res.cu: the resident trilinear fast path (DistMult / ComplEx / HolE, all rows of a positive resident, eta <= 32, one
-// table); p.rows_bytes / p.region_bytes carry ITS slot geometry (kge_create: res_*), threads = res_warps * 32
-cudaError_t launch_train_res(const TrainParams &p, int nit, int sm_count, int threads, size_t smem, cudaStream_t st);
+// table)
+cudaError_t launch_train_res(const TrainParams &p, int nit, const TrainSlot &slot, int sm_count, cudaStream_t st);
 // kge_train_bucket.cu: the owner-computes sum of the replaced rows' gradients around launch_train_res (p.bk set):
 // before it, bucket the eta*B corruptions by replaced entity (count + scan); after it, one warp per run of entries
 // forms each entity's gradient row and adds it to p.grad_ent once
 cudaError_t launch_bucket_prepass(const TrainParams &p, cudaStream_t st);
 cudaError_t launch_bucket_sum(const TrainParams &p, int nit, cudaStream_t st);
 // kge_train_rot.cu: the RotatE fast path (one column window, single table, any eta in groups of p.G with two buffers -- or one
-// group when everything fits); p.G / p.rows_bytes / p.region_bytes carry ITS slot geometry (kge_create: rot_*), threads = rot_warps * 32
-cudaError_t launch_train_rot(const TrainParams &p, int nit, int sm_count, int threads, size_t smem, cudaStream_t st);
+// group when everything fits)
+cudaError_t launch_train_rot(const TrainParams &p, int nit, const TrainSlot &slot, int sm_count, cudaStream_t st);
 cudaError_t launch_rotation_table(const float *rel, float *rot, long long n_rel, int kp, int ld, float div,
                                   cudaStream_t st);
 cudaError_t launch_corruptions(const int32_t *triples, long long B, int eta, unsigned long long seed,

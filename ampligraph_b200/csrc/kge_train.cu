@@ -860,44 +860,32 @@ __global__ void kge_corruptions_kernel(const int32_t *__restrict__ triples, long
 // --------------------------------------------------------------------------
 // host launchers
 // --------------------------------------------------------------------------
-template <int MODEL>
-static cudaError_t launch_train_model(const TrainParams &p, int nit, int sm_count, int threads, size_t smem,
-                                      cudaStream_t st)
+template <int MODEL, int NIT>
+static cudaError_t launch_train_nit(const TrainParams &p, const TrainSlot &slot, int sm_count, cudaStream_t st)
 {
-#define KGE_LAUNCH(N)                                                                                       \
-    {                                                                                                       \
-        auto kern = p.resident ? kge_train_kernel<MODEL, N, true> : kge_train_kernel<MODEL, N, false>;      \
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-        if (e != cudaSuccess) return e;                                                                     \
-        int occ = 0;                                                                                        \
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem);                       \
-        if (e != cudaSuccess) return e;                                                                     \
-        if (occ < 1) return cudaErrorLaunchOutOfResources;                                                  \
-        long long want = (p.B + (threads / 32) - 1) / (threads / 32);                                       \
-        long long cap = (long long)occ * sm_count;                                                          \
-        int grid = (int)(want < cap ? want : cap);                                                          \
-        kern<<<grid, threads, smem, st>>>(p);                                                               \
-        return cudaGetLastError();                                                                          \
-    }
-    switch (nit) {
-    case 1: KGE_LAUNCH(1)
-    case 2: KGE_LAUNCH(2)
-    case 4: KGE_LAUNCH(4)
-    default: return cudaErrorInvalidValue;
-    }
-#undef KGE_LAUNCH
+    return launch_persistent(p.resident ? kge_train_kernel<MODEL, NIT, true> : kge_train_kernel<MODEL, NIT, false>, p, slot,
+                             sm_count, st);
 }
 
-
-cudaError_t launch_train(const TrainParams &p, int nit, int sm_count, int threads, size_t smem, cudaStream_t st)
+template <int MODEL>
+static cudaError_t launch_train_model(const TrainParams &p, int nit, const TrainSlot &slot, int sm_count, cudaStream_t st)
 {
-    if (p.B == 0) return cudaSuccess;
+    switch (nit) {
+    case 1: return launch_train_nit<MODEL, 1>(p, slot, sm_count, st);
+    case 2: return launch_train_nit<MODEL, 2>(p, slot, sm_count, st);
+    case 4: return launch_train_nit<MODEL, 4>(p, slot, sm_count, st);
+    }
+    return cudaErrorInvalidValue;
+}
+
+cudaError_t launch_train(const TrainParams &p, int nit, const TrainSlot &slot, int sm_count, cudaStream_t st)
+{
     switch (p.model) {
-    case KGE_TRANSE: return launch_train_model<KGE_TRANSE>(p, nit, sm_count, threads, smem, st);
-    case KGE_DISTMULT: return launch_train_model<KGE_DISTMULT>(p, nit, sm_count, threads, smem, st);
-    case KGE_COMPLEX: return launch_train_model<KGE_COMPLEX>(p, nit, sm_count, threads, smem, st);
-    case KGE_HOLE: return launch_train_model<KGE_HOLE>(p, nit, sm_count, threads, smem, st);
-    case KGE_ROTATE: return launch_train_model<KGE_ROTATE>(p, nit, sm_count, threads, smem, st);
+    case KGE_TRANSE: return launch_train_model<KGE_TRANSE>(p, nit, slot, sm_count, st);
+    case KGE_DISTMULT: return launch_train_model<KGE_DISTMULT>(p, nit, slot, sm_count, st);
+    case KGE_COMPLEX: return launch_train_model<KGE_COMPLEX>(p, nit, slot, sm_count, st);
+    case KGE_HOLE: return launch_train_model<KGE_HOLE>(p, nit, slot, sm_count, st);
+    case KGE_ROTATE: return launch_train_model<KGE_ROTATE>(p, nit, slot, sm_count, st);
     }
     return cudaErrorInvalidValue;
 }

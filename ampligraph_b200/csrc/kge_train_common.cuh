@@ -1,6 +1,6 @@
 // kge_train_common.cuh -- device helpers shared by the training kernels (kge_train.cu: the general kernel;
 // kge_train_res.cu: the resident trilinear fast path): fp32-pair float4 arithmetic, the gradient sink, warp
-// reductions, and the per-positive loss + dL/dscore of the five reference losses.
+// reductions, and the per-positive loss + dL/dscore of the five reference losses; on the host, the launch they share.
 #pragma once
 #include <math.h>
 
@@ -390,5 +390,23 @@ static __device__ __forceinline__ float loss_and_dscores(const TrainParams &p, f
     return loss;
 }
 
+// Host side of every training launcher: slot.warps warps per CTA, each with its slot of shared memory, on as many CTAs as
+// are co-resident (each strides over the positives) but no more than the positives need.
+template <class Kernel>
+static cudaError_t launch_persistent(Kernel kern, const TrainParams &p, const TrainSlot &slot, int sm_count, cudaStream_t st)
+{
+    if (p.B == 0) return cudaSuccess;
+    const int threads = slot.warps * 32;
+    const size_t smem = (size_t)slot.warps * slot.region_bytes;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    int occ = 0;
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem);
+    if (e != cudaSuccess) return e;
+    if (occ < 1) return cudaErrorLaunchOutOfResources;
+    const long long want = (p.B + slot.warps - 1) / slot.warps, cap = (long long)occ * sm_count;
+    kern<<<(int)(want < cap ? want : cap), threads, smem, st>>>(p);
+    return cudaGetLastError();
+}
 
 }  // namespace kge

@@ -32,7 +32,7 @@ __device__ __forceinline__ void red_repl_v4(float *g, float4 v)
 // HALVES = 1: DistMult (f = sum s p o, DistMult.py:48); HALVES = 2: ComplEx / HolE (ComplEx.py:52-62; HolE.py:45 scales by
 // 2/k, folded into the gradient scalars).  Lane l owns float4 chunks c = l + 32*it (it < NIT) of every half-row; lanes past
 // the end of the row read its last chunk with zero query vectors (exact zeros in every sum) and never store.
-// Shared-memory slot of a warp (kge_create: res_rows_bytes / res_region_bytes):
+// Shared-memory slot of a warp (kge_create: the resident trilinear TrainSlot, p.rows_bytes / p.region_bytes):
 //   [ s | o | eta replaced rows ] [ sc: eta_pad floats ] [ nid ] [ jorig ] [ mbarrier ]
 // The relation row is NOT staged: each lane loads its chunks of p straight into registers (ld.global.nc, issued before
 // the wait for the gather, so the latency hides behind it) and keeps them until the gradient rows of s, p, o are formed.
@@ -373,29 +373,20 @@ __global__ void __launch_bounds__(THREADS) kge_train_res_kernel(const TrainParam
 
 // ---- host side -------------------------------------------------------------------------------------------------------------
 template <int HALVES, int NIT>
-static cudaError_t launch_res(const TrainParams &p, int sm_count, int threads, size_t smem, cudaStream_t st)
+static cudaError_t launch_res(const TrainParams &p, const TrainSlot &slot, int sm_count, cudaStream_t st)
 {
     constexpr int THREADS = KGE_TRAIN_THREADS(KGE_COMPLEX, NIT);
-    auto kern = p.bk.g ? kge_train_res_kernel<HALVES, NIT, THREADS, true> : kge_train_res_kernel<HALVES, NIT, THREADS, false>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    int occ = 0;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem);
-    if (e != cudaSuccess) return e;
-    if (occ < 1) return cudaErrorLaunchOutOfResources;
-    const long long want = (p.B + (threads / 32) - 1) / (threads / 32), cap = (long long)occ * sm_count;
-    kern<<<(int)(want < cap ? want : cap), threads, smem, st>>>(p);
-    return cudaGetLastError();
+    return launch_persistent(p.bk.g ? kge_train_res_kernel<HALVES, NIT, THREADS, true> : kge_train_res_kernel<HALVES, NIT, THREADS, false>,
+                             p, slot, sm_count, st);
 }
 
-cudaError_t launch_train_res(const TrainParams &p, int nit, int sm_count, int threads, size_t smem, cudaStream_t st)
+cudaError_t launch_train_res(const TrainParams &p, int nit, const TrainSlot &slot, int sm_count, cudaStream_t st)
 {
-    if (p.B == 0) return cudaSuccess;
     const bool two = p.model != KGE_DISTMULT;
-    if (nit <= 1) return two ? launch_res<2, 1>(p, sm_count, threads, smem, st) : launch_res<1, 1>(p, sm_count, threads, smem, st);
-    if (nit == 2) return two ? launch_res<2, 2>(p, sm_count, threads, smem, st) : launch_res<1, 2>(p, sm_count, threads, smem, st);
+    if (nit <= 1) return two ? launch_res<2, 1>(p, slot, sm_count, st) : launch_res<1, 1>(p, slot, sm_count, st);
+    if (nit == 2) return two ? launch_res<2, 2>(p, slot, sm_count, st) : launch_res<1, 2>(p, slot, sm_count, st);
     if (two) return cudaErrorInvalidValue;  // rows of 512+ floats per half: only DistMult's per-lane state fits the register file (kge_create)
-    return launch_res<1, 4>(p, sm_count, threads, smem, st);
+    return launch_res<1, 4>(p, slot, sm_count, st);
 }
 
 }  // namespace kge

@@ -51,7 +51,7 @@ __device__ __forceinline__ float4 ldg4_nc(const char *p)
 
 // Lane l owns float4 chunks c = l + 32*it (it < NIT) of every half-row; lanes past the end of the row read its last chunk,
 // are masked arithmetically in the scores (nlive) and never store.
-// Shared-memory slot of a warp (kge_create: rot_rows_bytes / rot_region_bytes):
+// Shared-memory slot of a warp (kge_create: the RotatE TrainSlot, p.rows_bytes / p.region_bytes):
 //   [ nbuf group buffers of G rows ] [ sc: eta_pad floats ] [ nid ] [ jorig ] [ side: scratch ] [ 2 mbarriers ]
 template <int NIT>
 __global__ void __launch_bounds__(256) kge_train_rot_kernel(const TrainParams p)
@@ -343,26 +343,10 @@ __global__ void __launch_bounds__(256) kge_train_rot_kernel(const TrainParams p)
 }
 
 // ---- host side -------------------------------------------------------------------------------------------------------------
-template <int NIT>
-static cudaError_t launch_rot(const TrainParams &p, int sm_count, int threads, size_t smem, cudaStream_t st)
+cudaError_t launch_train_rot(const TrainParams &p, int nit, const TrainSlot &slot, int sm_count, cudaStream_t st)
 {
-    auto kern = kge_train_rot_kernel<NIT>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    int occ = 0;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem);
-    if (e != cudaSuccess) return e;
-    if (occ < 1) return cudaErrorLaunchOutOfResources;
-    const long long want = (p.B + (threads / 32) - 1) / (threads / 32), cap = (long long)occ * sm_count;
-    kern<<<(int)(want < cap ? want : cap), threads, smem, st>>>(p);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_train_rot(const TrainParams &p, int nit, int sm_count, int threads, size_t smem, cudaStream_t st)
-{
-    if (p.B == 0) return cudaSuccess;
-    if (nit <= 1) return launch_rot<1>(p, sm_count, threads, smem, st);
-    if (nit == 2) return launch_rot<2>(p, sm_count, threads, smem, st);
+    if (nit <= 1) return launch_persistent(kge_train_rot_kernel<1>, p, slot, sm_count, st);
+    if (nit == 2) return launch_persistent(kge_train_rot_kernel<2>, p, slot, sm_count, st);
     return cudaErrorInvalidValue;  // rows of 512+ floats per half stay on the general kernel (kge_create)
 }
 

@@ -20,7 +20,7 @@ REDUCTIONS = {"sum": 0, "mean": 1}
 OPTIMIZERS = {"sgd": 0, "adam": 1, "adagrad": 2}
 SIDES = {"s": 0, "o": 1}
 STRATEGIES = {"worst": 0, "best": 1, "middle": 2}
-STEP_FUSED, STEP_FORWARD_ONLY, STEP_BACKWARD_EXT = 0, 1, 2
+STEP_FUSED, STEP_FORWARD_ONLY, STEP_BACKWARD_EXT, STEP_FUSED_DEFER = 0, 1, 2, 3
 RANK_MODES = {"auto": 0, "exact": 1}
 INIT_KINDS = {"uniform": 0, "normal": 1, "truncated_normal": 2, "constant": 3}
 METRICS = {"euclidean": 0, "manhattan": 1}
@@ -72,6 +72,8 @@ PROTOTYPES = {
                                    _P, _P, C.c_int64, _P, _P, _P, C.c_int64, _P]),
     "kge_optimizer_step": (C.c_int, [_P, C.POINTER(KgeOptimizerConfig), C.c_int64, _P, _P, _P, _P, C.c_int64,
                                      _P, _P]),
+    "kge_optimizer_step_deferred": (C.c_int, [_P, C.POINTER(KgeOptimizerConfig), C.c_int64, _P, _P, _P, _P, _P,
+                                              C.c_int64, _P, _P]),
     "kge_set_row_stamps": (C.c_int, [_P, _P, _P]),
     "kge_set_row_stash": (C.c_int, [_P, _P, C.c_int64]),
     "kge_set_hot_entities": (C.c_int, [_P, _P, C.c_int32]),

@@ -42,6 +42,9 @@ struct kge_handle {
     long long topk_chunk;        // KGE_B200_TOPK_CHUNK: candidates per kge_topk chunk (0: sized to L2)
     void *train_ws;              // caller-owned training workspace (kge_set_train_workspace) or nullptr
     long long train_ws_bytes;
+    // KGE_STEP_FUSED_DEFER: the step whose replaced-row sum waits in the workspace for kge_optimizer_step_deferred
+    bool sum_pending;
+    TrainParams pending;
 };
 
 // Make the handle's device current for the duration of an entry point (ADVICE r1: two handles on different GPUs
@@ -392,16 +395,40 @@ static TrainParams::Buckets carve_train_workspace(const kge_handle *h, int64_t B
     return bk;
 }
 
+// The caller's row stash, where it holds the eta*B replaced rows of a step of B positives (kge_set_row_stash), else nullptr.
+static float *row_stash(const kge_handle *h, int64_t B)
+{
+    return (h->stash && h->stash_rows >= B * (int64_t)h->cfg.eta) ? h->stash : nullptr;
+}
+
+// The kernel a training step runs: a fast path where its slot applies, on one (not row-sharded) table and without a row
+// stash; the general kernel otherwise, and for every shape under KGE_B200_TRAIN_KERNEL=general (A/B runs, and the tests
+// that cover its resident trilinear instantiations).
+static TrainPath train_path(const kge_handle *h, const kge_shard_map *map, const float *stash)
+{
+    const char *force = getenv("KGE_B200_TRAIN_KERNEL");
+    if ((map && map->world > 1) || stash || (force && strcmp(force, "general") == 0)) return TRAIN_GENERAL;
+    if (h->slot[TRAIN_ROT].warps > 0) return TRAIN_ROT;
+    if (h->slot[TRAIN_RES].warps > 0) return TRAIN_RES;
+    return TRAIN_GENERAL;
+}
+
 // Bytes of training workspace the owner-computes path needs for a step of B positives, or 0 where it does not apply: it
-// applies where the resident kernel does, the step replaces every entity at least once on average (eta*B >= n_ent), and
-// KGE_B200_TRAIN_REPL=scatter (A/B runs, the tests that compare the two) does not keep the REDs.  The bucket sum reads one
+// applies where an unsharded step runs the resident kernel (train_path: not under KGE_B200_TRAIN_KERNEL=general, not with
+// a row stash), the step replaces every entity at least once on average (eta*B >= n_ent), the entries fit int32 offsets
+// (eta*B < 2^31), and KGE_B200_TRAIN_REPL=scatter (A/B runs, the tests that compare the two) does not keep the REDs.  This is
+// the one place that decides whether a step buckets: kge_train_step gathers exactly when this is > 0 and the workspace set
+// holds it, and callers decide from it whether a step can be deferred (KGE_STEP_FUSED_DEFER).  The bucket sum reads one
 // kept-side entity row per corruption; it pays where replaced entities repeat within a step (measured on H100: cfg2, 19
 // corruptions per entity, and cfg3, 4.2, gain) and loses where they do not ('big' in scripts/kbench.py: 2 M entities, 0.33
 // per entity, HBM-resident, 1.65 -> 1.88 ms; DESIGN.md 5).
 static int64_t bucket_workspace_bytes(const kge_handle *h, int64_t B)
 {
     const char *rv = getenv("KGE_B200_TRAIN_REPL");
-    if (h->slot[TRAIN_RES].warps == 0 || (long long)h->cfg.eta * B < h->cfg.n_ent || (rv && strcmp(rv, "scatter") == 0)) return 0;
+    const long long n = (long long)h->cfg.eta * B;
+    if (train_path(h, nullptr, row_stash(h, B)) != TRAIN_RES || n < h->cfg.n_ent || n >= (1ll << 31) ||
+        (rv && strcmp(rv, "scatter") == 0))
+        return 0;
     Carve c(nullptr);
     carve_train_workspace(h, B, c);
     return (int64_t)c.at;
@@ -417,6 +444,9 @@ extern "C" int kge_set_train_workspace(kge_handle *h, void *ws_dev, int64_t byte
     KGE_CHECK_HANDLE(h, "kge_set_train_workspace");
     if (bytes < 0 || (ws_dev && ((uintptr_t)ws_dev & 15)))
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_set_train_workspace: bytes < 0 or workspace not 16-byte aligned");
+    if (h->sum_pending)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_set_train_workspace: the replaced-row sum of a deferred step is pending "
+                                              "in the current workspace (kge_optimizer_step_deferred first)");
     Carve counts(nullptr);
     carve_train_workspace(h, 0, counts);
     if (ws_dev && bytes < (int64_t)counts.at)
@@ -427,18 +457,6 @@ extern "C" int kge_set_train_workspace(kge_handle *h, void *ws_dev, int64_t byte
     return KGE_OK;
 }
 
-// The kernel a training step runs: a fast path where its slot applies, on one (not row-sharded) table and without a row
-// stash; the general kernel otherwise, and for every shape under KGE_B200_TRAIN_KERNEL=general (A/B runs, and the tests
-// that cover its resident trilinear instantiations).
-static TrainPath train_path(const kge_handle *h, const kge_shard_map *map, const float *stash)
-{
-    const char *force = getenv("KGE_B200_TRAIN_KERNEL");
-    if ((map && map->world > 1) || stash || (force && strcmp(force, "general") == 0)) return TRAIN_GENERAL;
-    if (h->slot[TRAIN_ROT].warps > 0) return TRAIN_ROT;
-    if (h->slot[TRAIN_RES].warps > 0) return TRAIN_RES;
-    return TRAIN_GENERAL;
-}
-
 static int train_step_impl(kge_handle *h, int32_t mode, const kge_shard_map *map, const float *ent_dev,
                            const float *rel_dev, float *grad_ent_dev, float *grad_rel_dev,
                            const int32_t *triples_dev, int64_t B, const int32_t *neg_ent_dev,
@@ -447,8 +465,13 @@ static int train_step_impl(kge_handle *h, int32_t mode, const kge_shard_map *map
                            const float *dneg_dev, void *stream)
 {
     KGE_CHECK_HANDLE(h, "kge_train_step");
-    if (mode < KGE_STEP_FUSED || mode > KGE_STEP_BACKWARD_EXT)
+    if (mode < KGE_STEP_FUSED || mode > KGE_STEP_FUSED_DEFER)
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_train_step: unknown mode %d", mode);
+    if (h->sum_pending)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_train_step: the replaced-row sum of a deferred step is pending "
+                                              "(kge_optimizer_step_deferred first)");
+    const bool defer = mode == KGE_STEP_FUSED_DEFER;
+    if (defer) mode = KGE_STEP_FUSED;
     if (B < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_train_step: B < 0");
     if (B == 0) return KGE_OK;
     if (!ent_dev || !rel_dev || !triples_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_train_step: null table/triples");
@@ -507,7 +530,7 @@ static int train_step_impl(kge_handle *h, int32_t mode, const kge_shard_map *map
     p.stamp_rel = h->stamp_rel;
     p.hot_ent[0] = h->hot_ent[0];
     p.hot_ent[1] = h->hot_ent[1];
-    p.stash = (h->stash && h->stash_rows >= B * (int64_t)h->cfg.eta) ? h->stash : nullptr;
+    p.stash = row_stash(h, B);
     if (map) {
         // the map's stamps replace the handle's for any world (a one-rank map runs the unsharded kernels, which stamp
         // p.stamp_ent directly); all or nothing
@@ -542,7 +565,12 @@ static int train_step_impl(kge_handle *h, int32_t mode, const kge_shard_map *map
         // time in bench.py's workload.  It stays in effect for the static stride, where it pays.
         if (p.sched) p.hot_ent[0] = p.hot_ent[1] = -1;
     }
+    auto defer_unsupported = [&]() {
+        return fail(KGE_ERR_UNSUPPORTED, "kge_train_step: KGE_STEP_FUSED_DEFER needs a step that sums the replaced rows per "
+                                         "entity (kge_train_workspace_bytes(h, B) > 0 and a workspace that holds it)");
+    };
     if (path == TRAIN_ROT) {
+        if (defer) return defer_unsupported();
         KGE_CUDA(launch_train_rot(p, h->nit, slot, h->sm_count, st), "kge_train_step");
         return KGE_OK;
     }
@@ -551,16 +579,23 @@ static int train_step_impl(kge_handle *h, int32_t mode, const kge_shard_map *map
         // (train_ws_bytes is 0 without one): on H100 the eta*B uniformly scattered row REDs it removes cost about half the
         // kernel (DESIGN.md 3.2, 5).
         const int64_t need = mode != KGE_STEP_FORWARD_ONLY ? bucket_workspace_bytes(h, B) : 0;
-        const bool gather = need > 0 && need <= h->train_ws_bytes && (long long)h->cfg.eta * B < (1ll << 31);
+        const bool gather = need > 0 && need <= h->train_ws_bytes;
+        if (defer && !gather) return defer_unsupported();
         if (gather) {
             Carve c(h->train_ws);
             p.bk = carve_train_workspace(h, B, c);
             KGE_CUDA(launch_bucket_prepass(p, st), "kge_train_step (bucket pre-pass)");
         }
         KGE_CUDA(launch_train_res(p, h->nit, slot, h->sm_count, st), "kge_train_step");
-        if (gather) KGE_CUDA(launch_bucket_sum(p, h->nit, st), "kge_train_step (bucket sum)");
+        if (defer) {
+            h->pending = p;
+            h->sum_pending = true;
+        } else if (gather) {
+            KGE_CUDA(launch_bucket_sum(p, h->nit, st), "kge_train_step (bucket sum)");
+        }
         return KGE_OK;
     }
+    if (defer) return defer_unsupported();
     KGE_CUDA(launch_train(p, h->nit, slot, h->sm_count, st), "kge_train_step");
     return KGE_OK;
 }
@@ -645,6 +680,35 @@ extern "C" int kge_optimizer_step(kge_handle *h, const kge_optimizer_config *opt
     KGE_CUDA(launch_optimizer(o, table_dev, grad_dev, slot0_dev, slot1_dev, rows * (long long)h->L.ld, reg_loss_dev,
                               h->sm_count, (cudaStream_t)stream),
              "kge_optimizer_step");
+    return KGE_OK;
+}
+
+extern "C" int kge_optimizer_step_deferred(kge_handle *h, const kge_optimizer_config *opt, int64_t t, const float *params_in,
+                                           float *params_out, float *grad_dev, float *slot0_dev, float *slot1_dev,
+                                           int64_t rows, double *reg_loss_dev, void *stream)
+{
+    KGE_CHECK_HANDLE(h, "kge_optimizer_step_deferred");
+    if (!h->sum_pending) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_deferred: no deferred step is pending");
+    if (int rc = check_optim(opt, "kge_optimizer_step_deferred")) return rc;
+    if (t < 1) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_deferred: t >= 1 required");
+    const TrainParams &p = h->pending;
+    const size_t ent_floats = (size_t)h->cfg.n_ent * h->L.ld;
+    if (rows != h->cfg.n_ent + h->cfg.n_rel || params_in != p.ent || params_in + ent_floats != p.rel ||
+        grad_dev != p.grad_ent || grad_dev + ent_floats != p.grad_rel)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_deferred: params_in / grad_dev must be the [ent | rel] blocks "
+                                              "(n_ent + n_rel rows) the deferred step trained on");
+    if (!params_out || params_out == params_in)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_deferred: params_out must be a second block");
+    if (!slots_ok(opt, slot0_dev, slot1_dev))
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_deferred: optimizer slot buffer missing");
+    OptimParams o;
+    fill_optim(opt, t, o);
+    // the checks above refuse without touching the pending step (the caller may repeat the call); from here on it is
+    // consumed, and the workspace is free again, whether or not the launch succeeds
+    h->sum_pending = false;
+    KGE_CUDA(launch_bucket_sum_optimizer(p, h->nit, o, params_in, params_out, grad_dev, slot0_dev, slot1_dev, rows,
+                                         reg_loss_dev, (cudaStream_t)stream),
+             "kge_optimizer_step_deferred");
     return KGE_OK;
 }
 

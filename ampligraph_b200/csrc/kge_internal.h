@@ -135,6 +135,12 @@ cudaError_t launch_optimizer_sharded(const OptimParams &o, int world, int rank, 
                                      double *reg_loss, int sm_count, cudaStream_t st);
 cudaError_t launch_optimizer_exchange(const OptimParams &o, const ExchangeParams &x, int sm_count, cudaStream_t st);
 cudaError_t launch_peer_barrier(int world, int rank, unsigned *const *flags, int slot, unsigned token, cudaStream_t st);
+// kge_train_bucket.cu: the same per-entity sum with the dense optimizer as its epilogue, one warp per row of the
+// [ent | rel] block (rows = n_ent + n_rel; p.ent / p.rel and p.grad_ent / p.grad_rel are the two parts of `in` and `grad`):
+// reads `in`, writes every element of `out`, updates the slots in place and zeroes `grad`
+cudaError_t launch_bucket_sum_optimizer(const TrainParams &p, int nit, const OptimParams &o, const float *in, float *out,
+                                        float *grad, float *slot0, float *slot1, long long rows, double *reg_loss,
+                                        cudaStream_t st);
 
 // kge_rank.cu
 struct ShardView {  // row-sharded entity table seen through peer pointers (world <= 1: not sharded)

@@ -15,8 +15,14 @@
 //      with the fused kernel's operations, accumulates g * Q in registers in entry order, and adds the sum to the
 //      gradient row with one set of REDs per entity and run.  A RED rather than a store, so that a bucket split over
 //      two runs, and the s / o rows the fused kernel scatters into the same table, add up without ordering.
+//   5. Or, for a step run with KGE_STEP_FUSED_DEFER, step 4 waits for kge_optimizer_step_deferred, whose kernel
+//      (kge_bucket_owner_kernel) gives each row of the [ent | rel] block to one warp: it sums the row's whole bucket in
+//      entry order, adds it to the row's gradient and applies the dense optimizer, reading the parameter block the step
+//      trained on and writing the new rows to a second block.  The bucket sum's row reads are latency bound and the
+//      optimizer's streams are HBM bound, so in one kernel each runs under the other (DESIGN.md 3.2).
 // Every g * Q term is bit-identical to the one the scatter path sends; only the order of the fp32 additions differs
 // (within a run: entry order; across runs and with the other REDs: atomic order).
+#include "kge_optim_common.cuh"
 #include "kge_train_common.cuh"
 
 namespace kge {
@@ -241,6 +247,187 @@ cudaError_t launch_bucket_sum(const TrainParams &p, int nit, cudaStream_t st)
     if (nit == 2) return two ? launch_sum<2, 2>(p, st) : launch_sum<1, 2>(p, st);
     if (two) return cudaErrorInvalidValue;
     return launch_sum<1, 4>(p, st);
+}
+
+// kge_optimizer_step_deferred: one warp per row e of the [ent | rel] block, the row's OWNER.  It walks e's bucket
+// [off[e], off[e+1]) in entry order (relation rows and entities nobody replaced have none), re-forms each entry's Q from
+// the kept-side entity row and the relation row with the fused kernel's operations and sums g * Q in registers; then the
+// dense optimizer: g = grad[e] + sum (in that order; grad[e] holds the fused kernel's s / o / relation REDs), the update4 of
+// kge_optim_common.cuh, the new row to the SECOND block x.out, m / v in place, grad[e] = 0.  Every row is updated, so the
+// dense semantics hold (empty buckets and relation rows still decay m / v and take the regulariser).
+// Hazards: the bucket walk and the epilogue read only x.in (p.ent / p.rel are its parts), which nothing writes during the
+// kernel, so no warp sees another's new row; row e of grad, slots and x.out has this one writer, so plain loads / stores.
+struct OwnerOptim {
+    const float *in;  // [rows, ld] parameter block the step read (p.ent and p.rel are its two parts)
+    float *out;       // [rows, ld] parameter block written, every column of every row
+    float *grad;      // [rows, ld] gradient block (p.grad_ent and p.grad_rel are its two parts), zeroed
+    float *s0, *s1;
+    long long rows;
+    double *reg_loss;
+    OptimParams o;
+};
+
+__device__ __forceinline__ void prefetch_l2(const void *p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
+
+template <int HALVES, int NIT, int KIND, bool REG>
+__global__ void __launch_bounds__(256, 2) kge_bucket_owner_kernel(const TrainParams p, const OwnerOptim x)
+{
+    constexpr bool S1 = KIND == KGE_OPT_ADAM;
+    const bool S0 = KIND != KGE_OPT_SGD || x.o.momentum != 0.f;
+    const int lane = threadIdx.x & 31;
+    const long long e = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    float racc = 0.f;
+    if (e < x.rows) {
+        const int nch = p.kp >> 2;
+        const uint32_t hsB = (uint32_t)p.kp * 4u;
+        const size_t row_bytes = (size_t)p.ld * 4u, roff = (size_t)e * row_bytes;
+        uint32_t off[NIT];
+        bool live[NIT];
+#pragma unroll
+        for (int it = 0; it < NIT; ++it) {
+            const int c = lane + 32 * it;
+            live[it] = c < nch;
+            off[it] = 16u * (uint32_t)min(c, nch - 1);
+        }
+        {
+            // the epilogue's HBM streams are requested now, so that their latency runs under the bucket walk: one lane per
+            // 128-byte line of the row (at most 17 lines for the 2 KB rows of NIT <= 4), into L2 rather than registers
+            const size_t line0 = roff & ~(size_t)127, span = roff + row_bytes - line0;
+            if ((size_t)lane * 128u < span) {
+                const size_t a = line0 + (size_t)lane * 128u;
+                prefetch_l2(reinterpret_cast<const char *>(x.in) + a);
+                prefetch_l2(reinterpret_cast<const char *>(x.grad) + a);
+                if (S0) prefetch_l2(reinterpret_cast<const char *>(x.s0) + a);
+                if (S1) prefetch_l2(reinterpret_cast<const char *>(x.s1) + a);
+            }
+        }
+        const bool ent_row = e < (long long)p.n_ent;
+        const int b0 = ent_row ? p.bk.off[e] : 0, b1 = ent_row ? p.bk.off[e + 1] : 0;
+        const char *const ent = reinterpret_cast<const char *>(p.ent);
+        const char *const rel = reinterpret_cast<const char *>(p.rel);
+        float4 ar[NIT], ai[NIT];
+#pragma unroll
+        for (int it = 0; it < NIT; ++it) ar[it] = ai[it] = f4zero();
+        for (int base = b0; base < b1; base += 32) {
+            // the next 32 entries, one per lane, broadcast one at a time below
+            const int cnt = min(32, b1 - base);
+            int m_o = 0, m_r = 0;
+            float m_g = 0.f;
+            if (lane < cnt) {
+                m_o = p.bk.other[base + lane];
+                m_r = p.bk.rel[base + lane];
+                m_g = p.bk.g[base + lane];
+            }
+            // two entries per trip: both entries' rows are requested before either is used
+            for (int k = 0; k < cnt; k += 2) {
+                const bool has_b = k + 1 < cnt;
+                const int kb = has_b ? k + 1 : k;
+                const int oa = __shfl_sync(0xffffffffu, m_o, k), ob = __shfl_sync(0xffffffffu, m_o, kb);
+                const int ra = __shfl_sync(0xffffffffu, m_r, k), rb = __shfl_sync(0xffffffffu, m_r, kb);
+                const float ga = __shfl_sync(0xffffffffu, m_g, k), gb = __shfl_sync(0xffffffffu, m_g, kb);
+                const char *const xa = ent + (size_t)oa * row_bytes, *const xb = ent + (size_t)ob * row_bytes;
+                const char *const pa = rel + (size_t)(ra & 0x7fffffff) * row_bytes, *const pb = rel + (size_t)(rb & 0x7fffffff) * row_bytes;
+                float4 xar[NIT], xai[NIT], xbr[NIT], xbi[NIT], par[NIT], pai[NIT], pbr[NIT], pbi[NIT];
+#pragma unroll
+                for (int it = 0; it < NIT; ++it) {
+                    xar[it] = __ldg(reinterpret_cast<const float4 *>(xa + off[it]));
+                    xbr[it] = __ldg(reinterpret_cast<const float4 *>(xb + off[it]));
+                    par[it] = __ldg(reinterpret_cast<const float4 *>(pa + off[it]));
+                    pbr[it] = __ldg(reinterpret_cast<const float4 *>(pb + off[it]));
+                    if constexpr (HALVES == 2) {
+                        xai[it] = __ldg(reinterpret_cast<const float4 *>(xa + off[it] + hsB));
+                        xbi[it] = __ldg(reinterpret_cast<const float4 *>(xb + off[it] + hsB));
+                        pai[it] = __ldg(reinterpret_cast<const float4 *>(pa + off[it] + hsB));
+                        pbi[it] = __ldg(reinterpret_cast<const float4 *>(pb + off[it] + hsB));
+                    } else {
+                        xai[it] = xbi[it] = pai[it] = pbi[it] = f4zero();
+                    }
+                }
+                auto add = [&](int r, float g, const float4(&xr)[NIT], const float4(&xi)[NIT], const float4(&pr)[NIT],
+                               const float4(&pi)[NIT]) {
+#pragma unroll
+                    for (int it = 0; it < NIT; ++it) {
+                        float4 qr, qi = f4zero();
+                        if (r < 0) query_obj<HALVES>(xr[it], xi[it], pr[it], pi[it], qr, qi);  // object replaced: x is the subject
+                        else query_subj<HALVES>(pr[it], pi[it], xr[it], xi[it], qr, qi);      // subject replaced: x is the object
+                        ar[it] = ar[it] + g * qr;
+                        if constexpr (HALVES == 2) ai[it] = ai[it] + g * qi;
+                    }
+                };
+                add(ra, ga, xar, xai, par, pai);
+                if (has_b) add(rb, gb, xbr, xbi, pbr, pbi);
+            }
+        }
+        {
+            // all loads first (L2 hits after the prefetch), then the updates and the stores (m, v, the new row and the
+            // zeroed gradient are not read again this step: evict-first)
+            const OptimParams op = x.o;
+            const char *const xin = reinterpret_cast<const char *>(x.in) + roff;
+            char *const gr = reinterpret_cast<char *>(x.grad) + roff;
+            char *const xo = reinterpret_cast<char *>(x.out) + roff;
+            char *const m0 = reinterpret_cast<char *>(x.s0) + roff;
+            char *const m1 = reinterpret_cast<char *>(x.s1) + roff;
+            float4 g4[HALVES][NIT], x4[HALVES][NIT], a4[HALVES][NIT], b4[HALVES][NIT];
+#pragma unroll
+            for (int h = 0; h < HALVES; ++h)
+#pragma unroll
+                for (int it = 0; it < NIT; ++it) {
+                    g4[h][it] = x4[h][it] = a4[h][it] = b4[h][it] = f4zero();
+                    if (!live[it]) continue;
+                    const uint32_t o = off[it] + (h ? hsB : 0u);
+                    g4[h][it] = __ldcs(reinterpret_cast<const float4 *>(gr + o));
+                    x4[h][it] = __ldg(reinterpret_cast<const float4 *>(xin + o));
+                    if (S0) a4[h][it] = __ldcs(reinterpret_cast<const float4 *>(m0 + o));
+                    if (S1) b4[h][it] = __ldcs(reinterpret_cast<const float4 *>(m1 + o));
+                }
+#pragma unroll
+            for (int h = 0; h < HALVES; ++h)
+#pragma unroll
+                for (int it = 0; it < NIT; ++it) {
+                    if (!live[it]) continue;
+                    const uint32_t o = off[it] + (h ? hsB : 0u);
+                    const float4 g = g4[h][it] + (h ? ai[it] : ar[it]);
+                    const float4 xn = update4<KIND, REG>(x4[h][it], g, a4[h][it], b4[h][it], op, op.reg, racc);
+                    __stcs(reinterpret_cast<float4 *>(xo + o), xn);
+                    if (S0) __stcs(reinterpret_cast<float4 *>(m0 + o), a4[h][it]);
+                    if (S1) __stcs(reinterpret_cast<float4 *>(m1 + o), b4[h][it]);
+                    __stcs(reinterpret_cast<float4 *>(gr + o), f4zero());
+                }
+        }
+    }
+    if (REG && x.reg_loss) flush_reg_loss(racc, x.reg_loss);
+}
+
+template <int HALVES, int NIT, int KIND, bool REG>
+static cudaError_t launch_owner(const TrainParams &p, const OwnerOptim &x, cudaStream_t st)
+{
+    kge_bucket_owner_kernel<HALVES, NIT, KIND, REG><<<(int)((x.rows + 7) / 8), 256, 0, st>>>(p, x);
+    return cudaGetLastError();
+}
+
+template <int KIND, bool REG>
+static cudaError_t launch_owner_shape(const TrainParams &p, const OwnerOptim &x, int nit, cudaStream_t st)
+{
+    const bool two = p.model != KGE_DISTMULT;
+    if (nit <= 1) return two ? launch_owner<2, 1, KIND, REG>(p, x, st) : launch_owner<1, 1, KIND, REG>(p, x, st);
+    if (nit == 2) return two ? launch_owner<2, 2, KIND, REG>(p, x, st) : launch_owner<1, 2, KIND, REG>(p, x, st);
+    if (two) return cudaErrorInvalidValue;
+    return launch_owner<1, 4, KIND, REG>(p, x, st);
+}
+
+cudaError_t launch_bucket_sum_optimizer(const TrainParams &p, int nit, const OptimParams &o, const float *in, float *out,
+                                        float *grad, float *slot0, float *slot1, long long rows, double *reg_loss,
+                                        cudaStream_t st)
+{
+    if (rows == 0) return cudaSuccess;
+    const OwnerOptim x{in, out, grad, slot0, slot1, rows, reg_loss, o};
+    const bool reg = o.reg.p > 0;
+    switch (o.kind) {
+    case KGE_OPT_SGD: return reg ? launch_owner_shape<KGE_OPT_SGD, true>(p, x, nit, st) : launch_owner_shape<KGE_OPT_SGD, false>(p, x, nit, st);
+    case KGE_OPT_ADAM: return reg ? launch_owner_shape<KGE_OPT_ADAM, true>(p, x, nit, st) : launch_owner_shape<KGE_OPT_ADAM, false>(p, x, nit, st);
+    case KGE_OPT_ADAGRAD: return reg ? launch_owner_shape<KGE_OPT_ADAGRAD, true>(p, x, nit, st) : launch_owner_shape<KGE_OPT_ADAGRAD, false>(p, x, nit, st);
+    default: return cudaErrorInvalidValue;
+    }
 }
 
 }  // namespace kge

@@ -203,6 +203,8 @@ class KGEEngine:
         self.set_optimizer(optimizer, optimizer_params, regularizer)
         self.launches = 0  # kernels launched by this engine (bench.py reports it)
         self._rank_ws = None  # caller-owned ranking workspace (kge_rank_workspace_bytes), grown on demand
+        self._pblock_next = None  # second [ent | rel] parameter block of the deferred steps, allocated on first use
+        self._deferred = False  # a forward_backward(defer=True) left its replaced-row sum for apply_gradients
 
     # -- lifetime ---------------------------------------------------------
     def close(self):
@@ -333,9 +335,18 @@ class KGEEngine:
     # -- training ------------------------------------------------------------
     @_traced("kge.train_step")
     def forward_backward(self, triples, negatives=None, seed=0, step=0, mode=_lib.STEP_FUSED,
-                         scores_pos=None, scores_neg=None, dpos=None, dneg=None):
-        """train_step up to tape.gradient: accumulates into g_ent/g_rel and loss_acc[0]."""
+                         scores_pos=None, scores_neg=None, dpos=None, dneg=None, defer=False):
+        """train_step up to tape.gradient: accumulates into g_ent/g_rel and loss_acc[0].
+
+        defer=True (callers that call apply_gradients() next and read nothing in between): where the step sums the
+        replaced entities' gradient rows per entity and the dense optimizer takes both tables in one launch, that sum is
+        left pending (KGE_STEP_FUSED_DEFER) and apply_gradients() runs it together with the optimizer
+        (kge_optimizer_step_deferred); g_ent / g_rel are then incomplete until it does.  The step defers exactly where
+        kge_train_workspace_bytes(h, B) > 0 (the library's one decision whether a step buckets); elsewhere defer has no
+        effect.  That apply_gradients() writes the new tables to a second block: see its docstring."""
         assert triples.dtype == torch.int32 and triples.is_cuda and triples.is_contiguous()
+        if self._deferred:  # its entries live in the training workspace, which this step would overwrite or regrow
+            raise ValueError("forward_backward: the replaced-row sum of a deferred step is pending (apply_gradients first)")
         B = triples.shape[0]
         neg_ent = neg_keep = None
         if negatives is not None:
@@ -343,13 +354,16 @@ class KGEEngine:
             assert neg_ent.dtype == torch.int32 and neg_keep.dtype == torch.uint8
             assert neg_ent.numel() == B * self.eta and neg_keep.numel() == B * self.eta
         bucketed = mode != _lib.STEP_FORWARD_ONLY and self.ensure_train_workspace(B)
+        defer = bool(defer) and bucketed and mode == _lib.STEP_FUSED and self._one_block()
         _lib.check(self.lib.kge_train_step(
-            self.h, mode, _ptr(self.ent), _ptr(self.rel), _ptr(self.g_ent), _ptr(self.g_rel), _ptr(triples), B,
-            _ptr(neg_ent), _ptr(neg_keep), int(seed), int(step), _ptr(self.loss_acc), _ptr(scores_pos),
-            _ptr(scores_neg), _ptr(dpos), _ptr(dneg), self._stream()))
+            self.h, _lib.STEP_FUSED_DEFER if defer else mode, _ptr(self.ent), _ptr(self.rel), _ptr(self.g_ent),
+            _ptr(self.g_rel), _ptr(triples), B, _ptr(neg_ent), _ptr(neg_keep), int(seed), int(step), _ptr(self.loss_acc),
+            _ptr(scores_pos), _ptr(scores_neg), _ptr(dpos), _ptr(dneg), self._stream()))
+        self._deferred = defer
         self._last_step = int(step)
-        # RotatE: rotation table + kernel; bucketed: count, two scan launches, kernel, bucket sum
-        self.launches += 2 if self.scoring_type == "RotatE" else 5 if bucketed else 1
+        # RotatE: rotation table + kernel; bucketed: count, two scan launches, kernel, bucket sum (deferred: in
+        # apply_gradients' launch)
+        self.launches += 2 if self.scoring_type == "RotatE" else (4 if defer else 5) if bucketed else 1
 
     def _one_block(self):
         """True when tables, gradients and slots still ARE the [ent | rel] blocks allocated here (callers may rebind them: the
@@ -372,8 +386,32 @@ class KGEEngine:
 
     @_traced("kge.optimizer_step")
     def apply_gradients(self):
-        """optimizer.apply_gradients on both tables (dense semantics) + LP regulariser."""
+        """optimizer.apply_gradients on both tables (dense semantics) + LP regulariser.
+
+        After a deferred forward_backward the new tables are written to the engine's second parameter block, which then
+        becomes the current one: self.ent / self.rel are re-sliced from it, and the block they viewed before is
+        overwritten by the next deferred step.  Read self.ent / self.rel (or get_embeddings()) after the step; do not
+        hold them across steps."""
         self.t += 1
+        if self._deferred:
+            # the pending replaced-row sum and the optimizer in one launch: it reads the current block and writes every
+            # element of the other one, which becomes the current block (ent / rel are re-sliced from it)
+            if self._pblock_next is None:
+                self._pblock_next = torch.empty_like(self._pblock)
+            rows = self.ent_rows + self.n_rel
+            rc = self.lib.kge_optimizer_step_deferred(
+                self.h, C.byref(self.opt_cfgs["ent"]), self.t, _ptr(self._pblock), _ptr(self._pblock_next),
+                _ptr(self._gblock), _ptr(self._sblocks[0]), _ptr(self._sblocks[1]), rows,
+                C.c_void_p(self.loss_acc.data_ptr() + 8), self._stream())
+            if rc == _lib.KGE_ERR_INVALID_ARGUMENT:
+                self.t -= 1  # arguments refused: nothing ran, and the step stays pending in the library too
+            else:
+                self._deferred = False  # the library consumed the pending sum, whether or not its launch succeeded
+            _lib.check(rc)
+            self._pblock, self._pblock_next = self._pblock_next, self._pblock
+            self.ent, self.rel = self._pblock[:self.ent_rows], self._pblock[self.ent_rows:]
+            self.launches += 1
+            return
         if self._one_block():
             _lib.check(self.lib.kge_optimizer_step(
                 self.h, C.byref(self.opt_cfgs["ent"]), self.t, _ptr(self._pblock), _ptr(self._gblock), _ptr(self._sblocks[0]),
@@ -395,8 +433,10 @@ class KGEEngine:
         self.launches += 2
 
     def train_step(self, triples, negatives=None, seed=0, step=None):
-        """One reference train_step (models/ScoringBasedEmbeddingModel.py:370-429)."""
-        self.forward_backward(triples, negatives, seed, self.t if step is None else step)
+        """One reference train_step (models/ScoringBasedEmbeddingModel.py:370-429).  Deferred where it can be
+        (forward_backward(defer=True)), so self.ent / self.rel may be views of another block afterwards: do not hold them
+        across steps (apply_gradients)."""
+        self.forward_backward(triples, negatives, seed, self.t if step is None else step, defer=True)
         self.apply_gradients()
 
     def read_loss(self, reset=True):

@@ -242,7 +242,7 @@ class ScoringBasedEmbeddingModel:
                 elif user_loss:
                     self._user_loss_step(batch)
                 else:
-                    eng.forward_backward(batch, None, seed=self.seed, step=self._step)
+                    eng.forward_backward(batch, None, seed=self.seed, step=self._step, defer=True)
                     eng.apply_gradients()
                 self._step += 1
                 self._loss_cnt += 1
@@ -299,7 +299,7 @@ class ScoringBasedEmbeddingModel:
         elif isinstance(self.compiled_loss, loss_functions.LossFunctionWrapper):
             self._user_loss_step(batch)
         else:
-            self.engine.forward_backward(batch, None, seed=self.seed, step=self._step)
+            self.engine.forward_backward(batch, None, seed=self.seed, step=self._step, defer=True)
             self.engine.apply_gradients()
         self._step += 1
         if self._world() > 1:
@@ -382,7 +382,7 @@ class ScoringBasedEmbeddingModel:
             elif user_loss:
                 self._user_loss_step(batch)
             else:
-                eng.forward_backward(batch, None, seed=self.seed, step=self._step)
+                eng.forward_backward(batch, None, seed=self.seed, step=self._step, defer=True)
                 eng.apply_gradients()
             P["free"][s].record(main)
             P["loss_pin"][s].copy_(eng.loss_acc, non_blocking=True)  # D2H of this step's (cumulative) loss record

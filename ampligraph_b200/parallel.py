@@ -173,7 +173,8 @@ class DataParallelTrainer:
         if self.mode in ("p2p", "nvls"):
             blk = self._k & 1
             eng.g_ent, eng.g_rel = self._gviews[blk]
-        eng.forward_backward(batch, negatives, seed=seed, step=step)
+        # one GPU: the replaced-row sum runs inside the optimizer launch (KGEEngine.forward_backward(defer=True))
+        eng.forward_backward(batch, negatives, seed=seed, step=step, defer=self.mode == "single")
         if kernel_done is not None:
             kernel_done.record()  # CUDA event: lets bench.py time the fused kernel alone
         if self.mode == "single":

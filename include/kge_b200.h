@@ -83,7 +83,9 @@ enum kge_init {
 enum kge_step_mode {
     KGE_STEP_FUSED = 0,         /* scores -> built-in loss -> gradients, one kernel */
     KGE_STEP_FORWARD_ONLY = 1,  /* scores only (user-callable loss / FocusE, phase 1) */
-    KGE_STEP_BACKWARD_EXT = 2   /* gradients from caller-supplied dL/dscore (phase 2) */
+    KGE_STEP_BACKWARD_EXT = 2,  /* gradients from caller-supplied dL/dscore (phase 2) */
+    KGE_STEP_FUSED_DEFER = 3    /* KGE_STEP_FUSED, but the gradient rows of the replaced entities are left pending in the
+                                   training workspace: kge_optimizer_step_deferred adds them and applies the optimizer */
 };
 
 /* ScoringBasedEmbeddingModel.__init__ (models/ScoringBasedEmbeddingModel.py:100-171)
@@ -235,9 +237,10 @@ int kge_set_hot_entities(kge_handle *h, const int32_t *ids_host, int32_t n);
  * kge_train_workspace_bytes(h, B) bytes is set, a fused step sums the gradient rows of the replaced entities per entity
  * (bucket the eta*B corruptions by replaced entity, then one warp forms each entity's row and adds it once) instead of
  * scattering every corruption's row with atomics; DESIGN.md 3.2.  kge_train_workspace_bytes returns 0 where the path
- * does not apply.  kge_set_train_workspace zeroes the first bytes of the buffer on `stream`; afterwards the library keeps
- * them zero between steps, so the buffer must not be used for anything else (ws_dev = NULL detaches it).  16-byte
- * aligned.  The environment variable KGE_B200_TRAIN_REPL=scatter keeps the atomic scatter for A/B runs (and makes
+ * does not apply (the shape, eta*B >= 2^31, a row stash that covers the step, KGE_B200_TRAIN_KERNEL=general): it is the
+ * one decision whether a step buckets.  kge_set_train_workspace zeroes the first bytes of the buffer on `stream`;
+ * afterwards the library keeps them zero between steps, so the buffer must not be used for anything else (ws_dev = NULL
+ * detaches it).  16-byte aligned.  The environment variable KGE_B200_TRAIN_REPL=scatter keeps the atomic scatter for A/B runs (and makes
  * kge_train_workspace_bytes return 0). */
 int64_t kge_train_workspace_bytes(const kge_handle *h, int64_t B);
 int kge_set_train_workspace(kge_handle *h, void *ws_dev, int64_t bytes, void *stream);
@@ -262,6 +265,23 @@ int kge_train_step_sharded(kge_handle *h, int32_t mode, const kge_shard_map *map
 int kge_optimizer_step(kge_handle *h, const kge_optimizer_config *opt, int64_t t, float *table_dev,
                        float *grad_dev, float *slot0_dev, float *slot1_dev, int64_t rows,
                        double *reg_loss_dev, void *stream);
+
+/* kge_optimizer_step over the [ent | rel] block of a KGE_STEP_FUSED_DEFER step, fused with that step's pending sum of
+ * the replaced entities' gradient rows: one warp per row adds the row's bucket (DESIGN.md 3.2) to grad_dev's row,
+ * applies the optimizer and the regulariser as kge_optimizer_step does, and zeroes the gradient row.
+ *   params_in   the block the step trained on: ent_dev, with rel_dev directly after its n_ent rows.  Only READ.
+ *   params_out  a second [rows, ld] block: every element of every row is written (pad columns stay 0), so it needs no
+ *               initialisation; the caller uses it as the parameter block from then on (double buffering).
+ *   grad_dev    the step's grad_ent_dev, with grad_rel_dev directly after it; zeroed on the way out.
+ *   rows        n_ent + n_rel.  slot0/slot1 and reg_loss_dev as in kge_optimizer_step (one regulariser for both tables).
+ * Fails with KGE_ERR_INVALID_ARGUMENT if no deferred step is pending or the blocks are not the ones it used.  Refused
+ * arguments (KGE_ERR_INVALID_ARGUMENT) launch nothing and leave the step pending, so the call can be repeated; any other
+ * outcome, a launch failure included, consumes it.  While a step is pending, kge_train_step and kge_set_train_workspace
+ * refuse on the handle.  A step can be deferred exactly where kge_train_workspace_bytes(h, B) > 0 and a workspace of that
+ * size is set; elsewhere KGE_STEP_FUSED_DEFER returns KGE_ERR_UNSUPPORTED and launches nothing. */
+int kge_optimizer_step_deferred(kge_handle *h, const kge_optimizer_config *opt, int64_t t, const float *params_in,
+                                float *params_out, float *grad_dev, float *slot0_dev, float *slot1_dev, int64_t rows,
+                                double *reg_loss_dev, void *stream);
 
 /* LAZY optimizer (opt-in extension, NOT the reference's dense rule): only rows touched by the
  * step are read and updated; m, v of untouched rows do not decay and the rows do not move (the

@@ -269,8 +269,17 @@ struct OwnerOptim {
 
 __device__ __forceinline__ void prefetch_l2(const void *p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
+// Warps (rows) per CTA.  A CTA retires when its longest bucket is walked, and bucket lengths vary (cfg2: about 19
+// entries on average), so every warp of a CTA would wait for the slowest: one-warp CTAs free each row's slot as soon as
+// that row is done.  With the regulariser each CTA adds its loss with one fp64 atomic to a single address, so those
+// steps keep eight rows per CTA rather than issue one such atomic per row.
+__host__ __device__ constexpr int owner_warps(bool reg) { return reg ? 8 : 1; }
+
+// -DKGE_PROFILE_OWNER_WALKONLY builds a profiling variant that walks the buckets but drops the epilogue's prefetches,
+// loads and stores; -DKGE_PROFILE_OWNER_NOWALK one that runs the epilogue on empty sums.  Together they attribute the
+// kernel's time to its two halves (DESIGN.md 5).  The default build sets neither.
 template <int HALVES, int NIT, int KIND, bool REG>
-__global__ void __launch_bounds__(256, 2) kge_bucket_owner_kernel(const TrainParams p, const OwnerOptim x)
+__global__ void __launch_bounds__(32 * owner_warps(REG), 16 / owner_warps(REG)) kge_bucket_owner_kernel(const TrainParams p, const OwnerOptim x)
 {
     constexpr bool S1 = KIND == KGE_OPT_ADAM;
     const bool S0 = KIND != KGE_OPT_SGD || x.o.momentum != 0.f;
@@ -289,6 +298,7 @@ __global__ void __launch_bounds__(256, 2) kge_bucket_owner_kernel(const TrainPar
             live[it] = c < nch;
             off[it] = 16u * (uint32_t)min(c, nch - 1);
         }
+#ifndef KGE_PROFILE_OWNER_WALKONLY
         {
             // the epilogue's HBM streams are requested now, so that their latency runs under the bucket walk: one lane per
             // 128-byte line of the row (at most 17 lines for the 2 KB rows of NIT <= 4), into L2 rather than registers
@@ -301,7 +311,12 @@ __global__ void __launch_bounds__(256, 2) kge_bucket_owner_kernel(const TrainPar
                 if (S1) prefetch_l2(reinterpret_cast<const char *>(x.s1) + a);
             }
         }
+#endif
+#ifdef KGE_PROFILE_OWNER_NOWALK
+        const bool ent_row = false;
+#else
         const bool ent_row = e < (long long)p.n_ent;
+#endif
         const int b0 = ent_row ? p.bk.off[e] : 0, b1 = ent_row ? p.bk.off[e + 1] : 0;
         const char *const ent = reinterpret_cast<const char *>(p.ent);
         const char *const rel = reinterpret_cast<const char *>(p.rel);
@@ -358,6 +373,13 @@ __global__ void __launch_bounds__(256, 2) kge_bucket_owner_kernel(const TrainPar
                 if (has_b) add(rb, gb, xbr, xbi, pbr, pbi);
             }
         }
+#ifdef KGE_PROFILE_OWNER_WALKONLY
+        float keep = 0.f;  // keeps the walk alive: a store no real sum takes
+#pragma unroll
+        for (int it = 0; it < NIT; ++it) keep += ar[it].x + ar[it].y + ar[it].z + ar[it].w + ai[it].x + ai[it].w;
+        if (__float_as_uint(keep) == 0x7fc0deadu) x.out[roff / 4 + lane] = keep;
+        if (false)
+#endif
         {
             // all loads first (L2 hits after the prefetch), then the updates and the stores (m, v, the new row and the
             // zeroed gradient are not read again this step: evict-first)
@@ -401,7 +423,7 @@ __global__ void __launch_bounds__(256, 2) kge_bucket_owner_kernel(const TrainPar
 template <int HALVES, int NIT, int KIND, bool REG>
 static cudaError_t launch_owner(const TrainParams &p, const OwnerOptim &x, cudaStream_t st)
 {
-    kge_bucket_owner_kernel<HALVES, NIT, KIND, REG><<<(int)((x.rows + 7) / 8), 256, 0, st>>>(p, x);
+    kge_bucket_owner_kernel<HALVES, NIT, KIND, REG><<<(int)((x.rows + owner_warps(REG) - 1) / owner_warps(REG)), 32 * owner_warps(REG), 0, st>>>(p, x);
     return cudaGetLastError();
 }
 

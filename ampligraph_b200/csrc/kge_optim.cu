@@ -105,19 +105,11 @@ cudaError_t launch_optimizer_sharded(const OptimParams &o, int world, int rank, 
     long long want = (n4 + 255) / 256;
     int grid = (int)(want < (long long)sm_count * 8 ? want : (long long)sm_count * 8);
     float4 *a = (float4 *)slot0, *b = (float4 *)slot1;
-    const bool reg = o.reg.p > 0;
     const long long off4 = off_floats / 4;
-#define KGE_OPTS(K)                                                                                          \
-    if (reg) kge_optim_sharded_kernel<K, true><<<grid, 256, 0, st>>>(pp, world, rank, a, b, off4, n4, o, reg_loss); \
-    else kge_optim_sharded_kernel<K, false><<<grid, 256, 0, st>>>(pp, world, rank, a, b, off4, n4, o, reg_loss);
-    switch (o.kind) {
-    case KGE_OPT_SGD: KGE_OPTS(KGE_OPT_SGD) break;
-    case KGE_OPT_ADAM: KGE_OPTS(KGE_OPT_ADAM) break;
-    case KGE_OPT_ADAGRAD: KGE_OPTS(KGE_OPT_ADAGRAD) break;
-    default: return cudaErrorInvalidValue;
-    }
-#undef KGE_OPTS
-    return cudaGetLastError();
+    return dispatch_optimizer(o.kind, o.reg.p > 0, [&](auto kind, auto reg) {
+        kge_optim_sharded_kernel<kind, reg><<<grid, 256, 0, st>>>(pp, world, rank, a, b, off4, n4, o, reg_loss);
+        return cudaGetLastError();
+    });
 }
 
 // --------------------------------------------------------------------------
@@ -405,35 +397,25 @@ cudaError_t launch_optimizer_exchange(const OptimParams &o, const ExchangeParams
     const long long zero_want = (a.total4 / 8 + 255) / 256;  // the zeroing of the next gradient block wants enough threads too
     if (!mc || trips <= 1) want = want > zero_want ? want : zero_want;
     if (want < 1) want = 1;
-    const bool reg = xp.reg_ent.p > 0 || xp.reg_rel.p > 0;
-#define KGE_OPTX2(K, W)                                                                          \
-    if (mc) {                                                                                    \
-        if (reg) return launch_exchange_variant<K, true, W, true>(a, o, want, sm_count, st);     \
-        return launch_exchange_variant<K, false, W, true>(a, o, want, sm_count, st);             \
-    }                                                                                            \
-    if (reg) return launch_exchange_variant<K, true, W, false>(a, o, want, sm_count, st);        \
-    return launch_exchange_variant<K, false, W, false>(a, o, want, sm_count, st);
-#define KGE_OPTX(K)                                                                       \
-    switch (xp.world) {                                                                   \
-    case 1: KGE_OPTX2(K, 1) break;                                                        \
-    case 2: KGE_OPTX2(K, 2) break;                                                        \
-    case 3: KGE_OPTX2(K, 3) break;                                                        \
-    case 4: KGE_OPTX2(K, 4) break;                                                        \
-    case 5: KGE_OPTX2(K, 5) break;                                                        \
-    case 6: KGE_OPTX2(K, 6) break;                                                        \
-    case 7: KGE_OPTX2(K, 7) break;                                                        \
-    case 8: KGE_OPTX2(K, 8) break;                                                        \
-    default: return cudaErrorInvalidValue;                                                \
-    }
-    switch (o.kind) {
-    case KGE_OPT_SGD: KGE_OPTX(KGE_OPT_SGD) break;
-    case KGE_OPT_ADAM: KGE_OPTX(KGE_OPT_ADAM) break;
-    case KGE_OPT_ADAGRAD: KGE_OPTX(KGE_OPT_ADAGRAD) break;
-    default: break;
-    }
-#undef KGE_OPTX
-#undef KGE_OPTX2
-    return cudaErrorInvalidValue;
+    return dispatch_optimizer(o.kind, xp.reg_ent.p > 0 || xp.reg_rel.p > 0, [&](auto kind, auto reg) {
+        auto variant = [&](auto world) {
+            constexpr int K = decltype(kind)::value;
+            constexpr bool R = decltype(reg)::value;
+            return mc ? launch_exchange_variant<K, R, world, true>(a, o, want, sm_count, st)
+                      : launch_exchange_variant<K, R, world, false>(a, o, want, sm_count, st);
+        };
+        switch (xp.world) {
+        case 1: return variant(std::integral_constant<int, 1>{});
+        case 2: return variant(std::integral_constant<int, 2>{});
+        case 3: return variant(std::integral_constant<int, 3>{});
+        case 4: return variant(std::integral_constant<int, 4>{});
+        case 5: return variant(std::integral_constant<int, 5>{});
+        case 6: return variant(std::integral_constant<int, 6>{});
+        case 7: return variant(std::integral_constant<int, 7>{});
+        case 8: return variant(std::integral_constant<int, 8>{});
+        default: return cudaErrorInvalidValue;
+        }
+    });
 }
 
 // --------------------------------------------------------------------------
@@ -489,18 +471,10 @@ cudaError_t launch_optimizer_lazy(const OptimParams &o, float *table, float *gra
     if (rows == 0) return cudaSuccess;
     long long want = (rows + 255) / 256;  // 8 warps x 32 rows per block
     int grid = (int)(want < (long long)sm_count * 8 ? want : (long long)sm_count * 8);
-    const bool reg = o.reg.p > 0;
-#define KGE_OPTL(K)                                                                                                      \
-    if (reg) kge_optim_lazy_kernel<K, true><<<grid, 256, 0, st>>>(table, grad, slot0, slot1, rows, ld, row_stamp, stamp, o, reg_loss); \
-    else kge_optim_lazy_kernel<K, false><<<grid, 256, 0, st>>>(table, grad, slot0, slot1, rows, ld, row_stamp, stamp, o, reg_loss);
-    switch (o.kind) {
-    case KGE_OPT_SGD: KGE_OPTL(KGE_OPT_SGD) break;
-    case KGE_OPT_ADAM: KGE_OPTL(KGE_OPT_ADAM) break;
-    case KGE_OPT_ADAGRAD: KGE_OPTL(KGE_OPT_ADAGRAD) break;
-    default: return cudaErrorInvalidValue;
-    }
-#undef KGE_OPTL
-    return cudaGetLastError();
+    return dispatch_optimizer(o.kind, o.reg.p > 0, [&](auto kind, auto reg) {
+        kge_optim_lazy_kernel<kind, reg><<<grid, 256, 0, st>>>(table, grad, slot0, slot1, rows, ld, row_stamp, stamp, o, reg_loss);
+        return cudaGetLastError();
+    });
 }
 
 cudaError_t launch_optimizer(const OptimParams &o, float *table, float *grad, float *slot0, float *slot1,
@@ -511,18 +485,10 @@ cudaError_t launch_optimizer(const OptimParams &o, float *table, float *grad, fl
     long long want = (n4 + 255) / 256;
     int grid = (int)(want < (long long)sm_count * 8 ? want : (long long)sm_count * 8);
     float4 *v = (float4 *)table, *g = (float4 *)grad, *a = (float4 *)slot0, *b = (float4 *)slot1;
-    const bool reg = o.reg.p > 0;
-#define KGE_OPT(K)                                                                            \
-    if (reg) kge_optim_kernel<K, true><<<grid, 256, 0, st>>>(v, g, a, b, n4, o, reg_loss);    \
-    else kge_optim_kernel<K, false><<<grid, 256, 0, st>>>(v, g, a, b, n4, o, reg_loss);
-    switch (o.kind) {
-    case KGE_OPT_SGD: KGE_OPT(KGE_OPT_SGD) break;
-    case KGE_OPT_ADAM: KGE_OPT(KGE_OPT_ADAM) break;
-    case KGE_OPT_ADAGRAD: KGE_OPT(KGE_OPT_ADAGRAD) break;
-    default: return cudaErrorInvalidValue;
-    }
-#undef KGE_OPT
-    return cudaGetLastError();
+    return dispatch_optimizer(o.kind, o.reg.p > 0, [&](auto kind, auto reg) {
+        kge_optim_kernel<kind, reg><<<grid, 256, 0, st>>>(v, g, a, b, n4, o, reg_loss);
+        return cudaGetLastError();
+    });
 }
 
 }  // namespace kge

@@ -1,12 +1,14 @@
 // kge_optim_common.cuh -- the per-element optimizer update and regulariser (sm_90a), shared by the dense, lazy,
 // sharded and exchange kernels of kge_optim.cu and by the owner-per-row kernel of kge_train_bucket.cu, so that every
-// path applies the same fp32 arithmetic.
+// path applies the same fp32 arithmetic; on the host, their launchers' choice of instantiation.
 //
 // Replaces OptimizerWrapper.minimize -> tf.keras.optimizers.legacy.*.apply_gradients (optimizers.py:136-168) and the
 // regularisers attached to the tables (regularizers.py:14-37, EmbeddingLookupLayer.py:131-155).  The regulariser's
 // gradient and loss are taken at the PRE-update value of each element.
 #pragma once
 #include <math.h>
+
+#include <type_traits>
 
 #include "kge_internal.h"
 
@@ -72,6 +74,20 @@ __device__ __forceinline__ void flush_reg_loss(float racc, double *reg_loss)
         double t = 0.0;
         for (int w = 0; w < (int)((blockDim.x + 31) >> 5); ++w) t += (double)part[w];
         if (t != 0.0) atomicAdd(reg_loss, t);
+    }
+}
+
+// Host side of every optimizer launcher: returns launch(std::integral_constant<int, KIND>, std::integral_constant<bool,
+// REG>) for the optimizer kind and whether a regulariser is set, or cudaErrorInvalidValue for an unknown kind.
+template <class Launch>
+static cudaError_t dispatch_optimizer(int kind, bool reg, Launch &&launch)
+{
+    auto with_reg = [&](auto k) { return reg ? launch(k, std::true_type{}) : launch(k, std::false_type{}); };
+    switch (kind) {
+    case KGE_OPT_SGD: return with_reg(std::integral_constant<int, KGE_OPT_SGD>{});
+    case KGE_OPT_ADAM: return with_reg(std::integral_constant<int, KGE_OPT_ADAM>{});
+    case KGE_OPT_ADAGRAD: return with_reg(std::integral_constant<int, KGE_OPT_ADAGRAD>{});
+    default: return cudaErrorInvalidValue;
     }
 }
 

@@ -125,55 +125,55 @@ __global__ void __launch_bounds__(KGE_SCAN_THREADS) kge_bucket_scan_kernel(int *
     if (blockIdx.x == gridDim.x - 1 && t == 0) off[n_ent] = carry + warp_tot[KGE_SCAN_THREADS / 32 - 1];
 }
 
-template <int HALVES, int NIT>
-__global__ void __launch_bounds__(256) kge_bucket_sum_kernel(const TrainParams p)
-{
-    const int lane = threadIdx.x & 31;
-    const long long n = (long long)p.eta * p.B;
-    const long long base = ((long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * 32;
-    if (base >= n) return;
-    const int cnt = (int)min(32ll, n - base);
-    const int nch = p.kp >> 2;
-    const uint32_t hsB = (uint32_t)p.kp * 4u;
+// A lane's share of a row of the parameter, gradient and slot tables: float4 chunk c = lane + 32 * it of each half sits
+// at byte offset off[it] (+ hsB for the im half).  live[it] is false past the row's kp / 4 chunks; there off[it] repeats
+// the last chunk, so that loads stay inside the row, and the result is dropped.
+template <int NIT>
+struct LaneRow {
     uint32_t off[NIT];
     bool live[NIT];
+    uint32_t hsB;
+    size_t row_bytes;
+    __device__ __forceinline__ LaneRow(const TrainParams &p, int lane)
+    {
+        const int nch = p.kp >> 2;
+        hsB = (uint32_t)p.kp * 4u;
+        row_bytes = (size_t)p.ld * 4u;
 #pragma unroll
-    for (int it = 0; it < NIT; ++it) {
-        const int c = lane + 32 * it;
-        live[it] = c < nch;
-        off[it] = 16u * (uint32_t)min(c, nch - 1);
+        for (int it = 0; it < NIT; ++it) {
+            const int c = lane + 32 * it;
+            live[it] = c < nch;
+            off[it] = 16u * (uint32_t)min(c, nch - 1);
+        }
     }
-    // this run's entries, one per lane, broadcast one at a time below
-    int m_e = -1, m_o = 0, m_r = 0;
+};
+
+// The bucket walk of both replaced-row sums: adds g * Q of the cnt <= 32 bucket entries from base on to the lane's chunks
+// ar / ai (re / im halves) in entry order.  Q is re-formed from the kept-side entity row and the relation row with the
+// fused kernel's operations.  The entries are read one per lane and broadcast, two per trip, so that both entries' rows
+// are requested before either is used.  Lane k's key goes with entry base + k: before_add(key) runs before the entry is
+// added (kge_bucket_sum_kernel passes the entity and flushes its sum when that changes).
+template <int HALVES, int NIT, class Index, class Hook>
+__device__ __forceinline__ void bucket_walk(const TrainParams &p, const LaneRow<NIT> &w, Index base, int cnt, int key,
+                                            float4 (&ar)[NIT], float4 (&ai)[NIT], Hook &&before_add)
+{
+    const int lane = threadIdx.x & 31;
+    const uint32_t(&off)[NIT] = w.off;
+    const uint32_t hsB = w.hsB;
+    const size_t row_bytes = w.row_bytes;
+    const char *const ent = reinterpret_cast<const char *>(p.ent);
+    const char *const rel = reinterpret_cast<const char *>(p.rel);
+    int m_o = 0, m_r = 0;
     float m_g = 0.f;
     if (lane < cnt) {
-        m_e = p.bk.eid[base + lane];
         m_o = p.bk.other[base + lane];
         m_r = p.bk.rel[base + lane];
         m_g = p.bk.g[base + lane];
     }
-    const char *const ent = reinterpret_cast<const char *>(p.ent);
-    const char *const rel = reinterpret_cast<const char *>(p.rel);
-    const size_t row_bytes = (size_t)p.ld * 4u;
-    float4 ar[NIT], ai[NIT];
-#pragma unroll
-    for (int it = 0; it < NIT; ++it) ar[it] = ai[it] = f4zero();
-    int cur = __shfl_sync(0xffffffffu, m_e, 0);
-    auto flush = [&]() {
-        char *const g0 = reinterpret_cast<char *>(p.grad_ent) + (size_t)cur * row_bytes;
-#pragma unroll
-        for (int it = 0; it < NIT; ++it) {
-            if (!live[it]) continue;
-            red4(g0, off[it], ar[it]);
-            if constexpr (HALVES == 2) red4(g0, off[it] + hsB, ai[it]);
-            ar[it] = ai[it] = f4zero();
-        }
-    };
-    // two entries per trip: both entries' rows are requested before either is used
     for (int k = 0; k < cnt; k += 2) {
         const bool has_b = k + 1 < cnt;
         const int kb = has_b ? k + 1 : k;
-        const int ea = __shfl_sync(0xffffffffu, m_e, k), eb = __shfl_sync(0xffffffffu, m_e, kb);
+        const int key_a = __shfl_sync(0xffffffffu, key, k), key_b = __shfl_sync(0xffffffffu, key, kb);
         const int oa = __shfl_sync(0xffffffffu, m_o, k), ob = __shfl_sync(0xffffffffu, m_o, kb);
         const int ra = __shfl_sync(0xffffffffu, m_r, k), rb = __shfl_sync(0xffffffffu, m_r, kb);
         const float ga = __shfl_sync(0xffffffffu, m_g, k), gb = __shfl_sync(0xffffffffu, m_g, kb);
@@ -195,12 +195,8 @@ __global__ void __launch_bounds__(256) kge_bucket_sum_kernel(const TrainParams p
                 xai[it] = xbi[it] = pai[it] = pbi[it] = f4zero();
             }
         }
-        auto add = [&](int e, int r, float g, const float4(&xr)[NIT], const float4(&xi)[NIT], const float4(&pr)[NIT],
+        auto add = [&](int r, float g, const float4(&xr)[NIT], const float4(&xi)[NIT], const float4(&pr)[NIT],
                        const float4(&pi)[NIT]) {
-            if (e != cur) {
-                flush();
-                cur = e;
-            }
 #pragma unroll
             for (int it = 0; it < NIT; ++it) {
                 float4 qr, qi = f4zero();
@@ -210,9 +206,45 @@ __global__ void __launch_bounds__(256) kge_bucket_sum_kernel(const TrainParams p
                 if constexpr (HALVES == 2) ai[it] = ai[it] + g * qi;
             }
         };
-        add(ea, ra, ga, xar, xai, par, pai);
-        if (has_b) add(eb, rb, gb, xbr, xbi, pbr, pbi);
+        before_add(key_a);
+        add(ra, ga, xar, xai, par, pai);
+        if (has_b) {
+            before_add(key_b);
+            add(rb, gb, xbr, xbi, pbr, pbi);
+        }
     }
+}
+
+template <int HALVES, int NIT>
+__global__ void __launch_bounds__(256) kge_bucket_sum_kernel(const TrainParams p)
+{
+    const int lane = threadIdx.x & 31;
+    const long long n = (long long)p.eta * p.B;
+    const long long base = ((long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * 32;
+    if (base >= n) return;
+    const int cnt = (int)min(32ll, n - base);
+    const LaneRow<NIT> w(p, lane);
+    const int m_e = lane < cnt ? p.bk.eid[base + lane] : -1;  // this run's entities, one per lane
+    float4 ar[NIT], ai[NIT];
+#pragma unroll
+    for (int it = 0; it < NIT; ++it) ar[it] = ai[it] = f4zero();
+    int cur = __shfl_sync(0xffffffffu, m_e, 0);
+    auto flush = [&]() {
+        char *const g0 = reinterpret_cast<char *>(p.grad_ent) + (size_t)cur * w.row_bytes;
+#pragma unroll
+        for (int it = 0; it < NIT; ++it) {
+            if (!w.live[it]) continue;
+            red4(g0, w.off[it], ar[it]);
+            if constexpr (HALVES == 2) red4(g0, w.off[it] + w.hsB, ai[it]);
+            ar[it] = ai[it] = f4zero();
+        }
+    };
+    bucket_walk<HALVES>(p, w, base, cnt, m_e, ar, ai, [&](int e) {
+        if (e != cur) {
+            flush();
+            cur = e;
+        }
+    });
     flush();
 }
 
@@ -231,22 +263,14 @@ cudaError_t launch_bucket_prepass(const TrainParams &p, cudaStream_t st)
     return cudaGetLastError();
 }
 
-template <int HALVES, int NIT>
-static cudaError_t launch_sum(const TrainParams &p, cudaStream_t st)
-{
-    const long long runs = ((long long)p.eta * p.B + 31) / 32;
-    kge_bucket_sum_kernel<HALVES, NIT><<<(int)((runs + 7) / 8), 256, 0, st>>>(p);
-    return cudaGetLastError();
-}
-
 cudaError_t launch_bucket_sum(const TrainParams &p, int nit, cudaStream_t st)
 {
     if (p.B == 0) return cudaSuccess;
-    const bool two = p.model != KGE_DISTMULT;
-    if (nit <= 1) return two ? launch_sum<2, 1>(p, st) : launch_sum<1, 1>(p, st);
-    if (nit == 2) return two ? launch_sum<2, 2>(p, st) : launch_sum<1, 2>(p, st);
-    if (two) return cudaErrorInvalidValue;
-    return launch_sum<1, 4>(p, st);
+    const long long runs = ((long long)p.eta * p.B + 31) / 32;
+    return dispatch_trilinear_shape(p.model, nit, [&](auto halves, auto nits) {
+        kge_bucket_sum_kernel<halves, nits><<<(int)((runs + 7) / 8), 256, 0, st>>>(p);
+        return cudaGetLastError();
+    });
 }
 
 // kge_optimizer_step_deferred: one warp per row e of the [ent | rel] block, the row's OWNER.  It walks e's bucket
@@ -287,17 +311,8 @@ __global__ void __launch_bounds__(32 * owner_warps(REG), 16 / owner_warps(REG)) 
     const long long e = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     float racc = 0.f;
     if (e < x.rows) {
-        const int nch = p.kp >> 2;
-        const uint32_t hsB = (uint32_t)p.kp * 4u;
-        const size_t row_bytes = (size_t)p.ld * 4u, roff = (size_t)e * row_bytes;
-        uint32_t off[NIT];
-        bool live[NIT];
-#pragma unroll
-        for (int it = 0; it < NIT; ++it) {
-            const int c = lane + 32 * it;
-            live[it] = c < nch;
-            off[it] = 16u * (uint32_t)min(c, nch - 1);
-        }
+        const LaneRow<NIT> w(p, lane);
+        const size_t row_bytes = w.row_bytes, roff = (size_t)e * row_bytes;
 #ifndef KGE_PROFILE_OWNER_WALKONLY
         {
             // the epilogue's HBM streams are requested now, so that their latency runs under the bucket walk: one lane per
@@ -318,61 +333,10 @@ __global__ void __launch_bounds__(32 * owner_warps(REG), 16 / owner_warps(REG)) 
         const bool ent_row = e < (long long)p.n_ent;
 #endif
         const int b0 = ent_row ? p.bk.off[e] : 0, b1 = ent_row ? p.bk.off[e + 1] : 0;
-        const char *const ent = reinterpret_cast<const char *>(p.ent);
-        const char *const rel = reinterpret_cast<const char *>(p.rel);
         float4 ar[NIT], ai[NIT];
 #pragma unroll
         for (int it = 0; it < NIT; ++it) ar[it] = ai[it] = f4zero();
-        for (int base = b0; base < b1; base += 32) {
-            // the next 32 entries, one per lane, broadcast one at a time below
-            const int cnt = min(32, b1 - base);
-            int m_o = 0, m_r = 0;
-            float m_g = 0.f;
-            if (lane < cnt) {
-                m_o = p.bk.other[base + lane];
-                m_r = p.bk.rel[base + lane];
-                m_g = p.bk.g[base + lane];
-            }
-            // two entries per trip: both entries' rows are requested before either is used
-            for (int k = 0; k < cnt; k += 2) {
-                const bool has_b = k + 1 < cnt;
-                const int kb = has_b ? k + 1 : k;
-                const int oa = __shfl_sync(0xffffffffu, m_o, k), ob = __shfl_sync(0xffffffffu, m_o, kb);
-                const int ra = __shfl_sync(0xffffffffu, m_r, k), rb = __shfl_sync(0xffffffffu, m_r, kb);
-                const float ga = __shfl_sync(0xffffffffu, m_g, k), gb = __shfl_sync(0xffffffffu, m_g, kb);
-                const char *const xa = ent + (size_t)oa * row_bytes, *const xb = ent + (size_t)ob * row_bytes;
-                const char *const pa = rel + (size_t)(ra & 0x7fffffff) * row_bytes, *const pb = rel + (size_t)(rb & 0x7fffffff) * row_bytes;
-                float4 xar[NIT], xai[NIT], xbr[NIT], xbi[NIT], par[NIT], pai[NIT], pbr[NIT], pbi[NIT];
-#pragma unroll
-                for (int it = 0; it < NIT; ++it) {
-                    xar[it] = __ldg(reinterpret_cast<const float4 *>(xa + off[it]));
-                    xbr[it] = __ldg(reinterpret_cast<const float4 *>(xb + off[it]));
-                    par[it] = __ldg(reinterpret_cast<const float4 *>(pa + off[it]));
-                    pbr[it] = __ldg(reinterpret_cast<const float4 *>(pb + off[it]));
-                    if constexpr (HALVES == 2) {
-                        xai[it] = __ldg(reinterpret_cast<const float4 *>(xa + off[it] + hsB));
-                        xbi[it] = __ldg(reinterpret_cast<const float4 *>(xb + off[it] + hsB));
-                        pai[it] = __ldg(reinterpret_cast<const float4 *>(pa + off[it] + hsB));
-                        pbi[it] = __ldg(reinterpret_cast<const float4 *>(pb + off[it] + hsB));
-                    } else {
-                        xai[it] = xbi[it] = pai[it] = pbi[it] = f4zero();
-                    }
-                }
-                auto add = [&](int r, float g, const float4(&xr)[NIT], const float4(&xi)[NIT], const float4(&pr)[NIT],
-                               const float4(&pi)[NIT]) {
-#pragma unroll
-                    for (int it = 0; it < NIT; ++it) {
-                        float4 qr, qi = f4zero();
-                        if (r < 0) query_obj<HALVES>(xr[it], xi[it], pr[it], pi[it], qr, qi);  // object replaced: x is the subject
-                        else query_subj<HALVES>(pr[it], pi[it], xr[it], xi[it], qr, qi);      // subject replaced: x is the object
-                        ar[it] = ar[it] + g * qr;
-                        if constexpr (HALVES == 2) ai[it] = ai[it] + g * qi;
-                    }
-                };
-                add(ra, ga, xar, xai, par, pai);
-                if (has_b) add(rb, gb, xbr, xbi, pbr, pbi);
-            }
-        }
+        for (int base = b0; base < b1; base += 32) bucket_walk<HALVES>(p, w, base, min(32, b1 - base), 0, ar, ai, [](int) {});
 #ifdef KGE_PROFILE_OWNER_WALKONLY
         float keep = 0.f;  // keeps the walk alive: a store no real sum takes
 #pragma unroll
@@ -395,8 +359,8 @@ __global__ void __launch_bounds__(32 * owner_warps(REG), 16 / owner_warps(REG)) 
 #pragma unroll
                 for (int it = 0; it < NIT; ++it) {
                     g4[h][it] = x4[h][it] = a4[h][it] = b4[h][it] = f4zero();
-                    if (!live[it]) continue;
-                    const uint32_t o = off[it] + (h ? hsB : 0u);
+                    if (!w.live[it]) continue;
+                    const uint32_t o = w.off[it] + (h ? w.hsB : 0u);
                     g4[h][it] = __ldcs(reinterpret_cast<const float4 *>(gr + o));
                     x4[h][it] = __ldg(reinterpret_cast<const float4 *>(xin + o));
                     if (S0) a4[h][it] = __ldcs(reinterpret_cast<const float4 *>(m0 + o));
@@ -406,8 +370,8 @@ __global__ void __launch_bounds__(32 * owner_warps(REG), 16 / owner_warps(REG)) 
             for (int h = 0; h < HALVES; ++h)
 #pragma unroll
                 for (int it = 0; it < NIT; ++it) {
-                    if (!live[it]) continue;
-                    const uint32_t o = off[it] + (h ? hsB : 0u);
+                    if (!w.live[it]) continue;
+                    const uint32_t o = w.off[it] + (h ? w.hsB : 0u);
                     const float4 g = g4[h][it] + (h ? ai[it] : ar[it]);
                     const float4 xn = update4<KIND, REG>(x4[h][it], g, a4[h][it], b4[h][it], op, op.reg, racc);
                     __stcs(reinterpret_cast<float4 *>(xo + o), xn);
@@ -420,36 +384,19 @@ __global__ void __launch_bounds__(32 * owner_warps(REG), 16 / owner_warps(REG)) 
     if (REG && x.reg_loss) flush_reg_loss(racc, x.reg_loss);
 }
 
-template <int HALVES, int NIT, int KIND, bool REG>
-static cudaError_t launch_owner(const TrainParams &p, const OwnerOptim &x, cudaStream_t st)
-{
-    kge_bucket_owner_kernel<HALVES, NIT, KIND, REG><<<(int)((x.rows + owner_warps(REG) - 1) / owner_warps(REG)), 32 * owner_warps(REG), 0, st>>>(p, x);
-    return cudaGetLastError();
-}
-
-template <int KIND, bool REG>
-static cudaError_t launch_owner_shape(const TrainParams &p, const OwnerOptim &x, int nit, cudaStream_t st)
-{
-    const bool two = p.model != KGE_DISTMULT;
-    if (nit <= 1) return two ? launch_owner<2, 1, KIND, REG>(p, x, st) : launch_owner<1, 1, KIND, REG>(p, x, st);
-    if (nit == 2) return two ? launch_owner<2, 2, KIND, REG>(p, x, st) : launch_owner<1, 2, KIND, REG>(p, x, st);
-    if (two) return cudaErrorInvalidValue;
-    return launch_owner<1, 4, KIND, REG>(p, x, st);
-}
-
 cudaError_t launch_bucket_sum_optimizer(const TrainParams &p, int nit, const OptimParams &o, const float *in, float *out,
                                         float *grad, float *slot0, float *slot1, long long rows, double *reg_loss,
                                         cudaStream_t st)
 {
     if (rows == 0) return cudaSuccess;
     const OwnerOptim x{in, out, grad, slot0, slot1, rows, reg_loss, o};
-    const bool reg = o.reg.p > 0;
-    switch (o.kind) {
-    case KGE_OPT_SGD: return reg ? launch_owner_shape<KGE_OPT_SGD, true>(p, x, nit, st) : launch_owner_shape<KGE_OPT_SGD, false>(p, x, nit, st);
-    case KGE_OPT_ADAM: return reg ? launch_owner_shape<KGE_OPT_ADAM, true>(p, x, nit, st) : launch_owner_shape<KGE_OPT_ADAM, false>(p, x, nit, st);
-    case KGE_OPT_ADAGRAD: return reg ? launch_owner_shape<KGE_OPT_ADAGRAD, true>(p, x, nit, st) : launch_owner_shape<KGE_OPT_ADAGRAD, false>(p, x, nit, st);
-    default: return cudaErrorInvalidValue;
-    }
+    return dispatch_optimizer(o.kind, o.reg.p > 0, [&](auto kind, auto reg) {
+        constexpr int W = owner_warps(reg);
+        return dispatch_trilinear_shape(p.model, nit, [&](auto halves, auto nits) {
+            kge_bucket_owner_kernel<halves, nits, decltype(kind)::value, decltype(reg)::value><<<(int)((rows + W - 1) / W), 32 * W, 0, st>>>(p, x);
+            return cudaGetLastError();
+        });
+    });
 }
 
 }  // namespace kge

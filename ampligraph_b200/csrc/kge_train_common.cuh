@@ -1,8 +1,11 @@
 // kge_train_common.cuh -- device helpers shared by the training kernels (kge_train.cu: the general kernel;
 // kge_train_res.cu: the resident trilinear fast path): fp32-pair float4 arithmetic, the gradient sink, warp
-// reductions, and the per-positive loss + dL/dscore of the five reference losses; on the host, the launch they share.
+// reductions, and the per-positive loss + dL/dscore of the five reference losses; on the host, the launch they share and the
+// trilinear row-shape dispatch.
 #pragma once
 #include <math.h>
+
+#include <type_traits>
 
 #include "kge_internal.h"
 
@@ -407,6 +410,22 @@ static cudaError_t launch_persistent(Kernel kern, const TrainParams &p, const Tr
     const long long want = (p.B + slot.warps - 1) / slot.warps, cap = (long long)occ * sm_count;
     kern<<<(int)(want < cap ? want : cap), threads, smem, st>>>(p);
     return cudaGetLastError();
+}
+
+// Host side of the trilinear fast paths: returns launch(std::integral_constant<int, HALVES>, std::integral_constant<int,
+// NIT>) for the row shape of model and nit.  HALVES = 1 for DistMult, 2 (re / im) for ComplEx and HolE; NIT is the number
+// of float4 chunks per lane and half.  NIT = 4 (rows of 512+ floats per half) is DistMult's alone: only its per-lane state
+// fits the register file (kge_create).
+template <class Launch>
+static cudaError_t dispatch_trilinear_shape(int model, int nit, Launch &&launch)
+{
+    using one = std::integral_constant<int, 1>;
+    using two = std::integral_constant<int, 2>;
+    const bool halves2 = model != KGE_DISTMULT;
+    if (nit <= 1) return halves2 ? launch(two{}, one{}) : launch(one{}, one{});
+    if (nit == 2) return halves2 ? launch(two{}, two{}) : launch(one{}, two{});
+    if (halves2) return cudaErrorInvalidValue;
+    return launch(one{}, std::integral_constant<int, 4>{});
 }
 
 }  // namespace kge

@@ -372,21 +372,13 @@ __global__ void __launch_bounds__(THREADS) kge_train_res_kernel(const TrainParam
 }
 
 // ---- host side -------------------------------------------------------------------------------------------------------------
-template <int HALVES, int NIT>
-static cudaError_t launch_res(const TrainParams &p, const TrainSlot &slot, int sm_count, cudaStream_t st)
-{
-    constexpr int THREADS = KGE_TRAIN_THREADS(KGE_COMPLEX, NIT);
-    return launch_persistent(p.bk.g ? kge_train_res_kernel<HALVES, NIT, THREADS, true> : kge_train_res_kernel<HALVES, NIT, THREADS, false>,
-                             p, slot, sm_count, st);
-}
-
 cudaError_t launch_train_res(const TrainParams &p, int nit, const TrainSlot &slot, int sm_count, cudaStream_t st)
 {
-    const bool two = p.model != KGE_DISTMULT;
-    if (nit <= 1) return two ? launch_res<2, 1>(p, slot, sm_count, st) : launch_res<1, 1>(p, slot, sm_count, st);
-    if (nit == 2) return two ? launch_res<2, 2>(p, slot, sm_count, st) : launch_res<1, 2>(p, slot, sm_count, st);
-    if (two) return cudaErrorInvalidValue;  // rows of 512+ floats per half: only DistMult's per-lane state fits the register file (kge_create)
-    return launch_res<1, 4>(p, slot, sm_count, st);
+    return dispatch_trilinear_shape(p.model, nit, [&](auto halves, auto nits) {
+        constexpr int THREADS = KGE_TRAIN_THREADS(KGE_COMPLEX, nits);
+        return launch_persistent(p.bk.g ? kge_train_res_kernel<halves, nits, THREADS, true> : kge_train_res_kernel<halves, nits, THREADS, false>,
+                                 p, slot, sm_count, st);
+    });
 }
 
 }  // namespace kge

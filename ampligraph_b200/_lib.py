@@ -17,7 +17,7 @@ KGE_OK, KGE_ERR_INVALID_ARGUMENT, KGE_ERR_CUDA, KGE_ERR_UNSUPPORTED = 0, 1, 2, 3
 SCORING = {"TransE": 0, "DistMult": 1, "ComplEx": 2, "HolE": 3, "RotatE": 4}
 LOSSES = {"pairwise": 0, "nll": 1, "absolute_margin": 2, "self_adversarial": 3, "multiclass_nll": 4}
 REDUCTIONS = {"sum": 0, "mean": 1}
-OPTIMIZERS = {"sgd": 0, "adam": 1, "adagrad": 2}
+OPTIMIZERS = {"sgd": 0, "adam": 1, "adagrad": 2, "rmsprop": 3, "adadelta": 4, "adamax": 5}
 SIDES = {"s": 0, "o": 1}
 STRATEGIES = {"worst": 0, "best": 1, "middle": 2}
 STEP_FUSED, STEP_FORWARD_ONLY, STEP_BACKWARD_EXT, STEP_FUSED_DEFER = 0, 1, 2, 3
@@ -38,7 +38,7 @@ class KgeOptimizerConfig(C.Structure):
     _fields_ = [("struct_size", C.c_int32), ("kind", C.c_int32), ("learning_rate", C.c_float),
                 ("beta_1", C.c_float), ("beta_2", C.c_float), ("epsilon", C.c_float), ("momentum", C.c_float),
                 ("initial_accumulator_value", C.c_float), ("reg_p", C.c_int32), ("reg_lambda", C.c_float),
-                ("reg_p2", C.c_int32), ("reg_lambda2", C.c_float)]
+                ("reg_p2", C.c_int32), ("reg_lambda2", C.c_float), ("rho", C.c_float), ("centered", C.c_int32)]
 
 
 class KgeShardMap(C.Structure):

@@ -1,5 +1,6 @@
 // kge_api.cu -- the extern "C" boundary of libkge_b200.so (see include/kge_b200.h).
 #include <stdarg.h>
+#include <stddef.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -7,6 +8,7 @@
 #include <new>
 
 #include "kge_internal.h"
+#include "kge_optim_common.cuh"  // uses_slot0 / uses_slot1: which slot buffers a kind needs
 #include "kge_rank_common.cuh"  // the OP_* chains kge_knn / kge_radius_neighbors choose by metric
 
 using namespace kge;
@@ -628,14 +630,24 @@ extern "C" int kge_train_step_sharded(kge_handle *h, int32_t mode, const kge_sha
                            dpos_dev, dneg_dev, stream);
 }
 
-static int check_optim(const kge_optimizer_config *opt, const char *fn)
+// Checks a caller's config and copies it into *out, widened to the current layout.  A config of the layout before rho
+// (struct_size == offsetof(kge_optimizer_config, rho)) is accepted for the kinds that layout knew; its new fields read
+// as 0.
+static int check_optim(const kge_optimizer_config *opt, const char *fn, kge_optimizer_config *out)
 {
-    if (!opt || opt->struct_size != (int32_t)sizeof(kge_optimizer_config))
+    const int32_t old_size = (int32_t)offsetof(kge_optimizer_config, rho);
+    if (!opt || (opt->struct_size != (int32_t)sizeof(kge_optimizer_config) && opt->struct_size != old_size))
         return fail(KGE_ERR_INVALID_ARGUMENT, "%s: bad kge_optimizer_config (ABI mismatch)", fn);
-    if (opt->kind < KGE_OPT_SGD || opt->kind > KGE_OPT_ADAGRAD)
+    const int last = opt->struct_size == old_size ? KGE_OPT_ADAGRAD : KGE_OPT_ADAMAX;
+    if (opt->kind < KGE_OPT_SGD || opt->kind > last)
         return fail(KGE_ERR_INVALID_ARGUMENT, "Could not interpret optimizer identifier: %d", opt->kind);
     if (opt->reg_p < 0 || opt->reg_p2 < 0 || (opt->reg_p == 0 && opt->reg_p2 != 0))
         return fail(KGE_ERR_INVALID_ARGUMENT, "%s: bad regulariser (reg_p >= 0; reg_p2 needs reg_p)", fn);
+    memset(out, 0, sizeof(*out));
+    memcpy(out, opt, (size_t)opt->struct_size);
+    out->struct_size = (int32_t)sizeof(kge_optimizer_config);
+    if (out->kind == KGE_OPT_RMSPROP && out->centered && out->momentum != 0.f)
+        return fail(KGE_ERR_UNSUPPORTED, "%s: centered RMSprop with momentum needs a third slot buffer (not supported)", fn);
     return KGE_OK;
 }
 static RegParams reg_of(const kge_optimizer_config *opt)
@@ -653,14 +665,20 @@ static void fill_optim(const kge_optimizer_config *opt, int64_t t, OptimParams &
     o.eps = opt->epsilon;
     o.momentum = opt->momentum;
     o.reg = reg_of(opt);
-    // legacy Adam: lr_t = lr * sqrt(1 - beta2^t) / (1 - beta1^t), in fp64 on the host
-    o.lr_t = (float)((double)opt->learning_rate * sqrt(1.0 - pow((double)opt->beta_2, (double)t)) /
-                     (1.0 - pow((double)opt->beta_1, (double)t)));
+    o.rho = opt->rho;
+    o.centered = opt->centered;
+    // the bias-corrected step, in fp64 on the host and rounded once: legacy Adam lr*sqrt(1 - beta2^t)/(1 - beta1^t),
+    // Adamax lr/(1 - beta1^t)
+    if (opt->kind == KGE_OPT_ADAMAX)
+        o.lr_t = (float)((double)opt->learning_rate / (1.0 - pow((double)opt->beta_1, (double)t)));
+    else
+        o.lr_t = (float)((double)opt->learning_rate * sqrt(1.0 - pow((double)opt->beta_2, (double)t)) /
+                         (1.0 - pow((double)opt->beta_1, (double)t)));
 }
 static bool slots_ok(const kge_optimizer_config *opt, const float *s0, const float *s1)
 {
-    const bool need0 = opt->kind != KGE_OPT_SGD || opt->momentum != 0.f;
-    const bool need1 = opt->kind == KGE_OPT_ADAM;
+    const bool need0 = uses_slot0(opt->kind, opt->momentum);
+    const bool need1 = uses_slot1(opt->kind, opt->momentum, opt->centered);
     return !((need0 && !s0) || (need1 && !s1));
 }
 
@@ -669,7 +687,9 @@ extern "C" int kge_optimizer_step(kge_handle *h, const kge_optimizer_config *opt
                                   double *reg_loss_dev, void *stream)
 {
     KGE_CHECK_HANDLE(h, "kge_optimizer_step");
-    if (int rc = check_optim(opt, "kge_optimizer_step")) return rc;
+    kge_optimizer_config cfg;
+    if (int rc = check_optim(opt, "kge_optimizer_step", &cfg)) return rc;
+    opt = &cfg;
     if (rows < 0 || t < 1) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step: rows >= 0 and t >= 1 required");
     if (rows == 0) return KGE_OK;
     if (!table_dev || !grad_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step: null table/grad");
@@ -689,7 +709,9 @@ extern "C" int kge_optimizer_step_deferred(kge_handle *h, const kge_optimizer_co
 {
     KGE_CHECK_HANDLE(h, "kge_optimizer_step_deferred");
     if (!h->sum_pending) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_deferred: no deferred step is pending");
-    if (int rc = check_optim(opt, "kge_optimizer_step_deferred")) return rc;
+    kge_optimizer_config cfg;
+    if (int rc = check_optim(opt, "kge_optimizer_step_deferred", &cfg)) return rc;
+    opt = &cfg;
     if (t < 1) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_deferred: t >= 1 required");
     const TrainParams &p = h->pending;
     const size_t ent_floats = (size_t)h->cfg.n_ent * h->L.ld;
@@ -751,7 +773,9 @@ extern "C" int kge_optimizer_step_lazy(kge_handle *h, const kge_optimizer_config
                                        const int32_t *row_stamp_dev, int32_t stamp, double *reg_loss_dev, void *stream)
 {
     KGE_CHECK_HANDLE(h, "kge_optimizer_step_lazy");
-    if (int rc = check_optim(opt, "kge_optimizer_step_lazy")) return rc;
+    kge_optimizer_config cfg;
+    if (int rc = check_optim(opt, "kge_optimizer_step_lazy", &cfg)) return rc;
+    opt = &cfg;
     if (rows < 0 || t < 1) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_lazy: rows >= 0 and t >= 1 required");
     if (rows == 0) return KGE_OK;
     if (!table_dev || !grad_dev || !row_stamp_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_lazy: null pointer");
@@ -778,7 +802,9 @@ extern "C" int kge_optimizer_step_sharded(kge_handle *h, const kge_optimizer_con
                                           int64_t row_end, double *reg_loss_dev, void *stream)
 {
     KGE_CHECK_HANDLE(h, "kge_optimizer_step_sharded");
-    if (int rc = check_optim(opt, "kge_optimizer_step_sharded")) return rc;
+    kge_optimizer_config cfg;
+    if (int rc = check_optim(opt, "kge_optimizer_step_sharded", &cfg)) return rc;
+    opt = &cfg;
     if (int rc = check_world(world, rank, "kge_optimizer_step_sharded")) return rc;
     if (row_begin < 0 || row_end < row_begin || t < 1) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_sharded: bad row range / t");
     if (row_end == row_begin) return KGE_OK;
@@ -805,11 +831,15 @@ extern "C" int kge_optimizer_step_exchange(kge_handle *h, const kge_optimizer_co
                                            double *reg_loss_dev, void *stream)
 {
     KGE_CHECK_HANDLE(h, "kge_optimizer_step_exchange");
-    if (int rc = check_optim(opt_ent, "kge_optimizer_step_exchange")) return rc;
-    if (int rc = check_optim(opt_rel, "kge_optimizer_step_exchange")) return rc;
+    kge_optimizer_config cfg_ent, cfg_rel;
+    if (int rc = check_optim(opt_ent, "kge_optimizer_step_exchange", &cfg_ent)) return rc;
+    if (int rc = check_optim(opt_rel, "kge_optimizer_step_exchange", &cfg_rel)) return rc;
+    opt_ent = &cfg_ent;
+    opt_rel = &cfg_rel;
     if (int rc = check_world(world, rank, "kge_optimizer_step_exchange")) return rc;
     if (opt_ent->kind != opt_rel->kind || opt_ent->learning_rate != opt_rel->learning_rate || opt_ent->beta_1 != opt_rel->beta_1 ||
-        opt_ent->beta_2 != opt_rel->beta_2 || opt_ent->epsilon != opt_rel->epsilon || opt_ent->momentum != opt_rel->momentum)
+        opt_ent->beta_2 != opt_rel->beta_2 || opt_ent->epsilon != opt_rel->epsilon || opt_ent->momentum != opt_rel->momentum ||
+        opt_ent->rho != opt_rel->rho || opt_ent->centered != opt_rel->centered)
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_exchange: the two tables may differ in their regulariser only");
     const int64_t total_rows = h->cfg.n_ent + h->cfg.n_rel;
     if (row_begin < 0 || row_end < row_begin || row_end > total_rows || t < 1)

@@ -105,6 +105,8 @@ struct OptimParams {
     int kind;
     float lr, lr_t, beta1, beta2, eps, momentum;
     RegParams reg;
+    float rho;     // RMSprop / Adadelta decay
+    int centered;  // RMSprop
 };
 struct ExchangeParams {  // kge_optimizer_step_exchange
     int world, rank, phases;

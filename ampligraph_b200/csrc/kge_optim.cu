@@ -25,17 +25,16 @@ __global__ void __launch_bounds__(256) kge_optim_kernel(float4 *__restrict__ var
                                                         float4 *__restrict__ s0, float4 *__restrict__ s1,
                                                         long long n4, OptimParams o, double *reg_loss)
 {
-    constexpr bool S0 = KIND != KGE_OPT_SGD, S1 = KIND == KGE_OPT_ADAM;
-    const bool mom = KIND == KGE_OPT_SGD && o.momentum != 0.f;
+    const bool S0 = uses_slot0(KIND, o.momentum), S1 = uses_slot1(KIND, o.momentum, o.centered);
     float racc = 0.f;
     const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
     const long long stride = (long long)gridDim.x * blockDim.x;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
         float4 x4 = var[i], g4 = grad[i], a4 = z, b4 = z;
-        if (S0 || mom) a4 = s0[i];
+        if (S0) a4 = s0[i];
         if (S1) b4 = s1[i];
         var[i] = update4<KIND, REG>(x4, g4, a4, b4, o, o.reg, racc);
-        if (S0 || mom) s0[i] = a4;
+        if (S0) s0[i] = a4;
         if (S1) s1[i] = b4;
         grad[i] = z;
     }
@@ -63,8 +62,7 @@ __global__ void __launch_bounds__(256) kge_optim_sharded_kernel(PeerPtrs pp, int
                                                                 float4 *__restrict__ s1, long long off4,
                                                                 long long n4, OptimParams o, double *reg_loss)
 {
-    constexpr bool S0 = KIND != KGE_OPT_SGD, S1 = KIND == KGE_OPT_ADAM;
-    const bool mom = KIND == KGE_OPT_SGD && o.momentum != 0.f;
+    const bool S0 = uses_slot0(KIND, o.momentum), S1 = uses_slot1(KIND, o.momentum, o.centered);
     float racc = 0.f;
     const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
     const long long stride = (long long)gridDim.x * blockDim.x;
@@ -79,13 +77,13 @@ __global__ void __launch_bounds__(256) kge_optim_sharded_kernel(PeerPtrs pp, int
         for (int q = 0; q < KGE_MAX_PEERS; ++q)
             if (q < world) { g4.x += gq[q].x; g4.y += gq[q].y; g4.z += gq[q].z; g4.w += gq[q].w; }
         float4 x4 = pp.table[rank][gi], a4 = z, b4 = z;  // all replicas are identical; read the local one
-        if (S0 || mom) a4 = s0[i];
+        if (S0) a4 = s0[i];
         if (S1) b4 = s1[i];
         const float4 xn = update4<KIND, REG>(x4, g4, a4, b4, o, o.reg, racc);
 #pragma unroll
         for (int q = 0; q < KGE_MAX_PEERS; ++q)
             if (q < world) __stcg(pp.table[q] + gi, xn);  // deliver the updated rows to every replica
-        if (S0 || mom) s0[i] = a4;
+        if (S0) s0[i] = a4;
         if (S1) s1[i] = b4;
     }
     if (REG && reg_loss) flush_reg_loss(racc, reg_loss);
@@ -230,9 +228,8 @@ __device__ __forceinline__ unsigned long long globaltimer_ns()
 template <int KIND, bool REG, int WORLD, bool MC>
 __global__ void __launch_bounds__(256) kge_optim_exchange_kernel(const ExchangeArgs x, const OptimParams o)
 {
-    constexpr bool S0 = KIND != KGE_OPT_SGD, S1 = KIND == KGE_OPT_ADAM;
+    const bool S0 = uses_slot0(KIND, o.momentum), S1 = uses_slot1(KIND, o.momentum, o.centered);
     constexpr int U = WORLD <= 4 ? 4 : 2;  // float4s per thread per trip (U*WORLD peer loads in flight per thread)
-    const bool mom = KIND == KGE_OPT_SGD && o.momentum != 0.f;
     const int rank = x.rank;
     const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
     const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -258,7 +255,7 @@ __global__ void __launch_bounds__(256) kge_optim_exchange_kernel(const ExchangeA
     auto update_and_deliver = [&](long long i, float4 g4) {
         const long long gi = x.off4 + i;
         float4 x4 = x.table[rank][gi], a4 = z, b4 = z;
-        if (S0 || mom) a4 = x.s0[i];
+        if (S0) a4 = x.s0[i];
         if (S1) b4 = x.s1[i];
         const float4 xn = update4<KIND, REG>(x4, g4, a4, b4, o, gi < x.ent4 ? x.reg_ent : x.reg_rel, racc);
         if (MC) {
@@ -267,7 +264,7 @@ __global__ void __launch_bounds__(256) kge_optim_exchange_kernel(const ExchangeA
 #pragma unroll
             for (int q = 0; q < WORLD; ++q) __stcg(x.table[q] + gi, xn);
         }
-        if (S0 || mom) x.s0[i] = a4;
+        if (S0) x.s0[i] = a4;
         if (S1) x.s1[i] = b4;
     };
     if constexpr (MC) {
@@ -432,8 +429,7 @@ __global__ void __launch_bounds__(256) kge_optim_lazy_kernel(float *__restrict__
                                                              long long rows, int ld, const int *__restrict__ row_stamp,
                                                              int stamp, OptimParams o, double *reg_loss)
 {
-    constexpr bool S0 = KIND != KGE_OPT_SGD, S1 = KIND == KGE_OPT_ADAM;
-    const bool mom = KIND == KGE_OPT_SGD && o.momentum != 0.f;
+    const bool S0 = uses_slot0(KIND, o.momentum), S1 = uses_slot1(KIND, o.momentum, o.centered);
     const int lane = threadIdx.x & 31;
     const long long warp0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const long long n_warps = ((long long)gridDim.x * blockDim.x) >> 5;
@@ -449,10 +445,10 @@ __global__ void __launch_bounds__(256) kge_optim_lazy_kernel(float *__restrict__
             for (int c = lane * 4; c < ld; c += 128) {
                 float4 x4 = *reinterpret_cast<float4 *>(var + off + c), g4 = *reinterpret_cast<float4 *>(grad + off + c);
                 float4 a4 = z, b4 = z;
-                if (S0 || mom) a4 = *reinterpret_cast<float4 *>(s0 + off + c);
+                if (S0) a4 = *reinterpret_cast<float4 *>(s0 + off + c);
                 if (S1) b4 = *reinterpret_cast<float4 *>(s1 + off + c);
                 *reinterpret_cast<float4 *>(var + off + c) = update4<KIND, REG>(x4, g4, a4, b4, o, o.reg, racc);
-                if (S0 || mom) *reinterpret_cast<float4 *>(s0 + off + c) = a4;
+                if (S0) *reinterpret_cast<float4 *>(s0 + off + c) = a4;
                 if (S1) *reinterpret_cast<float4 *>(s1 + off + c) = b4;
                 *reinterpret_cast<float4 *>(grad + off + c) = z;
             }

@@ -29,7 +29,35 @@ __device__ __forceinline__ float reg_grad(float x, const RegParams &r, float *lo
     return g;
 }
 
-// one element of the legacy update rules (optimizers.py:255-291 -> tf.keras.optimizers.legacy.*)
+// Which of the two slot buffers a kind reads and writes (kge_b200.h documents what each holds).  SGD's slot 0 exists
+// only with momentum, RMSprop's slot 1 only when centered (mg) or with momentum (mom); every other use is fixed by the
+// kind.  Every kernel and the host's argument check ask this one function.
+__host__ __device__ __forceinline__ constexpr bool uses_slot0(int kind, float momentum)
+{
+    return kind != KGE_OPT_SGD || momentum != 0.f;
+}
+__host__ __device__ __forceinline__ constexpr bool uses_slot1(int kind, float momentum, int centered)
+{
+    return kind == KGE_OPT_ADAM || kind == KGE_OPT_ADADELTA || kind == KGE_OPT_ADAMAX ||
+           (kind == KGE_OPT_RMSPROP && (centered != 0 || momentum != 0.f));
+}
+
+// One element of the legacy update rules (optimizers.py:255-291 -> tf.keras.optimizers.legacy.* and the training ops
+// they call).  g is the summed gradient plus the regulariser's, a / b are slot 0 / slot 1, fma is one rounding, every
+// other operation rounds to fp32 on its own (oracle/ref_step.py and tests/optim_oracle.py restate this order):
+//   SGD       momentum 0: x -= lr*g;  else a = mu*a - lr*g, x += a
+//   Adam      a = fma(g - a, 1-b1, a); b = fma(g*g - b, 1-b2, b); x -= (a*lr_t) / (sqrt(b) + eps)
+//             lr_t = lr*sqrt(1-b2^t)/(1-b1^t), fp64 on the host
+//   Adagrad   a = fma(g, g, a); x -= lr*g / (sqrt(a) + eps)
+//   RMSprop   momentum 0: a = fma(rho, a, (1-rho)*(g*g)); d = a, or when centered b = fma(rho, b, (1-rho)*g),
+//             d = fma(-b, b, a); x -= (lr*g) / (sqrt(d) + eps)
+//             momentum mu > 0 (ApplyRMSProp, never centered): a = fma(g*g - a, 1-rho, a);
+//             b = fma(mu, b, (lr*g) / sqrt(a + eps)); x -= b
+//   Adadelta  a = fma(rho, a, (1-rho)*(g*g)); u = sqrt(b + eps) / sqrt(a + eps) * g; x = fma(-lr, u, x);
+//             b = fma(rho, b, (1-rho)*(u*u))
+//   Adamax    a = fma(g - a, 1-b1, a); b = max(b2*b, |g|); x = fma(-lr_t, a / (b + eps), x)
+//             lr_t = lr/(1-b1^t), fp64 on the host
+// The new rules spell their products as __fmul_rn so that the compiler cannot contract them into an fma.
 template <int KIND>
 __device__ __forceinline__ void apply_rule(float &x, float gg, float &a, float &b, const OptimParams &o)
 {
@@ -40,6 +68,30 @@ __device__ __forceinline__ void apply_rule(float &x, float gg, float &a, float &
     } else if (KIND == KGE_OPT_ADAGRAD) {
         a = fmaf(gg, gg, a);
         x -= o.lr * gg / (sqrtf(a) + o.eps);
+    } else if (KIND == KGE_OPT_RMSPROP) {
+        const float g2 = __fmul_rn(gg, gg), step = __fmul_rn(o.lr, gg);
+        if (o.momentum != 0.f) {
+            a = fmaf(__fsub_rn(g2, a), 1.f - o.rho, a);
+            b = fmaf(o.momentum, b, step / sqrtf(a + o.eps));
+            x -= b;
+        } else {
+            a = fmaf(o.rho, a, __fmul_rn(1.f - o.rho, g2));
+            float d = a;
+            if (o.centered) {
+                b = fmaf(o.rho, b, __fmul_rn(1.f - o.rho, gg));
+                d = fmaf(-b, b, a);
+            }
+            x -= step / (sqrtf(d) + o.eps);
+        }
+    } else if (KIND == KGE_OPT_ADADELTA) {
+        a = fmaf(o.rho, a, __fmul_rn(1.f - o.rho, __fmul_rn(gg, gg)));
+        const float u = __fmul_rn(sqrtf(b + o.eps) / sqrtf(a + o.eps), gg);
+        x = fmaf(-o.lr, u, x);
+        b = fmaf(o.rho, b, __fmul_rn(1.f - o.rho, __fmul_rn(u, u)));
+    } else if (KIND == KGE_OPT_ADAMAX) {
+        a = fmaf(gg - a, 1.f - o.beta1, a);
+        b = fmaxf(__fmul_rn(o.beta2, b), fabsf(gg));
+        x = fmaf(-o.lr_t, a / (b + o.eps), x);
     } else {  // SGD (momentum optional)
         if (o.momentum != 0.f) { a = o.momentum * a - o.lr * gg; x += a; }
         else x -= o.lr * gg;
@@ -87,6 +139,9 @@ static cudaError_t dispatch_optimizer(int kind, bool reg, Launch &&launch)
     case KGE_OPT_SGD: return with_reg(std::integral_constant<int, KGE_OPT_SGD>{});
     case KGE_OPT_ADAM: return with_reg(std::integral_constant<int, KGE_OPT_ADAM>{});
     case KGE_OPT_ADAGRAD: return with_reg(std::integral_constant<int, KGE_OPT_ADAGRAD>{});
+    case KGE_OPT_RMSPROP: return with_reg(std::integral_constant<int, KGE_OPT_RMSPROP>{});
+    case KGE_OPT_ADADELTA: return with_reg(std::integral_constant<int, KGE_OPT_ADADELTA>{});
+    case KGE_OPT_ADAMAX: return with_reg(std::integral_constant<int, KGE_OPT_ADAMAX>{});
     default: return cudaErrorInvalidValue;
     }
 }

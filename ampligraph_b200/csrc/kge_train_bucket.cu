@@ -305,8 +305,7 @@ __host__ __device__ constexpr int owner_warps(bool reg) { return reg ? 8 : 1; }
 template <int HALVES, int NIT, int KIND, bool REG>
 __global__ void __launch_bounds__(32 * owner_warps(REG), 16 / owner_warps(REG)) kge_bucket_owner_kernel(const TrainParams p, const OwnerOptim x)
 {
-    constexpr bool S1 = KIND == KGE_OPT_ADAM;
-    const bool S0 = KIND != KGE_OPT_SGD || x.o.momentum != 0.f;
+    const bool S0 = uses_slot0(KIND, x.o.momentum), S1 = uses_slot1(KIND, x.o.momentum, x.o.centered);
     const int lane = threadIdx.x & 31;
     const long long e = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     float racc = 0.f;

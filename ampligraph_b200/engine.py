@@ -35,6 +35,21 @@ def fp32_floor(x):
     return float(r)
 
 
+def optimizer_slots(cfg):
+    """The slot buffers an optimizer config uses (kge_b200.h, kge_optimizer_config; the library's uses_slot0 / uses_slot1)
+    -> (initial value of slot 0, of slot 1), None for a slot the kind does not use."""
+    O = _lib.OPTIMIZERS
+    s0 = None if cfg.kind == O["sgd"] and cfg.momentum == 0.0 else 0.0
+    if cfg.kind == O["adagrad"]:
+        s0 = float(cfg.initial_accumulator_value)
+    s1 = 0.0 if (cfg.kind in (O["adam"], O["adadelta"], O["adamax"])
+                 or (cfg.kind == O["rmsprop"] and (cfg.centered or cfg.momentum != 0.0))) else None
+    return s0, s1
+
+
+RHO_DEFAULT = {"rmsprop": 0.9, "adadelta": 0.95}  # Keras legacy defaults; unused by the other kinds
+
+
 INT32_MAX = 2 ** 31 - 1
 DBSCAN_BATCH = 1024  # queries per kge_radius_* call of KGEEngine.dbscan (discovery.find_duplicates' batch)
 
@@ -154,9 +169,9 @@ def _traced(name):
 class KGEEngine:
     def __init__(self, scoring_type, k, eta, n_ent, n_rel, loss="pairwise", loss_params=None,
                  optimizer="adam", optimizer_params=None, regularizer=None, device=0, neg_group=0,
-                 table_alloc=None, ent_rows=None, max_rel_size=None, rank_mode=None, rank_pair_cap=0):
+                 table_alloc=None, ent_rows=None, max_rel_size=None, rank_mode=None, rank_pair_cap=0, lazy_tables=None):
         """regularizer: None | {"p":, "lambda": [, "p2":, "lambda2":]} | a pair [entities, relations] of those
-        (EmbeddingLookupLayer.py:131-155).  max_rel_size: RotatE phase normalisation when it differs from the
+        (EmbeddingLookupLayer.py:131-155).  lazy_tables: see set_optimizer.  max_rel_size: RotatE phase normalisation when it differs from the
         relation-table rows (RotatE.py:96).  rank_mode: 'auto' (tensor-core filter + exact refine for the bilinear
         models) | 'exact' (FP32 canonical chain for every pair); env KGE_B200_RANK_MODE overrides the default."""
         self.lib = _lib.load()
@@ -200,7 +215,7 @@ class KGEEngine:
                 self.ent, self.rel = self._pblock[:self.ent_rows], self._pblock[self.ent_rows:]
                 self.g_ent, self.g_rel = self._gblock[:self.ent_rows], self._gblock[self.ent_rows:]
             self.loss_acc = torch.zeros(2, dtype=torch.float64, device=self.device)  # [batch loss, reg loss]
-        self.set_optimizer(optimizer, optimizer_params, regularizer)
+        self.set_optimizer(optimizer, optimizer_params, regularizer, lazy_tables)
         self.launches = 0  # kernels launched by this engine (bench.py reports it)
         self._rank_ws = None  # caller-owned ranking workspace (kge_rank_workspace_bytes), grown on demand
         self._pblock_next = None  # second [ent | rel] parameter block of the deferred steps, allocated on first use
@@ -222,15 +237,24 @@ class KGEEngine:
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
     # -- optimizer state (optimizers.py:255-291) ---------------------------
-    def set_optimizer(self, name="adam", params=None, regularizer=None):
+    def set_optimizer(self, name="adam", params=None, regularizer=None, lazy_tables=None):
+        """name: a key of _lib.OPTIMIZERS, or 'lazy_<name>' (extension): update only the rows the step looked up
+        (kge_optimizer_step_lazy) in both tables.  lazy_tables: None (the name decides) or a pair (entities, relations)
+        of bools that chooses the looked-up-rows rule per table, e.g. the reference's rule for Adamax with a regulariser
+        on the entities only (latent_features.optimizers.table_rules)."""
         name = name.lower()
-        # 'lazy_<name>' (extension): update only the rows touched by the step (kge_optimizer_step_lazy)
-        self.lazy = name.startswith("lazy_")
-        if self.lazy:
+        prefixed = name.startswith("lazy_")
+        if prefixed:
             name = name[len("lazy_"):]
         if name not in _lib.OPTIMIZERS:
             raise ValueError("Could not interpret optimizer identifier: %r" % (name,))
+        lazy = (prefixed, prefixed) if lazy_tables is None else tuple(bool(x) for x in lazy_tables)
+        assert len(lazy) == 2, "Incorrect length for lazy_tables. Expected 2, got {}".format(len(lazy))
+        self.lazy_tables = {"ent": lazy[0], "rel": lazy[1]}
+        self.lazy = any(lazy)
         p = dict(params or {})
+        if name == "rmsprop" and p.get("centered") and float(p.get("momentum", 0.0)) != 0.0:
+            raise NotImplementedError("centered RMSprop with momentum needs a third slot buffer (not supported)")
         regs = list(regularizer) if isinstance(regularizer, (list, tuple)) else [regularizer, regularizer]
         assert len(regs) == 2, "Incorrect length for regularizer. Expected 2, got {}".format(len(regs))
 
@@ -241,25 +265,21 @@ class KGEEngine:
                 float(p.get("beta_1", 0.9)), float(p.get("beta_2", 0.999)), float(p.get("epsilon", 1e-7)),
                 float(p.get("momentum", 0.0)), float(p.get("initial_accumulator_value", 0.1)),
                 int(reg.get("p", 2)) if reg else 0, float(reg.get("lambda", 1e-5)),
-                int(reg.get("p2", 0)) if reg else 0, float(reg.get("lambda2", 0.0)))
+                int(reg.get("p2", 0)) if reg else 0, float(reg.get("lambda2", 0.0)),
+                float(p.get("rho", RHO_DEFAULT.get(name, 0.0))), int(bool(p.get("centered", False))))
         self.opt_cfgs = {"ent": cfg_for(regs[0]), "rel": cfg_for(regs[1])}
         self.opt_cfg = self.opt_cfgs["ent"]  # hyper-parameters are common to both tables; only the regulariser differs
         self.opt_name = name
         self.t = 0
         # slots as [ent | rel] blocks, like the tables (see __init__): slots[key] are row slices of them
-        mk = lambda v=0.0: torch.full((self.ent_rows + self.n_rel, self.ld), v, dtype=torch.float32, device=self.device)
+        mk = lambda v: None if v is None else torch.full((self.ent_rows + self.n_rel, self.ld), v, dtype=torch.float32,
+                                                         device=self.device)
         cut = lambda blk: {"ent": None if blk is None else blk[:self.ent_rows], "rel": None if blk is None else blk[self.ent_rows:]}
-        b0 = b1 = None
-        if name == "adam":
-            b0, b1 = mk(), mk()
-        elif name == "adagrad":
-            b0 = mk(self.opt_cfg.initial_accumulator_value)
-        elif self.opt_cfg.momentum != 0.0:
-            b0 = mk()
+        b0, b1 = (mk(v) for v in optimizer_slots(self.opt_cfg))
         self._sblocks = (b0, b1)
         self.slots = {key: [cut(b0)[key], cut(b1)[key]] for key in ("ent", "rel")}
         self.stamps = {"ent": None, "rel": None}
-        if self.lazy:
+        if self.lazy:  # both: the training kernels stamp only while the entity buffer is set
             self.stamps = {"ent": torch.zeros(self.ent_rows, dtype=torch.int32, device=self.device),
                            "rel": torch.zeros(self.n_rel, dtype=torch.int32, device=self.device)}
         _lib.check(self.lib.kge_set_row_stamps(self.h, _ptr(self.stamps["ent"]), _ptr(self.stamps["rel"])))
@@ -421,7 +441,7 @@ class KGEEngine:
         for key, table, grad, rows in (("ent", self.ent, self.g_ent, self.ent_rows),
                                        ("rel", self.rel, self.g_rel, self.n_rel)):
             s0, s1 = self.slots[key]
-            if self.lazy:
+            if self.lazy_tables[key]:
                 _lib.check(self.lib.kge_optimizer_step_lazy(
                     self.h, C.byref(self.opt_cfgs[key]), self.t, _ptr(table), _ptr(grad), _ptr(s0), _ptr(s1), rows,
                     _ptr(self.stamps[key]), self.lib.kge_step_stamp(self._last_step),

@@ -120,11 +120,14 @@ class ScoringBasedEmbeddingModel:
         reg = [r.kernel_params() if r is not None else None for r in self._regularizer]
         if self.scoring_type == "RotatE":
             self.scoring_layer.max_rel_size = self.max_rel_size  # :338
+        # the reference's per-table rule: which tables its optimizer updates on the looked-up rows only
+        lazy = optimizers.table_rules(self.optimizer.name, self.optimizer.hyperparams, [r is not None for r in reg])
+
         def make_engine(alloc=None):
             return KGEEngine(self.scoring_type, self.k, self.eta, self.max_ent_size, self.max_rel_size,
                              loss=name or "pairwise", loss_params=lp, optimizer=self.optimizer.name,
                              optimizer_params=self.optimizer.hyperparams, regularizer=reg, device=self.device,
-                             table_alloc=alloc)
+                             table_alloc=alloc, lazy_tables=lazy)
         if self._world() > 1:
             from ..parallel import DataParallelTrainer
             self._dp = DataParallelTrainer(make_engine)

@@ -154,15 +154,9 @@ class DataParallelTrainer:
         lo, hi = self.shard
         # optimizer slots only for this rank's row shard of the concatenated block
         rows = hi - lo
-        mkslot = lambda v=0.0: torch.full((max(rows, 1), ld), v, dtype=torch.float32, device=eng.device)
-        if eng.opt_name == "adam":
-            self.slots = [mkslot(), mkslot()]
-        elif eng.opt_name == "adagrad":
-            self.slots = [mkslot(eng.opt_cfg.initial_accumulator_value), None]
-        elif eng.opt_cfg.momentum != 0.0:
-            self.slots = [mkslot(), None]
-        else:
-            self.slots = [None, None]
+        from .engine import optimizer_slots
+        self.slots = [None if v is None else torch.full((max(rows, 1), ld), v, dtype=torch.float32, device=eng.device)
+                      for v in optimizer_slots(eng.opt_cfg)]
         eng.slots = {"ent": [None, None], "rel": [None, None]}  # the full-size slots are not used on this path
         torch.cuda.synchronize()
         self.hdl.barrier(channel=0)  # one-off: every rank's buffer (zeroed flags included) exists before the first step

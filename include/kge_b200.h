@@ -65,7 +65,14 @@ enum kge_loss {
     KGE_LOSS_MULTICLASS_NLL = 4
 };
 enum kge_reduction { KGE_REDUCE_SUM = 0, KGE_REDUCE_MEAN = 1 }; /* loss_functions.py:124-129 */
-enum kge_optimizer { KGE_OPT_SGD = 0, KGE_OPT_ADAM = 1, KGE_OPT_ADAGRAD = 2 };
+enum kge_optimizer {
+    KGE_OPT_SGD = 0,
+    KGE_OPT_ADAM = 1,
+    KGE_OPT_ADAGRAD = 2,
+    KGE_OPT_RMSPROP = 3,
+    KGE_OPT_ADADELTA = 4,
+    KGE_OPT_ADAMAX = 5
+};
 enum kge_side { KGE_SIDE_S = 0, KGE_SIDE_O = 1 };
 enum kge_rank_strategy { KGE_RANK_WORST = 0, KGE_RANK_BEST = 1, KGE_RANK_MIDDLE = 2 };
 /* how kge_rank scores the candidates of DistMult / ComplEx / HolE (the bilinear models, a [b,K]x[K,E] contraction):
@@ -110,20 +117,32 @@ typedef struct kge_config {
                               filter -- a testing knob for its overflow fallback */
 } kge_config;
 
-/* optimizers.get (optimizers.py:255-291) -> tf.keras.optimizers.legacy.{SGD,Adam,Adagrad};
- * regularizers.LP_regularizer (regularizers.py:14-37) folded into the update. */
+/* optimizers.get (optimizers.py:255-291) -> tf.keras.optimizers.legacy.{SGD,Adam,Adagrad,RMSprop,Adadelta,Adamax};
+ * regularizers.LP_regularizer (regularizers.py:14-37) folded into the update.
+ * What the two slot buffers of the optimizer calls (slot0 / slot1, [rows, ld], zero-initialised unless noted) hold:
+ *   SGD       momentum accumulator (only with momentum != 0) / -
+ *   Adam      m / v
+ *   Adagrad   accumulator (initial_accumulator_value) / -
+ *   RMSprop   ms / mg when centered, the momentum accumulator when momentum != 0, else -
+ *             (centered with momentum needs a third slot: refused, KGE_ERR_UNSUPPORTED)
+ *   Adadelta  accum / accum_update
+ *   Adamax    m / v (the exponentially weighted infinity norm)
+ * A config whose struct_size stops before `rho` (the layout before RMSprop, Adadelta and Adamax) is accepted for the
+ * first three kinds; its rho and centered read as 0. */
 typedef struct kge_optimizer_config {
     int32_t struct_size;
     int32_t kind;         /* enum kge_optimizer */
     float learning_rate;  /* default 0.001 (optimizers.py:284) */
-    float beta_1, beta_2; /* Adam: 0.9, 0.999 */
+    float beta_1, beta_2; /* Adam, Adamax: 0.9, 0.999 */
     float epsilon;        /* 1e-7 */
-    float momentum;       /* SGD: 0 */
+    float momentum;       /* SGD, RMSprop: 0 */
     float initial_accumulator_value; /* Adagrad: 0.1 */
     int32_t reg_p;        /* 0 = no regulariser, else p of LP (1, 2, 3, ...) */
     float reg_lambda;     /* LP lambda (default 1e-5) */
     int32_t reg_p2;       /* optional second LP term (Keras 'l1_l2' = p 1 + p 2); 0 = none */
     float reg_lambda2;
+    float rho;            /* RMSprop: 0.9, Adadelta: 0.95 */
+    int32_t centered;     /* RMSprop: 0 */
 } kge_optimizer_config;
 
 const char *kge_last_error(void);
@@ -259,7 +278,7 @@ int kge_train_step_sharded(kge_handle *h, int32_t mode, const kge_shard_map *map
  * block, one launch per step), dense semantics, plus the LP regulariser's loss/gradient over the whole table
  * (regularizers.py:14-37; added to the loss at loss_functions.py:215-223).
  *   t            1-based iteration count (Adam bias correction)
- *   slot0/slot1  Adam m,v / SGD momentum,- / Adagrad accumulator,-  ([rows,ld] or NULL)
+ *   slot0/slot1  the kind's slots, as listed at kge_optimizer_config ([rows,ld] or NULL where the kind has none)
  *   reg_loss_dev double accumulator += lambda*sum|x|^p of the PRE-update table (may be NULL)
  * The gradient buffer is zeroed on the way out. */
 int kge_optimizer_step(kge_handle *h, const kge_optimizer_config *opt, int64_t t, float *table_dev,
@@ -288,8 +307,12 @@ int kge_optimizer_step_deferred(kge_handle *h, const kge_optimizer_config *opt, 
  * semantics of TensorFlow-Addons' LazyAdam).  Needed when the dense pass is unaffordable
  * (BASELINE configs[4]: 80 GB table).  kge_set_row_stamps registers caller-owned int32 [rows]
  * buffers; from then on kge_train_step writes kge_step_stamp(step) into the stamp of every row it
- * scatters a gradient to, and kge_optimizer_step_lazy(..., row_stamp_dev, kge_step_stamp(step))
- * updates exactly those rows (and zeroes their gradient rows). */
+ * looks up (whether or not its summed gradient is 0: the rows TensorFlow lists in the IndexedSlices of
+ * tf.nn.embedding_lookup), and kge_optimizer_step_lazy(..., row_stamp_dev, kge_step_stamp(step))
+ * updates exactly those rows (and zeroes their gradient rows).  Stamping is on only while the entity
+ * buffer is set, so a caller that updates only the relation table lazily registers both.  For
+ * RMSprop with momentum and Adamax this IS the reference's rule on a table without a regulariser
+ * (ResourceSparseApplyRMSProp, and Adamax's gather / scatter of the looked-up rows). */
 int kge_set_row_stamps(kge_handle *h, int32_t *ent_stamps_dev, int32_t *rel_stamps_dev);
 int32_t kge_step_stamp(uint64_t step);
 int kge_optimizer_step_lazy(kge_handle *h, const kge_optimizer_config *opt, int64_t t, float *table_dev,

@@ -11,7 +11,7 @@ import torch
 from .. import _lib
 from ..datasets import DataIndexer, FilterIndex, as_triple_array
 from ..engine import KGEEngine
-from ..evaluation import hits_at_n_score, mr_score, mrr_score
+from ..evaluation import hits_at_n_score, mr_score, mrr_score, train_test_split_no_unseen
 from . import initializers, loss_functions, optimizers, regularizers
 from .layers.scoring import SCORING_LAYER_REGISTRY
 
@@ -30,27 +30,48 @@ class History:
 
 
 class EarlyStopping:
-    """tf.keras.callbacks.EarlyStopping subset used with fit(validation_data=...): stop when `monitor`
-    (e.g. 'val_mrr') has not improved by `min_delta` for `patience` validations."""
+    """tf.keras.callbacks.EarlyStopping (Keras 2.15) used with fit(validation_data=...): stop when `monitor`
+    (e.g. 'val_mrr') has not improved by more than `min_delta` for `patience` epochs that report it.
 
-    def __init__(self, monitor="val_mrr", min_delta=0.0, patience=0, mode="auto", restore_best_weights=False):
+    Keras's rule: epochs without the monitored value are skipped; every other epoch counts one towards `wait`, and an
+    improvement sets `best`, resets `wait` to 0 and, with restore_best_weights, snapshots the tables (the first monitored
+    epoch always does).  Training stops when wait >= patience at an epoch other than the first, and the tables are then
+    set back to the snapshot.  The snapshot is the entity and relation tables only, as Keras's get_weights: optimizer
+    slots and the step count keep their values.  fit() calls on_train_begin, which starts each fit afresh, so one
+    instance can serve several fits.  mode='auto' means 'min' for a monitor containing 'loss' or ending in 'mr', else
+    'max' (Keras's own 'auto' would minimise MRR and hits).  stopped_epoch is None when training was not stopped."""
+
+    def __init__(self, monitor="val_mrr", min_delta=0.0, patience=0, mode="auto", restore_best_weights=False, verbose=0):
         self.monitor, self.min_delta, self.patience = monitor, abs(min_delta), patience
+        self.restore_best_weights, self.verbose = restore_best_weights, verbose
         if mode == "auto":
             mode = "min" if ("loss" in monitor or monitor.endswith("mr")) else "max"
         self.sign = 1.0 if mode == "max" else -1.0
-        self.best, self.wait, self.stopped_epoch, self.model = None, 0, None, None
+        self.model = None
+        self.on_train_begin()
+
+    def on_train_begin(self, logs=None):
+        self.best, self.best_epoch, self.wait, self.stopped_epoch, self.best_weights = -self.sign * np.inf, 0, 0, None, None
 
     def on_epoch_end(self, epoch, logs):
         if self.monitor not in logs:
             return
-        v = self.sign * float(logs[self.monitor])
-        if self.best is None or v > self.best + self.min_delta:
-            self.best, self.wait = v, 0
-        else:
-            self.wait += 1
-            if self.wait >= self.patience and self.model is not None:
-                self.stopped_epoch = epoch
-                self.model.stop_training = True
+        current = float(logs[self.monitor])
+        if self.restore_best_weights and self.best_weights is None:
+            self.best_weights = self.model._snapshot_tables()
+        self.wait += 1
+        if self.sign * (current - self.best) - self.min_delta > 0:
+            self.best, self.best_epoch, self.wait = current, epoch, 0
+            if self.restore_best_weights:
+                self.best_weights = self.model._snapshot_tables()
+            return
+        if self.wait >= self.patience and epoch > 0 and self.model is not None:
+            self.stopped_epoch = epoch
+            self.model.stop_training = True
+            if self.restore_best_weights:
+                if self.verbose > 0:
+                    print("Restoring model weights from the end of the best epoch: %d." % (self.best_epoch + 1))
+                self.model._restore_tables(self.best_weights)
 
 
 class ScoringBasedEmbeddingModel:
@@ -189,8 +210,14 @@ class ScoringBasedEmbeddingModel:
             validation_corrupt_side="s,o", validation_freq=10, validation_burn_in=0, validation_filter=False,
             validation_entities_subset=None, partitioning_k=1, focusE=False, focusE_params={}):
         """fit (:544-883).  `shuffle` is accepted and ignored exactly like the reference
-        (batches are the sequential slices of graph_data_loader.py:495-500)."""
+        (batches are the sequential slices of graph_data_loader.py:495-500).  validation_split: carve the validation
+        set out of x with train_test_split_no_unseen(x, test_size=validation_split, seed=self.seed), as the reference
+        does (:719-727).  The filter of the validations (validation_filter) is indexed once per fit, not per validation."""
         self._assert_compile_was_called()
+        if validation_split:
+            assert isinstance(x, np.ndarray), "Validation split supported for numpy arrays only!"
+            x, validation_data = train_test_split_no_unseen(x, test_size=validation_split, seed=self.seed,
+                                                            allow_duplication=False)
         if partitioning_k != 1:
             raise NotImplementedError("bucket partitioning is replaced by HBM-resident tables (DESIGN.md)")
         x = as_triple_array(x)
@@ -231,6 +258,14 @@ class ScoringBasedEmbeddingModel:
         world, rank = self._world(), self._rank()
         if world > 1 and (user_loss or self.use_focusE):
             raise NotImplementedError("user-callable losses / focusE are single-GPU only")
+        val_findex = None  # the FilterIndex of validation_filter, built at the first validation and kept for the others
+        for cb in (callbacks or []):  # Keras's set_model + on_train_begin: a callback instance may serve several fits
+            try:
+                cb.model = self
+            except Exception:
+                pass
+            if hasattr(cb, "on_train_begin"):
+                cb.on_train_begin({})
         for epoch in range(initial_epoch, epochs):
             if self.use_focusE and self._focuse_stop > 0:  # linear decay of the structural weight (:536-543)
                 self._focuse_sw = max(1 - epoch / self._focuse_stop, 0.001)
@@ -259,19 +294,17 @@ class ScoringBasedEmbeddingModel:
                         and (epoch + 1) % validation_freq == 0)
             if validate:
                 self.is_fitted = True
+                if val_findex is None:
+                    val_findex = self._build_filter(validation_filter, lambda: self._index(validation_data))
                 ranks = self.evaluate(validation_data, batch_size=validation_batch_size or batch_size, verbose=False,
                                       use_filter=validation_filter, corrupt_side=validation_corrupt_side,
-                                      entities_subset=validation_entities_subset, dataset_type="valid")
+                                      entities_subset=validation_entities_subset, dataset_type="valid",
+                                      _filter_index=val_findex)
                 logs.update({"val_mrr": mrr_score(ranks), "val_mr": mr_score(ranks),
                              "val_hits@1": hits_at_n_score(ranks, 1), "val_hits@10": hits_at_n_score(ranks, 10),
                              "val_hits@100": hits_at_n_score(ranks, 100)})
             history._log(epoch, logs)
             for cb in (callbacks or []):  # minimal Keras callback protocol: on_epoch_end + model.stop_training
-                if getattr(cb, "model", None) is None:
-                    try:
-                        cb.model = self
-                    except Exception:
-                        pass
                 if hasattr(cb, "on_epoch_end"):
                     cb.on_epoch_end(epoch, logs)
             if verbose:
@@ -455,10 +488,19 @@ class ScoringBasedEmbeddingModel:
         return self.engine.score(self._to_dev(t, np.int32)).cpu().numpy()
 
     # ------------------------------------------------------------------ evaluate
+    def _build_filter(self, use_filter, indexed_x):
+        """FilterIndex of evaluate's use_filter: a dict of datasets (train/valid/test), or True for the evaluated data
+        itself (indexed_x() returns it indexed); None for no filter."""
+        if not (isinstance(use_filter, dict) or use_filter is True):
+            return None
+        parts = [indexed_x()] if use_filter is True else [self._index(v) for v in use_filter.values()]
+        return FilterIndex(np.concatenate(parts), self.max_ent_size)
+
     def evaluate(self, x=None, batch_size=10, verbose=True, use_filter=False, corrupt_side="s,o",
-                 entities_subset=None, ranking_strategy="worst", callbacks=None, dataset_type="test"):
+                 entities_subset=None, ranking_strategy="worst", callbacks=None, dataset_type="test", _filter_index=None):
         """evaluate (:1516-1692) -> int32 ranks [n, 2] for 's,o', [n, 1] otherwise.
-        `batch_size` only lower-bounds the device chunk: results do not depend on it."""
+        `batch_size` only lower-bounds the device chunk: results do not depend on it.  _filter_index: the FilterIndex
+        that use_filter would build (_build_filter), when the caller keeps one across calls (fit's validations)."""
         assert corrupt_side in ["s", "o", "s,o", "s+o"], "Invalid value for corrupt_side"
         assert ranking_strategy in ["best", "middle", "worst"], "Invalid value for ranking_strategy"
         if not self.is_fitted:
@@ -475,11 +517,7 @@ class ScoringBasedEmbeddingModel:
             cand_ids = self._to_dev(sub, np.int32)
             position_of = np.full(self.max_ent_size, -1, np.int64)
             position_of[sub] = np.arange(len(sub))
-        # filters: dict of datasets (train/valid/test), or True = the evaluated data itself
-        findex = None
-        if isinstance(use_filter, dict) or use_filter is True:
-            parts = [t] if use_filter is True else [self._index(v) for v in use_filter.values()]
-            findex = FilterIndex(np.concatenate(parts), self.max_ent_size)
+        findex = _filter_index if _filter_index is not None else self._build_filter(use_filter, lambda: t)
         out = np.zeros((n, len(sides)), np.int32)
         chunk = max(int(batch_size), 4096)
         for start in range(0, n, chunk):
@@ -575,6 +613,17 @@ class ScoringBasedEmbeddingModel:
             else np.asarray(entities, np.int64)
         table = ent if embedding_type == "e" else rel
         return table[torch.as_tensor(idx, dtype=torch.long, device=table.device)].cpu().numpy()
+
+    def _snapshot_tables(self):
+        """Device copies of the live entity and relation tables (what Keras's get_weights returns for the reference:
+        no optimizer slots, no step count).  engine.ent / engine.rel view whichever parameter block is current, also
+        after the deferred steps swapped the engine's two blocks."""
+        return self.engine.ent.clone(), self.engine.rel.clone()
+
+    def _restore_tables(self, snapshot):
+        """Write a _snapshot_tables() copy back into the live tables."""
+        self.engine.ent.copy_(snapshot[0])
+        self.engine.rel.copy_(snapshot[1])
 
     def save_weights(self, filepath):
         """Tables + optimizer slots + indexer in one pickle (the reference's Keras format is TF-specific)."""

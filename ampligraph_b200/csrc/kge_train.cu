@@ -37,9 +37,10 @@ namespace kge {
 // PAIRS (a, b) so two independent dependency chains are in flight.
 //   prep(s,p,o)                      per-positive state; returns this lane's partial of f(s,p,o)
 //   partial2<SIDE>(ra,rb,pa,pb)      partials of f for two corruptions with replaced rows ra, rb
-//   grad2<SIDE,Sink>(...)            emit g * df/dr for both rows, accumulate what the kept rows need
-//   finish<Sink>(...)                emit the total gradient rows of s, p, o
-// Unscaled f; HolE's 2/k factor is folded into g by the caller.
+//   grad2<SIDE>(...)                 RED g * df/dr for both rows, accumulate what the kept rows need
+//   finish(...)                      RED the total gradient rows of s, p, o
+// Unscaled f; HolE's 2/k factor is folded into g by the caller.  The formulas of DistMult, ComplEx / HolE and RotatE are
+// the shared ones of kge_train_common.cuh (the fast paths use the same); TransE exists only here.
 // --------------------------------------------------------------------------
 template <int MODEL, int NIT>
 struct Scorer;
@@ -62,8 +63,8 @@ struct Scorer<KGE_DISTMULT, NIT> {
             int c = lane + cs * it;
             float4 vs = f4zero(), vp = f4zero(), vo = f4zero();
             if (c < nch) { vs = f4ld(s + 4 * c); vp = f4ld(p + 4 * c); vo = f4ld(o + 4 * c); }
-            A[it] = vp * vo;
-            C[it] = vs * vp;
+            A[it] = query_subj<1, 0>(vp, vp, vo, vo);
+            C[it] = query_obj<1, 0>(vs, vs, vp, vp);
             Ws[it] = f4zero();
             Wo[it] = f4zero();
             acc = f4fma(vs, A[it], acc);
@@ -101,7 +102,7 @@ struct Scorer<KGE_DISTMULT, NIT> {
         }
         p0 = f4hsum(a); p1 = f4hsum(b); p2 = f4hsum(c4); p3 = f4hsum(d);
     }
-    template <int SIDE, class Sink>
+    template <int SIDE>
     __device__ __forceinline__ void grad2(float *ra, float *rb, float *ga_row, float *gb_row, float ga, float gb,
                                           bool has_b)
     {
@@ -114,11 +115,10 @@ struct Scorer<KGE_DISTMULT, NIT> {
             float4 &W = SIDE ? Wo[it] : Ws[it];
             W = f4fma(ga, va, W);
             W = f4fma(gb, vb, W);
-            if (live) Sink::put(ra, ga_row, 4 * c, 4 * c, ga * q);
-            if (live && has_b) Sink::put(rb, gb_row, 4 * c, 4 * c, gb * q);
+            if (live) red_add_v4(ga_row, 4 * c, ga * q);
+            if (live && has_b) red_add_v4(gb_row, 4 * c, gb * q);
         }
     }
-    template <class Sink>
     __device__ __forceinline__ void finish(float *s, float *p, float *o, float *gs, float *gp, float *go, float gP,
                                            float)
     {
@@ -129,9 +129,9 @@ struct Scorer<KGE_DISTMULT, NIT> {
                 float4 vs = f4ld(s + 4 * c), vp = f4ld(p + 4 * c), vo = f4ld(o + 4 * c);
                 float4 U = f4fma(gP, vs, Ws[it]);  // everything that sat in the subject slot
                 float4 X = f4fma(gP, vo, Wo[it]);  // everything that sat in the object slot
-                Sink::put(s, gs, 4 * c, 4 * c, vp * X);
-                Sink::put(o, go, 4 * c, 4 * c, U * vp);
-                Sink::put(p, gp, 4 * c, 4 * c, f4fma(U, vo, vs * Wo[it]));
+                red_add_v4(gs, 4 * c, query_subj<1, 0>(vp, vp, X, X));  // d/ds f(s,p,X)
+                red_add_v4(go, 4 * c, query_obj<1, 0>(U, U, vp, vp));   // d/do f(U,p,o)
+                red_add_v4(gp, 4 * c, trilinear_grad_p<1, 0>(vs, vs, vo, vo, U, U, Wo[it], Wo[it]));
             }
         }
     }
@@ -159,10 +159,8 @@ struct ComplexScorer {
                 pr = f4ld(p + 4 * c); pi = f4ld(p + hs + 4 * c);
                 orr = f4ld(o + 4 * c); oi = f4ld(o + hs + 4 * c);
             }
-            A[it] = f4fma(pi, oi, pr * orr);
-            Bv[it] = pr * oi - pi * orr;
-            C[it] = sr * pr - si * pi;
-            D[it] = f4fma(sr, pi, si * pr);
+            A[it] = query_subj<2, 0>(pr, pi, orr, oi); Bv[it] = query_subj<2, 1>(pr, pi, orr, oi);
+            C[it] = query_obj<2, 0>(sr, si, pr, pi); D[it] = query_obj<2, 1>(sr, si, pr, pi);
             Wsr[it] = Wsi[it] = Wor[it] = Woi[it] = f4zero();
             acc = f4fma(sr, A[it], acc);
             acc = f4fma(si, Bv[it], acc);
@@ -206,7 +204,7 @@ struct ComplexScorer {
         }
         p0 = f4hsum(a); p1 = f4hsum(b); p2 = f4hsum(c4); p3 = f4hsum(d);
     }
-    template <int SIDE, class Sink>
+    template <int SIDE>
     __device__ __forceinline__ void grad2(float *ra, float *rb, float *ga_row, float *gb_row, float ga, float gb,
                                           bool has_b)
     {
@@ -222,16 +220,15 @@ struct ComplexScorer {
             Wr = f4fma(ga, ar, Wr); Wi = f4fma(ga, ai, Wi);
             Wr = f4fma(gb, br, Wr); Wi = f4fma(gb, bi, Wi);
             if (live) {
-                Sink::put(ra, ga_row, 4 * c, 4 * c, ga * qr);
-                Sink::put(ra, ga_row, hs + 4 * c, kp + 4 * c, ga * qi);
+                red_add_v4(ga_row, 4 * c, ga * qr);
+                red_add_v4(ga_row, kp + 4 * c, ga * qi);
             }
             if (live && has_b) {
-                Sink::put(rb, gb_row, 4 * c, 4 * c, gb * qr);
-                Sink::put(rb, gb_row, hs + 4 * c, kp + 4 * c, gb * qi);
+                red_add_v4(gb_row, 4 * c, gb * qr);
+                red_add_v4(gb_row, kp + 4 * c, gb * qi);
             }
         }
     }
-    template <class Sink>
     __device__ __forceinline__ void finish(float *s, float *p, float *o, float *gs, float *gp, float *go, float gP,
                                            float)
     {
@@ -244,15 +241,12 @@ struct ComplexScorer {
                 float4 orr = f4ld(o + 4 * c), oi = f4ld(o + hs + 4 * c);
                 float4 Ur = f4fma(gP, sr, Wsr[it]), Ui = f4fma(gP, si, Wsi[it]);    // subject-slot mass
                 float4 Xr = f4fma(gP, orr, Wor[it]), Xi = f4fma(gP, oi, Woi[it]);   // object-slot mass
-                // d/ds f(s,p,X)
-                Sink::put(s, gs, 4 * c, 4 * c, f4fma(pi, Xi, pr * Xr));
-                Sink::put(s, gs, hs + 4 * c, kp + 4 * c, pr * Xi - pi * Xr);
-                // d/do f(U,p,o)
-                Sink::put(o, go, 4 * c, 4 * c, Ur * pr - Ui * pi);
-                Sink::put(o, go, hs + 4 * c, kp + 4 * c, f4fma(Ur, pi, Ui * pr));
-                // d/dp [f(U,p,o) + f(s,p,Wo)]
-                Sink::put(p, gp, 4 * c, 4 * c, f4fma(Ur, orr, Ui * oi) + f4fma(sr, Wor[it], si * Woi[it]));
-                Sink::put(p, gp, hs + 4 * c, kp + 4 * c, (Ur * oi - Ui * orr) + (sr * Woi[it] - si * Wor[it]));
+                red_add_v4(gs, 4 * c, query_subj<2, 0>(pr, pi, Xr, Xi));  // d/ds f(s,p,X)
+                red_add_v4(gs, kp + 4 * c, query_subj<2, 1>(pr, pi, Xr, Xi));
+                red_add_v4(go, 4 * c, query_obj<2, 0>(Ur, Ui, pr, pi));   // d/do f(U,p,o)
+                red_add_v4(go, kp + 4 * c, query_obj<2, 1>(Ur, Ui, pr, pi));
+                red_add_v4(gp, 4 * c, trilinear_grad_p<2, 0>(sr, si, orr, oi, Ur, Ui, Wor[it], Woi[it]));
+                red_add_v4(gp, kp + 4 * c, trilinear_grad_p<2, 1>(sr, si, orr, oi, Ur, Ui, Wor[it], Woi[it]));
             }
         }
     }
@@ -298,7 +292,7 @@ struct Scorer<KGE_TRANSE, NIT> {
         pa = a;
         pb = b;
     }
-    template <int SIDE, class Sink>
+    template <int SIDE>
     __device__ __forceinline__ void grad2(float *ra, float *rb, float *ga_row, float *gb_row, float ga, float gb,
                                           bool has_b)
     {
@@ -312,12 +306,11 @@ struct Scorer<KGE_TRANSE, NIT> {
                 float4 sb = gb * f4sgn(SIDE ? (Qo[it] - vb) : (vb + Qs[it]));
                 float4 &V = SIDE ? Vo[it] : Vs[it];
                 V = V + sa + sb;
-                Sink::put(ra, ga_row, 4 * c, 4 * c, SIDE ? sa : f4neg(sa));
-                if (has_b) Sink::put(rb, gb_row, 4 * c, 4 * c, SIDE ? sb : f4neg(sb));
+                red_add_v4(ga_row, 4 * c, SIDE ? sa : f4neg(sa));
+                if (has_b) red_add_v4(gb_row, 4 * c, SIDE ? sb : f4neg(sb));
             }
         }
     }
-    template <class Sink>
     __device__ __forceinline__ void finish(float *s, float *p, float *o, float *gs, float *gp, float *go, float gP,
                                            float)
     {
@@ -327,27 +320,18 @@ struct Scorer<KGE_TRANSE, NIT> {
             if (c < nch) {
                 float4 vo = f4ld(o + 4 * c);
                 float4 Vp = gP * f4sgn(Qo[it] - vo);
-                Sink::put(s, gs, 4 * c, 4 * c, f4neg(Vp + Vo[it]));
-                Sink::put(p, gp, 4 * c, 4 * c, f4neg(Vp + Vs[it] + Vo[it]));
-                Sink::put(o, go, 4 * c, 4 * c, Vp + Vs[it]);
+                red_add_v4(gs, 4 * c, f4neg(Vp + Vo[it]));
+                red_add_v4(gp, 4 * c, f4neg(Vp + Vs[it] + Vo[it]));
+                red_add_v4(go, 4 * c, Vp + Vs[it]);
             }
         }
     }
 };
 
-// ---- RotatE (RotatE.py:76-104) --------------------------------------------
-// The relation row handed to this kernel is the per-step rotation table row
-// [cos(phi) | sin(phi)], phi = theta/div (kge_rotation_table_kernel).
-// f = -sum_d |R(phi) s - o|.  With (a,b) = g * residual/|residual|:
-//   df/do = (a,b); df/ds = -R(-phi)(a,b); df/dphi = a*y_im - b*y_re, y = R(phi) s.
-// The reference's gradient is NaN at an exactly-zero residual; here it is 0.
-//
-// The kernel is FP32-issue bound on this model, so the scorer is written to a per-element instruction budget:
-// every float4 operation is four fp32 instructions (negations and subtractions are operand modifiers of FADD /
-// FFMA, never separate instructions), a residual is two dependent fmas per component, the modulus is one MUFU.SQRT, the unit vector one MUFU.RSQ
-// on max(x, tiny) (an exactly-zero residual gives 0 * finite = 0), and lanes past the end of the window are
-// masked arithmetically (they read the window's last chunk; only their stores are predicated) so the row
-// loops carry no divergence bookkeeping.
+// ---- RotatE (kge_train_common.cuh: rot_*) ----------------------------------
+// The relation row handed to this kernel is the per-step rotation table row [cos(phi) | sin(phi)], phi = theta/div
+// (kge_rotation_table_kernel).  Lanes past the end of the window are masked arithmetically (they read the window's
+// last chunk; only their stores are predicated) so the row loops carry no divergence bookkeeping.
 template <int NIT>
 struct Scorer<KGE_ROTATE, NIT> {
     static constexpr bool kQuad = false;
@@ -356,21 +340,6 @@ struct Scorer<KGE_ROTATE, NIT> {
     float nlive[NIT];  // -1 for a lane that owns a chunk of this window, 0 past its end
     int lane, nch, cs = 32, kp, hs;  // cs: chunk stride = lanes on one positive; kp: half stride in HBM rows, hs: half stride of the staged row window
     __device__ __forceinline__ int chunk(int it) const { return min(lane + cs * it, nch - 1); }
-    // sum of the four moduli of (re, im)
-    static __device__ __forceinline__ float modsum(float4 re, float4 im)
-    {
-        const float4 x = f4fma(im, im, re * re);
-        return (sqrt_approx(x.x) + sqrt_approx(x.y)) + (sqrt_approx(x.z) + sqrt_approx(x.w));
-    }
-    // (a, b) = g * (re, im) / |(re, im)|, zero where the residual is exactly zero
-    static __device__ __forceinline__ void unit(float4 re, float4 im, float g, float4 &a, float4 &b)
-    {
-        const float4 x = f4fma(im, im, re * re);
-        const float4 inv = g * make_float4(rsqrt_approx(fmaxf(x.x, 1e-30f)), rsqrt_approx(fmaxf(x.y, 1e-30f)),
-                                           rsqrt_approx(fmaxf(x.z, 1e-30f)), rsqrt_approx(fmaxf(x.w, 1e-30f)));
-        a = re * inv;
-        b = im * inv;
-    }
     __device__ __forceinline__ float prep(const float *s, const float *p, const float *o, int ln)
     {
         lane = ln;
@@ -387,18 +356,12 @@ struct Scorer<KGE_ROTATE, NIT> {
                 Or_[it] = f4ld(o + 4 * c); Oi[it] = f4ld(o + hs + 4 * c);
                 nlive[it] = -1.f;
             }
-            Yr[it] = f4fma(f4neg(si), Sn[it], sr * C[it]);  // sr c - si s
-            Yi[it] = f4fma(sr, Sn[it], si * C[it]);         // sr s + si c
+            Yr[it] = rot_rotate<0>(sr, si, C[it], Sn[it]);
+            Yi[it] = rot_rotate<1>(sr, si, C[it], Sn[it]);
             Zor[it] = Zoi[it] = Zsr[it] = Zsi[it] = Aphi[it] = f4zero();
-            acc = fmaf(modsum(Yr[it] - Or_[it], Yi[it] - Oi[it]), nlive[it], acc);
+            acc = fmaf(rot_modsum(Yr[it] - Or_[it], Yi[it] - Oi[it]), nlive[it], acc);
         }
         return acc;
-    }
-    // R(phi) r - o, as two dependent packed fmas per component
-    __device__ __forceinline__ void residual_subj(int it, float4 rr, float4 ri, float4 &re, float4 &im) const
-    {
-        re = f4fma(f4neg(ri), Sn[it], f4fma(rr, C[it], f4neg(Or_[it])));
-        im = f4fma(ri, C[it], f4fma(rr, Sn[it], f4neg(Oi[it])));
     }
     template <int SIDE>
     __device__ __forceinline__ void partial2(const float *ra, const float *rb, float &pa, float &pb) const
@@ -410,40 +373,41 @@ struct Scorer<KGE_ROTATE, NIT> {
             const float4 ar = f4ld(ra + 4 * c), ai = f4ld(ra + hs + 4 * c);
             const float4 br = f4ld(rb + 4 * c), bi = f4ld(rb + hs + 4 * c);
             if (SIDE) {  // y - r
-                a = fmaf(modsum(Yr[it] - ar, Yi[it] - ai), nlive[it], a);
-                b = fmaf(modsum(Yr[it] - br, Yi[it] - bi), nlive[it], b);
+                a = fmaf(rot_modsum(Yr[it] - ar, Yi[it] - ai), nlive[it], a);
+                b = fmaf(rot_modsum(Yr[it] - br, Yi[it] - bi), nlive[it], b);
             } else {
-                float4 e0, e1, e2, e3;
-                residual_subj(it, ar, ai, e0, e1);
-                residual_subj(it, br, bi, e2, e3);
-                a = fmaf(modsum(e0, e1), nlive[it], a);
-                b = fmaf(modsum(e2, e3), nlive[it], b);
+                const float4 e0 = rot_residual_subj<0>(ar, ai, C[it], Sn[it], Or_[it], Oi[it]);
+                const float4 e1 = rot_residual_subj<1>(ar, ai, C[it], Sn[it], Or_[it], Oi[it]);
+                const float4 e2 = rot_residual_subj<0>(br, bi, C[it], Sn[it], Or_[it], Oi[it]);
+                const float4 e3 = rot_residual_subj<1>(br, bi, C[it], Sn[it], Or_[it], Oi[it]);
+                a = fmaf(rot_modsum(e0, e1), nlive[it], a);
+                b = fmaf(rot_modsum(e2, e3), nlive[it], b);
             }
         }
         pa = a;
         pb = b;
     }
-    template <int SIDE, class Sink>
+    template <int SIDE>
     __device__ __forceinline__ void grad1(float *r, float *grow, float g, int it, int c, bool emit)
     {
         const float4 rr = f4ld(r + 4 * c), ri = f4ld(r + hs + 4 * c);
         float4 a, b;
         if (SIDE) {  // residual = y(s) - r ; df/dr = +(a,b)
-            unit(Yr[it] - rr, Yi[it] - ri, g, a, b);
+            rot_unit(Yr[it] - rr, Yi[it] - ri, g, a, b);
             Zor[it] = Zor[it] + a; Zoi[it] = Zoi[it] + b;
-            if (emit) { Sink::put(r, grow, 4 * c, 4 * c, a); Sink::put(r, grow, hs + 4 * c, kp + 4 * c, b); }
+            if (emit) { red_add_v4(grow, 4 * c, a); red_add_v4(grow, kp + 4 * c, b); }
         } else {  // residual = R(phi) r - o ; df/dr = -R(-phi)(a,b)
-            const float4 yr = f4fma(f4neg(ri), Sn[it], rr * C[it]), yi = f4fma(rr, Sn[it], ri * C[it]);  // R(phi) r
-            unit(yr - Or_[it], yi - Oi[it], g, a, b);
+            const float4 yr = rot_rotate<0>(rr, ri, C[it], Sn[it]), yi = rot_rotate<1>(rr, ri, C[it], Sn[it]);  // R(phi) r
+            rot_unit(yr - Or_[it], yi - Oi[it], g, a, b);
             Zsr[it] = Zsr[it] + a; Zsi[it] = Zsi[it] + b;
-            Aphi[it] = f4fma(f4neg(b), yr, f4fma(a, yi, Aphi[it]));  // a*y_im - b*y_re
+            Aphi[it] = rot_dphi(a, b, yr, yi, Aphi[it]);
             if (emit) {
-                Sink::put(r, grow, 4 * c, 4 * c, f4fma(f4neg(b), Sn[it], f4neg(a) * C[it]));  // -(a c + b s)
-                Sink::put(r, grow, hs + 4 * c, kp + 4 * c, f4fma(f4neg(b), C[it], a * Sn[it]));  // a s - b c
+                red_add_v4(grow, 4 * c, rot_back<0>(a, b, C[it], Sn[it]));
+                red_add_v4(grow, kp + 4 * c, rot_back<1>(a, b, C[it], Sn[it]));
             }
         }
     }
-    template <int SIDE, class Sink>
+    template <int SIDE>
     __device__ __forceinline__ void grad2(float *ra, float *rb, float *ga_row, float *gb_row, float ga, float gb,
                                           bool has_b)
     {
@@ -451,13 +415,12 @@ struct Scorer<KGE_ROTATE, NIT> {
         for (int it = 0; it < NIT; ++it) {
             const int c = chunk(it);
             const bool live = lane + cs * it < nch;  // dead lanes run the arithmetic on the last chunk; their accumulators are never read
-            grad1<SIDE, Sink>(ra, ga_row, ga, it, c, live);
-            grad1<SIDE, Sink>(rb, gb_row, gb, it, c, live && has_b);  // gb == 0 when !has_b: contributes nothing
+            grad1<SIDE>(ra, ga_row, ga, it, c, live);
+            grad1<SIDE>(rb, gb_row, gb, it, c, live && has_b);  // gb == 0 when !has_b: contributes nothing
         }
     }
     // p row receives d/dtheta = (1/div) d/dphi in its first half, zeros in the second
     // (the second half of a RotatE relation row is allocated but unused, RotatE.py:76).
-    template <class Sink>
     __device__ __forceinline__ void finish(float *s, float *p, float *o, float *gs, float *gp, float *go, float gP,
                                            float inv_div)
     {
@@ -466,13 +429,13 @@ struct Scorer<KGE_ROTATE, NIT> {
             int c = lane + cs * it;
             if (c < nch) {
                 float4 a, b;
-                unit(Yr[it] - Or_[it], Yi[it] - Oi[it], gP, a, b);
+                rot_unit(Yr[it] - Or_[it], Yi[it] - Oi[it], gP, a, b);
                 const float4 Zr = a + Zor[it], Zi = b + Zoi[it];  // everything with y = R(phi) s
-                Sink::put(s, gs, 4 * c, 4 * c, f4fma(f4neg(Zi), Sn[it], f4neg(Zr) * C[it]));   // -(Zr c + Zi s)
-                Sink::put(s, gs, hs + 4 * c, kp + 4 * c, f4fma(f4neg(Zi), C[it], Zr * Sn[it]));  // Zr s - Zi c
-                Sink::put(o, go, 4 * c, 4 * c, a + Zsr[it]);
-                Sink::put(o, go, hs + 4 * c, kp + 4 * c, b + Zsi[it]);
-                Sink::put(p, gp, 4 * c, 4 * c, inv_div * f4fma(f4neg(Zi), Yr[it], f4fma(Zr, Yi[it], Aphi[it])));
+                red_add_v4(gs, 4 * c, rot_back<0>(Zr, Zi, C[it], Sn[it]));
+                red_add_v4(gs, kp + 4 * c, rot_back<1>(Zr, Zi, C[it], Sn[it]));
+                red_add_v4(go, 4 * c, a + Zsr[it]);
+                red_add_v4(go, kp + 4 * c, b + Zsi[it]);
+                red_add_v4(gp, 4 * c, inv_div * rot_dphi(Zr, Zi, Yr[it], Yi[it], Aphi[it]));
             }
         }
     }
@@ -537,7 +500,6 @@ __device__ __forceinline__ float *gent_row(const TrainParams &p, int id)
 template <int MODEL, int NIT, bool RESIDENT>
 __global__ void __launch_bounds__(KGE_TRAIN_THREADS(MODEL, NIT)) kge_train_kernel(const TrainParams p)
 {
-    using Sink = SinkRed;
     constexpr int HALVES = (MODEL == KGE_TRANSE || MODEL == KGE_DISTMULT) ? 1 : 2;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -588,9 +550,7 @@ __global__ void __launch_bounds__(KGE_TRAIN_THREADS(MODEL, NIT)) kge_train_kerne
             const int j = base + lane;
             int keep = 1, repl = 0;
             if (j < eta) {
-                const unsigned long long r = (unsigned long long)j * (unsigned long long)p.B + (unsigned long long)i;
-                if (p.neg_ent) { repl = p.neg_ent[r]; keep = p.neg_keep[r] ? 1 : 0; }
-                else draw_corruption(p.seed, p.step, r, p.n_ent, &keep, &repl);
+                corruption_of(p, (unsigned long long)j * (unsigned long long)p.B + (unsigned long long)i, keep, repl);
                 nside[j] = keep;  // keep_subj = 1 -> object replaced -> side 1
                 sc[j] = __int_as_float(repl);
                 if (p.stamp_ent && p.mode != KGE_STEP_FORWARD_ONLY) stamp_ent_row(p, repl);  // lazy optimizer: row touched
@@ -800,22 +760,22 @@ __global__ void __launch_bounds__(KGE_TRAIN_THREADS(MODEL, NIT)) kge_train_kerne
                     const int a = t - j0;
                     const bool has_b = t + 1 < e0;
                     const int b = has_b ? a + 1 : a;
-                    S.template grad2<0, Sink>(nrows + (size_t)a * lw, nrows + (size_t)b * lw, gent_row(p, nid[j0 + a]) + gofs,
-                                              gent_row(p, nid[j0 + b]) + gofs, scale * sc[j0 + a],
-                                              has_b ? scale * sc[j0 + b] : 0.f, has_b);
+                    S.template grad2<0>(nrows + (size_t)a * lw, nrows + (size_t)b * lw, gent_row(p, nid[j0 + a]) + gofs,
+                                        gent_row(p, nid[j0 + b]) + gofs, scale * sc[j0 + a],
+                                        has_b ? scale * sc[j0 + b] : 0.f, has_b);
                 }
                 for (int t = b1; t < j0 + gsz; t += 2) {
                     const int a = t - j0;
                     const bool has_b = t + 1 < j0 + gsz;
                     const int b = has_b ? a + 1 : a;
-                    S.template grad2<1, Sink>(nrows + (size_t)a * lw, nrows + (size_t)b * lw, gent_row(p, nid[j0 + a]) + gofs,
-                                              gent_row(p, nid[j0 + b]) + gofs, scale * sc[j0 + a],
-                                              has_b ? scale * sc[j0 + b] : 0.f, has_b);
+                    S.template grad2<1>(nrows + (size_t)a * lw, nrows + (size_t)b * lw, gent_row(p, nid[j0 + a]) + gofs,
+                                        gent_row(p, nid[j0 + b]) + gofs, scale * sc[j0 + a],
+                                        has_b ? scale * sc[j0 + b] : 0.f, has_b);
                 }
                 __syncwarp();
                 if (!dbuf && g > 0) issue(0, cb, false, j0 - G, G, use_stash);  // single buffer: the next (lower) group over this one
             }
-            S.template finish<Sink>(srow, prow, orow, gs_row + gofs, gp_row + gofs, go_row + gofs, scale * dP, p.inv_div);
+            S.finish(srow, prow, orow, gs_row + gofs, gp_row + gofs, go_row + gofs, scale * dP, p.inv_div);
         }
         __syncwarp();
     }

@@ -32,8 +32,7 @@ __global__ void kge_bucket_count_kernel(const TrainParams p)
     const long long n = (long long)p.eta * p.B;
     for (long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (long long)gridDim.x * blockDim.x) {
         int keep, repl;
-        if (p.neg_ent) repl = p.neg_ent[r];
-        else draw_corruption(p.seed, p.step, (unsigned long long)r, p.n_ent, &keep, &repl);
+        corruption_of(p, (unsigned long long)r, keep, repl);
         p.bk.pos[r] = atomicAdd(p.bk.cnt + repl, 1);
     }
 }

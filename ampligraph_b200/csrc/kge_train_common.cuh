@@ -1,7 +1,8 @@
 // kge_train_common.cuh -- device helpers shared by the training kernels (kge_train.cu: the general kernel;
-// kge_train_res.cu: the resident trilinear fast path): fp32-pair float4 arithmetic, the gradient sink, warp
-// reductions, and the per-positive loss + dL/dscore of the five reference losses; on the host, the launch they share and the
-// trilinear row-shape dispatch.
+// kge_train_res.cu / kge_train_rot.cu: the trilinear and RotatE fast paths; kge_train_bucket.cu: the replaced-row bucket
+// sum): fp32-pair float4 arithmetic, the gradient scatter, warp reductions, the per-model score and gradient arithmetic,
+// the corruption draw, and the per-positive loss + dL/dscore of the five reference losses; on the host, the launch they
+// share and the trilinear row-shape dispatch.
 #pragma once
 #include <math.h>
 
@@ -78,8 +79,10 @@ __device__ __forceinline__ float4 f4sgn(float4 a) { return make_float4(sgnf(a.x)
 __device__ __forceinline__ float f4abssum(float4 a) { return (fabsf(a.x) + fabsf(a.y)) + (fabsf(a.z) + fabsf(a.w)); }
 
 // --------------------------------------------------------------------------
-// gradient sink: red.global.add.v4.f32 straight from registers into the gradient table
-// (the scorers keep a Sink template parameter so that a profiling build can swap it).
+// gradient scatter: red.global.add.v4.f32 straight from registers into the gradient table.
+// -DKGE_PROFILE_NOSCATTER builds a profiling variant that drops the scatter (how much of the kernel the atomics cost).
+// The product never tests a run-time flag here: a branch around every RED was measured to cost several percent before
+// the H100 port (not re-measured).
 // --------------------------------------------------------------------------
 __device__ __forceinline__ void red_add_v4(float *g, float4 v)
 {
@@ -89,12 +92,9 @@ __device__ __forceinline__ void red_add_v4(float *g, float4 v)
     asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(g), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
                  : "memory");
 }
-// -DKGE_PROFILE_NOSCATTER builds a profiling variant that drops the gradient scatter (how much of the kernel the atomics
-// cost).  The product never tests a run-time flag here: a branch around every RED was measured to cost several percent
-// before the H100 port (not re-measured).
-struct SinkRed {
-    static __device__ __forceinline__ void put(float *, float *grow, int, int goff, float4 v) { red_add_v4(grow + goff, v); }
-};
+// The general kernel's form: a gradient row plus a float offset, added after v has been formed (writing row + off at the
+// call site, before v, gives ptxas a different instruction order and changes the schedule of the general kernel).
+__device__ __forceinline__ void red_add_v4(float *row, int off, float4 v) { red_add_v4(row + off, v); }
 
 // RotatE's modulus and unit vector use the MUFU approximations (sqrt.approx: 2^-23 relative, rsqrt.approx: 2 ulp), far
 // inside the 1e-4 training tolerance; the RANKING kernels keep the correctly rounded sqrt because their scores must be
@@ -112,8 +112,6 @@ __device__ __forceinline__ float rsqrt_approx(float x)
     asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
     return r;
 }
-
-
 
 __device__ __forceinline__ void warp_sum2(float &a, float &b)
 {
@@ -215,31 +213,109 @@ __device__ __forceinline__ void bulk_load_s(uint32_t smem_dst, const void *gmem_
 #define KGE_KEEPF(x) asm volatile("" : "+f"(x))
 __device__ __forceinline__ void red4(char *row, uint32_t byte_off, float4 v) { red_add_v4(reinterpret_cast<float *>(row + byte_off), v); }
 
-// Query vectors of the trilinear models (DistMult: HALVES = 1; ComplEx / HolE: HALVES = 2, re / im halves), one float4
-// chunk: the score of a corruption is <row, Q>, and its replaced row's gradient is g * Q.  The fused kernel
-// (kge_train_res.cu) and the owner-computes gradient sum (kge_train_bucket.cu) both form Q here, so every g * Q term is
-// bit-identical between them.  Subject replaced: Q0(p, o); object replaced: Q1(s, p).
+// --------------------------------------------------------------------------
+// Per-model arithmetic of the training kernels, one float4 chunk at a time.  The general kernel (kge_train.cu), the fast
+// paths (kge_train_res.cu, kge_train_rot.cu) and the owner-computes gradient sum (kge_train_bucket.cu) all compute a
+// model's scores and gradients with these functions, so their scores agree bit for bit and every g * Q term the bucket
+// sum forms is the one the fused kernel would scatter.  A two-half (re / im) result is returned one half (H = 0: re,
+// 1: im) at a time, so each half can be scattered as soon as it is formed (results returned through reference
+// arguments were measured to change the fast paths' instruction schedule).
+// --------------------------------------------------------------------------
+
+// Query vectors of the trilinear models (DistMult: HALVES = 1; ComplEx / HolE: HALVES = 2): the score of a corruption
+// is <row, Q>, and its replaced row's gradient is g * Q.  Subject replaced: Q0(p, o); object replaced: Q1(s, p).
+template <int HALVES, int H>
+__device__ __forceinline__ float4 query_subj(float4 pr, float4 pi, float4 orr, float4 oi)
+{
+    if constexpr (HALVES == 1) return pr * orr;
+    else if constexpr (H == 0) return f4fma(pi, oi, pr * orr);
+    else return pr * oi - pi * orr;
+}
+template <int HALVES, int H>
+__device__ __forceinline__ float4 query_obj(float4 sr, float4 si, float4 pr, float4 pi)
+{
+    if constexpr (HALVES == 1) return sr * pr;
+    else if constexpr (H == 0) return sr * pr - si * pi;
+    else return f4fma(sr, pi, si * pr);
+}
+// both halves at once, for the bucket sum (with HALVES = 1, qi is not written)
 template <int HALVES>
 __device__ __forceinline__ void query_subj(float4 pr, float4 pi, float4 orr, float4 oi, float4 &qr, float4 &qi)
 {
-    if constexpr (HALVES == 2) {
-        qr = f4fma(pi, oi, pr * orr);
-        qi = pr * oi - pi * orr;
-    } else {
-        qr = pr * orr;
-    }
+    qr = query_subj<HALVES, 0>(pr, pi, orr, oi);
+    if constexpr (HALVES == 2) qi = query_subj<HALVES, 1>(pr, pi, orr, oi);
 }
 template <int HALVES>
 __device__ __forceinline__ void query_obj(float4 sr, float4 si, float4 pr, float4 pi, float4 &qr, float4 &qi)
 {
-    if constexpr (HALVES == 2) {
-        qr = sr * pr - si * pi;
-        qi = f4fma(sr, pi, si * pr);
-    } else {
-        qr = sr * pr;
-    }
+    qr = query_obj<HALVES, 0>(sr, si, pr, pi);
+    if constexpr (HALVES == 2) qi = query_obj<HALVES, 1>(sr, si, pr, pi);
+}
+// Gradient rows of a trilinear positive's kept rows.  U is everything that sat in the subject slot (gP s + the
+// subject-replaced corruptions' sum_j g_j r_j), X everything in the object slot, W1 the object-replaced share of X.
+// Entity rows: d/ds f(s,p,X) = Q0(p, X), d/do f(U,p,o) = Q1(U, p).  Relation row: d/dp [f(U,p,o) + f(s,p,W1)].
+template <int HALVES, int H>
+__device__ __forceinline__ float4 trilinear_grad_p(float4 sr, float4 si, float4 orr, float4 oi, float4 Ur, float4 Ui,
+                                                   float4 W1r, float4 W1i)
+{
+    if constexpr (HALVES == 1) return f4fma(Ur, orr, sr * W1r);
+    else if constexpr (H == 0) return f4fma(Ur, orr, Ui * oi) + f4fma(sr, W1r, si * W1i);
+    else return (Ur * oi - Ui * orr) + (sr * W1i - si * W1r);
 }
 
+// RotatE (RotatE.py:76-104), relation row = rotation table row [cos(phi) | sin(phi)] = (c, sn), f = -sum_d |R(phi) s - o|.
+// With (a, b) = g * residual / |residual|: df/do = (a, b); df/ds = -R(-phi)(a, b); df/dphi = a y_im - b y_re, y = R(phi) s.
+// FP32-issue bound: every float4 operation is four fp32 instructions (negations are FADD / FFMA operand modifiers).
+// sum of the four moduli of (re, im): x = re^2 + im^2, one MUFU.SQRT each
+__device__ __forceinline__ float rot_modsum(float4 re, float4 im)
+{
+    const float4 x = f4fma(im, im, re * re);
+    return (sqrt_approx(x.x) + sqrt_approx(x.y)) + (sqrt_approx(x.z) + sqrt_approx(x.w));
+}
+// (a, b) = g * (re, im) / |(re, im)|: one MUFU.RSQ on max(x, tiny), so an exactly-zero residual gives 0 * finite = 0
+// (the reference's gradient is NaN there)
+__device__ __forceinline__ void rot_unit(float4 re, float4 im, float g, float4 &a, float4 &b)
+{
+    const float4 x = f4fma(im, im, re * re);
+    const float4 inv = g * make_float4(rsqrt_approx(fmaxf(x.x, 1e-30f)), rsqrt_approx(fmaxf(x.y, 1e-30f)),
+                                       rsqrt_approx(fmaxf(x.z, 1e-30f)), rsqrt_approx(fmaxf(x.w, 1e-30f)));
+    a = re * inv;
+    b = im * inv;
+}
+// R(phi)(rr, ri) = (rr c - ri sn, rr sn + ri c)
+template <int H>
+__device__ __forceinline__ float4 rot_rotate(float4 rr, float4 ri, float4 c, float4 sn)
+{
+    if constexpr (H == 0) return f4fma(f4neg(ri), sn, rr * c);
+    else return f4fma(rr, sn, ri * c);
+}
+// the residual of a replaced subject, R(phi) r - o, as two dependent fmas per component
+template <int H>
+__device__ __forceinline__ float4 rot_residual_subj(float4 rr, float4 ri, float4 c, float4 sn, float4 orr, float4 oi)
+{
+    if constexpr (H == 0) return f4fma(f4neg(ri), sn, f4fma(rr, c, f4neg(orr)));
+    else return f4fma(ri, c, f4fma(rr, sn, f4neg(oi)));
+}
+// -R(-phi)(a, b) = (-(a c + b sn), a sn - b c): the subject-side gradient of a residual whose unit vector is (a, b)
+template <int H>
+__device__ __forceinline__ float4 rot_back(float4 a, float4 b, float4 c, float4 sn)
+{
+    if constexpr (H == 0) return f4fma(f4neg(b), sn, f4neg(a) * c);
+    else return f4fma(f4neg(b), c, a * sn);
+}
+// acc + a y_im - b y_re: the dphi accumulation
+__device__ __forceinline__ float4 rot_dphi(float4 a, float4 b, float4 yr, float4 yi, float4 acc)
+{
+    return f4fma(f4neg(b), yr, f4fma(a, yi, acc));
+}
+
+// Corruption r = j*B + i of the step (the reference's tile order): the injected negatives when the caller supplied
+// them, else the Philox draw.  keep = 1: the subject is kept and the object replaced by repl.
+__device__ __forceinline__ void corruption_of(const TrainParams &p, unsigned long long r, int &keep, int &repl)
+{
+    if (p.neg_ent) { repl = p.neg_ent[r]; keep = p.neg_keep[r] ? 1 : 0; }
+    else draw_corruption(p.seed, p.step, r, p.n_ent, &keep, &repl);
+}
 
 // --------------------------------------------------------------------------
 // Dynamic assignment of positives to warps.  A static stride (warp w takes w, w + n_warps, ...) quantises the launch to

@@ -8,8 +8,9 @@
 // instructions of the gradient loop are loads / FMAs / REDs): all shared-memory traffic goes through explicit 32-bit shared addresses (one IADD per
 // 128-bit load instead of 64-bit generic pointer arithmetic re-derived every trip), gradient rows are addressed as
 // one 64-bit base per row plus the lane's byte offset, the shard/window/group machinery does not exist, and the
-// corruption sort is one ballot pair.  Arithmetic per element is identical to the general kernel's (same fp32 FMAs in
-// the same order), so both produce the same scores; gradients differ only in the order of the fp32 atomics.
+// corruption sort is one ballot pair.  The per-element arithmetic is the general kernel's: both form the query vectors
+// and the kept rows' gradients with query_subj / query_obj / trilinear_grad_p (kge_train_common.cuh), so both
+// produce the same scores; gradients differ only in the order of the fp32 atomics.
 #include "kge_train_common.cuh"
 
 namespace kge {
@@ -117,9 +118,8 @@ __global__ void __launch_bounds__(THREADS) kge_train_res_kernel(const TrainParam
         const int s_id = __shfl_sync(0xffffffffu, tv, 0), p_id = __shfl_sync(0xffffffffu, tv, 1), o_id = __shfl_sync(0xffffffffu, tv, 2);
         int keep = -1, repl = 0, bk_at = 0;
         if (lane < eta) {
-            const unsigned long long r = (unsigned long long)lane * (unsigned long long)p.B + (unsigned long long)i;  // tile order j*B+i
-            if (p.neg_ent) { repl = p.neg_ent[r]; keep = p.neg_keep[r] ? 1 : 0; }
-            else draw_corruption(p.seed, p.step, r, p.n_ent, &keep, &repl);
+            const unsigned long long r = (unsigned long long)lane * (unsigned long long)p.B + (unsigned long long)i;
+            corruption_of(p, r, keep, repl);
             if constexpr (GATHER) bk_at = p.bk.off[repl] + p.bk.pos[r];  // consumed after the loss: the loads are long done
         }
         // slots [0, n0) replaced the subject (keep_subj == 0), slots [n0, eta) the object; jorig[slot] = j
@@ -178,15 +178,15 @@ __global__ void __launch_bounds__(THREADS) kge_train_res_kernel(const TrainParam
                 if constexpr (HALVES == 2) {
                     const float4 sr = lds4(a), si = lds4(a + hsB);
                     const float4 orr = lds4(a + lwB), oi = lds4(a + lwB + hsB);
-                    query_subj<2>(pr[it], pi[it], orr, oi, Q0r[it], Q0i[it]);
-                    query_obj<2>(sr, si, pr[it], pi[it], Q1r[it], Q1i[it]);
+                    Q0r[it] = query_subj<2, 0>(pr[it], pi[it], orr, oi); Q0i[it] = query_subj<2, 1>(pr[it], pi[it], orr, oi);
+                    Q1r[it] = query_obj<2, 0>(sr, si, pr[it], pi[it]); Q1i[it] = query_obj<2, 1>(sr, si, pr[it], pi[it]);
                     acc = f4fma(sr, Q0r[it], acc);
                     acc = f4fma(si, Q0i[it], acc);
                     W0i[it] = W1i[it] = f4zero();
                 } else {
                     const float4 vs = lds4(a), vo = lds4(a + lwB);
-                    query_subj<1>(pr[it], pi[it], vo, vo, Q0r[it], Q0i[it]);
-                    query_obj<1>(vs, vs, pr[it], pi[it], Q1r[it], Q1i[it]);
+                    Q0r[it] = query_subj<1, 0>(pr[it], pi[it], vo, vo);
+                    Q1r[it] = query_obj<1, 0>(vs, vs, pr[it], pi[it]);
                     acc = f4fma(vs, Q0r[it], acc);
                 }
                 W0r[it] = W1r[it] = f4zero();
@@ -326,27 +326,27 @@ __global__ void __launch_bounds__(THREADS) kge_train_res_kernel(const TrainParam
                     const float4 orr = lds4(a + lwB), oi = lds4(a + lwB + hsB);
                     const float4 Ur = f4fma(gP, sr, W0r[it]), Ui = f4fma(gP, si, W0i[it]);    // everything that sat in the subject slot
                     const float4 Xr = f4fma(gP, orr, W1r[it]), Xi = f4fma(gP, oi, W1i[it]);   // everything that sat in the object slot
-                    const float4 gsr = f4fma(pi[it], Xi, pr[it] * Xr), gsi = pr[it] * Xi - pi[it] * Xr;      // d/ds f(s,p,X)
-                    const float4 gor = Ur * pr[it] - Ui * pi[it], goi = f4fma(Ur, pi[it], Ui * pr[it]);      // d/do f(U,p,o)
+                    const float4 gsr = query_subj<2, 0>(pr[it], pi[it], Xr, Xi), gsi = query_subj<2, 1>(pr[it], pi[it], Xr, Xi);  // d/ds f(s,p,X)
+                    const float4 gor = query_obj<2, 0>(Ur, Ui, pr[it], pi[it]), goi = query_obj<2, 1>(Ur, Ui, pr[it], pi[it]);    // d/do f(U,p,o)
                     if (s_id == hot0) { H0r[it] = H0r[it] + gsr; H0i[it] = H0i[it] + gsi; }
                     else if (KGE_HOT > 1 && s_id == hot1) { H1r[it] = H1r[it] + gsr; H1i[it] = H1i[it] + gsi; }
                     else { red4(gs_row, o, gsr); red4(gs_row, o + hsB, gsi); }
                     if (o_id == hot0) { H0r[it] = H0r[it] + gor; H0i[it] = H0i[it] + goi; }
                     else if (KGE_HOT > 1 && o_id == hot1) { H1r[it] = H1r[it] + gor; H1i[it] = H1i[it] + goi; }
                     else { red4(go_row, o, gor); red4(go_row, o + hsB, goi); }
-                    red4(gp_row, o, f4fma(Ur, orr, Ui * oi) + f4fma(sr, W1r[it], si * W1i[it]));   // d/dp [f(U,p,o) + f(s,p,W1)]
-                    red4(gp_row, o + hsB, (Ur * oi - Ui * orr) + (sr * W1i[it] - si * W1r[it]));
+                    red4(gp_row, o, trilinear_grad_p<2, 0>(sr, si, orr, oi, Ur, Ui, W1r[it], W1i[it]));
+                    red4(gp_row, o + hsB, trilinear_grad_p<2, 1>(sr, si, orr, oi, Ur, Ui, W1r[it], W1i[it]));
                 } else {
                     const float4 vs = lds4(a), vo = lds4(a + lwB);
                     const float4 U = f4fma(gP, vs, W0r[it]), X = f4fma(gP, vo, W1r[it]);
-                    const float4 gsr = pr[it] * X, gor = U * pr[it];
+                    const float4 gsr = query_subj<1, 0>(pr[it], pi[it], X, X), gor = query_obj<1, 0>(U, U, pr[it], pi[it]);
                     if (s_id == hot0) H0r[it] = H0r[it] + gsr;
                     else if (KGE_HOT > 1 && s_id == hot1) H1r[it] = H1r[it] + gsr;
                     else red4(gs_row, o, gsr);
                     if (o_id == hot0) H0r[it] = H0r[it] + gor;
                     else if (KGE_HOT > 1 && o_id == hot1) H1r[it] = H1r[it] + gor;
                     else red4(go_row, o, gor);
-                    red4(gp_row, o, f4fma(U, vo, vs * W1r[it]));
+                    red4(gp_row, o, trilinear_grad_p<1, 0>(vs, vs, vo, vo, U, U, W1r[it], W1r[it]));
                 }
             }
         }

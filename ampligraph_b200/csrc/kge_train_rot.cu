@@ -14,30 +14,14 @@
 //     into the buffer that has just been consumed (the general kernel re-gathers all but the last);
 //   * explicit 32-bit shared addresses, loop invariants kept in registers (KGE_KEEP*), one 64-bit gradient base per replaced
 //     row with the second chunk and the imaginary half as immediate / register offsets of the RED.
-// Arithmetic per element is the general kernel's (same fp32 operations in the same order), so both produce the same
-// scores bit for bit; gradients differ only in the order of the fp32 atomics
-// (tests/test_gpu_parity.py::test_resident_fast_path_equals_general_kernel).
+// The per-element arithmetic is the general kernel's: both compute RotatE with the rot_* functions of
+// kge_train_common.cuh, so both produce the same scores bit for bit; gradients differ only in the order of the fp32
+// atomics (tests/test_gpu_parity.py::test_resident_fast_path_equals_general_kernel).
 #include "kge_train_common.cuh"
 
 namespace kge {
 
 namespace {
-
-// sum of the four moduli of (re, im): x = re^2 + im^2, one MUFU.SQRT each (kge_train.cu: Scorer<KGE_ROTATE>::modsum)
-__device__ __forceinline__ float rot_modsum(float4 re, float4 im)
-{
-    const float4 x = f4fma(im, im, re * re);
-    return (sqrt_approx(x.x) + sqrt_approx(x.y)) + (sqrt_approx(x.z) + sqrt_approx(x.w));
-}
-// (a, b) = g * (re, im) / |(re, im)|, zero where the residual is exactly zero (Scorer<KGE_ROTATE>::unit)
-__device__ __forceinline__ void rot_unit(float4 re, float4 im, float g, float4 &a, float4 &b)
-{
-    const float4 x = f4fma(im, im, re * re);
-    const float4 inv = g * make_float4(rsqrt_approx(fmaxf(x.x, 1e-30f)), rsqrt_approx(fmaxf(x.y, 1e-30f)),
-                                       rsqrt_approx(fmaxf(x.z, 1e-30f)), rsqrt_approx(fmaxf(x.w, 1e-30f)));
-    a = re * inv;
-    b = im * inv;
-}
 
 // 16-byte read-only load that stays where it is written (asm volatile: the compiler may not sink it to its first use)
 __device__ __forceinline__ float4 ldg4_nc(const char *p)
@@ -144,9 +128,7 @@ __global__ void __launch_bounds__(256) kge_train_rot_kernel(const TrainParams p)
             const int j = base + lane;
             int keep = -1, repl = 0;
             if (j < eta) {
-                const unsigned long long r = (unsigned long long)j * (unsigned long long)p.B + (unsigned long long)i;  // tile order j*B+i
-                if (p.neg_ent) { repl = p.neg_ent[r]; keep = p.neg_keep[r] ? 1 : 0; }
-                else draw_corruption(p.seed, p.step, r, p.n_ent, &keep, &repl);
+                corruption_of(p, (unsigned long long)j * (unsigned long long)p.B + (unsigned long long)i, keep, repl);
                 sts_i(side_s + 4u * (uint32_t)j, keep);  // keep_subj = 1 -> object replaced -> side 1
                 sts_i(sc_s + 4u * (uint32_t)j, repl);
                 if (stamping) p.stamp_ent[repl] = p.stamp;  // lazy optimizer: row touched
@@ -186,8 +168,8 @@ __global__ void __launch_bounds__(256) kge_train_rot_kernel(const TrainParams p)
 #pragma unroll
             for (int it = 0; it < NIT; ++it) {
                 if (!live[it]) { sr[it] = si[it] = f4zero(); C[it] = Sn[it] = Or_[it] = Oi[it] = f4zero(); }
-                Yr[it] = f4fma(f4neg(si[it]), Sn[it], sr[it] * C[it]);  // sr c - si s
-                Yi[it] = f4fma(sr[it], Sn[it], si[it] * C[it]);         // sr s + si c
+                Yr[it] = rot_rotate<0>(sr[it], si[it], C[it], Sn[it]);
+                Yi[it] = rot_rotate<1>(sr[it], si[it], C[it], Sn[it]);
                 Zor[it] = Zoi[it] = Zsr[it] = Zsi[it] = Aphi[it] = f4zero();
                 acc = fmaf(rot_modsum(Yr[it] - Or_[it], Yi[it] - Oi[it]), nlive[it], acc);
             }
@@ -212,10 +194,10 @@ __global__ void __launch_bounds__(256) kge_train_rot_kernel(const TrainParams p)
                 for (int it = 0; it < NIT; ++it) {
                     const float4 ar = lds4(ra + off[it]), ai = lds4(ra + off[it] + hsB);
                     const float4 br = lds4(rb + off[it]), bi = lds4(rb + off[it] + hsB);
-                    const float4 e0r = f4fma(f4neg(ai), Sn[it], f4fma(ar, C[it], f4neg(Or_[it])));
-                    const float4 e0i = f4fma(ai, C[it], f4fma(ar, Sn[it], f4neg(Oi[it])));
-                    const float4 e1r = f4fma(f4neg(bi), Sn[it], f4fma(br, C[it], f4neg(Or_[it])));
-                    const float4 e1i = f4fma(bi, C[it], f4fma(br, Sn[it], f4neg(Oi[it])));
+                    const float4 e0r = rot_residual_subj<0>(ar, ai, C[it], Sn[it], Or_[it], Oi[it]);
+                    const float4 e0i = rot_residual_subj<1>(ar, ai, C[it], Sn[it], Or_[it], Oi[it]);
+                    const float4 e1r = rot_residual_subj<0>(br, bi, C[it], Sn[it], Or_[it], Oi[it]);
+                    const float4 e1i = rot_residual_subj<1>(br, bi, C[it], Sn[it], Or_[it], Oi[it]);
                     a = fmaf(rot_modsum(e0r, e0i), nlive[it], a);
                     b = fmaf(rot_modsum(e1r, e1i), nlive[it], b);
                 }
@@ -274,22 +256,22 @@ __global__ void __launch_bounds__(256) kge_train_rot_kernel(const TrainParams p)
                 for (int it = 0; it < NIT; ++it) {
                     const float4 ar = lds4(ra + off[it]), ai = lds4(ra + off[it] + hsB);
                     const float4 br = lds4(rb + off[it]), bi = lds4(rb + off[it] + hsB);
-                    const float4 yar = f4fma(f4neg(ai), Sn[it], ar * C[it]), yai = f4fma(ar, Sn[it], ai * C[it]);  // R(phi) r
-                    const float4 ybr = f4fma(f4neg(bi), Sn[it], br * C[it]), ybi = f4fma(br, Sn[it], bi * C[it]);
+                    const float4 yar = rot_rotate<0>(ar, ai, C[it], Sn[it]), yai = rot_rotate<1>(ar, ai, C[it], Sn[it]);  // R(phi) r
+                    const float4 ybr = rot_rotate<0>(br, bi, C[it], Sn[it]), ybi = rot_rotate<1>(br, bi, C[it], Sn[it]);
                     float4 a, b, c, d;
                     rot_unit(yar - Or_[it], yai - Oi[it], ga, a, b);
                     rot_unit(ybr - Or_[it], ybi - Oi[it], gb, c, d);
                     Zsr[it] = Zsr[it] + a; Zsi[it] = Zsi[it] + b;
                     Zsr[it] = Zsr[it] + c; Zsi[it] = Zsi[it] + d;
-                    Aphi[it] = f4fma(f4neg(b), yar, f4fma(a, yai, Aphi[it]));  // a*y_im - b*y_re
-                    Aphi[it] = f4fma(f4neg(d), ybr, f4fma(c, ybi, Aphi[it]));
+                    Aphi[it] = rot_dphi(a, b, yar, yai, Aphi[it]);
+                    Aphi[it] = rot_dphi(c, d, ybr, ybi, Aphi[it]);
                     if (live[it]) {
-                        red_add_v4(reinterpret_cast<float *>(ga0 + 512 * it), f4fma(f4neg(b), Sn[it], f4neg(a) * C[it]));      // -(a c + b s)
-                        red_add_v4(reinterpret_cast<float *>(ga0 + hsB + 512 * it), f4fma(f4neg(b), C[it], a * Sn[it]));        // a s - b c
+                        red_add_v4(reinterpret_cast<float *>(ga0 + 512 * it), rot_back<0>(a, b, C[it], Sn[it]));
+                        red_add_v4(reinterpret_cast<float *>(ga0 + hsB + 512 * it), rot_back<1>(a, b, C[it], Sn[it]));
                     }
                     if (live[it] && has_b) {
-                        red_add_v4(reinterpret_cast<float *>(gb0 + 512 * it), f4fma(f4neg(d), Sn[it], f4neg(c) * C[it]));
-                        red_add_v4(reinterpret_cast<float *>(gb0 + hsB + 512 * it), f4fma(f4neg(d), C[it], c * Sn[it]));
+                        red_add_v4(reinterpret_cast<float *>(gb0 + 512 * it), rot_back<0>(c, d, C[it], Sn[it]));
+                        red_add_v4(reinterpret_cast<float *>(gb0 + hsB + 512 * it), rot_back<1>(c, d, C[it], Sn[it]));
                     }
                 }
             }
@@ -330,12 +312,12 @@ __global__ void __launch_bounds__(256) kge_train_rot_kernel(const TrainParams p)
             float4 a, b;
             rot_unit(Yr[it] - Or_[it], Yi[it] - Oi[it], dP, a, b);
             const float4 Zr = a + Zor[it], Zi = b + Zoi[it];  // everything with y = R(phi) s
-            red4(gs_row, off[it], f4fma(f4neg(Zi), Sn[it], f4neg(Zr) * C[it]));   // -(Zr c + Zi s)
-            red4(gs_row, off[it] + hsB, f4fma(f4neg(Zi), C[it], Zr * Sn[it]));    // Zr s - Zi c
+            red4(gs_row, off[it], rot_back<0>(Zr, Zi, C[it], Sn[it]));
+            red4(gs_row, off[it] + hsB, rot_back<1>(Zr, Zi, C[it], Sn[it]));
             red4(go_row, off[it], a + Zsr[it]);
             red4(go_row, off[it] + hsB, b + Zsi[it]);
             // d/dtheta = (1/div) d/dphi in the first half of the relation row (the second half is allocated but unused, RotatE.py:76)
-            red4(gp_row, off[it], inv_div * f4fma(f4neg(Zi), Yr[it], f4fma(Zr, Yi[it], Aphi[it])));
+            red4(gp_row, off[it], inv_div * rot_dphi(Zr, Zi, Yr[it], Yi[it], Aphi[it]));
         }
         __syncwarp();  // the bookkeeping arrays are rewritten by the next positive
     }

@@ -956,23 +956,34 @@ static int check_candidates(const char *fn, const int32_t *cand_ids, int64_t can
     return KGE_OK;
 }
 
-// The scoring parameters of b model queries prepared into w (launch_rank_prepare) against the entity rows ent; the
-// candidate window and the outputs are the caller's
-static RankParams query_rank_params(const kge_handle *h, const RankWorkspace &w, int32_t side, int32_t strategy,
-                                    const float *ent, int64_t b)
+// The query side of a ranking call: refresh the rotation table (RotatE), prepare the b triples' query vectors and
+// quantised positive scores into w (launch_rank_prepare; entity rows ent, or the shards of map), and set *p to their
+// scoring parameters against ent.  The candidate window and the outputs are the caller's; a CUDA error is reported as
+// `what`.
+static int prepare_queries(kge_handle *h, const kge_shard_map *map, const RankWorkspace &w, int32_t side, int32_t strategy,
+                           const float *ent, const float *rel, const int32_t *triples, int64_t b, cudaStream_t st,
+                           const char *what, RankParams *p)
 {
-    RankParams p;
-    memset(&p, 0, sizeof(p));
-    p.L = h->L;
-    p.side = side;
-    p.strategy = strategy;
-    p.ent = ent;
-    p.qvec = side == KGE_SIDE_S ? w.qs : w.qo;
-    p.qaux = w.qaux;
-    p.qpos = w.qpos;
-    p.b = b;
-    p.scale = h->score_scale;
-    return p;
+    if (int rc = refresh_rotation(h, rel, st)) return rc;
+    ShardView sv;
+    memset(&sv, 0, sizeof(sv));
+    if (map && map->world > 1) {
+        sv.world = map->world;
+        sv.rows_per_shard = (int)map->rows_per_shard;
+        for (int q = 0; q < map->world; ++q) sv.ent[q] = map->ent[q];
+    }
+    KGE_CUDA(launch_rank_prepare(h->L, sv, ent, rel, h->rot, triples, b, h->score_scale, w.qs, w.qo, w.qaux, w.qpos, st), what);
+    memset(p, 0, sizeof(*p));
+    p->L = h->L;
+    p->side = side;
+    p->strategy = strategy;
+    p->ent = ent;
+    p->qvec = side == KGE_SIDE_S ? w.qs : w.qo;
+    p->qaux = w.qaux;
+    p->qpos = w.qpos;
+    p->b = b;
+    p->scale = h->score_scale;
+    return KGE_OK;
 }
 
 static int rank_impl(kge_handle *h, const kge_shard_map *map, int64_t filt_base, int32_t side, int32_t strategy,
@@ -999,21 +1010,12 @@ static int rank_impl(kge_handle *h, const kge_shard_map *map, int64_t filt_base,
     cudaStream_t st = (cudaStream_t)stream;
     Carve c(workspace_dev);
     const RankWorkspace w = carve_rank_workspace(h, c, b, n_cand, true);
-    if (int rc = refresh_rotation(h, rel_dev, st)) return rc;
-    ShardView sv;
-    memset(&sv, 0, sizeof(sv));
-    if (map && map->world > 1) {
-        sv.world = map->world;
-        sv.rows_per_shard = (int)map->rows_per_shard;
-        for (int q = 0; q < map->world; ++q) sv.ent[q] = map->ent[q];
-    }
-    KGE_CUDA(launch_rank_prepare(h->L, sv, ent_dev, rel_dev, h->rot, triples_dev, b, h->score_scale, w.qs, w.qo, w.qaux,
-                                 w.qpos, st),
-             "kge_rank: prepare");
+    RankParams p;
+    if (int rc = prepare_queries(h, map, w, side, strategy, ent_dev, rel_dev, triples_dev, b, st, "kge_rank: prepare", &p))
+        return rc;
     // raw counters of THIS call in a zeroed scratch; added to the caller's accumulator or finalized into ranks_dev below
     int32_t *cnt = w.cnt;
     KGE_CUDA(cudaMemsetAsync(cnt, 0, (size_t)3 * b * sizeof(int32_t), st), "kge_rank: memset");
-    RankParams p = query_rank_params(h, w, side, strategy, ent_dev, b);
     p.cand_ids = cand_ids_dev;
     p.cand_begin = cand_begin;
     p.n_cand = n_cand;
@@ -1225,15 +1227,11 @@ extern "C" int kge_topk(kge_handle *h, int32_t side, const float *ent_dev, const
     cudaStream_t st = (cudaStream_t)stream;
     Carve c(workspace_dev);
     const TopkWorkspace w = carve_topk_workspace(h, c, b, n_cand, k);
-    if (int rc = refresh_rotation(h, rel_dev, st)) return rc;
-    ShardView sv;
-    memset(&sv, 0, sizeof(sv));
-    KGE_CUDA(launch_rank_prepare(h->L, sv, ent_dev, rel_dev, h->rot, triples_dev, b, h->score_scale, w.r.qs, w.r.qo, w.r.qaux,
-                                 w.r.qpos, st),
-             "kge_topk: prepare");
+    RankParams p;
+    if (int rc = prepare_queries(h, nullptr, w.r, side, KGE_RANK_WORST, ent_dev, rel_dev, triples_dev, b, st, "kge_topk: prepare", &p))
+        return rc;
     KGE_CUDA(cudaMemsetAsync(w.l.state, 0, (size_t)b * sizeof(int2), st), "kge_topk: memset");
     // the exact FP32 chain in every rank_mode: scores bit-identical to kge_corruption_scores
-    RankParams p = query_rank_params(h, w.r, side, KGE_RANK_WORST, ent_dev, b);
     p.scores = w.chunk;
     const TopkSelectParams s = topk_select_params(w.chunk, b, k, w.l, filt_off_dev, filt_idx_dev, n_filt, cand_ids_dev ? 0 : cand_begin);
     if (int rc = sweep(h, "kge_topk", "select", p, rank_op(h->L.model, side), w.r.cnt, cand_ids_dev, cand_begin, n_cand, st,

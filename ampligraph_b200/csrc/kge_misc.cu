@@ -1,6 +1,8 @@
 // kge_misc.cu -- predict-path scoring, layout packing, Glorot initialisation (sm_90a).
 #include <math.h>
 
+#include <type_traits>
+
 #include "kge_internal.h"
 
 namespace kge {
@@ -44,6 +46,20 @@ __global__ void kge_score_kernel(const float *__restrict__ ent, const float *__r
     }
 }
 
+// returns launch(std::integral_constant<int, MODEL>) for the scoring model, or cudaErrorInvalidValue for an unknown one
+template <class Launch>
+static cudaError_t dispatch_model(int model, Launch &&launch)
+{
+    switch (model) {
+    case KGE_TRANSE: return launch(std::integral_constant<int, KGE_TRANSE>{});
+    case KGE_DISTMULT: return launch(std::integral_constant<int, KGE_DISTMULT>{});
+    case KGE_COMPLEX: return launch(std::integral_constant<int, KGE_COMPLEX>{});
+    case KGE_HOLE: return launch(std::integral_constant<int, KGE_HOLE>{});
+    case KGE_ROTATE: return launch(std::integral_constant<int, KGE_ROTATE>{});
+    default: return cudaErrorInvalidValue;
+    }
+}
+
 cudaError_t launch_score_triples(const Layout &L, int, const float *ent, const float *rel_or_rot,
                                  const int32_t *triples, long long n, float scale, float *out, int sm_count,
                                  cudaStream_t st)
@@ -52,15 +68,10 @@ cudaError_t launch_score_triples(const Layout &L, int, const float *ent, const f
     const int threads = 256;
     long long want = (n + 7) / 8;
     int grid = (int)(want < (long long)sm_count * 8 ? want : (long long)sm_count * 8);
-    switch (L.model) {
-    case KGE_TRANSE: kge_score_kernel<KGE_TRANSE><<<grid, threads, 0, st>>>(ent, rel_or_rot, triples, n, L.k, L.kp, L.ld, scale, out); break;
-    case KGE_DISTMULT: kge_score_kernel<KGE_DISTMULT><<<grid, threads, 0, st>>>(ent, rel_or_rot, triples, n, L.k, L.kp, L.ld, scale, out); break;
-    case KGE_COMPLEX: kge_score_kernel<KGE_COMPLEX><<<grid, threads, 0, st>>>(ent, rel_or_rot, triples, n, L.k, L.kp, L.ld, scale, out); break;
-    case KGE_HOLE: kge_score_kernel<KGE_HOLE><<<grid, threads, 0, st>>>(ent, rel_or_rot, triples, n, L.k, L.kp, L.ld, scale, out); break;
-    case KGE_ROTATE: kge_score_kernel<KGE_ROTATE><<<grid, threads, 0, st>>>(ent, rel_or_rot, triples, n, L.k, L.kp, L.ld, scale, out); break;
-    default: return cudaErrorInvalidValue;
-    }
-    return cudaGetLastError();
+    return dispatch_model(L.model, [&](auto model) {
+        kge_score_kernel<decltype(model)::value><<<grid, threads, 0, st>>>(ent, rel_or_rot, triples, n, L.k, L.kp, L.ld, scale, out);
+        return cudaGetLastError();
+    });
 }
 
 // --------------------------------------------------------------------------

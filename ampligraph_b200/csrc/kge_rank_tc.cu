@@ -429,20 +429,13 @@ cudaError_t launch_rank_count_tc(const RankParams &p, const RankTcLayout &w, voi
     t.ctas_per_qb = per;
     t.probe_a = probe_a; t.probe_d = probe_d; t.scale = p.scale;
     const size_t smem = (size_t)TC_STAGES * TC_STAGE_BYTES + 1024 /*alignment*/ + 128 /*barriers*/;
-    if (probe_a) {
-        if ((e = cudaFuncSetAttribute(kge_rank_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return e;
-        kge_rank_tc_kernel<true><<<(unsigned)(w.n_qb * per), TC_THREADS, smem, st>>>(t);
-        return cudaGetLastError();
-    }
-    if ((e = cudaFuncSetAttribute(kge_rank_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return e;
-    kge_rank_tc_kernel<false><<<(unsigned)(w.n_qb * per), TC_THREADS, smem, st>>>(t);
-    {
-        const int wpc = pair_score_warps(ld, 2);
-        const size_t rsm = (size_t)wpc * 2 * ld * sizeof(float);
-        if ((e = cudaFuncSetAttribute(kge_rank_refine_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rsm)) != cudaSuccess) return e;
-        kge_rank_refine_kernel<<<sm_count * 2, wpc * 32, rsm, st>>>(p, pairs, count, w.pair_cap, cnt);
-    }
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    const unsigned grid = (unsigned)(w.n_qb * per);
+    if (probe_a) return launch_with_smem(kge_rank_tc_kernel<true>, grid, TC_THREADS, smem, st, t);
+    if ((e = launch_with_smem(kge_rank_tc_kernel<false>, grid, TC_THREADS, smem, st, t)) != cudaSuccess) return e;
+    const int wpc = pair_score_warps(ld, 2);
+    if ((e = launch_with_smem(kge_rank_refine_kernel, sm_count * 2, wpc * 32, (size_t)wpc * 2 * ld * sizeof(float), st, p, pairs,
+                              count, w.pair_cap, cnt)) != cudaSuccess)
+        return e;
     // overflow fallback: the exact FP32 kernel, every CTA of which returns at once unless the pair list overflowed
     RankParams g = p;
     g.gate = count;

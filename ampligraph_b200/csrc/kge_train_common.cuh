@@ -18,34 +18,7 @@ namespace kge {
 __device__ __forceinline__ float4 f4zero() { return make_float4(0.f, 0.f, 0.f, 0.f); }
 __device__ __forceinline__ float4 f4ld(const float *p) { return *reinterpret_cast<const float4 *>(p); }
 __device__ __forceinline__ void f4st(float *p, float4 v) { *reinterpret_cast<float4 *>(p) = v; }
-// fp32 pairs: two values in a 64-bit register pair.  Hopper has no packed fp32 instruction, so a pair operation is two
-// IEEE fp32 operations (FFMA / FMUL / FADD, round to nearest), one per half; pk2 / upk2 are register renames.
-typedef unsigned long long f32x2_t;
-__device__ __forceinline__ f32x2_t pk2(float lo, float hi)
-{
-    f32x2_t r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
-}
-__device__ __forceinline__ void upk2(f32x2_t v, float &lo, float &hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ f32x2_t fma2(f32x2_t a, f32x2_t b, f32x2_t c)
-{
-    float a0, a1, b0, b1, c0, c1;
-    upk2(a, a0, a1); upk2(b, b0, b1); upk2(c, c0, c1);
-    return pk2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
-}
-__device__ __forceinline__ f32x2_t mul2(f32x2_t a, f32x2_t b)
-{
-    float a0, a1, b0, b1;
-    upk2(a, a0, a1); upk2(b, b0, b1);
-    return pk2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
-}
-__device__ __forceinline__ f32x2_t add2(f32x2_t a, f32x2_t b)
-{
-    float a0, a1, b0, b1;
-    upk2(a, a0, a1); upk2(b, b0, b1);
-    return pk2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
-}
+// float4 arithmetic as two fp32 pairs (pk2 / fma2 / mul2 / add2 of kge_common.cuh)
 __device__ __forceinline__ float4 f4from(f32x2_t lo, f32x2_t hi)
 {
     float4 r;

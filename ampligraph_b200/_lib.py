@@ -18,7 +18,7 @@ SCORING = {"TransE": 0, "DistMult": 1, "ComplEx": 2, "HolE": 3, "RotatE": 4}
 LOSSES = {"pairwise": 0, "nll": 1, "absolute_margin": 2, "self_adversarial": 3, "multiclass_nll": 4}
 REDUCTIONS = {"sum": 0, "mean": 1}
 OPTIMIZERS = {"sgd": 0, "adam": 1, "adagrad": 2, "rmsprop": 3, "adadelta": 4, "adamax": 5}
-SIDES = {"s": 0, "o": 1}
+SIDES = {"s": 0, "o": 1, "p": 2}  # "p": relation prediction, candidates are relation rows
 STRATEGIES = {"worst": 0, "best": 1, "middle": 2}
 STEP_FUSED, STEP_FORWARD_ONLY, STEP_BACKWARD_EXT, STEP_FUSED_DEFER = 0, 1, 2, 3
 RANK_MODES = {"auto": 0, "exact": 1}

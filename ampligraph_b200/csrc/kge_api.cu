@@ -956,6 +956,20 @@ static int check_candidates(const char *fn, const int32_t *cand_ids, int64_t can
     return KGE_OK;
 }
 
+// The candidate window of a ranking / top-k call on `side`: entity rows, or relation rows on KGE_SIDE_P
+static int check_side_candidates(const kge_handle *h, const char *fn, int32_t side, const int32_t *cand_ids, int64_t cand_begin,
+                                 int64_t n_cand)
+{
+    if (side == KGE_SIDE_P) return check_candidates(fn, cand_ids, cand_begin, n_cand, h->cfg.n_rel, "n_rel");
+    return check_candidates(fn, cand_ids, cand_begin, n_cand, h->cfg.n_ent, "n_ent");
+}
+
+// The relation-side candidate rows: the relation table, or for RotatE the rotation table prepare_queries refreshed
+static const float *relation_rows(const kge_handle *h, const float *rel_dev)
+{
+    return h->cfg.scoring == KGE_ROTATE ? h->rot : rel_dev;
+}
+
 // The query side of a ranking call: refresh the rotation table (RotatE), prepare the b triples' query vectors and
 // quantised positive scores into w (launch_rank_prepare; entity rows ent, or the shards of map), and set *p to their
 // scoring parameters against ent.  The candidate window and the outputs are the caller's; a CUDA error is reported as
@@ -994,7 +1008,7 @@ static int rank_impl(kge_handle *h, const kge_shard_map *map, int64_t filt_base,
                      float *probe_delta_dev = nullptr)
 {
     KGE_CHECK_HANDLE(h, "kge_rank");
-    if (side != KGE_SIDE_S && side != KGE_SIDE_O) return fail(KGE_ERR_INVALID_ARGUMENT, "Invalid value for corrupt_side");
+    if (side != KGE_SIDE_S && side != KGE_SIDE_O && side != KGE_SIDE_P) return fail(KGE_ERR_INVALID_ARGUMENT, "Invalid value for corrupt_side");
     if (strategy < KGE_RANK_WORST || strategy > KGE_RANK_MIDDLE)
         return fail(KGE_ERR_INVALID_ARGUMENT, "Invalid value for ranking_strategy");
     if (b < 0 || n_cand < 0 || cand_begin < 0 || n_filt < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_rank: negative size");
@@ -1002,7 +1016,7 @@ static int rank_impl(kge_handle *h, const kge_shard_map *map, int64_t filt_base,
     if (!ent_dev || !rel_dev || !triples_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_rank: null pointer");
     if (!ranks_dev && !counts_dev && !scores_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_rank: no output buffer");
     // (a shard's window [0, n_local) always lies inside n_ent)
-    if (int rc = check_candidates("kge_rank", cand_ids_dev, cand_begin, n_cand, h->cfg.n_ent, "n_ent")) return rc;
+    if (int rc = check_side_candidates(h, "kge_rank", side, cand_ids_dev, cand_begin, n_cand)) return rc;
     // both filter pointers null with n_filt > 0: nothing is filtered (kge_topk / kge_knn reject that)
     if ((filt_off_dev == nullptr) != (filt_idx_dev == nullptr) && n_filt > 0)
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_rank: filter offsets and indices must be given together");
@@ -1027,12 +1041,20 @@ static int rank_impl(kge_handle *h, const kge_shard_map *map, int64_t filt_base,
         KGE_CUDA(launch_rank_count_tc(p, w.tcl, w.tc_base, cnt, h->sm_count, st, scores_dev, probe_delta_dev), "kge_rank_filter_probe");
         return KGE_OK;
     }
-    if (w.tc && !scores_dev && n_cand > 0)  // tensor-core filter + exact refine: bit-identical counters (kge_rank_tc.cu)
-        KGE_CUDA(launch_rank_count_tc(p, w.tcl, w.tc_base, cnt, h->sm_count, st), "kge_rank: tensor-core count");
-    else
-        KGE_CUDA(launch_rank_count(p, cnt, st), "kge_rank: count");
-    if (filt_off_dev && n_filt > 0)
-        KGE_CUDA(launch_rank_filter_n(p, (const long long *)filt_off_dev, filt_idx_dev, n_filt, cnt, h->sm_count, st), "kge_rank: filter");
+    if (side == KGE_SIDE_P) {  // relation candidates: the exact chain of every pair in every rank_mode (kge_rank_rel.cu)
+        const float *rel_rows = relation_rows(h, rel_dev);
+        KGE_CUDA(launch_rank_rel_count(p, rel_rows, triples_dev, cnt, st), "kge_rank: count");
+        if (filt_off_dev && n_filt > 0)
+            KGE_CUDA(launch_rank_rel_filter(p, rel_rows, triples_dev, (const long long *)filt_off_dev, filt_idx_dev, n_filt, cnt,
+                                            h->sm_count, st), "kge_rank: filter");
+    } else {
+        if (w.tc && !scores_dev && n_cand > 0)  // tensor-core filter + exact refine: bit-identical counters (kge_rank_tc.cu)
+            KGE_CUDA(launch_rank_count_tc(p, w.tcl, w.tc_base, cnt, h->sm_count, st), "kge_rank: tensor-core count");
+        else
+            KGE_CUDA(launch_rank_count(p, cnt, st), "kge_rank: count");
+        if (filt_off_dev && n_filt > 0)
+            KGE_CUDA(launch_rank_filter_n(p, (const long long *)filt_off_dev, filt_idx_dev, n_filt, cnt, h->sm_count, st), "kge_rank: filter");
+    }
     if (counts_dev) KGE_CUDA(launch_rank_accumulate(cnt, b, counts_dev, st), "kge_rank: accumulate");
     else if (ranks_dev) KGE_CUDA(launch_rank_finalize(cnt, b, strategy, ranks_dev, st), "kge_rank: finalize");
     return KGE_OK;
@@ -1053,6 +1075,9 @@ extern "C" int kge_rank_sharded(kge_handle *h, const kge_shard_map *map, int32_t
                                 int32_t *ranks_dev, int32_t *counts_dev, void *workspace_dev, int64_t workspace_bytes,
                                 void *stream)
 {
+    if (side == KGE_SIDE_P)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_rank_sharded: the relation side is not sharded (the relation table is "
+                    "replicated): rank it with kge_rank");
     if (!h) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_rank_sharded: null handle");
     if (int rc = check_shard_map(h, map, "kge_rank_sharded")) return rc;
     if (rank < 0 || rank >= map->world) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_rank_sharded: rank out of range");
@@ -1093,6 +1118,7 @@ extern "C" int kge_rank_filter_probe(kge_handle *h, int32_t side, const float *e
                                      int64_t workspace_bytes, void *stream)
 {
     if (!approx_dev || !delta_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_rank_filter_probe: null output");
+    if (side == KGE_SIDE_P) return fail(KGE_ERR_UNSUPPORTED, "kge_rank_filter_probe: the tensor-core filter does not apply to the relation side");
     return rank_impl(h, nullptr, 0, side, KGE_RANK_WORST, ent_dev, rel_dev, triples_dev, b, cand_ids_dev, cand_begin, n_cand,
                      nullptr, nullptr, 0, nullptr, nullptr, approx_dev, workspace_dev, workspace_bytes, stream, delta_dev);
 }
@@ -1190,11 +1216,11 @@ static int stage_fail(cudaError_t e, const char *fn, const char *stage)
 }
 
 // The chunked candidate sweep of kge_topk, kge_knn and the radius calls, over the b queries the caller prepared for p:
-// for every chunk of topk_chunk candidates, score them with chain `op` into p.scores ([b, nc], row stride nc), then run
+// for every chunk of topk_chunk candidates, score them with score(p) into p.scores ([b, nc], row stride nc), then run
 // epilogue(nc, c0).  CUDA errors are reported as "<fn>: <stage>".
-template <class Epilogue>
-static int sweep(const kge_handle *h, const char *fn, const char *stage, RankParams p, int op, int32_t *cnt,
-                 const int32_t *cand_ids, int64_t cand_begin, int64_t n_cand, cudaStream_t st, Epilogue epilogue)
+template <class Score, class Epilogue>
+static int sweep(const kge_handle *h, const char *fn, const char *stage, RankParams p, Score score, const int32_t *cand_ids,
+                 int64_t cand_begin, int64_t n_cand, cudaStream_t st, Epilogue epilogue)
 {
     const int64_t C = topk_chunk(h, p.b, n_cand);
     for (int64_t c0 = 0; c0 < n_cand; c0 += C) {
@@ -1202,7 +1228,7 @@ static int sweep(const kge_handle *h, const char *fn, const char *stage, RankPar
         p.cand_ids = cand_ids ? cand_ids + c0 : nullptr;
         p.cand_begin = cand_ids ? 0 : cand_begin + c0;
         p.n_cand = nc;
-        if (cudaError_t e = launch_rank_count_op(p, op, cnt, st)) return stage_fail(e, fn, "scores");
+        if (cudaError_t e = score(p)) return stage_fail(e, fn, "scores");
         if (cudaError_t e = epilogue(nc, c0)) return stage_fail(e, fn, stage);
     }
     return KGE_OK;
@@ -1214,13 +1240,13 @@ extern "C" int kge_topk(kge_handle *h, int32_t side, const float *ent_dev, const
                         int32_t *ids_dev, float *scores_dev, void *workspace_dev, int64_t workspace_bytes, void *stream)
 {
     KGE_CHECK_HANDLE(h, "kge_topk");
-    if (side != KGE_SIDE_S && side != KGE_SIDE_O) return fail(KGE_ERR_INVALID_ARGUMENT, "Invalid value for corrupt_side");
+    if (side != KGE_SIDE_S && side != KGE_SIDE_O && side != KGE_SIDE_P) return fail(KGE_ERR_INVALID_ARGUMENT, "Invalid value for corrupt_side");
     if (k < 1) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_topk: k must be >= 1, got %d", k);
     if (b < 0 || n_cand < 0 || cand_begin < 0 || n_filt < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_topk: negative size");
     if (n_cand > 0x7fffffffLL) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_topk: n_cand must be < 2^31");
     if (b == 0) return KGE_OK;
     if (!ent_dev || !rel_dev || !triples_dev || !ids_dev || !scores_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_topk: null pointer");
-    if (int rc = check_candidates("kge_topk", cand_ids_dev, cand_begin, n_cand, h->cfg.n_ent, "n_ent")) return rc;
+    if (int rc = check_side_candidates(h, "kge_topk", side, cand_ids_dev, cand_begin, n_cand)) return rc;
     if ((filt_off_dev == nullptr || filt_idx_dev == nullptr) && n_filt > 0)
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_topk: filter offsets and indices must be given together");
     if (int rc = check_workspace(workspace_dev, workspace_bytes, kge_topk_workspace_bytes(h, b, n_cand, k), "kge_topk")) return rc;
@@ -1234,7 +1260,12 @@ extern "C" int kge_topk(kge_handle *h, int32_t side, const float *ent_dev, const
     // the exact FP32 chain in every rank_mode: scores bit-identical to kge_corruption_scores
     p.scores = w.chunk;
     const TopkSelectParams s = topk_select_params(w.chunk, b, k, w.l, filt_off_dev, filt_idx_dev, n_filt, cand_ids_dev ? 0 : cand_begin);
-    if (int rc = sweep(h, "kge_topk", "select", p, rank_op(h->L.model, side), w.r.cnt, cand_ids_dev, cand_begin, n_cand, st,
+    const float *rel_rows = relation_rows(h, rel_dev);
+    auto score = [&](const RankParams &q) {
+        return side == KGE_SIDE_P ? launch_rank_rel_count(q, rel_rows, triples_dev, w.r.cnt, st)
+                                  : launch_rank_count_op(q, rank_op(h->L.model, side), w.r.cnt, st);
+    };
+    if (int rc = sweep(h, "kge_topk", "select", p, score, cand_ids_dev, cand_begin, n_cand, st,
                        [&](int64_t nc, int64_t c0) { return select_chunk(s, nc, c0, st); }))
         return rc;
     KGE_CUDA(launch_topk_write(w.l.state, w.l.keys, w.l.vals, b, k, cand_ids_dev, cand_begin, ids_dev, scores_dev, st),
@@ -1339,8 +1370,10 @@ static int point_sweep(const kge_handle *h, const char *fn, const char *stage, i
 {
     if (cudaError_t e = launch_knn_gather(points_dev, ld, query_ids_dev, b, w.qvec, st)) return stage_fail(e, fn, "gather");
     if (cudaError_t e = cudaMemsetAsync(w.cnt, 0, (size_t)4 * b * sizeof(int32_t), st)) return stage_fail(e, fn, "memset");
-    return sweep(h, fn, stage, knn_rank_params(ld, points_dev, w, b), metric == KGE_METRIC_EUCLIDEAN ? OP_L2_SUB : OP_L1_SUB,
-                 w.cnt, cand_ids_dev, cand_begin, n_cand, st, epilogue);
+    const int op = metric == KGE_METRIC_EUCLIDEAN ? OP_L2_SUB : OP_L1_SUB;
+    return sweep(h, fn, stage, knn_rank_params(ld, points_dev, w, b),
+                 [&](const RankParams &q) { return launch_rank_count_op(q, op, w.cnt, st); }, cand_ids_dev, cand_begin, n_cand,
+                 st, epilogue);
 }
 
 extern "C" int kge_knn(kge_handle *h, int32_t metric, const float *points_dev, int64_t n_points, int32_t ld,

@@ -177,6 +177,14 @@ cudaError_t launch_rank_filter_n(const RankParams &p, const long long *filt_off,
 cudaError_t launch_rank_finalize(const int32_t *cnt, long long b, int strategy, int32_t *ranks, cudaStream_t st);
 cudaError_t launch_rank_accumulate(const int32_t *cnt, long long b, int32_t *counts, cudaStream_t st);  // counts += cnt
 
+// kge_rank_rel.cu: the relation side (KGE_SIDE_P).  Candidates are rows of rel (the relation table, or RotatE's rotation
+// table) through p.cand_ids / p.cand_begin; each query's s and o rows are those of triples[i] in p.ent; p.qpos as
+// prepared by launch_rank_prepare; p.qvec / p.qaux are not read.  Same counter and p.scores contract as
+// launch_rank_count / launch_rank_filter_n.
+cudaError_t launch_rank_rel_count(const RankParams &p, const float *rel, const int32_t *triples, int32_t *cnt, cudaStream_t st);
+cudaError_t launch_rank_rel_filter(const RankParams &p, const float *rel, const int32_t *triples, const long long *filt_off,
+                                   const int32_t *filt_idx, long long n_pairs, int32_t *cnt, int sm_count, cudaStream_t st);
+
 // kge_topk.cu: running top-k per query over chunks of candidate scores (ordering contract: see the file)
 struct TopkSelectParams {
     const float *scores;                 // [b, ld]: this chunk's scores in columns [0, n)

@@ -3,7 +3,7 @@
 * DataIndexer  -- label <-> int32 id mapping with the reference's first-seen order
   (ampligraph/datasets/data_indexer.py:373-428: scan rows, subject then object for
   entities; predicates separately), unknown labels dropped on lookup (:525-542).
-* FilterIndex  -- known-true entities per (p,o) / (s,p) as CSR, built ONCE, replacing
+* FilterIndex  -- known-true entities per (p,o) / (s,p) (and relations per (s,o)) as CSR, built ONCE, replacing
   the per-batch pandas groupby/reindex + tf.ragged.constant of
   ampligraph/datasets/graph_data_loader.py:287-350, :382-439, :501-521.
 """
@@ -78,13 +78,16 @@ class DataIndexer:
 
 
 class FilterIndex:
-    """CSR of known-true subjects per (p,o) and objects per (s,p) over a set of indexed triples."""
+    """CSR of known-true subjects per (p,o) and objects per (s,p) over a set of indexed triples; relations per (s,o)
+    are grouped on the first 'p' lookup, so callers that rank entities only never pay for them."""
 
     def __init__(self, indexed_triples, n_ent):
         t = np.unique(np.asarray(indexed_triples, dtype=np.int64).reshape(-1, 3), axis=0)
         self.n_ent = int(n_ent)
         self._sub = self._group(t[:, 1] * self.n_ent + t[:, 2], t[:, 0])  # (p,o) -> subjects
         self._obj = self._group(t[:, 1] * self.n_ent + t[:, 0], t[:, 2])  # (s,p) -> objects
+        self._t = t
+        self._rel = None  # (s,o) -> relations, built by the first 'p' lookup
 
     @staticmethod
     def _group(keys, vals):
@@ -93,12 +96,18 @@ class FilterIndex:
 
     def lookup(self, triples, side, position_of=None):
         """-> (offsets int64 [b+1], ids int32 [nnz]) for a batch of indexed test triples.
-        position_of: optional int array mapping entity id -> candidate position (or -1) when an
-        entities_subset is used (the mapping_dict of AbstractScoringLayer.py:266-275)."""
+        side: 's' (known subjects), 'o' (known objects) or 'p' (known relations of each (s, o)).
+        position_of: optional int array mapping entity id (relation id for 'p') -> candidate position (or -1) when a
+        subset of candidates is used (the mapping_dict of AbstractScoringLayer.py:266-275)."""
         t = np.asarray(triples, dtype=np.int64)
         if side == "s":
             keys, vals = self._sub
             q = t[:, 1] * self.n_ent + t[:, 2]
+        elif side == "p":
+            if self._rel is None:
+                self._rel = self._group(self._t[:, 0] * self.n_ent + self._t[:, 2], self._t[:, 1])
+            keys, vals = self._rel
+            q = t[:, 0] * self.n_ent + t[:, 2]
         else:
             keys, vals = self._obj
             q = t[:, 1] * self.n_ent + t[:, 0]

@@ -6,7 +6,8 @@
   one kge_topk call (csrc/kge_topk.cu): the candidates are scored on the device by the exact ranking chain and only the
   top_n leave it.  Relation completion scores the R completed triples with the kernel predict uses and orders them
   with kge_select_topk.
-* query_topn_batch  -- extension: many (s, p, ?) or (?, p, o) queries in one call, optionally filtered like evaluate.
+* query_topn_batch  -- extension: many (s, p, ?), (?, p, o) or (s, ?, o) queries in one call, optionally filtered like
+  evaluate.  Relation prediction (s, ?, o) is one kge_topk call on the relation side (csrc/kge_rank_rel.cu).
 * find_nearest_neighbours -- discovery.find_nearest_neighbours (discovery.py:1171-1244): the n_neighbors nearest
   entities of each given entity in embedding space, one kge_knn call per batch of queries instead of sklearn
   NearestNeighbors on the host.
@@ -100,7 +101,9 @@ def query_topn(model, top_n=10, head=None, relation=None, tail=None, ents_to_con
     Returns (X, S): X [n, 3] the completed triples (labels), S [n] their fp32 scores, n = min(top_n, candidates); as in
     the reference (:1165, np.squeeze) a single result comes back as X [3] and a scalar score.  Known-true triples are
     not filtered out.  Entity-completion scores are those of the ranking kernels (kge_corruption_scores), which agree
-    with model.predict to fp32 rounding; relation-completion scores are model.predict's bit for bit."""
+    with model.predict to fp32 rounding; relation-completion scores are model.predict's bit for bit.  The batched
+    relation prediction, query_topn_batch(side='p'), scores with the canonical triple score of the ranking kernels
+    instead: its scores agree with these to about 1e-4 relative, so the two may order near-ties differently."""
     eng = _check_fitted(model)
     if sum(x is None for x in (head, relation, tail)) != 1:  # :1076-1079
         raise _error("Exactly one of `head`, `relation` or `tail` arguments must be None.")
@@ -159,43 +162,57 @@ def query_topn(model, top_n=10, head=None, relation=None, tail=None, ents_to_con
     return X, S
 
 
-def query_topn_batch(model, X, side="o", top_n=10, use_filter=False, ents_to_consider=None):
-    """Extension (no reference counterpart): the top_n entities completing each triple of X on `side` -- 'o' answers
-    (s, p, ?), 's' answers (?, p, o).  X holds raw triples (labels); the `side` column is ignored (any value).
+def query_topn_batch(model, X, side="o", top_n=10, use_filter=False, ents_to_consider=None, rels_to_consider=None):
+    """Extension (no reference counterpart): the top_n completions of each triple of X on `side` -- 'o' answers
+    (s, p, ?), 's' answers (?, p, o) (entities), 'p' answers (s, ?, o) (relations).  X holds raw triples (labels); the
+    `side` column is ignored (any value).
 
     use_filter: as in evaluate -- a dict of datasets, or True for X itself; the known-true completions are excluded
-    (a (s, p, o) in a dataset removes o from the answers to (s, p, ?) and s from those to (?, p, o)).
-    ents_to_consider: candidate entities (default: all).
+    (a (s, p, o) in a dataset removes o from the answers to (s, p, ?), s from those to (?, p, o) and p from those to
+    (s, ?, o)).
+    ents_to_consider: candidate entities of side 's' / 'o'; rels_to_consider: candidate relations of side 'p' (default:
+    all).
     Returns (labels [n, top_n] object array, scores [n, top_n] fp32), sorted per row; rows with fewer than top_n
     eligible candidates end in None / -inf.  Every label of the other two columns must be known to the model.
+    Relation scores are the canonical triple scores of the ranking kernels (see query_topn for how they relate to
+    model.predict).
 
     Under torchrun with data-parallel training the tables are replicated, so every rank answers its calls locally."""
+    if side not in ("s", "o", "p"):
+        raise _error("`side` must be 's', 'o' or 'p', got {!r}".format(side))
+    if side == "p" and ents_to_consider is not None:
+        raise _error("`ents_to_consider` does not apply to side 'p' (the candidates are relations): use `rels_to_consider`.")
+    if side != "p" and rels_to_consider is not None:
+        raise _error("`rels_to_consider` applies to side 'p' only (the candidates of side {!r} are entities).".format(side))
     eng = _check_fitted(model)
-    if side not in ("s", "o"):
-        raise _error("`side` must be 's' or 'o', got {!r}".format(side))
     if int(top_n) < 1:
         raise _error("`top_n` must be >= 1")
     X = as_triple_array(X)
     if X.ndim != 2 or X.shape[1] < 3:
         raise _error("X must be an array of triples")
     n = len(X)
-    keep_col = 0 if side == "o" else 2
     q = np.zeros((n, 3), np.int64)
-    q[:, keep_col] = _ids(model, X[:, keep_col], "e")
-    q[:, 1] = _ids(model, X[:, 1], "r")
-    unseen = (q[:, keep_col] < 0) | (q[:, 1] < 0)
+    known = [(0, "e"), (2, "e")] if side == "p" else [(0 if side == "o" else 2, "e"), (1, "r")]
+    for col, kind in known:
+        q[:, col] = _ids(model, X[:, col], kind)
+    unseen = np.zeros(n, bool)
+    for col, _ in known:
+        unseen |= q[:, col] < 0
     if unseen.any():
         raise _error("{} queries contain entities or relations not seen by the model".format(int(unseen.sum())))
 
-    cand, n_cand, position_of = None, _count(model, "e"), None
-    if ents_to_consider is not None:
-        if not isinstance(ents_to_consider, (list, np.ndarray)):
-            raise _error("`ents_to_consider` must be a list or numpy array.")
-        sub = _ids(model, ents_to_consider, "e")
+    kind = "r" if side == "p" else "e"
+    consider, name, what = (rels_to_consider, "rels_to_consider", "Relations") if side == "p" else \
+        (ents_to_consider, "ents_to_consider", "Entities")
+    cand, n_cand, position_of = None, _count(model, kind), None
+    if consider is not None:
+        if not isinstance(consider, (list, np.ndarray)):
+            raise _error("`{}` must be a list or numpy array.".format(name))
+        sub = _ids(model, consider, kind)
         if (sub < 0).any():
-            raise _error("Entities in `ents_to_consider` have not been seen by the model.")
+            raise _error("{} in `{}` have not been seen by the model.".format(what, name))
         cand, n_cand = _dev(eng, sub, np.int32), len(sub)
-        position_of = np.full(eng.n_ent, -1, np.int64)
+        position_of = np.full(eng.n_rel if side == "p" else eng.n_ent, -1, np.int64)
         position_of[sub] = np.arange(len(sub))
     findex = None
     if isinstance(use_filter, dict) or use_filter is True:
@@ -212,7 +229,7 @@ def query_topn_batch(model, X, side="o", top_n=10, use_filter=False, ents_to_con
             o_np, i_np = findex.lookup(qb, side, position_of)
             off, idx = _dev(eng, o_np, np.int64), _dev(eng, i_np, np.int32)
         ids, val = eng.topk(_dev(eng, qb, np.int32), side, int(top_n), off, idx, cand_ids=cand, n_cand=n_cand)
-        labels[start:start + len(qb)] = _labels(model, ids.cpu().numpy(), "e")
+        labels[start:start + len(qb)] = _labels(model, ids.cpu().numpy(), kind)
         scores[start:start + len(qb)] = val.cpu().numpy()
     return labels, scores
 

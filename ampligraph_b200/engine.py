@@ -482,6 +482,13 @@ class KGEEngine:
         self.launches += 2 if self.scoring_type == "RotatE" else 1
         return out
 
+    def _n_cand(self, side, cand_ids, cand_begin):
+        """The default candidate count of a ranking / top-k call: every row from cand_begin on of the table `side`
+        replaces from (relation rows for 'p', entity rows otherwise), or the length of cand_ids."""
+        if cand_ids is not None:
+            return cand_ids.numel()
+        return (self.n_rel if side == "p" else self.n_ent) - cand_begin
+
     def rank_workspace(self, b, n_cand):
         """The caller-owned scratch kge_rank needs (kge_rank_workspace_bytes): one cached torch buffer, grown on demand.
         Growing frees the old buffer through torch's stream-ordered caching allocator, so no synchronisation is needed."""
@@ -498,7 +505,8 @@ class KGEEngine:
     @_traced("kge.rank")
     def rank(self, triples, side, strategy="worst", filt_off=None, filt_idx=None, cand_ids=None, cand_begin=0,
              n_cand=None, out=None, counts=None):
-        """get_ranks for one side.  Default: returns/accumulates int32 rank counts in `out` (caller adds 1).
+        """get_ranks for one side ('s', 'o', or 'p': relation prediction, candidates are relation ids / rows).  Default:
+        returns/accumulates int32 rank counts in `out` (caller adds 1).
         counts=[b,3] int32: accumulate the RAW counters {greater, equal, filtered} there instead (candidate
         partitions must do this and call finalize_ranks once: 'middle' is not additive over partitions)."""
         assert triples.dtype == torch.int32 and triples.is_cuda and triples.is_contiguous()
@@ -506,7 +514,7 @@ class KGEEngine:
         if out is None and counts is None:
             out = torch.zeros(b, dtype=torch.int32, device=self.device)
         if n_cand is None:
-            n_cand = cand_ids.numel() if cand_ids is not None else self.n_ent - cand_begin
+            n_cand = self._n_cand(side, cand_ids, cand_begin)
         n_filt = int(filt_idx.numel()) if filt_idx is not None else 0
         ws, ws_bytes = self.rank_workspace(b, n_cand)
         _lib.check(self.lib.kge_rank(self.h, _lib.SIDES[side], _lib.STRATEGIES[strategy], _ptr(self.ent), _ptr(self.rel),
@@ -529,7 +537,7 @@ class KGEEngine:
         """Diagnostic (kge_rank_filter_probe): (approximate tensor-core scores, assumed error bound), both [b, n_cand]."""
         b = triples.shape[0]
         if n_cand is None:
-            n_cand = cand_ids.numel() if cand_ids is not None else self.n_ent - cand_begin
+            n_cand = self._n_cand(side, cand_ids, cand_begin)
         approx = torch.empty((b, int(n_cand)), dtype=torch.float32, device=self.device)
         delta = torch.empty_like(approx)
         ws, ws_bytes = self.rank_workspace(b, n_cand)
@@ -543,7 +551,7 @@ class KGEEngine:
         assert triples.dtype == torch.int32 and triples.is_cuda and triples.is_contiguous()
         b = triples.shape[0]
         if n_cand is None:
-            n_cand = cand_ids.numel() if cand_ids is not None else self.n_ent - cand_begin
+            n_cand = self._n_cand(side, cand_ids, cand_begin)
         out = torch.empty((b, int(n_cand)), dtype=torch.float32, device=self.device)
         ws, ws_bytes = self.rank_workspace(b, n_cand)
         _lib.check(self.lib.kge_corruption_scores(self.h, _lib.SIDES[side], _ptr(self.ent), _ptr(self.rel), _ptr(triples), b,
@@ -561,7 +569,7 @@ class KGEEngine:
         assert triples.dtype == torch.int32 and triples.is_cuda and triples.is_contiguous()
         b = triples.shape[0]
         if n_cand is None:
-            n_cand = cand_ids.numel() if cand_ids is not None else self.n_ent - cand_begin
+            n_cand = self._n_cand(side, cand_ids, cand_begin)
         n_filt = int(filt_idx.numel()) if filt_idx is not None else 0
         ids = torch.empty((b, max(int(k), 0)), dtype=torch.int32, device=self.device)
         scores = torch.empty((b, max(int(k), 0)), dtype=torch.float32, device=self.device)

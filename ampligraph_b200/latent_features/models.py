@@ -499,16 +499,21 @@ class ScoringBasedEmbeddingModel:
     def evaluate(self, x=None, batch_size=10, verbose=True, use_filter=False, corrupt_side="s,o",
                  entities_subset=None, ranking_strategy="worst", callbacks=None, dataset_type="test", _filter_index=None):
         """evaluate (:1516-1692) -> int32 ranks [n, 2] for 's,o', [n, 1] otherwise.
-        `batch_size` only lower-bounds the device chunk: results do not depend on it.  _filter_index: the FilterIndex
-        that use_filter would build (_build_filter), when the caller keeps one across calls (fit's validations)."""
-        assert corrupt_side in ["s", "o", "s,o", "s+o"], "Invalid value for corrupt_side"
+        corrupt_side='p' (extension: relation prediction) ranks each triple's relation among all relations for its
+        (s, o), by the same count, ranking_strategy and use_filter rules (a known (s, r, o) removes r); entities_subset
+        does not apply to it.  `batch_size` only lower-bounds the device chunk: results do not depend on it.
+        _filter_index: the FilterIndex that use_filter would build (_build_filter), when the caller keeps one across calls
+        (fit's validations)."""
+        assert corrupt_side in ["s", "o", "s,o", "s+o", "p"], "Invalid value for corrupt_side"
         assert ranking_strategy in ["best", "middle", "worst"], "Invalid value for ranking_strategy"
+        if corrupt_side == "p" and entities_subset is not None:
+            raise ValueError("entities_subset does not apply to corrupt_side='p': the candidates are the relations")
         if not self.is_fitted:
             raise RuntimeError("Model has not been fitted.")
         eng = self.engine
         t = self._index(x)
         n = len(t)
-        sides = [s for s in ("s", "o") if s in corrupt_side]
+        sides = ["p"] if corrupt_side == "p" else [s for s in ("s", "o") if s in corrupt_side]
         # candidates: all entities or a subset (:1634-1643)
         cand_ids, position_of = None, None
         if entities_subset is not None:
@@ -528,9 +533,10 @@ class ScoringBasedEmbeddingModel:
                 if findex is not None:
                     o_np, i_np = findex.lookup(tb, side, position_of)
                     off, idx = self._to_dev(o_np, np.int64), self._to_dev(i_np, np.int32)
-                if self._world() > 1 and cand_ids is None:
+                if self._world() > 1 and cand_ids is None and side != "p":
                     # row-sharded candidates: RAW counters summed over ranks, tie strategy applied once ('middle' is not
-                    # additive over partitions, AbstractScoringLayer.py:232-244)
+                    # additive over partitions, AbstractScoringLayer.py:232-244); the relation side runs on each rank
+                    # locally (the relation table is replicated)
                     from ..parallel import allreduce_sum_, row_shard
                     lo, hi = row_shard(self.max_ent_size, self._world(), self._rank())
                     cnt = torch.zeros((len(tb), 3), dtype=torch.int32, device=eng.device)

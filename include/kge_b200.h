@@ -73,7 +73,9 @@ enum kge_optimizer {
     KGE_OPT_ADADELTA = 4,
     KGE_OPT_ADAMAX = 5
 };
-enum kge_side { KGE_SIDE_S = 0, KGE_SIDE_O = 1 };
+/* the element of (s, p, o) a ranking / top-k call replaces by its candidates: subject or object (entity rows), or the
+ * relation (KGE_SIDE_P, relation prediction: candidates are relation rows, see kge_rank) */
+enum kge_side { KGE_SIDE_S = 0, KGE_SIDE_O = 1, KGE_SIDE_P = 2 };
 enum kge_rank_strategy { KGE_RANK_WORST = 0, KGE_RANK_BEST = 1, KGE_RANK_MIDDLE = 2 };
 /* how kge_rank scores the candidates of DistMult / ComplEx / HolE (the bilinear models, a [b,K]x[K,E] contraction):
  * AUTO = tensor cores (wgmma, split-bf16 operands) decide every (query, candidate) pair whose approximate score is
@@ -397,7 +399,16 @@ int kge_peer_barrier(kge_handle *h, int32_t world, int32_t rank, uint32_t *const
  *                 kge_rank_finalize once: 'middle' is best + ceil(equal/2) (:232-244), which is not
  *                 additive over partitions; 'worst'/'best' are, so ranks_dev may be accumulated directly.
  *   workspace_dev caller-owned scratch of at least kge_rank_workspace_bytes(h, b, n_cand) bytes, 1024-byte
- *                 aligned; contents are undefined afterwards.  The library never allocates or synchronises. */
+ *                 aligned; contents are undefined afterwards.  The library never allocates or synchronises.
+ * side = KGE_SIDE_P (relation prediction, (s, ?, o)): the candidates are RELATION rows -- cand_ids_dev holds relation
+ *   ids, or the candidates are rows [cand_begin, cand_begin+n_cand) of the relation table (a range beyond n_rel is
+ *   refused); filter entries are candidate positions as above.  Column 1 of triples_dev is the positive relation, scored
+ *   whether or not it is among the candidates.  A candidate r's score is the canonical triple score of (s, r, o)
+ *   (oracle/kge_oracle.c: kgeo_score_triple, the value quantised as the positive's score, bit for bit): the object-side
+ *   chain of TransE / DistMult / RotatE with the query vector built from (s, r), the subject-side chain of ComplEx /
+ *   HolE with the query vector built from (r, o).  Counting, strategies, filter and counts_dev are those of the entity
+ *   sides.  Every rank_mode runs the exact chain: each pair has its own query vector, so the tensor-core filter has no
+ *   per-query operand. */
 int kge_rank(kge_handle *h, int32_t side, int32_t strategy, const float *ent_dev,
              const float *rel_dev, const int32_t *triples_dev, int64_t b,
              const int32_t *cand_ids_dev, int64_t cand_begin, int64_t n_cand,
@@ -408,7 +419,8 @@ int kge_rank(kge_handle *h, int32_t side, int32_t strategy, const float *ent_dev
 /* kge_rank against THIS rank's row shard of a sharded table: query rows are fetched from whichever
  * rank owns them, candidates are the local shard's rows, filter ids are GLOBAL entity ids (those
  * outside the shard are ignored, AbstractScoringLayer.py:280-288).  Sum counts_dev over ranks
- * (int32 all-reduce) and finalize once (ScoringBasedEmbeddingModel.py:1449-1452). */
+ * (int32 all-reduce) and finalize once (ScoringBasedEmbeddingModel.py:1449-1452).  KGE_SIDE_P is refused
+ * (KGE_ERR_INVALID_ARGUMENT): the relation table is replicated, never sharded -- rank relations with kge_rank. */
 int kge_rank_sharded(kge_handle *h, const kge_shard_map *map, int32_t rank, int32_t side, int32_t strategy,
                      const float *rel_dev, const int32_t *triples_dev, int64_t b,
                      const int64_t *filt_off_dev, const int32_t *filt_idx_dev, int64_t n_filt,
@@ -422,7 +434,8 @@ int kge_rank_finalize(kge_handle *h, const int32_t *counts_dev /*[b,3]*/, int64_
 /* _get_subject_corruption_scores / _get_object_corruption_scores (TransE.py:56-114, DistMult.py:51-99,
  * ComplEx.py:65-151, HolE.py:47-89, RotatE.py:107-217): the [b, n_cand] fp32 score matrix of every candidate
  * substituted on `side`, canonical summation order (the scores kge_rank quantises).  Same candidate
- * addressing and workspace contract as kge_rank. */
+ * addressing and workspace contract as kge_rank; KGE_SIDE_P gives the canonical triple score of every (s, r, o) with
+ * r a candidate relation (the relation column of triples_dev is not read). */
 int kge_corruption_scores(kge_handle *h, int32_t side, const float *ent_dev, const float *rel_dev,
                           const int32_t *triples_dev, int64_t b, const int32_t *cand_ids_dev,
                           int64_t cand_begin, int64_t n_cand, float *scores_dev /*[b, n_cand]*/,
@@ -431,7 +444,7 @@ int kge_corruption_scores(kge_handle *h, int32_t side, const float *ent_dev, con
 /* Diagnostic for KGE_RANK_MODE_AUTO (used by the tests that pin its error bound): the APPROXIMATE scores of the
  * tensor-core filter pass and the error bound delta the filter assumes for each pair, both [b, n_cand] fp32, in the
  * units of kge_corruption_scores.  The filter is sound iff |approx - kge_corruption_scores| <= delta everywhere.
- * KGE_ERR_UNSUPPORTED when the filter does not apply (model, mode or size). */
+ * KGE_ERR_UNSUPPORTED when the filter does not apply (model, mode, size, or KGE_SIDE_P). */
 int kge_rank_filter_probe(kge_handle *h, int32_t side, const float *ent_dev, const float *rel_dev,
                           const int32_t *triples_dev, int64_t b, const int32_t *cand_ids_dev, int64_t cand_begin,
                           int64_t n_cand, float *approx_dev, float *delta_dev, void *workspace_dev,
@@ -439,12 +452,14 @@ int kge_rank_filter_probe(kge_handle *h, int32_t side, const float *ent_dev, con
 
 /* bytes of caller-owned scratch kge_rank / kge_rank_sharded / kge_corruption_scores need for b queries
  * against n_cand candidates (query vectors, counters and -- in KGE_RANK_MODE_AUTO for the bilinear models --
- * the split-bf16 copies of the candidate rows and query vectors the tensor-core pass reads). */
+ * the split-bf16 copies of the candidate rows and query vectors the tensor-core pass reads).  The size takes no side:
+ * it is an upper bound for KGE_SIDE_P too, which uses the same query-side buffers and never the tensor-core part. */
 int64_t kge_rank_workspace_bytes(const kge_handle *h, int64_t b, int64_t n_cand);
 
 /* discovery.query_topn (discovery.py:985-1168), batched: the k best candidates on `side` for each of b queries.
  * Candidates, cand_ids / cand_begin / n_cand and the filter CSR (candidate POSITIONS; those are excluded) follow
- * kge_rank.  Every id in triples_dev must be valid; the column of `side` does not affect the result.
+ * kge_rank, KGE_SIDE_P (the k best relations of each (s, ?, o), candidates relation rows) included.  Every id in
+ * triples_dev must be valid; the column of `side` does not affect the result.
  * ids_dev/scores_dev [b,k]: sorted by (score desc, position asc), NaN first; scores are kge_corruption_scores' bit
  * for bit; rows with fewer than k eligible candidates are padded with id -1, score -inf.
  * The reference scores every completed triple on the host and sorts them all (:1143-1168); here the candidates are
@@ -456,7 +471,8 @@ int kge_topk(kge_handle *h, int32_t side, const float *ent_dev, const float *rel
              const int64_t *filt_off_dev, const int32_t *filt_idx_dev, int64_t n_filt, int32_t k,
              int32_t *ids_dev, float *scores_dev, void *workspace_dev, int64_t workspace_bytes, void *stream);
 /* bytes of scratch kge_topk needs: query vectors, one [b, C] score chunk (C sized to half the L2, or
- * KGE_B200_TOPK_CHUNK) and the double-buffered running lists (12 bytes per slot, 2 * b * k slots). */
+ * KGE_B200_TOPK_CHUNK) and the double-buffered running lists (12 bytes per slot, 2 * b * k slots).  The size takes no
+ * side: it is an upper bound for KGE_SIDE_P too. */
 int64_t kge_topk_workspace_bytes(const kge_handle *h, int64_t b, int64_t n_cand, int32_t k);
 
 /* the same selection over a caller's [b, n] score matrix (positions out); relation completion uses it

@@ -1527,3 +1527,114 @@ extern "C" int kge_graph_counts(const int64_t *offsets_dev, const int32_t *nbr_d
              "kge_graph_counts");
     return KGE_OK;
 }
+
+// ---- 1vsAll training (kge_train_1vsall.cu) ------------------------------------------------------------------
+
+// Carve-up of the workspace of a 1vsAll step of B positives: both sides' query vectors (and the quantised positive
+// scores launch_rank_prepare also writes), then the per-side scratch, reused by the second side.
+struct OneVsAllWorkspace {
+    float *qs, *qo;
+    int32_t *qpos;
+    float *pm, *pz, *lt, *row_m, *row_inv, *pgq;
+    int nsplit;
+};
+static OneVsAllWorkspace carve_one_vs_all(const kge_handle *h, int64_t B, Carve &c)
+{
+    OneVsAllWorkspace w;
+    w.nsplit = one_vs_all_splits(B, h->cfg.n_ent);
+    const size_t rows = (size_t)B * h->L.ld * sizeof(float), col = (size_t)B * sizeof(float), ns = (size_t)w.nsplit;
+    w.qs = c.take<float>(rows, 16);
+    w.qo = c.take<float>(rows, 16);
+    w.qpos = c.take<int32_t>(col, 16);
+    w.pm = c.take<float>(ns * col, 16);
+    w.pz = c.take<float>(ns * col, 16);
+    w.lt = c.take<float>(col, 16);
+    w.row_m = c.take<float>(col, 16);
+    w.row_inv = c.take<float>(col, 16);
+    w.pgq = c.take<float>(ns * rows, 16);
+    return w;
+}
+
+extern "C" int64_t kge_one_vs_all_workspace_bytes(const kge_handle *h, int64_t B)
+{
+    if (!h || B < 0) return 0;
+    Carve c(nullptr);
+    carve_one_vs_all(h, B, c);
+    return (int64_t)c.at;
+}
+
+extern "C" int kge_one_vs_all_step(kge_handle *h, int32_t sides, int32_t loss_reduction, const float *ent_dev,
+                                   const float *rel_dev, float *grad_ent_dev, float *grad_rel_dev,
+                                   const int32_t *triples_dev, int64_t B, uint64_t step, double *loss_dev, void *ws_dev,
+                                   int64_t ws_bytes, void *stream)
+{
+    KGE_CHECK_HANDLE(h, "kge_one_vs_all_step");
+    const int model = h->cfg.scoring;
+    if (model != KGE_DISTMULT && model != KGE_COMPLEX && model != KGE_HOLE)
+        return fail(KGE_ERR_UNSUPPORTED, "kge_one_vs_all_step: 1vsAll training is implemented for DistMult, ComplEx and HolE "
+                                         "(inner-product scores); not for scoring type %d", model);
+    if (sides < KGE_ONE_VS_ALL_S || sides > (KGE_ONE_VS_ALL_S | KGE_ONE_VS_ALL_O))
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_step: sides must be a non-empty set of KGE_ONE_VS_ALL_S | "
+                                              "KGE_ONE_VS_ALL_O, got %d", sides);
+    if (loss_reduction != KGE_REDUCE_SUM && loss_reduction != KGE_REDUCE_MEAN)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "Invalid value for reduction!");
+    if (h->sum_pending)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_step: the replaced-row sum of a deferred step is pending "
+                                              "(kge_optimizer_step_deferred first)");
+    if (h->cfg.n_ent < 2) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_step: needs n_ent >= 2");
+    if ((long long)one_vs_all_smem_bytes(h->L.ld) > h->max_smem)
+        return fail(KGE_ERR_UNSUPPORTED, "kge_one_vs_all_step: rows of %d floats exceed the shared-memory tiles of the 1vsAll "
+                                         "kernels (%d B)", h->L.ld, h->max_smem);
+    if (B < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_step: B < 0");
+    if (B == 0) return KGE_OK;
+    if (!ent_dev || !rel_dev || !grad_ent_dev || !grad_rel_dev || !triples_dev)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_step: null table, gradient or triples");
+    const int64_t need = kge_one_vs_all_workspace_bytes(h, B);
+    if (!ws_dev || ws_bytes < need || ((uintptr_t)ws_dev & 15))
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_step: a 16-byte aligned workspace of %lld bytes is needed "
+                                              "(kge_one_vs_all_workspace_bytes), got %lld", (long long)need,
+                    (long long)(ws_dev ? ws_bytes : 0));
+    cudaStream_t st = (cudaStream_t)stream;
+    Carve c(ws_dev);
+    const OneVsAllWorkspace w = carve_one_vs_all(h, B, c);
+    ShardView sv;
+    memset(&sv, 0, sizeof(sv));
+    KGE_CUDA(launch_rank_prepare(h->L, sv, ent_dev, rel_dev, nullptr, triples_dev, B, h->score_scale, w.qs, w.qo, nullptr,
+                                 w.qpos, st),
+             "kge_one_vs_all_step (query vectors)");
+    const int stamp = kge_step_stamp(step);
+    // every entity row is a candidate of the step: all of them count as looked up (stamped only while the entity
+    // buffer is set, like kge_train_step); the relation rows of the batch are stamped by the chain pass
+    if (h->stamp_ent) KGE_CUDA(launch_one_vs_all_stamps(h->stamp_ent, h->cfg.n_ent, stamp, st), "kge_one_vs_all_step (stamps)");
+    OneVsAllSide s;
+    memset(&s, 0, sizeof(s));
+    s.ent = ent_dev;
+    s.rel = rel_dev;
+    s.grad_ent = grad_ent_dev;
+    s.grad_rel = grad_rel_dev;
+    s.triples = triples_dev;
+    s.B = B;
+    s.n_ent = h->cfg.n_ent;
+    s.kp = h->L.kp;
+    s.ld = h->L.ld;
+    s.nsplit = w.nsplit;
+    s.scale = h->score_scale;
+    s.w = loss_reduction == KGE_REDUCE_MEAN ? (float)(1.0 / (double)(h->cfg.n_ent - 1)) : 1.f;
+    s.loss = loss_dev;
+    s.stamp = stamp;
+    s.stamp_rel = h->stamp_ent ? h->stamp_rel : nullptr;
+    s.pm = w.pm;
+    s.pz = w.pz;
+    s.lt = w.lt;
+    s.row_m = w.row_m;
+    s.row_inv = w.row_inv;
+    s.pgq = w.pgq;
+    for (int side = KGE_SIDE_S; side <= KGE_SIDE_O; ++side) {
+        if (!(sides & (side == KGE_SIDE_S ? KGE_ONE_VS_ALL_S : KGE_ONE_VS_ALL_O))) continue;
+        s.side = side;
+        s.col = side == KGE_SIDE_S ? 0 : 2;
+        s.q = side == KGE_SIDE_S ? w.qs : w.qo;
+        KGE_CUDA(launch_one_vs_all_side(s, h->L.halves, st), "kge_one_vs_all_step");
+    }
+    return KGE_OK;
+}

@@ -87,6 +87,27 @@ cudaError_t launch_rotation_table(const float *rel, float *rot, long long n_rel,
 cudaError_t launch_corruptions(const int32_t *triples, long long B, int eta, unsigned long long seed,
                                unsigned long long step, unsigned n_ent, int32_t *out, cudaStream_t st);
 
+// kge_train_1vsall.cu: one side of a 1vsAll multiclass-NLL step of the trilinear models (kge_one_vs_all_step)
+struct OneVsAllSide {
+    const float *q;          // [B, ld] query vectors of the side (launch_rank_prepare: qvec_s for side s, qvec_o for o)
+    const float *ent, *rel;  // [n_ent, ld], [n_rel, ld]
+    float *grad_ent, *grad_rel;
+    const int32_t *triples;  // [B, 3]
+    long long B, n_ent;
+    int side, col;           // KGE_SIDE_S / KGE_SIDE_O; the triple column of the positive's own entity (0 / 2)
+    int kp, ld, nsplit;      // nsplit = one_vs_all_splits(B, n_ent) entity ranges per query tile
+    float scale, w;          // HolE's score scale (1 otherwise); weight of a negative's exp (1 or 1 / (n_ent - 1))
+    double *loss;            // += sum of the row losses, or nullptr
+    int stamp;
+    int *stamp_rel;          // lazy-optimizer stamps of the relation rows, or nullptr
+    // workspace: [nsplit, B] partial maxima and sums; [B] l_t, max and 1 / D per row; [nsplit, B, ld] partial Gq rows
+    float *pm, *pz, *lt, *row_m, *row_inv, *pgq;
+};
+int one_vs_all_splits(long long B, long long n_ent);
+size_t one_vs_all_smem_bytes(int ld);  // dynamic shared memory of the dQ and dX passes
+cudaError_t launch_one_vs_all_side(const OneVsAllSide &s, int halves, cudaStream_t st);
+cudaError_t launch_one_vs_all_stamps(int *stamp_ent, long long n_ent, int stamp, cudaStream_t st);
+
 // kge_misc.cu
 cudaError_t launch_score_triples(const Layout &L, int nit, const float *ent, const float *rel_or_rot,
                                  const int32_t *triples, long long n, float scale, float *out, int sm_count,

@@ -1,0 +1,430 @@
+// kge_train_1vsall.cu -- 1vsAll training of the trilinear models (DistMult / ComplEx / HolE): the multiclass NLL of
+// every positive against EVERY entity on one side (kge_one_vs_all_step; DESIGN.md 3.12).
+//
+// For a positive (s, p, o) and side o the logits are l_e = f(s, p, e) = scale * <x_e, q> over all entities e, with
+// q = Q1(s, p) the query vector of kge_rank_qvec_kernel (side s: l_e = f(e, p, o), q = Q0(p, o)); scale is HolE's, 1
+// otherwise.  Every logit is clipped to [-75, 75] (loss_functions.py:32-35) and the gradient is zero outside that range.
+// With t the positive's own entity, w = 1 (reduction sum) or 1 / (n_ent - 1) (mean) and m the row's largest clipped
+// logit:  D = w * sum_{e != t} exp(l_e - m) + exp(l_t - m),  loss = m + log(D) - l_t,
+//         dL/dl_e = in_e * (w_e * exp(l_e - m) / D - [e == t]),  w_t = 1, w_e = w otherwise.
+// Sum: logsumexp - l_t; mean: the reference's NLLMulticlass with the exp of the n_ent - 1 negatives averaged.
+//
+// Five passes per side, each a [B, ld] x [ld, n_ent]-shaped fp32 contraction on CUDA cores (FMA chains, no tensor
+// cores); every CTA works on tiles of 32 queries x 32 entities, staged column chunk by column chunk with cp.async:
+//   stats  (query tile x entity split): online max-subtracted (max, sum exp) of each row over its split, and l_t;
+//   merge  (one thread per row): combines the splits, the row loss -> *loss, m and 1 / D per row;
+//   dQ     (query tile x entity split): recomputes the logits, forms g, accumulates Gq = sum_e g_e x_e in shared memory
+//          and writes its split's partial rows once;
+//   dX     (entity tile, every query tile): recomputes the logits, accumulates sum_b g_be q_b in shared memory and adds
+//          it to each of its grad_ent rows once (one owner per row: no atomics, deterministic);
+//   chain  (one thread per row chunk): sums the split partials in order (scale included), and by linearity of f in the
+//          query row forms the gradient rows of the positive's kept rows -- side o: d/ds = Q0(p, Gq), d/dp of f(s, p, Gq);
+//          side s: d/do = Q1(Gq, p), d/dp of f(Gq, p, o) -- with the training kernels' own arithmetic
+//          (kge_train_common.cuh), added with red.global.add like theirs.
+// Every pass scores a (query, entity) pair with the same chain: one fma per column in ascending order, so the logits
+// of the three passes that form them are bit-identical.
+#include <math.h>
+
+#include "kge_train_common.cuh"
+
+namespace kge {
+
+constexpr int OVA_T = 32;                       // queries per query tile = entities per entity tile
+constexpr int OVA_DK = 32;                      // columns per staged chunk
+constexpr int OVA_LDS = OVA_DK + 4;             // padded shared row: the per-thread 128-bit reads are conflict free
+constexpr int OVA_THREADS = 256;
+constexpr int OVA_CHUNK = OVA_T * OVA_LDS;      // floats of one staged chunk of 32 rows
+constexpr int OVA_STAGE = 4 * OVA_CHUNK;        // two buffers of (query chunk, entity chunk)
+constexpr int OVA_GS = OVA_T * (OVA_T + 1);     // the g tile [query][entity], padded rows
+constexpr int OVA_TARGET_CTAS = 264;            // two CTAs on each of the H100's 132 SMs
+constexpr int OVA_MAX_SPLITS = 64;
+
+int one_vs_all_splits(long long B, long long n_ent)
+{
+    const long long n_qt = (B + OVA_T - 1) / OVA_T, n_et = (n_ent + OVA_T - 1) / OVA_T;
+    long long s = n_qt > 0 ? (OVA_TARGET_CTAS + n_qt - 1) / n_qt : 1;
+    if (s > OVA_MAX_SPLITS) s = OVA_MAX_SPLITS;
+    if (s > n_et) s = n_et;
+    return s < 1 ? 1 : (int)s;
+}
+
+size_t one_vs_all_smem_bytes(int ld) { return (OVA_STAGE + OVA_GS + (size_t)OVA_T * ld) * sizeof(float); }
+
+__device__ __forceinline__ void ova_cp16(float *smem, const float *gmem, bool valid)
+{
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(smem)), "l"(gmem), "r"(valid ? 16 : 0)
+                 : "memory");
+}
+__device__ __forceinline__ void ova_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void ova_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+// rows [r0, r0 + 32) x columns [c0, c0 + 32) of the [nrows, ld] matrix M -> dst (row stride OVA_LDS), zero past its ends
+__device__ __forceinline__ void ova_stage(float *dst, const float *M, long long r0, long long nrows, int ld, int c0, int tid)
+{
+    const int r = tid >> 3, c = (tid & 7) * 4;
+    const bool ok = r0 + r < nrows && c0 + c < ld;
+    ova_cp16(dst + r * OVA_LDS + c, ok ? M + (size_t)(r0 + r) * ld + c0 + c : M, ok);
+}
+
+__device__ __forceinline__ float4 ova_lds4(const float *p) { return *reinterpret_cast<const float4 *>(p); }
+__device__ __forceinline__ float ova_dot4(float4 a, float4 b, float acc)
+{
+    acc = __fmaf_rn(a.x, b.x, acc);
+    acc = __fmaf_rn(a.y, b.y, acc);
+    acc = __fmaf_rn(a.z, b.z, acc);
+    return __fmaf_rn(a.w, b.w, acc);
+}
+
+// acc[i][j] = <Q[q0 + 2 ty + i], X[e0 + tx + 16 j]> (ty = tid / 16, tx = tid % 16), zero for rows past nq / ne.
+// Ends with a barrier: the caller may reuse `stage` and read what other threads wrote before the call.
+__device__ __forceinline__ void ova_logits(const float *Q, long long q0, long long nq, const float *X, long long e0,
+                                           long long ne, int ld, float *stage, int tid, float acc[2][2])
+{
+    const int ty = tid >> 4, tx = tid & 15;
+    acc[0][0] = acc[0][1] = acc[1][0] = acc[1][1] = 0.f;
+    const int nchunk = (ld + OVA_DK - 1) / OVA_DK;
+    ova_stage(stage, Q, q0, nq, ld, 0, tid);
+    ova_stage(stage + OVA_CHUNK, X, e0, ne, ld, 0, tid);
+    ova_commit();
+    for (int c = 0; c < nchunk; ++c) {
+        const float *buf = stage + (c & 1) * 2 * OVA_CHUNK;
+        if (c + 1 < nchunk) {
+            float *nb = stage + ((c + 1) & 1) * 2 * OVA_CHUNK;
+            ova_stage(nb, Q, q0, nq, ld, (c + 1) * OVA_DK, tid);
+            ova_stage(nb + OVA_CHUNK, X, e0, ne, ld, (c + 1) * OVA_DK, tid);
+            ova_commit();
+            ova_wait<1>();
+        } else {
+            ova_wait<0>();
+        }
+        __syncthreads();
+        const float *qs = buf + 2 * ty * OVA_LDS, *xs = buf + OVA_CHUNK + tx * OVA_LDS;
+#pragma unroll
+        for (int k = 0; k < OVA_DK; k += 4) {
+            const float4 a0 = ova_lds4(qs + k), a1 = ova_lds4(qs + OVA_LDS + k);
+            const float4 b0 = ova_lds4(xs + k), b1 = ova_lds4(xs + 16 * OVA_LDS + k);
+            acc[0][0] = ova_dot4(a0, b0, acc[0][0]);
+            acc[0][1] = ova_dot4(a0, b1, acc[0][1]);
+            acc[1][0] = ova_dot4(a1, b0, acc[1][0]);
+            acc[1][1] = ova_dot4(a1, b1, acc[1][1]);
+        }
+        __syncthreads();
+    }
+}
+
+// acc_s[o][:] += sum_r G(o, r) M[r0 + r][:] over the 32 rows of M from r0 (G(o, r) = gs[o][r], or gs[r][o] when
+// TRANS); acc_s is [32, ld].  Thread (o = tid / 8, 4 columns) owns its part of acc_s.  Ends with a barrier.
+template <bool TRANS>
+__device__ __forceinline__ void ova_accumulate(float *acc_s, const float *gs, const float *M, long long r0, long long nrows,
+                                               int ld, float *stage, int tid)
+{
+    const int o = tid >> 3, c4 = (tid & 7) * 4;
+    const int nchunk = (ld + OVA_DK - 1) / OVA_DK;
+    ova_stage(stage, M, r0, nrows, ld, 0, tid);
+    ova_commit();
+    for (int c = 0; c < nchunk; ++c) {
+        const float *buf = stage + (c & 1) * OVA_CHUNK;
+        if (c + 1 < nchunk) {
+            ova_stage(stage + ((c + 1) & 1) * OVA_CHUNK, M, r0, nrows, ld, (c + 1) * OVA_DK, tid);
+            ova_commit();
+            ova_wait<1>();
+        } else {
+            ova_wait<0>();
+        }
+        __syncthreads();
+        const int col = c * OVA_DK + c4;
+        if (col < ld) {
+            float4 a = ova_lds4(acc_s + (size_t)o * ld + col);
+#pragma unroll 8
+            for (int r = 0; r < OVA_T; ++r) {
+                const float g = TRANS ? gs[r * (OVA_T + 1) + o] : gs[o * (OVA_T + 1) + r];
+                const float4 x = ova_lds4(buf + r * OVA_LDS + c4);
+                a.x = __fmaf_rn(g, x.x, a.x);
+                a.y = __fmaf_rn(g, x.y, a.y);
+                a.z = __fmaf_rn(g, x.z, a.z);
+                a.w = __fmaf_rn(g, x.w, a.w);
+            }
+            *reinterpret_cast<float4 *>(acc_s + (size_t)o * ld + col) = a;
+        }
+        __syncthreads();
+    }
+}
+
+__device__ __forceinline__ float ova_clip(float acc, float scale, bool &in)
+{
+    const float l = scale * acc;
+    in = l >= KGE_CLIP_LO && l <= KGE_CLIP_HI;
+    return fminf(fmaxf(l, KGE_CLIP_LO), KGE_CLIP_HI);
+}
+
+// dL/dl of entity e in a row with target t, max m, 1 / D = inv
+__device__ __forceinline__ float ova_grad(float acc, const OneVsAllSide &s, long long e, long long t, float m, float inv)
+{
+    bool in;
+    const float l = ova_clip(acc, s.scale, in);
+    if (!in) return 0.f;
+    const float p = expf(l - m) * inv;
+    return e == t ? p - 1.f : s.w * p;
+}
+
+__device__ __forceinline__ void ova_zero(float *a, int n, int tid)
+{
+    for (int i = tid * 4; i < n; i += OVA_THREADS * 4) *reinterpret_cast<float4 *>(a + i) = make_float4(0.f, 0.f, 0.f, 0.f);
+}
+
+// the entity-tile range [et0, et1) of split `split`
+__device__ __forceinline__ void ova_split_range(const OneVsAllSide &s, int split, long long &et0, long long &et1)
+{
+    const long long n_et = (s.n_ent + OVA_T - 1) / OVA_T;
+    et0 = split * n_et / s.nsplit;
+    et1 = (split + 1) * n_et / s.nsplit;
+}
+
+__global__ void __launch_bounds__(OVA_THREADS) kge_ova_stats_kernel(const OneVsAllSide s)
+{
+    extern __shared__ __align__(16) float ova_sm[];
+    const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15, split = blockIdx.y;
+    const long long q0 = (long long)blockIdx.x * OVA_T;
+    long long et0, et1;
+    ova_split_range(s, split, et0, et1);
+    long long tgt[2];
+    float m[2], z[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        const long long b = q0 + 2 * ty + i;
+        tgt[i] = b < s.B ? s.triples[3 * b + s.col] : -1;
+        m[i] = -INFINITY;
+        z[i] = 0.f;
+    }
+    for (long long et = et0; et < et1; ++et) {
+        const long long e0 = et * OVA_T;
+        float acc[2][2];
+        ova_logits(s.q, q0, s.B, s.ent, e0, s.n_ent, s.ld, ova_sm, tid, acc);
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+                const long long e = e0 + tx + 16 * j;
+                if (tgt[i] < 0 || e >= s.n_ent) continue;
+                bool in;
+                const float l = ova_clip(acc[i][j], s.scale, in);
+                if (e == tgt[i]) {  // the positive's own logit: counted in m, kept out of the sum
+                    const long long b = q0 + 2 * ty + i;
+                    s.lt[b] = l;
+                    const float mn = fmaxf(m[i], l);
+                    z[i] *= expf(m[i] - mn);
+                    m[i] = mn;
+                } else if (l > m[i]) {
+                    z[i] = __fmaf_rn(z[i], expf(m[i] - l), 1.f);
+                    m[i] = l;
+                } else {
+                    z[i] += expf(l - m[i]);
+                }
+            }
+    }
+    // the 16 threads of a query row are lanes of one half-warp
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+#pragma unroll
+        for (int o = 8; o > 0; o >>= 1) {
+            const float m2 = __shfl_xor_sync(0xffffffffu, m[i], o), z2 = __shfl_xor_sync(0xffffffffu, z[i], o);
+            const float mn = fmaxf(m[i], m2);
+            z[i] = mn == -INFINITY ? 0.f : z[i] * expf(m[i] - mn) + z2 * expf(m2 - mn);
+            m[i] = mn;
+        }
+        const long long b = q0 + 2 * ty + i;
+        if (tx == 0 && b < s.B) {
+            s.pm[split * s.B + b] = m[i];
+            s.pz[split * s.B + b] = z[i];
+        }
+    }
+}
+
+__global__ void __launch_bounds__(256) kge_ova_merge_kernel(const OneVsAllSide s)
+{
+    const long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    float loss = 0.f;
+    if (b < s.B) {
+        float m = -INFINITY, z = 0.f;
+        for (int k = 0; k < s.nsplit; ++k) m = fmaxf(m, s.pm[k * s.B + b]);
+        for (int k = 0; k < s.nsplit; ++k) {
+            const float mk = s.pm[k * s.B + b];
+            if (mk != -INFINITY) z += s.pz[k * s.B + b] * expf(mk - m);
+        }
+        const float lt = s.lt[b];
+        const float D = __fmaf_rn(s.w, z, expf(lt - m));
+        s.row_m[b] = m;
+        s.row_inv[b] = 1.f / D;
+        loss = (m + logf(D)) - lt;
+    }
+    loss = warp_sum(loss);
+    if ((threadIdx.x & 31) == 0 && s.loss) atomicAdd(s.loss, (double)loss);
+}
+
+__global__ void __launch_bounds__(OVA_THREADS) kge_ova_dq_kernel(const OneVsAllSide s)
+{
+    extern __shared__ __align__(16) float ova_sm[];
+    float *stage = ova_sm, *gs = ova_sm + OVA_STAGE, *acc_s = gs + OVA_GS;
+    const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15, split = blockIdx.y;
+    const long long q0 = (long long)blockIdx.x * OVA_T;
+    long long et0, et1;
+    ova_split_range(s, split, et0, et1);
+    ova_zero(acc_s, OVA_T * s.ld, tid);
+    long long tgt[2];
+    float m[2], inv[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        const long long b = q0 + 2 * ty + i;
+        tgt[i] = b < s.B ? s.triples[3 * b + s.col] : -1;
+        m[i] = b < s.B ? s.row_m[b] : 0.f;
+        inv[i] = b < s.B ? s.row_inv[b] : 0.f;
+    }
+    for (long long et = et0; et < et1; ++et) {
+        const long long e0 = et * OVA_T;
+        float acc[2][2];
+        ova_logits(s.q, q0, s.B, s.ent, e0, s.n_ent, s.ld, stage, tid, acc);
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+                const long long e = e0 + tx + 16 * j;
+                gs[(2 * ty + i) * (OVA_T + 1) + tx + 16 * j] =
+                    (tgt[i] >= 0 && e < s.n_ent) ? ova_grad(acc[i][j], s, e, tgt[i], m[i], inv[i]) : 0.f;
+            }
+        __syncthreads();
+        ova_accumulate<false>(acc_s, gs, s.ent, e0, s.n_ent, s.ld, stage, tid);
+    }
+    // this split's partial Gq rows, scale included
+    const int o = tid >> 3;
+    const long long b = q0 + o;
+    if (b < s.B)
+        for (int c = (tid & 7) * 4; c < s.ld; c += 32) {
+            const float4 a = ova_lds4(acc_s + (size_t)o * s.ld + c);
+            *reinterpret_cast<float4 *>(s.pgq + ((size_t)split * s.B + b) * s.ld + c) = s.scale * a;
+        }
+}
+
+__global__ void __launch_bounds__(OVA_THREADS) kge_ova_dx_kernel(const OneVsAllSide s)
+{
+    extern __shared__ __align__(16) float ova_sm[];
+    float *stage = ova_sm, *gs = ova_sm + OVA_STAGE, *acc_s = gs + OVA_GS;
+    const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
+    const long long e0 = (long long)blockIdx.x * OVA_T;
+    ova_zero(acc_s, OVA_T * s.ld, tid);
+    const long long n_qt = (s.B + OVA_T - 1) / OVA_T;
+    for (long long qt = 0; qt < n_qt; ++qt) {
+        const long long q0 = qt * OVA_T;
+        float acc[2][2];
+        ova_logits(s.q, q0, s.B, s.ent, e0, s.n_ent, s.ld, stage, tid, acc);
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const long long b = q0 + 2 * ty + i;
+            const bool row = b < s.B;
+            const long long t = row ? s.triples[3 * b + s.col] : -1;
+            const float m = row ? s.row_m[b] : 0.f, inv = row ? s.row_inv[b] : 0.f;
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+                const long long e = e0 + tx + 16 * j;
+                gs[(2 * ty + i) * (OVA_T + 1) + tx + 16 * j] = (row && e < s.n_ent) ? ova_grad(acc[i][j], s, e, t, m, inv) : 0.f;
+            }
+        }
+        __syncthreads();
+        ova_accumulate<true>(acc_s, gs, s.q, q0, s.B, s.ld, stage, tid);
+    }
+    // one add per gradient row: this CTA is the only writer of its rows in this launch
+    const int o = tid >> 3;
+    const long long e = e0 + o;
+    if (e < s.n_ent)
+        for (int c = (tid & 7) * 4; c < s.ld; c += 32) {
+            float *g = s.grad_ent + (size_t)e * s.ld + c;
+            const float4 a = ova_lds4(acc_s + (size_t)o * s.ld + c);
+            *reinterpret_cast<float4 *>(g) = *reinterpret_cast<const float4 *>(g) + s.scale * a;
+        }
+}
+
+// one thread per (positive, float4 chunk of a half)
+template <int HALVES>
+__global__ void __launch_bounds__(256) kge_ova_chain_kernel(const OneVsAllSide s)
+{
+    const int nq4 = s.kp / 4;
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= s.B * nq4) return;
+    const long long b = idx / nq4;
+    const int d = (int)(idx - b * nq4) * 4, di = HALVES == 2 ? s.kp + d : d;
+    float4 Gr = f4zero(), Gi = f4zero();
+    for (int k = 0; k < s.nsplit; ++k) {
+        const float *g = s.pgq + ((size_t)k * s.B + b) * s.ld;
+        Gr = Gr + f4ld(g + d);
+        if (HALVES == 2) Gi = Gi + f4ld(g + di);
+    }
+    const int si = s.triples[3 * b], pi_ = s.triples[3 * b + 1], oi_ = s.triples[3 * b + 2];
+    const float *prow = s.rel + (size_t)pi_ * s.ld;
+    const float4 pr = f4ld(prow + d), pi = HALVES == 2 ? f4ld(prow + di) : f4zero();
+    const float4 z = f4zero();
+    float *gp = s.grad_rel + (size_t)pi_ * s.ld;
+    if (s.side == KGE_SIDE_O) {  // q = Q1(s, p): d/ds = Q0(p, Gq), d/dp of f(s, p, Gq)
+        const float *srow = s.ent + (size_t)si * s.ld;
+        const float4 sr = f4ld(srow + d), sim = HALVES == 2 ? f4ld(srow + di) : f4zero();
+        float *ge = s.grad_ent + (size_t)si * s.ld;
+        red_add_v4(ge + d, query_subj<HALVES, 0>(pr, pi, Gr, Gi));
+        red_add_v4(gp + d, trilinear_grad_p<HALVES, 0>(sr, sim, z, z, z, z, Gr, Gi));
+        if (HALVES == 2) {
+            red_add_v4(ge + di, query_subj<HALVES, 1>(pr, pi, Gr, Gi));
+            red_add_v4(gp + di, trilinear_grad_p<HALVES, 1>(sr, sim, z, z, z, z, Gr, Gi));
+        }
+    } else {  // q = Q0(p, o): d/do = Q1(Gq, p), d/dp of f(Gq, p, o)
+        const float *orow = s.ent + (size_t)oi_ * s.ld;
+        const float4 orr = f4ld(orow + d), oim = HALVES == 2 ? f4ld(orow + di) : f4zero();
+        float *ge = s.grad_ent + (size_t)oi_ * s.ld;
+        red_add_v4(ge + d, query_obj<HALVES, 0>(Gr, Gi, pr, pi));
+        red_add_v4(gp + d, trilinear_grad_p<HALVES, 0>(z, z, orr, oim, Gr, Gi, z, z));
+        if (HALVES == 2) {
+            red_add_v4(ge + di, query_obj<HALVES, 1>(Gr, Gi, pr, pi));
+            red_add_v4(gp + di, trilinear_grad_p<HALVES, 1>(z, z, orr, oim, Gr, Gi, z, z));
+        }
+    }
+    if (d == 0 && s.stamp_rel) s.stamp_rel[pi_] = s.stamp;
+}
+
+__global__ void kge_ova_stamp_kernel(int *stamps, long long n, int stamp)
+{
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        stamps[i] = stamp;
+}
+
+template <class Kernel>
+static cudaError_t ova_launch(Kernel kern, dim3 grid, size_t smem, const OneVsAllSide &s, cudaStream_t st)
+{
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    kern<<<grid, OVA_THREADS, smem, st>>>(s);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_one_vs_all_side(const OneVsAllSide &s, int halves, cudaStream_t st)
+{
+    if (s.B == 0) return cudaSuccess;
+    const unsigned n_qt = (unsigned)((s.B + OVA_T - 1) / OVA_T), n_et = (unsigned)((s.n_ent + OVA_T - 1) / OVA_T);
+    const size_t big = one_vs_all_smem_bytes(s.ld);
+    cudaError_t e = ova_launch(kge_ova_stats_kernel, dim3(n_qt, s.nsplit), OVA_STAGE * sizeof(float), s, st);
+    if (e != cudaSuccess) return e;
+    kge_ova_merge_kernel<<<(unsigned)((s.B + 255) / 256), 256, 0, st>>>(s);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    if ((e = ova_launch(kge_ova_dq_kernel, dim3(n_qt, s.nsplit), big, s, st)) != cudaSuccess) return e;
+    if ((e = ova_launch(kge_ova_dx_kernel, dim3(n_et), big, s, st)) != cudaSuccess) return e;
+    const unsigned grid = (unsigned)((s.B * (s.kp / 4) + 255) / 256);
+    if (halves == 2) kge_ova_chain_kernel<2><<<grid, 256, 0, st>>>(s);
+    else kge_ova_chain_kernel<1><<<grid, 256, 0, st>>>(s);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_one_vs_all_stamps(int *stamp_ent, long long n_ent, int stamp, cudaStream_t st)
+{
+    if (!stamp_ent || n_ent == 0) return cudaSuccess;
+    const long long blocks = (n_ent + 255) / 256;
+    kge_ova_stamp_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, st>>>(stamp_ent, n_ent, stamp);
+    return cudaGetLastError();
+}
+
+}  // namespace kge

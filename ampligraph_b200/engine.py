@@ -50,6 +50,24 @@ def optimizer_slots(cfg):
 RHO_DEFAULT = {"rmsprop": 0.9, "adadelta": 0.95}  # Keras legacy defaults; unused by the other kinds
 
 
+def one_vs_all_splits(B, n_ent):
+    """Entity ranges per 32-query tile of the 1vsAll stats and dQ passes (kge_train_1vsall.cu, one_vs_all_splits):
+    enough for about 264 CTAs, at most 64 and at most one per 32-entity tile."""
+    n_qt, n_et = -(-int(B) // 32), -(-int(n_ent) // 32)
+    s = -(-264 // n_qt) if n_qt > 0 else 1
+    return max(1, min(s, 64, n_et))
+
+
+def one_vs_all_workspace_bytes(B, n_ent, ld):
+    """kge_one_vs_all_workspace_bytes(h, B) for a handle of n_ent entities and rows of ld floats: both sides' query
+    vectors [B, ld], the quantised positive scores [B], the per-split maxima and sums [nsplit, B], three [B] row arrays
+    and the per-split partial query gradients [nsplit, B, ld], each region padded to 16 bytes."""
+    r16 = lambda n: (n + 15) // 16 * 16
+    B, ns = int(B), one_vs_all_splits(B, n_ent)
+    rows, col = 4 * B * int(ld), 4 * B
+    return 2 * r16(rows) + r16(col) + 2 * r16(ns * col) + 3 * r16(col) + r16(ns * rows)
+
+
 INT32_MAX = 2 ** 31 - 1
 DBSCAN_BATCH = 1024  # queries per kge_radius_* call of KGEEngine.dbscan (discovery.find_duplicates' batch)
 
@@ -188,6 +206,7 @@ class KGEEngine:
         default_margin = 3.0 if loss == "self_adversarial" else 1.0  # loss_functions.py:23,:29
         self.scoring_type, self.k, self.eta = scoring_type, int(k), int(eta)
         self.n_ent, self.n_rel = int(n_ent), int(n_rel)
+        self.reduction = reduction
         # rows of the LOCAL entity table: n_ent, or one row shard of it (parallel.ShardedTrainer)
         self.ent_rows = int(ent_rows) if ent_rows is not None else self.n_ent
         self.device = torch.device("cuda", device)
@@ -384,6 +403,29 @@ class KGEEngine:
         # RotatE: rotation table + kernel; bucketed: count, two scan launches, kernel, bucket sum (deferred: in
         # apply_gradients' launch)
         self.launches += 2 if self.scoring_type == "RotatE" else (4 if defer else 5) if bucketed else 1
+
+    @_traced("kge.one_vs_all_step")
+    def one_vs_all_backward(self, triples, sides="s,o", step=0):
+        """1vsAll step up to tape.gradient (kge_one_vs_all_step, DESIGN.md 3.12): the multiclass NLL of every positive
+        against every entity on each side in `sides` ('s,o', 'o' or 's'), with the engine's reduction; accumulates into
+        g_ent / g_rel and loss_acc[0] like forward_backward.  step: the lazy optimizer's row stamp (every entity row and
+        the batch's relation rows count as looked up).  apply_gradients() takes its non-deferred path next."""
+        assert triples.dtype == torch.int32 and triples.is_cuda and triples.is_contiguous()
+        if sides not in _lib.ONE_VS_ALL_SIDES:
+            raise ValueError("one_vs_all must be one of %s, got %r" % (", ".join(map(repr, _lib.ONE_VS_ALL_SIDES)), sides))
+        if self._deferred:
+            raise ValueError("one_vs_all_backward: the replaced-row sum of a deferred step is pending (apply_gradients first)")
+        B = triples.shape[0]
+        need = int(self.lib.kge_one_vs_all_workspace_bytes(self.h, B))
+        if getattr(self, "_ova_ws", None) is None or self._ova_ws.numel() < need:
+            self._ova_ws = torch.empty(max(need, 16), dtype=torch.uint8, device=self.device)  # 256-byte aligned (torch)
+        _lib.check(self.lib.kge_one_vs_all_step(
+            self.h, _lib.ONE_VS_ALL_SIDES[sides], _lib.REDUCTIONS[self.reduction], _ptr(self.ent), _ptr(self.rel),
+            _ptr(self.g_ent), _ptr(self.g_rel), _ptr(triples), B, int(step), _ptr(self.loss_acc), _ptr(self._ova_ws), need,
+            self._stream()))
+        self._last_step = int(step)
+        # query vectors (two kernels), entity stamps, five passes per side
+        self.launches += 2 + (1 if self.lazy else 0) + 5 * (2 if sides == "s,o" else 1)
 
     def _one_block(self):
         """True when tables, gradients and slots still ARE the [ent | rel] blocks allocated here (callers may rebind them: the

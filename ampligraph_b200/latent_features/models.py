@@ -208,12 +208,21 @@ class ScoringBasedEmbeddingModel:
     def fit(self, x=None, batch_size=1000, epochs=100, verbose=True, callbacks=None, validation_split=0.0,
             validation_data=None, shuffle=True, initial_epoch=0, validation_batch_size=10,
             validation_corrupt_side="s,o", validation_freq=10, validation_burn_in=0, validation_filter=False,
-            validation_entities_subset=None, partitioning_k=1, focusE=False, focusE_params={}):
+            validation_entities_subset=None, partitioning_k=1, focusE=False, focusE_params={}, one_vs_all=None):
         """fit (:544-883).  `shuffle` is accepted and ignored exactly like the reference
         (batches are the sequential slices of graph_data_loader.py:495-500).  validation_split: carve the validation
         set out of x with train_test_split_no_unseen(x, test_size=validation_split, seed=self.seed), as the reference
-        does (:719-727).  The filter of the validations (validation_filter) is indexed once per fit, not per validation."""
+        does (:719-727).  The filter of the validations (validation_filter) is indexed once per fit, not per validation.
+
+        one_vs_all (extension): None trains against eta sampled corruptions per positive.  's,o', 'o' or 's' trains
+        1vsAll instead (Ruffinelli et al., ICLR 2020): every step scores each positive against every entity on the
+        given sides, with the multiclass NLL over all of them (the setting of the reference's multiclass_nll
+        docstring, loss_functions.py:580-590; DESIGN.md 3.12).  eta and the corruption seed are then unused.  It needs
+        DistMult, ComplEx or HolE and the compiled loss 'multiclass_nll' (either reduction), on one GPU without
+        focusE."""
         self._assert_compile_was_called()
+        if one_vs_all is not None:
+            self._check_one_vs_all(one_vs_all, focusE)
         if validation_split:
             assert isinstance(x, np.ndarray), "Validation split supported for numpy arrays only!"
             x, validation_data = train_test_split_no_unseen(x, test_size=validation_split, seed=self.seed,
@@ -271,7 +280,10 @@ class ScoringBasedEmbeddingModel:
                 self._focuse_sw = max(1 - epoch / self._focuse_stop, 0.001)
             for start in range(0, n, batch_size):
                 batch = data[start:start + batch_size]
-                if self.use_focusE:
+                if one_vs_all is not None:
+                    eng.one_vs_all_backward(batch, one_vs_all, step=self._step)
+                    eng.apply_gradients()
+                elif self.use_focusE:
                     self._two_phase_step(batch, weights[start:start + batch_size])
                 elif world > 1:  # this rank's slice of the global batch; the step is the global-batch step
                     from ..parallel import row_shard
@@ -314,6 +326,20 @@ class ScoringBasedEmbeddingModel:
         self.is_fitted = True
         self.history = history
         return history
+
+    def _check_one_vs_all(self, one_vs_all, focusE):
+        """The refusals of fit(one_vs_all=...), before anything is indexed or trained."""
+        if not isinstance(one_vs_all, str) or one_vs_all not in _lib.ONE_VS_ALL_SIDES:
+            raise ValueError("one_vs_all must be None, 's,o', 'o' or 's', got %r" % (one_vs_all,))
+        if self.scoring_type not in ("DistMult", "ComplEx", "HolE"):
+            raise NotImplementedError("1vsAll training is implemented for DistMult, ComplEx and HolE (inner-product "
+                                      "scores), not for %s" % self.scoring_type)
+        if isinstance(self.compiled_loss, loss_functions.LossFunctionWrapper) or self.compiled_loss.name != "multiclass_nll":
+            raise ValueError("1vsAll training needs the loss 'multiclass_nll', got %r" % (self.compiled_loss.name,))
+        if focusE:
+            raise NotImplementedError("1vsAll training does not support focusE")
+        if self._world() > 1:
+            raise NotImplementedError("1vsAll training is single-GPU only")
 
     def train_on_batch(self, x):
         """Keras Model.train_on_batch (the reference model is a tf.keras.Model): one train_step on ONE

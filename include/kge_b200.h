@@ -275,6 +275,26 @@ int kge_train_step_sharded(kge_handle *h, int32_t mode, const kge_shard_map *map
                            uint64_t step, double *loss_dev, float *scores_pos_dev, float *scores_neg_dev,
                            const float *dpos_dev, const float *dneg_dev, void *stream);
 
+/* 1vsAll training (Ruffinelli et al., ICLR 2020; the setting of the reference's multiclass_nll docstring,
+ * loss_functions.py:580-590): forward + backward of the multiclass NLL of every positive against EVERY entity, no
+ * sampled corruptions.  For each positive (s, p, o) and each side in `sides` (a set of the flags below) the logits are
+ * l_e = f(s, p, e) (side o) or f(e, p, o) (side s) for all e in [0, n_ent), the positive's own entity t included once;
+ * each is clipped to [-75, 75] (zero gradient outside).  loss_reduction KGE_REDUCE_SUM: logsumexp_e(l_e) - l_t;
+ * KGE_REDUCE_MEAN: -log(exp(l_t) / (mean_{e != t} exp(l_e) + exp(l_t))).  Other true triples count as negatives (no
+ * filtering).  DistMult, ComplEx and HolE only (KGE_ERR_UNSUPPORTED otherwise); the handle's loss, eta and corruption
+ * seed are not used; needs n_ent >= 2 and rows whose 32-query tile fits in shared memory (ld <= about 1600 floats).
+ *   grad_*_dev  ADDED to, as by kge_train_step; apply kge_optimizer_step (or _lazy) next
+ *   step        the lazy-optimizer stamp (kge_set_row_stamps): every entity row and the relation rows of the batch are
+ *               stamped with kge_step_stamp(step)
+ *   loss_dev    double accumulator += the sum over positives and sides of the loss (may be NULL)
+ *   ws_dev      caller-owned, 16-byte aligned, at least kge_one_vs_all_workspace_bytes(h, B) bytes
+ * Refused while a KGE_STEP_FUSED_DEFER step is pending.  Works on one (unsharded) entity table.  DESIGN.md 3.12. */
+enum kge_one_vs_all_side { KGE_ONE_VS_ALL_S = 1, KGE_ONE_VS_ALL_O = 2 };
+int64_t kge_one_vs_all_workspace_bytes(const kge_handle *h, int64_t B);
+int kge_one_vs_all_step(kge_handle *h, int32_t sides, int32_t loss_reduction, const float *ent_dev, const float *rel_dev,
+                        float *grad_ent_dev, float *grad_rel_dev, const int32_t *triples_dev, int64_t B, uint64_t step,
+                        double *loss_dev, void *ws_dev, int64_t ws_bytes, void *stream);
+
 /* OptimizerWrapper.minimize -> legacy apply_gradients (optimizers.py:136-168) for ONE
  * table (or any row-wise concatenation of tables of the same width and regulariser: the engine passes [ent | rel] as one
  * block, one launch per step), dense semantics, plus the LP regulariser's loss/gradient over the whole table

@@ -441,14 +441,22 @@ extern "C" int64_t kge_train_workspace_bytes(const kge_handle *h, int64_t B)
     return h && B >= 0 ? bucket_workspace_bytes(h, B) : 0;
 }
 
+// A KGE_STEP_FUSED_DEFER step leaves its replaced-row sum in the training workspace until kge_optimizer_step_deferred
+// consumes it: until then no call may train or replace the workspace
+static int check_no_pending(const kge_handle *h, const char *fn)
+{
+    if (h->sum_pending)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "%s: the replaced-row sum of a deferred step is pending in the training workspace "
+                                              "(kge_optimizer_step_deferred first)", fn);
+    return KGE_OK;
+}
+
 extern "C" int kge_set_train_workspace(kge_handle *h, void *ws_dev, int64_t bytes, void *stream)
 {
     KGE_CHECK_HANDLE(h, "kge_set_train_workspace");
     if (bytes < 0 || (ws_dev && ((uintptr_t)ws_dev & 15)))
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_set_train_workspace: bytes < 0 or workspace not 16-byte aligned");
-    if (h->sum_pending)
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_set_train_workspace: the replaced-row sum of a deferred step is pending "
-                                              "in the current workspace (kge_optimizer_step_deferred first)");
+    if (int rc = check_no_pending(h, "kge_set_train_workspace")) return rc;
     Carve counts(nullptr);
     carve_train_workspace(h, 0, counts);
     if (ws_dev && bytes < (int64_t)counts.at)
@@ -469,9 +477,7 @@ static int train_step_impl(kge_handle *h, int32_t mode, const kge_shard_map *map
     KGE_CHECK_HANDLE(h, "kge_train_step");
     if (mode < KGE_STEP_FUSED || mode > KGE_STEP_FUSED_DEFER)
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_train_step: unknown mode %d", mode);
-    if (h->sum_pending)
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_train_step: the replaced-row sum of a deferred step is pending "
-                                              "(kge_optimizer_step_deferred first)");
+    if (int rc = check_no_pending(h, "kge_train_step")) return rc;
     const bool defer = mode == KGE_STEP_FUSED_DEFER;
     if (defer) mode = KGE_STEP_FUSED;
     if (B < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_train_step: B < 0");
@@ -630,10 +636,10 @@ extern "C" int kge_train_step_sharded(kge_handle *h, int32_t mode, const kge_sha
                            dpos_dev, dneg_dev, stream);
 }
 
-// Checks a caller's config and copies it into *out, widened to the current layout.  A config of the layout before rho
-// (struct_size == offsetof(kge_optimizer_config, rho)) is accepted for the kinds that layout knew; its new fields read
-// as 0.
-static int check_optim(const kge_optimizer_config *opt, const char *fn, kge_optimizer_config *out)
+// Checks a caller's config, copies it into out, widened to the current layout, and re-points opt at the copy.  A config
+// of the layout before rho (struct_size == offsetof(kge_optimizer_config, rho)) is accepted for the kinds that layout
+// knew; its new fields read as 0.
+static int check_optim(const kge_optimizer_config *&opt, const char *fn, kge_optimizer_config &out)
 {
     const int32_t old_size = (int32_t)offsetof(kge_optimizer_config, rho);
     if (!opt || (opt->struct_size != (int32_t)sizeof(kge_optimizer_config) && opt->struct_size != old_size))
@@ -643,10 +649,11 @@ static int check_optim(const kge_optimizer_config *opt, const char *fn, kge_opti
         return fail(KGE_ERR_INVALID_ARGUMENT, "Could not interpret optimizer identifier: %d", opt->kind);
     if (opt->reg_p < 0 || opt->reg_p2 < 0 || (opt->reg_p == 0 && opt->reg_p2 != 0))
         return fail(KGE_ERR_INVALID_ARGUMENT, "%s: bad regulariser (reg_p >= 0; reg_p2 needs reg_p)", fn);
-    memset(out, 0, sizeof(*out));
-    memcpy(out, opt, (size_t)opt->struct_size);
-    out->struct_size = (int32_t)sizeof(kge_optimizer_config);
-    if (out->kind == KGE_OPT_RMSPROP && out->centered && out->momentum != 0.f)
+    memset(&out, 0, sizeof(out));
+    memcpy(&out, opt, (size_t)opt->struct_size);
+    out.struct_size = (int32_t)sizeof(kge_optimizer_config);
+    opt = &out;
+    if (out.kind == KGE_OPT_RMSPROP && out.centered && out.momentum != 0.f)
         return fail(KGE_ERR_UNSUPPORTED, "%s: centered RMSprop with momentum needs a third slot buffer (not supported)", fn);
     return KGE_OK;
 }
@@ -656,8 +663,9 @@ static RegParams reg_of(const kge_optimizer_config *opt)
     r.p = opt->reg_p; r.lambda = opt->reg_lambda; r.p2 = opt->reg_p2; r.lambda2 = opt->reg_lambda2;
     return r;
 }
-static void fill_optim(const kge_optimizer_config *opt, int64_t t, OptimParams &o)
+static OptimParams optim_params(const kge_optimizer_config *opt, int64_t t)
 {
+    OptimParams o;
     o.kind = opt->kind;
     o.lr = opt->learning_rate;
     o.beta1 = opt->beta_1;
@@ -674,12 +682,14 @@ static void fill_optim(const kge_optimizer_config *opt, int64_t t, OptimParams &
     else
         o.lr_t = (float)((double)opt->learning_rate * sqrt(1.0 - pow((double)opt->beta_2, (double)t)) /
                          (1.0 - pow((double)opt->beta_1, (double)t)));
+    return o;
 }
-static bool slots_ok(const kge_optimizer_config *opt, const float *s0, const float *s1)
+// Every slot buffer the config's update reads and writes must be given
+static int check_slots(const kge_optimizer_config *opt, const float *s0, const float *s1, const char *fn)
 {
-    const bool need0 = uses_slot0(opt->kind, opt->momentum);
-    const bool need1 = uses_slot1(opt->kind, opt->momentum, opt->centered);
-    return !((need0 && !s0) || (need1 && !s1));
+    if ((uses_slot0(opt->kind, opt->momentum) && !s0) || (uses_slot1(opt->kind, opt->momentum, opt->centered) && !s1))
+        return fail(KGE_ERR_INVALID_ARGUMENT, "%s: optimizer slot buffer missing", fn);
+    return KGE_OK;
 }
 
 extern "C" int kge_optimizer_step(kge_handle *h, const kge_optimizer_config *opt, int64_t t, float *table_dev,
@@ -688,15 +698,12 @@ extern "C" int kge_optimizer_step(kge_handle *h, const kge_optimizer_config *opt
 {
     KGE_CHECK_HANDLE(h, "kge_optimizer_step");
     kge_optimizer_config cfg;
-    if (int rc = check_optim(opt, "kge_optimizer_step", &cfg)) return rc;
-    opt = &cfg;
+    if (int rc = check_optim(opt, "kge_optimizer_step", cfg)) return rc;
     if (rows < 0 || t < 1) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step: rows >= 0 and t >= 1 required");
     if (rows == 0) return KGE_OK;
     if (!table_dev || !grad_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step: null table/grad");
-    if (!slots_ok(opt, slot0_dev, slot1_dev))
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step: optimizer slot buffer missing");
-    OptimParams o;
-    fill_optim(opt, t, o);
+    if (int rc = check_slots(opt, slot0_dev, slot1_dev, "kge_optimizer_step")) return rc;
+    const OptimParams o = optim_params(opt, t);
     KGE_CUDA(launch_optimizer(o, table_dev, grad_dev, slot0_dev, slot1_dev, rows * (long long)h->L.ld, reg_loss_dev,
                               h->sm_count, (cudaStream_t)stream),
              "kge_optimizer_step");
@@ -710,8 +717,7 @@ extern "C" int kge_optimizer_step_deferred(kge_handle *h, const kge_optimizer_co
     KGE_CHECK_HANDLE(h, "kge_optimizer_step_deferred");
     if (!h->sum_pending) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_deferred: no deferred step is pending");
     kge_optimizer_config cfg;
-    if (int rc = check_optim(opt, "kge_optimizer_step_deferred", &cfg)) return rc;
-    opt = &cfg;
+    if (int rc = check_optim(opt, "kge_optimizer_step_deferred", cfg)) return rc;
     if (t < 1) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_deferred: t >= 1 required");
     const TrainParams &p = h->pending;
     const size_t ent_floats = (size_t)h->cfg.n_ent * h->L.ld;
@@ -721,10 +727,8 @@ extern "C" int kge_optimizer_step_deferred(kge_handle *h, const kge_optimizer_co
                                               "(n_ent + n_rel rows) the deferred step trained on");
     if (!params_out || params_out == params_in)
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_deferred: params_out must be a second block");
-    if (!slots_ok(opt, slot0_dev, slot1_dev))
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_deferred: optimizer slot buffer missing");
-    OptimParams o;
-    fill_optim(opt, t, o);
+    if (int rc = check_slots(opt, slot0_dev, slot1_dev, "kge_optimizer_step_deferred")) return rc;
+    const OptimParams o = optim_params(opt, t);
     // the checks above refuse without touching the pending step (the caller may repeat the call); from here on it is
     // consumed, and the workspace is free again, whether or not the launch succeeds
     h->sum_pending = false;
@@ -774,15 +778,12 @@ extern "C" int kge_optimizer_step_lazy(kge_handle *h, const kge_optimizer_config
 {
     KGE_CHECK_HANDLE(h, "kge_optimizer_step_lazy");
     kge_optimizer_config cfg;
-    if (int rc = check_optim(opt, "kge_optimizer_step_lazy", &cfg)) return rc;
-    opt = &cfg;
+    if (int rc = check_optim(opt, "kge_optimizer_step_lazy", cfg)) return rc;
     if (rows < 0 || t < 1) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_lazy: rows >= 0 and t >= 1 required");
     if (rows == 0) return KGE_OK;
     if (!table_dev || !grad_dev || !row_stamp_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_lazy: null pointer");
-    if (!slots_ok(opt, slot0_dev, slot1_dev))
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_lazy: optimizer slot buffer missing");
-    OptimParams o;
-    fill_optim(opt, t, o);
+    if (int rc = check_slots(opt, slot0_dev, slot1_dev, "kge_optimizer_step_lazy")) return rc;
+    const OptimParams o = optim_params(opt, t);
     KGE_CUDA(launch_optimizer_lazy(o, table_dev, grad_dev, slot0_dev, slot1_dev, rows, h->L.ld, (const int *)row_stamp_dev,
                                    stamp, reg_loss_dev, h->sm_count, (cudaStream_t)stream),
              "kge_optimizer_step_lazy");
@@ -803,18 +804,15 @@ extern "C" int kge_optimizer_step_sharded(kge_handle *h, const kge_optimizer_con
 {
     KGE_CHECK_HANDLE(h, "kge_optimizer_step_sharded");
     kge_optimizer_config cfg;
-    if (int rc = check_optim(opt, "kge_optimizer_step_sharded", &cfg)) return rc;
-    opt = &cfg;
+    if (int rc = check_optim(opt, "kge_optimizer_step_sharded", cfg)) return rc;
     if (int rc = check_world(world, rank, "kge_optimizer_step_sharded")) return rc;
     if (row_begin < 0 || row_end < row_begin || t < 1) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_sharded: bad row range / t");
     if (row_end == row_begin) return KGE_OK;
     if (!peer_tables || !peer_grads) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_sharded: null pointer arrays");
     for (int q = 0; q < world; ++q)
         if (!peer_tables[q] || !peer_grads[q]) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_sharded: null peer pointer for rank %d", q);
-    if (!slots_ok(opt, slot0_shard_dev, slot1_shard_dev))
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_sharded: optimizer slot buffer missing");
-    OptimParams o;
-    fill_optim(opt, t, o);
+    if (int rc = check_slots(opt, slot0_shard_dev, slot1_shard_dev, "kge_optimizer_step_sharded")) return rc;
+    const OptimParams o = optim_params(opt, t);
     KGE_CUDA(launch_optimizer_sharded(o, world, rank, peer_tables, peer_grads, slot0_shard_dev, slot1_shard_dev,
                                       row_begin * (long long)h->L.ld, (row_end - row_begin) * (long long)h->L.ld,
                                       reg_loss_dev, h->sm_count, (cudaStream_t)stream),
@@ -832,10 +830,8 @@ extern "C" int kge_optimizer_step_exchange(kge_handle *h, const kge_optimizer_co
 {
     KGE_CHECK_HANDLE(h, "kge_optimizer_step_exchange");
     kge_optimizer_config cfg_ent, cfg_rel;
-    if (int rc = check_optim(opt_ent, "kge_optimizer_step_exchange", &cfg_ent)) return rc;
-    if (int rc = check_optim(opt_rel, "kge_optimizer_step_exchange", &cfg_rel)) return rc;
-    opt_ent = &cfg_ent;
-    opt_rel = &cfg_rel;
+    if (int rc = check_optim(opt_ent, "kge_optimizer_step_exchange", cfg_ent)) return rc;
+    if (int rc = check_optim(opt_rel, "kge_optimizer_step_exchange", cfg_rel)) return rc;
     if (int rc = check_world(world, rank, "kge_optimizer_step_exchange")) return rc;
     if (opt_ent->kind != opt_rel->kind || opt_ent->learning_rate != opt_rel->learning_rate || opt_ent->beta_1 != opt_rel->beta_1 ||
         opt_ent->beta_2 != opt_rel->beta_2 || opt_ent->epsilon != opt_rel->epsilon || opt_ent->momentum != opt_rel->momentum ||
@@ -850,10 +846,9 @@ extern "C" int kge_optimizer_step_exchange(kge_handle *h, const kge_optimizer_co
     for (int q = 0; q < world; ++q)
         if (!peer_tables[q] || !peer_grads[q] || (phases && !peer_flags[q]))
             return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_exchange: null peer pointer for rank %d", q);
-    if (row_end > row_begin && !slots_ok(opt_ent, slot0_shard_dev, slot1_shard_dev))
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_exchange: optimizer slot buffer missing");
-    OptimParams o;
-    fill_optim(opt_ent, t, o);
+    if (row_end > row_begin)
+        if (int rc = check_slots(opt_ent, slot0_shard_dev, slot1_shard_dev, "kge_optimizer_step_exchange")) return rc;
+    const OptimParams o = optim_params(opt_ent, t);
     ExchangeParams x;
     memset(&x, 0, sizeof(x));
     x.world = world; x.rank = rank; x.phases = phases;
@@ -934,13 +929,13 @@ extern "C" int64_t kge_rank_workspace_bytes(const kge_handle *h, int64_t b, int6
     return (int64_t)c.at;
 }
 
-// A caller-owned workspace of `need` bytes (fn_workspace_bytes), 1024-byte aligned
-static int check_workspace(void *ws, int64_t bytes, int64_t need, const char *fn)
+// A caller-owned workspace of `need` bytes (what the sizing function `sizer` returns), `align`-byte aligned
+static int check_workspace(void *ws, int64_t bytes, int64_t need, unsigned align, const char *fn, const char *sizer)
 {
     if (!ws || bytes < need)
-        return fail(KGE_ERR_INVALID_ARGUMENT, "%s: workspace of %lld bytes needed (%s_workspace_bytes), got %lld", fn,
-                    (long long)need, fn, (long long)(ws ? bytes : 0));
-    if (((uintptr_t)ws & 1023u) != 0) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: workspace must be 1024-byte aligned", fn);
+        return fail(KGE_ERR_INVALID_ARGUMENT, "%s: workspace of %lld bytes needed (%s), got %lld", fn, (long long)need, sizer,
+                    (long long)(ws ? bytes : 0));
+    if ((uintptr_t)ws % align != 0) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: workspace must be %u-byte aligned", fn, align);
     return KGE_OK;
 }
 
@@ -1020,7 +1015,9 @@ static int rank_impl(kge_handle *h, const kge_shard_map *map, int64_t filt_base,
     // both filter pointers null with n_filt > 0: nothing is filtered (kge_topk / kge_knn reject that)
     if ((filt_off_dev == nullptr) != (filt_idx_dev == nullptr) && n_filt > 0)
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_rank: filter offsets and indices must be given together");
-    if (int rc = check_workspace(workspace_dev, workspace_bytes, kge_rank_workspace_bytes(h, b, n_cand), "kge_rank")) return rc;
+    if (int rc = check_workspace(workspace_dev, workspace_bytes, kge_rank_workspace_bytes(h, b, n_cand), 1024, "kge_rank",
+                                 "kge_rank_workspace_bytes"))
+        return rc;
     cudaStream_t st = (cudaStream_t)stream;
     Carve c(workspace_dev);
     const RankWorkspace w = carve_rank_workspace(h, c, b, n_cand, true);
@@ -1249,7 +1246,9 @@ extern "C" int kge_topk(kge_handle *h, int32_t side, const float *ent_dev, const
     if (int rc = check_side_candidates(h, "kge_topk", side, cand_ids_dev, cand_begin, n_cand)) return rc;
     if ((filt_off_dev == nullptr || filt_idx_dev == nullptr) && n_filt > 0)
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_topk: filter offsets and indices must be given together");
-    if (int rc = check_workspace(workspace_dev, workspace_bytes, kge_topk_workspace_bytes(h, b, n_cand, k), "kge_topk")) return rc;
+    if (int rc = check_workspace(workspace_dev, workspace_bytes, kge_topk_workspace_bytes(h, b, n_cand, k), 1024, "kge_topk",
+                                 "kge_topk_workspace_bytes"))
+        return rc;
     cudaStream_t st = (cudaStream_t)stream;
     Carve c(workspace_dev);
     const TopkWorkspace w = carve_topk_workspace(h, c, b, n_cand, k);
@@ -1282,7 +1281,8 @@ extern "C" int kge_select_topk(kge_handle *h, const float *scores_dev, int64_t b
     if (n > 0x7fffffffLL) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_select_topk: n must be < 2^31");
     if (b == 0) return KGE_OK;
     if ((n > 0 && !scores_dev) || !pos_dev || !out_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_select_topk: null pointer");
-    if (int rc = check_workspace(workspace_dev, workspace_bytes, kge_select_topk_workspace_bytes(h, b, n, k), "kge_select_topk"))
+    if (int rc = check_workspace(workspace_dev, workspace_bytes, kge_select_topk_workspace_bytes(h, b, n, k), 1024, "kge_select_topk",
+                                 "kge_select_topk_workspace_bytes"))
         return rc;
     cudaStream_t st = (cudaStream_t)stream;
     Carve c(workspace_dev);
@@ -1390,7 +1390,9 @@ extern "C" int kge_knn(kge_handle *h, int32_t metric, const float *points_dev, i
     if (!ids_dev || !dist_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_knn: null pointer");
     if ((filt_off_dev == nullptr || filt_idx_dev == nullptr) && n_filt > 0)
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_knn: filter offsets and indices must be given together");
-    if (int rc = check_workspace(workspace_dev, workspace_bytes, kge_knn_workspace_bytes(h, b, n_cand, k, ld), "kge_knn")) return rc;
+    if (int rc = check_workspace(workspace_dev, workspace_bytes, kge_knn_workspace_bytes(h, b, n_cand, k, ld), 1024, "kge_knn",
+                                 "kge_knn_workspace_bytes"))
+        return rc;
     cudaStream_t st = (cudaStream_t)stream;
     Carve c(workspace_dev);
     const KnnWorkspace w = carve_knn_workspace(h, c, b, n_cand, k, ld);
@@ -1419,7 +1421,8 @@ static int check_radius(kge_handle *h, const char *fn, int32_t metric, const flo
     if (n_cand > 0x7fffffffLL) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: n_cand must be < 2^31", fn);
     if (b == 0) return KGE_OK;
     if (int rc = check_points(fn, metric, points_dev, n_points, ld, query_ids_dev, cand_ids_dev, cand_begin, n_cand)) return rc;
-    if (int rc = check_workspace(workspace_dev, workspace_bytes, kge_radius_workspace_bytes(h, b, n_cand, ld), "kge_radius"))
+    if (int rc = check_workspace(workspace_dev, workspace_bytes, kge_radius_workspace_bytes(h, b, n_cand, ld), 1024, "kge_radius",
+                                 "kge_radius_workspace_bytes"))
         return rc;
     Carve c(workspace_dev);
     *w = carve_knn_workspace(h, c, b, n_cand, 0, ld);
@@ -1578,9 +1581,7 @@ extern "C" int kge_one_vs_all_step(kge_handle *h, int32_t sides, int32_t loss_re
                                               "KGE_ONE_VS_ALL_O, got %d", sides);
     if (loss_reduction != KGE_REDUCE_SUM && loss_reduction != KGE_REDUCE_MEAN)
         return fail(KGE_ERR_INVALID_ARGUMENT, "Invalid value for reduction!");
-    if (h->sum_pending)
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_step: the replaced-row sum of a deferred step is pending "
-                                              "(kge_optimizer_step_deferred first)");
+    if (int rc = check_no_pending(h, "kge_one_vs_all_step")) return rc;
     if (h->cfg.n_ent < 2) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_step: needs n_ent >= 2");
     if ((long long)one_vs_all_smem_bytes(h->L.ld) > h->max_smem)
         return fail(KGE_ERR_UNSUPPORTED, "kge_one_vs_all_step: rows of %d floats exceed the shared-memory tiles of the 1vsAll "
@@ -1589,11 +1590,9 @@ extern "C" int kge_one_vs_all_step(kge_handle *h, int32_t sides, int32_t loss_re
     if (B == 0) return KGE_OK;
     if (!ent_dev || !rel_dev || !grad_ent_dev || !grad_rel_dev || !triples_dev)
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_step: null table, gradient or triples");
-    const int64_t need = kge_one_vs_all_workspace_bytes(h, B);
-    if (!ws_dev || ws_bytes < need || ((uintptr_t)ws_dev & 15))
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_step: a 16-byte aligned workspace of %lld bytes is needed "
-                                              "(kge_one_vs_all_workspace_bytes), got %lld", (long long)need,
-                    (long long)(ws_dev ? ws_bytes : 0));
+    if (int rc = check_workspace(ws_dev, ws_bytes, kge_one_vs_all_workspace_bytes(h, B), 16, "kge_one_vs_all_step",
+                                 "kge_one_vs_all_workspace_bytes"))
+        return rc;
     cudaStream_t st = (cudaStream_t)stream;
     Carve c(ws_dev);
     const OneVsAllWorkspace w = carve_one_vs_all(h, B, c);

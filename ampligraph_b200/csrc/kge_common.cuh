@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "../../include/kge_b200.h"
 
 #if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900 || !defined(__CUDA_ARCH_FEAT_SM90_ALL))
@@ -141,6 +143,27 @@ __device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bu
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------
+// PTX: per-thread async copies global -> shared (cp.async).  With valid false nothing is read and the destination is
+// zero-filled.  The 16-byte copy bypasses L1 (.cg), the 4-byte one goes through it (.ca).
+// ---------------------------------------------------------------------------
+__device__ __forceinline__ void cp_async16(void *smem_dst, const void *gmem_src, bool valid)
+{
+    unsigned sz = valid ? 16u : 0u;
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(sz)
+                 : "memory");
+}
+__device__ __forceinline__ void cp_async4(void *smem_dst, const void *gmem_src, bool valid)
+{
+    unsigned sz = valid ? 4u : 0u;
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(sz)
+                 : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+// wait until at most N of this thread's committed groups are still in flight
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+// ---------------------------------------------------------------------------
 // Philox4x32-10 (counter-based; the in-kernel replacement for TF's stateful
 // tf.random.uniform draws at CorruptionGenerationLayerTrain.py:55-74)
 // ---------------------------------------------------------------------------
@@ -232,5 +255,36 @@ __host__ inline float hole_scale(int K) { return (float)(2.0 / ((double)K / 2.0)
 
 // AbstractScoringLayer.py:11,:201: int32(score * 1e3), truncation toward zero
 __device__ __forceinline__ int quantise(float score) { return __float2int_rz(__fmul_rn(score, 1000.0f)); }
+
+// ---------------------------------------------------------------------------
+// host-side launch helpers
+// ---------------------------------------------------------------------------
+// Let kern use up to smem bytes of dynamic shared memory (a kernel gets 48 KB unless it is raised).  Occupancy queries
+// for more than 48 KB need it too.
+template <class Kernel>
+static cudaError_t allow_dynamic_smem(Kernel kern, size_t smem)
+{
+    return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+}
+
+// Raise kern's shared-memory limit to smem bytes, launch, and return the launch's status
+template <class Kernel, class... Args>
+static cudaError_t launch_with_smem(Kernel kern, dim3 grid, int threads, size_t smem, cudaStream_t st, Args... args)
+{
+    cudaError_t e = allow_dynamic_smem(kern, smem);
+    if (e != cudaSuccess) return e;
+    kern<<<grid, threads, smem, st>>>(args...);
+    return cudaGetLastError();
+}
+
+// Returns launch(std::integral_constant<int, V>) for the V of VS equal to v, the template arguments a launcher's kernel
+// is instantiated for, or cudaErrorInvalidValue when v is none of them.
+template <int... VS, class Launch>
+static cudaError_t dispatch_value(int v, Launch &&launch)
+{
+    cudaError_t e = cudaErrorInvalidValue;
+    (void)((v == VS && ((e = launch(std::integral_constant<int, VS>{})), true)) || ...);
+    return e;
+}
 
 }  // namespace kge

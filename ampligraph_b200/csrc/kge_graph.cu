@@ -200,7 +200,7 @@ cudaError_t launch_graph_counts(const long long *off, const int32_t *nbr, const 
     if (e != cudaSuccess) return e;
     const size_t smem = shared_counter_bytes(n, dev);
     if (smem > 0) {
-        e = cudaFuncSetAttribute(kge_graph_counts_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        e = allow_dynamic_smem(kge_graph_counts_kernel<true>, smem);
         if (e != cudaSuccess) return e;
         int per_sm = 0, sms = 0;
         e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kge_graph_counts_kernel<true>, GR_THREADS, smem);

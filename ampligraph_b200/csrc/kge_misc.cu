@@ -1,8 +1,6 @@
 // kge_misc.cu -- predict-path scoring, layout packing, Glorot initialisation (sm_90a).
 #include <math.h>
 
-#include <type_traits>
-
 #include "kge_internal.h"
 
 namespace kge {
@@ -46,20 +44,6 @@ __global__ void kge_score_kernel(const float *__restrict__ ent, const float *__r
     }
 }
 
-// returns launch(std::integral_constant<int, MODEL>) for the scoring model, or cudaErrorInvalidValue for an unknown one
-template <class Launch>
-static cudaError_t dispatch_model(int model, Launch &&launch)
-{
-    switch (model) {
-    case KGE_TRANSE: return launch(std::integral_constant<int, KGE_TRANSE>{});
-    case KGE_DISTMULT: return launch(std::integral_constant<int, KGE_DISTMULT>{});
-    case KGE_COMPLEX: return launch(std::integral_constant<int, KGE_COMPLEX>{});
-    case KGE_HOLE: return launch(std::integral_constant<int, KGE_HOLE>{});
-    case KGE_ROTATE: return launch(std::integral_constant<int, KGE_ROTATE>{});
-    default: return cudaErrorInvalidValue;
-    }
-}
-
 cudaError_t launch_score_triples(const Layout &L, int, const float *ent, const float *rel_or_rot,
                                  const int32_t *triples, long long n, float scale, float *out, int sm_count,
                                  cudaStream_t st)
@@ -68,7 +52,7 @@ cudaError_t launch_score_triples(const Layout &L, int, const float *ent, const f
     const int threads = 256;
     long long want = (n + 7) / 8;
     int grid = (int)(want < (long long)sm_count * 8 ? want : (long long)sm_count * 8);
-    return dispatch_model(L.model, [&](auto model) {
+    return dispatch_value<KGE_TRANSE, KGE_DISTMULT, KGE_COMPLEX, KGE_HOLE, KGE_ROTATE>(L.model, [&](auto model) {
         kge_score_kernel<decltype(model)::value><<<grid, threads, 0, st>>>(ent, rel_or_rot, triples, n, L.k, L.kp, L.ld, scale, out);
         return cudaGetLastError();
     });

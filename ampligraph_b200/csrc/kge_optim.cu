@@ -401,17 +401,7 @@ cudaError_t launch_optimizer_exchange(const OptimParams &o, const ExchangeParams
             return mc ? launch_exchange_variant<K, R, world, true>(a, o, want, sm_count, st)
                       : launch_exchange_variant<K, R, world, false>(a, o, want, sm_count, st);
         };
-        switch (xp.world) {
-        case 1: return variant(std::integral_constant<int, 1>{});
-        case 2: return variant(std::integral_constant<int, 2>{});
-        case 3: return variant(std::integral_constant<int, 3>{});
-        case 4: return variant(std::integral_constant<int, 4>{});
-        case 5: return variant(std::integral_constant<int, 5>{});
-        case 6: return variant(std::integral_constant<int, 6>{});
-        case 7: return variant(std::integral_constant<int, 7>{});
-        case 8: return variant(std::integral_constant<int, 8>{});
-        default: return cudaErrorInvalidValue;
-        }
+        return dispatch_value<1, 2, 3, 4, 5, 6, 7, 8>(xp.world, variant);
     });
 }
 

@@ -134,16 +134,8 @@ __device__ __forceinline__ void flush_reg_loss(float racc, double *reg_loss)
 template <class Launch>
 static cudaError_t dispatch_optimizer(int kind, bool reg, Launch &&launch)
 {
-    auto with_reg = [&](auto k) { return reg ? launch(k, std::true_type{}) : launch(k, std::false_type{}); };
-    switch (kind) {
-    case KGE_OPT_SGD: return with_reg(std::integral_constant<int, KGE_OPT_SGD>{});
-    case KGE_OPT_ADAM: return with_reg(std::integral_constant<int, KGE_OPT_ADAM>{});
-    case KGE_OPT_ADAGRAD: return with_reg(std::integral_constant<int, KGE_OPT_ADAGRAD>{});
-    case KGE_OPT_RMSPROP: return with_reg(std::integral_constant<int, KGE_OPT_RMSPROP>{});
-    case KGE_OPT_ADADELTA: return with_reg(std::integral_constant<int, KGE_OPT_ADADELTA>{});
-    case KGE_OPT_ADAMAX: return with_reg(std::integral_constant<int, KGE_OPT_ADAMAX>{});
-    default: return cudaErrorInvalidValue;
-    }
+    return dispatch_value<KGE_OPT_SGD, KGE_OPT_ADAM, KGE_OPT_ADAGRAD, KGE_OPT_RMSPROP, KGE_OPT_ADADELTA, KGE_OPT_ADAMAX>(
+        kind, [&](auto k) { return reg ? launch(k, std::true_type{}) : launch(k, std::false_type{}); });
 }
 
 }  // namespace kge

@@ -9,8 +9,6 @@
 //   ComplEx / HolE: the subject-side chain with candidate s, its query vector built from (r, o).
 // Each step below builds one column of that vector and feeds it to rank_step / rank_step_rot of kge_rank_common.cuh,
 // so the count kernel and the filter kernel run the same operations in the same order as the positive.
-#include <type_traits>
-
 #include "kge_rank_common.cuh"
 
 namespace kge {
@@ -73,12 +71,6 @@ constexpr int RL_TQ = 32, RL_TR = 64, RL_RPW = 8, RL_DK = 32, RL_LDS = RL_DK + 4
 constexpr int RL_Q_FLOATS = RL_TQ * RL_LDS, RL_R_FLOATS = RL_TR * RL_LDS;
 constexpr int RL_STAGE_FLOATS = 2 * RL_Q_FLOATS + RL_R_FLOATS;
 
-__device__ __forceinline__ void rl_cp_async16(float *smem_dst, const float *gmem_src, bool valid)
-{
-    const unsigned sz = valid ? 16u : 0u;
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(sz) : "memory");
-}
-
 template <int M>
 __global__ void __launch_bounds__(RL_THREADS, 2) kge_rank_rel_kernel(const RankParams p, const float *__restrict__ rel,
                                                                      const int32_t *__restrict__ triples, int32_t *__restrict__ cnt)
@@ -114,11 +106,11 @@ __global__ void __launch_bounds__(RL_THREADS, 2) kge_rank_rel_kernel(const RankP
         const bool cvalid = d < (HALVES ? kp : ld);
         const int col = cvalid ? (HALVES && c4 >= 4 ? kp : 0) + d : 0;
         const int so = lrow * RL_LDS + 4 * c4;
-        rl_cp_async16(Ss + so, srow + col, cvalid && qvalid);
-        rl_cp_async16(Os + so, orow + col, cvalid && qvalid);
+        cp_async16(Ss + so, srow + col, cvalid && qvalid);
+        cp_async16(Os + so, orow + col, cvalid && qvalid);
 #pragma unroll
-        for (int n = 0; n < 2; ++n) rl_cp_async16(Rs + so + 32 * n * RL_LDS, rrow[n] + col, cvalid && rvalid[n]);
-        asm volatile("cp.async.commit_group;" ::: "memory");
+        for (int n = 0; n < 2; ++n) cp_async16(Rs + so + 32 * n * RL_LDS, rrow[n] + col, cvalid && rvalid[n]);
+        cp_async_commit();
     };
 
     float acc[RL_RPW];
@@ -130,9 +122,9 @@ __global__ void __launch_bounds__(RL_THREADS, 2) kge_rank_rel_kernel(const RankP
         const int buf = it & 1;
         if (it + 1 < n_iter) {
             stage_load(it + 1, buf ^ 1);
-            asm volatile("cp.async.wait_group 1;" ::: "memory");
+            cp_async_wait<1>();
         } else {
-            asm volatile("cp.async.wait_group 0;" ::: "memory");
+            cp_async_wait<0>();
         }
         __syncthreads();
         const float *Ss = smem + buf * RL_STAGE_FLOATS + lane * RL_LDS, *Os = Ss + RL_Q_FLOATS;
@@ -209,9 +201,8 @@ __global__ void __launch_bounds__(RL_THREADS, 2) kge_rank_rel_kernel(const RankP
 }
 
 // --------------------------------------------------------------------------
-// filter kernel (AbstractScoringLayer.py:260-307 on the relation side): one warp per (query, known-true relation) pair
-// stages the pair's s, relation and o rows in shared memory with coalesced 16-byte loads, lane 0 runs rel_score, and the
-// pair counts qpos <= q_f (always '<=').  sm = 3 * ld floats per warp.
+// filter kernel: the filter walk on the relation side, each (query, known-true relation) pair scored by rel_score from
+// its staged s, relation and o rows
 // --------------------------------------------------------------------------
 template <int M>
 __global__ void kge_rank_rel_filter_kernel(const RankParams p, const float *__restrict__ rel, const int32_t *__restrict__ triples,
@@ -219,46 +210,21 @@ __global__ void kge_rank_rel_filter_kernel(const RankParams p, const float *__re
                                            int32_t *__restrict__ cnt)
 {
     extern __shared__ __align__(16) float pair_sm[];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wpc = blockDim.x >> 5;
-    const int ld = p.L.ld;
-    float *sm = pair_sm + (size_t)warp * 3 * ld;
-    const long long total = off[p.b];
-    for (long long f = (long long)blockIdx.x * wpc + warp; f < total; f += (long long)gridDim.x * wpc) {
-        long long lo = 0, hi = p.b;  // largest i with off[i] <= f
-        while (hi - lo > 1) {
-            const long long mid = (lo + hi) >> 1;
-            if (off[mid] <= f) lo = mid; else hi = mid;
-        }
-        const long long i = lo;
-        const long long pos = (long long)idx[f] - p.filt_base;
-        if (pos < p.cand_begin || pos >= p.cand_begin + p.n_cand) continue;  // :280-288 (warp-uniform)
-        const long long id = p.cand_ids ? (long long)p.cand_ids[pos] : pos;
-        const float *s = p.ent + (size_t)triples[3 * i] * ld, *o = p.ent + (size_t)triples[3 * i + 2] * ld;
-        const float *r = rel + (size_t)id * ld;
-        for (int c = lane * 4; c < ld; c += 128) {
-            *reinterpret_cast<float4 *>(sm + c) = *reinterpret_cast<const float4 *>(s + c);
-            *reinterpret_cast<float4 *>(sm + ld + c) = *reinterpret_cast<const float4 *>(r + c);
-            *reinterpret_cast<float4 *>(sm + 2 * ld + c) = *reinterpret_cast<const float4 *>(o + c);
-        }
-        __syncwarp();
-        if (lane == 0 && p.qpos[i] <= quantise(rel_score<M>(sm, sm + ld, sm + 2 * ld, p.L.kp, ld, p.scale)))
-            atomicAdd(&cnt[3 * i + 2], 1);
-        __syncwarp();  // the slice is reused for the warp's next pair
-    }
+    const int lane = threadIdx.x & 31, ld = p.L.ld;
+    float *sm = pair_sm + (size_t)(threadIdx.x >> 5) * 3 * ld;
+    filter_walk(p, off, idx, cnt, [&](long long i, long long id) {
+        return warp_chain<3>(p.ent + (size_t)triples[3 * i] * ld, rel + (size_t)id * ld, p.ent + (size_t)triples[3 * i + 2] * ld, ld,
+                             sm, lane, [&](const float *s, const float *r, const float *o) {
+                                 return rel_score<M>(s, r, o, p.L.kp, ld, p.scale);
+                             });
+    });
 }
 
-// Host side: launch(std::integral_constant<int, M>) for the model's relation-side kernel instance
+// Host side: launch(std::integral_constant<int, M>) for the model's relation-side kernel instance; HolE runs ComplEx's
 template <class Launch>
 static cudaError_t dispatch_rel_model(int model, Launch &&launch)
 {
-    switch (model) {
-    case KGE_TRANSE: return launch(std::integral_constant<int, KGE_TRANSE>{});
-    case KGE_DISTMULT: return launch(std::integral_constant<int, KGE_DISTMULT>{});
-    case KGE_COMPLEX:
-    case KGE_HOLE: return launch(std::integral_constant<int, KGE_COMPLEX>{});
-    case KGE_ROTATE: return launch(std::integral_constant<int, KGE_ROTATE>{});
-    }
-    return cudaErrorInvalidValue;
+    return dispatch_value<KGE_TRANSE, KGE_DISTMULT, KGE_COMPLEX, KGE_ROTATE>(model == KGE_HOLE ? KGE_COMPLEX : model, launch);
 }
 
 cudaError_t launch_rank_rel_count(const RankParams &p, const float *rel, const int32_t *triples, int32_t *cnt, cudaStream_t st)
@@ -275,12 +241,11 @@ cudaError_t launch_rank_rel_filter(const RankParams &p, const float *rel, const 
                                    const int32_t *filt_idx, long long n_pairs, int32_t *cnt, int sm_count, cudaStream_t st)
 {
     if (n_pairs == 0 || p.b == 0) return cudaSuccess;
-    const int wpc = pair_score_warps(p.L.ld, 3);
-    const size_t sm = (size_t)wpc * 3 * p.L.ld * sizeof(float);
-    const long long want = (n_pairs + wpc - 1) / wpc;
+    const PairLaunch pl = pair_launch(p.L.ld, 3);
+    const long long want = (n_pairs + pl.warps - 1) / pl.warps;
     const unsigned grid = (unsigned)(want < (long long)sm_count * 8 ? want : (long long)sm_count * 8);
     return dispatch_rel_model(p.L.model, [&](auto m) {
-        return launch_with_smem(kge_rank_rel_filter_kernel<decltype(m)::value>, grid, wpc * 32, sm, st, p, rel, triples,
+        return launch_with_smem(kge_rank_rel_filter_kernel<decltype(m)::value>, grid, pl.warps * 32, pl.smem, st, p, rel, triples,
                                 filt_off, filt_idx, cnt);
     });
 }

@@ -432,9 +432,9 @@ cudaError_t launch_rank_count_tc(const RankParams &p, const RankTcLayout &w, voi
     const unsigned grid = (unsigned)(w.n_qb * per);
     if (probe_a) return launch_with_smem(kge_rank_tc_kernel<true>, grid, TC_THREADS, smem, st, t);
     if ((e = launch_with_smem(kge_rank_tc_kernel<false>, grid, TC_THREADS, smem, st, t)) != cudaSuccess) return e;
-    const int wpc = pair_score_warps(ld, 2);
-    if ((e = launch_with_smem(kge_rank_refine_kernel, sm_count * 2, wpc * 32, (size_t)wpc * 2 * ld * sizeof(float), st, p, pairs,
-                              count, w.pair_cap, cnt)) != cudaSuccess)
+    const PairLaunch pl = pair_launch(ld, 2);
+    if ((e = launch_with_smem(kge_rank_refine_kernel, sm_count * 2, pl.warps * 32, pl.smem, st, p, pairs, count, w.pair_cap, cnt)) !=
+        cudaSuccess)
         return e;
     // overflow fallback: the exact FP32 kernel, every CTA of which returns at once unless the pair list overflowed
     RankParams g = p;

@@ -50,21 +50,12 @@ int one_vs_all_splits(long long B, long long n_ent)
 
 size_t one_vs_all_smem_bytes(int ld) { return (OVA_STAGE + OVA_GS + (size_t)OVA_T * ld) * sizeof(float); }
 
-__device__ __forceinline__ void ova_cp16(float *smem, const float *gmem, bool valid)
-{
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(smem)), "l"(gmem), "r"(valid ? 16 : 0)
-                 : "memory");
-}
-__device__ __forceinline__ void ova_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void ova_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
 // rows [r0, r0 + 32) x columns [c0, c0 + 32) of the [nrows, ld] matrix M -> dst (row stride OVA_LDS), zero past its ends
 __device__ __forceinline__ void ova_stage(float *dst, const float *M, long long r0, long long nrows, int ld, int c0, int tid)
 {
     const int r = tid >> 3, c = (tid & 7) * 4;
     const bool ok = r0 + r < nrows && c0 + c < ld;
-    ova_cp16(dst + r * OVA_LDS + c, ok ? M + (size_t)(r0 + r) * ld + c0 + c : M, ok);
+    cp_async16(dst + r * OVA_LDS + c, ok ? M + (size_t)(r0 + r) * ld + c0 + c : M, ok);
 }
 
 __device__ __forceinline__ float4 ova_lds4(const float *p) { return *reinterpret_cast<const float4 *>(p); }
@@ -86,17 +77,17 @@ __device__ __forceinline__ void ova_logits(const float *Q, long long q0, long lo
     const int nchunk = (ld + OVA_DK - 1) / OVA_DK;
     ova_stage(stage, Q, q0, nq, ld, 0, tid);
     ova_stage(stage + OVA_CHUNK, X, e0, ne, ld, 0, tid);
-    ova_commit();
+    cp_async_commit();
     for (int c = 0; c < nchunk; ++c) {
         const float *buf = stage + (c & 1) * 2 * OVA_CHUNK;
         if (c + 1 < nchunk) {
             float *nb = stage + ((c + 1) & 1) * 2 * OVA_CHUNK;
             ova_stage(nb, Q, q0, nq, ld, (c + 1) * OVA_DK, tid);
             ova_stage(nb + OVA_CHUNK, X, e0, ne, ld, (c + 1) * OVA_DK, tid);
-            ova_commit();
-            ova_wait<1>();
+            cp_async_commit();
+            cp_async_wait<1>();
         } else {
-            ova_wait<0>();
+            cp_async_wait<0>();
         }
         __syncthreads();
         const float *qs = buf + 2 * ty * OVA_LDS, *xs = buf + OVA_CHUNK + tx * OVA_LDS;
@@ -122,15 +113,15 @@ __device__ __forceinline__ void ova_accumulate(float *acc_s, const float *gs, co
     const int o = tid >> 3, c4 = (tid & 7) * 4;
     const int nchunk = (ld + OVA_DK - 1) / OVA_DK;
     ova_stage(stage, M, r0, nrows, ld, 0, tid);
-    ova_commit();
+    cp_async_commit();
     for (int c = 0; c < nchunk; ++c) {
         const float *buf = stage + (c & 1) * OVA_CHUNK;
         if (c + 1 < nchunk) {
             ova_stage(stage + ((c + 1) & 1) * OVA_CHUNK, M, r0, nrows, ld, (c + 1) * OVA_DK, tid);
-            ova_commit();
-            ova_wait<1>();
+            cp_async_commit();
+            cp_async_wait<1>();
         } else {
-            ova_wait<0>();
+            cp_async_wait<0>();
         }
         __syncthreads();
         const int col = c * OVA_DK + c4;
@@ -393,26 +384,17 @@ __global__ void kge_ova_stamp_kernel(int *stamps, long long n, int stamp)
         stamps[i] = stamp;
 }
 
-template <class Kernel>
-static cudaError_t ova_launch(Kernel kern, dim3 grid, size_t smem, const OneVsAllSide &s, cudaStream_t st)
-{
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    kern<<<grid, OVA_THREADS, smem, st>>>(s);
-    return cudaGetLastError();
-}
-
 cudaError_t launch_one_vs_all_side(const OneVsAllSide &s, int halves, cudaStream_t st)
 {
     if (s.B == 0) return cudaSuccess;
     const unsigned n_qt = (unsigned)((s.B + OVA_T - 1) / OVA_T), n_et = (unsigned)((s.n_ent + OVA_T - 1) / OVA_T);
     const size_t big = one_vs_all_smem_bytes(s.ld);
-    cudaError_t e = ova_launch(kge_ova_stats_kernel, dim3(n_qt, s.nsplit), OVA_STAGE * sizeof(float), s, st);
+    cudaError_t e = launch_with_smem(kge_ova_stats_kernel, dim3(n_qt, s.nsplit), OVA_THREADS, OVA_STAGE * sizeof(float), st, s);
     if (e != cudaSuccess) return e;
     kge_ova_merge_kernel<<<(unsigned)((s.B + 255) / 256), 256, 0, st>>>(s);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    if ((e = ova_launch(kge_ova_dq_kernel, dim3(n_qt, s.nsplit), big, s, st)) != cudaSuccess) return e;
-    if ((e = ova_launch(kge_ova_dx_kernel, dim3(n_et), big, s, st)) != cudaSuccess) return e;
+    if ((e = launch_with_smem(kge_ova_dq_kernel, dim3(n_qt, s.nsplit), OVA_THREADS, big, st, s)) != cudaSuccess) return e;
+    if ((e = launch_with_smem(kge_ova_dx_kernel, dim3(n_et), OVA_THREADS, big, st, s)) != cudaSuccess) return e;
     const unsigned grid = (unsigned)((s.B * (s.kp / 4) + 255) / 256);
     if (halves == 2) kge_ova_chain_kernel<2><<<grid, 256, 0, st>>>(s);
     else kge_ova_chain_kernel<1><<<grid, 256, 0, st>>>(s);

@@ -450,7 +450,7 @@ static cudaError_t launch_persistent(Kernel kern, const TrainParams &p, const Tr
     if (p.B == 0) return cudaSuccess;
     const int threads = slot.warps * 32;
     const size_t smem = (size_t)slot.warps * slot.region_bytes;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = allow_dynamic_smem(kern, smem);
     if (e != cudaSuccess) return e;
     int occ = 0;
     e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem);

@@ -1637,3 +1637,104 @@ extern "C" int kge_one_vs_all_step(kge_handle *h, int32_t sides, int32_t loss_re
     }
     return KGE_OK;
 }
+
+// ---- KvsAll training (kge_train_1vsall.cu) ------------------------------------------------------------------
+
+// Carve-up of the workspace of a KvsAll step of B queries: what launch_rank_prepare writes (both sides' query vectors
+// and the quantised positive scores) and the per-split partial Gq rows.  The loss is element-wise: no row statistics.
+struct KVsAllWorkspace {
+    float *qs, *qo;
+    int32_t *qpos;
+    float *pgq;
+    int nsplit;
+};
+static KVsAllWorkspace carve_k_vs_all(const kge_handle *h, int64_t B, Carve &c)
+{
+    KVsAllWorkspace w;
+    w.nsplit = one_vs_all_splits(B, h->cfg.n_ent);
+    const size_t rows = (size_t)B * h->L.ld * sizeof(float);
+    w.qs = c.take<float>(rows, 16);
+    w.qo = c.take<float>(rows, 16);
+    w.qpos = c.take<int32_t>((size_t)B * sizeof(int32_t), 16);
+    w.pgq = c.take<float>((size_t)w.nsplit * rows, 16);
+    return w;
+}
+
+extern "C" int64_t kge_k_vs_all_workspace_bytes(const kge_handle *h, int64_t B)
+{
+    if (!h || B < 0) return 0;
+    Carve c(nullptr);
+    carve_k_vs_all(h, B, c);
+    return (int64_t)c.at;
+}
+
+extern "C" int kge_k_vs_all_step(kge_handle *h, int32_t side, int32_t loss_reduction, float label_smoothing,
+                                 const float *ent_dev, const float *rel_dev, float *grad_ent_dev, float *grad_rel_dev,
+                                 const int32_t *queries_dev, int64_t B, const int64_t *label_offsets_dev,
+                                 const int32_t *label_ids_dev, uint64_t step, double *loss_dev, void *ws_dev,
+                                 int64_t ws_bytes, void *stream)
+{
+    KGE_CHECK_HANDLE(h, "kge_k_vs_all_step");
+    const int model = h->cfg.scoring;
+    if (model != KGE_DISTMULT && model != KGE_COMPLEX && model != KGE_HOLE)
+        return fail(KGE_ERR_UNSUPPORTED, "kge_k_vs_all_step: KvsAll training is implemented for DistMult, ComplEx and HolE "
+                                         "(inner-product scores); not for scoring type %d", model);
+    if (side != KGE_ONE_VS_ALL_S && side != KGE_ONE_VS_ALL_O)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_k_vs_all_step: side must be KGE_ONE_VS_ALL_S or KGE_ONE_VS_ALL_O, got %d",
+                    side);
+    if (loss_reduction != KGE_REDUCE_SUM && loss_reduction != KGE_REDUCE_MEAN)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "Invalid value for reduction!");
+    if (!(label_smoothing >= 0.f && label_smoothing < 1.f))
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_k_vs_all_step: label_smoothing must be in [0, 1), got %g",
+                    (double)label_smoothing);
+    if (int rc = check_no_pending(h, "kge_k_vs_all_step")) return rc;
+    if (h->cfg.n_ent < 2) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_k_vs_all_step: needs n_ent >= 2");
+    if ((long long)k_vs_all_smem_bytes(h->L.ld) > h->max_smem)
+        return fail(KGE_ERR_UNSUPPORTED, "kge_k_vs_all_step: rows of %d floats exceed the shared-memory tiles of the KvsAll "
+                                         "kernels (%d B)", h->L.ld, h->max_smem);
+    if (B < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_k_vs_all_step: B < 0");
+    if (B == 0) return KGE_OK;
+    if (!ent_dev || !rel_dev || !grad_ent_dev || !grad_rel_dev || !queries_dev || !label_offsets_dev || !label_ids_dev)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_k_vs_all_step: null table, gradient, queries or labels");
+    if (int rc = check_workspace(ws_dev, ws_bytes, kge_k_vs_all_workspace_bytes(h, B), 16, "kge_k_vs_all_step",
+                                 "kge_k_vs_all_workspace_bytes"))
+        return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    Carve c(ws_dev);
+    const KVsAllWorkspace w = carve_k_vs_all(h, B, c);
+    ShardView sv;
+    memset(&sv, 0, sizeof(sv));
+    KGE_CUDA(launch_rank_prepare(h->L, sv, ent_dev, rel_dev, nullptr, queries_dev, B, h->score_scale, w.qs, w.qo, nullptr,
+                                 w.qpos, st),
+             "kge_k_vs_all_step (query vectors)");
+    const int stamp = kge_step_stamp(step);
+    // the same looked-up rows as a 1vsAll step: every entity row, and the relation rows of the batch (chain pass)
+    if (h->stamp_ent) KGE_CUDA(launch_one_vs_all_stamps(h->stamp_ent, h->cfg.n_ent, stamp, st), "kge_k_vs_all_step (stamps)");
+    OneVsAllSide s;
+    memset(&s, 0, sizeof(s));
+    s.ent = ent_dev;
+    s.rel = rel_dev;
+    s.grad_ent = grad_ent_dev;
+    s.grad_rel = grad_rel_dev;
+    s.triples = queries_dev;
+    s.B = B;
+    s.n_ent = h->cfg.n_ent;
+    s.side = side == KGE_ONE_VS_ALL_S ? KGE_SIDE_S : KGE_SIDE_O;
+    s.col = side == KGE_ONE_VS_ALL_S ? 0 : 2;
+    s.q = side == KGE_ONE_VS_ALL_S ? w.qs : w.qo;
+    s.kp = h->L.kp;
+    s.ld = h->L.ld;
+    s.nsplit = w.nsplit;
+    s.scale = h->score_scale;
+    s.w = loss_reduction == KGE_REDUCE_MEAN ? (float)(1.0 / (double)h->cfg.n_ent) : 1.f;
+    s.loss = loss_dev;
+    s.stamp = stamp;
+    s.stamp_rel = h->stamp_ent ? h->stamp_rel : nullptr;
+    s.pgq = w.pgq;
+    s.label_off = (const long long *)label_offsets_dev;
+    s.label_ids = label_ids_dev;
+    s.y0 = (float)((double)label_smoothing / (double)h->cfg.n_ent);
+    s.y1 = (float)(1.0 - (double)label_smoothing);
+    KGE_CUDA(launch_k_vs_all_side(s, h->L.halves, st), "kge_k_vs_all_step");
+    return KGE_OK;
+}

@@ -96,16 +96,26 @@ struct OneVsAllSide {
     long long B, n_ent;
     int side, col;           // KGE_SIDE_S / KGE_SIDE_O; the triple column of the positive's own entity (0 / 2)
     int kp, ld, nsplit;      // nsplit = one_vs_all_splits(B, n_ent) entity ranges per query tile
-    float scale, w;          // HolE's score scale (1 otherwise); weight of a negative's exp (1 or 1 / (n_ent - 1))
+    float scale, w;          // HolE's score scale (1 otherwise); weight of a negative's exp (1 or 1 / (n_ent - 1));
+                             // KvsAll: weight of every element (1 or 1 / n_ent)
     double *loss;            // += sum of the row losses, or nullptr
     int stamp;
     int *stamp_rel;          // lazy-optimizer stamps of the relation rows, or nullptr
-    // workspace: [nsplit, B] partial maxima and sums; [B] l_t, max and 1 / D per row; [nsplit, B, ld] partial Gq rows
+    // workspace: [nsplit, B] partial maxima and sums; [B] l_t, max and 1 / D per row (1vsAll only); [nsplit, B, ld]
+    // partial Gq rows
     float *pm, *pz, *lt, *row_m, *row_inv, *pgq;
+    // KvsAll: the labels of query b are label_ids[label_off[b] .. label_off[b + 1]) (ascending, distinct, < n_ent);
+    // target of an entity: y0 = eps / n_ent, plus y1 = 1 - eps for a label
+    const long long *label_off;
+    const int32_t *label_ids;
+    float y0, y1;
 };
 int one_vs_all_splits(long long B, long long n_ent);
 size_t one_vs_all_smem_bytes(int ld);  // dynamic shared memory of the dQ and dX passes
+size_t k_vs_all_smem_bytes(int ld);    // the same with KvsAll's label masks
 cudaError_t launch_one_vs_all_side(const OneVsAllSide &s, int halves, cudaStream_t st);
+// one side of a KvsAll multi-label step (kge_k_vs_all_step): s.triples are the [B, 3] queries, s.label_* set
+cudaError_t launch_k_vs_all_side(const OneVsAllSide &s, int halves, cudaStream_t st);
 cudaError_t launch_one_vs_all_stamps(int *stamp_ent, long long n_ent, int stamp, cudaStream_t st);
 
 // kge_misc.cu

@@ -23,6 +23,13 @@
 //          (kge_train_common.cuh), added with red.global.add like theirs.
 // Every pass scores a (query, entity) pair with the same chain: one fma per column in ascending order, so the logits
 // of the three passes that form them are bit-identical.
+//
+// KvsAll (kge_k_vs_all_step; DESIGN.md 3.13) trains each distinct (s, p) (side o) or (p, o) (side s) query against
+// every entity with the multi-label NLL: target y'_e = (1 - eps) [e is a label] + eps / n_ent, weight w = 1 (sum) or
+// 1 / n_ent (mean), loss = w * sum_e softplus(l_e) - y'_e l_e, dL/dl_e = in_e * w * (sigmoid(l_e) - y'_e).  The loss is
+// element-wise, so a side is the dQ pass (which also adds the loss), the dX pass and the chain pass above, with the
+// multi-label rule in place of the multiclass one.  The labels are a CSR (ascending ids per query); each 32 x 32 tile
+// reads them as one 32-bit mask per query row, built in shared memory from the row's slice.
 #include <math.h>
 
 #include "kge_train_common.cuh"
@@ -253,6 +260,107 @@ __global__ void __launch_bounds__(256) kge_ova_merge_kernel(const OneVsAllSide s
     if ((threadIdx.x & 31) == 0 && s.loss) atomicAdd(s.loss, (double)loss);
 }
 
+// The per-element rules of the dQ and dX passes.  Each pass calls, per CTA and tile:
+//   dq_begin(q0, first entity of the split)   once, before the dQ pass's first entity tile;
+//   dq_tile(e0) / dx_tile(q0, e0)             before the tile's ova_logits (whose barriers publish what it writes);
+//   grad<LOSS>(acc, b, i, c, e)               dL/dl of row b = q0 + 2 ty + i (the thread's i-th row) and entity
+//                                             e = e0 + c, zero outside the batch or past n_ent; LOSS (dQ only) also
+//                                             adds the element's loss to the thread's partial sum;
+//   dq_end()                                  once, after the dQ pass.
+// 1vsAll: the multiclass rule, with each row's target, max and 1 / D from the merge pass.
+struct OvaMulticlass {
+    const OneVsAllSide &s;
+    long long tgt[2];
+    float m[2], inv[2];
+    __device__ __forceinline__ OvaMulticlass(const OneVsAllSide &s_, float *) : s(s_) {}
+    __device__ __forceinline__ void rows(long long q0, int tid)
+    {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const long long b = q0 + 2 * (tid >> 4) + i;
+            tgt[i] = b < s.B ? s.triples[3 * b + s.col] : -1;
+            m[i] = b < s.B ? s.row_m[b] : 0.f;
+            inv[i] = b < s.B ? s.row_inv[b] : 0.f;
+        }
+    }
+    __device__ __forceinline__ void dq_begin(long long q0, long long, int tid) { rows(q0, tid); }
+    __device__ __forceinline__ void dq_tile(long long, int) {}
+    __device__ __forceinline__ void dx_tile(long long q0, long long, int tid) { rows(q0, tid); }
+    template <bool LOSS>
+    __device__ __forceinline__ float grad(float acc, long long, int i, int, long long e)
+    {
+        return (tgt[i] >= 0 && e < s.n_ent) ? ova_grad(acc, s, e, tgt[i], m[i], inv[i]) : 0.f;
+    }
+    __device__ __forceinline__ void dq_end() {}
+};
+
+// KvsAll: the multi-label rule.  Thread r < 32 keeps row q0 + r's cursor into its label slice and writes the row's
+// mask of the current entity tile (bit c: entity e0 + c is a label) to shared memory.
+struct KvaMultiLabel {
+    const OneVsAllSide &s;
+    unsigned *mask;       // [32] in shared memory
+    long long cur, end;   // thread r < 32: next label of row q0 + r not yet in a mask, and the end of its slice
+    float loss;           // the thread's partial loss (dQ)
+    __device__ __forceinline__ KvaMultiLabel(const OneVsAllSide &s_, float *mask_)
+        : s(s_), mask(reinterpret_cast<unsigned *>(mask_)), cur(0), end(0), loss(0.f) {}
+    // thread r < 32: the cursor of row q0 + r at its first label >= e (lower_bound over the ascending slice)
+    __device__ __forceinline__ void seek(long long q0, long long e, int tid)
+    {
+        if (tid >= OVA_T) return;
+        const long long b = q0 + tid;
+        cur = end = 0;
+        if (b >= s.B) return;
+        long long lo = s.label_off[b], hi = s.label_off[b + 1];
+        end = hi;
+        while (lo < hi) {
+            const long long mid = (lo + hi) >> 1;
+            if (s.label_ids[mid] < e) lo = mid + 1;
+            else hi = mid;
+        }
+        cur = lo;
+    }
+    // thread r < 32: the labels of row q0 + r in [e0, e0 + 32) -> mask[r]; the cursor moves past them
+    __device__ __forceinline__ void build(long long e0, int tid)
+    {
+        if (tid >= OVA_T) return;
+        unsigned bits = 0;
+        for (; cur < end; ++cur) {
+            const long long d = s.label_ids[cur] - e0;
+            if (d >= OVA_T) break;
+            bits |= 1u << d;
+        }
+        mask[tid] = bits;
+    }
+    __device__ __forceinline__ void dq_begin(long long q0, long long e_first, int tid) { seek(q0, e_first, tid); }
+    __device__ __forceinline__ void dq_tile(long long e0, int tid) { build(e0, tid); }
+    __device__ __forceinline__ void dx_tile(long long q0, long long e0, int tid)
+    {
+        seek(q0, e0, tid);
+        build(e0, tid);
+    }
+    template <bool LOSS>
+    __device__ __forceinline__ float grad(float acc, long long b, int i, int c, long long e)
+    {
+        if (b >= s.B || e >= s.n_ent) return 0.f;
+        const int r = 2 * (threadIdx.x >> 4) + i;
+        const float y = (mask[r] >> c) & 1u ? s.y0 + s.y1 : s.y0;
+        bool in;
+        const float l = ova_clip(acc, s.scale, in);
+        const float z = expf(-fabsf(l));  // e^-|l| <= 1: neither the sigmoid nor the softplus can overflow
+        if (LOSS) loss += (fmaxf(l, 0.f) - y * l) + log1pf(z);
+        if (!in) return 0.f;
+        const float r1 = 1.f / (1.f + z);
+        return s.w * ((l >= 0.f ? r1 : z * r1) - y);
+    }
+    __device__ __forceinline__ void dq_end()
+    {
+        const float t = warp_sum(loss);
+        if ((threadIdx.x & 31) == 0 && s.loss) atomicAdd(s.loss, (double)(s.w * t));
+    }
+};
+
+// dQ (query tile x entity split).  Shared memory: stage, g tile, [32, ld] accumulator, then the rule's [32] masks.
+template <class Rule>
 __global__ void __launch_bounds__(OVA_THREADS) kge_ova_dq_kernel(const OneVsAllSide s)
 {
     extern __shared__ __align__(16) float ova_sm[];
@@ -262,17 +370,11 @@ __global__ void __launch_bounds__(OVA_THREADS) kge_ova_dq_kernel(const OneVsAllS
     long long et0, et1;
     ova_split_range(s, split, et0, et1);
     ova_zero(acc_s, OVA_T * s.ld, tid);
-    long long tgt[2];
-    float m[2], inv[2];
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-        const long long b = q0 + 2 * ty + i;
-        tgt[i] = b < s.B ? s.triples[3 * b + s.col] : -1;
-        m[i] = b < s.B ? s.row_m[b] : 0.f;
-        inv[i] = b < s.B ? s.row_inv[b] : 0.f;
-    }
+    Rule rule(s, acc_s + (size_t)OVA_T * s.ld);
+    rule.dq_begin(q0, et0 * OVA_T, tid);
     for (long long et = et0; et < et1; ++et) {
         const long long e0 = et * OVA_T;
+        rule.dq_tile(e0, tid);
         float acc[2][2];
         ova_logits(s.q, q0, s.B, s.ent, e0, s.n_ent, s.ld, stage, tid, acc);
 #pragma unroll
@@ -281,11 +383,12 @@ __global__ void __launch_bounds__(OVA_THREADS) kge_ova_dq_kernel(const OneVsAllS
             for (int j = 0; j < 2; ++j) {
                 const long long e = e0 + tx + 16 * j;
                 gs[(2 * ty + i) * (OVA_T + 1) + tx + 16 * j] =
-                    (tgt[i] >= 0 && e < s.n_ent) ? ova_grad(acc[i][j], s, e, tgt[i], m[i], inv[i]) : 0.f;
+                    rule.template grad<true>(acc[i][j], q0 + 2 * ty + i, i, tx + 16 * j, e);
             }
         __syncthreads();
         ova_accumulate<false>(acc_s, gs, s.ent, e0, s.n_ent, s.ld, stage, tid);
     }
+    rule.dq_end();
     // this split's partial Gq rows, scale included
     const int o = tid >> 3;
     const long long b = q0 + o;
@@ -296,6 +399,8 @@ __global__ void __launch_bounds__(OVA_THREADS) kge_ova_dq_kernel(const OneVsAllS
         }
 }
 
+// dX (one entity tile, every query tile); the same shared memory as dQ
+template <class Rule>
 __global__ void __launch_bounds__(OVA_THREADS) kge_ova_dx_kernel(const OneVsAllSide s)
 {
     extern __shared__ __align__(16) float ova_sm[];
@@ -303,23 +408,21 @@ __global__ void __launch_bounds__(OVA_THREADS) kge_ova_dx_kernel(const OneVsAllS
     const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
     const long long e0 = (long long)blockIdx.x * OVA_T;
     ova_zero(acc_s, OVA_T * s.ld, tid);
+    Rule rule(s, acc_s + (size_t)OVA_T * s.ld);
     const long long n_qt = (s.B + OVA_T - 1) / OVA_T;
     for (long long qt = 0; qt < n_qt; ++qt) {
         const long long q0 = qt * OVA_T;
+        rule.dx_tile(q0, e0, tid);
         float acc[2][2];
         ova_logits(s.q, q0, s.B, s.ent, e0, s.n_ent, s.ld, stage, tid, acc);
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-            const long long b = q0 + 2 * ty + i;
-            const bool row = b < s.B;
-            const long long t = row ? s.triples[3 * b + s.col] : -1;
-            const float m = row ? s.row_m[b] : 0.f, inv = row ? s.row_inv[b] : 0.f;
+        for (int i = 0; i < 2; ++i)
 #pragma unroll
             for (int j = 0; j < 2; ++j) {
                 const long long e = e0 + tx + 16 * j;
-                gs[(2 * ty + i) * (OVA_T + 1) + tx + 16 * j] = (row && e < s.n_ent) ? ova_grad(acc[i][j], s, e, t, m, inv) : 0.f;
+                gs[(2 * ty + i) * (OVA_T + 1) + tx + 16 * j] =
+                    rule.template grad<false>(acc[i][j], q0 + 2 * ty + i, i, tx + 16 * j, e);
             }
-        }
         __syncthreads();
         ova_accumulate<true>(acc_s, gs, s.q, q0, s.B, s.ld, stage, tid);
     }
@@ -384,21 +487,37 @@ __global__ void kge_ova_stamp_kernel(int *stamps, long long n, int stamp)
         stamps[i] = stamp;
 }
 
-cudaError_t launch_one_vs_all_side(const OneVsAllSide &s, int halves, cudaStream_t st)
+// the dQ, dX and chain passes of one side under the per-element rule Rule (smem: dynamic bytes of dQ and dX)
+template <class Rule>
+static cudaError_t launch_grad_passes(const OneVsAllSide &s, int halves, size_t smem, cudaStream_t st)
 {
-    if (s.B == 0) return cudaSuccess;
     const unsigned n_qt = (unsigned)((s.B + OVA_T - 1) / OVA_T), n_et = (unsigned)((s.n_ent + OVA_T - 1) / OVA_T);
-    const size_t big = one_vs_all_smem_bytes(s.ld);
-    cudaError_t e = launch_with_smem(kge_ova_stats_kernel, dim3(n_qt, s.nsplit), OVA_THREADS, OVA_STAGE * sizeof(float), st, s);
-    if (e != cudaSuccess) return e;
-    kge_ova_merge_kernel<<<(unsigned)((s.B + 255) / 256), 256, 0, st>>>(s);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    if ((e = launch_with_smem(kge_ova_dq_kernel, dim3(n_qt, s.nsplit), OVA_THREADS, big, st, s)) != cudaSuccess) return e;
-    if ((e = launch_with_smem(kge_ova_dx_kernel, dim3(n_et), OVA_THREADS, big, st, s)) != cudaSuccess) return e;
+    cudaError_t e;
+    if ((e = launch_with_smem(kge_ova_dq_kernel<Rule>, dim3(n_qt, s.nsplit), OVA_THREADS, smem, st, s)) != cudaSuccess) return e;
+    if ((e = launch_with_smem(kge_ova_dx_kernel<Rule>, dim3(n_et), OVA_THREADS, smem, st, s)) != cudaSuccess) return e;
     const unsigned grid = (unsigned)((s.B * (s.kp / 4) + 255) / 256);
     if (halves == 2) kge_ova_chain_kernel<2><<<grid, 256, 0, st>>>(s);
     else kge_ova_chain_kernel<1><<<grid, 256, 0, st>>>(s);
     return cudaGetLastError();
+}
+
+cudaError_t launch_one_vs_all_side(const OneVsAllSide &s, int halves, cudaStream_t st)
+{
+    if (s.B == 0) return cudaSuccess;
+    const unsigned n_qt = (unsigned)((s.B + OVA_T - 1) / OVA_T);
+    cudaError_t e = launch_with_smem(kge_ova_stats_kernel, dim3(n_qt, s.nsplit), OVA_THREADS, OVA_STAGE * sizeof(float), st, s);
+    if (e != cudaSuccess) return e;
+    kge_ova_merge_kernel<<<(unsigned)((s.B + 255) / 256), 256, 0, st>>>(s);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    return launch_grad_passes<OvaMulticlass>(s, halves, one_vs_all_smem_bytes(s.ld), st);
+}
+
+size_t k_vs_all_smem_bytes(int ld) { return one_vs_all_smem_bytes(ld) + OVA_T * sizeof(unsigned); }
+
+cudaError_t launch_k_vs_all_side(const OneVsAllSide &s, int halves, cudaStream_t st)
+{
+    if (s.B == 0) return cudaSuccess;
+    return launch_grad_passes<KvaMultiLabel>(s, halves, k_vs_all_smem_bytes(s.ld), st);
 }
 
 cudaError_t launch_one_vs_all_stamps(int *stamp_ent, long long n_ent, int stamp, cudaStream_t st)

@@ -128,3 +128,33 @@ class FilterIndex:
             off = np.zeros(len(t) + 1, dtype=np.int64)
             np.cumsum(np.bincount(row, minlength=len(t)), out=off[1:])
         return off, np.ascontiguousarray(ids, dtype=np.int32)
+
+
+def k_vs_all_queries(findex, triples, side):
+    """The KvsAll training rows of one side (DESIGN.md 3.13): every distinct (s, p) of `triples` for side 'o', every
+    distinct (p, o) for side 's', in order of first appearance, each labelled with its known objects (subjects) in
+    `findex` (a FilterIndex of the same triples).  -> (queries int32 [n, 3], offsets int64 [n + 1], ids int32 [nnz]):
+    the labels of query i are ids[offsets[i]:offsets[i + 1]], ascending and distinct; the answer column of a query
+    holds its first label, so that every column is a valid entity id."""
+    t = np.asarray(triples, dtype=np.int64).reshape(-1, 3)
+    col = 2 if side == "o" else 0
+    keys = t[:, 1] * findex.n_ent + t[:, 2 - col]
+    _, first = np.unique(keys, return_index=True)
+    queries = np.ascontiguousarray(t[np.sort(first)], dtype=np.int32)
+    off, ids = findex.lookup(queries, side)
+    queries[:, col] = ids[off[:-1]]
+    return queries, off, ids
+
+
+def k_vs_all_steps(n_o, n_s, batch_size):
+    """The steps of one KvsAll epoch over n_o side-o and n_s side-s queries -> list of ((o_lo, o_hi), (s_lo, s_hi)).
+    A single side (the other count 0) is cut into sequential slices of batch_size queries.  Both sides: S =
+    ceil((n_o + n_s) / batch_size) steps, step i taking the queries [floor(i n / S), floor((i + 1) n / S)) of each
+    side, so that every step mixes the two in proportion and holds at most batch_size + 1 queries."""
+    n_o, n_s, bs = int(n_o), int(n_s), int(batch_size)
+    if n_o == 0 or n_s == 0:
+        n = n_o + n_s
+        cut = [(lo, min(lo + bs, n)) for lo in range(0, n, bs)]
+        return [(c, (0, 0)) if n_o else ((0, 0), c) for c in cut]
+    S = -(-(n_o + n_s) // bs)
+    return [((i * n_o // S, (i + 1) * n_o // S), (i * n_s // S, (i + 1) * n_s // S)) for i in range(S)]

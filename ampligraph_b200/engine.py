@@ -68,6 +68,15 @@ def one_vs_all_workspace_bytes(B, n_ent, ld):
     return 2 * r16(rows) + r16(col) + 2 * r16(ns * col) + 3 * r16(col) + r16(ns * rows)
 
 
+def k_vs_all_workspace_bytes(B, n_ent, ld):
+    """kge_k_vs_all_workspace_bytes(h, B): both sides' query vectors [B, ld], the quantised positive scores [B] and the
+    per-split partial query gradients [nsplit, B, ld], each region padded to 16 bytes (no row statistics)."""
+    r16 = lambda n: (n + 15) // 16 * 16
+    B, ns = int(B), one_vs_all_splits(B, n_ent)
+    rows = 4 * B * int(ld)
+    return 2 * r16(rows) + r16(4 * B) + r16(ns * rows)
+
+
 INT32_MAX = 2 ** 31 - 1
 DBSCAN_BATCH = 1024  # queries per kge_radius_* call of KGEEngine.dbscan (discovery.find_duplicates' batch)
 
@@ -426,6 +435,36 @@ class KGEEngine:
         self._last_step = int(step)
         # query vectors (two kernels), entity stamps, five passes per side
         self.launches += 2 + (1 if self.lazy else 0) + 5 * (2 if sides == "s,o" else 1)
+
+    @_traced("kge.k_vs_all_step")
+    def k_vs_all_backward(self, queries, side, label_offsets, label_ids, label_smoothing=0.0, step=0):
+        """KvsAll step up to tape.gradient (kge_k_vs_all_step, DESIGN.md 3.13): the multi-label NLL of every query row
+        of `queries` (int32 [B, 3] on the device) against every entity on `side` ('o': (s, p) queries, 's': (p, o)),
+        with the engine's reduction and label smoothing eps; accumulates into g_ent / g_rel and loss_acc[0] like
+        forward_backward.  The labels of query b are label_ids[label_offsets[b]:label_offsets[b + 1]] (int64 offsets
+        [B + 1], absolute into the int32 id array; ascending and distinct per query): a batch is a slice of the
+        queries and of the offsets over the same id array.  step: the lazy optimizer's row stamp (every entity row and
+        the batch's relation rows count as looked up).  apply_gradients() takes its non-deferred path next."""
+        assert queries.dtype == torch.int32 and queries.is_cuda and queries.is_contiguous()
+        assert label_offsets.dtype == torch.int64 and label_offsets.is_cuda and label_offsets.is_contiguous()
+        assert label_ids.dtype == torch.int32 and label_ids.is_cuda and label_ids.is_contiguous()
+        if side not in ("s", "o"):
+            raise ValueError("k_vs_all_backward: side must be 's' or 'o', got %r" % (side,))
+        if self._deferred:
+            raise ValueError("k_vs_all_backward: the replaced-row sum of a deferred step is pending (apply_gradients first)")
+        B = queries.shape[0]
+        assert label_offsets.numel() == B + 1
+        need = int(self.lib.kge_k_vs_all_workspace_bytes(self.h, B))
+        if getattr(self, "_kva_ws", None) is None or self._kva_ws.numel() < need:
+            self._kva_ws = torch.empty(max(need, 16), dtype=torch.uint8, device=self.device)  # 256-byte aligned (torch)
+        _lib.check(self.lib.kge_k_vs_all_step(
+            self.h, _lib.ONE_VS_ALL_SIDES[side], _lib.REDUCTIONS[self.reduction], float(label_smoothing), _ptr(self.ent),
+            _ptr(self.rel), _ptr(self.g_ent), _ptr(self.g_rel), _ptr(queries), B, _ptr(label_offsets), _ptr(label_ids),
+            int(step), _ptr(self.loss_acc), _ptr(self._kva_ws), need, self._stream()))
+        self._last_step = int(step)
+        # query vectors (two kernels), entity stamps, dQ, dX and chain
+        if B:
+            self.launches += 2 + (1 if self.lazy else 0) + 3
 
     def _one_block(self):
         """True when tables, gradients and slots still ARE the [ent | rel] blocks allocated here (callers may rebind them: the

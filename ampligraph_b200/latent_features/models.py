@@ -3,13 +3,15 @@
 KGEEngine.  Only the loops and the host-side data plumbing live here; every number is
 produced by libkge_b200.so.
 """
+import math
+import numbers
 import pickle
 
 import numpy as np
 import torch
 
 from .. import _lib
-from ..datasets import DataIndexer, FilterIndex, as_triple_array
+from ..datasets import DataIndexer, FilterIndex, as_triple_array, k_vs_all_queries, k_vs_all_steps
 from ..engine import KGEEngine
 from ..evaluation import hits_at_n_score, mr_score, mrr_score, train_test_split_no_unseen
 from . import initializers, loss_functions, optimizers, regularizers
@@ -208,7 +210,8 @@ class ScoringBasedEmbeddingModel:
     def fit(self, x=None, batch_size=1000, epochs=100, verbose=True, callbacks=None, validation_split=0.0,
             validation_data=None, shuffle=True, initial_epoch=0, validation_batch_size=10,
             validation_corrupt_side="s,o", validation_freq=10, validation_burn_in=0, validation_filter=False,
-            validation_entities_subset=None, partitioning_k=1, focusE=False, focusE_params={}, one_vs_all=None):
+            validation_entities_subset=None, partitioning_k=1, focusE=False, focusE_params={}, one_vs_all=None,
+            k_vs_all=None, label_smoothing=0.0):
         """fit (:544-883).  `shuffle` is accepted and ignored exactly like the reference
         (batches are the sequential slices of graph_data_loader.py:495-500).  validation_split: carve the validation
         set out of x with train_test_split_no_unseen(x, test_size=validation_split, seed=self.seed), as the reference
@@ -219,8 +222,20 @@ class ScoringBasedEmbeddingModel:
         given sides, with the multiclass NLL over all of them (the setting of the reference's multiclass_nll
         docstring, loss_functions.py:580-590; DESIGN.md 3.12).  eta and the corruption seed are then unused.  It needs
         DistMult, ComplEx or HolE and the compiled loss 'multiclass_nll' (either reduction), on one GPU without
-        focusE."""
+        focusE.
+
+        k_vs_all (extension): 's,o', 'o' or 's' trains KvsAll instead (Ruffinelli et al., ICLR 2020; DESIGN.md 3.13):
+        every distinct (s, p) of x (side 'o') or (p, o) (side 's') is one training row, scored against every entity,
+        with target 1 for its known objects (subjects) in x and 0 for the rest, under the compiled loss 'nll' (binary
+        cross-entropy on each (query, entity) pair; reduction 'mean' averages over the n_ent entities).  Queries keep
+        the order of their first appearance in x.  With both sides an epoch has ceil((n_o + n_s) / batch_size)
+        steps, each taking its share of both sides' queries; one side is cut into slices of batch_size queries.
+        label_smoothing eps in [0, 1) sets the targets to (1 - eps) y + eps / n_ent (PyKEEN's convention).  eta and
+        the corruption seed are then unused.  It needs DistMult, ComplEx or HolE, on one GPU without focusE, and
+        cannot be combined with one_vs_all."""
         self._assert_compile_was_called()
+        if k_vs_all is not None or label_smoothing != 0.0:
+            self._check_k_vs_all(k_vs_all, label_smoothing, one_vs_all, focusE)
         if one_vs_all is not None:
             self._check_one_vs_all(one_vs_all, focusE)
         if validation_split:
@@ -275,12 +290,21 @@ class ScoringBasedEmbeddingModel:
                 pass
             if hasattr(cb, "on_train_begin"):
                 cb.on_train_begin({})
+        kva = kva_steps = None
+        if k_vs_all is not None:  # each side's queries, label offsets and label ids, uploaded once; steps slice them
+            findex = FilterIndex(triples, self.max_ent_size)
+            kva = {side: tuple(self._to_dev(a, a.dtype) for a in k_vs_all_queries(findex, triples, side))
+                   for side in k_vs_all.split(",")}
+            count = lambda side: kva[side][0].shape[0] if side in kva else 0
+            kva_steps = k_vs_all_steps(count("o"), count("s"), batch_size)
         for epoch in range(initial_epoch, epochs):
             if self.use_focusE and self._focuse_stop > 0:  # linear decay of the structural weight (:536-543)
                 self._focuse_sw = max(1 - epoch / self._focuse_stop, 0.001)
-            for start in range(0, n, batch_size):
-                batch = data[start:start + batch_size]
-                if one_vs_all is not None:
+            for start in (kva_steps if kva is not None else range(0, n, batch_size)):
+                batch = data[start:start + batch_size] if kva is None else None
+                if kva is not None:  # start: this step's query ranges of sides o and s
+                    self._k_vs_all_step(kva, start, label_smoothing)
+                elif one_vs_all is not None:
                     eng.one_vs_all_backward(batch, one_vs_all, step=self._step)
                     eng.apply_gradients()
                 elif self.use_focusE:
@@ -340,6 +364,37 @@ class ScoringBasedEmbeddingModel:
             raise NotImplementedError("1vsAll training does not support focusE")
         if self._world() > 1:
             raise NotImplementedError("1vsAll training is single-GPU only")
+
+    def _check_k_vs_all(self, k_vs_all, label_smoothing, one_vs_all, focusE):
+        """The refusals of fit(k_vs_all=..., label_smoothing=...), before anything is indexed or trained."""
+        if k_vs_all is not None:
+            if not isinstance(k_vs_all, str) or k_vs_all not in _lib.ONE_VS_ALL_SIDES:
+                raise ValueError("k_vs_all must be None, 's,o', 'o' or 's', got %r" % (k_vs_all,))
+            if one_vs_all is not None:
+                raise ValueError("k_vs_all and one_vs_all are two training types: give one of them")
+            if self.scoring_type not in ("DistMult", "ComplEx", "HolE"):
+                raise NotImplementedError("KvsAll training is implemented for DistMult, ComplEx and HolE (inner-product "
+                                          "scores), not for %s" % self.scoring_type)
+            if isinstance(self.compiled_loss, loss_functions.LossFunctionWrapper) or self.compiled_loss.name != "nll":
+                raise ValueError("KvsAll training needs the loss 'nll', got %r" % (self.compiled_loss.name,))
+        if (isinstance(label_smoothing, bool) or not isinstance(label_smoothing, numbers.Real)
+                or not math.isfinite(label_smoothing) or not 0.0 <= label_smoothing < 1.0):
+            raise ValueError("label_smoothing must be a number in [0, 1), got %r" % (label_smoothing,))
+        if k_vs_all is None:
+            raise ValueError("label_smoothing applies to KvsAll training only (k_vs_all=...)")
+        if focusE:
+            raise NotImplementedError("KvsAll training does not support focusE")
+        if self._world() > 1:
+            raise NotImplementedError("KvsAll training is single-GPU only")
+
+    def _k_vs_all_step(self, kva, ranges, label_smoothing):
+        """One KvsAll step: the query rows [lo, hi) of side o and of side s (ranges, from k_vs_all_steps), then the
+        optimizer."""
+        for side, (lo, hi) in zip(("o", "s"), ranges):
+            if hi > lo:
+                q, off, ids = kva[side]
+                self.engine.k_vs_all_backward(q[lo:hi], side, off[lo:hi + 1], ids, label_smoothing, step=self._step)
+        self.engine.apply_gradients()
 
     def train_on_batch(self, x):
         """Keras Model.train_on_batch (the reference model is a tf.keras.Model): one train_step on ONE

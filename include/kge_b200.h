@@ -295,6 +295,29 @@ int kge_one_vs_all_step(kge_handle *h, int32_t sides, int32_t loss_reduction, co
                         float *grad_ent_dev, float *grad_rel_dev, const int32_t *triples_dev, int64_t B, uint64_t step,
                         double *loss_dev, void *ws_dev, int64_t ws_bytes, void *stream);
 
+/* KvsAll training (Ruffinelli et al., ICLR 2020): forward + backward of the multi-label binary cross-entropy of B
+ * queries against EVERY entity on one side.  Query b is row b of queries_dev [B, 3] = (s, p, o): side
+ * KGE_ONE_VS_ALL_O scores l_e = f(s, p, e) (the query is (s, p)), side KGE_ONE_VS_ALL_S scores l_e = f(e, p, o) (the
+ * query is (p, o)), for all e in [0, n_ent); the answer column (2 or 0) must hold a valid entity id (it is not scored).
+ * Its labels are label_ids_dev[label_offsets_dev[b] .. label_offsets_dev[b + 1]): the offsets are absolute into the
+ * id array, and each query's labels are ascending, distinct and in [0, n_ent).  Each logit is clipped to [-75, 75]
+ * (zero gradient outside).  Target y'_e = (1 - eps) [e is a label] + eps / n_ent (eps = label_smoothing in [0, 1)).
+ * loss = w * sum_e softplus(l_e) - y'_e l_e per query, w = 1 (KGE_REDUCE_SUM) or 1 / n_ent (KGE_REDUCE_MEAN): the
+ * reference's nll over every (query, entity) pair.  DistMult, ComplEx and HolE only (KGE_ERR_UNSUPPORTED otherwise); the
+ * handle's loss, eta and corruption seed are not used; needs n_ent >= 2 and rows whose 32-query tile fits in shared
+ * memory (ld <= about 1600 floats).  B = 0 is a no-op.
+ *   grad_*_dev  ADDED to, as by kge_train_step; apply kge_optimizer_step (or _lazy) next
+ *   step        the lazy-optimizer stamp: every entity row and the relation rows of the batch are stamped with
+ *               kge_step_stamp(step)
+ *   loss_dev    double accumulator += the sum over queries of the loss (may be NULL)
+ *   ws_dev      caller-owned, 16-byte aligned, at least kge_k_vs_all_workspace_bytes(h, B) bytes
+ * Refused while a KGE_STEP_FUSED_DEFER step is pending.  Works on one (unsharded) entity table.  DESIGN.md 3.13. */
+int64_t kge_k_vs_all_workspace_bytes(const kge_handle *h, int64_t B);
+int kge_k_vs_all_step(kge_handle *h, int32_t side, int32_t loss_reduction, float label_smoothing, const float *ent_dev,
+                      const float *rel_dev, float *grad_ent_dev, float *grad_rel_dev, const int32_t *queries_dev, int64_t B,
+                      const int64_t *label_offsets_dev, const int32_t *label_ids_dev, uint64_t step, double *loss_dev,
+                      void *ws_dev, int64_t ws_bytes, void *stream);
+
 /* OptimizerWrapper.minimize -> legacy apply_gradients (optimizers.py:136-168) for ONE
  * table (or any row-wise concatenation of tables of the same width and regulariser: the engine passes [ent | rel] as one
  * block, one launch per step), dense semantics, plus the LP regulariser's loss/gradient over the whole table

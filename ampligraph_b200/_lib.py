@@ -119,6 +119,9 @@ PROTOTYPES = {
     "kge_one_vs_all_workspace_bytes": (C.c_int64, [_P, C.c_int64]),
     "kge_one_vs_all_step": (C.c_int, [_P, C.c_int32, C.c_int32, _P, _P, _P, _P, _P, C.c_int64, C.c_uint64, _P, _P,
                                       C.c_int64, _P]),
+    "kge_one_vs_all_relation_workspace_bytes": (C.c_int64, [_P, C.c_int64]),
+    "kge_one_vs_all_relation_step": (C.c_int, [_P, C.c_float, C.c_int32, _P, _P, _P, _P, _P, C.c_int64, C.c_uint64, _P,
+                                               _P, C.c_int64, _P]),
     "kge_k_vs_all_workspace_bytes": (C.c_int64, [_P, C.c_int64]),
     "kge_k_vs_all_step": (C.c_int, [_P, C.c_int32, C.c_int32, C.c_float, _P, _P, _P, _P, _P, C.c_int64, _P, _P, C.c_uint64,
                                     _P, _P, C.c_int64, _P]),

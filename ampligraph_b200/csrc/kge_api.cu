@@ -1,4 +1,5 @@
 // kge_api.cu -- the extern "C" boundary of libkge_b200.so (see include/kge_b200.h).
+#include <float.h>
 #include <stdarg.h>
 #include <stddef.h>
 #include <stdio.h>
@@ -1613,7 +1614,11 @@ extern "C" int kge_one_vs_all_step(kge_handle *h, int32_t sides, int32_t loss_re
     s.grad_rel = grad_rel_dev;
     s.triples = triples_dev;
     s.B = B;
-    s.n_ent = h->cfg.n_ent;
+    s.cand = ent_dev;
+    s.grad_cand = grad_ent_dev;
+    s.n_cand = h->cfg.n_ent;
+    s.weight = 1.f;
+    s.xsplit = 1;
     s.kp = h->L.kp;
     s.ld = h->L.ld;
     s.nsplit = w.nsplit;
@@ -1635,6 +1640,111 @@ extern "C" int kge_one_vs_all_step(kge_handle *h, int32_t sides, int32_t loss_re
         s.q = side == KGE_SIDE_S ? w.qs : w.qo;
         KGE_CUDA(launch_one_vs_all_side(s, h->L.halves, st), "kge_one_vs_all_step");
     }
+    return KGE_OK;
+}
+
+// ---- relation prediction as an auxiliary 1vsAll term (kge_train_1vsall.cu) --------------------------------------
+
+// Carve-up of the workspace of a relation-prediction step of B positives: the relation queries Qp [B, ld], the row
+// statistics of the 1vsAll passes over the n_rel relations, the per-split partial query gradients and, when dX is
+// split over the query tiles, its [xsplit, n_rel, ld] partial relation rows.
+struct RelationPredictionWorkspace {
+    float *qp, *pm, *pz, *lt, *row_m, *row_inv, *pgq, *pgx;
+    int nsplit, xsplit;
+};
+static RelationPredictionWorkspace carve_relation_prediction(const kge_handle *h, int64_t B, Carve &c)
+{
+    RelationPredictionWorkspace w;
+    const long long n_rel = h->cfg.n_rel;
+    w.nsplit = one_vs_all_splits(B, n_rel);
+    w.xsplit = one_vs_all_splits(n_rel, B);  // the same split rule with the roles swapped: query tiles per relation tile
+    const size_t rows = (size_t)B * h->L.ld * sizeof(float), col = (size_t)B * sizeof(float), ns = (size_t)w.nsplit;
+    w.qp = c.take<float>(rows, 16);
+    w.pm = c.take<float>(ns * col, 16);
+    w.pz = c.take<float>(ns * col, 16);
+    w.lt = c.take<float>(col, 16);
+    w.row_m = c.take<float>(col, 16);
+    w.row_inv = c.take<float>(col, 16);
+    w.pgq = c.take<float>(ns * rows, 16);
+    w.pgx = c.take<float>(w.xsplit > 1 ? (size_t)w.xsplit * n_rel * h->L.ld * sizeof(float) : 0, 16);
+    return w;
+}
+
+extern "C" int64_t kge_one_vs_all_relation_workspace_bytes(const kge_handle *h, int64_t B)
+{
+    if (!h || B < 0) return 0;
+    Carve c(nullptr);
+    carve_relation_prediction(h, B, c);
+    return (int64_t)c.at;
+}
+
+extern "C" int kge_one_vs_all_relation_step(kge_handle *h, float weight, int32_t loss_reduction, const float *ent_dev,
+                                            const float *rel_dev, float *grad_ent_dev, float *grad_rel_dev,
+                                            const int32_t *triples_dev, int64_t B, uint64_t step, double *loss_dev,
+                                            void *ws_dev, int64_t ws_bytes, void *stream)
+{
+    KGE_CHECK_HANDLE(h, "kge_one_vs_all_relation_step");
+    const int model = h->cfg.scoring;
+    if (model != KGE_DISTMULT && model != KGE_COMPLEX && model != KGE_HOLE)
+        return fail(KGE_ERR_UNSUPPORTED, "kge_one_vs_all_relation_step: relation prediction training is implemented for "
+                                         "DistMult, ComplEx and HolE (inner-product scores); not for scoring type %d", model);
+    if (loss_reduction != KGE_REDUCE_SUM && loss_reduction != KGE_REDUCE_MEAN)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "Invalid value for reduction!");
+    if (!(weight > 0.f && weight <= FLT_MAX))
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_relation_step: weight must be finite and > 0, got %g",
+                    (double)weight);
+    if (int rc = check_no_pending(h, "kge_one_vs_all_relation_step")) return rc;
+    if (h->cfg.n_rel < 2) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_relation_step: needs n_rel >= 2");
+    if ((long long)one_vs_all_smem_bytes(h->L.ld) > h->max_smem)
+        return fail(KGE_ERR_UNSUPPORTED, "kge_one_vs_all_relation_step: rows of %d floats exceed the shared-memory tiles of "
+                                         "the 1vsAll kernels (%d B)", h->L.ld, h->max_smem);
+    if (B < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_relation_step: B < 0");
+    if (B == 0) return KGE_OK;
+    if (!ent_dev || !rel_dev || !grad_ent_dev || !grad_rel_dev || !triples_dev)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_relation_step: null table, gradient or triples");
+    if (int rc = check_workspace(ws_dev, ws_bytes, kge_one_vs_all_relation_workspace_bytes(h, B), 16,
+                                 "kge_one_vs_all_relation_step", "kge_one_vs_all_relation_workspace_bytes"))
+        return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    Carve c(ws_dev);
+    const RelationPredictionWorkspace w = carve_relation_prediction(h, B, c);
+    const int stamp = kge_step_stamp(step);
+    // every relation row is a candidate of the step: all of them count as looked up; the batch's s and o rows are
+    // stamped by the chain pass (only while the entity buffer is set, like kge_one_vs_all_step)
+    if (h->stamp_ent && h->stamp_rel)
+        KGE_CUDA(launch_one_vs_all_stamps(h->stamp_rel, h->cfg.n_rel, stamp, st), "kge_one_vs_all_relation_step (stamps)");
+    OneVsAllSide s;
+    memset(&s, 0, sizeof(s));
+    s.q = w.qp;
+    s.ent = ent_dev;
+    s.rel = rel_dev;
+    s.grad_ent = grad_ent_dev;
+    s.grad_rel = grad_rel_dev;
+    s.cand = rel_dev;
+    s.grad_cand = grad_rel_dev;
+    s.triples = triples_dev;
+    s.B = B;
+    s.n_cand = h->cfg.n_rel;
+    s.side = KGE_SIDE_P;
+    s.col = 1;
+    s.kp = h->L.kp;
+    s.ld = h->L.ld;
+    s.nsplit = w.nsplit;
+    s.scale = h->score_scale;
+    s.w = loss_reduction == KGE_REDUCE_MEAN ? (float)(1.0 / (double)(h->cfg.n_rel - 1)) : 1.f;
+    s.weight = weight;
+    s.xsplit = w.xsplit;
+    s.loss = loss_dev;
+    s.stamp = stamp;
+    s.stamp_ent = h->stamp_ent;
+    s.pm = w.pm;
+    s.pz = w.pz;
+    s.lt = w.lt;
+    s.row_m = w.row_m;
+    s.row_inv = w.row_inv;
+    s.pgq = w.pgq;
+    s.pgx = w.pgx;
+    KGE_CUDA(launch_relation_prediction_side(s, w.qp, h->L.halves, st), "kge_one_vs_all_relation_step");
     return KGE_OK;
 }
 
@@ -1718,7 +1828,11 @@ extern "C" int kge_k_vs_all_step(kge_handle *h, int32_t side, int32_t loss_reduc
     s.grad_rel = grad_rel_dev;
     s.triples = queries_dev;
     s.B = B;
-    s.n_ent = h->cfg.n_ent;
+    s.cand = ent_dev;
+    s.grad_cand = grad_ent_dev;
+    s.n_cand = h->cfg.n_ent;
+    s.weight = 1.f;
+    s.xsplit = 1;
     s.side = side == KGE_ONE_VS_ALL_S ? KGE_SIDE_S : KGE_SIDE_O;
     s.col = side == KGE_ONE_VS_ALL_S ? 0 : 2;
     s.q = side == KGE_ONE_VS_ALL_S ? w.qs : w.qo;

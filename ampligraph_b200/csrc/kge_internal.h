@@ -89,21 +89,29 @@ cudaError_t launch_corruptions(const int32_t *triples, long long B, int eta, uns
 
 // kge_train_1vsall.cu: one side of a 1vsAll multiclass-NLL step of the trilinear models (kge_one_vs_all_step)
 struct OneVsAllSide {
-    const float *q;          // [B, ld] query vectors of the side (launch_rank_prepare: qvec_s for side s, qvec_o for o)
+    const float *q;          // [B, ld] query vectors of the side (launch_rank_prepare: qvec_s for side s, qvec_o for o;
+                             // side p: Qp(s, o) of launch_relation_prediction_side)
     const float *ent, *rel;  // [n_ent, ld], [n_rel, ld]
     float *grad_ent, *grad_rel;
+    const float *cand;       // [n_cand, ld] candidate rows: ent (sides s, o) or rel (side p)
+    float *grad_cand;        // their gradient rows: grad_ent or grad_rel
     const int32_t *triples;  // [B, 3]
-    long long B, n_ent;
-    int side, col;           // KGE_SIDE_S / KGE_SIDE_O; the triple column of the positive's own entity (0 / 2)
-    int kp, ld, nsplit;      // nsplit = one_vs_all_splits(B, n_ent) entity ranges per query tile
-    float scale, w;          // HolE's score scale (1 otherwise); weight of a negative's exp (1 or 1 / (n_ent - 1));
+    long long B, n_cand;
+    int side, col;           // KGE_SIDE_S / KGE_SIDE_O / KGE_SIDE_P; the triple column of the positive's own candidate
+    int kp, ld, nsplit;      // nsplit = one_vs_all_splits(B, n_cand) candidate ranges per query tile
+    float scale, w;          // HolE's score scale (1 otherwise); weight of a negative's exp (1 or 1 / (n_cand - 1));
                              // KvsAll: weight of every element (1 or 1 / n_ent)
+    float weight;            // 1vsAll: the side's weight on its loss and dL/dl (1 for sides s and o; lambda for side p)
+    int xsplit;              // dX query-tile ranges per candidate tile: 1 adds to grad_cand directly, > 1 writes
+                             // [xsplit, n_cand, ld] partial rows to pgx, summed in split order by launch_grad_passes
     double *loss;            // += sum of the row losses, or nullptr
     int stamp;
-    int *stamp_rel;          // lazy-optimizer stamps of the relation rows, or nullptr
+    int *stamp_rel;          // lazy-optimizer stamps of the relation rows, or nullptr (sides s, o: the batch's rows)
+    int *stamp_ent;          // side p: lazy-optimizer stamps of the entity rows (the batch's s and o rows), or nullptr
     // workspace: [nsplit, B] partial maxima and sums; [B] l_t, max and 1 / D per row (1vsAll only); [nsplit, B, ld]
     // partial Gq rows
     float *pm, *pz, *lt, *row_m, *row_inv, *pgq;
+    float *pgx;              // [xsplit, n_cand, ld] partial candidate gradient rows (xsplit > 1 only)
     // KvsAll: the labels of query b are label_ids[label_off[b] .. label_off[b + 1]) (ascending, distinct, < n_ent);
     // target of an entity: y0 = eps / n_ent, plus y1 = 1 - eps for a label
     const long long *label_off;
@@ -117,6 +125,10 @@ cudaError_t launch_one_vs_all_side(const OneVsAllSide &s, int halves, cudaStream
 // one side of a KvsAll multi-label step (kge_k_vs_all_step): s.triples are the [B, 3] queries, s.label_* set
 cudaError_t launch_k_vs_all_side(const OneVsAllSide &s, int halves, cudaStream_t st);
 cudaError_t launch_one_vs_all_stamps(int *stamp_ent, long long n_ent, int stamp, cudaStream_t st);
+// relation prediction as a 1vsAll side (kge_one_vs_all_relation_step): s.side = KGE_SIDE_P, s.cand = rel, s.n_cand =
+// n_rel, s.q = qp; writes qp[b] = Qp(s_b, o_b) = d f(s_b, p, o_b) / dp, then runs the 1vsAll passes with dX split
+// s.xsplit ways over the query tiles (partials in s.pgx), and a chain pass that adds d/ds and d/do to grad_ent
+cudaError_t launch_relation_prediction_side(const OneVsAllSide &s, float *qp, int halves, cudaStream_t st);
 
 // kge_misc.cu
 cudaError_t launch_score_triples(const Layout &L, int nit, const float *ent, const float *rel_or_rot,

@@ -30,6 +30,12 @@
 // element-wise, so a side is the dQ pass (which also adds the loss), the dX pass and the chain pass above, with the
 // multi-label rule in place of the multiclass one.  The labels are a CSR (ascending ids per query); each 32 x 32 tile
 // reads them as one 32-bit mask per query row, built in shared memory from the row's slice.
+//
+// Relation prediction as an auxiliary 1vsAll term (kge_one_vs_all_relation_step; DESIGN.md 3.14) is a third side,
+// KGE_SIDE_P, whose candidates are the n_rel relation rows: l_r = f(s, r, o) = scale * <x_r, Qp(s, o)> with Qp = df/dp,
+// the positive's relation the target, the row loss and dL/dl times the side's weight lambda.  It runs the same five
+// passes; its dX pass is split over the query tiles too (n_rel / 32 relation tiles alone would leave most SMs idle), the
+// partial rows summed in split order, and its chain pass adds d/ds = Q0(Gq, o) and d/do = Q1(s, Gq).
 #include <math.h>
 
 #include "kge_train_common.cuh"
@@ -156,14 +162,14 @@ __device__ __forceinline__ float ova_clip(float acc, float scale, bool &in)
     return fminf(fmaxf(l, KGE_CLIP_LO), KGE_CLIP_HI);
 }
 
-// dL/dl of entity e in a row with target t, max m, 1 / D = inv
+// dL/dl of candidate e in a row with target t, max m, 1 / D = inv (times the side's weight: 1, or lambda for side p)
 __device__ __forceinline__ float ova_grad(float acc, const OneVsAllSide &s, long long e, long long t, float m, float inv)
 {
     bool in;
     const float l = ova_clip(acc, s.scale, in);
     if (!in) return 0.f;
     const float p = expf(l - m) * inv;
-    return e == t ? p - 1.f : s.w * p;
+    return s.weight * (e == t ? p - 1.f : s.w * p);
 }
 
 __device__ __forceinline__ void ova_zero(float *a, int n, int tid)
@@ -174,7 +180,7 @@ __device__ __forceinline__ void ova_zero(float *a, int n, int tid)
 // the entity-tile range [et0, et1) of split `split`
 __device__ __forceinline__ void ova_split_range(const OneVsAllSide &s, int split, long long &et0, long long &et1)
 {
-    const long long n_et = (s.n_ent + OVA_T - 1) / OVA_T;
+    const long long n_et = (s.n_cand + OVA_T - 1) / OVA_T;
     et0 = split * n_et / s.nsplit;
     et1 = (split + 1) * n_et / s.nsplit;
 }
@@ -198,13 +204,13 @@ __global__ void __launch_bounds__(OVA_THREADS) kge_ova_stats_kernel(const OneVsA
     for (long long et = et0; et < et1; ++et) {
         const long long e0 = et * OVA_T;
         float acc[2][2];
-        ova_logits(s.q, q0, s.B, s.ent, e0, s.n_ent, s.ld, ova_sm, tid, acc);
+        ova_logits(s.q, q0, s.B, s.cand, e0, s.n_cand, s.ld, ova_sm, tid, acc);
 #pragma unroll
         for (int i = 0; i < 2; ++i)
 #pragma unroll
             for (int j = 0; j < 2; ++j) {
                 const long long e = e0 + tx + 16 * j;
-                if (tgt[i] < 0 || e >= s.n_ent) continue;
+                if (tgt[i] < 0 || e >= s.n_cand) continue;
                 bool in;
                 const float l = ova_clip(acc[i][j], s.scale, in);
                 if (e == tgt[i]) {  // the positive's own logit: counted in m, kept out of the sum
@@ -254,7 +260,7 @@ __global__ void __launch_bounds__(256) kge_ova_merge_kernel(const OneVsAllSide s
         const float D = __fmaf_rn(s.w, z, expf(lt - m));
         s.row_m[b] = m;
         s.row_inv[b] = 1.f / D;
-        loss = (m + logf(D)) - lt;
+        loss = s.weight * ((m + logf(D)) - lt);
     }
     loss = warp_sum(loss);
     if ((threadIdx.x & 31) == 0 && s.loss) atomicAdd(s.loss, (double)loss);
@@ -289,7 +295,7 @@ struct OvaMulticlass {
     template <bool LOSS>
     __device__ __forceinline__ float grad(float acc, long long, int i, int, long long e)
     {
-        return (tgt[i] >= 0 && e < s.n_ent) ? ova_grad(acc, s, e, tgt[i], m[i], inv[i]) : 0.f;
+        return (tgt[i] >= 0 && e < s.n_cand) ? ova_grad(acc, s, e, tgt[i], m[i], inv[i]) : 0.f;
     }
     __device__ __forceinline__ void dq_end() {}
 };
@@ -341,7 +347,7 @@ struct KvaMultiLabel {
     template <bool LOSS>
     __device__ __forceinline__ float grad(float acc, long long b, int i, int c, long long e)
     {
-        if (b >= s.B || e >= s.n_ent) return 0.f;
+        if (b >= s.B || e >= s.n_cand) return 0.f;
         const int r = 2 * (threadIdx.x >> 4) + i;
         const float y = (mask[r] >> c) & 1u ? s.y0 + s.y1 : s.y0;
         bool in;
@@ -376,7 +382,7 @@ __global__ void __launch_bounds__(OVA_THREADS) kge_ova_dq_kernel(const OneVsAllS
         const long long e0 = et * OVA_T;
         rule.dq_tile(e0, tid);
         float acc[2][2];
-        ova_logits(s.q, q0, s.B, s.ent, e0, s.n_ent, s.ld, stage, tid, acc);
+        ova_logits(s.q, q0, s.B, s.cand, e0, s.n_cand, s.ld, stage, tid, acc);
 #pragma unroll
         for (int i = 0; i < 2; ++i)
 #pragma unroll
@@ -386,7 +392,7 @@ __global__ void __launch_bounds__(OVA_THREADS) kge_ova_dq_kernel(const OneVsAllS
                     rule.template grad<true>(acc[i][j], q0 + 2 * ty + i, i, tx + 16 * j, e);
             }
         __syncthreads();
-        ova_accumulate<false>(acc_s, gs, s.ent, e0, s.n_ent, s.ld, stage, tid);
+        ova_accumulate<false>(acc_s, gs, s.cand, e0, s.n_cand, s.ld, stage, tid);
     }
     rule.dq_end();
     // this split's partial Gq rows, scale included
@@ -399,22 +405,22 @@ __global__ void __launch_bounds__(OVA_THREADS) kge_ova_dq_kernel(const OneVsAllS
         }
 }
 
-// dX (one entity tile, every query tile); the same shared memory as dQ
+// dX (candidate tile x query-tile split: every query tile when s.xsplit = 1); the same shared memory as dQ
 template <class Rule>
 __global__ void __launch_bounds__(OVA_THREADS) kge_ova_dx_kernel(const OneVsAllSide s)
 {
     extern __shared__ __align__(16) float ova_sm[];
     float *stage = ova_sm, *gs = ova_sm + OVA_STAGE, *acc_s = gs + OVA_GS;
-    const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
+    const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15, split = blockIdx.y;
     const long long e0 = (long long)blockIdx.x * OVA_T;
     ova_zero(acc_s, OVA_T * s.ld, tid);
     Rule rule(s, acc_s + (size_t)OVA_T * s.ld);
     const long long n_qt = (s.B + OVA_T - 1) / OVA_T;
-    for (long long qt = 0; qt < n_qt; ++qt) {
+    for (long long qt = split; qt < n_qt; qt += s.xsplit) {  // split k takes the query tiles k, k + xsplit, ...
         const long long q0 = qt * OVA_T;
         rule.dx_tile(q0, e0, tid);
         float acc[2][2];
-        ova_logits(s.q, q0, s.B, s.ent, e0, s.n_ent, s.ld, stage, tid, acc);
+        ova_logits(s.q, q0, s.B, s.cand, e0, s.n_cand, s.ld, stage, tid, acc);
 #pragma unroll
         for (int i = 0; i < 2; ++i)
 #pragma unroll
@@ -426,19 +432,36 @@ __global__ void __launch_bounds__(OVA_THREADS) kge_ova_dx_kernel(const OneVsAllS
         __syncthreads();
         ova_accumulate<true>(acc_s, gs, s.q, q0, s.B, s.ld, stage, tid);
     }
-    // one add per gradient row: this CTA is the only writer of its rows in this launch
+    // one add per gradient row: this CTA is the only writer of its rows in this launch (split: of its partial rows)
     const int o = tid >> 3;
     const long long e = e0 + o;
-    if (e < s.n_ent)
+    if (e < s.n_cand)
         for (int c = (tid & 7) * 4; c < s.ld; c += 32) {
-            float *g = s.grad_ent + (size_t)e * s.ld + c;
             const float4 a = ova_lds4(acc_s + (size_t)o * s.ld + c);
-            *reinterpret_cast<float4 *>(g) = *reinterpret_cast<const float4 *>(g) + s.scale * a;
+            if (s.xsplit == 1) {
+                float *g = s.grad_cand + (size_t)e * s.ld + c;
+                *reinterpret_cast<float4 *>(g) = *reinterpret_cast<const float4 *>(g) + s.scale * a;
+            } else {
+                *reinterpret_cast<float4 *>(s.pgx + ((size_t)split * s.n_cand + e) * s.ld + c) = s.scale * a;
+            }
         }
 }
 
-// one thread per (positive, float4 chunk of a half)
-template <int HALVES>
+// grad_cand[e] += sum of the xsplit partial dX rows of e, in split order (one thread per float4: one writer per row)
+__global__ void __launch_bounds__(256) kge_ova_dx_sum_kernel(const OneVsAllSide s)
+{
+    const int nq4 = s.ld / 4;
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= s.n_cand * nq4) return;
+    const size_t off = (size_t)idx * 4;  // = e * ld + 4 * chunk
+    float4 a = f4ld(s.pgx + off);
+    for (int k = 1; k < s.xsplit; ++k) a = a + f4ld(s.pgx + (size_t)k * s.n_cand * s.ld + off);
+    f4st(s.grad_cand + off, f4ld(s.grad_cand + off) + a);
+}
+
+// one thread per (positive, float4 chunk of a half).  REL: the relation side, whose query is Qp(s, o) = d f / dp, so
+// by linearity in the relation row d/ds = Q0(Gq, o) and d/do = Q1(s, Gq), with Gq in the relation slot.
+template <int HALVES, bool REL>
 __global__ void __launch_bounds__(256) kge_ova_chain_kernel(const OneVsAllSide s)
 {
     const int nq4 = s.kp / 4;
@@ -453,6 +476,23 @@ __global__ void __launch_bounds__(256) kge_ova_chain_kernel(const OneVsAllSide s
         if (HALVES == 2) Gi = Gi + f4ld(g + di);
     }
     const int si = s.triples[3 * b], pi_ = s.triples[3 * b + 1], oi_ = s.triples[3 * b + 2];
+    if constexpr (REL) {
+        const float *srow = s.ent + (size_t)si * s.ld, *orow = s.ent + (size_t)oi_ * s.ld;
+        const float4 sr = f4ld(srow + d), sim = HALVES == 2 ? f4ld(srow + di) : f4zero();
+        const float4 orr = f4ld(orow + d), oim = HALVES == 2 ? f4ld(orow + di) : f4zero();
+        float *gs_ = s.grad_ent + (size_t)si * s.ld, *go = s.grad_ent + (size_t)oi_ * s.ld;
+        red_add_v4(gs_ + d, query_subj<HALVES, 0>(Gr, Gi, orr, oim));
+        red_add_v4(go + d, query_obj<HALVES, 0>(sr, sim, Gr, Gi));
+        if (HALVES == 2) {
+            red_add_v4(gs_ + di, query_subj<HALVES, 1>(Gr, Gi, orr, oim));
+            red_add_v4(go + di, query_obj<HALVES, 1>(sr, sim, Gr, Gi));
+        }
+        if (d == 0 && s.stamp_ent) {
+            s.stamp_ent[si] = s.stamp;
+            s.stamp_ent[oi_] = s.stamp;
+        }
+        return;
+    }
     const float *prow = s.rel + (size_t)pi_ * s.ld;
     const float4 pr = f4ld(prow + d), pi = HALVES == 2 ? f4ld(prow + di) : f4zero();
     const float4 z = f4zero();
@@ -491,14 +531,44 @@ __global__ void kge_ova_stamp_kernel(int *stamps, long long n, int stamp)
 template <class Rule>
 static cudaError_t launch_grad_passes(const OneVsAllSide &s, int halves, size_t smem, cudaStream_t st)
 {
-    const unsigned n_qt = (unsigned)((s.B + OVA_T - 1) / OVA_T), n_et = (unsigned)((s.n_ent + OVA_T - 1) / OVA_T);
+    const unsigned n_qt = (unsigned)((s.B + OVA_T - 1) / OVA_T), n_et = (unsigned)((s.n_cand + OVA_T - 1) / OVA_T);
     cudaError_t e;
     if ((e = launch_with_smem(kge_ova_dq_kernel<Rule>, dim3(n_qt, s.nsplit), OVA_THREADS, smem, st, s)) != cudaSuccess) return e;
-    if ((e = launch_with_smem(kge_ova_dx_kernel<Rule>, dim3(n_et), OVA_THREADS, smem, st, s)) != cudaSuccess) return e;
+    if ((e = launch_with_smem(kge_ova_dx_kernel<Rule>, dim3(n_et, s.xsplit), OVA_THREADS, smem, st, s)) != cudaSuccess)
+        return e;
+    if (s.xsplit > 1) {
+        kge_ova_dx_sum_kernel<<<(unsigned)((s.n_cand * (s.ld / 4) + 255) / 256), 256, 0, st>>>(s);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    }
     const unsigned grid = (unsigned)((s.B * (s.kp / 4) + 255) / 256);
-    if (halves == 2) kge_ova_chain_kernel<2><<<grid, 256, 0, st>>>(s);
-    else kge_ova_chain_kernel<1><<<grid, 256, 0, st>>>(s);
+    const bool rel = s.side == KGE_SIDE_P;
+    if (halves == 2) {
+        if (rel) kge_ova_chain_kernel<2, true><<<grid, 256, 0, st>>>(s);
+        else kge_ova_chain_kernel<2, false><<<grid, 256, 0, st>>>(s);
+    } else {
+        if (rel) kge_ova_chain_kernel<1, true><<<grid, 256, 0, st>>>(s);
+        else kge_ova_chain_kernel<1, false><<<grid, 256, 0, st>>>(s);
+    }
     return cudaGetLastError();
+}
+
+// qp[b] = Qp(s_b, o_b) = d f(s_b, p, o_b) / dp (scale excluded), the relation side's query: one thread per (positive,
+// float4 chunk of a half), with the training kernels' relation-row gradient arithmetic (U = s in the subject slot)
+template <int HALVES>
+__global__ void __launch_bounds__(256) kge_ova_relation_query_kernel(const OneVsAllSide s, float *qp)
+{
+    const int nq4 = s.kp / 4;
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= s.B * nq4) return;
+    const long long b = idx / nq4;
+    const int d = (int)(idx - b * nq4) * 4, di = HALVES == 2 ? s.kp + d : d;
+    const float *srow = s.ent + (size_t)s.triples[3 * b] * s.ld, *orow = s.ent + (size_t)s.triples[3 * b + 2] * s.ld;
+    const float4 sr = f4ld(srow + d), sim = HALVES == 2 ? f4ld(srow + di) : f4zero();
+    const float4 orr = f4ld(orow + d), oim = HALVES == 2 ? f4ld(orow + di) : f4zero();
+    const float4 z = f4zero();
+    float *q = qp + (size_t)b * s.ld;
+    f4st(q + d, trilinear_grad_p<HALVES, 0>(z, z, orr, oim, sr, sim, z, z));
+    if (HALVES == 2) f4st(q + di, trilinear_grad_p<HALVES, 1>(z, z, orr, oim, sr, sim, z, z));
 }
 
 cudaError_t launch_one_vs_all_side(const OneVsAllSide &s, int halves, cudaStream_t st)
@@ -510,6 +580,17 @@ cudaError_t launch_one_vs_all_side(const OneVsAllSide &s, int halves, cudaStream
     kge_ova_merge_kernel<<<(unsigned)((s.B + 255) / 256), 256, 0, st>>>(s);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     return launch_grad_passes<OvaMulticlass>(s, halves, one_vs_all_smem_bytes(s.ld), st);
+}
+
+cudaError_t launch_relation_prediction_side(const OneVsAllSide &s, float *qp, int halves, cudaStream_t st)
+{
+    if (s.B == 0) return cudaSuccess;
+    const unsigned grid = (unsigned)((s.B * (s.kp / 4) + 255) / 256);
+    if (halves == 2) kge_ova_relation_query_kernel<2><<<grid, 256, 0, st>>>(s, qp);
+    else kge_ova_relation_query_kernel<1><<<grid, 256, 0, st>>>(s, qp);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    return launch_one_vs_all_side(s, halves, st);
 }
 
 size_t k_vs_all_smem_bytes(int ld) { return one_vs_all_smem_bytes(ld) + OVA_T * sizeof(unsigned); }

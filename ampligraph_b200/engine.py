@@ -68,6 +68,18 @@ def one_vs_all_workspace_bytes(B, n_ent, ld):
     return 2 * r16(rows) + r16(col) + 2 * r16(ns * col) + 3 * r16(col) + r16(ns * rows)
 
 
+def one_vs_all_relation_workspace_bytes(B, n_rel, ld):
+    """kge_one_vs_all_relation_workspace_bytes(h, B) for a handle of n_rel relations and rows of ld floats: the relation
+    queries [B, ld], the per-split maxima and sums [nsplit, B], three [B] row arrays, the per-split partial query
+    gradients [nsplit, B, ld] and, when the dX pass splits the query tiles (xsplit > 1), its partial relation rows
+    [xsplit, n_rel, ld], each region padded to 16 bytes."""
+    r16 = lambda n: (n + 15) // 16 * 16
+    B, ns, xs = int(B), one_vs_all_splits(B, n_rel), one_vs_all_splits(n_rel, B)
+    rows, col = 4 * B * int(ld), 4 * B
+    return (r16(rows) + 2 * r16(ns * col) + 3 * r16(col) + r16(ns * rows)
+            + (r16(4 * xs * int(n_rel) * int(ld)) if xs > 1 else 0))
+
+
 def k_vs_all_workspace_bytes(B, n_ent, ld):
     """kge_k_vs_all_workspace_bytes(h, B): both sides' query vectors [B, ld], the quantised positive scores [B] and the
     per-split partial query gradients [nsplit, B, ld], each region padded to 16 bytes (no row statistics)."""
@@ -435,6 +447,29 @@ class KGEEngine:
         self._last_step = int(step)
         # query vectors (two kernels), entity stamps, five passes per side
         self.launches += 2 + (1 if self.lazy else 0) + 5 * (2 if sides == "s,o" else 1)
+
+    @_traced("kge.one_vs_all_relation_step")
+    def one_vs_all_relation_backward(self, triples, weight, step=0):
+        """Relation-prediction term of a 1vsAll step up to tape.gradient (kge_one_vs_all_relation_step, DESIGN.md
+        3.14): weight * the multiclass NLL of every positive's relation against every relation, scored as f(s, r, o),
+        with the engine's reduction; accumulates into g_ent / g_rel and loss_acc[0] like one_vs_all_backward.  step:
+        the lazy optimizer's row stamp (every relation row and the batch's s and o rows count as looked up)."""
+        assert triples.dtype == torch.int32 and triples.is_cuda and triples.is_contiguous()
+        if self._deferred:
+            raise ValueError("one_vs_all_relation_backward: the replaced-row sum of a deferred step is pending "
+                             "(apply_gradients first)")
+        B = triples.shape[0]
+        need = int(self.lib.kge_one_vs_all_relation_workspace_bytes(self.h, B))
+        if getattr(self, "_ovr_ws", None) is None or self._ovr_ws.numel() < need:
+            self._ovr_ws = torch.empty(max(need, 16), dtype=torch.uint8, device=self.device)  # 256-byte aligned (torch)
+        _lib.check(self.lib.kge_one_vs_all_relation_step(
+            self.h, float(weight), _lib.REDUCTIONS[self.reduction], _ptr(self.ent), _ptr(self.rel), _ptr(self.g_ent),
+            _ptr(self.g_rel), _ptr(triples), B, int(step), _ptr(self.loss_acc), _ptr(self._ovr_ws), need,
+            self._stream()))
+        self._last_step = int(step)
+        # relation stamps, relation queries, five passes, the dX split sum when dX is split
+        if B > 0:
+            self.launches += (1 if self.lazy else 0) + 6 + (1 if one_vs_all_splits(self.n_rel, B) > 1 else 0)
 
     @_traced("kge.k_vs_all_step")
     def k_vs_all_backward(self, queries, side, label_offsets, label_ids, label_smoothing=0.0, step=0):

@@ -211,7 +211,7 @@ class ScoringBasedEmbeddingModel:
             validation_data=None, shuffle=True, initial_epoch=0, validation_batch_size=10,
             validation_corrupt_side="s,o", validation_freq=10, validation_burn_in=0, validation_filter=False,
             validation_entities_subset=None, partitioning_k=1, focusE=False, focusE_params={}, one_vs_all=None,
-            k_vs_all=None, label_smoothing=0.0):
+            k_vs_all=None, label_smoothing=0.0, relation_prediction_weight=0.0):
         """fit (:544-883).  `shuffle` is accepted and ignored exactly like the reference
         (batches are the sequential slices of graph_data_loader.py:495-500).  validation_split: carve the validation
         set out of x with train_test_split_no_unseen(x, test_size=validation_split, seed=self.seed), as the reference
@@ -232,12 +232,20 @@ class ScoringBasedEmbeddingModel:
         steps, each taking its share of both sides' queries; one side is cut into slices of batch_size queries.
         label_smoothing eps in [0, 1) sets the targets to (1 - eps) y + eps / n_ent (PyKEEN's convention).  eta and
         the corruption seed are then unused.  It needs DistMult, ComplEx or HolE, on one GPU without focusE, and
-        cannot be combined with one_vs_all."""
+        cannot be combined with one_vs_all.
+
+        relation_prediction_weight (extension): lambda >= 0.  With one_vs_all and lambda > 0, every step adds
+        lambda * L_p to the 1vsAll loss, L = L_s + L_o + lambda * L_p (Chen et al., "Relation Prediction as an Auxiliary
+        Training Objective for Improving Multi-Relational Graph Representations", AKBC 2021; DESIGN.md 3.14): L_p is
+        the multiclass NLL of each positive's relation against every relation, scored as f(s, r, o), under the same
+        reduction.  The logged loss includes the term.  It needs one_vs_all, at least two relations, and cannot be
+        combined with k_vs_all.  0.0 (the default) leaves training unchanged."""
         self._assert_compile_was_called()
         if k_vs_all is not None or label_smoothing != 0.0:
             self._check_k_vs_all(k_vs_all, label_smoothing, one_vs_all, focusE)
         if one_vs_all is not None:
             self._check_one_vs_all(one_vs_all, focusE)
+        self._check_relation_prediction(relation_prediction_weight, one_vs_all, k_vs_all)
         if validation_split:
             assert isinstance(x, np.ndarray), "Validation split supported for numpy arrays only!"
             x, validation_data = train_test_split_no_unseen(x, test_size=validation_split, seed=self.seed,
@@ -264,6 +272,8 @@ class ScoringBasedEmbeddingModel:
         elif self.max_ent_size is None or self.max_rel_size is None:
             self.max_ent_size = int(max(triples[:, 0].max(), triples[:, 2].max())) + 1
             self.max_rel_size = int(triples[:, 1].max()) + 1
+        if relation_prediction_weight > 0 and self.max_rel_size < 2:
+            raise ValueError("relation_prediction_weight needs at least two relations, got %d" % self.max_rel_size)
         if self.engine is None:
             self._build_engine()
         eng = self.engine
@@ -306,6 +316,8 @@ class ScoringBasedEmbeddingModel:
                     self._k_vs_all_step(kva, start, label_smoothing)
                 elif one_vs_all is not None:
                     eng.one_vs_all_backward(batch, one_vs_all, step=self._step)
+                    if relation_prediction_weight > 0:
+                        eng.one_vs_all_relation_backward(batch, relation_prediction_weight, step=self._step)
                     eng.apply_gradients()
                 elif self.use_focusE:
                     self._two_phase_step(batch, weights[start:start + batch_size])
@@ -386,6 +398,18 @@ class ScoringBasedEmbeddingModel:
             raise NotImplementedError("KvsAll training does not support focusE")
         if self._world() > 1:
             raise NotImplementedError("KvsAll training is single-GPU only")
+
+    @staticmethod
+    def _check_relation_prediction(weight, one_vs_all, k_vs_all):
+        """The refusals of fit(relation_prediction_weight=...), before anything is indexed or trained (n_rel >= 2 is
+        checked once the relations are indexed)."""
+        if (isinstance(weight, bool) or not isinstance(weight, numbers.Real) or not math.isfinite(weight)
+                or weight < 0):
+            raise ValueError("relation_prediction_weight must be a finite number >= 0, got %r" % (weight,))
+        if weight > 0 and k_vs_all is not None:
+            raise ValueError("relation_prediction_weight is a 1vsAll term: it cannot be combined with k_vs_all")
+        if weight > 0 and one_vs_all is None:
+            raise ValueError("relation_prediction_weight needs 1vsAll training (one_vs_all=...)")
 
     def _k_vs_all_step(self, kva, ranges, label_smoothing):
         """One KvsAll step: the query rows [lo, hi) of side o and of side s (ranges, from k_vs_all_steps), then the

@@ -295,6 +295,27 @@ int kge_one_vs_all_step(kge_handle *h, int32_t sides, int32_t loss_reduction, co
                         float *grad_ent_dev, float *grad_rel_dev, const int32_t *triples_dev, int64_t B, uint64_t step,
                         double *loss_dev, void *ws_dev, int64_t ws_bytes, void *stream);
 
+/* Relation prediction as an auxiliary 1vsAll training objective (Chen, Minervini, Riedel and Stenetorp, AKBC 2021):
+ * forward + backward of weight * the multiclass NLL of every positive (s, p, o) against EVERY relation, the term
+ * weight * L_p of L = L_s + L_o + weight * L_p (kge_one_vs_all_step gives L_s and L_o).  The logits are
+ * l_r = f(s, r, o) = scale * <x_r, Qp(s, o)> for all r in [0, n_rel), Qp = d f / dp (DistMult: s * o; ComplEx / HolE:
+ * [s_re o_re + s_im o_im | s_re o_im - s_im o_re]), the positive's own relation p the target; clipping, reductions and
+ * gradients as kge_one_vs_all_step's with relations in place of entities (KGE_REDUCE_MEAN averages the exp of the
+ * n_rel - 1 negatives).  Other relations that hold for (s, o) count as negatives (no filtering).  DistMult, ComplEx
+ * and HolE only (KGE_ERR_UNSUPPORTED otherwise, and for rows too wide for the 1vsAll tiles); needs n_rel >= 2 and a
+ * finite weight > 0.  B = 0 is a no-op.
+ *   grad_*_dev  ADDED to: every relation row, and the batch's s and o entity rows
+ *   step        the lazy-optimizer stamp: every relation row and the batch's s and o rows are stamped with
+ *               kge_step_stamp(step) (while an entity stamp buffer is set, as for kge_one_vs_all_step)
+ *   loss_dev    double accumulator += weight * the sum over positives of the loss (may be NULL)
+ *   ws_dev      caller-owned, 16-byte aligned, at least kge_one_vs_all_relation_workspace_bytes(h, B) bytes
+ * The relation gradient rows are summed in a fixed order (bit-for-bit repeatable); the entity rows are added with
+ * atomics.  Refused while a KGE_STEP_FUSED_DEFER step is pending.  DESIGN.md 3.14. */
+int64_t kge_one_vs_all_relation_workspace_bytes(const kge_handle *h, int64_t B);
+int kge_one_vs_all_relation_step(kge_handle *h, float weight, int32_t loss_reduction, const float *ent_dev,
+                                 const float *rel_dev, float *grad_ent_dev, float *grad_rel_dev, const int32_t *triples_dev,
+                                 int64_t B, uint64_t step, double *loss_dev, void *ws_dev, int64_t ws_bytes, void *stream);
+
 /* KvsAll training (Ruffinelli et al., ICLR 2020): forward + backward of the multi-label binary cross-entropy of B
  * queries against EVERY entity on one side.  Query b is row b of queries_dev [B, 3] = (s, p, o): side
  * KGE_ONE_VS_ALL_O scores l_e = f(s, p, e) (the query is (s, p)), side KGE_ONE_VS_ALL_S scores l_e = f(e, p, o) (the

@@ -13,6 +13,10 @@ returns 0 -- the oracle's modulus gradient is 0 there too (_Modulus).
 For the losses whose dL/dscore is not exact (nll, multiclass_nll, self_adversarial) the oracle also returns a
 per-element error budget: A = sum over the element's terms of |dL/dscore_j| * |d score_j / d element| (bounds), its term
 count n, and A1 = sum of |d score_j / d element| (for results below fp32's smallest normal); see grad_bound.
+
+For the 1vsAll family (1vsAll, KvsAll, relation prediction), whose every gradient element sums one term per (query,
+candidate) pair, OvaBound gives the per-element bound in the same form, with each pair's weight derived in its
+docstring from the kernels' split geometry (ova_chains) and the pair's logit error.
 """
 from collections import namedtuple
 
@@ -226,3 +230,160 @@ def zipf_triples(E, R, n, rng):
     perm = rng.permutation(E)
     s, o = perm[np.searchsorted(cdf, rng.random(n))], perm[np.searchsorted(cdf, rng.random(n))]
     return np.stack([s, rng.integers(0, R, n), o], 1).astype(np.int32)
+
+
+# --------------------------------------------------------------------------
+# 1vsAll, KvsAll and relation prediction: a per-element bound
+# --------------------------------------------------------------------------
+OVA_C = 32  # the roundings of one term outside the chains: query vector, scale, exp, 1 / D, y, the chain pass's products
+
+
+def abs_query(model, a, b):
+    """On |tables|: the query of the slot whose two other rows are a and b, every product term counted positive, so
+    that <abs_query, |x|> = abs_scores with x in that slot (HolE's scale included)."""
+    if model == "DistMult":
+        return a * b
+    h = a.shape[1] // 2
+    q = torch.cat([a[:, :h] * b[:, :h] + a[:, h:] * b[:, h:], a[:, :h] * b[:, h:] + a[:, h:] * b[:, :h]], 1)
+    return q * (2.0 / h) if model == "HolE" else q
+
+
+def row_stride(model, K):
+    """The kernel's row stride ld for K internal columns: each half padded to a multiple of 4 floats."""
+    halves = 1 if model in ("TransE", "DistMult") else 2
+    return halves * (-(-(K // halves) // 4) * 4)
+
+
+def ova_geometry(B, n_cand, relation=False):
+    """(nsplit, xsplit) of a 1vsAll-family side: candidate ranges per query tile of the stats and dQ passes, and query-
+    tile ranges per candidate tile of the dX pass (split on the relation side only)."""
+    from ampligraph_b200.engine import one_vs_all_splits
+    return one_vs_all_splits(B, n_cand), (one_vs_all_splits(n_cand, B) if relation else 1)
+
+
+def ova_chains(B, n_cand, nsplit, xsplit, kvsall):
+    """(n, n_loss): the longest fp32 chains one (query, candidate) term passes through on its way into a gradient
+    element, and into the loss.  Gq: 32 fmas per candidate tile of the split, then the sum of nsplit partials; dX: 32
+    per query tile of the split, then the sum of xsplit partials; D (1vsAll): two online updates (rescale and add, each
+    with an expf) per tile of the split, four shuffle levels and the merge of nsplit partials."""
+    n_qt, n_et = -(-B // 32), -(-n_cand // 32)
+    per_split = -(-n_et // nsplit)
+    n = max(32 * per_split + nsplit, 32 * -(-n_qt // xsplit) + xsplit)
+    if kvsall:  # 4 elements per thread and tile, the warp sum
+        return n, 4 * per_split + 5
+    n_D = 10 * per_split + 6 * nsplit + 64
+    return n + n_D, n_D
+
+
+class OvaBound:
+    """The per-element error bound of a 1vsAll-family step, side by side (add_side), checked with within_bound.
+
+    A gradient element is a sum of terms g_be * d l_be / d theta, one per (query b, candidate e) pair of each side;
+    |d l_be / d theta| <= d abs_score_be / d |theta| with abs_score_be = <abs_query_b, |x_e|>.  So for any weight W >= 0
+    per pair, u * d/d|theta| sum W_be abs_score_be (u = 2^-24; autograd on |tables|, matmul form) bounds the element's
+    error when W_be * u bounds the error of that pair's g_be relative to |d l_be / d theta|.  The weights:
+      1vsAll, relation side: W = (|g| + P) (n + c) + P ((Lam_be + max_e Lam_be) / u + |lc - m| + 3 G)
+      KvsAll:                W = |g| (n + c) + w (sig (1 - sig) Lam_be / u + c)
+    P = lambda w_e p_be is the softmax part of g = P - lambda [e == t]; |g| (n + c) is the rounding of the chains the
+    term passes through (ova_chains, plus the red.global.add chain into the row: n_red) and of c further operations;
+    P (n + c) is p's relative rounding error (D's chain is part of n).  Lam_be = (ld + 4) u abs_score_be bounds the
+    logit's error (ld fmas, the query's roundings, the scale), which moves p by at most p (Lam_be + max_e Lam_be)
+    (p = exp(l_b) / sum exp(l_e) does not depend on m) and sigmoid by sig (1 - sig) Lam.  |lc - m| is the rounding of
+    exp's argument, G = sum_e P_e (m - lc_e) that of the online rescales of D (m only grows, so their arguments
+    telescope).  The multi-label rule's sig - y is an absolute error of c u (w: the reduction's weight).  Lam is 0 on
+    dyadic tables, where every logit is exact.  A pair whose logit lies within Lam of +-75 may be clipped by one and not
+    the other: it is charged in full ((|g| + P + lambda [e == t]) / u; KvsAll w |sig - y| / u).  A pair outside the clip
+    range and not near it has g = 0 in both.  A1 (all W = 1) covers results below fp32's smallest normal.
+
+    The loss: 1vsAll rows lambda (m + log D - l_t) with rounding (n_D + c) u (1 + |m| + |log D| + |l_t|) and logit
+    error max Lam + Lam_t; KvsAll elements w (softplus(l) - y l) with rounding (n_loss + c) u (|softplus| + |y l|) and
+    logit error Lam |sig - y|."""
+
+    def __init__(self, model, ent, rel, triples, device="cpu"):
+        self.model, self.device = model, torch.device(device)
+        self.E = torch.as_tensor(np.asarray(ent), dtype=torch.float64, device=self.device)
+        self.R = torch.as_tensor(np.asarray(rel), dtype=torch.float64, device=self.device)
+        self.Ea = self.E.abs().requires_grad_(True)
+        self.Ra = self.R.abs().requires_grad_(True)
+        self.ld = row_stride(model, self.E.shape[1])
+        self.A = [torch.zeros_like(self.E), torch.zeros_like(self.R)]
+        self.A1 = [torch.zeros_like(self.E), torch.zeros_like(self.R)]
+        self.loss = 0.0
+        # red.global.add / in-place adds into one row: the chain pass per lookup on each side, and each side's dX add
+        t = torch.as_tensor(np.asarray(triples), dtype=torch.long, device=self.device).reshape(-1, 3)
+        lookups = max(int(torch.bincount(t[:, [0, 2]].reshape(-1)).max()) if len(t) else 0,
+                      int(torch.bincount(t[:, 1]).max()) if len(t) else 0)
+        self.n_red = 3 * lookups + 4
+
+    def add_side(self, queries, side, reduction="sum", weight=1.0, labels=None, eps=0.0, nsplit=None, xsplit=None):
+        """Adds one side: 's' / 'o' (1vsAll; KvsAll when `labels` is given) or 'p' (relation prediction, weight
+        lambda).  nsplit / xsplit default to the kernel's (ova_geometry).  -> (nsplit, xsplit)."""
+        import k_vs_all_oracle
+        import one_vs_all_oracle
+        import relation_prediction_oracle
+        u, model, E, R, Ea, Ra = FP32_EPS, self.model, self.E, self.R, self.Ea, self.Ra
+        t = torch.as_tensor(np.asarray(queries), dtype=torch.long, device=self.device).reshape(-1, 3)
+        B = t.shape[0]
+        s, p, o = t[:, 0], t[:, 1], t[:, 2]
+        if side == "p":
+            X, Xa, target = R, Ra, p
+            q = relation_prediction_oracle.relation_query(model, E[s], E[o])
+            qa = abs_query(model, Ea[s], Ea[o])
+        else:
+            X, Xa, target = E, Ea, (s if side == "s" else o)
+            q = one_vs_all_oracle.query_vectors(model, side, E[s], R[p], E[o])
+            qa = abs_query(model, *((Ra[p], Ea[o]) if side == "s" else (Ea[s], Ra[p])))
+        n_cand = X.shape[0]
+        geo = ova_geometry(B, n_cand, side == "p")
+        nsplit, xsplit = nsplit or geo[0], xsplit or geo[1]
+        n, n_loss = ova_chains(B, n_cand, nsplit, xsplit, labels is not None)
+        n = n + self.n_red + OVA_C
+        logits = (q @ X.T).detach()
+        AS = qa @ Xa.T
+        lam = (self.ld + 4) * u * AS.detach()
+        inr = (logits.abs() <= ref_step.CLIP_HI).double()
+        near = ((logits.abs() - ref_step.CLIP_HI).abs() < lam).double()
+        lg = logits.clone().requires_grad_(True)
+        if labels is None:
+            loss = weight * one_vs_all_oracle.side_loss(lg, target, reduction).sum()
+        else:
+            y = k_vs_all_oracle.targets(labels, n_cand, eps, self.device)
+            loss = k_vs_all_oracle.side_loss(lg, y, reduction).sum()
+        g = torch.autograd.grad(loss, lg)[0].abs()
+        if labels is None:
+            lc, P, m, D = one_vs_all_oracle.side_softmax(logits, target, reduction)
+            P = weight * P
+            T = torch.zeros_like(P).scatter_(1, target[:, None], weight)
+            G = (P * (m - lc)).sum(1, keepdim=True) / weight
+            W = (inr * ((g + P) * n + P * ((lam + lam.max(1, keepdim=True).values) / u + (lc - m).abs() + 3 * G))
+                 + near * (g + P + T) / u)
+            lt = lc.gather(1, target[:, None])
+            self.loss += weight * float(((n_loss + OVA_C) * u * (1 + m.abs() + torch.log(D).abs() + lt.abs())
+                                         + lam.max(1, keepdim=True).values + lam.gather(1, target[:, None])).sum())
+        else:
+            w = 1.0 / n_cand if reduction == "mean" else 1.0
+            lc = torch.clamp(logits, ref_step.CLIP_LO, ref_step.CLIP_HI)
+            sig = torch.sigmoid(lc)
+            W = inr * (g * n + w * (sig * (1 - sig) * lam / u + OVA_C)) + near * (g + w * (sig - y).abs()) / u
+            sp = torch.nn.functional.softplus(lc)
+            self.loss += w * float(((n_loss + OVA_C) * u * (sp + (y * lc).abs()) + lam * (sig - y).abs()).sum())
+        for acc, wt in ((self.A, W), (self.A1, torch.ones_like(W))):
+            Ea.grad = Ra.grad = None
+            (wt * AS).sum().backward(retain_graph=True)
+            acc[0] += Ea.grad
+            acc[1] += Ra.grad
+        return nsplit, xsplit
+
+    def check(self, got_ent, got_rel, want_ent, want_rel, where=""):
+        """Every element of both gradient tables within the bound (within_bound with the factors folded into A)."""
+        for name, got, want, A, A1 in (("g_ent", got_ent, want_ent, self.A[0], self.A1[0]),
+                                       ("g_rel", got_rel, want_rel, self.A[1], self.A1[1])):
+            got = torch.as_tensor(np.asarray(got), dtype=torch.float64, device=self.device)
+            want = torch.as_tensor(np.asarray(want), dtype=torch.float64, device=self.device)
+            assert bool(torch.isfinite(got).all()), (where, name)
+            ok, ratio = within_bound(got, want, A, A1, 1 - 8, 0)
+            assert ok, (where, name, "worst error / bound %.3g" % ratio)
+
+    def check_loss(self, got, want, where=""):
+        """The loss within its bound (and within 1e-4 of its value, the looser check this one tightens)."""
+        assert np.isfinite(got) and abs(got - want) <= min(self.loss, 1e-4 * abs(want)), (where, got, want, self.loss)

@@ -55,11 +55,12 @@ def side_loss(logits, y, reduction):
     return per / lc.shape[1] if reduction == "mean" else per
 
 
-def loss_and_grads(model, ent, rel, queries, labels, side, reduction="sum", eps=0.0, device="cpu", matmul=False):
-    """(loss, g_ent, g_rel) in float64 of one KvsAll step of one side on dense tables ent [n_ent, K], rel [n_rel, K];
-    queries [b, 3], labels a list of b label lists."""
-    E = torch.as_tensor(np.asarray(ent), dtype=torch.float64, device=device).clone().requires_grad_(True)
-    R = torch.as_tensor(np.asarray(rel), dtype=torch.float64, device=device).clone().requires_grad_(True)
+def loss_and_grads(model, ent, rel, queries, labels, side, reduction="sum", eps=0.0, device="cpu", matmul=False,
+                   dtype=torch.float64):
+    """(loss, g_ent, g_rel) of one KvsAll step of one side on dense tables ent [n_ent, K], rel [n_rel, K]; queries [b, 3],
+    labels a list of b label lists.  In float64; dtype float32 evaluates the same graph in fp32."""
+    E = torch.as_tensor(np.asarray(ent), dtype=dtype, device=device).clone().requires_grad_(True)
+    R = torch.as_tensor(np.asarray(rel), dtype=dtype, device=device).clone().requires_grad_(True)
     total = _side_total(model, E, R, queries, labels, side, reduction, eps, device, matmul)
     total.backward()
     return float(total.detach()), E.grad.cpu().numpy(), R.grad.cpu().numpy()
@@ -72,7 +73,7 @@ def _side_total(model, E, R, queries, labels, side, reduction, eps, device, matm
         logits = query_vectors(model, side, e_s, e_p, e_o) @ E.T
     else:
         logits = ref_step.corruption_scores(model, side, e_s, e_p, e_o, E)
-    return side_loss(logits, targets(labels, E.shape[0], eps, device), reduction).sum()
+    return side_loss(logits, targets(labels, E.shape[0], eps, device).to(E.dtype), reduction).sum()
 
 
 def fit_sgd(model, ent, rel, triples, sides, batch_size, epochs, lr, reduction="sum", eps=0.0):

@@ -37,13 +37,28 @@ def side_loss(logits, target, reduction):
     return -torch.log(et / (neg_mean + et))
 
 
-def loss_and_grads(model, ent, rel, triples, sides="s,o", reduction="sum", device="cpu", matmul=False):
-    """(loss, g_ent, g_rel) in float64 of one 1vsAll step on dense tables ent [n_ent, K], rel [n_rel, K]."""
-    E = torch.as_tensor(np.asarray(ent), dtype=torch.float64, device=device).clone().requires_grad_(True)
-    R = torch.as_tensor(np.asarray(rel), dtype=torch.float64, device=device).clone().requires_grad_(True)
+def side_softmax(logits, target, reduction):
+    """The row quantities behind side_loss, detached: (lc, P, m, D) with lc the clipped logits [b, n], m each row's
+    largest clipped logit, D = w sum_{e != t} exp(lc_e - m) + exp(lc_t - m) (w = 1 for sum, 1 / (n - 1) for mean) and
+    P = w_e exp(lc - m) / D (w_t = 1): dL/dl = P - [e == t] where the logit is inside the clip range."""
+    lc = torch.clamp(logits.detach(), ref_step.CLIP_LO, ref_step.CLIP_HI)
+    m = lc.max(1, keepdim=True).values
+    we = torch.full_like(lc, 1.0 if reduction == "sum" else 1.0 / (lc.shape[1] - 1))
+    we.scatter_(1, target[:, None], 1.0)
+    ex = we * torch.exp(lc - m)
+    D = ex.sum(1, keepdim=True)
+    return lc, ex / D, m, D
+
+
+def loss_and_grads(model, ent, rel, triples, sides="s,o", reduction="sum", device="cpu", matmul=False,
+                   dtype=torch.float64):
+    """(loss, g_ent, g_rel) of one 1vsAll step on dense tables ent [n_ent, K], rel [n_rel, K], in float64 (dtype float32
+    evaluates the same graph in fp32)."""
+    E = torch.as_tensor(np.asarray(ent), dtype=dtype, device=device).clone().requires_grad_(True)
+    R = torch.as_tensor(np.asarray(rel), dtype=dtype, device=device).clone().requires_grad_(True)
     t = torch.as_tensor(np.asarray(triples), dtype=torch.long, device=device)
     e_s, e_p, e_o = E[t[:, 0]], R[t[:, 1]], E[t[:, 2]]
-    total = torch.zeros((), dtype=torch.float64, device=device)
+    total = torch.zeros((), dtype=dtype, device=device)
     for side in sides.split(","):
         if matmul:
             logits = query_vectors(model, side, e_s, e_p, e_o) @ E.T

@@ -30,11 +30,13 @@ def relation_logits(model, e_s, e_o, R, matmul=False):
     return ref_step.compute_scores(model, rep(e_s), R.repeat(b, 1), rep(e_o)).view(b, n_rel)
 
 
-def loss_and_grads(model, ent, rel, triples, weight=1.0, reduction="sum", sides=None, device="cpu", matmul=False):
-    """(loss, g_ent, g_rel) in float64 of weight * L_p, plus L_s + L_o of one_vs_all_oracle on `sides` ('s,o', 'o',
-    's' or None for the relation term alone), on dense tables ent [n_ent, K], rel [n_rel, K]."""
-    E = torch.as_tensor(np.asarray(ent), dtype=torch.float64, device=device).clone().requires_grad_(True)
-    R = torch.as_tensor(np.asarray(rel), dtype=torch.float64, device=device).clone().requires_grad_(True)
+def loss_and_grads(model, ent, rel, triples, weight=1.0, reduction="sum", sides=None, device="cpu", matmul=False,
+                   dtype=torch.float64):
+    """(loss, g_ent, g_rel) of weight * L_p, plus L_s + L_o of one_vs_all_oracle on `sides` ('s,o', 'o', 's' or None
+    for the relation term alone), on dense tables ent [n_ent, K], rel [n_rel, K]; in float64 (dtype float32 evaluates
+    the same graph in fp32)."""
+    E = torch.as_tensor(np.asarray(ent), dtype=dtype, device=device).clone().requires_grad_(True)
+    R = torch.as_tensor(np.asarray(rel), dtype=dtype, device=device).clone().requires_grad_(True)
     t = torch.as_tensor(np.asarray(triples), dtype=torch.long, device=device)
     e_s, e_p, e_o = E[t[:, 0]], R[t[:, 1]], E[t[:, 2]]
     total = weight * one_vs_all_oracle.side_loss(relation_logits(model, e_s, e_o, R, matmul), t[:, 1], reduction).sum()

@@ -4,14 +4,15 @@ and HolE under both reductions, relation counts below one tile, off the tile gri
 clipping, the term added to both entity sides, the weight's scaling, repeatability, the looked-up-rows optimizer rule,
 the FB15k-237 shape, the C-ABI's refusals and fit(relation_prediction_weight=...).
 
-Tolerance: 1e-4 of the table's largest gradient entry, as for the entity sides (tests/test_gpu_one_vs_all.py): each
-logit is an fp32 dot product of ld terms, each gradient entry a sum of n_rel (or B) of them."""
+Tolerance: per element, exact_oracle.OvaBound, as for the entity sides (tests/test_gpu_one_vs_all.py), with the
+relation side's dX split over the query tiles (xsplit) in its chains and lambda in its weights."""
 import ctypes as C
 
 import numpy as np
 import pytest
 import torch
 
+import exact_oracle as xo
 import optim_oracle
 import relation_prediction_oracle
 from ampligraph_b200 import _lib
@@ -73,9 +74,12 @@ def _check(model, k, ent, rel, t, reduction, weight=1.0, sides=None, device="cpu
     g_ent, g_rel = _grads(eng)
     want_loss, want_ent, want_rel = relation_prediction_oracle.loss_and_grads(model, ent, rel, t, weight, reduction,
                                                                               sides, device, matmul)
-    assert np.isfinite(loss) and abs(loss - want_loss) <= RTOL * abs(want_loss), (loss, want_loss)
-    assert _close(g_ent, want_ent), np.abs(g_ent - want_ent).max()
-    assert _close(g_rel, want_rel), np.abs(g_rel - want_rel).max()
+    bound = xo.OvaBound(model, ent, rel, t, device)
+    for side in (sides.split(",") if sides else ()):
+        bound.add_side(t, side, reduction)
+    bound.add_side(t, "p", reduction, weight)
+    bound.check_loss(loss, want_loss, (model, reduction, weight, sides))
+    bound.check(g_ent, g_rel, want_ent, want_rel, (model, reduction, weight, sides))
     # pad columns of the gradient tables stay exactly 0
     assert bool((eng.g_ent[:, k:eng.kp] == 0).all()) and bool((eng.g_rel[:, k:eng.kp] == 0).all())
     eng.close()

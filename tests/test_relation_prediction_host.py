@@ -72,6 +72,7 @@ def test_workspace_formula():
 
 
 @pytest.mark.gpu
+@pytest.mark.gpu
 def test_workspace_formula_matches_the_library():
     """A handle needs a device."""
     from ampligraph_b200 import _lib

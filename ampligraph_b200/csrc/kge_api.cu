@@ -1852,3 +1852,61 @@ extern "C" int kge_k_vs_all_step(kge_handle *h, int32_t side, int32_t loss_reduc
     KGE_CUDA(launch_k_vs_all_side(s, h->L.halves, st), "kge_k_vs_all_step");
     return KGE_OK;
 }
+
+// ---- the N3 regulariser of a step's positives (kge_reg_n3.cu) -----------------------------------------------------
+
+extern "C" int64_t kge_n3_workspace_bytes(const kge_handle *h)
+{
+    if (!h) return 0;
+    return (int64_t)((4 * (size_t)(h->cfg.n_ent + h->cfg.n_rel) + 15) / 16 * 16);
+}
+
+// Allowed while a KGE_STEP_FUSED_DEFER step is pending: it only adds into gradient rows, which the pending step's owner
+// kernel (kge_optimizer_step_deferred) reads for every row of the [ent | rel] block afterwards, and it uses its own
+// workspace, not the training workspace that holds the pending sum.
+extern "C" int kge_n3_step(kge_handle *h, float lambda_ent, float lambda_rel, const float *ent_dev, const float *rel_dev,
+                           float *grad_ent_dev, float *grad_rel_dev, const int32_t *triples_dev, int64_t B, uint64_t step,
+                           double *loss_dev, void *ws_dev, int64_t ws_bytes, void *stream)
+{
+    KGE_CHECK_HANDLE(h, "kge_n3_step");
+    if (!(lambda_ent >= 0.f && lambda_ent <= FLT_MAX) || !(lambda_rel >= 0.f && lambda_rel <= FLT_MAX) ||
+        (lambda_ent == 0.f && lambda_rel == 0.f))
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_n3_step: lambda_ent and lambda_rel must be finite and >= 0, and not both 0; "
+                                              "got %g and %g", (double)lambda_ent, (double)lambda_rel);
+    if (lambda_rel > 0.f && h->cfg.scoring == KGE_ROTATE)
+        return fail(KGE_ERR_UNSUPPORTED, "kge_n3_step: RotatE's relation rows are phases, not embeddings: N3 applies to its "
+                                         "entity table only (lambda_rel = 0)");
+    if (B < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_n3_step: B < 0");
+    if (B == 0) return KGE_OK;
+    if (!triples_dev || (lambda_ent > 0.f && (!ent_dev || !grad_ent_dev)) || (lambda_rel > 0.f && (!rel_dev || !grad_rel_dev)))
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_n3_step: null table, gradient or triples");
+    if (int rc = check_workspace(ws_dev, ws_bytes, kge_n3_workspace_bytes(h), 16, "kge_n3_step", "kge_n3_workspace_bytes"))
+        return rc;
+    N3Params p;
+    memset(&p, 0, sizeof(p));
+    p.ent = ent_dev;
+    p.rel = rel_dev;
+    p.grad_ent = grad_ent_dev;
+    p.grad_rel = grad_rel_dev;
+    p.triples = triples_dev;
+    p.B = B;
+    p.n_ent = h->cfg.n_ent;
+    p.n_rel = h->cfg.n_rel;
+    p.row_begin = lambda_ent > 0.f ? 0 : h->cfg.n_ent;
+    p.row_end = lambda_rel > 0.f ? h->cfg.n_ent + h->cfg.n_rel : h->cfg.n_ent;
+    p.kp = h->L.kp;
+    p.ld = h->L.ld;
+    p.lambda_ent = lambda_ent;
+    p.lambda_rel = lambda_rel;
+    p.lambda3_ent = (float)(3.0 * (double)lambda_ent);
+    p.lambda3_rel = (float)(3.0 * (double)lambda_rel);
+    p.cnt = (int *)ws_dev;
+    p.loss = loss_dev;
+    // the rows the step's positives use are already looked up; stamped anyway (only while the entity buffer is set, as
+    // by every other step entry point)
+    p.stamp = kge_step_stamp(step);
+    p.stamp_ent = h->stamp_ent;
+    p.stamp_rel = h->stamp_ent ? h->stamp_rel : nullptr;
+    KGE_CUDA(launch_n3(p, h->L.halves, h->sm_count, (cudaStream_t)stream), "kge_n3_step");
+    return KGE_OK;
+}

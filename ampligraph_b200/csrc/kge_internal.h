@@ -130,6 +130,24 @@ cudaError_t launch_one_vs_all_stamps(int *stamp_ent, long long n_ent, int stamp,
 // s.xsplit ways over the query tiles (partials in s.pgx), and a chain pass that adds d/ds and d/do to grad_ent
 cudaError_t launch_relation_prediction_side(const OneVsAllSide &s, float *qp, int halves, cudaStream_t st);
 
+// kge_reg_n3.cu: the N3 regulariser of a step's positives (kge_n3_step)
+struct N3Params {
+    const float *ent, *rel;         // [n_ent, ld], [n_rel, ld] (nullptr for a table whose lambda is 0)
+    float *grad_ent, *grad_rel;
+    const int32_t *triples;         // [B, 3]
+    long long B, n_ent, n_rel;
+    long long row_begin, row_end;   // the rows of the [ent | rel] block with lambda > 0
+    int kp, ld;
+    float lambda_ent, lambda_rel;   // lambda of each table (0: not regularised)
+    float lambda3_ent, lambda3_rel; // 3 * lambda, rounded once
+    int *cnt;                       // [n_ent + n_rel] occurrences per row (workspace; zeroed by launch_n3)
+    double *loss;                   // += L_N3, or nullptr
+    int stamp;
+    int *stamp_ent, *stamp_rel;     // lazy-optimizer stamps of the rows with c > 0, or nullptr
+};
+// memset of p.cnt, the count pass and the apply pass, on st
+cudaError_t launch_n3(const N3Params &p, int halves, int sm_count, cudaStream_t st);
+
 // kge_misc.cu
 cudaError_t launch_score_triples(const Layout &L, int nit, const float *ent, const float *rel_or_rot,
                                  const int32_t *triples, long long n, float scale, float *out, int sm_count,

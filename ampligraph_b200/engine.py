@@ -209,8 +209,9 @@ class KGEEngine:
     def __init__(self, scoring_type, k, eta, n_ent, n_rel, loss="pairwise", loss_params=None,
                  optimizer="adam", optimizer_params=None, regularizer=None, device=0, neg_group=0,
                  table_alloc=None, ent_rows=None, max_rel_size=None, rank_mode=None, rank_pair_cap=0, lazy_tables=None):
-        """regularizer: None | {"p":, "lambda": [, "p2":, "lambda2":]} | a pair [entities, relations] of those
-        (EmbeddingLookupLayer.py:131-155).  lazy_tables: see set_optimizer.  max_rel_size: RotatE phase normalisation when it differs from the
+        """regularizer: None | {"p":, "lambda": [, "p2":, "lambda2":]} | {"kind": "N3", "lambda":} | a pair
+        [entities, relations] of those (EmbeddingLookupLayer.py:131-155).  An LP term goes to the optimizer; N3 is
+        n3_backward's.  lazy_tables: see set_optimizer.  max_rel_size: RotatE phase normalisation when it differs from the
         relation-table rows (RotatE.py:96).  rank_mode: 'auto' (tensor-core filter + exact refine for the bilinear
         models) | 'exact' (FP32 canonical chain for every pair); env KGE_B200_RANK_MODE overrides the default."""
         self.lib = _lib.load()
@@ -297,6 +298,11 @@ class KGEEngine:
             raise NotImplementedError("centered RMSprop with momentum needs a third slot buffer (not supported)")
         regs = list(regularizer) if isinstance(regularizer, (list, tuple)) else [regularizer, regularizer]
         assert len(regs) == 2, "Incorrect length for regularizer. Expected 2, got {}".format(len(regs))
+
+        # N3 (DESIGN.md 3.15) is not an optimizer term: its lambdas are n3_backward's, and the optimizer sees no regulariser
+        n3 = [float(r["lambda"]) if (r or {}).get("kind") == "N3" else 0.0 for r in regs]
+        self.n3_lambdas = {"ent": n3[0], "rel": n3[1]}
+        regs = [None if (r or {}).get("kind") == "N3" else r for r in regs]
 
         def cfg_for(reg):
             reg = dict(reg or {})
@@ -500,6 +506,35 @@ class KGEEngine:
         # query vectors (two kernels), entity stamps, dQ, dX and chain
         if B:
             self.launches += 2 + (1 if self.lazy else 0) + 3
+
+    @property
+    def n3_workspace_bytes(self):
+        """kge_n3_workspace_bytes(h): one int32 count per row of the [ent | rel] block, rounded up to 16 bytes."""
+        return (4 * (self.n_ent + self.n_rel) + 15) // 16 * 16
+
+    @_traced("kge.n3_step")
+    def n3_backward(self, triples, step=0):
+        """The N3 regulariser of a step's positives up to tape.gradient (kge_n3_step, DESIGN.md 3.15): lambda *
+        sum_d |z_d|^3 of each positive's s and o rows (entity lambda) and p row (relation lambda), lambdas from the
+        engine's regulariser config (n3_lambdas); adds into g_ent / g_rel and loss_acc[1], like the LP term of the
+        optimizer.  Call it once per step, after the data term(s) and before apply_gradients().  Allowed while a
+        deferred step is pending: the deferred optimizer reads every gradient row.  step: the lazy optimizer's row
+        stamp."""
+        assert triples.dtype == torch.int32 and triples.is_cuda and triples.is_contiguous()
+        lam_e, lam_r = self.n3_lambdas["ent"], self.n3_lambdas["rel"]
+        if lam_e == 0.0 and lam_r == 0.0:
+            raise ValueError("n3_backward: no table of this engine has the N3 regulariser")
+        if self.ent_rows != self.n_ent:
+            raise NotImplementedError("the N3 regulariser needs the whole entity table: row-sharded tables are not supported")
+        need = self.n3_workspace_bytes
+        if getattr(self, "_n3_ws", None) is None or self._n3_ws.numel() < need:
+            self._n3_ws = torch.empty(need, dtype=torch.uint8, device=self.device)  # 256-byte aligned (torch)
+        _lib.check(self.lib.kge_n3_step(
+            self.h, lam_e, lam_r, _ptr(self.ent), _ptr(self.rel), _ptr(self.g_ent), _ptr(self.g_rel), _ptr(triples),
+            triples.shape[0], int(step), C.c_void_p(self.loss_acc.data_ptr() + 8), _ptr(self._n3_ws), need, self._stream()))
+        self._last_step = int(step)
+        if triples.shape[0]:
+            self.launches += 2  # count and apply (and a memset)
 
     def _one_block(self):
         """True when tables, gradients and slots still ARE the [ent | rel] blocks allocated here (callers may rebind them: the

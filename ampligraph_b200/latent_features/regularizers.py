@@ -5,6 +5,10 @@ LP_regularizer = lambda * sum(|x|^p) over the WHOLE table (regularizers.py:14-37
 loss and dense gradient are fused into the optimizer kernel (csrc/kge_optim.cu).  Keras' 'l1', 'l2' and
 'l1_l2' are the same thing with p = 1 / 2 (/ both) and Keras' default factor 0.01.  `compile` accepts one
 regulariser for both tables or a list [entities, relations], exactly like the reference.
+
+N3 (extension, not in the reference): the weighted nuclear 3-norm of Lacroix, Usunier and Obozinski (ICML 2018, eq. 6),
+lambda * sum of |z_d|^3 over the rows the step's positives use, once per occurrence; |z_d| is the complex modulus for
+the two-half layouts.  Its loss and row-sparse gradient come from csrc/kge_reg_n3.cu (DESIGN.md 3.15).
 """
 
 
@@ -31,11 +35,35 @@ def LP_regularizer(regularizer_parameters=None):
     return LPRegularizer(regularizer_parameters)
 
 
+class N3Regularizer:
+    """N3: lambda * sum over the step's positives (s, p, o) of sum_d |z_d|^3 of each of their rows (DESIGN.md 3.15).
+    regularizer_parameters: {"lambda": lambda}, default 1e-3 (no precedent here: LP's 1e-5 is a whole-table weight)."""
+    __name__ = "N3"
+
+    def __init__(self, regularizer_parameters=None):
+        rp = dict(regularizer_parameters or {})
+        self.lam = float(rp.get("lambda", 0.001))
+        if not self.lam >= 0.0 or self.lam == float("inf"):
+            raise ValueError("N3 regularizer: lambda must be finite and >= 0, got %r" % (rp.get("lambda"),))
+
+    def kernel_params(self):
+        return {"kind": "N3", "lambda": self.lam}
+
+
+def N3_regularizer(regularizer_parameters=None):
+    return N3Regularizer(regularizer_parameters)
+
+
+def is_n3(params):
+    """Whether a regulariser's kernel_params() (or None) is N3's."""
+    return params is not None and params.get("kind") == "N3"
+
+
 def get(identifier, hyperparams=None):
     """regularizers.get (:40-73) + tf.keras.regularizers.get: 'LP' | 'l3' | 'l1' | 'l2' | 'l1_l2' |
-    {'class_name': 'L1'|'L2'|'L1L2', 'config': {...}} | LPRegularizer | None."""
+    {'class_name': 'L1'|'L2'|'L1L2', 'config': {...}} | LPRegularizer | None; and 'N3' / 'n3' | N3Regularizer."""
     hyperparams = dict(hyperparams or {})
-    if identifier is None or isinstance(identifier, LPRegularizer):
+    if identifier is None or isinstance(identifier, (LPRegularizer, N3Regularizer)):
         return identifier
     if isinstance(identifier, dict):
         cfg = dict(identifier.get("config", {}))
@@ -54,6 +82,8 @@ def get(identifier, hyperparams=None):
             return LPRegularizer(hyperparams)
         if identifier == "LP":
             return LPRegularizer(hyperparams)
+        if key == "n3":
+            return N3Regularizer(hyperparams)
         if key == "l2":  # Keras 'l2': 0.01 * sum(x^2)
             return LPRegularizer({"p": 2, "lambda": hyperparams.get("lambda", 0.01)})
         if key == "l1":

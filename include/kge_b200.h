@@ -339,6 +339,29 @@ int kge_k_vs_all_step(kge_handle *h, int32_t side, int32_t loss_reduction, float
                       const int64_t *label_offsets_dev, const int32_t *label_ids_dev, uint64_t step, double *loss_dev,
                       void *ws_dev, int64_t ws_bytes, void *stream);
 
+/* The N3 regulariser (Lacroix, Usunier and Obozinski, ICML 2018, eq. 6) of a step's B positives (s_b, p_b, o_b):
+ * L_N3 = lambda_ent * sum_b sum_d (|s_bd|^3 + |o_bd|^3) + lambda_rel * sum_b sum_d |p_bd|^3, duplicates counted every
+ * time they occur.  |z_d| is |x[d]| for TransE and DistMult, and the modulus sqrt(x[d]^2 + x[kp + d]^2) for ComplEx,
+ * HolE and RotatE; the gradient is 3 lambda |z_d| z_d, component-wise.  Only the rows the positives use get a gradient,
+ * so a table regularised with N3 keeps the looked-up-rows optimizer rule.  A table whose lambda is 0 is not read or
+ * written and may be passed as NULL (table and gradient).  B = 0 is a no-op.
+ *   grad_*_dev  ADDED to, one writer per row (bit-for-bit repeatable); call it after the step's data term(s) and before
+ *               the optimizer
+ *   step        the lazy-optimizer stamp: the rows with an occurrence are stamped with kge_step_stamp(step) (while an
+ *               entity stamp buffer is set, as for kge_train_step)
+ *   loss_dev    double accumulator += L_N3 (may be NULL)
+ *   ws_dev      caller-owned, 16-byte aligned, at least kge_n3_workspace_bytes(h) = (n_ent + n_rel) * 4 bytes rounded
+ *               up to 16: the per-row counts, zeroed by the call
+ * KGE_ERR_INVALID_ARGUMENT: a lambda not finite or < 0, both lambdas 0, B < 0, null pointers, a short or misaligned
+ * workspace.  KGE_ERR_UNSUPPORTED: lambda_rel > 0 for RotatE (its relation rows are phases).  Unlike the other step
+ * entry points it is accepted while a KGE_STEP_FUSED_DEFER step is pending: kge_optimizer_step_deferred reads every
+ * gradient row of the block, so the N3 rows added here are part of that update.  The tables are the ones the step
+ * trained on (the parameters before the update), whole: row-sharded tables are not supported.  DESIGN.md 3.15. */
+int64_t kge_n3_workspace_bytes(const kge_handle *h);
+int kge_n3_step(kge_handle *h, float lambda_ent, float lambda_rel, const float *ent_dev, const float *rel_dev,
+                float *grad_ent_dev, float *grad_rel_dev, const int32_t *triples_dev, int64_t B, uint64_t step,
+                double *loss_dev, void *ws_dev, int64_t ws_bytes, void *stream);
+
 /* OptimizerWrapper.minimize -> legacy apply_gradients (optimizers.py:136-168) for ONE
  * table (or any row-wise concatenation of tables of the same width and regulariser: the engine passes [ent | rel] as one
  * block, one launch per step), dense semantics, plus the LP regulariser's loss/gradient over the whole table

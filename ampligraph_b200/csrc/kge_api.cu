@@ -1532,39 +1532,148 @@ extern "C" int kge_graph_counts(const int64_t *offsets_dev, const int32_t *nbr_d
     return KGE_OK;
 }
 
-// ---- 1vsAll training (kge_train_1vsall.cu) ------------------------------------------------------------------
+// ---- all-candidate training: 1vsAll, relation prediction and KvsAll (kge_train_1vsall.cu) ---------------------------
 
-// Carve-up of the workspace of a 1vsAll step of B positives: both sides' query vectors (and the quantised positive
-// scores launch_rank_prepare also writes), then the per-side scratch, reused by the second side.
-struct OneVsAllWorkspace {
+// What sets the three all-candidate steps apart on the host
+struct CandidateRule {
+    const char *fn, *training, *sizer;  // entry point, what it trains, its workspace sizing function (messages)
+    const char *inputs;                 // its pointer arguments (message of the null-pointer refusal)
+    bool relation;    // the candidates are the relation rows (side p, queries Qp), else the entity rows (sides s, o)
+    bool multiclass;  // multiclass NLL (row statistics), else KvsAll's element-wise multi-label loss (label masks)
+};
+static const CandidateRule ONE_VS_ALL = {"kge_one_vs_all_step", "1vsAll", "kge_one_vs_all_workspace_bytes",
+                                         "table, gradient or triples", false, true};
+static const CandidateRule RELATION_PREDICTION = {"kge_one_vs_all_relation_step", "relation prediction",
+                                                  "kge_one_vs_all_relation_workspace_bytes", "table, gradient or triples",
+                                                  true, true};
+static const CandidateRule K_VS_ALL = {"kge_k_vs_all_step", "KvsAll", "kge_k_vs_all_workspace_bytes",
+                                       "table, gradient, queries or labels", false, false};
+
+// The query vectors of a step: the entity sides' (and the quantised positive scores launch_rank_prepare also writes),
+// or the relation step's Qp in qs
+struct CandidateQueries {
     float *qs, *qo;
     int32_t *qpos;
-    float *pm, *pz, *lt, *row_m, *row_inv, *pgq;
-    int nsplit;
 };
-static OneVsAllWorkspace carve_one_vs_all(const kge_handle *h, int64_t B, Carve &c)
+
+// Carve-up of the workspace of a step of s.B queries into the query vectors and the scratch of s's passes: the row
+// statistics of the multiclass loss, the per-split partial Gq rows and, when dX is split over the query tiles, its
+// [xsplit, n_cand, ld] partial candidate rows.  Sets s.nsplit and s.xsplit; regions a step does not hold stay nullptr.
+static CandidateQueries carve_candidates(const kge_handle *h, const CandidateRule &r, Carve &c, OneVsAllSide &s)
 {
-    OneVsAllWorkspace w;
-    w.nsplit = one_vs_all_splits(B, h->cfg.n_ent);
-    const size_t rows = (size_t)B * h->L.ld * sizeof(float), col = (size_t)B * sizeof(float), ns = (size_t)w.nsplit;
-    w.qs = c.take<float>(rows, 16);
-    w.qo = c.take<float>(rows, 16);
-    w.qpos = c.take<int32_t>(col, 16);
-    w.pm = c.take<float>(ns * col, 16);
-    w.pz = c.take<float>(ns * col, 16);
-    w.lt = c.take<float>(col, 16);
-    w.row_m = c.take<float>(col, 16);
-    w.row_inv = c.take<float>(col, 16);
-    w.pgq = c.take<float>(ns * rows, 16);
-    return w;
+    CandidateQueries q = {};
+    s.nsplit = one_vs_all_splits(s.B, s.n_cand);
+    // dX of the relation step: the same split rule with the roles swapped, query tiles per relation tile
+    s.xsplit = r.relation ? one_vs_all_splits(s.n_cand, s.B) : 1;
+    const size_t rows = (size_t)s.B * h->L.ld * sizeof(float), col = (size_t)s.B * sizeof(float), ns = (size_t)s.nsplit;
+    q.qs = c.take<float>(rows, 16);
+    if (!r.relation) {
+        q.qo = c.take<float>(rows, 16);
+        q.qpos = c.take<int32_t>(col, 16);
+    }
+    if (r.multiclass) {
+        s.pm = c.take<float>(ns * col, 16);
+        s.pz = c.take<float>(ns * col, 16);
+        s.lt = c.take<float>(col, 16);
+        s.row_m = c.take<float>(col, 16);
+        s.row_inv = c.take<float>(col, 16);
+    }
+    s.pgq = c.take<float>(ns * rows, 16);
+    if (s.xsplit > 1) s.pgx = c.take<float>((size_t)s.xsplit * s.n_cand * h->L.ld * sizeof(float), 16);
+    return q;
+}
+
+// The OneVsAllSide fields every all-candidate step shares; side, col and q are the entry point's, the workspace regions
+// carve_candidates' and w start_candidate_step's.  The stamps are written only while the entity buffer is set, like kge_train_step:
+// start_candidate_step stamps the candidate rows, the chain pass the batch's other rows (its relation rows; on the
+// relation step its s and o rows).
+static OneVsAllSide candidate_side(const kge_handle *h, const CandidateRule &r, const float *ent, const float *rel,
+                                   float *grad_ent, float *grad_rel, const int32_t *triples, int64_t B, uint64_t step,
+                                   double *loss)
+{
+    OneVsAllSide s;
+    memset(&s, 0, sizeof(s));
+    s.ent = ent;
+    s.rel = rel;
+    s.grad_ent = grad_ent;
+    s.grad_rel = grad_rel;
+    s.cand = r.relation ? rel : ent;
+    s.grad_cand = r.relation ? grad_rel : grad_ent;
+    s.triples = triples;
+    s.B = B;
+    s.n_cand = r.relation ? h->cfg.n_rel : h->cfg.n_ent;
+    s.kp = h->L.kp;
+    s.ld = h->L.ld;
+    s.scale = h->score_scale;
+    s.weight = 1.f;
+    s.loss = loss;
+    s.stamp = kge_step_stamp(step);
+    s.stamp_ent = h->stamp_ent;
+    s.stamp_rel = h->stamp_ent ? h->stamp_rel : nullptr;
+    return s;
+}
+
+static int64_t candidate_workspace_bytes(const kge_handle *h, const CandidateRule &r, int64_t B)
+{
+    if (!h || B < 0) return 0;
+    OneVsAllSide s = candidate_side(h, r, nullptr, nullptr, nullptr, nullptr, nullptr, B, 0, nullptr);
+    Carve c(nullptr);
+    carve_candidates(h, r, c, s);
+    return (int64_t)c.at;
+}
+
+// The refusals of an all-candidate step s, in this order, every one before the first launch: the model; the entry
+// point's own arguments (own(): KGE_OK or the code of the refusal it reported) and the reduction; a pending deferred
+// step; fewer than two candidates; rows too wide for the kernels' shared-memory tiles; B < 0.  An empty batch passes
+// before the pointers and the workspace are checked: the caller returns KGE_OK without launching.  Then null tables,
+// gradients or triples (own_null: the entry point's other pointers), and the workspace (16-byte aligned).
+template <class Own>
+static int check_candidate_step(const kge_handle *h, const CandidateRule &r, const OneVsAllSide &s, int32_t reduction,
+                                Own own, bool own_null, void *ws, int64_t ws_bytes)
+{
+    const int model = h->cfg.scoring;
+    if (model != KGE_DISTMULT && model != KGE_COMPLEX && model != KGE_HOLE)
+        return fail(KGE_ERR_UNSUPPORTED, "%s: %s training is implemented for DistMult, ComplEx and HolE (inner-product "
+                                         "scores); not for scoring type %d", r.fn, r.training, model);
+    if (int rc = own()) return rc;
+    if (reduction != KGE_REDUCE_SUM && reduction != KGE_REDUCE_MEAN)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "Invalid value for reduction!");
+    if (int rc = check_no_pending(h, r.fn)) return rc;
+    if (s.n_cand < 2) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: needs %s >= 2", r.fn, r.relation ? "n_rel" : "n_ent");
+    if ((long long)(r.multiclass ? one_vs_all_smem_bytes(s.ld) : k_vs_all_smem_bytes(s.ld)) > h->max_smem)
+        return fail(KGE_ERR_UNSUPPORTED, "%s: rows of %d floats exceed the shared-memory tiles of the %s kernels (%d B)",
+                    r.fn, s.ld, r.training, h->max_smem);
+    if (s.B < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: B < 0", r.fn);
+    if (s.B == 0) return KGE_OK;
+    if (!s.ent || !s.rel || !s.grad_ent || !s.grad_rel || !s.triples || own_null)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "%s: null %s", r.fn, r.inputs);
+    return check_workspace(ws, ws_bytes, candidate_workspace_bytes(h, r, s.B), 16, r.fn, r.sizer);
+}
+
+// What every checked all-candidate step does before its passes: set the loss weight of the reduction, carve the
+// workspace ws into s and *q, write the entity sides' query vectors, and stamp every candidate row as looked up
+static int start_candidate_step(const kge_handle *h, const CandidateRule &r, int32_t reduction, void *ws, cudaStream_t st,
+                                OneVsAllSide &s, CandidateQueries *q)
+{
+    // mean: a negative's exp weighs 1 / (n_cand - 1) in the multiclass loss, every element 1 / n_ent in KvsAll's
+    s.w = reduction == KGE_REDUCE_MEAN ? (float)(1.0 / (double)(r.multiclass ? s.n_cand - 1 : s.n_cand)) : 1.f;
+    Carve c(ws);
+    *q = carve_candidates(h, r, c, s);
+    if (!r.relation) {
+        ShardView sv;
+        memset(&sv, 0, sizeof(sv));
+        KGE_CUDA(launch_rank_prepare(h->L, sv, s.ent, s.rel, nullptr, s.triples, s.B, h->score_scale, q->qs, q->qo, nullptr,
+                                     q->qpos, st),
+                 r.fn);
+    }
+    if (h->stamp_ent)
+        KGE_CUDA(launch_one_vs_all_stamps(r.relation ? h->stamp_rel : h->stamp_ent, s.n_cand, s.stamp, st), r.fn);
+    return KGE_OK;
 }
 
 extern "C" int64_t kge_one_vs_all_workspace_bytes(const kge_handle *h, int64_t B)
 {
-    if (!h || B < 0) return 0;
-    Carve c(nullptr);
-    carve_one_vs_all(h, B, c);
-    return (int64_t)c.at;
+    return candidate_workspace_bytes(h, ONE_VS_ALL, B);
 }
 
 extern "C" int kge_one_vs_all_step(kge_handle *h, int32_t sides, int32_t loss_reduction, const float *ent_dev,
@@ -1573,109 +1682,32 @@ extern "C" int kge_one_vs_all_step(kge_handle *h, int32_t sides, int32_t loss_re
                                    int64_t ws_bytes, void *stream)
 {
     KGE_CHECK_HANDLE(h, "kge_one_vs_all_step");
-    const int model = h->cfg.scoring;
-    if (model != KGE_DISTMULT && model != KGE_COMPLEX && model != KGE_HOLE)
-        return fail(KGE_ERR_UNSUPPORTED, "kge_one_vs_all_step: 1vsAll training is implemented for DistMult, ComplEx and HolE "
-                                         "(inner-product scores); not for scoring type %d", model);
-    if (sides < KGE_ONE_VS_ALL_S || sides > (KGE_ONE_VS_ALL_S | KGE_ONE_VS_ALL_O))
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_step: sides must be a non-empty set of KGE_ONE_VS_ALL_S | "
-                                              "KGE_ONE_VS_ALL_O, got %d", sides);
-    if (loss_reduction != KGE_REDUCE_SUM && loss_reduction != KGE_REDUCE_MEAN)
-        return fail(KGE_ERR_INVALID_ARGUMENT, "Invalid value for reduction!");
-    if (int rc = check_no_pending(h, "kge_one_vs_all_step")) return rc;
-    if (h->cfg.n_ent < 2) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_step: needs n_ent >= 2");
-    if ((long long)one_vs_all_smem_bytes(h->L.ld) > h->max_smem)
-        return fail(KGE_ERR_UNSUPPORTED, "kge_one_vs_all_step: rows of %d floats exceed the shared-memory tiles of the 1vsAll "
-                                         "kernels (%d B)", h->L.ld, h->max_smem);
-    if (B < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_step: B < 0");
-    if (B == 0) return KGE_OK;
-    if (!ent_dev || !rel_dev || !grad_ent_dev || !grad_rel_dev || !triples_dev)
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_step: null table, gradient or triples");
-    if (int rc = check_workspace(ws_dev, ws_bytes, kge_one_vs_all_workspace_bytes(h, B), 16, "kge_one_vs_all_step",
-                                 "kge_one_vs_all_workspace_bytes"))
+    OneVsAllSide s = candidate_side(h, ONE_VS_ALL, ent_dev, rel_dev, grad_ent_dev, grad_rel_dev, triples_dev,
+                                    B, step, loss_dev);
+    if (int rc = check_candidate_step(h, ONE_VS_ALL, s, loss_reduction, [&]() -> int {
+            if (sides < KGE_ONE_VS_ALL_S || sides > (KGE_ONE_VS_ALL_S | KGE_ONE_VS_ALL_O))
+                return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_step: sides must be a non-empty set of "
+                                                      "KGE_ONE_VS_ALL_S | KGE_ONE_VS_ALL_O, got %d", sides);
+            return KGE_OK;
+        }, false, ws_dev, ws_bytes))
         return rc;
+    if (B == 0) return KGE_OK;
     cudaStream_t st = (cudaStream_t)stream;
-    Carve c(ws_dev);
-    const OneVsAllWorkspace w = carve_one_vs_all(h, B, c);
-    ShardView sv;
-    memset(&sv, 0, sizeof(sv));
-    KGE_CUDA(launch_rank_prepare(h->L, sv, ent_dev, rel_dev, nullptr, triples_dev, B, h->score_scale, w.qs, w.qo, nullptr,
-                                 w.qpos, st),
-             "kge_one_vs_all_step (query vectors)");
-    const int stamp = kge_step_stamp(step);
-    // every entity row is a candidate of the step: all of them count as looked up (stamped only while the entity
-    // buffer is set, like kge_train_step); the relation rows of the batch are stamped by the chain pass
-    if (h->stamp_ent) KGE_CUDA(launch_one_vs_all_stamps(h->stamp_ent, h->cfg.n_ent, stamp, st), "kge_one_vs_all_step (stamps)");
-    OneVsAllSide s;
-    memset(&s, 0, sizeof(s));
-    s.ent = ent_dev;
-    s.rel = rel_dev;
-    s.grad_ent = grad_ent_dev;
-    s.grad_rel = grad_rel_dev;
-    s.triples = triples_dev;
-    s.B = B;
-    s.cand = ent_dev;
-    s.grad_cand = grad_ent_dev;
-    s.n_cand = h->cfg.n_ent;
-    s.weight = 1.f;
-    s.xsplit = 1;
-    s.kp = h->L.kp;
-    s.ld = h->L.ld;
-    s.nsplit = w.nsplit;
-    s.scale = h->score_scale;
-    s.w = loss_reduction == KGE_REDUCE_MEAN ? (float)(1.0 / (double)(h->cfg.n_ent - 1)) : 1.f;
-    s.loss = loss_dev;
-    s.stamp = stamp;
-    s.stamp_rel = h->stamp_ent ? h->stamp_rel : nullptr;
-    s.pm = w.pm;
-    s.pz = w.pz;
-    s.lt = w.lt;
-    s.row_m = w.row_m;
-    s.row_inv = w.row_inv;
-    s.pgq = w.pgq;
+    CandidateQueries q;
+    if (int rc = start_candidate_step(h, ONE_VS_ALL, loss_reduction, ws_dev, st, s, &q)) return rc;
     for (int side = KGE_SIDE_S; side <= KGE_SIDE_O; ++side) {
         if (!(sides & (side == KGE_SIDE_S ? KGE_ONE_VS_ALL_S : KGE_ONE_VS_ALL_O))) continue;
         s.side = side;
         s.col = side == KGE_SIDE_S ? 0 : 2;
-        s.q = side == KGE_SIDE_S ? w.qs : w.qo;
+        s.q = side == KGE_SIDE_S ? q.qs : q.qo;
         KGE_CUDA(launch_one_vs_all_side(s, h->L.halves, st), "kge_one_vs_all_step");
     }
     return KGE_OK;
 }
 
-// ---- relation prediction as an auxiliary 1vsAll term (kge_train_1vsall.cu) --------------------------------------
-
-// Carve-up of the workspace of a relation-prediction step of B positives: the relation queries Qp [B, ld], the row
-// statistics of the 1vsAll passes over the n_rel relations, the per-split partial query gradients and, when dX is
-// split over the query tiles, its [xsplit, n_rel, ld] partial relation rows.
-struct RelationPredictionWorkspace {
-    float *qp, *pm, *pz, *lt, *row_m, *row_inv, *pgq, *pgx;
-    int nsplit, xsplit;
-};
-static RelationPredictionWorkspace carve_relation_prediction(const kge_handle *h, int64_t B, Carve &c)
-{
-    RelationPredictionWorkspace w;
-    const long long n_rel = h->cfg.n_rel;
-    w.nsplit = one_vs_all_splits(B, n_rel);
-    w.xsplit = one_vs_all_splits(n_rel, B);  // the same split rule with the roles swapped: query tiles per relation tile
-    const size_t rows = (size_t)B * h->L.ld * sizeof(float), col = (size_t)B * sizeof(float), ns = (size_t)w.nsplit;
-    w.qp = c.take<float>(rows, 16);
-    w.pm = c.take<float>(ns * col, 16);
-    w.pz = c.take<float>(ns * col, 16);
-    w.lt = c.take<float>(col, 16);
-    w.row_m = c.take<float>(col, 16);
-    w.row_inv = c.take<float>(col, 16);
-    w.pgq = c.take<float>(ns * rows, 16);
-    w.pgx = c.take<float>(w.xsplit > 1 ? (size_t)w.xsplit * n_rel * h->L.ld * sizeof(float) : 0, 16);
-    return w;
-}
-
 extern "C" int64_t kge_one_vs_all_relation_workspace_bytes(const kge_handle *h, int64_t B)
 {
-    if (!h || B < 0) return 0;
-    Carve c(nullptr);
-    carve_relation_prediction(h, B, c);
-    return (int64_t)c.at;
+    return candidate_workspace_bytes(h, RELATION_PREDICTION, B);
 }
 
 extern "C" int kge_one_vs_all_relation_step(kge_handle *h, float weight, int32_t loss_reduction, const float *ent_dev,
@@ -1684,98 +1716,30 @@ extern "C" int kge_one_vs_all_relation_step(kge_handle *h, float weight, int32_t
                                             void *ws_dev, int64_t ws_bytes, void *stream)
 {
     KGE_CHECK_HANDLE(h, "kge_one_vs_all_relation_step");
-    const int model = h->cfg.scoring;
-    if (model != KGE_DISTMULT && model != KGE_COMPLEX && model != KGE_HOLE)
-        return fail(KGE_ERR_UNSUPPORTED, "kge_one_vs_all_relation_step: relation prediction training is implemented for "
-                                         "DistMult, ComplEx and HolE (inner-product scores); not for scoring type %d", model);
-    if (loss_reduction != KGE_REDUCE_SUM && loss_reduction != KGE_REDUCE_MEAN)
-        return fail(KGE_ERR_INVALID_ARGUMENT, "Invalid value for reduction!");
-    if (!(weight > 0.f && weight <= FLT_MAX))
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_relation_step: weight must be finite and > 0, got %g",
-                    (double)weight);
-    if (int rc = check_no_pending(h, "kge_one_vs_all_relation_step")) return rc;
-    if (h->cfg.n_rel < 2) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_relation_step: needs n_rel >= 2");
-    if ((long long)one_vs_all_smem_bytes(h->L.ld) > h->max_smem)
-        return fail(KGE_ERR_UNSUPPORTED, "kge_one_vs_all_relation_step: rows of %d floats exceed the shared-memory tiles of "
-                                         "the 1vsAll kernels (%d B)", h->L.ld, h->max_smem);
-    if (B < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_relation_step: B < 0");
-    if (B == 0) return KGE_OK;
-    if (!ent_dev || !rel_dev || !grad_ent_dev || !grad_rel_dev || !triples_dev)
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_relation_step: null table, gradient or triples");
-    if (int rc = check_workspace(ws_dev, ws_bytes, kge_one_vs_all_relation_workspace_bytes(h, B), 16,
-                                 "kge_one_vs_all_relation_step", "kge_one_vs_all_relation_workspace_bytes"))
+    OneVsAllSide s = candidate_side(h, RELATION_PREDICTION, ent_dev, rel_dev, grad_ent_dev, grad_rel_dev, triples_dev, B,
+                                    step, loss_dev);
+    if (int rc = check_candidate_step(h, RELATION_PREDICTION, s, loss_reduction, [&]() -> int {
+            if (!(weight > 0.f && weight <= FLT_MAX))
+                return fail(KGE_ERR_INVALID_ARGUMENT, "kge_one_vs_all_relation_step: weight must be finite and > 0, got %g",
+                            (double)weight);
+            return KGE_OK;
+        }, false, ws_dev, ws_bytes))
         return rc;
+    if (B == 0) return KGE_OK;
     cudaStream_t st = (cudaStream_t)stream;
-    Carve c(ws_dev);
-    const RelationPredictionWorkspace w = carve_relation_prediction(h, B, c);
-    const int stamp = kge_step_stamp(step);
-    // every relation row is a candidate of the step: all of them count as looked up; the batch's s and o rows are
-    // stamped by the chain pass (only while the entity buffer is set, like kge_one_vs_all_step)
-    if (h->stamp_ent && h->stamp_rel)
-        KGE_CUDA(launch_one_vs_all_stamps(h->stamp_rel, h->cfg.n_rel, stamp, st), "kge_one_vs_all_relation_step (stamps)");
-    OneVsAllSide s;
-    memset(&s, 0, sizeof(s));
-    s.q = w.qp;
-    s.ent = ent_dev;
-    s.rel = rel_dev;
-    s.grad_ent = grad_ent_dev;
-    s.grad_rel = grad_rel_dev;
-    s.cand = rel_dev;
-    s.grad_cand = grad_rel_dev;
-    s.triples = triples_dev;
-    s.B = B;
-    s.n_cand = h->cfg.n_rel;
+    CandidateQueries q;
+    if (int rc = start_candidate_step(h, RELATION_PREDICTION, loss_reduction, ws_dev, st, s, &q)) return rc;
     s.side = KGE_SIDE_P;
     s.col = 1;
-    s.kp = h->L.kp;
-    s.ld = h->L.ld;
-    s.nsplit = w.nsplit;
-    s.scale = h->score_scale;
-    s.w = loss_reduction == KGE_REDUCE_MEAN ? (float)(1.0 / (double)(h->cfg.n_rel - 1)) : 1.f;
+    s.q = q.qs;
     s.weight = weight;
-    s.xsplit = w.xsplit;
-    s.loss = loss_dev;
-    s.stamp = stamp;
-    s.stamp_ent = h->stamp_ent;
-    s.pm = w.pm;
-    s.pz = w.pz;
-    s.lt = w.lt;
-    s.row_m = w.row_m;
-    s.row_inv = w.row_inv;
-    s.pgq = w.pgq;
-    s.pgx = w.pgx;
-    KGE_CUDA(launch_relation_prediction_side(s, w.qp, h->L.halves, st), "kge_one_vs_all_relation_step");
+    KGE_CUDA(launch_relation_prediction_side(s, q.qs, h->L.halves, st), "kge_one_vs_all_relation_step");
     return KGE_OK;
-}
-
-// ---- KvsAll training (kge_train_1vsall.cu) ------------------------------------------------------------------
-
-// Carve-up of the workspace of a KvsAll step of B queries: what launch_rank_prepare writes (both sides' query vectors
-// and the quantised positive scores) and the per-split partial Gq rows.  The loss is element-wise: no row statistics.
-struct KVsAllWorkspace {
-    float *qs, *qo;
-    int32_t *qpos;
-    float *pgq;
-    int nsplit;
-};
-static KVsAllWorkspace carve_k_vs_all(const kge_handle *h, int64_t B, Carve &c)
-{
-    KVsAllWorkspace w;
-    w.nsplit = one_vs_all_splits(B, h->cfg.n_ent);
-    const size_t rows = (size_t)B * h->L.ld * sizeof(float);
-    w.qs = c.take<float>(rows, 16);
-    w.qo = c.take<float>(rows, 16);
-    w.qpos = c.take<int32_t>((size_t)B * sizeof(int32_t), 16);
-    w.pgq = c.take<float>((size_t)w.nsplit * rows, 16);
-    return w;
 }
 
 extern "C" int64_t kge_k_vs_all_workspace_bytes(const kge_handle *h, int64_t B)
 {
-    if (!h || B < 0) return 0;
-    Carve c(nullptr);
-    carve_k_vs_all(h, B, c);
-    return (int64_t)c.at;
+    return candidate_workspace_bytes(h, K_VS_ALL, B);
 }
 
 extern "C" int kge_k_vs_all_step(kge_handle *h, int32_t side, int32_t loss_reduction, float label_smoothing,
@@ -1785,66 +1749,25 @@ extern "C" int kge_k_vs_all_step(kge_handle *h, int32_t side, int32_t loss_reduc
                                  int64_t ws_bytes, void *stream)
 {
     KGE_CHECK_HANDLE(h, "kge_k_vs_all_step");
-    const int model = h->cfg.scoring;
-    if (model != KGE_DISTMULT && model != KGE_COMPLEX && model != KGE_HOLE)
-        return fail(KGE_ERR_UNSUPPORTED, "kge_k_vs_all_step: KvsAll training is implemented for DistMult, ComplEx and HolE "
-                                         "(inner-product scores); not for scoring type %d", model);
-    if (side != KGE_ONE_VS_ALL_S && side != KGE_ONE_VS_ALL_O)
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_k_vs_all_step: side must be KGE_ONE_VS_ALL_S or KGE_ONE_VS_ALL_O, got %d",
-                    side);
-    if (loss_reduction != KGE_REDUCE_SUM && loss_reduction != KGE_REDUCE_MEAN)
-        return fail(KGE_ERR_INVALID_ARGUMENT, "Invalid value for reduction!");
-    if (!(label_smoothing >= 0.f && label_smoothing < 1.f))
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_k_vs_all_step: label_smoothing must be in [0, 1), got %g",
-                    (double)label_smoothing);
-    if (int rc = check_no_pending(h, "kge_k_vs_all_step")) return rc;
-    if (h->cfg.n_ent < 2) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_k_vs_all_step: needs n_ent >= 2");
-    if ((long long)k_vs_all_smem_bytes(h->L.ld) > h->max_smem)
-        return fail(KGE_ERR_UNSUPPORTED, "kge_k_vs_all_step: rows of %d floats exceed the shared-memory tiles of the KvsAll "
-                                         "kernels (%d B)", h->L.ld, h->max_smem);
-    if (B < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_k_vs_all_step: B < 0");
-    if (B == 0) return KGE_OK;
-    if (!ent_dev || !rel_dev || !grad_ent_dev || !grad_rel_dev || !queries_dev || !label_offsets_dev || !label_ids_dev)
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_k_vs_all_step: null table, gradient, queries or labels");
-    if (int rc = check_workspace(ws_dev, ws_bytes, kge_k_vs_all_workspace_bytes(h, B), 16, "kge_k_vs_all_step",
-                                 "kge_k_vs_all_workspace_bytes"))
+    OneVsAllSide s = candidate_side(h, K_VS_ALL, ent_dev, rel_dev, grad_ent_dev, grad_rel_dev, queries_dev,
+                                    B, step, loss_dev);
+    if (int rc = check_candidate_step(h, K_VS_ALL, s, loss_reduction, [&]() -> int {
+            if (side != KGE_ONE_VS_ALL_S && side != KGE_ONE_VS_ALL_O)
+                return fail(KGE_ERR_INVALID_ARGUMENT, "kge_k_vs_all_step: side must be KGE_ONE_VS_ALL_S or "
+                                                      "KGE_ONE_VS_ALL_O, got %d", side);
+            if (!(label_smoothing >= 0.f && label_smoothing < 1.f))
+                return fail(KGE_ERR_INVALID_ARGUMENT, "kge_k_vs_all_step: label_smoothing must be in [0, 1), got %g",
+                            (double)label_smoothing);
+            return KGE_OK;
+        }, !label_offsets_dev || !label_ids_dev, ws_dev, ws_bytes))
         return rc;
+    if (B == 0) return KGE_OK;
     cudaStream_t st = (cudaStream_t)stream;
-    Carve c(ws_dev);
-    const KVsAllWorkspace w = carve_k_vs_all(h, B, c);
-    ShardView sv;
-    memset(&sv, 0, sizeof(sv));
-    KGE_CUDA(launch_rank_prepare(h->L, sv, ent_dev, rel_dev, nullptr, queries_dev, B, h->score_scale, w.qs, w.qo, nullptr,
-                                 w.qpos, st),
-             "kge_k_vs_all_step (query vectors)");
-    const int stamp = kge_step_stamp(step);
-    // the same looked-up rows as a 1vsAll step: every entity row, and the relation rows of the batch (chain pass)
-    if (h->stamp_ent) KGE_CUDA(launch_one_vs_all_stamps(h->stamp_ent, h->cfg.n_ent, stamp, st), "kge_k_vs_all_step (stamps)");
-    OneVsAllSide s;
-    memset(&s, 0, sizeof(s));
-    s.ent = ent_dev;
-    s.rel = rel_dev;
-    s.grad_ent = grad_ent_dev;
-    s.grad_rel = grad_rel_dev;
-    s.triples = queries_dev;
-    s.B = B;
-    s.cand = ent_dev;
-    s.grad_cand = grad_ent_dev;
-    s.n_cand = h->cfg.n_ent;
-    s.weight = 1.f;
-    s.xsplit = 1;
+    CandidateQueries q;
+    if (int rc = start_candidate_step(h, K_VS_ALL, loss_reduction, ws_dev, st, s, &q)) return rc;
     s.side = side == KGE_ONE_VS_ALL_S ? KGE_SIDE_S : KGE_SIDE_O;
     s.col = side == KGE_ONE_VS_ALL_S ? 0 : 2;
-    s.q = side == KGE_ONE_VS_ALL_S ? w.qs : w.qo;
-    s.kp = h->L.kp;
-    s.ld = h->L.ld;
-    s.nsplit = w.nsplit;
-    s.scale = h->score_scale;
-    s.w = loss_reduction == KGE_REDUCE_MEAN ? (float)(1.0 / (double)h->cfg.n_ent) : 1.f;
-    s.loss = loss_dev;
-    s.stamp = stamp;
-    s.stamp_rel = h->stamp_ent ? h->stamp_rel : nullptr;
-    s.pgq = w.pgq;
+    s.q = side == KGE_ONE_VS_ALL_S ? q.qs : q.qo;
     s.label_off = (const long long *)label_offsets_dev;
     s.label_ids = label_ids_dev;
     s.y0 = (float)((double)label_smoothing / (double)h->cfg.n_ent);

@@ -431,28 +431,35 @@ class KGEEngine:
         # apply_gradients' launch)
         self.launches += 2 if self.scoring_type == "RotatE" else (4 if defer else 5) if bucketed else 1
 
+    def _step_call(self, name, fn, need, triples, step, head, tail, pending_ok=False):
+        """What the step entry points beside kge_train_step share: check the int32 [B, 3] triples (or queries), refuse
+        while a deferred step is pending (unless pending_ok), call fn(h, *head, ent, rel, g_ent, g_rel, triples, B,
+        *tail, workspace, need, stream) with the cached scratch of _workspace (the library wants 16-byte alignment;
+        every call runs on the engine's stream, so one buffer serves them all in stream order) and keep `step` as the
+        lazy optimizer's row stamp."""
+        assert triples.dtype == torch.int32 and triples.is_cuda and triples.is_contiguous()
+        if self._deferred and not pending_ok:
+            raise ValueError("%s: the replaced-row sum of a deferred step is pending (apply_gradients first)" % name)
+        ws, need = self._workspace(int(need))
+        _lib.check(fn(self.h, *head, _ptr(self.ent), _ptr(self.rel), _ptr(self.g_ent), _ptr(self.g_rel), _ptr(triples),
+                      triples.shape[0], *tail, _ptr(ws), need, self._stream()))
+        self._last_step = int(step)
+
     @_traced("kge.one_vs_all_step")
     def one_vs_all_backward(self, triples, sides="s,o", step=0):
         """1vsAll step up to tape.gradient (kge_one_vs_all_step, DESIGN.md 3.12): the multiclass NLL of every positive
         against every entity on each side in `sides` ('s,o', 'o' or 's'), with the engine's reduction; accumulates into
         g_ent / g_rel and loss_acc[0] like forward_backward.  step: the lazy optimizer's row stamp (every entity row and
         the batch's relation rows count as looked up).  apply_gradients() takes its non-deferred path next."""
-        assert triples.dtype == torch.int32 and triples.is_cuda and triples.is_contiguous()
         if sides not in _lib.ONE_VS_ALL_SIDES:
             raise ValueError("one_vs_all must be one of %s, got %r" % (", ".join(map(repr, _lib.ONE_VS_ALL_SIDES)), sides))
-        if self._deferred:
-            raise ValueError("one_vs_all_backward: the replaced-row sum of a deferred step is pending (apply_gradients first)")
         B = triples.shape[0]
-        need = int(self.lib.kge_one_vs_all_workspace_bytes(self.h, B))
-        if getattr(self, "_ova_ws", None) is None or self._ova_ws.numel() < need:
-            self._ova_ws = torch.empty(max(need, 16), dtype=torch.uint8, device=self.device)  # 256-byte aligned (torch)
-        _lib.check(self.lib.kge_one_vs_all_step(
-            self.h, _lib.ONE_VS_ALL_SIDES[sides], _lib.REDUCTIONS[self.reduction], _ptr(self.ent), _ptr(self.rel),
-            _ptr(self.g_ent), _ptr(self.g_rel), _ptr(triples), B, int(step), _ptr(self.loss_acc), _ptr(self._ova_ws), need,
-            self._stream()))
-        self._last_step = int(step)
+        self._step_call("one_vs_all_backward", self.lib.kge_one_vs_all_step,
+                        self.lib.kge_one_vs_all_workspace_bytes(self.h, B), triples, step,
+                        (_lib.ONE_VS_ALL_SIDES[sides], _lib.REDUCTIONS[self.reduction]), (int(step), _ptr(self.loss_acc)))
         # query vectors (two kernels), entity stamps, five passes per side
-        self.launches += 2 + (1 if self.lazy else 0) + 5 * (2 if sides == "s,o" else 1)
+        if B:
+            self.launches += 2 + (1 if self.lazy else 0) + 5 * (2 if sides == "s,o" else 1)
 
     @_traced("kge.one_vs_all_relation_step")
     def one_vs_all_relation_backward(self, triples, weight, step=0):
@@ -460,21 +467,12 @@ class KGEEngine:
         3.14): weight * the multiclass NLL of every positive's relation against every relation, scored as f(s, r, o),
         with the engine's reduction; accumulates into g_ent / g_rel and loss_acc[0] like one_vs_all_backward.  step:
         the lazy optimizer's row stamp (every relation row and the batch's s and o rows count as looked up)."""
-        assert triples.dtype == torch.int32 and triples.is_cuda and triples.is_contiguous()
-        if self._deferred:
-            raise ValueError("one_vs_all_relation_backward: the replaced-row sum of a deferred step is pending "
-                             "(apply_gradients first)")
         B = triples.shape[0]
-        need = int(self.lib.kge_one_vs_all_relation_workspace_bytes(self.h, B))
-        if getattr(self, "_ovr_ws", None) is None or self._ovr_ws.numel() < need:
-            self._ovr_ws = torch.empty(max(need, 16), dtype=torch.uint8, device=self.device)  # 256-byte aligned (torch)
-        _lib.check(self.lib.kge_one_vs_all_relation_step(
-            self.h, float(weight), _lib.REDUCTIONS[self.reduction], _ptr(self.ent), _ptr(self.rel), _ptr(self.g_ent),
-            _ptr(self.g_rel), _ptr(triples), B, int(step), _ptr(self.loss_acc), _ptr(self._ovr_ws), need,
-            self._stream()))
-        self._last_step = int(step)
+        self._step_call("one_vs_all_relation_backward", self.lib.kge_one_vs_all_relation_step,
+                        self.lib.kge_one_vs_all_relation_workspace_bytes(self.h, B), triples, step,
+                        (float(weight), _lib.REDUCTIONS[self.reduction]), (int(step), _ptr(self.loss_acc)))
         # relation stamps, relation queries, five passes, the dX split sum when dX is split
-        if B > 0:
+        if B:
             self.launches += (1 if self.lazy else 0) + 6 + (1 if one_vs_all_splits(self.n_rel, B) > 1 else 0)
 
     @_traced("kge.k_vs_all_step")
@@ -486,23 +484,16 @@ class KGEEngine:
         [B + 1], absolute into the int32 id array; ascending and distinct per query): a batch is a slice of the
         queries and of the offsets over the same id array.  step: the lazy optimizer's row stamp (every entity row and
         the batch's relation rows count as looked up).  apply_gradients() takes its non-deferred path next."""
-        assert queries.dtype == torch.int32 and queries.is_cuda and queries.is_contiguous()
         assert label_offsets.dtype == torch.int64 and label_offsets.is_cuda and label_offsets.is_contiguous()
         assert label_ids.dtype == torch.int32 and label_ids.is_cuda and label_ids.is_contiguous()
         if side not in ("s", "o"):
             raise ValueError("k_vs_all_backward: side must be 's' or 'o', got %r" % (side,))
-        if self._deferred:
-            raise ValueError("k_vs_all_backward: the replaced-row sum of a deferred step is pending (apply_gradients first)")
         B = queries.shape[0]
         assert label_offsets.numel() == B + 1
-        need = int(self.lib.kge_k_vs_all_workspace_bytes(self.h, B))
-        if getattr(self, "_kva_ws", None) is None or self._kva_ws.numel() < need:
-            self._kva_ws = torch.empty(max(need, 16), dtype=torch.uint8, device=self.device)  # 256-byte aligned (torch)
-        _lib.check(self.lib.kge_k_vs_all_step(
-            self.h, _lib.ONE_VS_ALL_SIDES[side], _lib.REDUCTIONS[self.reduction], float(label_smoothing), _ptr(self.ent),
-            _ptr(self.rel), _ptr(self.g_ent), _ptr(self.g_rel), _ptr(queries), B, _ptr(label_offsets), _ptr(label_ids),
-            int(step), _ptr(self.loss_acc), _ptr(self._kva_ws), need, self._stream()))
-        self._last_step = int(step)
+        self._step_call("k_vs_all_backward", self.lib.kge_k_vs_all_step, self.lib.kge_k_vs_all_workspace_bytes(self.h, B),
+                        queries, step,
+                        (_lib.ONE_VS_ALL_SIDES[side], _lib.REDUCTIONS[self.reduction], float(label_smoothing)),
+                        (_ptr(label_offsets), _ptr(label_ids), int(step), _ptr(self.loss_acc)))
         # query vectors (two kernels), entity stamps, dQ, dX and chain
         if B:
             self.launches += 2 + (1 if self.lazy else 0) + 3
@@ -520,19 +511,13 @@ class KGEEngine:
         optimizer.  Call it once per step, after the data term(s) and before apply_gradients().  Allowed while a
         deferred step is pending: the deferred optimizer reads every gradient row.  step: the lazy optimizer's row
         stamp."""
-        assert triples.dtype == torch.int32 and triples.is_cuda and triples.is_contiguous()
         lam_e, lam_r = self.n3_lambdas["ent"], self.n3_lambdas["rel"]
         if lam_e == 0.0 and lam_r == 0.0:
             raise ValueError("n3_backward: no table of this engine has the N3 regulariser")
         if self.ent_rows != self.n_ent:
-            raise NotImplementedError("the N3 regulariser needs the whole entity table: row-sharded tables are not supported")
-        need = self.n3_workspace_bytes
-        if getattr(self, "_n3_ws", None) is None or self._n3_ws.numel() < need:
-            self._n3_ws = torch.empty(need, dtype=torch.uint8, device=self.device)  # 256-byte aligned (torch)
-        _lib.check(self.lib.kge_n3_step(
-            self.h, lam_e, lam_r, _ptr(self.ent), _ptr(self.rel), _ptr(self.g_ent), _ptr(self.g_rel), _ptr(triples),
-            triples.shape[0], int(step), C.c_void_p(self.loss_acc.data_ptr() + 8), _ptr(self._n3_ws), need, self._stream()))
-        self._last_step = int(step)
+            raise NotImplementedError("the N3 regularizer needs the whole entity table: row-sharded tables are not supported")
+        self._step_call("n3_backward", self.lib.kge_n3_step, self.n3_workspace_bytes, triples, step, (lam_e, lam_r),
+                        (int(step), C.c_void_p(self.loss_acc.data_ptr() + 8)), pending_ok=True)
         if triples.shape[0]:
             self.launches += 2  # count and apply (and a memset)
 
@@ -646,7 +631,7 @@ class KGEEngine:
         return self._workspace(int(self.lib.kge_rank_workspace_bytes(self.h, int(b), int(n_cand))))
 
     def _workspace(self, need):
-        """The cached 1024-byte aligned scratch of rank_workspace, at least `need` bytes; top-k shares it."""
+        """The cached 1024-byte aligned scratch of rank_workspace, at least `need` bytes; top-k and _step_call share it."""
         if self._rank_ws is None or self._rank_ws.numel() < need:
             raw = torch.empty(max(need, 1024) + 1024, dtype=torch.uint8, device=self.device)
             off = (-raw.data_ptr()) % 1024  # the library wants a 1024-byte aligned base (operand tiles of the tensor-core pass)

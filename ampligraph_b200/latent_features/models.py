@@ -398,19 +398,24 @@ class ScoringBasedEmbeddingModel:
         if any(v > 0.0 for v in self.engine.n3_lambdas.values()):
             self.engine.n3_backward(batch, step=self._step)
 
+    def _check_all_candidates(self, training, loss, focusE):
+        """The refusals fit's all-candidate training types share: `training` ('1vsAll' or 'KvsAll') needs a trilinear
+        model, the compiled loss `loss`, no focusE and one GPU."""
+        if self.scoring_type not in ("DistMult", "ComplEx", "HolE"):
+            raise NotImplementedError("%s training is implemented for DistMult, ComplEx and HolE (inner-product "
+                                      "scores), not for %s" % (training, self.scoring_type))
+        if isinstance(self.compiled_loss, loss_functions.LossFunctionWrapper) or self.compiled_loss.name != loss:
+            raise ValueError("%s training needs the loss %r, got %r" % (training, loss, self.compiled_loss.name))
+        if focusE:
+            raise NotImplementedError("%s training does not support focusE" % training)
+        if self._world() > 1:
+            raise NotImplementedError("%s training is single-GPU only" % training)
+
     def _check_one_vs_all(self, one_vs_all, focusE):
         """The refusals of fit(one_vs_all=...), before anything is indexed or trained."""
         if not isinstance(one_vs_all, str) or one_vs_all not in _lib.ONE_VS_ALL_SIDES:
             raise ValueError("one_vs_all must be None, 's,o', 'o' or 's', got %r" % (one_vs_all,))
-        if self.scoring_type not in ("DistMult", "ComplEx", "HolE"):
-            raise NotImplementedError("1vsAll training is implemented for DistMult, ComplEx and HolE (inner-product "
-                                      "scores), not for %s" % self.scoring_type)
-        if isinstance(self.compiled_loss, loss_functions.LossFunctionWrapper) or self.compiled_loss.name != "multiclass_nll":
-            raise ValueError("1vsAll training needs the loss 'multiclass_nll', got %r" % (self.compiled_loss.name,))
-        if focusE:
-            raise NotImplementedError("1vsAll training does not support focusE")
-        if self._world() > 1:
-            raise NotImplementedError("1vsAll training is single-GPU only")
+        self._check_all_candidates("1vsAll", "multiclass_nll", focusE)
 
     def _check_k_vs_all(self, k_vs_all, label_smoothing, one_vs_all, focusE):
         """The refusals of fit(k_vs_all=..., label_smoothing=...), before anything is indexed or trained."""
@@ -419,20 +424,12 @@ class ScoringBasedEmbeddingModel:
                 raise ValueError("k_vs_all must be None, 's,o', 'o' or 's', got %r" % (k_vs_all,))
             if one_vs_all is not None:
                 raise ValueError("k_vs_all and one_vs_all are two training types: give one of them")
-            if self.scoring_type not in ("DistMult", "ComplEx", "HolE"):
-                raise NotImplementedError("KvsAll training is implemented for DistMult, ComplEx and HolE (inner-product "
-                                          "scores), not for %s" % self.scoring_type)
-            if isinstance(self.compiled_loss, loss_functions.LossFunctionWrapper) or self.compiled_loss.name != "nll":
-                raise ValueError("KvsAll training needs the loss 'nll', got %r" % (self.compiled_loss.name,))
         if (isinstance(label_smoothing, bool) or not isinstance(label_smoothing, numbers.Real)
                 or not math.isfinite(label_smoothing) or not 0.0 <= label_smoothing < 1.0):
             raise ValueError("label_smoothing must be a number in [0, 1), got %r" % (label_smoothing,))
         if k_vs_all is None:
             raise ValueError("label_smoothing applies to KvsAll training only (k_vs_all=...)")
-        if focusE:
-            raise NotImplementedError("KvsAll training does not support focusE")
-        if self._world() > 1:
-            raise NotImplementedError("KvsAll training is single-GPU only")
+        self._check_all_candidates("KvsAll", "nll", focusE)
 
     @staticmethod
     def _check_relation_prediction(weight, one_vs_all, k_vs_all):

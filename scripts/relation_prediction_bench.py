@@ -11,9 +11,10 @@ step's share of the entity step, its fp32 rate counted from the shapes (5 contra
 torch baseline's time, and a torch.profiler per-kernel breakdown of the relation step (a run of its own).
 
 With --parent-lib (a library built from the parent commit by scripts/build_variant.sh), the entity step is also timed
-in worker processes that alternate the parent library and this tree's (KGE_B200_LIB), and each worker's 1vsAll ("s,o")
-and KvsAll (both sides) outputs on batches whose positives share no subject, object or relation -- so every
-red.global.add target gets one add per kernel and the gradient tables are deterministic -- are compared bit for bit.
+in worker processes that alternate the parent library and this tree's (KGE_B200_LIB), and each worker's 1vsAll ("s,o"),
+relation-step and KvsAll (both sides) outputs on batches whose positives share no subject, object or relation -- so
+every red.global.add target gets one add per kernel and the gradient tables are deterministic -- are compared bit for
+bit: the gradient tables and losses under both reductions, and the row stamps of the looked-up-rows optimizer rule.
 Prints the GPU and its power limit first: every number depends on both.
 
     python scripts/relation_prediction_bench.py [--iters N] [--parent-lib PATH] [--out FILE.json]
@@ -67,9 +68,9 @@ def tables(n_ent, n_rel, seed=0):
             rng)
 
 
-def engine(ent, rel, loss="multiclass_nll"):
+def engine(ent, rel):
     from ampligraph_b200.engine import KGEEngine
-    eng = KGEEngine("ComplEx", K_USER, 1, ent.shape[0], rel.shape[0], loss=loss, optimizer="sgd")
+    eng = KGEEngine("ComplEx", K_USER, 1, ent.shape[0], rel.shape[0], loss="multiclass_nll", optimizer="sgd")
     eng.set_embeddings(ent, rel)
     return eng
 
@@ -169,35 +170,38 @@ def worker(out_dir, iters):
         times[B] = events(lambda: eng.one_vs_all_backward(t, "s,o"), iters)
     eng.close()
     outs = {}
+
+    def save(key, eng):
+        torch.cuda.synchronize()
+        outs[key + "_g_ent"], outs[key + "_g_rel"] = eng.g_ent.cpu().numpy(), eng.g_rel.cpu().numpy()
+        outs[key + "_loss"] = eng.loss_acc.cpu().numpy()
+        if eng.lazy:
+            outs[key + "_stamps_ent"], outs[key + "_stamps_rel"] = (eng.stamps[tb].cpu().numpy() for tb in ("ent", "rel"))
+
+    from ampligraph_b200.engine import KGEEngine
     for n_rel, B in ((R, R), (4096, 4096)):  # FB15k-237's relations, and a wide relation table for B = 4,096
         ent, rel, rng = tables(E, n_rel, seed=n_rel)
         X = distinct_batch(E, n_rel, B, rng)
-        for red in ("sum", "mean"):
-            from ampligraph_b200.engine import KGEEngine
-            eng = KGEEngine("ComplEx", K_USER, 1, E, n_rel, loss="multiclass_nll", loss_params={"reduction": red},
-                            optimizer="sgd")
-            eng.set_embeddings(ent, rel)
-            eng.one_vs_all_backward(torch.as_tensor(X).cuda(), "s,o")
-            torch.cuda.synchronize()
-            key = "ova_%d_%s" % (B, red)
-            outs[key + "_g_ent"], outs[key + "_g_rel"] = eng.g_ent.cpu().numpy(), eng.g_rel.cpu().numpy()
-            outs[key + "_loss"] = eng.loss_acc.cpu().numpy()
-            eng.close()
         # KvsAll: each positive is one query of each side, with a second label: (s, p, o + 1) and (s + 1, p, o)
         X2 = np.concatenate([X, X.copy(), X.copy()])
         X2[B:2 * B, 2] = (X[:, 2] + 1) % E
         X2[2 * B:, 0] = (X[:, 0] + 1) % E
         findex = FilterIndex(X2, E)
-        eng = engine(ent, rel, loss="nll")
-        for side in ("o", "s"):
-            q, off, ids = k_vs_all_queries(findex, X, side)
-            eng.k_vs_all_backward(torch.as_tensor(q).cuda(), side, torch.as_tensor(off).cuda(), torch.as_tensor(ids).cuda(),
-                                  0.1)
-            torch.cuda.synchronize()
-            key = "kva_%d_%s" % (B, side)
-            outs[key + "_g_ent"], outs[key + "_g_rel"] = eng.g_ent.cpu().numpy(), eng.g_rel.cpu().numpy()
-            outs[key + "_loss"] = eng.loss_acc.cpu().numpy()
-        eng.close()
+        kva = {side: [torch.as_tensor(a).cuda() for a in k_vs_all_queries(findex, X, side)] for side in ("o", "s")}
+        t = torch.as_tensor(X).cuda()
+        steps = {"ova": ("multiclass_nll", lambda eng: eng.one_vs_all_backward(t, "s,o", step=5)),
+                 "ovr": ("multiclass_nll", lambda eng: eng.one_vs_all_relation_backward(t, 1.0, step=5)),
+                 "kva": ("nll", lambda eng: [eng.k_vs_all_backward(q, side, off, ids, 0.1, step=5)
+                                             for side, (q, off, ids) in kva.items()])}
+        # every step under both reductions with SGD, and under sum with Adam's looked-up-rows rule on both tables
+        for name, (loss, fn) in steps.items():
+            for red, lazy in (("sum", None), ("mean", None), ("sum", (True, True))):
+                eng = KGEEngine("ComplEx", K_USER, 1, E, n_rel, loss=loss, loss_params={"reduction": red},
+                                optimizer="adam" if lazy else "sgd", lazy_tables=lazy)
+                eng.set_embeddings(ent, rel)
+                fn(eng)
+                save("%s_%d_%s%s" % (name, B, red, "_lazy" if lazy else ""), eng)
+                eng.close()
     np.savez(os.path.join(out_dir, "outputs.npz"), **outs)
     print(json.dumps({str(b): ms for b, ms in times.items()}), flush=True)
 
@@ -229,7 +233,8 @@ def ab(parent_lib, iters, rounds=2):
         print("    B=%-5d parent %s  new %s" % (B, ["%.3f" % x[B] for x in times["parent"]],
                                                  ["%.3f" % x[B] for x in times["new"]]), flush=True)
     bits = all(v for k, v in cmp.items() if not k.endswith("_loss"))
-    print("1vsAll / KvsAll gradient tables bit-identical to the parent build: %s; largest loss rel diff %.1e"
+    print("1vsAll / relation / KvsAll gradient tables and stamps bit-identical to the parent build: %s; largest loss rel "
+          "diff %.1e"
           % (bits, max(v for k, v in cmp.items() if k.endswith("_loss"))), flush=True)
     for k, v in cmp.items():
         if not k.endswith("_loss") and not v:

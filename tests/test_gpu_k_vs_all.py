@@ -1,7 +1,8 @@
 """KvsAll training on the GPU (kge_k_vs_all_step, DESIGN.md 3.13) against the float64 oracle of
 tests/k_vs_all_oracle.py: loss and both gradient tables for DistMult, ComplEx and HolE on both sides, both reductions,
 with and without label smoothing; label sets on and across the 32-entity tile edges, up to every entity; clipping;
-the looked-up-rows stamps and optimizer steps; the FB15k-237 shape; the C-ABI's refusals and the facade.
+the looked-up-rows stamps and optimizer steps; the FB15k-237 shape; the facade (the C-ABI's refusals:
+tests/test_gpu_all_candidates_abi.py).
 
 Tolerance: per element, exact_oracle.OvaBound, as for 1vsAll (tests/test_gpu_one_vs_all.py): each (query, entity)
 pair is charged the rounding of the fp32 chains it passes through, its logit's error carried through the sigmoid, a
@@ -18,7 +19,7 @@ import exact_oracle as xo
 import k_vs_all_oracle
 import optim_oracle
 from ampligraph_b200 import _lib
-from ampligraph_b200.engine import KGEEngine, k_vs_all_workspace_bytes
+from ampligraph_b200.engine import KGEEngine
 from oracle import ref_step
 
 pytestmark = pytest.mark.gpu
@@ -194,50 +195,6 @@ def test_fb15k237_shape_against_device_oracle():
     ent, rel = _tables(model, E, R, k, rng, scale=0.1)
     labels = [sorted(set(rng.integers(0, E, int(rng.integers(1, 61))).tolist())) for _ in range(B)]
     _check(model, k, ent, rel, _queries("o", labels, E, R, rng), labels, "o", "sum", 0.1, device="cuda", matmul=True)
-
-
-def test_c_abi_refusals_and_workspace():
-    lib = _lib.load()
-    rng = np.random.default_rng(4)
-    labels = _labels(100, 50, rng)
-    q = _dev(_queries("o", labels, 100, 3, rng))
-    off, ids = (_dev(a) for a in _csr(labels))
-    for model in ("TransE", "RotatE"):
-        eng = KGEEngine(model, 4, 1, 100, 3, loss="nll")
-        with pytest.raises(NotImplementedError, match="DistMult, ComplEx and HolE"):
-            eng.k_vs_all_backward(q, "o", off, ids)
-        eng.close()
-    eng = KGEEngine("DistMult", 6, 1, 100, 3, loss="nll")
-    for B in (0, 1, 50, 1000, 5000):
-        assert lib.kge_k_vs_all_workspace_bytes(eng.h, B) == k_vs_all_workspace_bytes(B, 100, eng.ld)
-    ws = torch.empty(k_vs_all_workspace_bytes(50, 100, eng.ld), dtype=torch.uint8, device="cuda")
-    ptr = lambda x: C.c_void_p(x.data_ptr()) if x is not None else C.c_void_p(0)
-
-    def call(side=2, reduction=0, eps=0.0, B=50, off_=off, ids_=ids, ws_=ws, nbytes=None):
-        return lib.kge_k_vs_all_step(eng.h, side, reduction, eps, ptr(eng.ent), ptr(eng.rel), ptr(eng.g_ent),
-                                     ptr(eng.g_rel), ptr(q), B, ptr(off_), ptr(ids_), 0, ptr(eng.loss_acc), ptr(ws_),
-                                     ws_.numel() if nbytes is None else nbytes, eng._stream())
-    for kw in ({"side": 0}, {"side": 3}, {"side": 4}, {"reduction": 2}, {"eps": -0.1}, {"eps": 1.0}, {"eps": float("nan")},
-               {"B": -1}, {"off_": None}, {"ids_": None}, {"nbytes": ws.numel() - 16},
-               {"ws_": ws[4:], "nbytes": ws.numel() - 16}):  # the last: not 16-byte aligned
-        assert call(**kw) == _lib.KGE_ERR_INVALID_ARGUMENT, kw
-    with pytest.raises(ValueError, match="side"):
-        eng.k_vs_all_backward(q, "s,o", off, ids)
-    assert call(B=0, off_=None, ids_=None) == _lib.KGE_OK  # an empty batch is a no-op
-    assert float(eng.loss_acc[0]) == 0.0
-    assert call() == _lib.KGE_OK and call(side=1, reduction=1, eps=0.5) == _lib.KGE_OK
-    eng.close()
-    # a pending deferred step (the bucketed fused step) is refused
-    eng = KGEEngine("ComplEx", 8, 4, 100, 3, loss="nll")
-    tt = _dev(np.stack([rng.integers(0, 100, 64), rng.integers(0, 3, 64), rng.integers(0, 100, 64)], 1).astype(np.int32))
-    eng.forward_backward(tt, None, defer=True)
-    if eng._deferred:
-        eng._deferred = False  # past the engine's own check, into the library's
-        with pytest.raises(ValueError, match="deferred"):
-            eng.k_vs_all_backward(q, "o", off, ids)
-        eng._deferred = True
-    eng.apply_gradients()
-    eng.close()
 
 
 def test_fit_k_vs_all_against_oracle():

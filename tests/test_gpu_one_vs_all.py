@@ -1,7 +1,7 @@
 """1vsAll training on the GPU (kge_one_vs_all_step, DESIGN.md 3.12) against the float64 oracle of
 tests/one_vs_all_oracle.py: loss and both gradient tables for DistMult, ComplEx and HolE on every side and reduction,
 clipping, a million-entity overflow case, optimizer steps with the dense and the looked-up-rows rule, the FB15k-237
-shape, the C-ABI's refusals and the facade.
+shape and the facade (the C-ABI's refusals: tests/test_gpu_all_candidates_abi.py).
 
 Tolerance: per element, exact_oracle.OvaBound.  A gradient element is a sum over (query, entity) pairs of
 g_be d l_be / d theta; the bound charges each pair the rounding of the fp32 chains it passes through (taken from the
@@ -19,7 +19,7 @@ import exact_oracle as xo
 import one_vs_all_oracle
 import optim_oracle
 from ampligraph_b200 import _lib
-from ampligraph_b200.engine import KGEEngine, one_vs_all_workspace_bytes
+from ampligraph_b200.engine import KGEEngine
 from oracle import ref_step
 
 pytestmark = pytest.mark.gpu
@@ -152,47 +152,6 @@ def test_fb15k237_shape_against_device_oracle():
     model, E, R, k, B = "ComplEx", 14541, 237, 200, 1000
     ent, rel = _tables(model, E, R, k, rng, scale=0.1)
     _check(model, k, ent, rel, _triples(E, R, B, rng), "s,o", "sum", device="cuda", matmul=True)
-
-
-def test_c_abi_refusals_and_workspace():
-    lib = _lib.load()
-    rng = np.random.default_rng(4)
-    for model in ("TransE", "RotatE"):
-        eng = KGEEngine(model, 4, 1, 10, 2, loss="multiclass_nll")
-        with pytest.raises(NotImplementedError, match="DistMult, ComplEx and HolE"):
-            eng.one_vs_all_backward(_dev(_triples(10, 2, 8, rng)), "s,o")
-        eng.close()
-    eng = KGEEngine("DistMult", 6, 1, 100, 3, loss="multiclass_nll")
-    t = _dev(_triples(100, 3, 50, rng))
-    for B in (0, 1, 50, 1000, 5000):
-        assert lib.kge_one_vs_all_workspace_bytes(eng.h, B) == one_vs_all_workspace_bytes(B, 100, eng.ld)
-    ws = torch.empty(one_vs_all_workspace_bytes(50, 100, eng.ld), dtype=torch.uint8, device="cuda")
-    ptr = lambda x: C.c_void_p(x.data_ptr())
-
-    def call(sides=3, reduction=0, ws_=ws, nbytes=None):
-        return lib.kge_one_vs_all_step(eng.h, sides, reduction, ptr(eng.ent), ptr(eng.rel), ptr(eng.g_ent), ptr(eng.g_rel),
-                                       ptr(t), 50, 0, ptr(eng.loss_acc), ptr(ws_), ws_.numel() if nbytes is None else nbytes,
-                                       eng._stream())
-    assert call(sides=0) == _lib.KGE_ERR_INVALID_ARGUMENT
-    assert call(sides=4) == _lib.KGE_ERR_INVALID_ARGUMENT
-    assert call(reduction=2) == _lib.KGE_ERR_INVALID_ARGUMENT
-    assert call(nbytes=ws.numel() - 16) == _lib.KGE_ERR_INVALID_ARGUMENT
-    assert call(ws_=ws[4:], nbytes=ws.numel() - 16) == _lib.KGE_ERR_INVALID_ARGUMENT  # not 16-byte aligned
-    with pytest.raises(ValueError, match="one_vs_all"):
-        eng.one_vs_all_backward(t, "p")
-    assert call() == _lib.KGE_OK
-    eng.close()
-    # a pending deferred step (the bucketed fused step) is refused
-    eng = KGEEngine("ComplEx", 8, 4, 64, 3, loss="multiclass_nll")
-    tt = _dev(_triples(64, 3, 64, rng))
-    eng.forward_backward(tt, None, defer=True)
-    if eng._deferred:
-        eng._deferred = False  # past the engine's own check, into the library's
-        with pytest.raises(ValueError, match="deferred"):
-            eng.one_vs_all_backward(tt, "s,o")
-        eng._deferred = True
-    eng.apply_gradients()
-    eng.close()
 
 
 def test_fit_one_vs_all():

@@ -2,7 +2,8 @@
 against the float64 oracle of tests/relation_prediction_oracle.py: loss and both gradient tables for DistMult, ComplEx
 and HolE under both reductions, relation counts below one tile, off the tile grid and at FB15k-237's 237 (split dX),
 clipping, the term added to both entity sides, the weight's scaling, repeatability, the looked-up-rows optimizer rule,
-the FB15k-237 shape, the C-ABI's refusals and fit(relation_prediction_weight=...).
+the FB15k-237 shape and fit(relation_prediction_weight=...) (the C-ABI's refusals:
+tests/test_gpu_all_candidates_abi.py).
 
 Tolerance: per element, exact_oracle.OvaBound, as for the entity sides (tests/test_gpu_one_vs_all.py), with the
 relation side's dX split over the query tiles (xsplit) in its chains and lambda in its weights."""
@@ -16,7 +17,7 @@ import exact_oracle as xo
 import optim_oracle
 import relation_prediction_oracle
 from ampligraph_b200 import _lib
-from ampligraph_b200.engine import KGEEngine, one_vs_all_relation_workspace_bytes, one_vs_all_splits
+from ampligraph_b200.engine import KGEEngine, one_vs_all_splits
 
 pytestmark = pytest.mark.gpu
 
@@ -196,56 +197,6 @@ def test_fb15k237_shape_against_device_oracle():
     model, E, R, k, B = "ComplEx", 14541, 237, 200, 1000
     ent, rel = _tables(model, E, R, k, rng, scale=0.3)
     _check(model, k, ent, rel, _triples(E, R, B, rng), "sum", device="cuda", matmul=True)
-
-
-def test_c_abi_refusals_and_workspace():
-    lib = _lib.load()
-    rng = np.random.default_rng(4)
-    for model in ("TransE", "RotatE"):
-        eng = KGEEngine(model, 4, 1, 10, 3, loss="multiclass_nll")
-        with pytest.raises(NotImplementedError, match="DistMult, ComplEx and HolE"):
-            eng.one_vs_all_relation_backward(_dev(_triples(10, 3, 12, rng)), 1.0)
-        eng.close()
-    eng = KGEEngine("ComplEx", 8, 1, 10, 1, loss="multiclass_nll")  # one relation: nothing to predict
-    with pytest.raises(ValueError, match="n_rel"):
-        eng.one_vs_all_relation_backward(_dev(_triples(10, 1, 12, rng)), 1.0)
-    eng.close()
-    eng = KGEEngine("DistMult", 6, 1, 100, 40, loss="multiclass_nll")
-    t = _dev(_triples(100, 40, 50, rng))
-    for B in (0, 1, 50, 1000, 5000):
-        assert lib.kge_one_vs_all_relation_workspace_bytes(eng.h, B) == one_vs_all_relation_workspace_bytes(B, 40, eng.ld)
-    ws = torch.empty(one_vs_all_relation_workspace_bytes(50, 40, eng.ld), dtype=torch.uint8, device="cuda")
-    ptr = lambda x: C.c_void_p(x.data_ptr())
-
-    def call(weight=1.0, reduction=0, ws_=ws, nbytes=None, B=50, ent=eng.ent):
-        return lib.kge_one_vs_all_relation_step(eng.h, weight, reduction, ptr(ent) if ent is not None else None,
-                                                ptr(eng.rel), ptr(eng.g_ent), ptr(eng.g_rel), ptr(t), B, 0,
-                                                ptr(eng.loss_acc), ptr(ws_), ws_.numel() if nbytes is None else nbytes,
-                                                eng._stream())
-    assert call(reduction=2) == _lib.KGE_ERR_INVALID_ARGUMENT
-    for w in (0.0, -1.0, float("nan"), float("inf")):
-        assert call(weight=w) == _lib.KGE_ERR_INVALID_ARGUMENT, w
-    assert call(B=-1) == _lib.KGE_ERR_INVALID_ARGUMENT
-    assert call(ent=None) == _lib.KGE_ERR_INVALID_ARGUMENT
-    assert call(nbytes=ws.numel() - 16) == _lib.KGE_ERR_INVALID_ARGUMENT
-    assert call(ws_=ws[4:], nbytes=ws.numel() - 16) == _lib.KGE_ERR_INVALID_ARGUMENT  # not 16-byte aligned
-    before = eng.g_rel.clone()
-    assert call(B=0, ws_=ws[:16], nbytes=0) == _lib.KGE_OK  # a no-op
-    torch.cuda.synchronize()
-    assert torch.equal(eng.g_rel, before)
-    assert call() == _lib.KGE_OK
-    eng.close()
-    # a pending deferred step (the bucketed fused step) is refused
-    eng = KGEEngine("ComplEx", 8, 4, 64, 3, loss="multiclass_nll")
-    tt = _dev(_triples(64, 3, 64, rng))
-    eng.forward_backward(tt, None, defer=True)
-    if eng._deferred:
-        eng._deferred = False  # past the engine's own check, into the library's
-        with pytest.raises(ValueError, match="deferred"):
-            eng.one_vs_all_relation_backward(tt, 1.0)
-        eng._deferred = True
-    eng.apply_gradients()
-    eng.close()
 
 
 def test_fit_relation_prediction():

@@ -128,6 +128,7 @@ PROTOTYPES = {
     "kge_n3_workspace_bytes": (C.c_int64, [_P]),
     "kge_n3_step": (C.c_int, [_P, C.c_float, C.c_float, _P, _P, _P, _P, _P, C.c_int64, C.c_uint64, _P, _P, C.c_int64,
                               _P]),
+    "kge_dura_step": (C.c_int, [_P, C.c_float, C.c_float, _P, _P, _P, _P, _P, C.c_int64, C.c_uint64, _P, _P]),
 }
 ONE_VS_ALL_SIDES = {"s": 1, "o": 2, "s,o": 3}  # kge_one_vs_all_side flags of fit(one_vs_all=...)
 

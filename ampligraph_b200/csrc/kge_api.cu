@@ -1833,3 +1833,46 @@ extern "C" int kge_n3_step(kge_handle *h, float lambda_ent, float lambda_rel, co
     KGE_CUDA(launch_n3(p, h->L.halves, h->sm_count, (cudaStream_t)stream), "kge_n3_step");
     return KGE_OK;
 }
+
+// ---- the DURA regulariser of a step's positives (kge_reg_dura.cu) -------------------------------------------------
+
+// Allowed while a KGE_STEP_FUSED_DEFER step is pending, like kge_n3_step: it only adds into gradient rows, which the
+// pending step's owner kernel (kge_optimizer_step_deferred) reads for every row of the [ent | rel] block afterwards, and it
+// takes no workspace.
+extern "C" int kge_dura_step(kge_handle *h, float weight_norm, float weight_prod, const float *ent_dev, const float *rel_dev,
+                             float *grad_ent_dev, float *grad_rel_dev, const int32_t *triples_dev, int64_t B, uint64_t step,
+                             double *loss_dev, void *stream)
+{
+    KGE_CHECK_HANDLE(h, "kge_dura_step");
+    if (h->cfg.scoring == KGE_TRANSE || h->cfg.scoring == KGE_ROTATE)
+        return fail(KGE_ERR_UNSUPPORTED, "kge_dura_step: DURA is defined for the tensor-factorisation scores (DistMult, "
+                                         "ComplEx, HolE); not for TransE or RotatE");
+    if (!(weight_norm >= 0.f && weight_norm <= FLT_MAX) || !(weight_prod >= 0.f && weight_prod <= FLT_MAX) ||
+        (weight_norm == 0.f && weight_prod == 0.f))
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_dura_step: weight_norm and weight_prod must be finite and >= 0, and not "
+                                              "both 0; got %g and %g", (double)weight_norm, (double)weight_prod);
+    if (B < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_dura_step: B < 0");
+    if (B == 0) return KGE_OK;
+    if (!triples_dev || !ent_dev || !grad_ent_dev || (weight_prod > 0.f && (!rel_dev || !grad_rel_dev)))
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_dura_step: null table, gradient or triples");
+    DuraParams p;
+    memset(&p, 0, sizeof(p));
+    p.ent = ent_dev;
+    p.rel = rel_dev;
+    p.grad_ent = grad_ent_dev;
+    p.grad_rel = grad_rel_dev;
+    p.triples = triples_dev;
+    p.B = B;
+    p.kp = h->L.kp;
+    p.ld = h->L.ld;
+    p.w_norm = weight_norm;
+    p.w_prod = weight_prod;
+    p.w_prod2 = 2.f * weight_prod;
+    p.loss = loss_dev;
+    // stamped only while the entity buffer is set, as by every other step entry point
+    p.stamp = kge_step_stamp(step);
+    p.stamp_ent = h->stamp_ent;
+    p.stamp_rel = h->stamp_ent ? h->stamp_rel : nullptr;
+    KGE_CUDA(launch_dura(p, h->L.halves, (cudaStream_t)stream), "kge_dura_step");
+    return KGE_OK;
+}

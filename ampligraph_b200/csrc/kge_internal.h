@@ -148,6 +148,22 @@ struct N3Params {
 // memset of p.cnt, the count pass and the apply pass, on st
 cudaError_t launch_n3(const N3Params &p, int halves, int sm_count, cudaStream_t st);
 
+// kge_reg_dura.cu: the DURA regulariser of a step's positives (kge_dura_step)
+struct DuraParams {
+    const float *ent, *rel;         // [n_ent, ld], [n_rel, ld] (rel: nullptr allowed when w_prod is 0)
+    float *grad_ent, *grad_rel;
+    const int32_t *triples;         // [B, 3]
+    long long B;
+    int kp, ld;
+    float w_norm, w_prod;           // lambda * alpha, lambda * beta
+    float w_prod2;                  // 2 * w_prod (exact)
+    double *loss;                   // += L_DURA, or nullptr
+    int stamp;
+    int *stamp_ent, *stamp_rel;     // lazy-optimizer stamps of the positives' rows, or nullptr
+};
+// one thread per (positive, float4 chunk of a half), gradients by RED, on st
+cudaError_t launch_dura(const DuraParams &p, int halves, cudaStream_t st);
+
 // kge_misc.cu
 cudaError_t launch_score_triples(const Layout &L, int nit, const float *ent, const float *rel_or_rot,
                                  const int32_t *triples, long long n, float scale, float *out, int sm_count,

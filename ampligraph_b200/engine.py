@@ -210,8 +210,9 @@ class KGEEngine:
                  optimizer="adam", optimizer_params=None, regularizer=None, device=0, neg_group=0,
                  table_alloc=None, ent_rows=None, max_rel_size=None, rank_mode=None, rank_pair_cap=0, lazy_tables=None):
         """regularizer: None | {"p":, "lambda": [, "p2":, "lambda2":]} | {"kind": "N3", "lambda":} | a pair
-        [entities, relations] of those (EmbeddingLookupLayer.py:131-155).  An LP term goes to the optimizer; N3 is
-        n3_backward's.  lazy_tables: see set_optimizer.  max_rel_size: RotatE phase normalisation when it differs from the
+        [entities, relations] of those (EmbeddingLookupLayer.py:131-155), or {"kind": "DURA", "lambda":, "alpha":,
+        "beta":} given for both tables.  An LP term goes to the optimizer; N3 is n3_backward's and DURA
+        dura_backward's.  lazy_tables: see set_optimizer.  max_rel_size: RotatE phase normalisation when it differs from the
         relation-table rows (RotatE.py:96).  rank_mode: 'auto' (tensor-core filter + exact refine for the bilinear
         models) | 'exact' (FP32 canonical chain for every pair); env KGE_B200_RANK_MODE overrides the default."""
         self.lib = _lib.load()
@@ -303,6 +304,14 @@ class KGEEngine:
         n3 = [float(r["lambda"]) if (r or {}).get("kind") == "N3" else 0.0 for r in regs]
         self.n3_lambdas = {"ent": n3[0], "rel": n3[1]}
         regs = [None if (r or {}).get("kind") == "N3" else r for r in regs]
+        # DURA (DESIGN.md 3.16) couples the tables, so it comes as the same config for both; its weights (w_n, w_p) =
+        # (lambda alpha, lambda beta), formed in double, are dura_backward's
+        dura = [r for r in regs if (r or {}).get("kind") == "DURA"]
+        if dura and not (len(dura) == 2 and dura[0] == dura[1]):
+            raise ValueError("the DURA regularizer couples the entity and relation tables: give it for both")
+        self.dura_weights = None if not dura else (float(dura[0]["lambda"]) * float(dura[0]["alpha"]),
+                                                   float(dura[0]["lambda"]) * float(dura[0]["beta"]))
+        regs = [None if (r or {}).get("kind") == "DURA" else r for r in regs]
 
         def cfg_for(reg):
             reg = dict(reg or {})
@@ -436,13 +445,15 @@ class KGEEngine:
         while a deferred step is pending (unless pending_ok), call fn(h, *head, ent, rel, g_ent, g_rel, triples, B,
         *tail, workspace, need, stream) with the cached scratch of _workspace (the library wants 16-byte alignment;
         every call runs on the engine's stream, so one buffer serves them all in stream order) and keep `step` as the
-        lazy optimizer's row stamp."""
+        lazy optimizer's row stamp.  need=None: the entry point takes no workspace, fn(..., *tail, stream)."""
         assert triples.dtype == torch.int32 and triples.is_cuda and triples.is_contiguous()
         if self._deferred and not pending_ok:
             raise ValueError("%s: the replaced-row sum of a deferred step is pending (apply_gradients first)" % name)
-        ws, need = self._workspace(int(need))
+        if need is not None:
+            ws, need = self._workspace(int(need))
+            tail = tuple(tail) + (_ptr(ws), need)
         _lib.check(fn(self.h, *head, _ptr(self.ent), _ptr(self.rel), _ptr(self.g_ent), _ptr(self.g_rel), _ptr(triples),
-                      triples.shape[0], *tail, _ptr(ws), need, self._stream()))
+                      triples.shape[0], *tail, self._stream()))
         self._last_step = int(step)
 
     @_traced("kge.one_vs_all_step")
@@ -520,6 +531,24 @@ class KGEEngine:
                         (int(step), C.c_void_p(self.loss_acc.data_ptr() + 8)), pending_ok=True)
         if triples.shape[0]:
             self.launches += 2  # count and apply (and a memset)
+
+    @_traced("kge.dura_step")
+    def dura_backward(self, triples, step=0):
+        """The DURA regulariser of a step's positives up to tape.gradient (kge_dura_step, DESIGN.md 3.16): w_n (|h|^2 +
+        |t|^2) + w_p (|h o r|^2 + |t o conj(r)|^2) of each positive, weights from the engine's regulariser config
+        (dura_weights); adds into g_ent / g_rel and loss_acc[1], like the LP term of the optimizer.  Call it once per
+        step, after the data term(s) and before apply_gradients().  Allowed while a deferred step is pending: the
+        deferred optimizer reads every gradient row.  step: the lazy optimizer's row stamp."""
+        if self.dura_weights is None:
+            raise ValueError("dura_backward: this engine has no DURA regulariser")
+        if self.ent_rows != self.n_ent:
+            raise NotImplementedError("the DURA regularizer needs the whole entity table: row-sharded tables are not "
+                                      "supported")
+        w_n, w_p = self.dura_weights
+        self._step_call("dura_backward", self.lib.kge_dura_step, None, triples, step, (w_n, w_p),
+                        (int(step), C.c_void_p(self.loss_acc.data_ptr() + 8)), pending_ok=True)
+        if triples.shape[0]:
+            self.launches += 1
 
     def _one_block(self):
         """True when tables, gradients and slots still ARE the [ent | rel] blocks allocated here (callers may rebind them: the

@@ -116,7 +116,12 @@ class ScoringBasedEmbeddingModel:
         'N3' | regularizers.N3Regularizer (extension; DESIGN.md 3.15): lambda * sum_d |z_d|^3 of the rows each step's
         positives use, once per occurrence (|z_d| the complex modulus for ComplEx, HolE and RotatE), default lambda
         1e-3, e.g. ['N3', None] for the entities only.  It is not defined for RotatE's relation phases, and not with
-        k_vs_all training or on several GPUs."""
+        k_vs_all training or on several GPUs.
+        'DURA' | regularizers.DURARegularizer (extension; DESIGN.md 3.16): lambda * (alpha (|h|^2 + |t|^2) + beta
+        (|h o r|^2 + |t o conj(r)|^2)) of each step's positives, once per occurrence (|.| the complex modulus for ComplEx
+        and HolE), defaults lambda 1e-3, alpha = beta = 1.  It couples each positive's entity and relation rows, so it is
+        only valid as the single regularizer of both tables, not in a list.  It needs DistMult, ComplEx or HolE, and is
+        not supported with k_vs_all training or on several GPUs."""
         self.optimizer = optimizers.get(optimizer)
         self.compiled_loss = loss_functions.get(loss)
         init = entity_relation_initializer
@@ -130,6 +135,12 @@ class ScoringBasedEmbeddingModel:
             assert isinstance(r, initializers.Initializer) and r.name == "glorot_uniform", \
                 "The relation initializer provided to a RotatE model must be glorot_uniform!"
         self._regularizer = regularizers.get_pair(entity_relation_regularizer)
+        if isinstance(entity_relation_regularizer, (list, tuple)) and self._uses_dura():
+            raise ValueError("the DURA regularizer couples each positive's entity and relation rows, so it cannot be "
+                             "given per table: pass it as the single entity_relation_regularizer, not in a list")
+        if self.scoring_type in ("TransE", "RotatE") and self._uses_dura():
+            raise NotImplementedError("the DURA regularizer is defined for the tensor-factorisation models (DistMult, "
+                                      "ComplEx, HolE), not for %s" % self.scoring_type)
         if self.scoring_type == "RotatE" and isinstance(self._regularizer[1], regularizers.N3Regularizer):
             raise NotImplementedError("the N3 regularizer is not defined for RotatE's relation table (its rows are "
                                       "phases, not embeddings): use ['N3', None]")
@@ -151,9 +162,10 @@ class ScoringBasedEmbeddingModel:
         if self.scoring_type == "RotatE":
             self.scoring_layer.max_rel_size = self.max_rel_size  # :338
         # the reference's per-table rule: which tables its optimizer updates on the looked-up rows only
-        # N3's gradient lives on the looked-up rows only, like the data term's: it does not make a table's gradient dense
+        # a per-occurrence regulariser's (N3, DURA) gradient lives on the looked-up rows only, like the data term's: it
+        # does not make a table's gradient dense
         lazy = optimizers.table_rules(self.optimizer.name, self.optimizer.hyperparams,
-                                      [r is not None and not regularizers.is_n3(r) for r in reg])
+                                      [r is not None and not regularizers.is_per_occurrence(r) for r in reg])
 
         def make_engine(alloc=None):
             return KGEEngine(self.scoring_type, self.k, self.eta, self.max_ent_size, self.max_rel_size,
@@ -250,12 +262,12 @@ class ScoringBasedEmbeddingModel:
         reduction.  The logged loss includes the term.  It needs one_vs_all, at least two relations, and cannot be
         combined with k_vs_all.  0.0 (the default) leaves training unchanged.
 
-        With the N3 regulariser (compile(entity_relation_regularizer='N3')), every step adds lambda * L_N3 of its batch
-        (once per step, also with one_vs_all and relation_prediction_weight; DESIGN.md 3.15) and the logged loss
-        includes it.  It cannot be combined with k_vs_all, whose steps have queries rather than triples, and is
-        single-GPU only."""
+        With the N3 or DURA regulariser (compile(entity_relation_regularizer='N3' or 'DURA')), every step adds its
+        term of the batch's positives (once per step, also with one_vs_all and relation_prediction_weight; DESIGN.md
+        3.15, 3.16) and the logged loss includes it.  Neither can be combined with k_vs_all, whose steps have queries
+        rather than triples, and both are single-GPU only."""
         self._assert_compile_was_called()
-        self._check_n3(k_vs_all)
+        self._check_per_occurrence(k_vs_all)
         if k_vs_all is not None or label_smoothing != 0.0:
             self._check_k_vs_all(k_vs_all, label_smoothing, one_vs_all, focusE)
         if one_vs_all is not None:
@@ -333,7 +345,7 @@ class ScoringBasedEmbeddingModel:
                     eng.one_vs_all_backward(batch, one_vs_all, step=self._step)
                     if relation_prediction_weight > 0:
                         eng.one_vs_all_relation_backward(batch, relation_prediction_weight, step=self._step)
-                    self._n3_backward(batch)
+                    self._per_occurrence_backward(batch)
                     eng.apply_gradients()
                 elif self.use_focusE:
                     self._two_phase_step(batch, weights[start:start + batch_size])
@@ -345,7 +357,7 @@ class ScoringBasedEmbeddingModel:
                     self._user_loss_step(batch)
                 else:
                     eng.forward_backward(batch, None, seed=self.seed, step=self._step, defer=True)
-                    self._n3_backward(batch)
+                    self._per_occurrence_backward(batch)
                     eng.apply_gradients()
                 self._step += 1
                 self._loss_cnt += 1
@@ -383,20 +395,28 @@ class ScoringBasedEmbeddingModel:
     def _uses_n3(self):
         return any(isinstance(r, regularizers.N3Regularizer) for r in self._regularizer)
 
-    def _check_n3(self, k_vs_all=None):
-        """The refusals of a training call with the N3 regulariser, before anything is indexed or trained."""
-        if not self._uses_n3():
-            return
-        if k_vs_all is not None:
-            raise NotImplementedError("the N3 regularizer is not supported with k_vs_all: a KvsAll step has queries, "
-                                      "not triples")
-        if self._world() > 1:
-            raise NotImplementedError("the N3 regularizer is single-GPU only")
+    def _uses_dura(self):
+        return any(isinstance(r, regularizers.DURARegularizer) for r in self._regularizer)
 
-    def _n3_backward(self, batch):
-        """The N3 term of this step's positives (KGEEngine.n3_backward), where a table has it with lambda > 0."""
+    def _check_per_occurrence(self, k_vs_all=None):
+        """The refusals of a training call with a per-occurrence regulariser (N3, DURA), before anything is indexed or
+        trained."""
+        for name, used in (("N3", self._uses_n3()), ("DURA", self._uses_dura())):
+            if not used:
+                continue
+            if k_vs_all is not None:
+                raise NotImplementedError("the %s regularizer is not supported with k_vs_all: a KvsAll step has "
+                                          "queries, not triples" % name)
+            if self._world() > 1:
+                raise NotImplementedError("the %s regularizer is single-GPU only" % name)
+
+    def _per_occurrence_backward(self, batch):
+        """The per-occurrence regulariser terms of this step's positives: N3 (KGEEngine.n3_backward) where a table has
+        it with lambda > 0, and DURA (KGEEngine.dura_backward)."""
         if any(v > 0.0 for v in self.engine.n3_lambdas.values()):
             self.engine.n3_backward(batch, step=self._step)
+        if self.engine.dura_weights is not None:
+            self.engine.dura_backward(batch, step=self._step)
 
     def _check_all_candidates(self, training, loss, focusE):
         """The refusals fit's all-candidate training types share: `training` ('1vsAll' or 'KvsAll') needs a trilinear
@@ -457,7 +477,7 @@ class ScoringBasedEmbeddingModel:
         host batch -- H2D copy of the batch, fused step, D2H read of the batch loss, which is returned.
         x: [B,3] raw triples (numpy) or an int32 torch tensor of already indexed ids (pinned for speed)."""
         self._assert_compile_was_called()
-        self._check_n3()
+        self._check_per_occurrence()
         if torch.is_tensor(x):
             host = x
         else:
@@ -474,7 +494,7 @@ class ScoringBasedEmbeddingModel:
             self._user_loss_step(batch)
         else:
             self.engine.forward_backward(batch, None, seed=self.seed, step=self._step, defer=True)
-            self._n3_backward(batch)
+            self._per_occurrence_backward(batch)
             self.engine.apply_gradients()
         self._step += 1
         if self._world() > 1:
@@ -492,7 +512,7 @@ class ScoringBasedEmbeddingModel:
         blocks: batch i+1 travels on a copy stream through a persistent pinned ring while step i runs, and the 16-byte
         loss record of step i is copied asynchronously and read one step later.  Returns the list of per-batch losses."""
         self._assert_compile_was_called()
-        self._check_n3()
+        self._check_per_occurrence()
         it = iter(batches)
         first = next(it, None)
         if first is None:
@@ -559,7 +579,7 @@ class ScoringBasedEmbeddingModel:
                 self._user_loss_step(batch)
             else:
                 eng.forward_backward(batch, None, seed=self.seed, step=self._step, defer=True)
-                self._n3_backward(batch)
+                self._per_occurrence_backward(batch)
                 eng.apply_gradients()
             P["free"][s].record(main)
             P["loss_pin"][s].copy_(eng.loss_acc, non_blocking=True)  # D2H of this step's (cumulative) loss record
@@ -615,7 +635,7 @@ class ScoringBasedEmbeddingModel:
         loss.backward()
         eng.forward_backward(batch, (repl, keep), seed=self.seed, step=self._step, mode=_lib.STEP_BACKWARD_EXT,
                              dpos=spg.grad.contiguous(), dneg=sng.grad.contiguous())  # step: the lazy rule's row stamp
-        self._n3_backward(batch)
+        self._per_occurrence_backward(batch)
         eng.apply_gradients()
         eng.loss_acc[0] += loss.detach().double()
 

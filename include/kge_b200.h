@@ -362,6 +362,30 @@ int kge_n3_step(kge_handle *h, float lambda_ent, float lambda_rel, const float *
                 float *grad_ent_dev, float *grad_rel_dev, const int32_t *triples_dev, int64_t B, uint64_t step,
                 double *loss_dev, void *ws_dev, int64_t ws_bytes, void *stream);
 
+/* The DURA regulariser (Zhang, Cai and Wang, NeurIPS 2020) of a step's B positives (h_b, r_b, t_b):
+ * L_DURA = sum_b sum_d [ weight_norm (m_h + m_t) + weight_prod m_r (m_h + m_t) ], m_x = |x_d|^2, duplicates counted every
+ * time they occur.  |x_d| is |x[d]| for DistMult and the modulus sqrt(x[d]^2 + x[kp + d]^2) for ComplEx and HolE.  With
+ * weight_norm = lambda alpha and weight_prod = lambda beta it is the paper's lambda (alpha (|h|^2 + |t|^2) + beta
+ * (|h o r|^2 + |t o conj(r)|^2)); with weight_prod = 0 it is the per-occurrence squared L2 of the entity rows.  The
+ * gradient, component-wise on each half: 2 (weight_norm + weight_prod m_r) h_d, the same with t_d, and
+ * 2 weight_prod (m_h + m_t) r_d.  Only the rows the positives use get a gradient, so a DURA model keeps the looked-up-rows
+ * optimizer rule.  With weight_prod = 0 the relation table is not read or written and may be passed as NULL (table and
+ * gradient).  B = 0 is a no-op.
+ *   grad_*_dev  ADDED to with red.global.add: the same fp32 sum in any order, but the order is the REDs' arrival order,
+ *               so it is bit-for-bit repeatable only where every partial sum is exact (as for kge_train_step's kept
+ *               rows); call it after the step's data term(s) and before the optimizer
+ *   step        the lazy-optimizer stamp: the positives' entity rows, and their relation rows when weight_prod > 0, are
+ *               stamped with kge_step_stamp(step) (while an entity stamp buffer is set, as for kge_train_step)
+ *   loss_dev    double accumulator += L_DURA (may be NULL)
+ * Refusals, in this order: KGE_ERR_UNSUPPORTED for TransE and RotatE; KGE_ERR_INVALID_ARGUMENT for a weight not finite
+ * or < 0, both weights 0, B < 0, then null table, gradient or triples pointers.  Like kge_n3_step it is accepted while a
+ * KGE_STEP_FUSED_DEFER step is pending: kge_optimizer_step_deferred reads every gradient row of the block, so the DURA
+ * rows added here are part of that update.  The tables are the ones the step trained on (the parameters before the
+ * update), whole: row-sharded tables are not supported.  DESIGN.md 3.16. */
+int kge_dura_step(kge_handle *h, float weight_norm, float weight_prod, const float *ent_dev, const float *rel_dev,
+                  float *grad_ent_dev, float *grad_rel_dev, const int32_t *triples_dev, int64_t B, uint64_t step,
+                  double *loss_dev, void *stream);
+
 /* OptimizerWrapper.minimize -> legacy apply_gradients (optimizers.py:136-168) for ONE
  * table (or any row-wise concatenation of tables of the same width and regulariser: the engine passes [ent | rel] as one
  * block, one launch per step), dense semantics, plus the LP regulariser's loss/gradient over the whole table

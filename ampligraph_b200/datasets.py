@@ -146,6 +146,24 @@ def k_vs_all_queries(findex, triples, side):
     return queries, off, ids
 
 
+def reciprocal_triples(triples, n_rel, sides="s", batch_size=None):
+    """The side-o rows of reciprocal relations (DESIGN.md 3.17), with n_rel forward relations and row p + n_rel the
+    inverse p^-1 of relation p: the forward triple (s, p, o) for side 'o', the inverse (o, p + n_rel, s) for side 's'.
+    A subject query of (s, p, o) is the object query of its inverse.  -> int32 [m n, 3], m the number of sides.  With
+    both sides, the rows of each batch of batch_size triples (all of them when None) are adjacent, its forward rows
+    first, so that batch i of the triples is rows[m i batch_size:m (i + 1) batch_size] with either number of sides."""
+    t = np.asarray(triples, dtype=np.int32).reshape(-1, 3)
+    inverse = np.ascontiguousarray(t[:, ::-1])
+    inverse[:, 1] += np.int32(n_rel)
+    if sides == "s":
+        return inverse
+    if sides == "o":
+        return np.ascontiguousarray(t)
+    batch = np.arange(len(t)) // (int(batch_size) if batch_size else max(len(t), 1))
+    order = np.argsort(np.concatenate([2 * batch, 2 * batch + 1]), kind="stable")
+    return np.ascontiguousarray(np.concatenate([t, inverse])[order])
+
+
 def k_vs_all_steps(n_o, n_s, batch_size):
     """The steps of one KvsAll epoch over n_o side-o and n_s side-s queries -> list of ((o_lo, o_hi), (s_lo, s_hi)).
     A single side (the other count 0) is cut into sequential slices of batch_size queries.  Both sides: S =

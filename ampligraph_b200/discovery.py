@@ -32,7 +32,7 @@ import logging
 import numpy as np
 import torch
 
-from .datasets import DataIndexer, FilterIndex, as_triple_array
+from .datasets import DataIndexer, FilterIndex, as_triple_array, reciprocal_triples
 from .engine import fp32_floor
 
 logger = logging.getLogger(__name__)
@@ -51,7 +51,10 @@ def _count(model, kind):
     di = model.data_indexer
     if isinstance(di, DataIndexer):
         return di.get_entities_count() if kind == "e" else di.get_relations_count()
-    return model.engine.n_ent if kind == "e" else model.engine.n_rel
+    if kind == "e":
+        return model.engine.n_ent
+    # with reciprocal relations the second half of the relation table holds the inverses, which are no candidates
+    return model.engine.n_rel // 2 if model.reciprocal_relations else model.engine.n_rel
 
 
 def _ids(model, values, kind):
@@ -150,8 +153,10 @@ def query_topn(model, top_n=10, head=None, relation=None, tail=None, ents_to_con
             if n_cand < top_n:
                 logger.warning("the model knows fewer than top_n entities, return set will be truncated.")
         side = "o" if tail is None else "s"
-        q = _dev(eng, [[h, r, t]], np.int32)
-        ids, val = eng.topk(q, side, int(top_n), cand_ids=cand, n_cand=n_cand)
+        q, qs = np.array([[h, r, t]], np.int32), side
+        if side == "s" and model.reciprocal_relations:  # (?, r, t) is the tail query (t, r^-1, ?)
+            q, qs = reciprocal_triples(q, model.max_rel_size, "s"), "o"
+        ids, val = eng.topk(_dev(eng, q, np.int32), qs, int(top_n), cand_ids=cand, n_cand=n_cand)
         ids, val = ids[0].cpu().numpy(), val[0].cpu().numpy()
         keep = ids >= 0
         ents = _labels(model, ids[keep], "e")
@@ -228,7 +233,10 @@ def query_topn_batch(model, X, side="o", top_n=10, use_filter=False, ents_to_con
         if findex is not None:
             o_np, i_np = findex.lookup(qb, side, position_of)
             off, idx = _dev(eng, o_np, np.int64), _dev(eng, i_np, np.int32)
-        ids, val = eng.topk(_dev(eng, qb, np.int32), side, int(top_n), off, idx, cand_ids=cand, n_cand=n_cand)
+        qs = side
+        if side == "s" and model.reciprocal_relations:  # (?, p, o) is the tail query (o, p^-1, ?), same filter list
+            qb, qs = reciprocal_triples(qb, model.max_rel_size, "s"), "o"
+        ids, val = eng.topk(_dev(eng, qb, np.int32), qs, int(top_n), off, idx, cand_ids=cand, n_cand=n_cand)
         labels[start:start + len(qb)] = _labels(model, ids.cpu().numpy(), kind)
         scores[start:start + len(qb)] = val.cpu().numpy()
     return labels, scores

@@ -277,7 +277,8 @@ def _as_int32(v):
 def _build_model(model_class, params, eta):
     from .latent_features import ScoringBasedEmbeddingModel
     from .latent_features import loss_functions, optimizers, regularizers
-    model = ScoringBasedEmbeddingModel(eta=eta, k=params.get("k", 100), scoring_type=model_class)
+    model = ScoringBasedEmbeddingModel(eta=eta, k=params.get("k", 100), scoring_type=model_class,
+                                       reciprocal_relations=params.get("reciprocal_relations", False))
     model.compile(optimizer=optimizers.get(params.get("optimizer", "adam"), params.get("optimizer_params", {})),
                   loss=loss_functions.get(params.get("loss", "multiclass_nll"), params.get("loss_params", {})),
                   entity_relation_regularizer=regularizers.get(params.get("regularizer"),
@@ -299,8 +300,10 @@ def select_best_model_ranking(model_class, X_train, X_valid, X_test, param_grid,
     hyper-parameters of a ScoringBasedEmbeddingModel of scoring type model_class (protocol.py:447-932).
 
     param_grid: keys batch_size, epochs, k, eta, loss, loss_params, regularizer, regularizer_params, optimizer,
-    optimizer_params, initializer, focusE_params; values are lists, scalars, dicts of those, or callables (random
-    search).  The caller's dict is not modified.
+    optimizer_params, initializer, focusE_params, reciprocal_relations (extension: the constructor's flag, default
+    False); values are lists, scalars, dicts of those, or callables (random search).  The caller's dict is not
+    modified.  Candidates train with sampled corruptions, so one with reciprocal_relations=True is recorded with the
+    model's refusal of that training.
 
     Each candidate is trained on X_train with early stopping on X_valid[::2] (EarlyStopping(monitor='val_<criteria>',
     mode='max', restore_best_weights=True); early_stopping_params: criteria 'mrr', burn_in 0, check_interval 10,

@@ -11,7 +11,8 @@ import numpy as np
 import torch
 
 from .. import _lib
-from ..datasets import DataIndexer, FilterIndex, as_triple_array, k_vs_all_queries, k_vs_all_steps
+from ..datasets import (DataIndexer, FilterIndex, as_triple_array, k_vs_all_queries, k_vs_all_steps,
+                        reciprocal_triples)
 from ..engine import KGEEngine
 from ..evaluation import hits_at_n_score, mr_score, mrr_score, train_test_split_no_unseen
 from . import initializers, loss_functions, optimizers, regularizers
@@ -77,11 +78,23 @@ class EarlyStopping:
 
 
 class ScoringBasedEmbeddingModel:
-    """Same constructor as the reference (ScoringBasedEmbeddingModel.py:100-171)."""
+    """Same constructor as the reference (ScoringBasedEmbeddingModel.py:100-171).
 
-    def __init__(self, eta, k, scoring_type="DistMult", seed=0, max_ent_size=None, max_rel_size=None):
+    reciprocal_relations (extension; DESIGN.md 3.17): True gives each of the max_rel_size (R) relations p a second,
+    independently learned row p^-1 (row p + R of the relation table, which has 2R rows).  Every training triple
+    (s, p, o) then also trains its inverse (o, p^-1, s), and a subject query (?, p, o) is answered as the object query
+    (o, p^-1, ?) (Lacroix et al., ICML 2018).  predict scores the forward triple f(s, p, o), and relation ranking and
+    top-n consider the forward relations only.  It needs DistMult, ComplEx or HolE trained with fit(one_vs_all=...) or
+    fit(k_vs_all=...) on one GPU, without the relation-prediction term: every other training path is refused."""
+
+    def __init__(self, eta, k, scoring_type="DistMult", seed=0, max_ent_size=None, max_rel_size=None,
+                 reciprocal_relations=False):
         if scoring_type not in SCORING_LAYER_REGISTRY:
             raise KeyError(scoring_type)  # the reference indexes the registry directly (:146)
+        if reciprocal_relations and scoring_type in ("TransE", "RotatE"):
+            raise NotImplementedError("reciprocal relations need 1vsAll or KvsAll training, which is implemented for "
+                                      "DistMult, ComplEx and HolE, not for %s" % scoring_type)
+        self.reciprocal_relations = bool(reciprocal_relations)
         self.eta, self.k, self.scoring_type, self.seed = int(eta), int(k), scoring_type, seed
         self.max_ent_size, self.max_rel_size = max_ent_size, max_rel_size
         self.scoring_layer = SCORING_LAYER_REGISTRY[scoring_type](k)
@@ -121,7 +134,10 @@ class ScoringBasedEmbeddingModel:
         (|h o r|^2 + |t o conj(r)|^2)) of each step's positives, once per occurrence (|.| the complex modulus for ComplEx
         and HolE), defaults lambda 1e-3, alpha = beta = 1.  It couples each positive's entity and relation rows, so it is
         only valid as the single regularizer of both tables, not in a list.  It needs DistMult, ComplEx or HolE, and is
-        not supported with k_vs_all training or on several GPUs."""
+        not supported with k_vs_all training or on several GPUs.
+        With reciprocal relations the relation initializer covers the 2R rows of the relation table, forward rows then
+        inverse rows: a callable is called with the shape (2R, internal_k), an ndarray must have that shape, and the
+        device-side Glorot draw's limit sqrt(6 / (fan_in + fan_out)) counts the 2R rows."""
         self.optimizer = optimizers.get(optimizer)
         self.compiled_loss = loss_functions.get(loss)
         init = entity_relation_initializer
@@ -167,8 +183,10 @@ class ScoringBasedEmbeddingModel:
         lazy = optimizers.table_rules(self.optimizer.name, self.optimizer.hyperparams,
                                       [r is not None and not regularizers.is_per_occurrence(r) for r in reg])
 
+        rel_rows = self._rel_rows()
+
         def make_engine(alloc=None):
-            return KGEEngine(self.scoring_type, self.k, self.eta, self.max_ent_size, self.max_rel_size,
+            return KGEEngine(self.scoring_type, self.k, self.eta, self.max_ent_size, rel_rows,
                              loss=name or "pairwise", loss_params=lp, optimizer=self.optimizer.name,
                              optimizer_params=self.optimizer.hyperparams, regularizer=reg, device=self.device,
                              table_alloc=alloc, lazy_tables=lazy)
@@ -179,7 +197,7 @@ class ScoringBasedEmbeddingModel:
         else:
             self.engine = make_engine()
         dense = [None, None]
-        for n, (init, rows, which) in enumerate(zip(self._initializer, (self.max_ent_size, self.max_rel_size), ("ent", "rel"))):
+        for n, (init, rows, which) in enumerate(zip(self._initializer, (self.max_ent_size, rel_rows), ("ent", "rel"))):
             if isinstance(init, initializers.Initializer):  # drawn on the device (Philox), no host table
                 seed = init.seed if getattr(init, "seed", None) is not None else self.seed
                 if init.name == "glorot_uniform":
@@ -191,8 +209,16 @@ class ScoringBasedEmbeddingModel:
                 dense[n] = np.asarray(init((rows, self.internal_k)), dtype=np.float32)
             else:
                 dense[n] = np.asarray(init, dtype=np.float32)
+                if which == "rel" and self.reciprocal_relations and dense[n].shape != (rows, self.internal_k):
+                    raise ValueError("with reciprocal relations the relation initializer needs shape %s (2R rows: the "
+                                     "%d forward relations, then their inverses), got shape %s"
+                                     % ((rows, self.internal_k), self.max_rel_size, dense[n].shape))
         self.engine.set_embeddings(dense[0], dense[1])
         self._step = 0
+
+    def _rel_rows(self):
+        """Rows of the relation table: R, or 2R with reciprocal relations (row p + R is the inverse of relation p)."""
+        return 2 * self.max_rel_size if self.reciprocal_relations else self.max_rel_size
 
     def _world(self):
         import torch.distributed as dist
@@ -212,7 +238,11 @@ class ScoringBasedEmbeddingModel:
     def _index(self, x, fit=False):
         x = as_triple_array(x)
         if self.data_indexer is False:  # use_indexer=False: data is already int ids
-            return np.ascontiguousarray(x[:, :3], dtype=np.int32)
+            t = np.ascontiguousarray(x[:, :3], dtype=np.int32)
+            if self.reciprocal_relations and self.max_rel_size is not None and (t[:, 1] >= self.max_rel_size).any():
+                raise ValueError("relation ids must be below max_rel_size = %d: with reciprocal relations the rows "
+                                 "from %d on are the inverse relations" % (self.max_rel_size, self.max_rel_size))
+            return t
         if fit and not isinstance(self.data_indexer, DataIndexer):
             self.data_indexer = DataIndexer(x[:, :3])
         return self.data_indexer.get_indexes(x[:, :3], "t", "raw2ind")
@@ -265,8 +295,16 @@ class ScoringBasedEmbeddingModel:
         With the N3 or DURA regulariser (compile(entity_relation_regularizer='N3' or 'DURA')), every step adds its
         term of the batch's positives (once per step, also with one_vs_all and relation_prediction_weight; DESIGN.md
         3.15, 3.16) and the logged loss includes it.  Neither can be combined with k_vs_all, whose steps have queries
-        rather than triples, and both are single-GPU only."""
+        rather than triples, and both are single-GPU only.
+
+        With reciprocal_relations (constructor; DESIGN.md 3.17) only one_vs_all and k_vs_all train.  one_vs_all: each
+        positive (s, p, o) gives the side-o row (s, p, o) for side 'o' and the side-o row (o, p^-1, s) for side 's', and
+        a step is one side-o 1vsAll call over the batch's forward rows, then its inverse rows; the logged loss sums
+        both, and N3 / DURA regularise every row the step trained.  k_vs_all: each side-s query (p, o) with labels {s}
+        becomes the side-o query (o, p^-1) with the same labels; the epoch's steps and label_smoothing are unchanged."""
         self._assert_compile_was_called()
+        if self.reciprocal_relations:
+            self._check_reciprocal("fit", one_vs_all, k_vs_all, focusE, relation_prediction_weight)
         self._check_per_occurrence(k_vs_all)
         if k_vs_all is not None or label_smoothing != 0.0:
             self._check_k_vs_all(k_vs_all, label_smoothing, one_vs_all, focusE)
@@ -307,6 +345,12 @@ class ScoringBasedEmbeddingModel:
         eng.set_hot_entities(triples=triples)  # the most frequent entities of the training set: their gradient rows are summed per warp
         data = self._to_dev(triples, np.int32)  # uploaded once; batches are device-side slices
         n = data.shape[0]
+        ova_rows, ova_sides = None, one_vs_all
+        if self.reciprocal_relations and one_vs_all is not None:
+            # each batch's forward and inverse rows, adjacent and uploaded once: a step is one side-o call over a slice
+            ova_rows = self._to_dev(reciprocal_triples(triples, self.max_rel_size, one_vs_all, batch_size), np.int32)
+            ova_sides = "o"
+        m = len(one_vs_all.split(",")) if ova_rows is not None else 1
         weights = None
         if self.use_focusE:
             if len(triples) != len(x):
@@ -330,8 +374,12 @@ class ScoringBasedEmbeddingModel:
         kva = kva_steps = None
         if k_vs_all is not None:  # each side's queries, label offsets and label ids, uploaded once; steps slice them
             findex = FilterIndex(triples, self.max_ent_size)
-            kva = {side: tuple(self._to_dev(a, a.dtype) for a in k_vs_all_queries(findex, triples, side))
-                   for side in k_vs_all.split(",")}
+            kva = {}
+            for side in k_vs_all.split(","):
+                q, off, ids = k_vs_all_queries(findex, triples, side)
+                if self.reciprocal_relations and side == "s":  # (p, o) with labels {s} -> the side-o query (o, p^-1)
+                    q = reciprocal_triples(q, self.max_rel_size, "s")
+                kva[side] = tuple(self._to_dev(a, a.dtype) for a in (q, off, ids))
             count = lambda side: kva[side][0].shape[0] if side in kva else 0
             kva_steps = k_vs_all_steps(count("o"), count("s"), batch_size)
         for epoch in range(initial_epoch, epochs):
@@ -342,7 +390,9 @@ class ScoringBasedEmbeddingModel:
                 if kva is not None:  # start: this step's query ranges of sides o and s
                     self._k_vs_all_step(kva, start, label_smoothing)
                 elif one_vs_all is not None:
-                    eng.one_vs_all_backward(batch, one_vs_all, step=self._step)
+                    if ova_rows is not None:
+                        batch = ova_rows[m * start:m * (start + batch_size)]
+                    eng.one_vs_all_backward(batch, ova_sides, step=self._step)
                     if relation_prediction_weight > 0:
                         eng.one_vs_all_relation_backward(batch, relation_prediction_weight, step=self._step)
                     self._per_occurrence_backward(batch)
@@ -418,6 +468,25 @@ class ScoringBasedEmbeddingModel:
         if self.engine.dura_weights is not None:
             self.engine.dura_backward(batch, step=self._step)
 
+    def _check_reciprocal(self, call, one_vs_all=None, k_vs_all=None, focusE=False, relation_prediction_weight=0.0):
+        """The refusals of a training call on a model with reciprocal relations, before anything is indexed or trained:
+        only fit(one_vs_all=...) and fit(k_vs_all=...) train the inverse rows."""
+        why = None
+        if one_vs_all is None and k_vs_all is None:
+            why = ("%s trains against sampled corruptions, whose fused kernels score both corruption sides of a positive "
+                   "with its one relation row: use fit(one_vs_all=...) or fit(k_vs_all=...)" % call)
+        elif focusE:
+            why = "focusE is a sampled-training option"
+        elif isinstance(self.compiled_loss, loss_functions.LossFunctionWrapper):
+            why = "a user loss is a sampled-training option"
+        elif (isinstance(relation_prediction_weight, numbers.Real) and not isinstance(relation_prediction_weight, bool)
+              and relation_prediction_weight > 0):
+            why = "the relation-prediction term is not defined for the inverse relations"
+        elif self.distributed:
+            why = "training is single-GPU only"
+        if why is not None:
+            raise NotImplementedError("reciprocal relations: %s" % why)
+
     def _check_all_candidates(self, training, loss, focusE):
         """The refusals fit's all-candidate training types share: `training` ('1vsAll' or 'KvsAll') needs a trilinear
         model, the compiled loss `loss`, no focusE and one GPU."""
@@ -469,7 +538,8 @@ class ScoringBasedEmbeddingModel:
         for side, (lo, hi) in zip(("o", "s"), ranges):
             if hi > lo:
                 q, off, ids = kva[side]
-                self.engine.k_vs_all_backward(q[lo:hi], side, off[lo:hi + 1], ids, label_smoothing, step=self._step)
+                self.engine.k_vs_all_backward(q[lo:hi], "o" if self.reciprocal_relations else side, off[lo:hi + 1],
+                                              ids, label_smoothing, step=self._step)
         self.engine.apply_gradients()
 
     def train_on_batch(self, x):
@@ -477,6 +547,8 @@ class ScoringBasedEmbeddingModel:
         host batch -- H2D copy of the batch, fused step, D2H read of the batch loss, which is returned.
         x: [B,3] raw triples (numpy) or an int32 torch tensor of already indexed ids (pinned for speed)."""
         self._assert_compile_was_called()
+        if self.reciprocal_relations:
+            self._check_reciprocal("train_on_batch")
         self._check_per_occurrence()
         if torch.is_tensor(x):
             host = x
@@ -512,6 +584,8 @@ class ScoringBasedEmbeddingModel:
         blocks: batch i+1 travels on a copy stream through a persistent pinned ring while step i runs, and the 16-byte
         loss record of step i is copied asynchronously and read one step later.  Returns the list of per-batch losses."""
         self._assert_compile_was_called()
+        if self.reciprocal_relations:
+            self._check_reciprocal("train_on_batches")
         self._check_per_occurrence()
         it = iter(batches)
         first = next(it, None)
@@ -664,6 +738,8 @@ class ScoringBasedEmbeddingModel:
         corrupt_side='p' (extension: relation prediction) ranks each triple's relation among all relations for its
         (s, o), by the same count, ranking_strategy and use_filter rules (a known (s, r, o) removes r); entities_subset
         does not apply to it.  `batch_size` only lower-bounds the device chunk: results do not depend on it.
+        With reciprocal relations, side s of (s, p, o) is ranked as side o of (o, p^-1, s) with the same filter and
+        candidates, and corrupt_side='p' ranks among the forward relations only.
         _filter_index: the FilterIndex that use_filter would build (_build_filter), when the caller keeps one across calls
         (fit's validations)."""
         assert corrupt_side in ["s", "o", "s,o", "s+o", "p"], "Invalid value for corrupt_side"
@@ -672,6 +748,8 @@ class ScoringBasedEmbeddingModel:
             raise ValueError("entities_subset does not apply to corrupt_side='p': the candidates are the relations")
         if not self.is_fitted:
             raise RuntimeError("Model has not been fitted.")
+        if self.reciprocal_relations and self._world() > 1:
+            raise NotImplementedError("reciprocal relations: evaluate is single-GPU only")
         eng = self.engine
         t = self._index(x)
         n = len(t)
@@ -695,7 +773,13 @@ class ScoringBasedEmbeddingModel:
                 if findex is not None:
                     o_np, i_np = findex.lookup(tb, side, position_of)
                     off, idx = self._to_dev(o_np, np.int64), self._to_dev(i_np, np.int32)
-                if self._world() > 1 and cand_ids is None and side != "p":
+                if self.reciprocal_relations and side != "o":
+                    # side s: the side-o rank of the inverse (o, p^-1, s), with the same filter list; side p: among the
+                    # forward relations only
+                    rd, rs, n_rel = (td, "p", self.max_rel_size) if side == "p" else \
+                        (self._to_dev(reciprocal_triples(tb, self.max_rel_size, "s"), np.int32), "o", None)
+                    r = eng.rank(rd, rs, ranking_strategy, off, idx, cand_ids=cand_ids, n_cand=n_rel)
+                elif self._world() > 1 and cand_ids is None and side != "p":
                     # row-sharded candidates: RAW counters summed over ranks, tie strategy applied once ('middle' is not
                     # additive over partitions, AbstractScoringLayer.py:232-244); the relation side runs on each rank
                     # locally (the relation table is replicated)
@@ -771,14 +855,21 @@ class ScoringBasedEmbeddingModel:
 
     # ------------------------------------------------------------------ embeddings / weights
     def get_embeddings(self, entities, embedding_type="e"):
-        """get_embeddings (:2214): rows of the dense [rows, internal_k] tables."""
+        """get_embeddings (:2214): rows of the dense [rows, internal_k] tables.  embedding_type 'e' (entities), 'r'
+        (relations; with reciprocal relations the forward rows) or 'r_inv' (extension: the inverse rows of the given
+        relations, on a model with reciprocal relations only)."""
         if not self.is_fitted:
             raise RuntimeError("Model has not been fitted.")
-        if embedding_type not in ("e", "r"):
+        if embedding_type not in ("e", "r", "r_inv"):
             raise ValueError("Invalid entity type: %s" % embedding_type)
+        if embedding_type == "r_inv" and not self.reciprocal_relations:
+            raise ValueError("embedding_type 'r_inv' needs a model with reciprocal relations")
         ent, rel = self.engine.get_embeddings()
-        idx = self.get_indexes(np.asarray(entities), embedding_type) if self.data_indexer is not False \
+        kind = "e" if embedding_type == "e" else "r"
+        idx = self.get_indexes(np.asarray(entities), kind) if self.data_indexer is not False \
             else np.asarray(entities, np.int64)
+        if embedding_type == "r_inv":
+            idx = np.asarray(idx, np.int64) + self.max_rel_size
         table = ent if embedding_type == "e" else rel
         return table[torch.as_tensor(idx, dtype=torch.long, device=table.device)].cpu().numpy()
 
@@ -798,7 +889,8 @@ class ScoringBasedEmbeddingModel:
         ent, rel = self.engine.get_embeddings()
         state = {"ent": ent.cpu().numpy(), "rel": rel.cpu().numpy(), "t": self.engine.t, "step": self._step,
                  "slots": {k: [None if s is None else s.cpu().numpy() for s in v] for k, v in self.engine.slots.items()},
-                 "indexer": self.data_indexer, "max_ent_size": self.max_ent_size, "max_rel_size": self.max_rel_size}
+                 "indexer": self.data_indexer, "max_ent_size": self.max_ent_size, "max_rel_size": self.max_rel_size,
+                 "reciprocal_relations": self.reciprocal_relations}
         with open(filepath, "wb") as f:
             pickle.dump(state, f)
 
@@ -806,6 +898,10 @@ class ScoringBasedEmbeddingModel:
         self._assert_compile_was_called()
         with open(filepath, "rb") as f:
             state = pickle.load(f)
+        saved = state.get("reciprocal_relations", False)  # files written before the flag existed have none
+        if saved != self.reciprocal_relations:
+            raise ValueError("the weights were saved by a model with reciprocal_relations=%s, this model has %s"
+                             % (saved, self.reciprocal_relations))
         self.data_indexer = state["indexer"]
         self.max_ent_size, self.max_rel_size = state["max_ent_size"], state["max_rel_size"]
         self._build_engine()

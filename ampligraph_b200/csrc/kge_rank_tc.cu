@@ -26,6 +26,11 @@
 //     |a - s_canonical| <= (2^-14 + 4 ld 2^-23) |q|_2 |e|_2  =: eps_rel |q| |e|.
 // tests/test_gpu_parity.py::test_tc_filter_error_bound measures the actual error (>= 10x smaller) and the bit-exact rank
 // tests run both modes.
+//
+// Non-finite operands.  A NaN or inf in a query or candidate row makes its norm, and so delta, NaN or inf (a tile's norm
+// is an atomicMax on the float bits, and NaN's bits are above every finite norm's); the filter takes an infinite delta
+// as NaN, so every pair of that query or tile is undecided and goes to the refine (or, past the list's capacity, to the gated exact kernel).  Ranks stay exact;
+// only the time such a broken table takes grows.  tests/test_gpu_rank_edges.py pins this.
 #include <cuda_bf16.h>
 #include <math.h>
 
@@ -108,12 +113,16 @@ __global__ void __launch_bounds__(256) kge_rank_split_kernel(const float *__rest
         } else if (!live) {
             thr[r] = make_float4(INFINITY, INFINITY, 0.f, 0.f);  // padding queries never count, never push
         } else {
-            const int n = qpos[r];
+            // in 64 bits: n + 1 must not wrap at INT_MAX.  quantise saturates, so nothing is greater than INT_MAX (U = +inf)
+            // and nothing is smaller than INT_MIN (L = -inf)
+            const long long n = qpos[r];
             const double edge_hi = (n + 1 >= 1) ? (double)(n + 1) : (double)n;  // T(n+1)
             const double edge_lo = (n >= 1) ? (double)n : (double)n - 1.0;      // T(n)
-            const float U = (float)(edge_hi / 1000.0 / (double)scale), L = (float)(edge_lo / 1000.0 / (double)scale);
-            // slack: rounding of U, L themselves, of fl(scale*acc) and of fl(score*1000), each <= 2^-24 relative (64x margin)
-            const float slack = fmaxf(fabsf(U), fabsf(L)) * 3.814697265625e-6f + 1e-37f;
+            const float U = n == INT_MAX ? INFINITY : (float)(edge_hi / 1000.0 / (double)scale);
+            const float L = n == INT_MIN ? -INFINITY : (float)(edge_lo / 1000.0 / (double)scale);
+            // slack: rounding of U, L themselves, of fl(scale*acc) and of fl(score*1000), each <= 2^-24 relative (64x margin);
+            // from the finite edges only (an infinite one is never near a finite score)
+            const float slack = fmaxf(n == INT_MAX ? 0.f : fabsf(U), n == INT_MIN ? 0.f : fabsf(L)) * 3.814697265625e-6f + 1e-37f;
             thr[r] = make_float4(U, L, __fmul_ru(eps_rel, norm), slack);
         }
     }
@@ -283,8 +292,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) kge_rank_tc_kernel(const TcPara
         const long long c0 = (long long)ct * TC_NC;
         const int nvalid = (int)min((long long)TC_NC, p.n_cand - c0);
         const float tn = p.tile_norm[ct];
-        const float delta0 = __fmaf_ru(__fmul_ru(thr0.z, tn), 1.0001f, thr0.w);
-        const float delta1 = __fmaf_ru(__fmul_ru(thr1.z, tn), 1.0001f, thr1.w);
+        // an infinite bound bounds nothing (an infinite score would compare >= it): NaN leaves every pair undecided
+        const float dl0 = __fmaf_ru(__fmul_ru(thr0.z, tn), 1.0001f, thr0.w), delta0 = dl0 < INFINITY ? dl0 : NAN;
+        const float dl1 = __fmaf_ru(__fmul_ru(thr1.z, tn), 1.0001f, thr1.w), delta1 = dl1 < INFINITY ? dl1 : NAN;
 #pragma unroll
         for (int j = 0; j < 128; ++j) {
             const bool second = (j >> 1) & 1;
@@ -300,7 +310,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) kge_rank_tc_kernel(const TcPara
                 }
                 continue;
             }
-            const bool undecided = fminf(fabsf(a - U), fabsf(a - L)) < delta;
+            // written as !(>=) so that a NaN score and a NaN or infinite delta (a non-finite entry in the query, or in a row
+            // of the tile: tile_norm is then NaN or inf) leave the pair undecided, for the exact refine to count
+            const bool undecided = !(fminf(fabsf(a - U), fabsf(a - L)) >= delta);
             const int g = (ok && !undecided && a >= U) ? 1 : 0, e = (ok && !undecided && a >= L) ? 1 : 0;
             if (second) { gt1 += g; ge1 += e; } else { gt0 += g; ge0 += e; }
             if (ok && undecided) {

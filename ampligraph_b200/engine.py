@@ -699,7 +699,9 @@ class KGEEngine:
         return out
 
     def rank_filter_probe(self, triples, side, cand_ids=None, cand_begin=0, n_cand=None):
-        """Diagnostic (kge_rank_filter_probe): (approximate tensor-core scores, assumed error bound), both [b, n_cand]."""
+        """Diagnostic (kge_rank_filter_probe): (approximate tensor-core scores, assumed error bound), both [b, n_cand].
+        The bound is NaN for every pair of a query or 256-candidate tile with a NaN or inf entry: the filter refines
+        all of them exactly."""
         b = triples.shape[0]
         if n_cand is None:
             n_cand = self._n_cand(side, cand_ids, cand_begin)

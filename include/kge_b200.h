@@ -555,6 +555,8 @@ int kge_corruption_scores(kge_handle *h, int32_t side, const float *ent_dev, con
 /* Diagnostic for KGE_RANK_MODE_AUTO (used by the tests that pin its error bound): the APPROXIMATE scores of the
  * tensor-core filter pass and the error bound delta the filter assumes for each pair, both [b, n_cand] fp32, in the
  * units of kge_corruption_scores.  The filter is sound iff |approx - kge_corruption_scores| <= delta everywhere.
+ * delta is NaN for every pair of a query or 256-candidate tile that holds a NaN or inf entry: no bound, the filter sends
+ * all those pairs to its exact refine.
  * KGE_ERR_UNSUPPORTED when the filter does not apply (model, mode, size, or KGE_SIDE_P). */
 int kge_rank_filter_probe(kge_handle *h, int32_t side, const float *ent_dev, const float *rel_dev,
                           const int32_t *triples_dev, int64_t b, const int32_t *cand_ids_dev, int64_t cand_begin,

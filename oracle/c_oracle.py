@@ -86,6 +86,14 @@ def corruption_scores(model, side, e_s, e_p, e_o, cand, max_rel_size=1):
     return out
 
 
+def quantise(x):
+    """kgeo_quantise on every element: int32(fl(x * 1000)) truncated toward zero, saturated, NaN -> 0."""
+    x = _f(x)
+    out = np.empty(x.shape, np.int32)
+    lib().kgeo_quantise_many(_p(x, C.c_float), C.c_int64(x.size), _p(out, C.c_int32))
+    return out
+
+
 def _csr(filters, b):
     if filters is None:
         return None, None

@@ -256,7 +256,23 @@ void kgeo_corruption_scores(int model, int side, int K, int max_rel_size, const 
     free(qv);
 }
 
-static int32_t kgeo_quant(float score) { return (int32_t)(score * 1000.0f); } /* AbstractScoringLayer.py:11,:201 */
+/* AbstractScoringLayer.py:11,:201: int32(score * 1000), the product rounded to fp32 and truncated toward zero.  C leaves
+ * the conversion undefined for NaN and out-of-range values (and TensorFlow's CPU cast inherits that), so the project
+ * defines it as the GPU's cvt.rzi.s32.f32 does: fl(score*1000) >= 2^31 saturates to INT32_MAX, <= -2^31 to INT32_MIN
+ * (-2^31 itself is exact), and NaN is 0. */
+int32_t kgeo_quantise(float score)
+{
+    float x = score * 1000.0f;
+    if (x != x) return 0;
+    if (x >= 2147483648.0f) return INT32_MAX;
+    if (x <= -2147483648.0f) return INT32_MIN;
+    return (int32_t)x;
+}
+
+void kgeo_quantise_many(const float *score, int64_t n, int32_t *out)
+{
+    for (int64_t i = 0; i < n; ++i) out[i] = kgeo_quantise(score[i]);
+}
 
 /* AbstractScoringLayer.get_ranks, one side, on already gathered embeddings.
  *   es/ep/eo   [b,K] embeddings of the test triples
@@ -273,11 +289,11 @@ void kgeo_ranks_side(int model, int side, int strategy, int K, int max_rel_size,
     float *qv = (float *)malloc(sizeof(float) * (size_t)K);
     for (int64_t i = 0; i < b; ++i) {
         const float *s = es + i * K, *p = ep + i * K, *o = eo + i * K;
-        int32_t qpos = kgeo_quant(kgeo_score_triple(model, K, max_rel_size, s, p, o));
+        int32_t qpos = kgeo_quantise(kgeo_score_triple(model, K, max_rel_size, s, p, o));
         kgeo_query_vector(model, side, K, max_rel_size, s, p, o, qv);
         int32_t gt = 0, ge = 0, eq = 0;
         for (int64_t c = 0; c < m; ++c) {
-            int32_t qc = kgeo_quant(kgeo_candidate_score(model, side, K, qv, o, cand + c * ld));
+            int32_t qc = kgeo_quantise(kgeo_candidate_score(model, side, K, qv, o, cand + c * ld));
             gt += qpos < qc;
             ge += qpos <= qc;
             eq += qpos == qc;
@@ -290,7 +306,7 @@ void kgeo_ranks_side(int model, int side, int strategy, int K, int max_rel_size,
             for (int64_t f = filt_off[i]; f < filt_off[i + 1]; ++f) {
                 int32_t id = filt_ids[f];
                 if (id < start_id || id > end_id) continue; /* :280-288 */
-                int32_t qf = kgeo_quant(
+                int32_t qf = kgeo_quantise(
                     kgeo_candidate_score(model, side, K, qv, o, cand + (int64_t)(id - start_id) * ld));
                 rank -= qpos <= qf;
             }

@@ -34,8 +34,9 @@ def score_grid(model, ent, rel, triples, cand, max_rel_size=None):
 
 
 def quantise(x):
-    """AbstractScoringLayer.py:11,:201: int32(score * 1000) in fp32, truncated toward zero."""
-    return (np.asarray(x, np.float32) * np.float32(1000.0)).astype(np.int32)
+    """AbstractScoringLayer.py:11,:201: int32(score * 1000) in fp32, truncated toward zero, saturated, NaN -> 0
+    (oracle/kge_oracle.c: kgeo_quantise)."""
+    return c_oracle.quantise(x)
 
 
 def counts(model, ent, rel, triples, filters=None, cand_ids=None, cand_begin=0, n_cand=None, max_rel_size=None):

@@ -257,7 +257,11 @@ __global__ void __launch_bounds__(256) kge_optim_exchange_kernel(const ExchangeA
         float4 x4 = x.table[rank][gi], a4 = z, b4 = z;
         if (S0) a4 = x.s0[i];
         if (S1) b4 = x.s1[i];
-        const float4 xn = update4<KIND, REG>(x4, g4, a4, b4, o, gi < x.ent4 ? x.reg_ent : x.reg_rel, racc);
+        // REG holds when either table has a regulariser; the other one (p = 0) takes the rule without it -- reg_grad
+        // would form lam*0*powf(|x|, -1), NaN at x = 0, and add lam per element to the loss
+        const RegParams &reg = gi < x.ent4 ? x.reg_ent : x.reg_rel;
+        const float4 xn = (REG && reg.p > 0) ? update4<KIND, REG>(x4, g4, a4, b4, o, reg, racc)
+                                             : update4<KIND, false>(x4, g4, a4, b4, o, reg, racc);
         if (MC) {
             multimem_st(x.table_mc + gi, xn);
         } else {

@@ -14,18 +14,21 @@
 
 namespace kge {
 
-// d/dx lam*|x|^p = lam*p*|x|^(p-1)*sign(x); *loss += lam*|x|^p
-__device__ __forceinline__ float lp_term(float x, int p, float lam, float *loss)
+// d/dx lam*|x|^p = sign(x)*(lam*p*|x|^(p-1)): returns the second factor; *loss += lam*|x|^p, as one fma
+__device__ __forceinline__ float lp_scale(float ax, int p, float lam, float *loss)
 {
-    const float ax = fabsf(x), sg = (x > 0.f) ? 1.f : ((x < 0.f) ? -1.f : 0.f);
-    const float pm1 = (p == 2) ? ax : (p == 3) ? ax * ax : (p == 1) ? 1.f : powf(ax, (float)(p - 1));
-    *loss += lam * (pm1 * ax);
-    return lam * (float)p * pm1 * sg;
+    const float pm1 = (p == 2) ? ax : (p == 3) ? __fmul_rn(ax, ax) : (p == 1) ? 1.f : powf(ax, (float)(p - 1));
+    *loss = fmaf(__fmul_rn(pm1, ax), lam, *loss);
+    return lam * (float)p * pm1;
 }
+// The regulariser's gradient sign(x)*s1, plus sign(x)*s2 in one fma for a second term; sign(+-0) = sign(NaN) = 0.
+// Needs r.p > 0: the kernels instantiate REG only for a table that has a regulariser (the exchange kernel, which takes
+// two tables, chooses per element).
 __device__ __forceinline__ float reg_grad(float x, const RegParams &r, float *loss)
 {
-    float g = lp_term(x, r.p, r.lambda, loss);
-    if (r.p2 > 0) g += lp_term(x, r.p2, r.lambda2, loss);
+    const float ax = fabsf(x), sg = (x > 0.f) ? 1.f : ((x < 0.f) ? -1.f : 0.f);
+    float g = __fmul_rn(sg, lp_scale(ax, r.p, r.lambda, loss));
+    if (r.p2 > 0) g = fmaf(sg, lp_scale(ax, r.p2, r.lambda2, loss), g);
     return g;
 }
 
@@ -43,27 +46,29 @@ __host__ __device__ __forceinline__ constexpr bool uses_slot1(int kind, float mo
 }
 
 // One element of the legacy update rules (optimizers.py:255-291 -> tf.keras.optimizers.legacy.* and the training ops
-// they call).  g is the summed gradient plus the regulariser's, a / b are slot 0 / slot 1, fma is one rounding, every
-// other operation rounds to fp32 on its own (oracle/ref_step.py and tests/optim_oracle.py restate this order):
-//   SGD       momentum 0: x -= lr*g;  else a = mu*a - lr*g, x += a
-//   Adam      a = fma(g - a, 1-b1, a); b = fma(g*g - b, 1-b2, b); x -= (a*lr_t) / (sqrt(b) + eps)
-//             lr_t = lr*sqrt(1-b2^t)/(1-b1^t), fp64 on the host
-//   Adagrad   a = fma(g, g, a); x -= lr*g / (sqrt(a) + eps)
+// they call).  g is the summed gradient plus the regulariser's, a / b are slot 0 / slot 1.  Every operation is spelled
+// out: fma is one rounding (fmaf), every other +, -, * rounds to fp32 on its own -- every product that feeds a sum is
+// __fmul_rn, so that the compiler cannot contract it into an fma; a product that feeds / or sqrt cannot be contracted --
+// / and sqrt are IEEE round-to-nearest (no fast-math), and 1-b1, 1-b2, 1-rho are fp32 subtractions.
+// tests/optim_exact_oracle.py restates this order bit for bit:
+//   SGD       momentum 0: x = fma(-g, lr, x);  else a = fma(a, mu, -(g*lr)), x = x + a
+//   Adam      a = fma(g - a, 1-b1, a); b = fma(fma(g, g, -b), 1-b2, b); x -= (a*lr_t) / (sqrt(b) + eps)
+//             lr_t = lr*sqrt(1-b2^t)/(1-b1^t), fp64 on the host, rounded once
+//   Adagrad   a = fma(g, g, a); x -= (lr*g) / (sqrt(a) + eps)
 //   RMSprop   momentum 0: a = fma(rho, a, (1-rho)*(g*g)); d = a, or when centered b = fma(rho, b, (1-rho)*g),
 //             d = fma(-b, b, a); x -= (lr*g) / (sqrt(d) + eps)
 //             momentum mu > 0 (ApplyRMSProp, never centered): a = fma(g*g - a, 1-rho, a);
 //             b = fma(mu, b, (lr*g) / sqrt(a + eps)); x -= b
-//   Adadelta  a = fma(rho, a, (1-rho)*(g*g)); u = sqrt(b + eps) / sqrt(a + eps) * g; x = fma(-lr, u, x);
+//   Adadelta  a = fma(rho, a, (1-rho)*(g*g)); u = (sqrt(b + eps) / sqrt(a + eps)) * g; x = fma(-lr, u, x);
 //             b = fma(rho, b, (1-rho)*(u*u))
-//   Adamax    a = fma(g - a, 1-b1, a); b = max(b2*b, |g|); x = fma(-lr_t, a / (b + eps), x)
-//             lr_t = lr/(1-b1^t), fp64 on the host
-// The new rules spell their products as __fmul_rn so that the compiler cannot contract them into an fma.
+//   Adamax    a = fma(g - a, 1-b1, a); b = fmaxf(b2*b, |g|) (a NaN g is dropped, as fmaxf does);
+//             x = fma(-lr_t, a / (b + eps), x);  lr_t = lr/(1-b1^t), fp64 on the host, rounded once
 template <int KIND>
 __device__ __forceinline__ void apply_rule(float &x, float gg, float &a, float &b, const OptimParams &o)
 {
     if (KIND == KGE_OPT_ADAM) {
-        a = fmaf(gg - a, 1.f - o.beta1, a);       // m += (g-m)(1-b1)
-        b = fmaf(gg * gg - b, 1.f - o.beta2, b);  // v += (g^2-v)(1-b2)
+        a = fmaf(gg - a, 1.f - o.beta1, a);          // m += (g-m)(1-b1)
+        b = fmaf(fmaf(gg, gg, -b), 1.f - o.beta2, b);  // v += (g^2-v)(1-b2)
         x -= (a * o.lr_t) / (sqrtf(b) + o.eps);
     } else if (KIND == KGE_OPT_ADAGRAD) {
         a = fmaf(gg, gg, a);
@@ -93,8 +98,8 @@ __device__ __forceinline__ void apply_rule(float &x, float gg, float &a, float &
         b = fmaxf(__fmul_rn(o.beta2, b), fabsf(gg));
         x = fmaf(-o.lr_t, a / (b + o.eps), x);
     } else {  // SGD (momentum optional)
-        if (o.momentum != 0.f) { a = o.momentum * a - o.lr * gg; x += a; }
-        else x -= o.lr * gg;
+        if (o.momentum != 0.f) { a = fmaf(a, o.momentum, -__fmul_rn(gg, o.lr)); x += a; }
+        else x = fmaf(-gg, o.lr, x);
     }
 }
 

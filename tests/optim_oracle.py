@@ -7,6 +7,7 @@ import numpy as np
 import torch
 
 from oracle import ref_step
+from optim_exact_oracle import fma32
 
 NEW_KINDS = ("rmsprop", "adadelta", "adamax")
 RHO_DEFAULT = {"rmsprop": 0.9, "adadelta": 0.95}
@@ -14,9 +15,9 @@ f32 = np.float32
 
 
 def _fma(a, b, c):
-    """fp32 fma(a, b, c): the product of two fp32 values is exact in fp64, the sum is rounded to fp32 (through fp64)."""
-    d = lambda v: v.double() if torch.is_tensor(v) else torch.tensor(float(v), dtype=torch.float64)
-    return (d(a) * d(b) + d(c)).float()
+    """fp32 fma(a, b, c), correctly rounded (optim_exact_oracle.fma32), as an fp32 tensor."""
+    n = lambda v: v.detach().cpu().numpy() if torch.is_tensor(v) else v
+    return torch.from_numpy(np.ascontiguousarray(fma32(n(a), n(b), n(c))))
 
 
 def rule(name, x, g, a, b, t, lr, hp):

@@ -46,6 +46,14 @@ class KgeShardMap(C.Structure):
                 ("ent", C.c_void_p * 8), ("grad_ent", C.c_void_p * 8), ("stamp_ent", C.c_void_p * 8)]
 
 
+class KgeNegativeSampler(C.Structure):
+    _fields_ = [("struct_size", C.c_int32), ("max_attempts", C.c_int32), ("thresholds", C.c_void_p),
+                ("sub_pool_off", C.c_void_p), ("sub_pool_ids", C.c_void_p), ("obj_pool_off", C.c_void_p),
+                ("obj_pool_ids", C.c_void_p), ("sub_filter_n", C.c_int64), ("sub_filter_keys", C.c_void_p),
+                ("sub_filter_vals", C.c_void_p), ("obj_filter_n", C.c_int64), ("obj_filter_keys", C.c_void_p),
+                ("obj_filter_vals", C.c_void_p)]
+
+
 _P = C.c_void_p
 # name -> (restype, argtypes); kept in one table so tests can check it against the header
 PROTOTYPES = {
@@ -64,6 +72,8 @@ PROTOTYPES = {
     "kge_generate_corruptions": (C.c_int, [_P, _P, C.c_int64, C.c_uint64, C.c_uint64, _P, _P]),
     "kge_philox4x32_10": (None, [_P, _P, _P]),
     "kge_host_corruptions": (C.c_int, [_P, C.c_int64, C.c_int32, C.c_int64, C.c_uint64, C.c_uint64, _P]),
+    "kge_sample_negatives": (C.c_int, [_P, C.POINTER(KgeNegativeSampler), _P, C.c_int64, C.c_uint64, C.c_uint64, _P, _P,
+                                       _P, _P]),
     "kge_train_step": (C.c_int, [_P, C.c_int32, _P, _P, _P, _P, _P, C.c_int64, _P, _P, C.c_uint64, C.c_uint64,
                                  _P, _P, _P, _P, _P, _P]),
     "kge_train_step_sharded": (C.c_int, [_P, C.c_int32, C.POINTER(KgeShardMap), _P, _P, _P, C.c_int64, _P, _P,

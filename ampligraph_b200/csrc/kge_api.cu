@@ -328,6 +328,56 @@ extern "C" int kge_generate_corruptions(kge_handle *h, const int32_t *triples_de
     return KGE_OK;
 }
 
+extern "C" int kge_sample_negatives(kge_handle *h, const kge_negative_sampler *sampler, const int32_t *triples_dev,
+                                    int64_t B, uint64_t seed, uint64_t step, int32_t *neg_ent_dev,
+                                    uint8_t *neg_keep_subj_dev, uint64_t *misses_dev, void *stream)
+{
+    KGE_CHECK_HANDLE(h, "kge_sample_negatives");
+    const kge_negative_sampler *q = sampler;
+    if (!q || q->struct_size != (int32_t)sizeof(kge_negative_sampler))
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_sample_negatives: bad kge_negative_sampler (ABI mismatch)");
+    if (q->max_attempts < 1 || q->max_attempts > 256)  // the attempt is the top byte of the counter's second word
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_sample_negatives: max_attempts must be 1..256, got %d", q->max_attempts);
+    if ((q->sub_pool_off_dev == nullptr) != (q->sub_pool_ids_dev == nullptr) ||
+        (q->obj_pool_off_dev == nullptr) != (q->obj_pool_ids_dev == nullptr))
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_sample_negatives: a pool needs both its offsets and its ids");
+    if (q->sub_filter_n < 0 || q->obj_filter_n < 0 ||
+        (q->sub_filter_n > 0 && (!q->sub_filter_keys_dev || !q->sub_filter_vals_dev)) ||
+        (q->obj_filter_n > 0 && (!q->obj_filter_keys_dev || !q->obj_filter_vals_dev)))
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_sample_negatives: a filter count < 0, or > 0 without its arrays");
+    if (B < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_sample_negatives: B < 0");
+    if (B > ((1ll << 56) - 1) / h->cfg.eta)  // eta*B >= 2^56 (the corruption index shares a counter word with the attempt)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_sample_negatives: eta*B >= 2^56");
+    if (B == 0) return KGE_OK;
+    if (!triples_dev || !neg_ent_dev || !neg_keep_subj_dev)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_sample_negatives: null triples or output pointer");
+    NegativeParams p;
+    memset(&p, 0, sizeof(p));
+    p.triples = triples_dev;
+    p.B = B;
+    p.eta = h->cfg.eta;
+    p.max_attempts = q->max_attempts;
+    p.n_ent = (unsigned)h->cfg.n_ent;
+    p.seed = seed;
+    p.step = step;
+    p.thr = q->thresholds_dev;
+    p.pool_off[0] = reinterpret_cast<const long long *>(q->sub_pool_off_dev);
+    p.pool_ids[0] = q->sub_pool_ids_dev;
+    p.pool_off[1] = reinterpret_cast<const long long *>(q->obj_pool_off_dev);
+    p.pool_ids[1] = q->obj_pool_ids_dev;
+    p.filt_n[0] = q->sub_filter_n;
+    p.filt_keys[0] = reinterpret_cast<const long long *>(q->sub_filter_keys_dev);
+    p.filt_vals[0] = q->sub_filter_vals_dev;
+    p.filt_n[1] = q->obj_filter_n;
+    p.filt_keys[1] = reinterpret_cast<const long long *>(q->obj_filter_keys_dev);
+    p.filt_vals[1] = q->obj_filter_vals_dev;
+    p.neg_ent = neg_ent_dev;
+    p.neg_keep = neg_keep_subj_dev;
+    p.misses = reinterpret_cast<unsigned long long *>(misses_dev);
+    KGE_CUDA(launch_negatives(p, h->sm_count, (cudaStream_t)stream), "kge_sample_negatives");
+    return KGE_OK;
+}
+
 // ---- host-side replay of the corruption stream (no GPU, no handle) -----------------------------------------
 extern "C" void kge_philox4x32_10(const uint32_t ctr[4], const uint32_t key[2], uint32_t out[4])
 {

@@ -87,6 +87,26 @@ cudaError_t launch_rotation_table(const float *rel, float *rot, long long n_rel,
 cudaError_t launch_corruptions(const int32_t *triples, long long B, int eta, unsigned long long seed,
                                unsigned long long step, unsigned n_ent, int32_t *out, cudaStream_t st);
 
+// kge_negatives.cu: the negative sampler (kge_sample_negatives).  Arrays indexed [side] are [0] for a replaced subject
+// and [1] for a replaced object (= keep_subj).
+struct NegativeParams {
+    const int32_t *triples;  // [B, 3]
+    long long B;
+    int eta, max_attempts;   // 1 <= max_attempts <= 256
+    unsigned n_ent;
+    unsigned long long seed, step;
+    const uint32_t *thr;            // [n_rel] Bernoulli thresholds, or nullptr: fair coin
+    const long long *pool_off[2];   // [n_rel + 1] pool CSR offsets of each side, or nullptr: all entities
+    const int32_t *pool_ids[2];
+    long long filt_n[2];            // known (key, value) pairs of each side (0: that side is not filtered)
+    const long long *filt_keys[2];  // p * n_ent + kept entity, lexsorted with the values
+    const int32_t *filt_vals[2];    // the replaced entity
+    int32_t *neg_ent;               // [eta * B]
+    uint8_t *neg_keep;              // [eta * B]
+    unsigned long long *misses;     // += corruptions still known after the last attempt, or nullptr
+};
+cudaError_t launch_negatives(const NegativeParams &p, int sm_count, cudaStream_t st);
+
 // kge_train_1vsall.cu: one side of a 1vsAll multiclass-NLL step of the trilinear models (kge_one_vs_all_step)
 struct OneVsAllSide {
     const float *q;          // [B, ld] query vectors of the side (launch_rank_prepare: qvec_s for side s, qvec_o for o;

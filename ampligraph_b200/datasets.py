@@ -130,6 +130,41 @@ class FilterIndex:
         return off, np.ascontiguousarray(ids, dtype=np.int32)
 
 
+NEGATIVE_SAMPLERS = ("uniform", "bernoulli", "pseudo_typed")
+
+
+def negative_sampler_tables(triples, n_ent, n_rel, sampler="uniform", filtered=False):
+    """The host tables of kge_sample_negatives for one fit (DESIGN.md 3.18), from the distinct training triples
+    (duplicates count once) -> dict of numpy arrays, None where the sampler does not use them:
+      thresholds  uint32 [n_rel] ('bernoulli'): t_p = floor(2^32 |T_p| / (|H_p| + |T_p|)) with H_p (T_p) the distinct
+                  subjects (objects) of relation p, so that the subject is replaced with probability tph / (tph + hpt)
+                  (Wang et al., AAAI 2014); 2^31 for a relation without triples
+      pools       {'s': (offsets int64 [n_rel + 1], ids int32), 'o': ...} ('pseudo_typed'): the sorted distinct subjects
+                  (objects) of each relation, the only entities a replaced subject (object) is drawn from
+      filter      {'s': (keys int64, values int32), 'o': ...} (filtered): FilterIndex._sub and ._obj of the triples,
+                  the lexsorted known (p * n_ent + o, s) and (p * n_ent + s, o) pairs"""
+    if sampler not in NEGATIVE_SAMPLERS:
+        raise ValueError("negative_sampler must be one of %s, got %r" % (", ".join(map(repr, NEGATIVE_SAMPLERS)), sampler))
+    n_ent, n_rel = int(n_ent), int(n_rel)
+    t = np.unique(np.asarray(triples, dtype=np.int64).reshape(-1, 3), axis=0)
+    pairs = {"s": np.unique(t[:, 1] * n_ent + t[:, 0]), "o": np.unique(t[:, 1] * n_ent + t[:, 2])}  # sorted (p, e)
+    count = {side: np.bincount(pairs[side] // n_ent, minlength=n_rel).astype(np.int64) for side in pairs}
+    out = {"thresholds": None, "pools": None, "filter": None}
+    if sampler == "bernoulli":
+        h, o = count["s"], count["o"]
+        out["thresholds"] = np.where(h + o > 0, (o << 32) // np.maximum(h + o, 1), 1 << 31).astype(np.uint32)
+    if sampler == "pseudo_typed":
+        out["pools"] = {}
+        for side in ("s", "o"):
+            off = np.zeros(n_rel + 1, dtype=np.int64)
+            np.cumsum(count[side], out=off[1:])
+            out["pools"][side] = (off, (pairs[side] % n_ent).astype(np.int32))
+    if filtered:
+        f = FilterIndex(t, n_ent)
+        out["filter"] = {"s": f._sub, "o": f._obj}
+    return out
+
+
 def k_vs_all_queries(findex, triples, side):
     """The KvsAll training rows of one side (DESIGN.md 3.13): every distinct (s, p) of `triples` for side 'o', every
     distinct (p, o) for side 's', in order of first appearance, each labelled with its known objects (subjects) in

@@ -184,6 +184,40 @@ def graph_counts(triples, n_nodes, device=None):
     return {"degree": degree, "d": d, "tri2": tri2, "sq": sq, "pot": pot}
 
 
+class NegativeSamplerTables:
+    """The device copy of a fit's negative-sampler tables (datasets.negative_sampler_tables) and the
+    kge_negative_sampler that points at them; the tensors live as long as this object."""
+
+    def __init__(self, tables, max_attempts, device):
+        up = lambda a: torch.as_tensor(np.ascontiguousarray(a)).to(device)
+        self._keep = []
+
+        def ptr(a):
+            if a is None or len(a) == 0:  # an empty array has no data pointer: NULL, as for an absent one
+                return None
+            t = up(a)
+            self._keep.append(t)
+            return t.data_ptr()
+        q = _lib.KgeNegativeSampler(C.sizeof(_lib.KgeNegativeSampler), int(max_attempts))
+        q.thresholds = ptr(tables.get("thresholds"))
+        pools = tables.get("pools") or {}
+        for side, name in (("s", "sub"), ("o", "obj")):
+            if side in pools:
+                off, ids = pools[side]
+                ids_ptr = ptr(ids)
+                if ids_ptr is not None:  # no ids at all: every row is empty, i.e. no pool
+                    setattr(q, name + "_pool_off", ptr(off))
+                    setattr(q, name + "_pool_ids", ids_ptr)
+        filt = tables.get("filter") or {}
+        for side, name in (("s", "sub"), ("o", "obj")):
+            if side in filt:
+                keys, vals = filt[side]
+                setattr(q, name + "_filter_n", len(keys))
+                setattr(q, name + "_filter_keys", ptr(keys))
+                setattr(q, name + "_filter_vals", ptr(vals))
+        self.struct = q
+
+
 _NVTX = os.environ.get("KGE_B200_NVTX", "0") == "1"
 
 
@@ -629,6 +663,36 @@ class KGEEngine:
         v = float(self.loss_acc.cpu().sum())  # one 16-byte D2H copy (synchronising), summed on the host: no reduce kernel
         if reset:
             self.loss_acc.zero_()
+        return v
+
+    @_traced("kge.sample_negatives")
+    def sample_negatives(self, triples, tables, seed=0, step=0):
+        """The step's corruptions under a negative sampler (kge_sample_negatives, DESIGN.md 3.18): tables is a
+        NegativeSamplerTables.  -> (repl int32 [eta*B], keep uint8 [eta*B]), the negatives forward_backward takes, as
+        views of persistent buffers that the next call overwrites.  Corruptions still known after the last attempt add
+        to a device counter (read_negative_misses); nothing synchronises."""
+        assert triples.dtype == torch.int32 and triples.is_cuda and triples.is_contiguous()
+        n = triples.shape[0] * self.eta
+        if getattr(self, "_neg_ent", None) is None or self._neg_ent.numel() < n:
+            self._neg_ent = torch.empty(max(n, 1), dtype=torch.int32, device=self.device)
+            self._neg_keep = torch.empty(max(n, 1), dtype=torch.uint8, device=self.device)
+        if getattr(self, "_neg_misses", None) is None:
+            self._neg_misses = torch.zeros(1, dtype=torch.int64, device=self.device)
+        _lib.check(self.lib.kge_sample_negatives(self.h, C.byref(tables.struct), _ptr(triples), triples.shape[0], int(seed),
+                                                 int(step), _ptr(self._neg_ent), _ptr(self._neg_keep),
+                                                 _ptr(self._neg_misses), self._stream()))
+        if n:
+            self.launches += 1
+        return self._neg_ent[:n], self._neg_keep[:n]
+
+    def read_negative_misses(self, reset=True):
+        """Corruptions sample_negatives emitted although they were known (every attempt drawn) since the last reset;
+        synchronises."""
+        if getattr(self, "_neg_misses", None) is None:
+            return 0
+        v = int(self._neg_misses.item())
+        if reset:
+            self._neg_misses.zero_()
         return v
 
     def generate_corruptions(self, triples, seed=0, step=0):

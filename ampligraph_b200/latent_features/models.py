@@ -11,12 +11,14 @@ import numpy as np
 import torch
 
 from .. import _lib
-from ..datasets import (DataIndexer, FilterIndex, as_triple_array, k_vs_all_queries, k_vs_all_steps,
-                        reciprocal_triples)
-from ..engine import KGEEngine
+from ..datasets import (NEGATIVE_SAMPLERS, DataIndexer, FilterIndex, as_triple_array, k_vs_all_queries, k_vs_all_steps,
+                        negative_sampler_tables, reciprocal_triples)
+from ..engine import KGEEngine, NegativeSamplerTables
 from ..evaluation import hits_at_n_score, mr_score, mrr_score, train_test_split_no_unseen
 from . import initializers, loss_functions, optimizers, regularizers
 from .layers.scoring import SCORING_LAYER_REGISTRY
+
+NEGATIVE_FILTER_ATTEMPTS = 10  # draws of a corruption's entity under fit(filter_negatives=True) (DESIGN.md 3.18)
 
 
 class History:
@@ -117,6 +119,7 @@ class ScoringBasedEmbeddingModel:
         self.distributed = False
         self._dp = None
         self.use_focusE = False
+        self.negative_filter_misses = 0  # known corruptions the last fit(filter_negatives=True) trained on
 
     # ------------------------------------------------------------------ compile
     def compile(self, optimizer="adam", loss=None, entity_relation_initializer="glorot_uniform",
@@ -262,7 +265,8 @@ class ScoringBasedEmbeddingModel:
             validation_data=None, shuffle=True, initial_epoch=0, validation_batch_size=10,
             validation_corrupt_side="s,o", validation_freq=10, validation_burn_in=0, validation_filter=False,
             validation_entities_subset=None, partitioning_k=1, focusE=False, focusE_params={}, one_vs_all=None,
-            k_vs_all=None, label_smoothing=0.0, relation_prediction_weight=0.0):
+            k_vs_all=None, label_smoothing=0.0, relation_prediction_weight=0.0, negative_sampler="uniform",
+            filter_negatives=False):
         """fit (:544-883).  `shuffle` is accepted and ignored exactly like the reference
         (batches are the sequential slices of graph_data_loader.py:495-500).  validation_split: carve the validation
         set out of x with train_test_split_no_unseen(x, test_size=validation_split, seed=self.seed), as the reference
@@ -301,10 +305,21 @@ class ScoringBasedEmbeddingModel:
         positive (s, p, o) gives the side-o row (s, p, o) for side 'o' and the side-o row (o, p^-1, s) for side 's', and
         a step is one side-o 1vsAll call over the batch's forward rows, then its inverse rows; the logged loss sums
         both, and N3 / DURA regularise every row the step trained.  k_vs_all: each side-s query (p, o) with labels {s}
-        becomes the side-o query (o, p^-1) with the same labels; the epoch's steps and label_smoothing are unchanged."""
+        becomes the side-o query (o, p^-1) with the same labels; the epoch's steps and label_smoothing are unchanged.
+
+        negative_sampler, filter_negatives (extension; DESIGN.md 3.18): how sampled training draws its corruptions.
+        'uniform' (default) replaces the subject or the object on a fair coin, by any entity.  'bernoulli' replaces the
+        subject of relation p with probability tph / (tph + hpt) (Wang et al., AAAI 2014), by any entity.
+        'pseudo_typed' keeps the fair coin and draws the replacement from the entities seen in that slot of p in x
+        (PyKEEN's PseudoTypedNegativeSampler).  filter_negatives=True draws a corruption that is a triple of x again,
+        up to NEGATIVE_FILTER_ATTEMPTS draws; those still known after the last are trained on and counted in
+        self.negative_filter_misses (read once per epoch).  The tables are built once per fit from x.  They apply to
+        every single-GPU sampled step of fit (the fused step, user losses, focusE), not to one_vs_all or k_vs_all;
+        train_on_batch and train_on_batches stay uniform.  'uniform' without the filter is the path fit always took."""
         self._assert_compile_was_called()
         if self.reciprocal_relations:
             self._check_reciprocal("fit", one_vs_all, k_vs_all, focusE, relation_prediction_weight)
+        sampled_option = self._check_negative_sampler(negative_sampler, filter_negatives, one_vs_all, k_vs_all)
         self._check_per_occurrence(k_vs_all)
         if k_vs_all is not None or label_smoothing != 0.0:
             self._check_k_vs_all(k_vs_all, label_smoothing, one_vs_all, focusE)
@@ -382,6 +397,13 @@ class ScoringBasedEmbeddingModel:
                 kva[side] = tuple(self._to_dev(a, a.dtype) for a in (q, off, ids))
             count = lambda side: kva[side][0].shape[0] if side in kva else 0
             kva_steps = k_vs_all_steps(count("o"), count("s"), batch_size)
+        sampler = None
+        if sampled_option:
+            sampler = NegativeSamplerTables(
+                negative_sampler_tables(triples, self.max_ent_size, self.max_rel_size, negative_sampler, filter_negatives),
+                NEGATIVE_FILTER_ATTEMPTS, eng.device)
+            eng.read_negative_misses()  # start this fit's count at 0
+        self.negative_filter_misses = 0
         for epoch in range(initial_epoch, epochs):
             if self.use_focusE and self._focuse_stop > 0:  # linear decay of the structural weight (:536-543)
                 self._focuse_sw = max(1 - epoch / self._focuse_stop, 0.001)
@@ -398,15 +420,16 @@ class ScoringBasedEmbeddingModel:
                     self._per_occurrence_backward(batch)
                     eng.apply_gradients()
                 elif self.use_focusE:
-                    self._two_phase_step(batch, weights[start:start + batch_size])
+                    self._two_phase_step(batch, weights[start:start + batch_size], sampler)
                 elif world > 1:  # this rank's slice of the global batch; the step is the global-batch step
                     from ..parallel import row_shard
                     lo, hi = row_shard(batch.shape[0], world, rank)
                     self._dp.train_step(batch[lo:hi], None, seed=self.seed + 7919 * rank, step=self._step)
                 elif user_loss:
-                    self._user_loss_step(batch)
+                    self._user_loss_step(batch, sampler)
                 else:
-                    eng.forward_backward(batch, None, seed=self.seed, step=self._step, defer=True)
+                    negatives = None if sampler is None else eng.sample_negatives(batch, sampler, self.seed, self._step)
+                    eng.forward_backward(batch, negatives, seed=self.seed, step=self._step, defer=True)
                     self._per_occurrence_backward(batch)
                     eng.apply_gradients()
                 self._step += 1
@@ -416,6 +439,8 @@ class ScoringBasedEmbeddingModel:
             if world > 1:
                 self._dp.reduce_loss_()
             self._loss_sum += eng.read_loss()
+            if sampler is not None:  # after read_loss's synchronisation: no step waits for it
+                self.negative_filter_misses += eng.read_negative_misses()
             logs = {"loss": self._loss_sum / max(self._loss_cnt, 1)}
             validate = (epoch >= (validation_burn_in - 1) and validation_data is not None
                         and (epoch + 1) % validation_freq == 0)
@@ -486,6 +511,23 @@ class ScoringBasedEmbeddingModel:
             why = "training is single-GPU only"
         if why is not None:
             raise NotImplementedError("reciprocal relations: %s" % why)
+
+    def _check_negative_sampler(self, negative_sampler, filter_negatives, one_vs_all, k_vs_all):
+        """The refusals of fit(negative_sampler=..., filter_negatives=...), before anything is indexed or trained ->
+        whether the step draws its corruptions with kge_sample_negatives ('uniform' without the filter does not)."""
+        if not isinstance(negative_sampler, str) or negative_sampler not in NEGATIVE_SAMPLERS:
+            raise ValueError("negative_sampler must be one of %s, got %r"
+                             % (", ".join(map(repr, NEGATIVE_SAMPLERS)), negative_sampler))
+        if not isinstance(filter_negatives, bool):
+            raise ValueError("filter_negatives must be a bool, got %r" % (filter_negatives,))
+        if negative_sampler == "uniform" and not filter_negatives:
+            return False
+        if one_vs_all is not None or k_vs_all is not None:
+            raise ValueError("negative_sampler and filter_negatives are sampled-training options: they cannot be "
+                             "combined with one_vs_all or k_vs_all")
+        if self._world() > 1:
+            raise NotImplementedError("negative_sampler and filter_negatives are single-GPU only")
+        return True
 
     def _check_all_candidates(self, training, loss, focusE):
         """The refusals fit's all-candidate training types share: `training` ('1vsAll' or 'KvsAll') needs a trilinear
@@ -678,17 +720,21 @@ class ScoringBasedEmbeddingModel:
         self.is_fitted = True
         return losses
 
-    def _user_loss_step(self, batch):
-        self._two_phase_step(batch, None)
+    def _user_loss_step(self, batch, sampler=None):
+        self._two_phase_step(batch, None, sampler)
 
-    def _two_phase_step(self, batch, weights):
+    def _two_phase_step(self, batch, weights, sampler=None):
         """LossFunctionWrapper / FocusE path: scores from the kernel, dL/dscore from torch autograd
-        over a handful of elementwise ops, gradients from the kernel again."""
+        over a handful of elementwise ops, gradients from the kernel again.  sampler: the fit's NegativeSamplerTables,
+        or None for the uniform corruptions."""
         eng, B = self.engine, batch.shape[0]
-        neg = eng.generate_corruptions(batch, self.seed, self._step)
-        tiled = batch.repeat(self.eta, 1)
-        keep = (neg[:, 0] == tiled[:, 0]).to(torch.uint8).contiguous()
-        repl = torch.where(keep.bool(), neg[:, 2], neg[:, 0]).contiguous()
+        if sampler is not None:
+            repl, keep = eng.sample_negatives(batch, sampler, self.seed, self._step)
+        else:
+            neg = eng.generate_corruptions(batch, self.seed, self._step)
+            tiled = batch.repeat(self.eta, 1)
+            keep = (neg[:, 0] == tiled[:, 0]).to(torch.uint8).contiguous()
+            repl = torch.where(keep.bool(), neg[:, 2], neg[:, 0]).contiguous()
         sp = torch.empty(B, dtype=torch.float32, device=eng.device)
         sn = torch.empty(B * self.eta, dtype=torch.float32, device=eng.device)
         eng.forward_backward(batch, (repl, keep), seed=self.seed, step=self._step, mode=_lib.STEP_FORWARD_ONLY,

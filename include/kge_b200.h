@@ -194,6 +194,41 @@ void kge_philox4x32_10(const uint32_t ctr[4], const uint32_t key[2], uint32_t ou
 int kge_host_corruptions(const int32_t *triples_host /*[B,3]*/, int64_t B, int32_t eta, int64_t n_ent,
                          uint64_t seed, uint64_t step, int32_t *corruptions_host /*[eta*B,3]*/);
 
+/* Negative sampler of sampled training (extension; DESIGN.md 3.18): Bernoulli side choice (Wang et al., AAAI 2014),
+ * pseudo-typed pools (PyKEEN's PseudoTypedNegativeSampler) and filtered negatives.  kge_sample_negatives writes the
+ * [eta*B] neg_ent_dev / neg_keep_subj_dev arrays kge_train_step takes.  Corruption r = j*B+i (tile order) draws its
+ * attempt a from Philox4x32-10 with counter (r_lo, r_hi | a << 24, step_lo, step_hi) and key = seed (attempt 0 is the
+ * block kge_generate_corruptions uses):
+ *   side    attempt 0 only: keep_subj = x & 1 without thresholds; with them the subject is replaced iff x < thresholds[p]
+ *   entity  pool[(y * |pool|) >> 32], the pool of (p, replaced side); all entities [0, n_ent) without pools or where
+ *           the pool row is empty
+ *   filter  a corruption (s, p, c) (object replaced) or (c, p, o) (subject replaced) whose pair (p * n_ent + kept
+ *           entity, c) is in that side's filter arrays is drawn again (entity only) with attempt a + 1 while
+ *           a + 1 < max_attempts; after the last attempt it is emitted and *misses_dev is incremented.
+ * With every optional array NULL the output is the stream of kge_generate_corruptions.  Deterministic, stream-ordered,
+ * allocates nothing. */
+typedef struct kge_negative_sampler {
+    int32_t struct_size;              /* sizeof(kge_negative_sampler), ABI guard */
+    int32_t max_attempts;             /* 1..256 draws of a corruption's entity (1: no re-draw) */
+    const uint32_t *thresholds_dev;   /* [n_rel] t_p = floor(2^32 |T_p| / (|H_p| + |T_p|)), or NULL: fair coin */
+    const int64_t *sub_pool_off_dev;  /* [n_rel + 1] CSR offsets into sub_pool_ids_dev of each relation's subject pool */
+    const int32_t *sub_pool_ids_dev;  /*   (both or neither; NULL: every subject is drawn from all entities) */
+    const int64_t *obj_pool_off_dev;  /* the same for the object pools */
+    const int32_t *obj_pool_ids_dev;
+    int64_t sub_filter_n;             /* known pairs of a replaced subject: key p * n_ent + o, value s; lexsorted */
+    const int64_t *sub_filter_keys_dev;
+    const int32_t *sub_filter_vals_dev;
+    int64_t obj_filter_n;             /* known pairs of a replaced object: key p * n_ent + s, value o; lexsorted */
+    const int64_t *obj_filter_keys_dev;
+    const int32_t *obj_filter_vals_dev;
+} kge_negative_sampler;
+/* triples_dev [B,3]; eta from the handle; misses_dev: uint64 counter added to, or NULL.  KGE_ERR_INVALID_ARGUMENT
+ * without a launch for a bad struct, max_attempts outside 1..256, pool offsets without ids or the reverse, a filter
+ * count < 0 or > 0 without its arrays, B < 0, eta*B >= 2^56, or null triples / outputs when B > 0; B = 0 is a no-op. */
+int kge_sample_negatives(kge_handle *h, const kge_negative_sampler *sampler, const int32_t *triples_dev, int64_t B,
+                         uint64_t seed, uint64_t step, int32_t *neg_ent_dev, uint8_t *neg_keep_subj_dev,
+                         uint64_t *misses_dev, void *stream);
+
 /* train_step forward+backward (ScoringBasedEmbeddingModel.py:370-429, call :237-269,
  * Loss.__call__ loss_functions.py:185-225, tape.gradient optimizers.py:166).
  *   triples_dev     [B,3] int32 positives

@@ -17,7 +17,7 @@ KGE_OK, KGE_ERR_INVALID_ARGUMENT, KGE_ERR_CUDA, KGE_ERR_UNSUPPORTED = 0, 1, 2, 3
 SCORING = {"TransE": 0, "DistMult": 1, "ComplEx": 2, "HolE": 3, "RotatE": 4}
 LOSSES = {"pairwise": 0, "nll": 1, "absolute_margin": 2, "self_adversarial": 3, "multiclass_nll": 4}
 REDUCTIONS = {"sum": 0, "mean": 1}
-OPTIMIZERS = {"sgd": 0, "adam": 1, "adagrad": 2, "rmsprop": 3, "adadelta": 4, "adamax": 5}
+OPTIMIZERS = {"sgd": 0, "adam": 1, "adagrad": 2, "rmsprop": 3, "adadelta": 4, "adamax": 5, "nadam": 6, "ftrl": 7}
 SIDES = {"s": 0, "o": 1, "p": 2}  # "p": relation prediction, candidates are relation rows
 STRATEGIES = {"worst": 0, "best": 1, "middle": 2}
 STEP_FUSED, STEP_FORWARD_ONLY, STEP_BACKWARD_EXT, STEP_FUSED_DEFER = 0, 1, 2, 3
@@ -38,7 +38,10 @@ class KgeOptimizerConfig(C.Structure):
     _fields_ = [("struct_size", C.c_int32), ("kind", C.c_int32), ("learning_rate", C.c_float),
                 ("beta_1", C.c_float), ("beta_2", C.c_float), ("epsilon", C.c_float), ("momentum", C.c_float),
                 ("initial_accumulator_value", C.c_float), ("reg_p", C.c_int32), ("reg_lambda", C.c_float),
-                ("reg_p2", C.c_int32), ("reg_lambda2", C.c_float), ("rho", C.c_float), ("centered", C.c_int32)]
+                ("reg_p2", C.c_int32), ("reg_lambda2", C.c_float), ("rho", C.c_float), ("centered", C.c_int32),
+                ("l1", C.c_float), ("l2", C.c_float), ("l2_shrinkage", C.c_float), ("lr_power", C.c_float),
+                ("ftrl_beta", C.c_float), ("nadam_m_t", C.c_float), ("nadam_m_t1", C.c_float), ("nadam_s_new", C.c_float),
+                ("nadam_s_next", C.c_float), ("nadam_v_den", C.c_float)]
 
 
 class KgeShardMap(C.Structure):
@@ -93,6 +96,8 @@ PROTOTYPES = {
     "kge_step_stamp": (C.c_int32, [C.c_uint64]),
     "kge_optimizer_step_lazy": (C.c_int, [_P, C.POINTER(KgeOptimizerConfig), C.c_int64, _P, _P, _P, _P, C.c_int64, _P,
                                           C.c_int32, _P, _P]),
+    "kge_optimizer_step_decay": (C.c_int, [_P, C.POINTER(KgeOptimizerConfig), C.c_int64, _P, _P, _P, _P, C.c_int64, _P,
+                                           C.c_int32, _P]),
     "kge_optimizer_step_sharded": (C.c_int, [_P, C.POINTER(KgeOptimizerConfig), C.c_int64, C.c_int32, C.c_int32,
                                              C.POINTER(_P), C.POINTER(_P), _P, _P, C.c_int64, C.c_int64, _P, _P]),
     "kge_optimizer_step_exchange": (C.c_int, [_P, C.POINTER(KgeOptimizerConfig), C.POINTER(KgeOptimizerConfig), C.c_int64,

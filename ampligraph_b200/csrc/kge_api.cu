@@ -688,14 +688,15 @@ extern "C" int kge_train_step_sharded(kge_handle *h, int32_t mode, const kge_sha
 }
 
 // Checks a caller's config, copies it into out, widened to the current layout, and re-points opt at the copy.  A config
-// of the layout before rho (struct_size == offsetof(kge_optimizer_config, rho)) is accepted for the kinds that layout
-// knew; its new fields read as 0.
+// of an older layout -- before rho (struct_size == offsetof(kge_optimizer_config, rho)) or before l1 -- is accepted for
+// the kinds that layout knew; its new fields read as 0.
 static int check_optim(const kge_optimizer_config *&opt, const char *fn, kge_optimizer_config &out)
 {
-    const int32_t old_size = (int32_t)offsetof(kge_optimizer_config, rho);
-    if (!opt || (opt->struct_size != (int32_t)sizeof(kge_optimizer_config) && opt->struct_size != old_size))
+    const int32_t size_v1 = (int32_t)offsetof(kge_optimizer_config, rho), size_v2 = (int32_t)offsetof(kge_optimizer_config, l1);
+    if (!opt || (opt->struct_size != (int32_t)sizeof(kge_optimizer_config) && opt->struct_size != size_v1 &&
+                 opt->struct_size != size_v2))
         return fail(KGE_ERR_INVALID_ARGUMENT, "%s: bad kge_optimizer_config (ABI mismatch)", fn);
-    const int last = opt->struct_size == old_size ? KGE_OPT_ADAGRAD : KGE_OPT_ADAMAX;
+    const int last = opt->struct_size == size_v1 ? KGE_OPT_ADAGRAD : opt->struct_size == size_v2 ? KGE_OPT_ADAMAX : KGE_OPT_FTRL;
     if (opt->kind < KGE_OPT_SGD || opt->kind > last)
         return fail(KGE_ERR_INVALID_ARGUMENT, "Could not interpret optimizer identifier: %d", opt->kind);
     if (opt->reg_p < 0 || opt->reg_p2 < 0 || (opt->reg_p == 0 && opt->reg_p2 != 0))
@@ -706,6 +707,9 @@ static int check_optim(const kge_optimizer_config *&opt, const char *fn, kge_opt
     opt = &out;
     if (out.kind == KGE_OPT_RMSPROP && out.centered && out.momentum != 0.f)
         return fail(KGE_ERR_UNSUPPORTED, "%s: centered RMSprop with momentum needs a third slot buffer (not supported)", fn);
+    // Keras' legacy Ftrl refuses the same values (and the NaNs these comparisons also refuse)
+    if (out.kind == KGE_OPT_FTRL && !(out.lr_power <= 0.f && out.l1 >= 0.f && out.l2 >= 0.f && out.l2_shrinkage >= 0.f))
+        return fail(KGE_ERR_INVALID_ARGUMENT, "%s: Ftrl needs lr_power <= 0 and l1, l2, l2_shrinkage >= 0", fn);
     return KGE_OK;
 }
 static RegParams reg_of(const kge_optimizer_config *opt)
@@ -735,6 +739,27 @@ static OptimParams optim_params(const kge_optimizer_config *opt, int64_t t)
                          (1.0 - pow((double)opt->beta_1, (double)t)));
     return o;
 }
+// Nadam's and Ftrl's per-step scalars, in fp32 as Keras forms them (1 - m_t, 1 - s_new, 1 - s_next: _prepare_local;
+// Ftrl's l2 + beta / (2 lr): _resource_apply_dense), and no row-decay mode
+static OptimStep optim_step(const kge_optimizer_config *opt)
+{
+    OptimStep q;
+    memset(&q, 0, sizeof(q));
+    if (opt->kind == KGE_OPT_FTRL) {
+        const float l2 = opt->l2 + opt->ftrl_beta / (2.f * opt->learning_rate);
+        q.l1 = opt->l1;
+        q.l2x2 = 2.f * l2;
+        q.shrinkx2 = 2.f * opt->l2_shrinkage;
+        q.lr_power = opt->lr_power;
+    } else if (opt->kind == KGE_OPT_NADAM) {
+        q.one_m_mt = 1.f - opt->nadam_m_t;
+        q.m_t1 = opt->nadam_m_t1;
+        q.one_m_snew = 1.f - opt->nadam_s_new;
+        q.one_m_snext = 1.f - opt->nadam_s_next;
+        q.v_den = opt->nadam_v_den;
+    }
+    return q;
+}
 // Every slot buffer the config's update reads and writes must be given
 static int check_slots(const kge_optimizer_config *opt, const float *s0, const float *s1, const char *fn)
 {
@@ -755,7 +780,7 @@ extern "C" int kge_optimizer_step(kge_handle *h, const kge_optimizer_config *opt
     if (!table_dev || !grad_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step: null table/grad");
     if (int rc = check_slots(opt, slot0_dev, slot1_dev, "kge_optimizer_step")) return rc;
     const OptimParams o = optim_params(opt, t);
-    KGE_CUDA(launch_optimizer(o, table_dev, grad_dev, slot0_dev, slot1_dev, rows * (long long)h->L.ld, reg_loss_dev,
+    KGE_CUDA(launch_optimizer(o, optim_step(opt), table_dev, grad_dev, slot0_dev, slot1_dev, rows * (long long)h->L.ld, reg_loss_dev,
                               h->sm_count, (cudaStream_t)stream),
              "kge_optimizer_step");
     return KGE_OK;
@@ -783,7 +808,7 @@ extern "C" int kge_optimizer_step_deferred(kge_handle *h, const kge_optimizer_co
     // the checks above refuse without touching the pending step (the caller may repeat the call); from here on it is
     // consumed, and the workspace is free again, whether or not the launch succeeds
     h->sum_pending = false;
-    KGE_CUDA(launch_bucket_sum_optimizer(p, h->nit, o, params_in, params_out, grad_dev, slot0_dev, slot1_dev, rows,
+    KGE_CUDA(launch_bucket_sum_optimizer(p, h->nit, o, optim_step(opt), params_in, params_out, grad_dev, slot0_dev, slot1_dev, rows,
                                          reg_loss_dev, (cudaStream_t)stream),
              "kge_optimizer_step_deferred");
     return KGE_OK;
@@ -835,9 +860,35 @@ extern "C" int kge_optimizer_step_lazy(kge_handle *h, const kge_optimizer_config
     if (!table_dev || !grad_dev || !row_stamp_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_lazy: null pointer");
     if (int rc = check_slots(opt, slot0_dev, slot1_dev, "kge_optimizer_step_lazy")) return rc;
     const OptimParams o = optim_params(opt, t);
-    KGE_CUDA(launch_optimizer_lazy(o, table_dev, grad_dev, slot0_dev, slot1_dev, rows, h->L.ld, (const int *)row_stamp_dev,
+    KGE_CUDA(launch_optimizer_lazy(o, optim_step(opt), table_dev, grad_dev, slot0_dev, slot1_dev, rows, h->L.ld, (const int *)row_stamp_dev,
                                    stamp, reg_loss_dev, h->sm_count, (cudaStream_t)stream),
              "kge_optimizer_step_lazy");
+    return KGE_OK;
+}
+
+extern "C" int kge_optimizer_step_decay(kge_handle *h, const kge_optimizer_config *opt, int64_t t, float *table_dev,
+                                        float *grad_dev, float *slot0_dev, float *slot1_dev, int64_t rows,
+                                        const int32_t *row_stamp_dev, int32_t stamp, void *stream)
+{
+    KGE_CHECK_HANDLE(h, "kge_optimizer_step_decay");
+    kge_optimizer_config cfg;
+    if (int rc = check_optim(opt, "kge_optimizer_step_decay", cfg)) return rc;
+    if (opt->kind != KGE_OPT_NADAM)
+        return fail(KGE_ERR_UNSUPPORTED, "kge_optimizer_step_decay: only Nadam has a row-decay rule");
+    if (opt->reg_p != 0)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_decay: a regularised table's gradient is dense "
+                                              "(kge_optimizer_step)");
+    if (rows < 0 || t < 1) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_decay: rows >= 0 and t >= 1 required");
+    if (rows == 0) return KGE_OK;
+    if (!table_dev || !grad_dev || !row_stamp_dev) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_decay: null pointer");
+    if (int rc = check_slots(opt, slot0_dev, slot1_dev, "kge_optimizer_step_decay")) return rc;
+    OptimStep q = optim_step(opt);
+    q.row_stamp = (const int *)row_stamp_dev;
+    q.stamp = stamp;
+    q.ld4 = h->L.ld / 4;
+    KGE_CUDA(launch_optimizer(optim_params(opt, t), q, table_dev, grad_dev, slot0_dev, slot1_dev, rows * (long long)h->L.ld,
+                              nullptr, h->sm_count, (cudaStream_t)stream),
+             "kge_optimizer_step_decay");
     return KGE_OK;
 }
 
@@ -864,7 +915,7 @@ extern "C" int kge_optimizer_step_sharded(kge_handle *h, const kge_optimizer_con
         if (!peer_tables[q] || !peer_grads[q]) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_sharded: null peer pointer for rank %d", q);
     if (int rc = check_slots(opt, slot0_shard_dev, slot1_shard_dev, "kge_optimizer_step_sharded")) return rc;
     const OptimParams o = optim_params(opt, t);
-    KGE_CUDA(launch_optimizer_sharded(o, world, rank, peer_tables, peer_grads, slot0_shard_dev, slot1_shard_dev,
+    KGE_CUDA(launch_optimizer_sharded(o, optim_step(opt), world, rank, peer_tables, peer_grads, slot0_shard_dev, slot1_shard_dev,
                                       row_begin * (long long)h->L.ld, (row_end - row_begin) * (long long)h->L.ld,
                                       reg_loss_dev, h->sm_count, (cudaStream_t)stream),
              "kge_optimizer_step_sharded");
@@ -886,7 +937,8 @@ extern "C" int kge_optimizer_step_exchange(kge_handle *h, const kge_optimizer_co
     if (int rc = check_world(world, rank, "kge_optimizer_step_exchange")) return rc;
     if (opt_ent->kind != opt_rel->kind || opt_ent->learning_rate != opt_rel->learning_rate || opt_ent->beta_1 != opt_rel->beta_1 ||
         opt_ent->beta_2 != opt_rel->beta_2 || opt_ent->epsilon != opt_rel->epsilon || opt_ent->momentum != opt_rel->momentum ||
-        opt_ent->rho != opt_rel->rho || opt_ent->centered != opt_rel->centered)
+        opt_ent->rho != opt_rel->rho || opt_ent->centered != opt_rel->centered ||
+        memcmp(&opt_ent->l1, &opt_rel->l1, sizeof(kge_optimizer_config) - offsetof(kge_optimizer_config, l1)) != 0)
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_optimizer_step_exchange: the two tables may differ in their regulariser only");
     const int64_t total_rows = h->cfg.n_ent + h->cfg.n_rel;
     if (row_begin < 0 || row_end < row_begin || row_end > total_rows || t < 1)
@@ -921,7 +973,7 @@ extern "C" int kge_optimizer_step_exchange(kge_handle *h, const kge_optimizer_co
     x.reg_loss = reg_loss_dev;
     x.done_counter = h->done_counter;
     x.trace = h->exchange_trace;
-    KGE_CUDA(launch_optimizer_exchange(o, x, h->sm_count, (cudaStream_t)stream), "kge_optimizer_step_exchange");
+    KGE_CUDA(launch_optimizer_exchange(o, optim_step(opt_ent), x, h->sm_count, (cudaStream_t)stream), "kge_optimizer_step_exchange");
     return KGE_OK;
 }
 

@@ -205,6 +205,14 @@ struct OptimParams {
     float rho;     // RMSprop / Adadelta decay
     int centered;  // RMSprop
 };
+// What Nadam and Ftrl read beyond OptimParams, and Nadam's row-decay mode.  Every optimizer kernel takes it as its LAST
+// parameter, so the parameters of the kinds before them kept their offsets (and those instantiations their code).
+struct OptimStep {
+    float l1, l2x2, shrinkx2, lr_power;  // Ftrl: l1, 2 * (l2 + beta / (2 lr)), 2 * l2_shrinkage, learning_rate_power
+    float one_m_mt, m_t1, one_m_snew, one_m_snext, v_den;  // Nadam: 1 - m_t, m_t1, 1 - s_new, 1 - s_next, 1 - b2^t
+    const int *row_stamp;  // Nadam's IndexedSlices rule (dense kernel only): a row whose stamp != stamp only decays m and
+    int stamp, ld4;        // v; nullptr: every row moves.  ld4 = float4s per row
+};
 struct ExchangeParams {  // kge_optimizer_step_exchange
     int world, rank, phases;
     float *table[KGE_MAX_PEERS];        // [ent|rel] parameter block of every rank
@@ -223,21 +231,21 @@ struct ExchangeParams {  // kge_optimizer_step_exchange
     unsigned *done_counter;             // handle-owned device counter (last-CTA detection), self-resetting
     unsigned long long *trace;          // nullptr or 8 x uint64 phase stamps (kge_set_exchange_trace)
 };
-cudaError_t launch_optimizer(const OptimParams &o, float *table, float *grad, float *slot0, float *slot1,
+cudaError_t launch_optimizer(const OptimParams &o, const OptimStep &os, float *table, float *grad, float *slot0, float *slot1,
                              long long n_floats, double *reg_loss, int sm_count, cudaStream_t st);
-cudaError_t launch_optimizer_lazy(const OptimParams &o, float *table, float *grad, float *slot0, float *slot1,
+cudaError_t launch_optimizer_lazy(const OptimParams &o, const OptimStep &os, float *table, float *grad, float *slot0, float *slot1,
                                   long long rows, int ld, const int *row_stamp, int stamp, double *reg_loss,
                                   int sm_count, cudaStream_t st);
 // tables/grads: HOST arrays of `world` device pointers (own rank first is NOT required; index = rank)
-cudaError_t launch_optimizer_sharded(const OptimParams &o, int world, int rank, float *const *tables, float *const *grads,
+cudaError_t launch_optimizer_sharded(const OptimParams &o, const OptimStep &os, int world, int rank, float *const *tables, float *const *grads,
                                      float *slot0, float *slot1, long long off_floats, long long n_floats,
                                      double *reg_loss, int sm_count, cudaStream_t st);
-cudaError_t launch_optimizer_exchange(const OptimParams &o, const ExchangeParams &x, int sm_count, cudaStream_t st);
+cudaError_t launch_optimizer_exchange(const OptimParams &o, const OptimStep &os, const ExchangeParams &x, int sm_count, cudaStream_t st);
 cudaError_t launch_peer_barrier(int world, int rank, unsigned *const *flags, int slot, unsigned token, cudaStream_t st);
 // kge_train_bucket.cu: the same per-entity sum with the dense optimizer as its epilogue, one warp per row of the
 // [ent | rel] block (rows = n_ent + n_rel; p.ent / p.rel and p.grad_ent / p.grad_rel are the two parts of `in` and `grad`):
 // reads `in`, writes every element of `out`, updates the slots in place and zeroes `grad`
-cudaError_t launch_bucket_sum_optimizer(const TrainParams &p, int nit, const OptimParams &o, const float *in, float *out,
+cudaError_t launch_bucket_sum_optimizer(const TrainParams &p, int nit, const OptimParams &o, const OptimStep &os, const float *in, float *out,
                                         float *grad, float *slot0, float *slot1, long long rows, double *reg_loss,
                                         cudaStream_t st);
 

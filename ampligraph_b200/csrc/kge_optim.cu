@@ -23,17 +23,29 @@ namespace kge {
 template <int KIND, bool REG>
 __global__ void __launch_bounds__(256) kge_optim_kernel(float4 *__restrict__ var, float4 *__restrict__ grad,
                                                         float4 *__restrict__ s0, float4 *__restrict__ s1,
-                                                        long long n4, OptimParams o, double *reg_loss)
+                                                        long long n4, OptimParams o, double *reg_loss,
+                                                        const OptimStep os)
 {
     const bool S0 = uses_slot0(KIND, o.momentum), S1 = uses_slot1(KIND, o.momentum, o.centered);
     float racc = 0.f;
     const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
     const long long stride = (long long)gridDim.x * blockDim.x;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
+        if constexpr (KIND == KGE_OPT_NADAM) {
+            // row-decay mode (kge_optimizer_step_decay): a row that was not looked up only decays m and v; its table row
+            // is not read or written, and its gradient row is already 0
+            if (os.row_stamp && __ldg(os.row_stamp + i / os.ld4) != os.stamp) {
+                float4 a4 = s0[i], b4 = s1[i];
+                nadam_decay4(a4, b4, o);
+                s0[i] = a4;
+                s1[i] = b4;
+                continue;
+            }
+        }
         float4 x4 = var[i], g4 = grad[i], a4 = z, b4 = z;
         if (S0) a4 = s0[i];
         if (S1) b4 = s1[i];
-        var[i] = update4<KIND, REG>(x4, g4, a4, b4, o, o.reg, racc);
+        var[i] = update4<KIND, REG>(x4, g4, a4, b4, o, os, o.reg, racc);
         if (S0) s0[i] = a4;
         if (S1) s1[i] = b4;
         grad[i] = z;
@@ -60,7 +72,8 @@ struct PeerPtrs {
 template <int KIND, bool REG>
 __global__ void __launch_bounds__(256) kge_optim_sharded_kernel(PeerPtrs pp, int world, int rank, float4 *__restrict__ s0,
                                                                 float4 *__restrict__ s1, long long off4,
-                                                                long long n4, OptimParams o, double *reg_loss)
+                                                                long long n4, OptimParams o, double *reg_loss,
+                                                                const OptimStep os)
 {
     const bool S0 = uses_slot0(KIND, o.momentum), S1 = uses_slot1(KIND, o.momentum, o.centered);
     float racc = 0.f;
@@ -79,7 +92,7 @@ __global__ void __launch_bounds__(256) kge_optim_sharded_kernel(PeerPtrs pp, int
         float4 x4 = pp.table[rank][gi], a4 = z, b4 = z;  // all replicas are identical; read the local one
         if (S0) a4 = s0[i];
         if (S1) b4 = s1[i];
-        const float4 xn = update4<KIND, REG>(x4, g4, a4, b4, o, o.reg, racc);
+        const float4 xn = update4<KIND, REG>(x4, g4, a4, b4, o, os, o.reg, racc);
 #pragma unroll
         for (int q = 0; q < KGE_MAX_PEERS; ++q)
             if (q < world) __stcg(pp.table[q] + gi, xn);  // deliver the updated rows to every replica
@@ -89,7 +102,7 @@ __global__ void __launch_bounds__(256) kge_optim_sharded_kernel(PeerPtrs pp, int
     if (REG && reg_loss) flush_reg_loss(racc, reg_loss);
 }
 
-cudaError_t launch_optimizer_sharded(const OptimParams &o, int world, int rank, float *const *tables, float *const *grads,
+cudaError_t launch_optimizer_sharded(const OptimParams &o, const OptimStep &os, int world, int rank, float *const *tables, float *const *grads,
                                      float *slot0, float *slot1, long long off_floats, long long n_floats,
                                      double *reg_loss, int sm_count, cudaStream_t st)
 {
@@ -105,7 +118,7 @@ cudaError_t launch_optimizer_sharded(const OptimParams &o, int world, int rank, 
     float4 *a = (float4 *)slot0, *b = (float4 *)slot1;
     const long long off4 = off_floats / 4;
     return dispatch_optimizer(o.kind, o.reg.p > 0, [&](auto kind, auto reg) {
-        kge_optim_sharded_kernel<kind, reg><<<grid, 256, 0, st>>>(pp, world, rank, a, b, off4, n4, o, reg_loss);
+        kge_optim_sharded_kernel<kind, reg><<<grid, 256, 0, st>>>(pp, world, rank, a, b, off4, n4, o, reg_loss, os);
         return cudaGetLastError();
     });
 }
@@ -226,7 +239,8 @@ __device__ __forceinline__ unsigned long long globaltimer_ns()
     } while (0)
 
 template <int KIND, bool REG, int WORLD, bool MC>
-__global__ void __launch_bounds__(256) kge_optim_exchange_kernel(const ExchangeArgs x, const OptimParams o)
+__global__ void __launch_bounds__(256) kge_optim_exchange_kernel(const ExchangeArgs x, const OptimParams o,
+                                                                    const OptimStep os)
 {
     const bool S0 = uses_slot0(KIND, o.momentum), S1 = uses_slot1(KIND, o.momentum, o.centered);
     constexpr int U = WORLD <= 4 ? 4 : 2;  // float4s per thread per trip (U*WORLD peer loads in flight per thread)
@@ -260,8 +274,8 @@ __global__ void __launch_bounds__(256) kge_optim_exchange_kernel(const ExchangeA
         // REG holds when either table has a regulariser; the other one (p = 0) takes the rule without it -- reg_grad
         // would form lam*0*powf(|x|, -1), NaN at x = 0, and add lam per element to the loss
         const RegParams &reg = gi < x.ent4 ? x.reg_ent : x.reg_rel;
-        const float4 xn = (REG && reg.p > 0) ? update4<KIND, REG>(x4, g4, a4, b4, o, reg, racc)
-                                             : update4<KIND, false>(x4, g4, a4, b4, o, reg, racc);
+        const float4 xn = (REG && reg.p > 0) ? update4<KIND, REG>(x4, g4, a4, b4, o, os, reg, racc)
+                                             : update4<KIND, false>(x4, g4, a4, b4, o, os, reg, racc);
         if (MC) {
             multimem_st(x.table_mc + gi, xn);
         } else {
@@ -350,8 +364,8 @@ __global__ void __launch_bounds__(256) kge_optim_exchange_kernel(const ExchangeA
 // the kernel (measured before the H100 port).  The loops are grid-stride, so fewer CTAs only
 // means more trips per thread.
 template <int KIND, bool REG, int WORLD, bool MC>
-static cudaError_t launch_exchange_variant(const ExchangeArgs &a, const OptimParams &o, long long want, int sm_count,
-                                           cudaStream_t st)
+static cudaError_t launch_exchange_variant(const ExchangeArgs &a, const OptimParams &o, const OptimStep &os, long long want,
+                                           int sm_count, cudaStream_t st)
 {
     auto kern = kge_optim_exchange_kernel<KIND, REG, WORLD, MC>;
     static int occ_cached = 0;  // per instantiation; the query is cheap but this is the per-step path
@@ -362,11 +376,11 @@ static cudaError_t launch_exchange_variant(const ExchangeArgs &a, const OptimPar
         occ_cached = occ < 1 ? 1 : (occ > 4 ? 4 : occ);
     }
     const long long cap = (long long)sm_count * occ_cached;
-    kern<<<(int)(want < cap ? want : cap), 256, 0, st>>>(a, o);
+    kern<<<(int)(want < cap ? want : cap), 256, 0, st>>>(a, o, os);
     return cudaGetLastError();
 }
 
-cudaError_t launch_optimizer_exchange(const OptimParams &o, const ExchangeParams &xp, int sm_count, cudaStream_t st)
+cudaError_t launch_optimizer_exchange(const OptimParams &o, const OptimStep &os, const ExchangeParams &xp, int sm_count, cudaStream_t st)
 {
     ExchangeArgs a;
     for (int q = 0; q < KGE_MAX_PEERS; ++q) {
@@ -402,8 +416,8 @@ cudaError_t launch_optimizer_exchange(const OptimParams &o, const ExchangeParams
         auto variant = [&](auto world) {
             constexpr int K = decltype(kind)::value;
             constexpr bool R = decltype(reg)::value;
-            return mc ? launch_exchange_variant<K, R, world, true>(a, o, want, sm_count, st)
-                      : launch_exchange_variant<K, R, world, false>(a, o, want, sm_count, st);
+            return mc ? launch_exchange_variant<K, R, world, true>(a, o, os, want, sm_count, st)
+                      : launch_exchange_variant<K, R, world, false>(a, o, os, want, sm_count, st);
         };
         return dispatch_value<1, 2, 3, 4, 5, 6, 7, 8>(xp.world, variant);
     });
@@ -421,7 +435,8 @@ template <int KIND, bool REG>
 __global__ void __launch_bounds__(256) kge_optim_lazy_kernel(float *__restrict__ var, float *__restrict__ grad,
                                                              float *__restrict__ s0, float *__restrict__ s1,
                                                              long long rows, int ld, const int *__restrict__ row_stamp,
-                                                             int stamp, OptimParams o, double *reg_loss)
+                                                             int stamp, OptimParams o, double *reg_loss,
+                                                             const OptimStep os)
 {
     const bool S0 = uses_slot0(KIND, o.momentum), S1 = uses_slot1(KIND, o.momentum, o.centered);
     const int lane = threadIdx.x & 31;
@@ -441,7 +456,7 @@ __global__ void __launch_bounds__(256) kge_optim_lazy_kernel(float *__restrict__
                 float4 a4 = z, b4 = z;
                 if (S0) a4 = *reinterpret_cast<float4 *>(s0 + off + c);
                 if (S1) b4 = *reinterpret_cast<float4 *>(s1 + off + c);
-                *reinterpret_cast<float4 *>(var + off + c) = update4<KIND, REG>(x4, g4, a4, b4, o, o.reg, racc);
+                *reinterpret_cast<float4 *>(var + off + c) = update4<KIND, REG>(x4, g4, a4, b4, o, os, o.reg, racc);
                 if (S0) *reinterpret_cast<float4 *>(s0 + off + c) = a4;
                 if (S1) *reinterpret_cast<float4 *>(s1 + off + c) = b4;
                 *reinterpret_cast<float4 *>(grad + off + c) = z;
@@ -454,7 +469,7 @@ __global__ void __launch_bounds__(256) kge_optim_lazy_kernel(float *__restrict__
     }
 }
 
-cudaError_t launch_optimizer_lazy(const OptimParams &o, float *table, float *grad, float *slot0, float *slot1,
+cudaError_t launch_optimizer_lazy(const OptimParams &o, const OptimStep &os, float *table, float *grad, float *slot0, float *slot1,
                                   long long rows, int ld, const int *row_stamp, int stamp, double *reg_loss,
                                   int sm_count, cudaStream_t st)
 {
@@ -462,12 +477,12 @@ cudaError_t launch_optimizer_lazy(const OptimParams &o, float *table, float *gra
     long long want = (rows + 255) / 256;  // 8 warps x 32 rows per block
     int grid = (int)(want < (long long)sm_count * 8 ? want : (long long)sm_count * 8);
     return dispatch_optimizer(o.kind, o.reg.p > 0, [&](auto kind, auto reg) {
-        kge_optim_lazy_kernel<kind, reg><<<grid, 256, 0, st>>>(table, grad, slot0, slot1, rows, ld, row_stamp, stamp, o, reg_loss);
+        kge_optim_lazy_kernel<kind, reg><<<grid, 256, 0, st>>>(table, grad, slot0, slot1, rows, ld, row_stamp, stamp, o, reg_loss, os);
         return cudaGetLastError();
     });
 }
 
-cudaError_t launch_optimizer(const OptimParams &o, float *table, float *grad, float *slot0, float *slot1,
+cudaError_t launch_optimizer(const OptimParams &o, const OptimStep &os, float *table, float *grad, float *slot0, float *slot1,
                              long long n_floats, double *reg_loss, int sm_count, cudaStream_t st)
 {
     long long n4 = n_floats / 4;  // ld is a multiple of 4
@@ -476,7 +491,7 @@ cudaError_t launch_optimizer(const OptimParams &o, float *table, float *grad, fl
     int grid = (int)(want < (long long)sm_count * 8 ? want : (long long)sm_count * 8);
     float4 *v = (float4 *)table, *g = (float4 *)grad, *a = (float4 *)slot0, *b = (float4 *)slot1;
     return dispatch_optimizer(o.kind, o.reg.p > 0, [&](auto kind, auto reg) {
-        kge_optim_kernel<kind, reg><<<grid, 256, 0, st>>>(v, g, a, b, n4, o, reg_loss);
+        kge_optim_kernel<kind, reg><<<grid, 256, 0, st>>>(v, g, a, b, n4, o, reg_loss, os);
         return cudaGetLastError();
     });
 }

@@ -41,8 +41,8 @@ __host__ __device__ __forceinline__ constexpr bool uses_slot0(int kind, float mo
 }
 __host__ __device__ __forceinline__ constexpr bool uses_slot1(int kind, float momentum, int centered)
 {
-    return kind == KGE_OPT_ADAM || kind == KGE_OPT_ADADELTA || kind == KGE_OPT_ADAMAX ||
-           (kind == KGE_OPT_RMSPROP && (centered != 0 || momentum != 0.f));
+    return kind == KGE_OPT_ADAM || kind == KGE_OPT_ADADELTA || kind == KGE_OPT_ADAMAX || kind == KGE_OPT_NADAM ||
+           kind == KGE_OPT_FTRL || (kind == KGE_OPT_RMSPROP && (centered != 0 || momentum != 0.f));
 }
 
 // One element of the legacy update rules (optimizers.py:255-291 -> tf.keras.optimizers.legacy.* and the training ops
@@ -63,8 +63,17 @@ __host__ __device__ __forceinline__ constexpr bool uses_slot1(int kind, float mo
 //             b = fma(rho, b, (1-rho)*(u*u))
 //   Adamax    a = fma(g - a, 1-b1, a); b = fmaxf(b2*b, |g|) (a NaN g is dropped, as fmaxf does);
 //             x = fma(-lr_t, a / (b + eps), x);  lr_t = lr/(1-b1^t), fp64 on the host, rounded once
+// Nadam and Ftrl round every operation on its own (no fma), as TensorFlow's separate ops (Nadam) and its CPU ApplyFtrl
+// expression evaluate them; q holds their per-step scalars (kge_api.cu, optim_step):
+//   Nadam     a = b1*a + (1-b1)*g; b = b2*b + (1-b2)*(g*g);
+//             mb = (1-m_t)*(g / (1-s_new)) + m_t1*(a / (1-s_next)); x -= (lr*mb) / (sqrt(b / v_den) + eps)
+//             row-decay mode, a row not looked up this step: a = b1*a, b = b2*b, x unchanged (nadam_decay)
+//   Ftrl      gs = g, or g + shrinkx2*x when l2_shrinkage > 0 (ApplyFtrlV2); n1 = a + g*g;
+//             P(y) = sqrt(y) when lr_power = -0.5, else powf(y, -lr_power);
+//             b += gs - ((P(n1) - P(a)) / lr)*x; x = |b| > l1 ? (sign(b)*l1 - b) / (P(n1)/lr + l2x2) : 0; a = n1
 template <int KIND>
-__device__ __forceinline__ void apply_rule(float &x, float gg, float &a, float &b, const OptimParams &o)
+__device__ __forceinline__ void apply_rule(float &x, float gg, float &a, float &b, const OptimParams &o,
+                                           const OptimStep &q)
 {
     if (KIND == KGE_OPT_ADAM) {
         a = fmaf(gg - a, 1.f - o.beta1, a);          // m += (g-m)(1-b1)
@@ -97,6 +106,20 @@ __device__ __forceinline__ void apply_rule(float &x, float gg, float &a, float &
         a = fmaf(gg - a, 1.f - o.beta1, a);
         b = fmaxf(__fmul_rn(o.beta2, b), fabsf(gg));
         x = fmaf(-o.lr_t, a / (b + o.eps), x);
+    } else if (KIND == KGE_OPT_NADAM) {
+        a = __fadd_rn(__fmul_rn(o.beta1, a), __fmul_rn(1.f - o.beta1, gg));
+        b = __fadd_rn(__fmul_rn(o.beta2, b), __fmul_rn(1.f - o.beta2, __fmul_rn(gg, gg)));
+        const float mb = __fadd_rn(__fmul_rn(q.one_m_mt, gg / q.one_m_snew), __fmul_rn(q.m_t1, a / q.one_m_snext));
+        x = __fsub_rn(x, __fmul_rn(o.lr, mb) / __fadd_rn(sqrtf(b / q.v_den), o.eps));
+    } else if (KIND == KGE_OPT_FTRL) {
+        const float gs = q.shrinkx2 > 0.f ? __fadd_rn(gg, __fmul_rn(q.shrinkx2, x)) : gg;
+        const float n1 = __fadd_rn(a, __fmul_rn(gg, gg));
+        const bool half = q.lr_power == -0.5f;
+        const float p1 = half ? sqrtf(n1) : powf(n1, -q.lr_power), p0 = half ? sqrtf(a) : powf(a, -q.lr_power);
+        b = __fadd_rn(b, __fsub_rn(gs, __fmul_rn(__fsub_rn(p1, p0) / o.lr, x)));
+        const float den = __fadd_rn(p1 / o.lr, q.l2x2);
+        x = fabsf(b) > q.l1 ? __fsub_rn(copysignf(q.l1, b), b) / den : 0.f;
+        a = n1;
     } else {  // SGD (momentum optional)
         if (o.momentum != 0.f) { a = fmaf(a, o.momentum, -__fmul_rn(gg, o.lr)); x += a; }
         else x = fmaf(-gg, o.lr, x);
@@ -105,7 +128,7 @@ __device__ __forceinline__ void apply_rule(float &x, float gg, float &a, float &
 
 template <int KIND, bool REG>
 __device__ __forceinline__ float4 update4(float4 x4, float4 g4, float4 &a4, float4 &b4, const OptimParams &o,
-                                          const RegParams &reg, float &racc)
+                                          const OptimStep &q, const RegParams &reg, float &racc)
 {
     float x[4] = {x4.x, x4.y, x4.z, x4.w}, g[4] = {g4.x, g4.y, g4.z, g4.w};
     float a[4] = {a4.x, a4.y, a4.z, a4.w}, b[4] = {b4.x, b4.y, b4.z, b4.w};
@@ -113,11 +136,18 @@ __device__ __forceinline__ float4 update4(float4 x4, float4 g4, float4 &a4, floa
     for (int e = 0; e < 4; ++e) {
         float gg = g[e];
         if (REG) gg += reg_grad(x[e], reg, &racc);
-        apply_rule<KIND>(x[e], gg, a[e], b[e], o);
+        apply_rule<KIND>(x[e], gg, a[e], b[e], o, q);
     }
     a4 = make_float4(a[0], a[1], a[2], a[3]);
     b4 = make_float4(b[0], b[1], b[2], b[3]);
     return make_float4(x[0], x[1], x[2], x[3]);
+}
+
+// Nadam's row-decay mode on a row that was not looked up: m *= b1, v *= b2
+__device__ __forceinline__ void nadam_decay4(float4 &a4, float4 &b4, const OptimParams &o)
+{
+    a4 = make_float4(__fmul_rn(o.beta1, a4.x), __fmul_rn(o.beta1, a4.y), __fmul_rn(o.beta1, a4.z), __fmul_rn(o.beta1, a4.w));
+    b4 = make_float4(__fmul_rn(o.beta2, b4.x), __fmul_rn(o.beta2, b4.y), __fmul_rn(o.beta2, b4.z), __fmul_rn(o.beta2, b4.w));
 }
 
 // block-reduce the per-thread regulariser loss and add it to the double accumulator
@@ -139,7 +169,8 @@ __device__ __forceinline__ void flush_reg_loss(float racc, double *reg_loss)
 template <class Launch>
 static cudaError_t dispatch_optimizer(int kind, bool reg, Launch &&launch)
 {
-    return dispatch_value<KGE_OPT_SGD, KGE_OPT_ADAM, KGE_OPT_ADAGRAD, KGE_OPT_RMSPROP, KGE_OPT_ADADELTA, KGE_OPT_ADAMAX>(
+    return dispatch_value<KGE_OPT_SGD, KGE_OPT_ADAM, KGE_OPT_ADAGRAD, KGE_OPT_RMSPROP, KGE_OPT_ADADELTA, KGE_OPT_ADAMAX,
+                          KGE_OPT_NADAM, KGE_OPT_FTRL>(
         kind, [&](auto k) { return reg ? launch(k, std::true_type{}) : launch(k, std::false_type{}); });
 }
 

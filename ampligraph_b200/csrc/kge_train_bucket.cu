@@ -302,7 +302,8 @@ __host__ __device__ constexpr int owner_warps(bool reg) { return reg ? 8 : 1; }
 // loads and stores; -DKGE_PROFILE_OWNER_NOWALK one that runs the epilogue on empty sums.  Together they attribute the
 // kernel's time to its two halves (DESIGN.md 5).  The default build sets neither.
 template <int HALVES, int NIT, int KIND, bool REG>
-__global__ void __launch_bounds__(32 * owner_warps(REG), 16 / owner_warps(REG)) kge_bucket_owner_kernel(const TrainParams p, const OwnerOptim x)
+__global__ void __launch_bounds__(32 * owner_warps(REG), 16 / owner_warps(REG)) kge_bucket_owner_kernel(const TrainParams p, const OwnerOptim x,
+                                                                                                             const OptimStep os)
 {
     const bool S0 = uses_slot0(KIND, x.o.momentum), S1 = uses_slot1(KIND, x.o.momentum, x.o.centered);
     const int lane = threadIdx.x & 31;
@@ -371,7 +372,7 @@ __global__ void __launch_bounds__(32 * owner_warps(REG), 16 / owner_warps(REG)) 
                     if (!w.live[it]) continue;
                     const uint32_t o = w.off[it] + (h ? w.hsB : 0u);
                     const float4 g = g4[h][it] + (h ? ai[it] : ar[it]);
-                    const float4 xn = update4<KIND, REG>(x4[h][it], g, a4[h][it], b4[h][it], op, op.reg, racc);
+                    const float4 xn = update4<KIND, REG>(x4[h][it], g, a4[h][it], b4[h][it], op, os, op.reg, racc);
                     __stcs(reinterpret_cast<float4 *>(xo + o), xn);
                     if (S0) __stcs(reinterpret_cast<float4 *>(m0 + o), a4[h][it]);
                     if (S1) __stcs(reinterpret_cast<float4 *>(m1 + o), b4[h][it]);
@@ -382,7 +383,7 @@ __global__ void __launch_bounds__(32 * owner_warps(REG), 16 / owner_warps(REG)) 
     if (REG && x.reg_loss) flush_reg_loss(racc, x.reg_loss);
 }
 
-cudaError_t launch_bucket_sum_optimizer(const TrainParams &p, int nit, const OptimParams &o, const float *in, float *out,
+cudaError_t launch_bucket_sum_optimizer(const TrainParams &p, int nit, const OptimParams &o, const OptimStep &os, const float *in, float *out,
                                         float *grad, float *slot0, float *slot1, long long rows, double *reg_loss,
                                         cudaStream_t st)
 {
@@ -391,7 +392,7 @@ cudaError_t launch_bucket_sum_optimizer(const TrainParams &p, int nit, const Opt
     return dispatch_optimizer(o.kind, o.reg.p > 0, [&](auto kind, auto reg) {
         constexpr int W = owner_warps(reg);
         return dispatch_trilinear_shape(p.model, nit, [&](auto halves, auto nits) {
-            kge_bucket_owner_kernel<halves, nits, decltype(kind)::value, decltype(reg)::value><<<(int)((rows + W - 1) / W), 32 * W, 0, st>>>(p, x);
+            kge_bucket_owner_kernel<halves, nits, decltype(kind)::value, decltype(reg)::value><<<(int)((rows + W - 1) / W), 32 * W, 0, st>>>(p, x, os);
             return cudaGetLastError();
         });
     });

@@ -40,14 +40,33 @@ def optimizer_slots(cfg):
     -> (initial value of slot 0, of slot 1), None for a slot the kind does not use."""
     O = _lib.OPTIMIZERS
     s0 = None if cfg.kind == O["sgd"] and cfg.momentum == 0.0 else 0.0
-    if cfg.kind == O["adagrad"]:
+    if cfg.kind in (O["adagrad"], O["ftrl"]):
         s0 = float(cfg.initial_accumulator_value)
-    s1 = 0.0 if (cfg.kind in (O["adam"], O["adadelta"], O["adamax"])
+    s1 = 0.0 if (cfg.kind in (O["adam"], O["adadelta"], O["adamax"], O["nadam"], O["ftrl"])
                  or (cfg.kind == O["rmsprop"] and (cfg.centered or cfg.momentum != 0.0))) else None
     return s0, s1
 
 
 RHO_DEFAULT = {"rmsprop": 0.9, "adadelta": 0.95}  # Keras legacy defaults; unused by the other kinds
+NADAM_DECAY_DEFAULT = 0.004  # Keras' legacy Nadam schedule_decay (stored as `decay`)
+
+
+def _pow32(a, b):
+    """fp32 a ** b, correctly rounded (up to an fp64 double rounding): TensorFlow's fp32 pow is within an ulp of it."""
+    return np.float32(float(np.float32(a)) ** float(np.float32(b)))
+
+
+def nadam_coefficients(beta_1, beta_2, decay, t, cache):
+    """The per-step scalars of Keras' legacy Nadam (_prepare_local) for step t (1-based: iterations + 1) with momentum
+    cache `cache` (1.0 before the first step), every operation in fp32 as TensorFlow forms them:
+    m_t = b1 (1 - 0.5 * 0.96^(decay t)), m_t1 = the same at t + 1, s_new = cache * m_t (the new cache),
+    s_next = s_new * m_t1, v_den = 1 - b2^t.  -> (m_t, m_t1, s_new, s_next, v_den), np.float32 each."""
+    f = np.float32
+    b1, d, one, half = f(beta_1), f(decay), f(1.0), f(0.5)
+    m_t = b1 * (one - half * _pow32(0.96, d * f(t)))
+    m_t1 = b1 * (one - half * _pow32(0.96, d * f(t + 1)))
+    s_new = f(cache) * m_t
+    return m_t, m_t1, s_new, s_new * m_t1, one - _pow32(beta_2, f(t))
 
 
 def one_vs_all_splits(B, n_ent):
@@ -316,8 +335,13 @@ class KGEEngine:
     def set_optimizer(self, name="adam", params=None, regularizer=None, lazy_tables=None):
         """name: a key of _lib.OPTIMIZERS, or 'lazy_<name>' (extension): update only the rows the step looked up
         (kge_optimizer_step_lazy) in both tables.  lazy_tables: None (the name decides) or a pair (entities, relations)
-        of bools that chooses the looked-up-rows rule per table, e.g. the reference's rule for Adamax with a regulariser
-        on the entities only (latent_features.optimizers.table_rules)."""
+        of bools that chooses the IndexedSlices rule per table, e.g. the reference's rule for Adamax with a regulariser
+        on the entities only (latent_features.optimizers.table_rules).  That rule is the looked-up-rows rule, except for
+        'nadam', whose IndexedSlices rule decays every row's m and v and moves the looked-up rows
+        (kge_optimizer_step_decay); 'lazy_nadam' is the looked-up-rows rule.  The per-table rule is
+        self.table_rules[key]: 'dense', 'rows' or 'decay'.  Hyper-parameters take Keras' names (Ftrl:
+        learning_rate_power, l1_regularization_strength, l2_regularization_strength,
+        l2_shrinkage_regularization_strength, beta, initial_accumulator_value; Nadam: decay or schedule_decay)."""
         name = name.lower()
         prefixed = name.startswith("lazy_")
         if prefixed:
@@ -327,10 +351,25 @@ class KGEEngine:
         lazy = (prefixed, prefixed) if lazy_tables is None else tuple(bool(x) for x in lazy_tables)
         assert len(lazy) == 2, "Incorrect length for lazy_tables. Expected 2, got {}".format(len(lazy))
         self.lazy_tables = {"ent": lazy[0], "rel": lazy[1]}
-        self.lazy = any(lazy)
+        self.table_rules = {key: "dense" if not v else "decay" if name == "nadam" and not prefixed else "rows"
+                            for key, v in self.lazy_tables.items()}
+        self.lazy = any(lazy)  # some table is not dense: the step stamps its looked-up rows
         p = dict(params or {})
         if name == "rmsprop" and p.get("centered") and float(p.get("momentum", 0.0)) != 0.0:
             raise NotImplementedError("centered RMSprop with momentum needs a third slot buffer (not supported)")
+        ftrl = {"lr_power": float(p.get("learning_rate_power", -0.5)),
+                "l1": float(p.get("l1_regularization_strength", 0.0)),
+                "l2": float(p.get("l2_regularization_strength", 0.0)),
+                "l2_shrinkage": float(p.get("l2_shrinkage_regularization_strength", 0.0)),
+                "ftrl_beta": float(p.get("beta", 0.0))}
+        if name == "ftrl":  # Keras' legacy Ftrl refuses the same values
+            if not ftrl["lr_power"] <= 0.0:
+                raise ValueError("learning_rate_power (%r) must be <= 0" % (ftrl["lr_power"],))
+            for key in ("l1", "l2", "l2_shrinkage"):
+                if not ftrl[key] >= 0.0:
+                    raise ValueError("%s regularization strength (%r) must be >= 0" % (key, ftrl[key]))
+            if not float(p.get("initial_accumulator_value", 0.1)) >= 0.0:
+                raise ValueError("initial_accumulator_value must be >= 0")
         regs = list(regularizer) if isinstance(regularizer, (list, tuple)) else [regularizer, regularizer]
         assert len(regs) == 2, "Incorrect length for regularizer. Expected 2, got {}".format(len(regs))
 
@@ -355,11 +394,14 @@ class KGEEngine:
                 float(p.get("momentum", 0.0)), float(p.get("initial_accumulator_value", 0.1)),
                 int(reg.get("p", 2)) if reg else 0, float(reg.get("lambda", 1e-5)),
                 int(reg.get("p2", 0)) if reg else 0, float(reg.get("lambda2", 0.0)),
-                float(p.get("rho", RHO_DEFAULT.get(name, 0.0))), int(bool(p.get("centered", False))))
+                float(p.get("rho", RHO_DEFAULT.get(name, 0.0))), int(bool(p.get("centered", False))), **ftrl)
         self.opt_cfgs = {"ent": cfg_for(regs[0]), "rel": cfg_for(regs[1])}
         self.opt_cfg = self.opt_cfgs["ent"]  # hyper-parameters are common to both tables; only the regulariser differs
         self.opt_name = name
         self.t = 0
+        # Nadam's momentum cache (fp32, Keras' m_cache) and schedule decay; begin_step advances the cache
+        self.nadam_decay = float(p.get("decay", p.get("schedule_decay", NADAM_DECAY_DEFAULT)))
+        self.nadam_cache = np.float32(1.0)
         # slots as [ent | rel] blocks, like the tables (see __init__): slots[key] are row slices of them
         mk = lambda v: None if v is None else torch.full((self.ent_rows + self.n_rel, self.ld), v, dtype=torch.float32,
                                                          device=self.device)
@@ -373,6 +415,35 @@ class KGEEngine:
                            "rel": torch.zeros(self.n_rel, dtype=torch.int32, device=self.device)}
         _lib.check(self.lib.kge_set_row_stamps(self.h, _ptr(self.stamps["ent"]), _ptr(self.stamps["rel"])))
         self._last_step = 0
+
+    def begin_step(self):
+        """Start an optimizer step: self.t += 1 and, for Nadam, advance the momentum cache and write the step's
+        nadam_coefficients into both tables' configs -- formed once per step for both tables, as Keras' _prepare_local
+        is.  Every caller of the kge_optimizer_step* entry points calls it once before them.  Returns what undo_step
+        needs to take the step back.
+        The configs must still be of the engine's optimizer: the slots were allocated and initialised for it and the
+        per-step state follows it (a config switched to Nadam behind set_optimizer's back would run with no momentum
+        schedule), so a config whose kind was changed is refused with ValueError before anything runs."""
+        want = _lib.OPTIMIZERS[self.opt_name]
+        for key, cfg in self.opt_cfgs.items():
+            if cfg.kind != want:
+                raise ValueError("the %s table's optimizer config has kind %d, not the engine's %r (%d): change the "
+                                 "optimizer with set_optimizer" % (key, cfg.kind, self.opt_name, want))
+        undo = (self.t, self.nadam_cache)
+        self.t += 1
+        if self.opt_name == "nadam":
+            c = self.opt_cfg
+            m_t, m_t1, s_new, s_next, v_den = nadam_coefficients(c.beta_1, c.beta_2, self.nadam_decay, self.t,
+                                                                 self.nadam_cache)
+            self.nadam_cache = s_new
+            for cfg in self.opt_cfgs.values():
+                cfg.nadam_m_t, cfg.nadam_m_t1, cfg.nadam_s_new, cfg.nadam_s_next, cfg.nadam_v_den = (
+                    m_t, m_t1, s_new, s_next, v_den)
+        return undo
+
+    def undo_step(self, undo):
+        """Take back a begin_step whose optimizer call was refused (nothing ran)."""
+        self.t, self.nadam_cache = undo
 
     # -- tables ------------------------------------------------------------
     def ensure_row_stash(self, B):
@@ -611,7 +682,7 @@ class KGEEngine:
         becomes the current one: self.ent / self.rel are re-sliced from it, and the block they viewed before is
         overwritten by the next deferred step.  Read self.ent / self.rel (or get_embeddings()) after the step; do not
         hold them across steps."""
-        self.t += 1
+        undo = self.begin_step()
         if self._deferred:
             # the pending replaced-row sum and the optimizer in one launch: it reads the current block and writes every
             # element of the other one, which becomes the current block (ent / rel are re-sliced from it)
@@ -623,7 +694,7 @@ class KGEEngine:
                 _ptr(self._gblock), _ptr(self._sblocks[0]), _ptr(self._sblocks[1]), rows,
                 C.c_void_p(self.loss_acc.data_ptr() + 8), self._stream())
             if rc == _lib.KGE_ERR_INVALID_ARGUMENT:
-                self.t -= 1  # arguments refused: nothing ran, and the step stays pending in the library too
+                self.undo_step(undo)  # arguments refused: nothing ran, and the step stays pending in the library too
             else:
                 self._deferred = False  # the library consumed the pending sum, whether or not its launch succeeded
             _lib.check(rc)
@@ -640,7 +711,12 @@ class KGEEngine:
         for key, table, grad, rows in (("ent", self.ent, self.g_ent, self.ent_rows),
                                        ("rel", self.rel, self.g_rel, self.n_rel)):
             s0, s1 = self.slots[key]
-            if self.lazy_tables[key]:
+            if self.table_rules[key] == "decay":
+                _lib.check(self.lib.kge_optimizer_step_decay(
+                    self.h, C.byref(self.opt_cfgs[key]), self.t, _ptr(table), _ptr(grad), _ptr(s0), _ptr(s1), rows,
+                    _ptr(self.stamps[key]), self.lib.kge_step_stamp(self._last_step), self._stream()))
+                continue
+            if self.table_rules[key] == "rows":
                 _lib.check(self.lib.kge_optimizer_step_lazy(
                     self.h, C.byref(self.opt_cfgs[key]), self.t, _ptr(table), _ptr(grad), _ptr(s0), _ptr(s1), rows,
                     _ptr(self.stamps[key]), self.lib.kge_step_stamp(self._last_step),

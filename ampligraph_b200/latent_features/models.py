@@ -931,9 +931,11 @@ class ScoringBasedEmbeddingModel:
         self.engine.rel.copy_(snapshot[1])
 
     def save_weights(self, filepath):
-        """Tables + optimizer slots + indexer in one pickle (the reference's Keras format is TF-specific)."""
+        """Tables + optimizer slots and state (step count, Nadam's momentum cache) + indexer in one pickle (the
+        reference's Keras format is TF-specific)."""
         ent, rel = self.engine.get_embeddings()
         state = {"ent": ent.cpu().numpy(), "rel": rel.cpu().numpy(), "t": self.engine.t, "step": self._step,
+                 "nadam_cache": float(getattr(self.engine, "nadam_cache", 1.0)),
                  "slots": {k: [None if s is None else s.cpu().numpy() for s in v] for k, v in self.engine.slots.items()},
                  "indexer": self.data_indexer, "max_ent_size": self.max_ent_size, "max_rel_size": self.max_rel_size,
                  "reciprocal_relations": self.reciprocal_relations}
@@ -953,6 +955,8 @@ class ScoringBasedEmbeddingModel:
         self._build_engine()
         self.engine.set_embeddings(state["ent"], state["rel"])
         self.engine.t, self._step = state["t"], state["step"]
+        # Nadam's momentum cache (an fp32 value, exact as a float); files written before Nadam have none
+        self.engine.nadam_cache = np.float32(state.get("nadam_cache", 1.0))
         for k, v in state["slots"].items():
             for n, s in enumerate(v):
                 if s is not None:

@@ -178,7 +178,7 @@ class DataParallelTrainer:
             eng.apply_gradients()
         else:
             C, _lib = self._C, self._lib
-            eng.t += 1
+            eng.begin_step()
             self._k += 1
             lo, hi = self.shard
             s0, s1 = self.slots
@@ -342,7 +342,7 @@ class ShardedTrainer:
         mark()
         self.barrier(0)  # every rank's scatters (into my shard too) and relation gradients are complete
         mark()
-        eng.t += 1
+        eng.begin_step()
         s0, s1 = eng.slots["ent"]
         if self.lazy:
             _lib.check(eng.lib.kge_optimizer_step_lazy(eng.h, C.byref(eng.opt_cfgs["ent"]), eng.t, p(eng.ent), p(eng.g_ent), p(s0), p(s1),

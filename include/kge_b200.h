@@ -71,7 +71,9 @@ enum kge_optimizer {
     KGE_OPT_ADAGRAD = 2,
     KGE_OPT_RMSPROP = 3,
     KGE_OPT_ADADELTA = 4,
-    KGE_OPT_ADAMAX = 5
+    KGE_OPT_ADAMAX = 5,
+    KGE_OPT_NADAM = 6,
+    KGE_OPT_FTRL = 7
 };
 /* the element of (s, p, o) a ranking / top-k call replaces by its candidates: subject or object (entity rows), or the
  * relation (KGE_SIDE_P, relation prediction: candidates are relation rows, see kge_rank) */
@@ -119,7 +121,8 @@ typedef struct kge_config {
                               filter -- a testing knob for its overflow fallback */
 } kge_config;
 
-/* optimizers.get (optimizers.py:255-291) -> tf.keras.optimizers.legacy.{SGD,Adam,Adagrad,RMSprop,Adadelta,Adamax};
+/* optimizers.get (optimizers.py:255-291) -> tf.keras.optimizers.legacy.{SGD,Adam,Adagrad,RMSprop,Adadelta,Adamax,Nadam,
+ * Ftrl};
  * regularizers.LP_regularizer (regularizers.py:14-37) folded into the update.
  * What the two slot buffers of the optimizer calls (slot0 / slot1, [rows, ld], zero-initialised unless noted) hold:
  *   SGD       momentum accumulator (only with momentum != 0) / -
@@ -129,8 +132,15 @@ typedef struct kge_config {
  *             (centered with momentum needs a third slot: refused, KGE_ERR_UNSUPPORTED)
  *   Adadelta  accum / accum_update
  *   Adamax    m / v (the exponentially weighted infinity norm)
- * A config whose struct_size stops before `rho` (the layout before RMSprop, Adadelta and Adamax) is accepted for the
- * first three kinds; its rho and centered read as 0. */
+ *   Nadam     m / v
+ *   Ftrl      accumulator n (initial_accumulator_value) / linear term z
+ * Two older layouts are accepted for the kinds they knew; their missing fields read as 0: a config whose struct_size
+ * stops before `rho` (the layout before RMSprop, Adadelta and Adamax) for the first three kinds, and one that stops
+ * before `l1` (the layout before Nadam and Ftrl) for the first six.
+ * Nadam's per-step scalars are the caller's: before each step t (1-based) it forms, in fp32 as Keras' legacy Nadam
+ * does (_prepare_local), m_t = b1 (1 - 0.5 * 0.96^(decay t)), m_t1 = b1 (1 - 0.5 * 0.96^(decay (t + 1))), advances its
+ * momentum cache c (1.0 before the first step) to s_new = c * m_t, and sets s_next = s_new * m_t1 and
+ * v_den = 1 - b2^t; the same values serve both tables of the step (DESIGN.md 3.3). */
 typedef struct kge_optimizer_config {
     int32_t struct_size;
     int32_t kind;         /* enum kge_optimizer */
@@ -145,6 +155,16 @@ typedef struct kge_optimizer_config {
     float reg_lambda2;
     float rho;            /* RMSprop: 0.9, Adadelta: 0.95 */
     int32_t centered;     /* RMSprop: 0 */
+    float l1;             /* Ftrl l1_regularization_strength: 0 */
+    float l2;             /* Ftrl l2_regularization_strength: 0 */
+    float l2_shrinkage;   /* Ftrl l2_shrinkage_regularization_strength: 0 (> 0: ApplyFtrlV2) */
+    float lr_power;       /* Ftrl learning_rate_power: -0.5 */
+    float ftrl_beta;      /* Ftrl beta: 0 (the rule uses l2 + beta / (2 learning_rate)) */
+    float nadam_m_t;      /* Nadam, this step's m_t, m_t1, s_new, s_next and v_den (see above) */
+    float nadam_m_t1;
+    float nadam_s_new;
+    float nadam_s_next;
+    float nadam_v_den;
 } kge_optimizer_config;
 
 const char *kge_last_error(void);
@@ -466,6 +486,16 @@ int32_t kge_step_stamp(uint64_t step);
 int kge_optimizer_step_lazy(kge_handle *h, const kge_optimizer_config *opt, int64_t t, float *table_dev,
                             float *grad_dev, float *slot0_dev, float *slot1_dev, int64_t rows,
                             const int32_t *row_stamp_dev, int32_t stamp, double *reg_loss_dev, void *stream);
+/* Nadam's rule on an IndexedSlices gradient (Keras' legacy Nadam, _resource_apply_sparse), the reference's rule for a
+ * Nadam table without a regulariser: one dense pass in which EVERY row's m and v decay (m *= b1, v *= b2) and only the
+ * rows stamped kge_step_stamp(step) add their gradient terms and move, as kge_optimizer_step moves every row (a stamped
+ * row whose summed gradient is exactly 0 still moves; an unstamped row with m != 0 does not).  Unstamped rows' table
+ * and gradient rows are not read or written (their gradient is 0 by the stamping contract).  KGE_ERR_UNSUPPORTED for
+ * any other kind; KGE_ERR_INVALID_ARGUMENT for a config with a regulariser (a regularised table's gradient is dense:
+ * kge_optimizer_step) and for the pointers kge_optimizer_step_lazy refuses. */
+int kge_optimizer_step_decay(kge_handle *h, const kge_optimizer_config *opt, int64_t t, float *table_dev,
+                             float *grad_dev, float *slot0_dev, float *slot1_dev, int64_t rows,
+                             const int32_t *row_stamp_dev, int32_t stamp, void *stream);
 
 /* Data-parallel variant of kge_optimizer_step FUSED with the gradient exchange over NVLink peer
  * memory (the reference has no distributed path; SURVEY.md 8e asks for replicated tables + a

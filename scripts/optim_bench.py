@@ -4,10 +4,12 @@
   kge_optimizer_step           the dense rule over the whole block (one launch)
   kge_optimizer_step_deferred  the owner-per-row kernel: a deferred step's replaced-row sum + the dense rule
                                (27,212 Zipf positives, eta 10, as bench.py), timed alone
+  kge_optimizer_step_decay     Nadam's IndexedSlices rule over the whole block with half of the rows stamped: the
+                               unstamped half moves only m and v (4 streams, plus the row stamps)
 
 Achieved GB/s counts the algorithmic streams of the dense rule, from shapes: per element the parameter and the gradient
 (read, then written / zeroed) and every slot the kind uses (read and written) -- 6 fp32 streams for one-slot RMSprop, 8 for
-the two-slot kinds and Adam.  The owner kernel also reads the bucket entries and their rows; its GB/s counts the same
+the two-slot kinds (Nadam and Ftrl among them) and Adam.  The owner kernel also reads the bucket entries and their rows; its GB/s counts the same
 streams, so it understates that kernel's traffic.
 
   python scripts/optim_bench.py [--iters 200] [--warmup 20]
@@ -27,7 +29,8 @@ from ampligraph_b200 import _lib  # noqa: E402
 from ampligraph_b200.engine import KGEEngine, optimizer_slots  # noqa: E402
 
 KINDS = [("adam", {}), ("rmsprop", {}), ("rmsprop", {"centered": True}), ("rmsprop", {"momentum": 0.9}),
-         ("adadelta", {"learning_rate": 1.0}), ("adamax", {})]
+         ("adadelta", {"learning_rate": 1.0}), ("adamax", {}), ("nadam", {}), ("ftrl", {}),
+         ("ftrl", {"learning_rate_power": -0.25})]
 E, R, K, ETA, B = 14505, 237, 200, 10, 27212
 
 
@@ -97,7 +100,7 @@ def main():
         ptr = lambda x: C.c_void_p(x.data_ptr()) if x is not None else None
 
         def dense():
-            eng.t += 1
+            eng.begin_step()
             _lib.check(eng.lib.kge_optimizer_step(eng.h, C.byref(eng.opt_cfg), eng.t, ptr(eng._pblock), ptr(eng._gblock),
                                                   ptr(eng._sblocks[0]), ptr(eng._sblocks[1]), rows, None, eng._stream()))
         us = time_calls(dense, args.iters, args.warmup)
@@ -114,6 +117,18 @@ def main():
         us = time_calls(eng.apply_gradients, args.iters, args.warmup, before=pend)
         print(json.dumps({"kernel": "kge_optimizer_step_deferred", "kind": label, "us": round(us, 2), "streams": streams,
                           "GB_per_s": round(nbytes / us / 1e3, 1)}))
+        if name == "nadam":
+            stamps = torch.as_tensor(np.where(rng.random(rows) < 0.5, 1, 0).astype(np.int32)).cuda()
+
+            def decay():
+                eng.begin_step()
+                _lib.check(eng.lib.kge_optimizer_step_decay(eng.h, C.byref(eng.opt_cfg), eng.t, ptr(eng._pblock),
+                                                            ptr(eng._gblock), ptr(eng._sblocks[0]), ptr(eng._sblocks[1]),
+                                                            rows, ptr(stamps), 1, eng._stream()))
+            us = time_calls(decay, args.iters, args.warmup)
+            dbytes = rows * ld * 4 * 6 + rows * 4  # half the rows 8 streams, half 4, and the stamps
+            print(json.dumps({"kernel": "kge_optimizer_step_decay", "kind": label, "us": round(us, 2), "streams": 6,
+                              "GB_per_s": round(dbytes / us / 1e3, 1)}))
         eng.close()
 
 

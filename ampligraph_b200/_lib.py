@@ -140,6 +140,7 @@ PROTOTYPES = {
     "kge_k_vs_all_workspace_bytes": (C.c_int64, [_P, C.c_int64]),
     "kge_k_vs_all_step": (C.c_int, [_P, C.c_int32, C.c_int32, C.c_float, _P, _P, _P, _P, _P, C.c_int64, _P, _P, C.c_uint64,
                                     _P, _P, C.c_int64, _P]),
+    "kge_set_embedding_dropout": (C.c_int, [_P, C.c_float, C.c_float, C.c_uint64]),
     "kge_n3_workspace_bytes": (C.c_int64, [_P]),
     "kge_n3_step": (C.c_int, [_P, C.c_float, C.c_float, _P, _P, _P, _P, _P, C.c_int64, C.c_uint64, _P, _P, C.c_int64,
                               _P]),

@@ -48,6 +48,9 @@ struct kge_handle {
     // KGE_STEP_FUSED_DEFER: the step whose replaced-row sum waits in the workspace for kge_optimizer_step_deferred
     bool sum_pending;
     TrainParams pending;
+    // kge_set_embedding_dropout: the all-candidate steps' embedding dropout (both 0: none)
+    float drop_p_ent, drop_p_rel;
+    uint64_t drop_seed;
 };
 
 // Make the handle's device current for the duration of an entry point (ADVICE r1: two handles on different GPUs
@@ -518,6 +521,17 @@ extern "C" int kge_set_train_workspace(kge_handle *h, void *ws_dev, int64_t byte
     return KGE_OK;
 }
 
+static bool dropout_set(const kge_handle *h) { return h->drop_p_ent != 0.f || h->drop_p_rel != 0.f; }
+
+// The sampled steps' fused kernels read the raw rows: they refuse while embedding dropout is set
+static int check_no_dropout(const kge_handle *h, const char *fn)
+{
+    if (!dropout_set(h)) return KGE_OK;
+    return fail(KGE_ERR_UNSUPPORTED, "%s: embedding dropout is set (kge_set_embedding_dropout), and the sampled training "
+                                     "kernels do not apply it: it applies to kge_one_vs_all_step, "
+                                     "kge_one_vs_all_relation_step and kge_k_vs_all_step; clear it with (0, 0)", fn);
+}
+
 static int train_step_impl(kge_handle *h, int32_t mode, const kge_shard_map *map, const float *ent_dev,
                            const float *rel_dev, float *grad_ent_dev, float *grad_rel_dev,
                            const int32_t *triples_dev, int64_t B, const int32_t *neg_ent_dev,
@@ -526,6 +540,7 @@ static int train_step_impl(kge_handle *h, int32_t mode, const kge_shard_map *map
                            const float *dneg_dev, void *stream)
 {
     KGE_CHECK_HANDLE(h, "kge_train_step");
+    if (int rc = check_no_dropout(h, map ? "kge_train_step_sharded" : "kge_train_step")) return rc;
     if (mode < KGE_STEP_FUSED || mode > KGE_STEP_FUSED_DEFER)
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_train_step: unknown mode %d", mode);
     if (int rc = check_no_pending(h, "kge_train_step")) return rc;
@@ -1656,6 +1671,7 @@ static const CandidateRule K_VS_ALL = {"kge_k_vs_all_step", "KvsAll", "kge_k_vs_
 struct CandidateQueries {
     float *qs, *qo;
     int32_t *qpos;
+    SideDropout drop;  // drop.cand / drop.grad_cand: the dropout regions while dropout is set, else nullptr
 };
 
 // Carve-up of the workspace of a step of s.B queries into the query vectors and the scratch of s's passes: the row
@@ -1682,6 +1698,11 @@ static CandidateQueries carve_candidates(const kge_handle *h, const CandidateRul
     }
     s.pgq = c.take<float>(ns * rows, 16);
     if (s.xsplit > 1) s.pgx = c.take<float>((size_t)s.xsplit * s.n_cand * h->L.ld * sizeof(float), 16);
+    if (dropout_set(h)) {  // one side at a time: its dropped candidate table and their gradient (kge_dropout.cu)
+        const size_t table = (size_t)s.n_cand * h->L.ld * sizeof(float);
+        q.drop.cand = c.take<float>(table, 16);
+        q.drop.grad_cand = c.take<float>(table, 16);
+    }
     return q;
 }
 
@@ -1754,14 +1775,22 @@ static int check_candidate_step(const kge_handle *h, const CandidateRule &r, con
 
 // What every checked all-candidate step does before its passes: set the loss weight of the reduction, carve the
 // workspace ws into s and *q, write the entity sides' query vectors, and stamp every candidate row as looked up
-static int start_candidate_step(const kge_handle *h, const CandidateRule &r, int32_t reduction, void *ws, cudaStream_t st,
-                                OneVsAllSide &s, CandidateQueries *q)
+static int start_candidate_step(const kge_handle *h, const CandidateRule &r, int32_t reduction, void *ws, uint64_t step,
+                                cudaStream_t st, OneVsAllSide &s, CandidateQueries *q)
 {
     // mean: a negative's exp weighs 1 / (n_cand - 1) in the multiclass loss, every element 1 / n_ent in KvsAll's
     s.w = reduction == KGE_REDUCE_MEAN ? (float)(1.0 / (double)(r.multiclass ? s.n_cand - 1 : s.n_cand)) : 1.f;
     Carve c(ws);
     *q = carve_candidates(h, r, c, s);
-    if (!r.relation) {
+    if (dropout_set(h)) {  // launch_dropout_prepare forms each side's queries from its dropped rows
+        // keep iff (word >> 8) >= round(p 2^24); scale = fp32(1 / (1 - p))
+        q->drop.seed = h->drop_seed;
+        q->drop.step = step;
+        q->drop.t_ent = (uint32_t)llround((double)h->drop_p_ent * 16777216.0);
+        q->drop.t_rel = (uint32_t)llround((double)h->drop_p_rel * 16777216.0);
+        q->drop.scale_ent = (float)(1.0 / (1.0 - (double)h->drop_p_ent));
+        q->drop.scale_rel = (float)(1.0 / (1.0 - (double)h->drop_p_rel));
+    } else if (!r.relation) {
         ShardView sv;
         memset(&sv, 0, sizeof(sv));
         KGE_CUDA(launch_rank_prepare(h->L, sv, s.ent, s.rel, nullptr, s.triples, s.B, h->score_scale, q->qs, q->qo, nullptr,
@@ -1796,13 +1825,13 @@ extern "C" int kge_one_vs_all_step(kge_handle *h, int32_t sides, int32_t loss_re
     if (B == 0) return KGE_OK;
     cudaStream_t st = (cudaStream_t)stream;
     CandidateQueries q;
-    if (int rc = start_candidate_step(h, ONE_VS_ALL, loss_reduction, ws_dev, st, s, &q)) return rc;
+    if (int rc = start_candidate_step(h, ONE_VS_ALL, loss_reduction, ws_dev, step, st, s, &q)) return rc;
     for (int side = KGE_SIDE_S; side <= KGE_SIDE_O; ++side) {
         if (!(sides & (side == KGE_SIDE_S ? KGE_ONE_VS_ALL_S : KGE_ONE_VS_ALL_O))) continue;
         s.side = side;
         s.col = side == KGE_SIDE_S ? 0 : 2;
         s.q = side == KGE_SIDE_S ? q.qs : q.qo;
-        KGE_CUDA(launch_one_vs_all_side(s, h->L.halves, st), "kge_one_vs_all_step");
+        KGE_CUDA(launch_one_vs_all_side(s, h->L.halves, st, q.drop.cand ? &q.drop : nullptr), "kge_one_vs_all_step");
     }
     return KGE_OK;
 }
@@ -1830,12 +1859,13 @@ extern "C" int kge_one_vs_all_relation_step(kge_handle *h, float weight, int32_t
     if (B == 0) return KGE_OK;
     cudaStream_t st = (cudaStream_t)stream;
     CandidateQueries q;
-    if (int rc = start_candidate_step(h, RELATION_PREDICTION, loss_reduction, ws_dev, st, s, &q)) return rc;
+    if (int rc = start_candidate_step(h, RELATION_PREDICTION, loss_reduction, ws_dev, step, st, s, &q)) return rc;
     s.side = KGE_SIDE_P;
     s.col = 1;
     s.q = q.qs;
     s.weight = weight;
-    KGE_CUDA(launch_relation_prediction_side(s, q.qs, h->L.halves, st), "kge_one_vs_all_relation_step");
+    KGE_CUDA(launch_relation_prediction_side(s, q.qs, h->L.halves, st, q.drop.cand ? &q.drop : nullptr),
+             "kge_one_vs_all_relation_step");
     return KGE_OK;
 }
 
@@ -1866,7 +1896,7 @@ extern "C" int kge_k_vs_all_step(kge_handle *h, int32_t side, int32_t loss_reduc
     if (B == 0) return KGE_OK;
     cudaStream_t st = (cudaStream_t)stream;
     CandidateQueries q;
-    if (int rc = start_candidate_step(h, K_VS_ALL, loss_reduction, ws_dev, st, s, &q)) return rc;
+    if (int rc = start_candidate_step(h, K_VS_ALL, loss_reduction, ws_dev, step, st, s, &q)) return rc;
     s.side = side == KGE_ONE_VS_ALL_S ? KGE_SIDE_S : KGE_SIDE_O;
     s.col = side == KGE_ONE_VS_ALL_S ? 0 : 2;
     s.q = side == KGE_ONE_VS_ALL_S ? q.qs : q.qo;
@@ -1874,7 +1904,21 @@ extern "C" int kge_k_vs_all_step(kge_handle *h, int32_t side, int32_t loss_reduc
     s.label_ids = label_ids_dev;
     s.y0 = (float)((double)label_smoothing / (double)h->cfg.n_ent);
     s.y1 = (float)(1.0 - (double)label_smoothing);
-    KGE_CUDA(launch_k_vs_all_side(s, h->L.halves, st), "kge_k_vs_all_step");
+    KGE_CUDA(launch_k_vs_all_side(s, h->L.halves, st, q.drop.cand ? &q.drop : nullptr), "kge_k_vs_all_step");
+    return KGE_OK;
+}
+
+// Embedding dropout of the three all-candidate steps (kge_dropout.cu; DESIGN.md 3.19).  Allowed while a deferred
+// step is pending: it only changes what the next all-candidate step computes.
+extern "C" int kge_set_embedding_dropout(kge_handle *h, float p_ent, float p_rel, uint64_t seed)
+{
+    if (!h) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_set_embedding_dropout: null handle");
+    if (!(p_ent >= 0.f && p_ent < 1.f) || !(p_rel >= 0.f && p_rel < 1.f))
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_set_embedding_dropout: p_ent and p_rel must be in [0, 1), got %g and %g",
+                    (double)p_ent, (double)p_rel);
+    h->drop_p_ent = p_ent == 0.f ? 0.f : p_ent;  // -0 clears too
+    h->drop_p_rel = p_rel == 0.f ? 0.f : p_rel;
+    h->drop_seed = seed;
     return KGE_OK;
 }
 

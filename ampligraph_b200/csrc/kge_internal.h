@@ -138,17 +138,38 @@ struct OneVsAllSide {
     const int32_t *label_ids;
     float y0, y1;
 };
+// kge_dropout.cu: embedding dropout of one side of an all-candidate step (kge_set_embedding_dropout; DESIGN.md 3.19).
+// Element c of row `row` under stream tag `tag` takes word c & 3 of philox4x32_10((row, (c >> 2) | (0x80 | tag) << 24,
+// step_lo, step_hi), (seed_lo, seed_hi)) and is kept iff (word >> 8) >= t; a kept element is fp32(x * scale), a
+// dropped one +0.  tag = 4 side + role: role 0 the candidate rows (row = table row), 1 + j the query's triple column j
+// (row = batch position).
+struct SideDropout {
+    uint64_t seed, step;
+    uint32_t t_ent, t_rel;    // keep thresholds of the entity and relation rows (0: keep every element)
+    float scale_ent, scale_rel;
+    float *cand;              // [n_cand, ld] workspace: the side's dropped candidate table
+    float *grad_cand;         // [n_cand, ld] workspace: the candidates' gradient wrt their dropped copies
+};
+// Writes the dropped candidate table, zeroes grad_cand, writes q[b] from the dropped query rows, and points s.cand,
+// s.grad_cand and s.q at them (s.side, s.triples, s.ent, s.rel set; s.cand / s.grad_cand still the raw rows)
+cudaError_t launch_dropout_prepare(OneVsAllSide &s, const SideDropout &d, float *q, int halves, cudaStream_t st);
+// After the dX pass: adds scale * m times grad_cand to the raw candidate gradient rows, then runs the chain pass on the
+// dropped query rows, with each row's own mask on the gradient it adds
+cudaError_t launch_dropout_finish(const OneVsAllSide &s, const SideDropout &d, int halves, cudaStream_t st);
+
 int one_vs_all_splits(long long B, long long n_ent);
 size_t one_vs_all_smem_bytes(int ld);  // dynamic shared memory of the dQ and dX passes
 size_t k_vs_all_smem_bytes(int ld);    // the same with KvsAll's label masks
-cudaError_t launch_one_vs_all_side(const OneVsAllSide &s, int halves, cudaStream_t st);
+// drop: the side's embedding dropout, or nullptr (the passes read the raw tables)
+cudaError_t launch_one_vs_all_side(const OneVsAllSide &s, int halves, cudaStream_t st, const SideDropout *drop = nullptr);
 // one side of a KvsAll multi-label step (kge_k_vs_all_step): s.triples are the [B, 3] queries, s.label_* set
-cudaError_t launch_k_vs_all_side(const OneVsAllSide &s, int halves, cudaStream_t st);
+cudaError_t launch_k_vs_all_side(const OneVsAllSide &s, int halves, cudaStream_t st, const SideDropout *drop = nullptr);
 cudaError_t launch_one_vs_all_stamps(int *stamp_ent, long long n_ent, int stamp, cudaStream_t st);
 // relation prediction as a 1vsAll side (kge_one_vs_all_relation_step): s.side = KGE_SIDE_P, s.cand = rel, s.n_cand =
 // n_rel, s.q = qp; writes qp[b] = Qp(s_b, o_b) = d f(s_b, p, o_b) / dp, then runs the 1vsAll passes with dX split
 // s.xsplit ways over the query tiles (partials in s.pgx), and a chain pass that adds d/ds and d/do to grad_ent
-cudaError_t launch_relation_prediction_side(const OneVsAllSide &s, float *qp, int halves, cudaStream_t st);
+cudaError_t launch_relation_prediction_side(const OneVsAllSide &s, float *qp, int halves, cudaStream_t st,
+                                            const SideDropout *drop = nullptr);
 
 // kge_reg_n3.cu: the N3 regulariser of a step's positives (kge_n3_step)
 struct N3Params {

@@ -21,6 +21,9 @@
 //          query row forms the gradient rows of the positive's kept rows -- side o: d/ds = Q0(p, Gq), d/dp of f(s, p, Gq);
 //          side s: d/do = Q1(Gq, p), d/dp of f(Gq, p, o) -- with the training kernels' own arithmetic
 //          (kge_train_common.cuh), added with red.global.add like theirs.
+// With embedding dropout (kge_dropout.cu; DESIGN.md 3.19) the passes read the side's dropped candidate table and the
+// queries of its dropped query rows; dX adds into a zeroed workspace table that is masked into grad_cand afterwards, and
+// kge_dropout.cu's chain pass replaces the one here.
 // Every pass scores a (query, entity) pair with the same chain: one fma per column in ascending order, so the logits
 // of the three passes that form them are bit-identical.
 //
@@ -529,7 +532,8 @@ __global__ void kge_ova_stamp_kernel(int *stamps, long long n, int stamp)
 
 // the dQ, dX and chain passes of one side under the per-element rule Rule (smem: dynamic bytes of dQ and dX)
 template <class Rule>
-static cudaError_t launch_grad_passes(const OneVsAllSide &s, int halves, size_t smem, cudaStream_t st)
+static cudaError_t launch_grad_passes(const OneVsAllSide &s, int halves, size_t smem, cudaStream_t st,
+                                      const SideDropout *drop)
 {
     const unsigned n_qt = (unsigned)((s.B + OVA_T - 1) / OVA_T), n_et = (unsigned)((s.n_cand + OVA_T - 1) / OVA_T);
     cudaError_t e;
@@ -540,6 +544,7 @@ static cudaError_t launch_grad_passes(const OneVsAllSide &s, int halves, size_t 
         kge_ova_dx_sum_kernel<<<(unsigned)((s.n_cand * (s.ld / 4) + 255) / 256), 256, 0, st>>>(s);
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
     }
+    if (drop) return launch_dropout_finish(s, *drop, halves, st);  // masked candidate rows, then the dropout chain pass
     const unsigned grid = (unsigned)((s.B * (s.kp / 4) + 255) / 256);
     const bool rel = s.side == KGE_SIDE_P;
     if (halves == 2) {
@@ -571,20 +576,26 @@ __global__ void __launch_bounds__(256) kge_ova_relation_query_kernel(const OneVs
     if (HALVES == 2) f4st(q + di, trilinear_grad_p<HALVES, 1>(z, z, orr, oim, sr, sim, z, z));
 }
 
-cudaError_t launch_one_vs_all_side(const OneVsAllSide &s, int halves, cudaStream_t st)
+// With dropout the side's passes read its dropped candidate table and queries (launch_dropout_prepare)
+cudaError_t launch_one_vs_all_side(const OneVsAllSide &s_, int halves, cudaStream_t st, const SideDropout *drop)
 {
-    if (s.B == 0) return cudaSuccess;
+    if (s_.B == 0) return cudaSuccess;
+    OneVsAllSide s = s_;
+    cudaError_t e;
+    if (drop && (e = launch_dropout_prepare(s, *drop, const_cast<float *>(s.q), halves, st)) != cudaSuccess) return e;
     const unsigned n_qt = (unsigned)((s.B + OVA_T - 1) / OVA_T);
-    cudaError_t e = launch_with_smem(kge_ova_stats_kernel, dim3(n_qt, s.nsplit), OVA_THREADS, OVA_STAGE * sizeof(float), st, s);
+    e = launch_with_smem(kge_ova_stats_kernel, dim3(n_qt, s.nsplit), OVA_THREADS, OVA_STAGE * sizeof(float), st, s);
     if (e != cudaSuccess) return e;
     kge_ova_merge_kernel<<<(unsigned)((s.B + 255) / 256), 256, 0, st>>>(s);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    return launch_grad_passes<OvaMulticlass>(s, halves, one_vs_all_smem_bytes(s.ld), st);
+    return launch_grad_passes<OvaMulticlass>(s, halves, one_vs_all_smem_bytes(s.ld), st, drop);
 }
 
-cudaError_t launch_relation_prediction_side(const OneVsAllSide &s, float *qp, int halves, cudaStream_t st)
+cudaError_t launch_relation_prediction_side(const OneVsAllSide &s, float *qp, int halves, cudaStream_t st,
+                                            const SideDropout *drop)
 {
     if (s.B == 0) return cudaSuccess;
+    if (drop) return launch_one_vs_all_side(s, halves, st, drop);  // the queries come from the dropped s and o rows
     const unsigned grid = (unsigned)((s.B * (s.kp / 4) + 255) / 256);
     if (halves == 2) kge_ova_relation_query_kernel<2><<<grid, 256, 0, st>>>(s, qp);
     else kge_ova_relation_query_kernel<1><<<grid, 256, 0, st>>>(s, qp);
@@ -595,10 +606,13 @@ cudaError_t launch_relation_prediction_side(const OneVsAllSide &s, float *qp, in
 
 size_t k_vs_all_smem_bytes(int ld) { return one_vs_all_smem_bytes(ld) + OVA_T * sizeof(unsigned); }
 
-cudaError_t launch_k_vs_all_side(const OneVsAllSide &s, int halves, cudaStream_t st)
+cudaError_t launch_k_vs_all_side(const OneVsAllSide &s_, int halves, cudaStream_t st, const SideDropout *drop)
 {
-    if (s.B == 0) return cudaSuccess;
-    return launch_grad_passes<KvaMultiLabel>(s, halves, k_vs_all_smem_bytes(s.ld), st);
+    if (s_.B == 0) return cudaSuccess;
+    OneVsAllSide s = s_;
+    cudaError_t e;
+    if (drop && (e = launch_dropout_prepare(s, *drop, const_cast<float *>(s.q), halves, st)) != cudaSuccess) return e;
+    return launch_grad_passes<KvaMultiLabel>(s, halves, k_vs_all_smem_bytes(s.ld), st, drop);
 }
 
 cudaError_t launch_one_vs_all_stamps(int *stamp_ent, long long n_ent, int stamp, cudaStream_t st)

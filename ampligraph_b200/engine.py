@@ -77,35 +77,46 @@ def one_vs_all_splits(B, n_ent):
     return max(1, min(s, 64, n_et))
 
 
-def one_vs_all_workspace_bytes(B, n_ent, ld):
+def dropout_workspace_bytes(n_cand, ld, dropout=False):
+    """The regions embedding dropout adds to an all-candidate step's workspace (kge_set_embedding_dropout; DESIGN.md
+    3.19): the side's dropped candidate table and their gradient, [n_cand, ld] floats each, padded to 16 bytes; 0
+    without dropout."""
+    return 2 * ((4 * int(n_cand) * int(ld) + 15) // 16 * 16) if dropout else 0
+
+
+def one_vs_all_workspace_bytes(B, n_ent, ld, dropout=False):
     """kge_one_vs_all_workspace_bytes(h, B) for a handle of n_ent entities and rows of ld floats: both sides' query
     vectors [B, ld], the quantised positive scores [B], the per-split maxima and sums [nsplit, B], three [B] row arrays
-    and the per-split partial query gradients [nsplit, B, ld], each region padded to 16 bytes."""
+    and the per-split partial query gradients [nsplit, B, ld], each region padded to 16 bytes; with dropout set, the
+    dropout regions (dropout_workspace_bytes) after them."""
     r16 = lambda n: (n + 15) // 16 * 16
     B, ns = int(B), one_vs_all_splits(B, n_ent)
     rows, col = 4 * B * int(ld), 4 * B
-    return 2 * r16(rows) + r16(col) + 2 * r16(ns * col) + 3 * r16(col) + r16(ns * rows)
+    return (2 * r16(rows) + r16(col) + 2 * r16(ns * col) + 3 * r16(col) + r16(ns * rows)
+            + dropout_workspace_bytes(n_ent, ld, dropout))
 
 
-def one_vs_all_relation_workspace_bytes(B, n_rel, ld):
+def one_vs_all_relation_workspace_bytes(B, n_rel, ld, dropout=False):
     """kge_one_vs_all_relation_workspace_bytes(h, B) for a handle of n_rel relations and rows of ld floats: the relation
     queries [B, ld], the per-split maxima and sums [nsplit, B], three [B] row arrays, the per-split partial query
     gradients [nsplit, B, ld] and, when the dX pass splits the query tiles (xsplit > 1), its partial relation rows
-    [xsplit, n_rel, ld], each region padded to 16 bytes."""
+    [xsplit, n_rel, ld], each region padded to 16 bytes; with dropout set, the dropout regions of the n_rel relation
+    rows after them."""
     r16 = lambda n: (n + 15) // 16 * 16
     B, ns, xs = int(B), one_vs_all_splits(B, n_rel), one_vs_all_splits(n_rel, B)
     rows, col = 4 * B * int(ld), 4 * B
     return (r16(rows) + 2 * r16(ns * col) + 3 * r16(col) + r16(ns * rows)
-            + (r16(4 * xs * int(n_rel) * int(ld)) if xs > 1 else 0))
+            + (r16(4 * xs * int(n_rel) * int(ld)) if xs > 1 else 0) + dropout_workspace_bytes(n_rel, ld, dropout))
 
 
-def k_vs_all_workspace_bytes(B, n_ent, ld):
+def k_vs_all_workspace_bytes(B, n_ent, ld, dropout=False):
     """kge_k_vs_all_workspace_bytes(h, B): both sides' query vectors [B, ld], the quantised positive scores [B] and the
-    per-split partial query gradients [nsplit, B, ld], each region padded to 16 bytes (no row statistics)."""
+    per-split partial query gradients [nsplit, B, ld], each region padded to 16 bytes (no row statistics); with dropout
+    set, the dropout regions after them."""
     r16 = lambda n: (n + 15) // 16 * 16
     B, ns = int(B), one_vs_all_splits(B, n_ent)
     rows = 4 * B * int(ld)
-    return 2 * r16(rows) + r16(4 * B) + r16(ns * rows)
+    return 2 * r16(rows) + r16(4 * B) + r16(ns * rows) + dropout_workspace_bytes(n_ent, ld, dropout)
 
 
 INT32_MAX = 2 ** 31 - 1
@@ -315,6 +326,7 @@ class KGEEngine:
         self._rank_ws = None  # caller-owned ranking workspace (kge_rank_workspace_bytes), grown on demand
         self._pblock_next = None  # second [ent | rel] parameter block of the deferred steps, allocated on first use
         self._deferred = False  # a forward_backward(defer=True) left its replaced-row sum for apply_gradients
+        self.dropout = (0.0, 0.0)  # set_embedding_dropout's (p_ent, p_rel)
 
     # -- lifetime ---------------------------------------------------------
     def close(self):
@@ -561,6 +573,19 @@ class KGEEngine:
                       triples.shape[0], *tail, self._stream()))
         self._last_step = int(step)
 
+    def set_embedding_dropout(self, p_ent=0.0, p_rel=0.0, seed=0):
+        """Embedding dropout of the all-candidate steps (kge_set_embedding_dropout, DESIGN.md 3.19): while p_ent or
+        p_rel is non-zero, one_vs_all_backward, one_vs_all_relation_backward and k_vs_all_backward score and
+        differentiate inverted-dropout copies of the entity (p_ent) and relation (p_rel) elements they read, with
+        masks drawn from (seed, step); forward_backward is refused.  (0, 0) clears it.  p in [0, 1) (ValueError)."""
+        _lib.check(self.lib.kge_set_embedding_dropout(self.h, float(p_ent), float(p_rel), int(seed)))
+        self.dropout = (float(p_ent), float(p_rel))
+
+    def _dropout_launches(self, sides):
+        """Launches dropout adds to a step of `sides` sides: per side the dropped table and the queries (a memset
+        besides), and the masked candidate gradient; the query vectors' two kernels are not launched."""
+        return 3 * sides - 2 if any(self.dropout) else 0
+
     @_traced("kge.one_vs_all_step")
     def one_vs_all_backward(self, triples, sides="s,o", step=0):
         """1vsAll step up to tape.gradient (kge_one_vs_all_step, DESIGN.md 3.12): the multiclass NLL of every positive
@@ -575,7 +600,8 @@ class KGEEngine:
                         (_lib.ONE_VS_ALL_SIDES[sides], _lib.REDUCTIONS[self.reduction]), (int(step), _ptr(self.loss_acc)))
         # query vectors (two kernels), entity stamps, five passes per side
         if B:
-            self.launches += 2 + (1 if self.lazy else 0) + 5 * (2 if sides == "s,o" else 1)
+            n = 2 if sides == "s,o" else 1
+            self.launches += 2 + (1 if self.lazy else 0) + 5 * n + self._dropout_launches(n)
 
     @_traced("kge.one_vs_all_relation_step")
     def one_vs_all_relation_backward(self, triples, weight, step=0):
@@ -589,7 +615,8 @@ class KGEEngine:
                         (float(weight), _lib.REDUCTIONS[self.reduction]), (int(step), _ptr(self.loss_acc)))
         # relation stamps, relation queries, five passes, the dX split sum when dX is split
         if B:
-            self.launches += (1 if self.lazy else 0) + 6 + (1 if one_vs_all_splits(self.n_rel, B) > 1 else 0)
+            self.launches += ((1 if self.lazy else 0) + 6 + (1 if one_vs_all_splits(self.n_rel, B) > 1 else 0)
+                              + (2 if any(self.dropout) else 0))
 
     @_traced("kge.k_vs_all_step")
     def k_vs_all_backward(self, queries, side, label_offsets, label_ids, label_smoothing=0.0, step=0):
@@ -612,7 +639,7 @@ class KGEEngine:
                         (_ptr(label_offsets), _ptr(label_ids), int(step), _ptr(self.loss_acc)))
         # query vectors (two kernels), entity stamps, dQ, dX and chain
         if B:
-            self.launches += 2 + (1 if self.lazy else 0) + 3
+            self.launches += 2 + (1 if self.lazy else 0) + 3 + self._dropout_launches(1)
 
     @property
     def n3_workspace_bytes(self):

@@ -266,7 +266,7 @@ class ScoringBasedEmbeddingModel:
             validation_corrupt_side="s,o", validation_freq=10, validation_burn_in=0, validation_filter=False,
             validation_entities_subset=None, partitioning_k=1, focusE=False, focusE_params={}, one_vs_all=None,
             k_vs_all=None, label_smoothing=0.0, relation_prediction_weight=0.0, negative_sampler="uniform",
-            filter_negatives=False):
+            filter_negatives=False, entity_dropout=0.0, relation_dropout=0.0):
         """fit (:544-883).  `shuffle` is accepted and ignored exactly like the reference
         (batches are the sequential slices of graph_data_loader.py:495-500).  validation_split: carve the validation
         set out of x with train_test_split_no_unseen(x, test_size=validation_split, seed=self.seed), as the reference
@@ -315,8 +315,18 @@ class ScoringBasedEmbeddingModel:
         up to NEGATIVE_FILTER_ATTEMPTS draws; those still known after the last are trained on and counted in
         self.negative_filter_misses (read once per epoch).  The tables are built once per fit from x.  They apply to
         every single-GPU sampled step of fit (the fused step, user losses, focusE), not to one_vs_all or k_vs_all;
-        train_on_batch and train_on_batches stay uniform.  'uniform' without the filter is the path fit always took."""
+        train_on_batch and train_on_batches stay uniform.  'uniform' without the filter is the path fit always took.
+
+        entity_dropout, relation_dropout (extension; DESIGN.md 3.19): p in [0, 1), inverted dropout on the entity and
+        relation embedding elements every training score of the fit reads (LibKGE's lookup-embedder dropout, tuned by
+        Ruffinelli et al., ICLR 2020): each kept element is scaled by 1 / (1 - p), each dropped one is 0.  A step's
+        candidate rows share one mask per side; each query row of the batch draws its own.  The masks come from the
+        model's seed and the step.  They apply to one_vs_all and k_vs_all training only (with reciprocal relations,
+        relation_prediction_weight, N3, DURA, label smoothing and either reduction); the regularisers, the optimizer,
+        validation, evaluate, predict and every later call read the raw embeddings.  The logged loss is that of the
+        dropped-out scores.  0.0 (the default) leaves training unchanged."""
         self._assert_compile_was_called()
+        self._check_dropout(entity_dropout, relation_dropout, one_vs_all, k_vs_all)
         if self.reciprocal_relations:
             self._check_reciprocal("fit", one_vs_all, k_vs_all, focusE, relation_prediction_weight)
         sampled_option = self._check_negative_sampler(negative_sampler, filter_negatives, one_vs_all, k_vs_all)
@@ -356,6 +366,24 @@ class ScoringBasedEmbeddingModel:
             raise ValueError("relation_prediction_weight needs at least two relations, got %d" % self.max_rel_size)
         if self.engine is None:
             self._build_engine()
+        eng = self.engine
+        dropout = (float(entity_dropout), float(relation_dropout))
+        if any(dropout):  # only the all-candidate steps read it; validation ranks the raw embeddings
+            eng.set_embedding_dropout(*dropout, seed=self.seed)
+        try:
+            return self._fit_loop(x, triples, batch_size, epochs, verbose, callbacks, validation_data, initial_epoch,
+                                  validation_batch_size, validation_corrupt_side, validation_freq, validation_burn_in,
+                                  validation_filter, validation_entities_subset, one_vs_all, k_vs_all, label_smoothing,
+                                  relation_prediction_weight, negative_sampler, filter_negatives, sampled_option)
+        finally:
+            if any(dropout):
+                eng.set_embedding_dropout(0.0, 0.0)
+
+    def _fit_loop(self, x, triples, batch_size, epochs, verbose, callbacks, validation_data, initial_epoch,
+                  validation_batch_size, validation_corrupt_side, validation_freq, validation_burn_in,
+                  validation_filter, validation_entities_subset, one_vs_all, k_vs_all, label_smoothing,
+                  relation_prediction_weight, negative_sampler, filter_negatives, sampled_option):
+        """fit's training loop, on the engine fit has built (with fit's embedding dropout set on it)."""
         eng = self.engine
         eng.set_hot_entities(triples=triples)  # the most frequent entities of the training set: their gradient rows are summed per warp
         data = self._to_dev(triples, np.int32)  # uploaded once; batches are device-side slices
@@ -466,6 +494,18 @@ class ScoringBasedEmbeddingModel:
         self.is_fitted = True
         self.history = history
         return history
+
+    @staticmethod
+    def _check_dropout(entity_dropout, relation_dropout, one_vs_all, k_vs_all):
+        """The refusals of fit(entity_dropout=..., relation_dropout=...), before anything is indexed or trained: each a
+        real, finite number in [0, 1) (not a bool), and a non-zero one needs one_vs_all or k_vs_all."""
+        for name, p in (("entity_dropout", entity_dropout), ("relation_dropout", relation_dropout)):
+            if (isinstance(p, bool) or not isinstance(p, numbers.Real) or not math.isfinite(p)
+                    or not 0.0 <= p < 1.0):
+                raise ValueError("%s must be a number in [0, 1), got %r" % (name, p))
+        if (entity_dropout or relation_dropout) and one_vs_all is None and k_vs_all is None:
+            raise ValueError("entity_dropout and relation_dropout apply to one_vs_all and k_vs_all training only: the "
+                             "sampled training kernels (also with focusE or a user loss) do not apply them")
 
     def _uses_n3(self):
         return any(isinstance(r, regularizers.N3Regularizer) for r in self._regularizer)

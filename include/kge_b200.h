@@ -394,6 +394,23 @@ int kge_k_vs_all_step(kge_handle *h, int32_t side, int32_t loss_reduction, float
                       const int64_t *label_offsets_dev, const int32_t *label_ids_dev, uint64_t step, double *loss_dev,
                       void *ws_dev, int64_t ws_bytes, void *stream);
 
+/* Embedding dropout of the all-candidate steps (LibKGE's lookup-embedder dropout; DESIGN.md 3.19).  While p_ent or
+ * p_rel is non-zero, kge_one_vs_all_step, kge_one_vs_all_relation_step and kge_k_vs_all_step score and differentiate
+ * inverted-dropout copies of the embedding elements they read: x~ = fp32(x * scale) where kept, +0 where dropped,
+ * scale = fp32(1 / (1 - p)), p_ent for entity rows and p_rel for relation rows (reciprocal relations' inverse rows
+ * included).  The raw element's gradient is fp32(scale * m * gradient of x~).  A side's candidate rows share one mask
+ * per call (keyed by row id); each query row of the batch takes its own mask per position b; the sides s, o and p draw
+ * independent masks.  Element c (column of the padded row) of row `row` takes word c & 3 of
+ * philox4x32_10((row, (c >> 2) | (0x80 | tag) << 24, step_lo, step_hi), (seed_lo, seed_hi)) and is kept iff
+ * (word >> 8) >= round(p 2^24), with step the step's `step` argument and tag = 4 side + role (side 1 = s, 2 = o,
+ * 3 = p; role 0 the candidates, row = table row; role 1 + j the query's triple column j, row = b).  The logged loss is
+ * that of the dropped-out scores.  While it is set, the three workspace sizers add two [n_cand, ld] float tables, and
+ * kge_train_step and kge_train_step_sharded are refused with KGE_ERR_UNSUPPORTED (their fused kernels do not apply
+ * it); kge_n3_step, kge_dura_step, the optimizer and every ranking, scoring and top-k entry point read the raw tables
+ * as before.  p_ent = p_rel = 0 clears it, and the steps then run exactly as without it.
+ * KGE_ERR_INVALID_ARGUMENT: p_ent or p_rel NaN, < 0 or >= 1. */
+int kge_set_embedding_dropout(kge_handle *h, float p_ent, float p_rel, uint64_t seed);
+
 /* The N3 regulariser (Lacroix, Usunier and Obozinski, ICML 2018, eq. 6) of a step's B positives (s_b, p_b, o_b):
  * L_N3 = lambda_ent * sum_b sum_d (|s_bd|^3 + |o_bd|^3) + lambda_rel * sum_b sum_d |p_bd|^3, duplicates counted every
  * time they occur.  |z_d| is |x[d]| for TransE and DistMult, and the modulus sqrt(x[d]^2 + x[kp + d]^2) for ComplEx,

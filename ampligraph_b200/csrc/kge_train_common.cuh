@@ -4,6 +4,7 @@
 // the corruption draw, and the per-positive loss + dL/dscore of the five reference losses; on the host, the launch they
 // share and the trilinear row-shape dispatch.
 #pragma once
+#include <float.h>
 #include <math.h>
 
 #include <type_traits>
@@ -245,13 +246,14 @@ __device__ __forceinline__ float rot_modsum(float4 re, float4 im)
     const float4 x = f4fma(im, im, re * re);
     return (sqrt_approx(x.x) + sqrt_approx(x.y)) + (sqrt_approx(x.z) + sqrt_approx(x.w));
 }
-// (a, b) = g * (re, im) / |(re, im)|: one MUFU.RSQ on max(x, tiny), so an exactly-zero residual gives 0 * finite = 0
-// (the reference's gradient is NaN there)
+// (a, b) = g * (re, im) / |(re, im)|: one MUFU.RSQ on max(x, FLT_MIN), the smallest x whose rsqrt.approx.ftz is finite,
+// so every normal x gets its own rsqrt and an exactly-zero residual gives 0 * 2^63 = 0 (the reference's gradient is NaN
+// there); below FLT_MIN the result is g * (re, im) * 2^63, at most |g| per component
 __device__ __forceinline__ void rot_unit(float4 re, float4 im, float g, float4 &a, float4 &b)
 {
     const float4 x = f4fma(im, im, re * re);
-    const float4 inv = g * make_float4(rsqrt_approx(fmaxf(x.x, 1e-30f)), rsqrt_approx(fmaxf(x.y, 1e-30f)),
-                                       rsqrt_approx(fmaxf(x.z, 1e-30f)), rsqrt_approx(fmaxf(x.w, 1e-30f)));
+    const float4 inv = g * make_float4(rsqrt_approx(fmaxf(x.x, FLT_MIN)), rsqrt_approx(fmaxf(x.y, FLT_MIN)),
+                                       rsqrt_approx(fmaxf(x.z, FLT_MIN)), rsqrt_approx(fmaxf(x.w, FLT_MIN)));
     a = re * inv;
     b = im * inv;
 }

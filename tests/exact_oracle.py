@@ -17,6 +17,9 @@ count n, and A1 = sum of |d score_j / d element| (for results below fp32's small
 For the 1vsAll family (1vsAll, KvsAll, relation prediction), whose every gradient element sums one term per (query,
 candidate) pair, OvaBound gives the per-element bound in the same form, with each pair's weight derived in its
 docstring from the kernels' split geometry (ova_chains) and the pair's logit error.
+
+RotatE's training arithmetic is not exact on any grid (approximate sqrt / rsqrt, fp32 cos / sin): oracle_step(...,
+rot_table=True) evaluates it on the rotation table the kernels read, and RotatEBound gives its per-element bound.
 """
 from collections import namedtuple
 
@@ -64,8 +67,9 @@ def assert_fp32_exact(x, what=""):
 # scores
 # --------------------------------------------------------------------------
 class _Modulus(torch.autograd.Function):
-    """sqrt(re^2 + im^2) whose gradient is 0 where the modulus is 0 (the reference's is NaN there; the kernel's rot_unit,
-    kge_train_common.cuh, takes g * 0 * rsqrt(max(x, tiny)) = 0)."""
+    """sqrt(re^2 + im^2) whose gradient is 0 where the modulus is 0 (the reference's is NaN there).  The kernel's rot_unit
+    (kge_train_common.cuh) takes g v rsqrt(max(|v|^2, 2^-126)): g v / |v| for |v|^2 >= 2^-126, g v 2^63 (at most |g|
+    per component, 0 at an exactly zero residual) below; RotatEBound charges those terms in full."""
 
     @staticmethod
     def forward(ctx, re, im):
@@ -81,14 +85,54 @@ class _Modulus(torch.autograd.Function):
         return unit * re, unit * im
 
 
-def scores(model, e_s, e_p, e_o, max_rel_size=None):
-    """ref_step.compute_scores, but RotatE's modulus through _Modulus."""
+def rotation_divisor32(K, max_rel_size):
+    """(div, inv_div) as the kernels have them: fp32(range / pi) (kge_create, kgeo_rotate_divisor) and fp32(1 / div)."""
+    div = np.float32(ref_step.rotate_divisor(K, max_rel_size))
+    return div, np.float32(1.0) / div
+
+
+def rotation_table(theta, div):
+    """(c, sn): the fp32 cos and sin of fp32(theta / div) by the canonical sincos -- the rotation table
+    kge_rotation_table_kernel computes with kge_sincosf (kgeo_sincosf in the C oracle; pinned bit for bit by
+    test_gpu_parity.py::test_corruption_scores_vs_oracle).  numpy float32 arrays of theta's shape."""
+    from oracle import c_oracle
+    phi = np.asarray(theta, np.float32) / np.float32(div)
+    uniq, inv = np.unique(phi, return_inverse=True)
+    s, c = c_oracle.sincos(uniq)
+    return c[inv].reshape(phi.shape), s[inv].reshape(phi.shape)
+
+
+class _KernelRotation(torch.autograd.Function):
+    """theta -> (c, sn) of rotation_table, whose derivative is inv_div (-sn, c): the kernels' relation gradient
+    fp32(1 / div) df/dphi, formed from the table's own values."""
+
+    @staticmethod
+    def forward(ctx, theta, div, inv_div):
+        c, sn = rotation_table(theta.detach().cpu().numpy(), div)
+        c = torch.as_tensor(c, dtype=theta.dtype, device=theta.device)
+        sn = torch.as_tensor(sn, dtype=theta.dtype, device=theta.device)
+        ctx.save_for_backward(c, sn)
+        ctx.inv_div = float(inv_div)
+        return c, sn
+
+    @staticmethod
+    def backward(ctx, gc, gs):
+        c, sn = ctx.saved_tensors
+        return ctx.inv_div * (c * gs - sn * gc), None, None
+
+
+def scores(model, e_s, e_p, e_o, max_rel_size=None, rot_table=False):
+    """ref_step.compute_scores, but RotatE's modulus through _Modulus; rot_table: RotatE's (cos, sin) from the fp32
+    rotation table (_KernelRotation) instead of float64 cos / sin of theta / div."""
     if model != "RotatE":
         return ref_step.compute_scores(model, e_s, e_p, e_o, max_rel_size)
     h = e_s.shape[1] // 2
-    div = ref_step.rotate_divisor(e_s.shape[1], max_rel_size if max_rel_size else 1)
     theta = e_p[:, :h]
-    p_re, p_im = torch.cos(theta / div), torch.sin(theta / div)
+    if rot_table:
+        p_re, p_im = _KernelRotation.apply(theta, *rotation_divisor32(e_s.shape[1], max_rel_size or 1))
+    else:
+        div = ref_step.rotate_divisor(e_s.shape[1], max_rel_size if max_rel_size else 1)
+        p_re, p_im = torch.cos(theta / div), torch.sin(theta / div)
     re = e_s[:, :h] * p_re - e_s[:, h:] * p_im - e_o[:, :h]
     im = e_s[:, :h] * p_im + e_s[:, h:] * p_re - e_o[:, h:]
     return -torch.sum(_Modulus.apply(re, im), dim=1)
@@ -101,9 +145,9 @@ def abs_scores(model, e_s, e_p, e_o):
         return (e_s + e_p + e_o).sum(1)
     if model == "DistMult":
         return torch.sum(e_s * e_p * e_o, dim=1)
+    assert model != "RotatE", "RotatE's bound is RotatEBound"
     h = e_s.shape[1] // 2
     s_re, s_im, p_re, p_im, o_re, o_im = e_s[:, :h], e_s[:, h:], e_p[:, :h], e_p[:, h:], e_o[:, :h], e_o[:, h:]
-    # (RotatE has no bound here: its training arithmetic uses approximate sqrt / rsqrt)
     sc = torch.sum(s_re * (p_re * o_re + p_im * o_im) + s_im * (p_re * o_im + p_im * o_re), dim=1)
     return sc * (2.0 / h) if model == "HolE" else sc
 
@@ -138,11 +182,12 @@ def loss_magnitudes(name, sp, sn, lp, dsp, dsn):
 # the step
 # --------------------------------------------------------------------------
 def oracle_step(model, ent, rel, triples, eta, neg_ent, neg_keep, loss="pairwise", loss_params=None, dpos=None,
-                dneg=None, device="cpu", dtype=torch.float64, chunk=None, max_rel_size=None):
+                dneg=None, device="cpu", dtype=torch.float64, chunk=None, max_rel_size=None, rot_table=False):
     """One step's scores, loss and gradient tables.  triples [B, 3]; neg_ent / neg_keep [eta*B], row j*B + i the j-th
     corruption of positive i (neg_keep = 1: the subject is kept, the object replaced).  dpos [B] / dneg [eta*B]: an
     external dL/dscore (KGE_STEP_BACKWARD_EXT) instead of the loss.  chunk: positives per autograd pass (the gradients
     of the loss, a sum over positives, are summed over the passes).  dtype float32 evaluates the same graph in fp32.
+    rot_table: RotatE on the kernels' fp32 rotation table (scores).
     -> Step of tensors on `device` (loss None with an external dL/dscore; sn, dsn, mag_neg as [eta*B])."""
     lp = dict(loss_params or {})
     dev = torch.device(device)
@@ -169,8 +214,8 @@ def oracle_step(model, ent, rel, triples, eta, neg_ent, neg_keep, loss="pairwise
             corr = given[:, a:b].reshape(-1, 3)
         else:
             corr = ref_step.corrupt(tc, eta, nk[:, a:b].reshape(-1), ne[:, a:b].reshape(-1))
-        sp = scores(model, E[tc[:, 0]], R[tc[:, 1]], E[tc[:, 2]], mrs)
-        sn = scores(model, E[corr[:, 0]], R[corr[:, 1]], E[corr[:, 2]], mrs).reshape(eta, -1)
+        sp = scores(model, E[tc[:, 0]], R[tc[:, 1]], E[tc[:, 2]], mrs, rot_table)
+        sn = scores(model, E[corr[:, 0]], R[corr[:, 1]], E[corr[:, 2]], mrs, rot_table).reshape(eta, -1)
         if dpos is not None:
             dsp, dsn = dpos[a:b], dneg[:, a:b]
             obj = (sp * dsp).sum() + (sn * dsn).sum()
@@ -212,11 +257,12 @@ def grad_bound(model, ent, rel, triples, corr, mag_pos, mag_neg, device="cpu"):
     return (out[0][0], out[1][0], n_e), (out[0][1], out[1][1], n_r)
 
 
-def within_bound(got, want, A, A1, n, extra):
-    """|got - want| <= (n + 8 + extra) 2^-24 A + 2^-126 A1 per element (extra: the loss's own rounding chain).
+def within_bound(got, want, A, A1, n, extra, absolute=0.0):
+    """|got - want| <= (n + 8 + extra) 2^-24 A + 2^-126 A1 + absolute per element (extra: the loss's own rounding
+    chain; absolute: per-term allowances that are not a multiple of A, RotatEBound's).
     -> (ok, worst ratio of error to bound)."""
     got = torch.as_tensor(got, dtype=torch.float64, device=want.device)
-    bound = (n + 8 + extra) * FP32_EPS * A + FP32_TINY * A1
+    bound = (n + 8 + extra) * FP32_EPS * A + FP32_TINY * A1 + absolute
     err = (got - want).abs()
     ratio = torch.where(bound > 0, err / torch.where(bound > 0, bound, torch.ones_like(bound)),
                         torch.where(err > 0, torch.full_like(err, float("inf")), torch.zeros_like(err)))
@@ -230,6 +276,159 @@ def zipf_triples(E, R, n, rng):
     perm = rng.permutation(E)
     s, o = perm[np.searchsorted(cdf, rng.random(n))], perm[np.searchsorted(cdf, rng.random(n))]
     return np.stack([s, rng.integers(0, R, n), o], 1).astype(np.int32)
+
+
+# --------------------------------------------------------------------------
+# RotatE: a per-element bound
+# --------------------------------------------------------------------------
+# The MUFU approximations of the RotatE training kernels (kge_train_common.cuh: sqrt_approx, rsqrt_approx), from the
+# PTX ISA's instruction descriptions: sqrt.approx.f32 has a maximum relative error of 2^-23 and rsqrt.approx.f32 one of
+# 2^-22.9 over the range of normal inputs (the .ftz forms flush subnormal inputs to 0).  scripts/check_sqrt.cu measures
+# both over every normal float: 2^-23.25 and 2^-22.94 on an H100 80GB HBM3 at 700 W (DESIGN.md 3.4).
+EPS_SQRT = 2.0 ** -23
+EPS_RSQ = 2.0 ** -22.9
+ROT_C = 8  # roundings of one gradient element outside the term sums: back-rotation (2), inv_div (1), the Z / Aphi fma
+
+
+def loss_score_sensitivity(loss, lp, sp, sn, dsp_err, dsn_err):
+    """Per score j of each positive: sum_i |d^2 L / d s_j d s_i| ds_i over the positive's eta + 1 scores (the
+    (eta+1)^2 Hessian block of per_positive_loss, float64 autograd): how far a score error ds moves dL/dscore.
+    sp [B], sn [eta, B] -> ([B], [eta, B]).  The hinge losses' Hessian is 0 (see RotatEBound for their premise)."""
+    lp = dict(lp or {})
+    s = torch.cat([sp.detach()[None], sn.detach()], 0).clone().requires_grad_(True)
+    err = torch.cat([dsp_err[None], dsn_err], 0)
+    L = ref_step.per_positive_loss(loss, s[0], s[1:], margin=lp.get("margin"), alpha=lp.get("alpha"),
+                                   reduction=lp.get("reduction", "sum")).sum()
+    G = torch.autograd.grad(L, s, create_graph=True)[0]
+    out = torch.zeros_like(err)
+    if G.requires_grad:
+        for k in range(s.shape[0]):  # row k of every positive's block at once (the blocks do not interact)
+            Hk = torch.autograd.grad(G[k].sum(), s, retain_graph=True, allow_unused=True)[0]
+            if Hk is not None:
+                out[k] = (Hk.abs() * err).sum(0)
+    return out[0], out[1:]
+
+
+class RotatEBound:
+    """The per-element error bound of one RotatE training step (kge_train_rot_kernel and the general kernel's RotatE
+    Scorer, which share the rot_* functions of kge_train_common.cuh), against oracle_step(..., rot_table=True): both
+    read the same fp32 rotation table (c, sn), so the bound covers the training arithmetic only.  u = 2^-24.
+
+    Every score row j (positive or corruption; x its subject-slot row, o its object-slot row, g_j = dL/dscore_j) adds,
+    per complex column d, one term to each of x's two elements, o's two and theta_d.  With y = R(phi) x, v = y - o,
+    m = |v| and U = g v / m:  d/do = U,  d/dx = -R(-phi) U,  d/dtheta = inv_div (U_re y_im - U_im y_re).
+      * Residual.  Object-slot chains rot_rotate then a subtraction (the gradient pass, and the score pass of the
+        positive and of object-replaced rows), or rot_residual_subj (two dependent fmas; score pass of subject-
+        replaced rows).  Either way each component is within 3 u S_c (1 + 2u) + 2^-125 of the exact one, S_re = |x_re c|
+        + |x_im sn| + |o_re|, S_im = |x_re sn| + |x_im c| + |o_im| (two or three roundings, each at most u times a
+        partial sum bounded by S_c; 2^-125 for flushed subnormal intermediates).  dv = delta_re + delta_im >= |dv|.
+      * Unit vector.  rot_unit forms |v|^2 = fma(im, im, re re) (2u relative, plus 2^-125 absolute when squares fall
+        below 2^-126), rsqrt.approx (EPS_RSQ) and two products (2u): every component of the kernel's (a, b) is within
+            E = |g| min(2 dv / m + EPS_RSQ + 4u + 2^-125 / m^2,  2 + EPS_RSQ + 4u) + |dg| (1 + EPS_RSQ + 4u)
+        of U's, dg the error of g.  2 dv / m bounds |v/|v| - v'/|v'|| for |v - v'| <= dv; it is ill-conditioned as m
+        -> 0 and is carried per term.  The cap holds because both vectors have norm at most |g| (1 + EPS_RSQ + 4u); it
+        also covers |v|^2 < 2^-126, where rot_unit returns g v 2^63 (at most |g| per component).
+      * Terms.  Per element the term's magnitude w and its absolute allowance X are: o's elements w = |g|, X = E;
+        x's elements w = |g| (|c| + |sn|), X = E (|c| + |sn|); theta_d w = inv_div |g| (|y_re| + |y_im|),
+        X = inv_div (E (|y_re| + |y_im|) + |g| dy), dy = 2u (|x_re c| + |x_im sn| + |x_re sn| + |x_im c|) the error of
+        the kernel's y.  A = sum of w, absolute = sum of X.
+      * Sums.  The register sums Z* / Aphi (up to eta + 1 terms, summed before the back-rotation in finish), the
+        back-rotation and the red.global.add atomics in any order: (n + 8 + ROT_C) u A with n = the element's lookups
+        + eta + 2; the atomics flush subnormal results, 2^-126 each (A1 = n + 8).
+      * Scores.  |delta s| <= sum_d (dv_d + (m_d + dv_d)(EPS_SQRT + 2u)) + (h + 16) u sum_d (m_d + dv_d) + h 2^-62:
+        the residual, |v|^2's rounding (2u relative, half of it through the sqrt) and sqrt.approx, the sum of h moduli
+        (float4 sums, fma with the lane mask, warp sum), and sqrt.approx.ftz flushing |v|^2 < 2^-126 to 0
+        (sqrt(2^-125) < 2^-62).
+      * Fused losses.  dg_j = sum_i |H_ji| delta s_i (loss_score_sensitivity: the positive's Hessian block) plus the
+        loss chain's own roundings (2 eta + 16) u mag_j (loss_magnitudes, as for the trilinear models).  For pairwise
+        and absolute_margin the Hessian is 0 away from the hinge, so the data must keep every hinge argument farther
+        than its score bound from 0 (asserted: a premise of the data, not a property of the kernel).
+      * Loss.  sum_i (sum_j |g_ij| delta s_ij + (2 eta + 32) u (|L_i| + sum_j |g_ij| (|s_ij| + |margin|) + eta)).
+    loss None: KGE_STEP_BACKWARD_EXT (g given and exact, dg = 0)."""
+
+    def __init__(self, ent, rel, triples, step, eta, loss=None, loss_params=None, max_rel_size=None, device="cpu"):
+        u = FP32_EPS
+        dev = self.device = torch.device(device)
+        E = torch.as_tensor(np.asarray(ent), dtype=torch.float64, device=dev)
+        R = torch.as_tensor(np.asarray(rel), dtype=torch.float64, device=dev)
+        K = E.shape[1]
+        h = K // 2
+        div, inv_div = rotation_divisor32(K, max_rel_size or R.shape[0])
+        inv_div = float(inv_div)
+        ct, st = rotation_table(np.asarray(rel, np.float32)[:, :h], div)
+        ct = torch.as_tensor(ct, dtype=torch.float64, device=dev)
+        st = torch.as_tensor(st, dtype=torch.float64, device=dev)
+        t = torch.as_tensor(np.asarray(triples), dtype=torch.long, device=dev)
+        B = t.shape[0]
+        T = torch.cat([t, step.corr.to(dev)], 0)
+        g = torch.cat([step.dsp, step.dsn]).to(dev).double()
+        X, O, c, sn = E[T[:, 0]], E[T[:, 2]], ct[T[:, 1]], st[T[:, 1]]
+        xr, xi, orr, oi = X[:, :h], X[:, h:], O[:, :h], O[:, h:]
+        yr, yi = xr * c - xi * sn, xr * sn + xi * c
+        m = torch.sqrt((yr - orr) ** 2 + (yi - oi) ** 2)
+        Sre = (xr * c).abs() + (xi * sn).abs() + orr.abs()
+        Sim = (xr * sn).abs() + (xi * c).abs() + oi.abs()
+        dv = 3 * u * (1 + 2 * u) * (Sre + Sim) + 2.0 ** -124
+        mm = m + dv
+        self.score_err = ((dv + mm * (EPS_SQRT + 2 * u)).sum(1) + (h + 16) * u * mm.sum(1) + h * 2.0 ** -62)
+        dsp_err, dsn_err = self.score_err[:B], self.score_err[B:].reshape(eta, B)
+        if loss is None:
+            dg = torch.zeros_like(g)
+        else:
+            lp = dict(loss_params or {})
+            sp, snn = step.sp.to(dev).double(), step.sn.to(dev).double().reshape(eta, B)
+            if loss in ("pairwise", "absolute_margin"):
+                mg = lp.get("margin", 1.0)
+                arg = mg - sp[None] + snn if loss == "pairwise" else mg + snn
+                near = arg.abs() <= dsn_err + (dsp_err[None] if loss == "pairwise" else 0)
+                assert not bool(near.any()), "premise: a hinge argument lies within its score bound of 0"
+            hp, hn = loss_score_sensitivity(loss, loss_params, sp, snn, dsp_err, dsn_err)
+            mag = torch.cat([step.mag_pos, step.mag_neg]).to(dev).double()
+            dg = torch.cat([hp, hn.reshape(-1)]) + (2 * eta + 16) * u * mag
+            gl = torch.cat([step.dsp[None], step.dsn.reshape(eta, B)], 0).to(dev).double().abs()
+            sc = torch.cat([sp[None], snn], 0).abs()
+            err = torch.cat([dsp_err[None], dsn_err], 0)
+            mg = abs(lp.get("margin", 3.0 if loss == "self_adversarial" else 1.0))
+            self.loss_err = float((gl * err).sum() + (2 * eta + 32) * u * (abs(step.loss) + (gl * (sc + mg)).sum()
+                                                                            + eta * B))
+        ga, dga = g.abs()[:, None], dg[:, None]
+        rel_e = torch.where(m > 0, 2 * dv / torch.where(m > 0, m, torch.ones_like(m)) + EPS_RSQ + 4 * u
+                            + 2.0 ** -125 / torch.where(m > 0, m * m, torch.ones_like(m)), torch.full_like(m, np.inf))
+        Eu = ga * torch.clamp(rel_e, max=2 + EPS_RSQ + 4 * u) + dga * (1 + EPS_RSQ + 4 * u)
+        cs = c.abs() + sn.abs()
+        ya = yr.abs() + yi.abs()
+        dy = 2 * u * (Sre + Sim - orr.abs() - oi.abs())
+        self.A = [torch.zeros_like(E), torch.zeros_like(R)]
+        self.X = [torch.zeros_like(E), torch.zeros_like(R)]
+        for rows, w, x in ((T[:, 0], ga * cs, Eu * cs), (T[:, 2], ga.expand(-1, h), Eu)):
+            self.A[0].index_add_(0, rows, torch.cat([w, w], 1))
+            self.X[0].index_add_(0, rows, torch.cat([x, x], 1))
+        self.A[1][:, :h].index_add_(0, T[:, 1], inv_div * ga * ya)
+        self.X[1][:, :h].index_add_(0, T[:, 1], inv_div * (Eu * ya + ga * (1 + 4 * u) * dy))
+        n_e = torch.bincount(torch.cat([T[:, 0], T[:, 2]]), minlength=E.shape[0]).double()[:, None]
+        n_r = torch.bincount(t[:, 1], minlength=R.shape[0]).double()[:, None]
+        self.n = [n_e + eta + 2, n_r + eta + 2]
+
+    def check(self, got_ent, got_rel, want_ent, want_rel):
+        """-> [(name, ok, worst error / bound)] for both gradient tables."""
+        out = []
+        for i, (name, got, want) in enumerate((("g_ent", got_ent, want_ent), ("g_rel", got_rel, want_rel))):
+            want = torch.as_tensor(want, dtype=torch.float64).to(self.device)
+            got = torch.as_tensor(got, dtype=torch.float64).to(self.device)
+            if not bool(torch.isfinite(got).all()):
+                out.append((name, False, float("inf")))
+                continue
+            ok, ratio = within_bound(got, want, self.A[i], self.n[i] + 8, self.n[i], ROT_C, self.X[i])
+            out.append((name, ok, ratio))
+        return out
+
+    def check_scores(self, got, want, which):
+        """got / want [B] (which 'sp') or [eta*B] ('sn') -> (ok, worst error / bound)."""
+        B = len(self.score_err) - len(want) if which == "sn" else 0
+        bound = self.score_err[B:B + len(want)] if which == "sn" else self.score_err[:len(want)]
+        got = torch.as_tensor(got, dtype=torch.float64).to(self.device)
+        err = (got - torch.as_tensor(want, dtype=torch.float64).to(self.device)).abs()
+        return bool((err <= bound).all()), float((err / bound).max()) if err.numel() else 0.0
 
 
 # --------------------------------------------------------------------------

@@ -532,7 +532,7 @@ def test_edge_rotate_zero_modulus(kernel, monkeypatch):
     ne, nk = ne.reshape(-1), nk.reshape(-1)
     lp = {"margin": 3.0, "alpha": 0.5}
     sp, sn, g_e, g_r, _ = _run_rows("RotatE", k, eta, ent, rel, t, ne, nk, "self_adversarial", lp, kernel, monkeypatch)
-    ref = xo.oracle_step("RotatE", ent, rel, t, eta, ne, nk, loss="self_adversarial", loss_params=lp)
+    ref = xo.oracle_step("RotatE", ent, rel, t, eta, ne, nk, loss="self_adversarial", loss_params=lp, rot_table=True)
     for x in (g_e, g_r, ref.g_ent, ref.g_rel):
         assert bool(torch.isfinite(x).all())
     assert float(ref.sp[0]) == 0.0 and float(sp[0]) == 0.0
@@ -543,5 +543,7 @@ def test_edge_rotate_zero_modulus(kernel, monkeypatch):
         assert bool((g_e[row, zero_cols] == 0).all()), row
         assert bool((g_e[row, np.r_[h:k, k + h:2 * k]] != 0).all()), row
     assert bool((g_r[0, :h] == 0).all()) and bool((g_r[0, h:k] != 0).all())
-    tol = 2.0 ** -14 * max(float(ref.g_ent.abs().max()), float(ref.g_rel.abs().max()))
-    assert float((g_e - ref.g_ent).abs().max()) <= tol and float((g_r - ref.g_rel).abs().max()) <= tol
+    bound = xo.RotatEBound(ent, rel, t, ref, eta, loss="self_adversarial", loss_params=lp)
+    for name, ok, ratio in bound.check(g_e, g_r, ref.g_ent, ref.g_rel):
+        assert ok, (kernel, name, ratio)
+    assert bound.check_scores(sp, ref.sp, "sp")[0] and bound.check_scores(sn, ref.sn, "sn")[0]

@@ -18,6 +18,8 @@ import numpy as np
 import pytest
 import torch
 
+import exact_oracle as xo
+
 pytestmark = pytest.mark.gpu
 
 MODELS = ["TransE", "DistMult", "ComplEx", "HolE", "RotatE"]
@@ -276,6 +278,12 @@ def test_train_step_sharded(geom, layout, mode, negatives, monkeypatch):
     if mode != "forward_only":
         assert _close(_dense(ref, g_e), o_ge.numpy()), np.abs(_dense(ref, g_e) - o_ge.numpy()).max()
         assert _close(_dense(ref, g_r), o_gr.numpy()), np.abs(_dense(ref, g_r) - o_gr.numpy()).max()
+    if model == "RotatE" and mode != "forward_only":  # every element against the dense oracle, within RotatEBound
+        ext = dict(dpos=dpos, dneg=dneg) if mode == "backward_ext" else {}
+        want = xo.oracle_step(model, ent, rel, t, eta, corr, None, loss=loss, rot_table=True, **ext)
+        bound = xo.RotatEBound(ent, rel, t, want, eta, loss=None if ext else loss)
+        for name, ok, ratio in bound.check(_dense(ref, g_e), _dense(ref, g_r), want.g_ent, want.g_rel):
+            assert ok, (name, "worst error / bound %.3g" % ratio)
     for e in ranks + [ref]:
         e.close()
 

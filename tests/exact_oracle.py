@@ -290,6 +290,89 @@ EPS_RSQ = 2.0 ** -22.9
 ROT_C = 8  # roundings of one gradient element outside the term sums: back-rotation (2), inv_div (1), the Z / Aphi fma
 
 
+def loss_chain(loss, lp, sp, sn):
+    """Per score of each positive ([eta+1, B], row 0 the positive): c such that the rounding of the kernels' loss chain
+    (loss_and_dscores, kge_train_common.cuh, built without fast math) moves its dL/dscore by at most c u mag
+    (loss_magnitudes), u = 2^-24.  Library maths (CUDA C Programming Guide, Mathematical Functions): expf 2 ulp (4u),
+    logf / log1pf 1 ulp (2u); x / y is the IEEE quotient (1u); w = fl(1 / eta) and w2 = fl(1 / (2 eta)) 1u each (2 eta
+    is exact).  A sum of m nonzero terms in any order (lane loops, warp sums: adds of exact zeros are exact) rounds each
+    term at most m - 1 times.  In units of u:
+      pairwise:        dN = w (1), dP = -(sum of eta copies of w) (eta);  absolute_margin: dP = -w eta (2).
+      nll:             q = e / (1 + e): e 4, 1 + e 5, quotient 1 -> 10; dN = (w2 inN) q: 12; dP = -w2 eta inP q: 13.
+      multiclass_nll:  D = w sum_j e_j + pe: e_j 4, the sum eta - 1, w and its product 2, the add 1 -> eta + 6;
+                       dN = ((w inN) e_j) / D: eta + 13; dP = inP (pe / D - 1): eta + 11, then 1 relative to
+                       pe / D + 1 (mag_pos) -> eta + 12.
+      -> 2 eta + 16 covers these three (and nll's 13).
+      self_adversarial (both code paths, eta <= 32 and the looped one): with A = max_j (alpha |N_j| + |alpha N_j - mx|)
+        (the rounding of exp's argument alpha N - mx, amplified by exp into a relative error) and X = max(|P + m|,
+        max_j |N_j + m|) (that of x = -N - m, and of the positive's m + P), e_j: 4 + A; z: eta - 1 + 4 + A;
+        p_j = e_j / z: eta + 8 + 2A; t = exp(-|x|): 4 + X; log1p(t): (6 + X) log1p(t) since t / (1 + t) <= log1p(t);
+        l_j = min(x, 0) - log1p(t): (7 + X) |l_j| (both parts have the sign of l_j); sg_j: 10 + 2X; S = sum p l:
+        (2 eta + 7 + 2 (4 + A) + X) |S| (all l_j <= 0, so |S| = sum p |l|); pj sg: eta + 19 + 2A + 2X;
+        alpha pj (l_j - S): (3 eta + 26 + 4A + X) (|l_j| + |S|); the difference, w and its product 3 more:
+        -> 3 eta + 30 + 4A + 2X relative to mag_neg = w p (sg + alpha (|l| + |S|)); dP = -1 / (1 + exp(m + P)): 6 + X."""
+    sp, sn = sp.detach(), sn.detach()
+    eta = sn.shape[0]
+    c = torch.full((eta + 1, sp.shape[0]), float(2 * eta + 16), dtype=torch.float64, device=sp.device)
+    if loss == "self_adversarial":
+        lp = dict(lp or {})
+        m, a = lp.get("margin", 3.0), lp.get("alpha", 0.5)
+        an = a * sn
+        A = (an.abs() + (an - an.max(0, keepdim=True).values).abs()).max(0).values
+        X = torch.maximum((sp + m).abs(), (sn + m).abs().max(0).values)
+        c = (3 * eta + 30 + 4 * A + 2 * X)[None].expand(eta + 1, -1).clone()
+    return c
+
+
+def loss_premises(loss, lp, sp, sn, dsp_err, dsn_err):
+    """The data's premises for a fused step whose scores are off by up to dsp_err / dsn_err: no hinge argument of
+    pairwise (m - P + N, two roundings of at most u (|m| + |P| + |N|) on top of the score errors) or absolute_margin
+    (m + N, one rounding, which keeps the sign) lies within its error of 0, where dL/dscore jumps; no clipped loss's
+    (nll, multiclass_nll) score lies within its error of +-75, where the clip mask flips.  Asserted, not assumed."""
+    lp = dict(lp or {})
+    u = FP32_EPS
+    if loss in ("pairwise", "absolute_margin"):
+        mg = lp.get("margin", 1.0)
+        if loss == "pairwise":
+            arg = mg - sp[None] + sn
+            err = dsn_err + dsp_err[None] + 2 * u * (1 + 2 * u) * (abs(mg) + sp.abs()[None] + sn.abs())
+        else:
+            arg, err = mg + sn, dsn_err
+        assert not bool((arg.abs() <= err).any()), "premise: a hinge argument lies within its score bound of 0"
+    if loss in ("nll", "multiclass_nll"):
+        for s, e in ((sp, dsp_err), (sn, dsn_err)):
+            assert not bool(((s.abs() - ref_step.CLIP_HI).abs() <= e).any()), "premise: a score within its bound of 75"
+
+
+def loss_error(loss, lp, step, eta, dsp_err, dsn_err, device):
+    """dL/dscore error and loss error of a fused step whose scores are off by up to dsp_err [B] / dsn_err [eta, B],
+    shared by RotatEBound and TrilinearBound.  -> (dg [B + eta*B] in step's score order, loss_err).
+      dg_j = sum_i |H_ji| ds_i (loss_score_sensitivity: the positive's Hessian block, first order) + c_j u mag_j
+      (loss_chain); loss None (KGE_STEP_BACKWARD_EXT): the given dL/dscore is exact, dg = 0.
+      The loss: per positive sum_j |g_j| ds_j + (c + 16) u (|L_i| + sum_j |g_j| (|s_j| + |margin|) + eta + 1), c the
+      positive's largest chain: each of its eta + 1 loss terms phi is evaluated with at most c roundings relative to
+      |phi|, to its argument (|phi'| |s + margin|, and |phi'| = |g| / w is carried by the loss's own factor w) and to 1
+      (logf / log1pf of a quantity near 1 err by a unit absolute), then summed (eta more) and accumulated in fp64."""
+    u = FP32_EPS
+    B = dsp_err.shape[0]
+    if loss is None:
+        return torch.zeros(B * (eta + 1), dtype=torch.float64, device=device), 0.0
+    lp = dict(lp or {})
+    sp, snn = step.sp.to(device).double(), step.sn.to(device).double().reshape(eta, B)
+    loss_premises(loss, lp, sp, snn, dsp_err, dsn_err)
+    hp, hn = loss_score_sensitivity(loss, lp, sp, snn, dsp_err, dsn_err)
+    c = loss_chain(loss, lp, sp, snn)
+    mag = torch.cat([step.mag_pos.to(device).double()[None], step.mag_neg.to(device).double().reshape(eta, B)], 0)
+    dg = torch.cat([hp, hn.reshape(-1)]) + u * torch.cat([(c * mag)[0], (c * mag)[1:].reshape(-1)])
+    gl = torch.cat([step.dsp[None], step.dsn.reshape(eta, B)], 0).to(device).double().abs()
+    sc = torch.cat([sp[None], snn], 0).abs()
+    err = torch.cat([dsp_err[None], dsn_err], 0)
+    mg = abs(lp.get("margin", 3.0 if loss == "self_adversarial" else 1.0))
+    loss_err = float((gl * err).sum() + (u * (c.max(0).values + 16) * (gl * (sc + mg)).sum(0)).sum()
+                     + (c.max(0).values + 16).max() * u * (abs(step.loss) + (eta + 1) * B))
+    return dg, loss_err
+
+
 def loss_score_sensitivity(loss, lp, sp, sn, dsp_err, dsn_err):
     """Per score j of each positive: sum_i |d^2 L / d s_j d s_i| ds_i over the positive's eta + 1 scores (the
     (eta+1)^2 Hessian block of per_positive_loss, float64 autograd): how far a score error ds moves dL/dscore.
@@ -339,11 +422,10 @@ class RotatEBound:
         the residual, |v|^2's rounding (2u relative, half of it through the sqrt) and sqrt.approx, the sum of h moduli
         (float4 sums, fma with the lane mask, warp sum), and sqrt.approx.ftz flushing |v|^2 < 2^-126 to 0
         (sqrt(2^-125) < 2^-62).
-      * Fused losses.  dg_j = sum_i |H_ji| delta s_i (loss_score_sensitivity: the positive's Hessian block) plus the
-        loss chain's own roundings (2 eta + 16) u mag_j (loss_magnitudes, as for the trilinear models).  For pairwise
-        and absolute_margin the Hessian is 0 away from the hinge, so the data must keep every hinge argument farther
-        than its score bound from 0 (asserted: a premise of the data, not a property of the kernel).
-      * Loss.  sum_i (sum_j |g_ij| delta s_ij + (2 eta + 32) u (|L_i| + sum_j |g_ij| (|s_ij| + |margin|) + eta)).
+      * Fused losses and the loss value: loss_error (shared with TrilinearBound).  dg_j = sum_i |H_ji| delta s_i (the
+        positive's Hessian block) plus the loss chain's own roundings (loss_chain).  For pairwise and absolute_margin
+        the Hessian is 0 away from the hinge, so the data must keep every hinge argument farther than its error from 0
+        (loss_premises: asserted, a premise of the data, not a property of the kernel).
     loss None: KGE_STEP_BACKWARD_EXT (g given and exact, dg = 0)."""
 
     def __init__(self, ent, rel, triples, step, eta, loss=None, loss_params=None, max_rel_size=None, device="cpu"):
@@ -372,25 +454,7 @@ class RotatEBound:
         mm = m + dv
         self.score_err = ((dv + mm * (EPS_SQRT + 2 * u)).sum(1) + (h + 16) * u * mm.sum(1) + h * 2.0 ** -62)
         dsp_err, dsn_err = self.score_err[:B], self.score_err[B:].reshape(eta, B)
-        if loss is None:
-            dg = torch.zeros_like(g)
-        else:
-            lp = dict(loss_params or {})
-            sp, snn = step.sp.to(dev).double(), step.sn.to(dev).double().reshape(eta, B)
-            if loss in ("pairwise", "absolute_margin"):
-                mg = lp.get("margin", 1.0)
-                arg = mg - sp[None] + snn if loss == "pairwise" else mg + snn
-                near = arg.abs() <= dsn_err + (dsp_err[None] if loss == "pairwise" else 0)
-                assert not bool(near.any()), "premise: a hinge argument lies within its score bound of 0"
-            hp, hn = loss_score_sensitivity(loss, loss_params, sp, snn, dsp_err, dsn_err)
-            mag = torch.cat([step.mag_pos, step.mag_neg]).to(dev).double()
-            dg = torch.cat([hp, hn.reshape(-1)]) + (2 * eta + 16) * u * mag
-            gl = torch.cat([step.dsp[None], step.dsn.reshape(eta, B)], 0).to(dev).double().abs()
-            sc = torch.cat([sp[None], snn], 0).abs()
-            err = torch.cat([dsp_err[None], dsn_err], 0)
-            mg = abs(lp.get("margin", 3.0 if loss == "self_adversarial" else 1.0))
-            self.loss_err = float((gl * err).sum() + (2 * eta + 32) * u * (abs(step.loss) + (gl * (sc + mg)).sum()
-                                                                            + eta * B))
+        dg, self.loss_err = loss_error(loss, loss_params, step, eta, dsp_err, dsn_err, dev)
         ga, dga = g.abs()[:, None], dg[:, None]
         rel_e = torch.where(m > 0, 2 * dv / torch.where(m > 0, m, torch.ones_like(m)) + EPS_RSQ + 4 * u
                             + 2.0 ** -125 / torch.where(m > 0, m * m, torch.ones_like(m)), torch.full_like(m, np.inf))
@@ -429,6 +493,127 @@ class RotatEBound:
         got = torch.as_tensor(got, dtype=torch.float64).to(self.device)
         err = (got - torch.as_tensor(want, dtype=torch.float64).to(self.device)).abs()
         return bool((err <= bound).all()), float((err / bound).max()) if err.numel() else 0.0
+
+
+# --------------------------------------------------------------------------
+# DistMult, ComplEx, HolE and TransE: a per-element bound
+# --------------------------------------------------------------------------
+TRI_C = 5  # roundings of one gradient term outside its register and row sums (TrilinearBound)
+
+
+def score_chain(model, K):
+    """Roundings any one product (TransE: column) of a score passes through in the training kernels (TrilinearBound)."""
+    halves = 1 if model in ("TransE", "DistMult") else 2
+    kp = -(-(K // halves) // 4) * 4
+    return halves * (-(-kp // 128) + -(-kp // 512)) + -(-kp // 512) + 11
+
+
+class TrilinearBound:
+    """The per-element error bound of one DistMult / ComplEx / HolE / TransE training step (the general kernel, the
+    resident fast path kge_train_res_kernel in its scatter and GATHER forms, the bucket sum and the deferred owner
+    kernel, which share the per-model functions of kge_train_common.cuh) against oracle_step in float64.  u = 2^-24;
+    |.| of a term below is its value with every product counted positive (abs_scores on |tables|).
+      * Scores.  A trilinear score is a sum of m products (DistMult m = k; ComplEx / HolE four per complex column).
+        Each product carries: its query vector (query_subj / query_obj: pr * orr is one rounding, the ComplEx forms
+        two: a product and an fma or a subtraction), the lane's fma chain into its float4 chunk sums (at most
+        HALVES ceil(kp / 128) fmas, plus one per column window of the general kernel: HALVES ceil(kp / 512)), f4hsum
+        (2), the warp sum (5 shuffle levels), the sum over column windows (ceil(kp / 512)), and HolE's scale: 2 / k is
+        stored as fl(2 / k) (1, exact when k is a power of two) and multiplied in (1).  TransE: the residual s + p - o
+        in two roundings (the residual has magnitude at most |s| + |p| + |o|, its sign is exact by the premise below),
+        f4abssum (2), the lane chain, the warp sum.  So |delta s| <= score_chain u |s| + m 2^-149 (subnormal
+        products), score_chain = HALVES (ceil(kp / 128) + ceil(kp / 512)) + ceil(kp / 512) + 11.
+      * dL/dscore.  loss_error: the score errors through each positive's Hessian block, plus loss_chain (derived there:
+        expf / logf / log1pf without fast math, w = 1 / eta and w2 = 1 / (2 eta), multiclass_nll's pe / D - 1 and
+        self_adversarial's p_j (l_j - S)), under loss_premises (hinge arguments and clip bounds away from the kinks).
+        KGE_STEP_BACKWARD_EXT: g is given and exact, dg = 0.
+      * Gradient elements.  Element x of a row is sum_j g_j d s_j / d x.  The kernel scales g by fl(2 / k) for HolE
+        (2 roundings, 0 otherwise).  A replaced row's term is g * Q (Q: 2, the product: 1).  The kept rows are formed
+        in factored form: U = gP s + sum_j g_j r_j (and X for the object slot) is a register sum of eta + 1 fmas, then
+        query_subj / query_obj (2) or trilinear_grad_p (3: two products / fmas and the final add); TransE sums
+        g_j sign(residual) (exact by the premise) over eta + 1 terms and adds the kept shares (2 adds).  So each term
+        passes through at most TRI_C = 5 roundings of its own and eta + 1 register adds.  The row's contributions (one
+        per positive lookup: the kept rows' REDs or hot-entity registers; one per replaced lookup: REDs, bucket runs, the
+        owner kernel's grad[e] + sum) are summed in some order with at most n - 1 adds, n the row's positive lookups
+        plus its replaced lookups (a corruption's kept side is folded into its positive's register sum).  With g's error dg (|g + dg| <= mag + dg, loss_magnitudes):
+            |err| <= (n + eta + 2 + 8 + TRI_C) u sum_j (mag_j + dg_j) |d s_j / d x| + sum_j dg_j |d s_j / d x|
+                     + 2^-126 (n + eta + 10)
+        (within_bound with A = grad_bound(mag + dg), absolute = grad_bound(dg)).  The 8 covers the second-order terms:
+        (1 + u)^N - 1 - N u <= N^2 u^2 / (1 - N u) <= 8 u for N <= 11,000 (asserted); 2^-126 per add for the
+        atomics' and sums' flushed subnormal results.
+      * Premise of TransE: no residual s + p - o lies within 2 u (1 + u) (|s| + |p| + |o|) of 0, where |x|' jumps
+        (asserted on the data).
+      * Loss: loss_error."""
+
+    def __init__(self, model, ent, rel, triples, step, eta, loss=None, loss_params=None, device="cpu"):
+        assert model in TRILINEAR + ("TransE",)
+        u = FP32_EPS
+        dev = self.device = torch.device(device)
+        E = torch.as_tensor(np.asarray(ent), dtype=torch.float64, device=dev)
+        R = torch.as_tensor(np.asarray(rel), dtype=torch.float64, device=dev)
+        K = E.shape[1]
+        t = torch.as_tensor(np.asarray(triples), dtype=torch.long, device=dev)
+        B = t.shape[0]
+        T = torch.cat([t, step.corr.to(dev)], 0)
+        Ea, Ra = E.abs(), R.abs()
+        asc = abs_scores(model, Ea[T[:, 0]], Ra[T[:, 1]], Ea[T[:, 2]])
+        m = K if model in ("TransE", "DistMult") else 2 * K
+        self.score_err = score_chain(model, K) * u * asc + m * 2.0 ** -149
+        if model == "TransE":
+            for a in range(0, T.shape[0], 1 << 16):
+                Tc = T[a:a + (1 << 16)]
+                res = E[Tc[:, 0]] + R[Tc[:, 1]] - E[Tc[:, 2]]
+                tol = 2 * u * (1 + 2 * u) * (Ea[Tc[:, 0]] + Ra[Tc[:, 1]] + Ea[Tc[:, 2]])
+                assert not bool((res.abs() <= tol).any()), "premise: a TransE residual lies within its rounding of 0"
+        dsp_err, dsn_err = self.score_err[:B], self.score_err[B:].reshape(eta, B)
+        dg, self.loss_err = loss_error(loss, loss_params, step, eta, dsp_err, dsn_err, dev)
+        mag = torch.cat([step.mag_pos, step.mag_neg]).to(dev).double() + dg
+        (A0, _, _), (A1, _, _) = grad_bound(model, ent, rel, triples, step.corr, mag[:B], mag[B:], dev)
+        (X0, _, _), (X1, _, _) = grad_bound(model, ent, rel, triples, step.corr, dg[:B], dg[B:], dev)
+        self.A, self.X = [A0, A1], [X0, X1]
+        # a row's contributions: one per positive lookup (the kept rows' register sums) and one per replaced lookup
+        tc = T[B:]
+        repl = torch.where(tc[:, 0] != t[:, 0].repeat(eta), tc[:, 0], tc[:, 2])
+        n_e = torch.bincount(torch.cat([t[:, 0], t[:, 2], repl]), minlength=E.shape[0]).double()[:, None]
+        n_r = torch.bincount(t[:, 1], minlength=R.shape[0]).double()[:, None]
+        self.n = [n_e + eta + 2, n_r + eta + 2]
+        assert max(float(n.max()) for n in self.n) + 8 + TRI_C <= 11000, "second-order allowance"
+
+    def check(self, got_ent, got_rel, want_ent, want_rel):
+        """-> [(name, ok, worst error / bound)] for both gradient tables."""
+        out = []
+        for i, (name, got, want) in enumerate((("g_ent", got_ent, want_ent), ("g_rel", got_rel, want_rel))):
+            want = torch.as_tensor(want, dtype=torch.float64).to(self.device)
+            got = torch.as_tensor(got, dtype=torch.float64).to(self.device)
+            if not bool(torch.isfinite(got).all()):
+                out.append((name, False, float("inf")))
+                continue
+            ok, ratio = within_bound(got, want, self.A[i], self.n[i] + 8, self.n[i], TRI_C, self.X[i])
+            out.append((name, ok, ratio))
+        return out
+
+    check_scores = RotatEBound.check_scores
+
+
+# --------------------------------------------------------------------------
+# engine plumbing shared by the GPU tests
+# --------------------------------------------------------------------------
+def dense(eng, table):
+    """padded [rows, ld] -> dense [rows, internal_k] float64 on the host, and whether every pad column is 0."""
+    t = table.detach().cpu()
+    k, kp = eng.k, eng.kp
+    if eng.internal_k == k:
+        return t[:, :k].double(), bool((t[:, k:] == 0).all())
+    d = torch.cat([t[:, :k], t[:, kp:kp + k]], 1).double()
+    return d, bool((t[:, k:kp] == 0).all()) and bool((t[:, kp + k:] == 0).all())
+
+
+def launched(run):
+    """Names of the library's kernels that run() launched (torch.profiler, CUDA activities)."""
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        run()
+        torch.cuda.synchronize()
+    return {e.key for e in prof.key_averages() if "kge_" in e.key}
 
 
 # --------------------------------------------------------------------------

@@ -36,16 +36,6 @@ def _dev(a):
     return torch.as_tensor(np.ascontiguousarray(a)).cuda().contiguous()
 
 
-def _dense(eng, table):
-    """padded [rows, ld] -> dense [rows, internal_k] float64 on the host, and whether every pad column is 0."""
-    t = table.detach().cpu()
-    k, kp = eng.k, eng.kp
-    if eng.internal_k == k:
-        return t[:, :k].double(), bool((t[:, k:] == 0).all())
-    dense = torch.cat([t[:, :k], t[:, kp:kp + k]], 1).double()
-    return dense, bool((t[:, k:kp] == 0).all()) and bool((t[:, kp + k:] == 0).all())
-
-
 def _bucketed_entries(eng):
     """Entries the bucket pre-pass placed in the last step (offset[n_ent] of the workspace's CSR)."""
     ws = eng._train_ws.view(torch.int32)
@@ -108,8 +98,8 @@ def train_exact(model, k, eta, E, R, B, kind, rng, neg_group=0, negatives="injec
     else:
         eng.forward_backward(_dev(t), neg, seed=seed, step=step, scores_pos=sp, scores_neg=sn)
     torch.cuda.synchronize()
-    g_ent, ent_pads = _dense(eng, eng.g_ent)
-    g_rel, rel_pads = _dense(eng, eng.g_rel)
+    g_ent, ent_pads = xo.dense(eng, eng.g_ent)
+    g_rel, rel_pads = xo.dense(eng, eng.g_rel)
     facts = dict(resident=eng.lib.kge_rows_resident(eng.h), loss=eng.read_loss(),
                  bucketed=_bucketed_entries(eng) if getattr(eng, "_train_ws", None) is not None else 0,
                  ws_bytes=int(eng.lib.kge_train_workspace_bytes(eng.h, B)), launches=eng.launches,
@@ -307,8 +297,8 @@ def test_exact_deferred_sgd(model, k, momentum, reg, monkeypatch):
                 acc[i] = (momentum * acc[i] if acc[i] is not None else 0.0) - lr * gg
                 new.append(x0 + acc[i])
             xo.assert_fp32_exact(new[-1], "updated table")
-        got_e, pe = _dense(eng, eng.ent)
-        got_r, pr = _dense(eng, eng.rel)
+        got_e, pe = xo.dense(eng, eng.ent)
+        got_r, pr = xo.dense(eng, eng.rel)
         assert torch.equal(got_e, new[0]) and torch.equal(got_r, new[1]), (step, (got_e - new[0]).abs().max())
         assert pe and pr  # pads of the block the step wrote
         reg_loss = lam * (float((torch.as_tensor(ent, dtype=torch.float64) ** 2).sum())
@@ -330,7 +320,7 @@ def _run_rows(model, k, eta, ent, rel, t, ne, nk, loss, lp, kernel=None, monkeyp
     sp, sn = torch.empty(B, device="cuda"), torch.empty(eta * B, device="cuda")
     eng.forward_backward(_dev(t), (_dev(ne), _dev(nk)), scores_pos=sp, scores_neg=sn)
     torch.cuda.synchronize()
-    out = (sp.cpu().double(), sn.cpu().double(), _dense(eng, eng.g_ent)[0], _dense(eng, eng.g_rel)[0], eng.read_loss())
+    out = (sp.cpu().double(), sn.cpu().double(), xo.dense(eng, eng.g_ent)[0], xo.dense(eng, eng.g_rel)[0], eng.read_loss())
     eng.close()
     return out
 

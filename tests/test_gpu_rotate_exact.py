@@ -26,14 +26,6 @@ def _dev(a):
     return torch.as_tensor(np.ascontiguousarray(a)).cuda().contiguous()
 
 
-def _dense(eng, table):
-    """padded [rows, ld] -> dense [rows, 2k] float64 on the host, and whether every pad column is 0."""
-    t = table.detach().cpu()
-    k, kp = eng.k, eng.kp
-    dense = torch.cat([t[:, :k], t[:, kp:kp + k]], 1).double()
-    return dense, bool((t[:, k:kp] == 0).all()) and bool((t[:, kp + k:] == 0).all())
-
-
 def _force(monkeypatch, **env):
     for var in ("KGE_B200_TRAIN_KERNEL", "KGE_B200_TRAIN_SCHED", "KGE_B200_TRAIN_NBUF", "KGE_B200_ROT_G"):
         monkeypatch.delenv(var, raising=False)
@@ -79,15 +71,6 @@ def _tables(rng, E, R, k, edge):
         rel[0] = 0.0
         rel[1:] = (rng.uniform(-1e4, 1e4, (R - 1, K)) * float(div)).astype(np.float32)
     return ent, rel
-
-
-def _launched(run):
-    """Names of the library's kernels that run() launched (torch.profiler, CUDA activities)."""
-    from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        run()
-        torch.cuda.synchronize()
-    return {e.key for e in prof.key_averages() if "kge_" in e.key}
 
 
 def run_case(monkeypatch, k, eta, *, E=2000, R=11, B=300, mode="ext", loss="self_adversarial", lp=None, path="rot",
@@ -139,14 +122,14 @@ def run_case(monkeypatch, k, eta, *, E=2000, R=11, B=300, mode="ext", loss="self
         kw.update(mode=_lib.STEP_BACKWARD_EXT, dpos=_dev(ext["dpos"]), dneg=_dev(ext["dneg"]))
     else:
         kw.update(mode=_lib.STEP_FORWARD_ONLY if mode == "forward" else _lib.STEP_FUSED, scores_pos=sp, scores_neg=sn)
-    names = _launched(lambda: eng.forward_backward(_dev(t), neg, **kw))
-    g_ent, ent_pads = _dense(eng, eng.g_ent)
-    g_rel, rel_pads = _dense(eng, eng.g_rel)
+    names = xo.launched(lambda: eng.forward_backward(_dev(t), neg, **kw))
+    g_ent, ent_pads = xo.dense(eng, eng.g_ent)
+    g_rel, rel_pads = xo.dense(eng, eng.g_rel)
     got_loss = eng.read_loss()
     for _ in range(3):  # a short profiling session now and then records no kernel at all: replay the step's scores
         if names:       # (FORWARD_ONLY into scratch buffers: the same kernel choice, nothing the checks read is written)
             break
-        names = _launched(lambda: eng.forward_backward(
+        names = xo.launched(lambda: eng.forward_backward(
             _dev(t), neg, seed=seed_, step=step_, mode=_lib.STEP_FORWARD_ONLY,
             scores_pos=torch.empty(B, device="cuda"), scores_neg=torch.empty(eta * B, device="cuda")))
     eng.close()

@@ -1,0 +1,303 @@
+"""DistMult, ComplEx, HolE and TransE training element by element on real-valued tables: the scores, the loss and every
+element of g_ent and g_rel of one step against the float64 oracle, within exact_oracle.TrilinearBound (derived in its
+docstring), for every loss, on the general kernel, the resident fast path (scatter with static and dynamic assignment
+and hot entities; GATHER with the bucket sum) and the deferred owner kernel.  The launched kernel names and the
+bucketed entry count tell which path ran.
+
+Each case asserts the kernels it targets ran (the library's path decision for the engine, its bucketed entry count and
+deferral, and the launched kernel names from torch.profiler whenever a profiling session records them), holds
+the exact properties with no tolerance (pad columns and every row no term touches are 0), prints its worst error /
+bound ratio, and shows the check is sensitive on the device: the kernel's output fails it against the oracle with one
+corruption's dL/dscore multiplied by 1 + 2^-10.
+
+The deferred step never leaves its gradient in g_ent.  It trains with SGD, momentum 0.5 and lr = 2^-6 from a zero slot:
+update4 forms a = fma(0, mu, -(g lr)) = -(g lr) exactly (lr a power of two), so -slot0 / lr is the owner kernel's full
+gradient (fused-kernel REDs plus bucket sum), checked against the bound, and the new table must be fl32(x0 + slot0)."""
+import os
+import zlib
+
+import numpy as np
+import pytest
+import torch
+
+import exact_oracle as xo
+from ampligraph_b200 import _lib
+
+pytestmark = pytest.mark.gpu
+
+SA = ("self_adversarial", {"margin": 3.0, "alpha": 0.5})
+LOSSES = [("nll", {}), ("multiclass_nll", {}), SA, ("pairwise", {"margin": 0.5}), ("absolute_margin", {"margin": 1.0}),
+          ("ext", {}), ("nll", {"reduction": "mean"}), ("multiclass_nll", {"reduction": "mean"}),
+          ("self_adversarial", {"margin": 3.0, "alpha": 0.5, "reduction": "mean"}),
+          ("pairwise", {"margin": 0.5, "reduction": "mean"})]
+RES_PATHS = ["general", "static", "dynamic", "hot", "gather", "deferred"]
+LR = 2.0 ** -6
+
+
+def _seed(*a):
+    return zlib.crc32(repr(a).encode())
+
+
+def _dev(a):
+    return torch.as_tensor(np.ascontiguousarray(a)).cuda().contiguous()
+
+
+def _glorot(rng, rows, K):
+    lim = np.sqrt(6.0 / (rows + K))
+    return rng.uniform(-lim, lim, (rows, K)).astype(np.float32)
+
+
+def _force(monkeypatch, **env):
+    for var in ("KGE_B200_TRAIN_KERNEL", "KGE_B200_TRAIN_SCHED", "KGE_B200_TRAIN_REPL", "KGE_B200_TRAIN_NBUF"):
+        monkeypatch.delenv(var, raising=False)
+    for var, val in env.items():
+        if val is not None:
+            monkeypatch.setenv(var, str(val))
+
+
+def _bucketed_entries(eng):
+    ws = eng._train_ws.view(torch.int32)
+    off0 = (4 * eng.n_ent + 15) // 16 * 4
+    return int(ws[off0 + eng.n_ent].item())
+
+
+def run_case(monkeypatch, model, k, eta, *, E=2000, R=11, B=600, loss="nll", lp=None, path="general", neg_group=0,
+             nbuf=None, stash=False, negatives="injected", triples=None, oracle_device="cpu", chunk=None, seed=0):
+    """One step on Glorot tables; every element checked against TrilinearBound.  path: 'general', the resident fast
+    path with the atomic scatter ('static', 'dynamic', 'hot': static with hot entities), 'gather' (the bucket sum) or
+    'deferred' (the owner kernel, read through the SGD momentum slot)."""
+    lp = dict(lp or {})
+    rng = np.random.default_rng(_seed(model, k, eta, E, B, loss, str(sorted(lp.items())), path, neg_group, nbuf, stash,
+                                      negatives, seed))
+    env = {"general": dict(KGE_B200_TRAIN_KERNEL="general"), "static": dict(KGE_B200_TRAIN_REPL="scatter",
+           KGE_B200_TRAIN_SCHED="static"), "dynamic": dict(KGE_B200_TRAIN_REPL="scatter", KGE_B200_TRAIN_SCHED="dynamic"),
+           "hot": dict(KGE_B200_TRAIN_REPL="scatter", KGE_B200_TRAIN_SCHED="static"),
+           "gather": dict(KGE_B200_TRAIN_REPL="gather"), "deferred": {}}[path]
+    _force(monkeypatch, KGE_B200_TRAIN_NBUF=nbuf, **env)
+    from ampligraph_b200.engine import KGEEngine
+    K = xo.internal_k(model, k)
+    ent, rel = _glorot(rng, E, K), _glorot(rng, R, K)
+    t = triples if triples is not None else xo.zipf_triples(E, R, B, rng)
+    ext = loss == "ext"
+    eloss, elp = ("pairwise", {}) if ext else (loss, lp)
+    opt = dict(optimizer="sgd", optimizer_params={"learning_rate": LR, "momentum": 0.5}) if path == "deferred" else {}
+    eng = KGEEngine(model, k, eta, E, R, loss=eloss, loss_params=elp, neg_group=neg_group, **opt)
+    if stash:
+        st = eng.ensure_row_stash(B)
+        assert st is not None, "expected a geometry that stashes"
+        st.fill_(float("nan"))
+    if path == "hot":
+        eng.set_hot_entities(triples=t)
+        assert len(eng.hot_entities) == 2
+    eng.set_embeddings(ent, rel)
+    sp = torch.full((B,), float("nan"), device="cuda")
+    sn = torch.full((eta * B,), float("nan"), device="cuda")
+    if negatives == "philox":
+        seed_, step_ = 7, 2
+        corr = eng.generate_corruptions(_dev(t), seed=seed_, step=step_).cpu().numpy()
+        neg, ne, nk = None, corr, None
+    else:
+        ne = rng.integers(0, E, eta * B).astype(np.int32)
+        nk = rng.integers(0, 2, eta * B).astype(np.uint8)
+        if negatives == "skewed":  # buckets of thousands: nearly every corruption replaces one of three entities
+            few = rng.random(eta * B) < 0.99
+            ne[few] = rng.choice(np.array([3, 77, 500], np.int32), int(few.sum()))
+        tiled = np.tile(t, (eta, 1))
+        same = rng.random(eta * B) < 0.03  # N = P: the replaced entity is the one it replaces
+        ne[same] = np.where(nk[same] == 1, tiled[same, 2], tiled[same, 0])
+        seed_, step_, neg = 0, 0, (_dev(ne), _dev(nk))
+    kw = dict(seed=seed_, step=step_)
+    dext = {}
+    if ext:
+        dext = dict(dpos=rng.uniform(-1, 1, B).astype(np.float32), dneg=rng.uniform(-1, 1, eta * B).astype(np.float32))
+        kw.update(mode=_lib.STEP_BACKWARD_EXT, dpos=_dev(dext["dpos"]), dneg=_dev(dext["dneg"]))
+    else:
+        kw.update(scores_pos=sp, scores_neg=sn)
+    x0 = [xo.dense(eng, eng.ent)[0], xo.dense(eng, eng.rel)[0]]
+    # The library's own decision for this handle (kge_api.cu: train_path, bucket_workspace_bytes, which read the
+    # environment at each call): without the scatter override a step of B positives buckets exactly where it runs the
+    # resident fast path.  It holds whether or not a profiling session records the kernels.
+    repl = os.environ.get("KGE_B200_TRAIN_REPL")
+    monkeypatch.delenv("KGE_B200_TRAIN_REPL", raising=False)
+    facts = dict(res_path=int(eng.lib.kge_train_workspace_bytes(eng.h, B)) > 0)
+    if repl is not None:
+        monkeypatch.setenv("KGE_B200_TRAIN_REPL", repl)
+
+    def step():
+        launches = eng.launches
+        eng.forward_backward(_dev(t), neg, defer=path == "deferred", **kw)
+        facts["deferred"] = eng._deferred
+        facts["loss"] = eng.read_loss() if not ext else None
+        if path == "deferred":
+            eng.apply_gradients()
+        facts["launches"] = eng.launches - launches
+
+    names = xo.launched(step)
+    facts.update(stash=getattr(eng, "row_stash", None) is not None,
+                 bucketed=_bucketed_entries(eng) if getattr(eng, "_train_ws", None) is not None else 0)
+    if path == "deferred":
+        slot = [xo.dense(eng, eng.slots[key][0]) for key in ("ent", "rel")]
+        new = [xo.dense(eng, eng.ent), xo.dense(eng, eng.rel)]
+        (g_ent, ent_pads), (g_rel, rel_pads) = [(-s / LR, pads) for s, pads in slot]
+    else:
+        g_ent, ent_pads = xo.dense(eng, eng.g_ent)
+        g_rel, rel_pads = xo.dense(eng, eng.g_rel)
+    fused = "kge_train_kernel<" if path == "general" else "kge_train_res_kernel<"
+    seen = set(names)
+    for _ in range(5):  # a short profiling session now and then records no kernel at all: replay the step's scores
+        if any(fused in n for n in seen):
+            break
+        seen |= xo.launched(lambda: eng.forward_backward(
+            _dev(t), neg, seed=seed_, step=step_, mode=_lib.STEP_FORWARD_ONLY,
+            scores_pos=torch.empty(B, device="cuda"), scores_neg=torch.empty(eta * B, device="cuda")))
+    eng.close()
+    where = "%s k=%d eta=%d %s %s %s group=%d nbuf=%s stash=%s %s E=%d B=%d" % (
+        model, k, eta, path, loss, lp, neg_group, nbuf, stash, negatives, E, B)
+
+    # the kernels that ran
+    assert facts["res_path"] == (path != "general" and not stash), where
+    if seen:  # a session that recorded the library's kernels must show the targeted one
+        assert any(fused in n for n in seen), (where, sorted(seen))
+    else:
+        print("\n%s: the profiler recorded no kernel in six sessions; the path rests on the library's decision" % where)
+    if path == "general":
+        assert facts["bucketed"] == 0, where
+    else:
+        if path in ("static", "dynamic", "hot"):
+            assert facts["bucketed"] == 0, where
+        else:
+            assert facts["bucketed"] == eta * B, where
+            after = {"gather": "kge_bucket_sum_kernel", "deferred": "kge_bucket_owner_kernel"}[path]
+            assert not names or any(after in n for n in names), (where, sorted(names))
+            assert facts["deferred"] == (path == "deferred"), where
+            if path == "deferred":
+                assert facts["launches"] == 5, where  # pre-pass (3), fused kernel, deferred sum + optimizer
+    assert facts["stash"] == stash, where
+
+    ref = xo.oracle_step(model, ent, rel, t, eta, ne, nk, loss=eloss, loss_params=elp, device=oracle_device,
+                         chunk=chunk, **dext)
+    bound = xo.TrilinearBound(model, ent, rel, t, ref, eta, loss=None if ext else loss, loss_params=lp,
+                              device=oracle_device)
+    ratios = {}
+    if not ext:
+        for name, got, want in (("sp", sp, ref.sp), ("sn", sn, ref.sn)):
+            ok, ratios[name] = bound.check_scores(got.cpu().double(), want, name)
+            assert ok, (where, name, ratios[name])
+        assert abs(facts["loss"] - ref.loss) <= bound.loss_err, (where, facts["loss"], ref.loss, bound.loss_err)
+        ratios["loss"] = abs(facts["loss"] - ref.loss) / bound.loss_err
+    for name, ok, r in bound.check(g_ent, g_rel, ref.g_ent, ref.g_rel):
+        ratios[name] = r
+        assert ok, (where, name, "worst error / bound %.3g" % r)
+    print("\n%s: worst error / bound %s" % (where, {n: round(r, 4) for n, r in ratios.items()}))
+
+    # exact properties
+    assert ent_pads and rel_pads, where + ": pad columns written"
+    corr = ref.corr.cpu().numpy()
+    touched_e = np.zeros(E, bool)
+    touched_e[np.concatenate([t[:, 0], t[:, 2], corr[:, 0], corr[:, 2]])] = True
+    touched_r = np.zeros(R, bool)
+    touched_r[t[:, 1]] = True
+    assert bool((g_ent[~touched_e] == 0).all()) and bool((g_rel[~touched_r] == 0).all()), where + ": untouched rows"
+    if path == "deferred":
+        for (got, pads), x, s in zip(new, x0, slot):
+            assert pads, where + ": pad columns of the new block"
+            assert torch.equal(got, (x.float() + s[0].float()).double()), where + ": new table != fl32(x0 + slot0)"
+
+    # sensitivity: one corruption's dL/dscore times 1 + 2^-10 (its replaced entity has at most 32 lookups)
+    lookups = np.bincount(np.concatenate([t[:, 0], t[:, 2], corr[:, 0], corr[:, 2]]), minlength=E)
+    tiled = np.tile(t, (eta, 1))
+    repl = np.where(corr[:, 0] != tiled[:, 0], corr[:, 0], corr[:, 2])
+    keep = (corr[:, 0] == tiled[:, 0]).astype(np.uint8)
+    g = ref.dsn.abs().cpu().numpy()
+    cands = np.nonzero((lookups[repl] <= 32) & (g > 0))[0]
+    assert len(cands), where + ": no corruption with a replaced entity of at most 32 lookups"
+    r = int(min(cands, key=lambda c: (lookups[repl[c]], -g[c])))
+    i = r % B
+    one = xo.oracle_step(model, ent, rel, t[i:i + 1], 1, [repl[r]], [keep[r]], dpos=[0.0],
+                         dneg=[float(ref.dsn[r]) * 2.0 ** -10], device=oracle_device)
+    res = bound.check(g_ent, g_rel, ref.g_ent + one.g_ent, ref.g_rel + one.g_rel)
+    assert not all(ok for _, ok, _ in res), where + ": the check accepts a perturbed dL/dscore"
+
+
+# ---------------------------------------------------------------------------
+# every loss on every path: the path of (model, loss) rotates, so each loss meets each path across the models
+# ---------------------------------------------------------------------------
+MODEL_K = [("DistMult", 130), ("ComplEx", 100), ("HolE", 100)]
+CASES = []
+for a, (m, k) in enumerate(MODEL_K):
+    for b, (l, p) in enumerate(LOSSES):
+        path = RES_PATHS[(a + 2 * b) % len(RES_PATHS)]
+        if path == "deferred" and l == "ext":
+            path = "gather"
+        CASES.append(pytest.param(m, k, l, p, path, id="%s-%s-%s-%s" % (m, l, p.get("reduction", "sum"), path)))
+for l, p in LOSSES:  # TransE scores lie near -12 here (the relation rows dominate): margin 15 keeps the hinges active
+    p = dict(p, margin=15.0) if l == "absolute_margin" else p
+    CASES.append(pytest.param("TransE", 100, l, p, "general", id="TransE-%s-%s-general" % (l, p.get("reduction", "sum"))))
+
+
+@pytest.mark.parametrize("model,k,loss,lp,path", CASES)
+def test_losses_and_paths(model, k, loss, lp, path, monkeypatch):
+    """eta = 10 (mean is not dyadic: w = fl(1 / 10)); k = 100 and 130 are not powers of two (HolE's 2 / k inexact)."""
+    run_case(monkeypatch, model, k, 10, loss=loss, lp=lp, path=path)
+
+
+# ---------------------------------------------------------------------------
+# the general kernel's groups, single buffering, column windows and row stash
+# ---------------------------------------------------------------------------
+GENERAL = [dict(model="DistMult", k=130, neg_group=1, loss="self_adversarial"),
+           dict(model="ComplEx", k=100, neg_group=3, loss="multiclass_nll"),
+           dict(model="HolE", k=100, neg_group=3, nbuf=1, loss="nll"),
+           dict(model="TransE", k=100, neg_group=3, nbuf=1, loss="self_adversarial"),
+           dict(model="DistMult", k=1100, loss="nll"), dict(model="ComplEx", k=520, neg_group=3, loss="self_adversarial"),
+           dict(model="ComplEx", k=130, neg_group=3, stash=True, loss="nll"),
+           dict(model="DistMult", k=1100, neg_group=1, stash=True, loss="multiclass_nll")]
+
+
+@pytest.mark.parametrize("case", GENERAL, ids=lambda c: "-".join("%s%s" % kv for kv in sorted(c.items())))
+def test_general_kernel_geometries(case, monkeypatch):
+    case = dict(case)
+    lp = SA[1] if case["loss"] == "self_adversarial" else {}
+    run_case(monkeypatch, case.pop("model"), case.pop("k"), 7, path="general", lp=lp, B=300, **case)
+
+
+# ---------------------------------------------------------------------------
+# edges
+# ---------------------------------------------------------------------------
+@pytest.mark.parametrize("eta", [33, 70])
+@pytest.mark.parametrize("model", ["DistMult", "ComplEx"])
+def test_self_adversarial_looped(model, eta, monkeypatch):
+    """eta > 32: self_adversarial's looped branch (general kernel), with Philox corruptions."""
+    run_case(monkeypatch, model, 100, eta, loss=SA[0], lp=SA[1], path="general", B=200, negatives="philox")
+
+
+@pytest.mark.parametrize("model,k,loss", [("ComplEx", 100, "self_adversarial"), ("DistMult", 130, "nll"),
+                                          ("HolE", 100, "multiclass_nll")])
+def test_bucket_edges(model, k, loss, monkeypatch):
+    """Buckets of thousands of entries (99 % of the corruptions replace one of three entities): the bucket sum and the
+    deferred owner kernel."""
+    lp = SA[1] if loss == "self_adversarial" else {}
+    for path in ("gather", "deferred"):
+        run_case(monkeypatch, model, k, 5, loss=loss, lp=lp, path=path, B=2000, negatives="skewed")
+
+
+def test_scan_tiles(monkeypatch):
+    """100,000 entities: 13 tiles of the bucket pre-pass's two-level scan, Philox corruptions, bucket sum."""
+    run_case(monkeypatch, "DistMult", 8, 5, E=100000, B=20000, loss="nll", path="gather", negatives="philox",
+             oracle_device="cuda")
+
+
+# ---------------------------------------------------------------------------
+# the workloads' full shapes (oracle in float64 on the GPU, chunked)
+# ---------------------------------------------------------------------------
+@pytest.mark.parametrize("path", ["gather", "deferred"])
+def test_cfg2_full_shape(path, monkeypatch):
+    """ComplEx k=200, eta=10, 14,505 entities, 237 relations, 27,212 Zipf positives, self_adversarial: fused with the
+    bucket sum, and deferred through the owner kernel."""
+    run_case(monkeypatch, "ComplEx", 200, 10, E=14505, R=237, B=27212, loss=SA[0], lp=SA[1], path=path,
+             oracle_device="cuda", chunk=4096)
+
+
+def test_cfg3_full_shape(monkeypatch):
+    """DistMult k=400, eta=20, 40,943 entities, 8,684 Zipf positives, pairwise (NIT = 4 rows), bucket sum."""
+    run_case(monkeypatch, "DistMult", 400, 20, E=40943, R=18, B=8684, loss="pairwise", lp={"margin": 0.5},
+             path="gather", oracle_device="cuda", chunk=4096)

@@ -17,9 +17,8 @@ import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import measure  # noqa: E402
 from ampligraph_b200.engine import DBSCAN_BATCH, INT32_MAX, KGEEngine, dbscan_labels  # noqa: E402
-from topk_bench import gpu_info  # noqa: E402
 
 PHASES = ("count", "compact", "union", "flatten", "border", "relabel")
 
@@ -138,7 +137,7 @@ def case_c(iters=3):
 
 
 if __name__ == "__main__":
-    print(gpu_info(), flush=True)
+    print(measure.card(), flush=True)
     which = sys.argv[1:] or ["ab", "c"]
     for c in which:
         {"ab": case_ab, "c": case_c}[c]()

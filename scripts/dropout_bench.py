@@ -11,36 +11,16 @@ pass).  Prints the GPU and its power limit first: every number depends on both.
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import measure  # noqa: E402
 
 E, R, K_USER, B = 14541, 237, 200, 1000  # FB15k-237, ComplEx k = 200
 DROPOUT = (0.4, 0.2)
-
-
-def gpu_info():
-    name = torch.cuda.get_device_name(0)
-    try:
-        pl = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                            stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True).stdout.strip()
-    except OSError:
-        pl = "unknown"
-    return "%s, power limit / max SM clock: %s" % (name, pl)
-
-
-def timed(fn, iters):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / iters
 
 
 def main():
@@ -52,7 +32,7 @@ def main():
     from ampligraph_b200.datasets import FilterIndex, k_vs_all_queries
     from ampligraph_b200.engine import KGEEngine
 
-    info = gpu_info()
+    info = measure.card()
     print(info)
     rng = np.random.default_rng(0)
     t = np.stack([rng.integers(0, E, B), rng.integers(0, R, B), rng.integers(0, E, B)], 1).astype(np.int32)
@@ -78,11 +58,12 @@ def main():
         times = {"off": [], "on": []}
         for setting in ("off", "on"):  # warm-up: modules, workspace, both settings
             eng.set_embedding_dropout(*(DROPOUT if setting == "on" else (0.0, 0.0)), seed=3)
-            timed(step, 3)
+            for _ in range(3):
+                step()
         for _ in range(a.rounds):
             for setting in ("off", "on"):
                 eng.set_embedding_dropout(*(DROPOUT if setting == "on" else (0.0, 0.0)), seed=3)
-                times[setting].append(timed(step, a.iters))
+                times[setting].append(measure.window_ms(step, a.iters, 0))
         off_ms, on_ms = float(np.median(times["off"])), float(np.median(times["on"]))
         # the dropout kernels' own time, profiled in a pass of its own
         eng.set_embedding_dropout(*DROPOUT, seed=3)

@@ -18,51 +18,13 @@ Prints the GPU and its power limit first: every number depends on both.
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-SA = {"margin": 3.0, "alpha": 0.5}
-
-
-def gpu_info():
-    name = torch.cuda.get_device_name(0)
-    try:
-        pl = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                            stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True).stdout.strip()
-    except OSError:
-        pl = "unknown"
-    return "%s, power limit / max SM clock: %s" % (name, pl)
-
-
-def events(fn, iters, warmup=3):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    ms = []
-    for _ in range(iters):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        fn()
-        e1.record()
-        torch.cuda.synchronize()
-        ms.append(e0.elapsed_time(e1))
-    return ms
-
-
-def triples(E, R, B, seed):
-    rng = np.random.default_rng(seed)
-    # Zipf(1.0) entities, as bench.py's synthetic KG: frequent entities repeat within a batch
-    w = 1.0 / np.arange(1, E + 1)
-    p = w / w.sum()
-    t = np.stack([rng.choice(E, B, p=p), rng.integers(0, R, B), rng.choice(E, B, p=p)], 1)
-    return torch.as_tensor(t.astype(np.int32)).cuda().contiguous()
-
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import measure  # noqa: E402
 
 
 W_N, W_P = 1e-3, 1e-3  # lambda 1e-3, alpha = beta = 1
@@ -73,7 +35,7 @@ def dura_engine(E, R, B, seed, **kw):
     from ampligraph_b200.engine import KGEEngine
     eng = KGEEngine("ComplEx", 200, kw.pop("eta", 1), E, R, regularizer=[DURA, DURA], **kw)
     eng.init_glorot_uniform(seed=seed)
-    return eng, triples(E, R, B, seed)
+    return eng, measure.zipf_triples(E, R, B, seed)
 
 
 def row_bytes(eng):
@@ -82,7 +44,7 @@ def row_bytes(eng):
 
 def alone(E, R, B, iters):
     eng, t = dura_engine(E, R, B, 1)
-    ms = float(np.median(events(lambda: eng.dura_backward(t), iters)))
+    ms = float(np.median(measure.per_call_ms(lambda: eng.dura_backward(t), iters, 3)))
     moved = B * (6 * row_bytes(eng) + 12)
     eng.close()
     return {"n_ent": E, "n_rel": R, "B": B, "ms": ms, "bytes": moved, "GB_per_s": moved / (ms * 1e-3) / 1e9}
@@ -109,7 +71,7 @@ def torch_baseline(iters):
         eng.g_ent.index_add_(0, ti[:, 2], o.grad)
         eng.g_rel.index_add_(0, ti[:, 1], r.grad)
         return loss.detach()
-    ms = float(np.median(events(step, iters)))
+    ms = float(np.median(measure.per_call_ms(step, iters, 3)))
     eng._gblock.zero_()
     eng.loss_acc.zero_()
     want = float(step())
@@ -120,41 +82,9 @@ def torch_baseline(iters):
     return {"B": B, "ms": ms, "loss_torch": want, "loss_kernel": got}
 
 
-def alternated(kind, rounds, iters):
-    """Median step time with DURA off and on, alternated round by round on one engine."""
-    from ampligraph_b200.engine import KGEEngine
-    if kind == "sampled":
-        E, R, B = 14505, 237, 27212
-        eng = KGEEngine("ComplEx", 200, 10, E, R, loss="self_adversarial", loss_params=SA, optimizer="adam",
-                        regularizer=[DURA, DURA])
-    else:
-        E, R, B = 14541, 237, 1000
-        eng = KGEEngine("ComplEx", 200, 1, E, R, loss="multiclass_nll", optimizer="adam", regularizer=[DURA, DURA])
-    eng.init_glorot_uniform(seed=2)
-    t = triples(E, R, B, 3)
-    eng.set_hot_entities(triples=t)
-    state = {"step": 0}
-
-    def step(dura):
-        s = state["step"]
-        if kind == "sampled":
-            eng.forward_backward(t, None, seed=0, step=s, defer=True)
-            assert eng._deferred
-        else:
-            eng.one_vs_all_backward(t, "s,o", step=s)
-        if dura:
-            eng.dura_backward(t, step=s)
-        eng.apply_gradients()
-        state["step"] += 1
-    res = {"off": [], "on": []}
-    for _ in range(rounds):
-        for key, dura in (("off", False), ("on", True)):
-            res[key] += events(lambda: step(dura), iters, warmup=2)
-    eng.close()
-    off, on = float(np.median(res["off"])), float(np.median(res["on"]))
-    return {"kind": kind, "B": B, "ms_off": off, "ms_on": on, "dura_share_pct": 100.0 * (on - off) / on,
-            "spread_off_ms": [float(np.percentile(res["off"], 10)), float(np.percentile(res["off"], 90))],
-            "spread_on_ms": [float(np.percentile(res["on"], 10)), float(np.percentile(res["on"], 90))]}
+def steps(kind, rounds, iters):
+    res = measure.regularizer_steps(kind, [DURA, DURA], lambda eng, t, s: eng.dura_backward(t, step=s), rounds, iters)
+    return dict(res, dura_share_pct=100.0 * (res["ms_on"] - res["ms_off"]) / res["ms_on"])
 
 
 def main():
@@ -165,11 +95,11 @@ def main():
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("dura_bench.py needs a CUDA device: there is no CPU measurement")
-    print(gpu_info(), flush=True)
-    res = {"gpu": gpu_info(), "alone": [alone(14505, 237, 27212, a.iters), alone(14541, 237, 1000, a.iters),
-                                        alone(10 ** 6, 237, 27212, a.iters)],
+    print(measure.card(), flush=True)
+    res = {"gpu": measure.card(), "alone": [alone(14505, 237, 27212, a.iters), alone(14541, 237, 1000, a.iters),
+                                            alone(10 ** 6, 237, 27212, a.iters)],
            "torch_baseline": torch_baseline(a.iters),
-           "steps": [alternated("sampled", a.rounds, a.iters), alternated("one_vs_all", a.rounds, a.iters)]}
+           "steps": [steps("sampled", a.rounds, a.iters), steps("one_vs_all", a.rounds, a.iters)]}
     print(json.dumps(res, indent=1))
     if a.out:
         with open(a.out, "w") as f:

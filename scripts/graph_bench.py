@@ -22,28 +22,13 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import bench  # noqa: E402
+import measure  # noqa: E402
 from ampligraph_b200 import discovery  # noqa: E402
 from ampligraph_b200.engine import graph_counts_csr, graph_csr  # noqa: E402
-from topk_bench import gpu_info  # noqa: E402
 
 STRATEGIES = ("random_uniform", "entity_frequency", "graph_degree", "cluster_coefficient", "cluster_triangles",
               "cluster_squares")
-
-
-def events(fn, iters):
-    fn()
-    torch.cuda.synchronize()
-    ms = []
-    for _ in range(iters):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        torch.cuda.synchronize()
-        ms.append(a.elapsed_time(b))
-    return float(np.median(ms))
 
 
 def kernel_arm(name, t, n, iters):
@@ -52,8 +37,8 @@ def kernel_arm(name, t, n, iters):
     degree, d, offsets, nbr, order = csr
     wedges = int((d * d).sum())
     res = {"graph": name, "nodes": n, "edges": int(nbr.numel() // 2), "max_d": int(d.max()), "wedges": wedges,
-           "csr_ms": events(lambda: graph_csr(td, n), iters),
-           "kernel_ms": events(lambda: graph_counts_csr(offsets, nbr, order), iters)}
+           "csr_ms": float(np.median(measure.per_call_ms(lambda: graph_csr(td, n), iters, 1))),
+           "kernel_ms": float(np.median(measure.per_call_ms(lambda: graph_counts_csr(offsets, nbr, order), iters, 1)))}
     res["wedges_per_s"] = 2 * wedges / (res["kernel_ms"] * 1e-3)  # pass 1 and pass 3 each walk every wedge
     print(json.dumps(res), flush=True)
     return res
@@ -73,7 +58,7 @@ def main():
     ap.add_argument("--networkx", action="store_true")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
-    info = gpu_info()
+    info = measure.card()
     print(info, flush=True)
     out = {"gpu": info, "kernel": [], "discovery": []}
 

@@ -17,48 +17,23 @@ Prints the GPU, its power limit and max SM clock first: every number depends on 
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import measure  # noqa: E402
 
 E, R, K_USER = 14541, 237, 200  # FB15k-237, ComplEx k = 200
 FP32_PEAK = 67e12  # H100 SXM data sheet, dense fp32, 700 W
 SMOOTHING = 0.1
 
 
-def gpu_info():
-    name = torch.cuda.get_device_name(0)
-    try:
-        pl = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                            stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True).stdout.strip()
-    except OSError:
-        pl = "unknown"
-    return "%s, power limit / max SM clock: %s" % (name, pl)
-
-
 def flops(B, ld):
     """Operations of one side: dQ and dX each form the logits and accumulate a gradient (4 contractions), an FMA
     counted as 2."""
     return 4 * 2 * B * E * ld
-
-
-def events(fn, iters, warmup=3):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    ms = []
-    for _ in range(iters):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        fn()
-        e1.record()
-        torch.cuda.synchronize()
-        ms.append(e0.elapsed_time(e1))
-    return float(np.median(ms))
 
 
 def torch_step(ent, rel, t, side, y):
@@ -107,8 +82,8 @@ def setup(B, side):
 
 def run(B, side, iters):
     ent, rel, q, off, ids, kva, ova, kva_step, ova_step = setup(B, side)
-    ms = events(kva_step, iters)
-    ms_ova = events(ova_step, iters)
+    ms = float(np.median(measure.per_call_ms(kva_step, iters, 3)))
+    ms_ova = float(np.median(measure.per_call_ms(ova_step, iters, 3)))
     # agreement with the baseline on one step from zeroed accumulators
     kva.loss_acc.zero_()
     kva_step()
@@ -120,7 +95,7 @@ def run(B, side, iters):
     y[torch.repeat_interleave(torch.arange(B), torch.as_tensor(np.diff(off))).cuda(), torch.as_tensor(ids).long().cuda()] = 1.0
     y = (1.0 - SMOOTHING) * y + SMOOTHING / E
     base_loss = float(torch_step(te, tr, tl, side, y).detach())
-    ms_torch = events(lambda: torch_step(te, tr, tl, side, y), iters)
+    ms_torch = float(np.median(measure.per_call_ms(lambda: torch_step(te, tr, tl, side, y), iters, 3)))
     ld = kva.ld
     kva.close()
     ova.close()
@@ -167,7 +142,7 @@ def main():
         sys.exit("k_vs_all_bench.py needs a GPU: times are measured on the device, never estimated")
     torch.backends.cuda.matmul.allow_tf32 = False
     torch.backends.cudnn.allow_tf32 = False
-    info = gpu_info()
+    info = measure.card()
     print(info, flush=True)
     if args.profile:
         profile(args.profile)

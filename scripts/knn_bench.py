@@ -18,9 +18,8 @@ import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import measure  # noqa: E402
 from ampligraph_b200.engine import KGEEngine  # noqa: E402
-from topk_bench import gpu_info, timed  # noqa: E402
 
 
 def case_a(iters=20, rounds=3):
@@ -36,9 +35,10 @@ def case_a(iters=20, rounds=3):
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
     res = {"euclidean": [], "manhattan": [], "topk": []}
     for _ in range(rounds):  # alternated, so that drift of the shared machine hits all three alike
-        res["topk"].append(timed(lambda: te.topk(t, "o", top), flush, iters))
+        res["topk"].append(np.median(measure.per_call_ms(lambda: te.topk(t, "o", top), iters, 2, before=flush.zero_)))
         for metric in ("euclidean", "manhattan"):
-            res[metric].append(timed(lambda: cx.knn(cx.ent, q, top, metric), flush, iters))
+            res[metric].append(np.median(measure.per_call_ms(lambda: cx.knn(cx.ent, q, top, metric), iters, 2,
+                                                             before=flush.zero_)))
     tk = np.median(res["topk"])
     print("(a) E=%d ld=400 b=%d top=%d: kge_topk TransE k=400 side o %.1f us" % (E, b, top, tk * 1e3))
     for metric in ("euclidean", "manhattan"):
@@ -64,7 +64,8 @@ def case_b(iters=10):
             off = torch.arange(qq.numel() + 1, dtype=torch.int64, device="cuda")
             eng.knn(pts, qq, 1, metric, n_cand=E, filt_off=off, filt_idx=qq)
     for metric in ("euclidean", "manhattan"):
-        print("(b) nearest-other-row pass, %d x 400, %-9s %.2f ms" % (E, metric, timed(lambda: d1_pass(metric), flush, iters)))
+        ms = np.median(measure.per_call_ms(lambda: d1_pass(metric), iters, 2, before=flush.zero_))
+        print("(b) nearest-other-row pass, %d x 400, %-9s %.2f ms" % (E, metric, ms))
     eng.close()
 
 
@@ -152,14 +153,14 @@ def case_d(iters=3):
     q = torch.as_tensor(rng.integers(0, E, b).astype(np.int32)).cuda()
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
     for metric in ("euclidean", "manhattan"):
-        ms = timed(lambda: eng.knn(eng.ent, q, top, metric), flush, iters)
+        ms = np.median(measure.per_call_ms(lambda: eng.knn(eng.ent, q, top, metric), iters, 2, before=flush.zero_))
         print("(d) kge_knn E=%d ld=400 b=%d top=%d %-9s %.2f ms (%.1f G distances/s)"
               % (E, b, top, metric, ms, b * E / ms / 1e6))
     eng.close()
 
 
 if __name__ == "__main__":
-    print(gpu_info(), flush=True)
+    print(measure.card(), flush=True)
     which = sys.argv[1:] or ["a", "b", "c", "d"]
     for c in which:
         {"a": case_a, "b": case_b, "c": case_c, "d": case_d}[c]()

@@ -26,9 +26,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "scripts"))
-
-from dura_bench import events, gpu_info  # noqa: E402
+import measure  # noqa: E402
 
 MODES = [(s, f) for s in ("uniform", "bernoulli", "pseudo_typed") for f in (False, True)]
 ATTEMPTS = 10  # models.NEGATIVE_FILTER_ATTEMPTS
@@ -50,7 +48,7 @@ def main():
     import bench
     from ampligraph_b200.datasets import negative_sampler_tables
     from ampligraph_b200.engine import KGEEngine, NegativeSamplerTables
-    print(gpu_info(), flush=True)
+    print(measure.card(), flush=True)
     c = bench.CFG
     E, R, B, eta = c["n_ent"], c["n_rel"], c["batch"], c["eta"]
     kg = bench.synthetic_kg(E, R, c["n_triples"])
@@ -64,7 +62,7 @@ def main():
     for mode in MODES:
         host = negative_sampler_tables(kg, E, R, mode[0], mode[1])
         tables[mode] = NegativeSamplerTables(host, ATTEMPTS, eng.device)
-    res = {"gpu": gpu_info(), "workload": "cfg2: ComplEx k=200, eta=10, B=27,212, FB15k-237-shaped synthetic KG",
+    res = {"gpu": measure.card(), "workload": "cfg2: ComplEx k=200, eta=10, B=27,212, FB15k-237-shaped synthetic KG",
            "kernel_us": {}, "step_ms": {}, "known_share": {}}
 
     # the kernel alone: its device time from torch.profiler (CUDA events around one call would also time the host's
@@ -76,7 +74,7 @@ def main():
         def call():
             eng.sample_negatives(batch, tables[mode], 0, state["step"])
             state["step"] += 1
-        call_ms = events(call, a.iters)
+        call_ms = measure.per_call_ms(call, a.iters, 3)
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             for _ in range(a.iters):
                 call()
@@ -109,10 +107,7 @@ def main():
         eng.apply_gradients()
         state["step"] += 1
     kinds = ["in-kernel", "injected", "injected pseudo_typed"] + MODES
-    times = {k: [] for k in map(str, kinds)}
-    for _ in range(a.rounds):
-        for kind in kinds:
-            times[str(kind)] += events(lambda: step(kind), a.iters, warmup=2)
+    times = measure.alternated({str(k): lambda k=k: step(k) for k in kinds}, a.rounds, a.iters, 2)
     for kind in kinds:
         ms = times[str(kind)]
         key = kind if isinstance(kind, str) else "sampler " + name(kind)

@@ -15,46 +15,21 @@ limit first: every number depends on both.
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import measure  # noqa: E402
 
 E, R, K_USER = 14541, 237, 200  # FB15k-237, ComplEx k = 200
 FP32_PEAK = 67e12  # H100 SXM data sheet, dense fp32, 700 W
 
 
-def gpu_info():
-    name = torch.cuda.get_device_name(0)
-    try:
-        pl = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                            stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True).stdout.strip()
-    except OSError:
-        pl = "unknown"
-    return "%s, power limit / max SM clock: %s" % (name, pl)
-
-
 def flops(B, ld, sides=2):
     """Operations of the five contractions per side (stats, dQ logits + Gq, dX logits + Gx), an FMA counted as 2."""
     return sides * 5 * 2 * B * E * ld
-
-
-def events(fn, iters, warmup=3):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    ms = []
-    for _ in range(iters):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        fn()
-        e1.record()
-        torch.cuda.synchronize()
-        ms.append(e0.elapsed_time(e1))
-    return float(np.median(ms))
 
 
 def torch_step(ent, rel, t):
@@ -86,7 +61,7 @@ def run(B, iters):
 
     def step():
         eng.one_vs_all_backward(t, "s,o")
-    ms = events(step, iters)
+    ms = float(np.median(measure.per_call_ms(step, iters, 3)))
     # agreement with the baseline on one step from zeroed accumulators
     eng.g_ent.zero_()
     eng.g_rel.zero_()
@@ -97,7 +72,7 @@ def run(B, iters):
     tr = torch.as_tensor(rel).cuda().requires_grad_(True)
     tl = torch.as_tensor(X).long().cuda()
     base_loss = float(torch_step(te, tr, tl).detach())
-    ms_torch = events(lambda: torch_step(te, tr, tl), iters)
+    ms_torch = float(np.median(measure.per_call_ms(lambda: torch_step(te, tr, tl), iters, 3)))
     ld = eng.ld
     eng.close()
     fl = flops(B, ld)
@@ -120,7 +95,7 @@ def main():
         sys.exit("one_vs_all_bench.py needs a GPU: times are measured on the device, never estimated")
     torch.backends.cuda.matmul.allow_tf32 = False
     torch.backends.cudnn.allow_tf32 = False
-    info = gpu_info()
+    info = measure.card()
     print(info, flush=True)
     results = {"gpu": info, "runs": [run(B, args.iters) for B in (256, 1000, 4096)]}
     if args.out:

@@ -18,13 +18,13 @@ import argparse
 import ctypes as C
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import measure  # noqa: E402
 from ampligraph_b200 import _lib  # noqa: E402
 from ampligraph_b200.engine import KGEEngine, optimizer_slots  # noqa: E402
 
@@ -32,12 +32,6 @@ KINDS = [("adam", {}), ("rmsprop", {}), ("rmsprop", {"centered": True}), ("rmspr
          ("adadelta", {"learning_rate": 1.0}), ("adamax", {}), ("nadam", {}), ("ftrl", {}),
          ("ftrl", {"learning_rate_power": -0.25})]
 E, R, K, ETA, B = 14505, 237, 200, 10, 27212
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                       text=True)
-    return q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name(0)
 
 
 def zipf_triples(n, rng):
@@ -48,28 +42,17 @@ def zipf_triples(n, rng):
     return np.stack([s, rng.integers(0, R, n), o], 1).astype(np.int32)
 
 
-def time_calls(call, iters, warmup, before=None):
-    """mean device time of call() in microseconds.  Without `before`: back-to-back calls between two events.  With it:
-    before() runs outside each timed call; it queues GPU work (a training step), so the timed call's launch waits on the
-    stream rather than on the host."""
+def time_calls(call, before, iters, warmup):
+    """mean device time of call() in microseconds, with before() run outside each timed call.  before() queues GPU work
+    (a training step), so the timed call's launch waits on the stream rather than on the host."""
     for _ in range(warmup):
-        if before:
-            before()
+        before()
         call()
     torch.cuda.synchronize()
-    ev = lambda: torch.cuda.Event(enable_timing=True)
-    if before is None:
-        a, b = ev(), ev()
-        a.record()
-        for _ in range(iters):
-            call()
-        b.record()
-        b.synchronize()
-        return 1e3 * a.elapsed_time(b) / iters
     marks = []
     for _ in range(iters):
         before()
-        a, b = ev(), ev()
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record()
         call()
         b.record()
@@ -85,7 +68,7 @@ def main():
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("optim_bench.py needs a CUDA device")
-    print("card, power limit: %s" % card())
+    print(measure.card())
     rng = np.random.default_rng(0)
     t = torch.as_tensor(zipf_triples(B, rng)).cuda()
     for name, params in KINDS:
@@ -103,7 +86,7 @@ def main():
             eng.begin_step()
             _lib.check(eng.lib.kge_optimizer_step(eng.h, C.byref(eng.opt_cfg), eng.t, ptr(eng._pblock), ptr(eng._gblock),
                                                   ptr(eng._sblocks[0]), ptr(eng._sblocks[1]), rows, None, eng._stream()))
-        us = time_calls(dense, args.iters, args.warmup)
+        us = 1e3 * measure.window_ms(dense, args.iters, args.warmup)
         print(json.dumps({"kernel": "kge_optimizer_step", "kind": label, "us": round(us, 2), "streams": streams,
                           "GB_per_s": round(nbytes / us / 1e3, 1)}))
 
@@ -114,7 +97,7 @@ def main():
             step[0] += 1
             assert eng._deferred
 
-        us = time_calls(eng.apply_gradients, args.iters, args.warmup, before=pend)
+        us = time_calls(eng.apply_gradients, pend, args.iters, args.warmup)
         print(json.dumps({"kernel": "kge_optimizer_step_deferred", "kind": label, "us": round(us, 2), "streams": streams,
                           "GB_per_s": round(nbytes / us / 1e3, 1)}))
         if name == "nadam":
@@ -125,7 +108,7 @@ def main():
                 _lib.check(eng.lib.kge_optimizer_step_decay(eng.h, C.byref(eng.opt_cfg), eng.t, ptr(eng._pblock),
                                                             ptr(eng._gblock), ptr(eng._sblocks[0]), ptr(eng._sblocks[1]),
                                                             rows, ptr(stamps), 1, eng._stream()))
-            us = time_calls(decay, args.iters, args.warmup)
+            us = 1e3 * measure.window_ms(decay, args.iters, args.warmup)
             dbytes = rows * ld * 4 * 6 + rows * 4  # half the rows 8 streams, half 4, and the stamps
             print(json.dumps({"kernel": "kge_optimizer_step_decay", "kind": label, "us": round(us, 2), "streams": 6,
                               "GB_per_s": round(dbytes / us / 1e3, 1)}))

@@ -15,7 +15,6 @@ import argparse
 import importlib.util
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -69,12 +68,11 @@ def bench_split(args):
 
 
 def bench_gpu(args):
+    import measure
     import torch
     from ampligraph_b200.evaluation import select_best_model_ranking
     from ampligraph_b200.latent_features import ScoringBasedEmbeddingModel
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                       text=True)
-    print(q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name(0))
+    print(measure.card())
     X = zipf_labels(272115 + 17535 + 20466, 1)
     train, valid, test = X[:272115], X[272115:272115 + 17535], X[272115 + 17535:]
     m = ScoringBasedEmbeddingModel(eta=10, k=200, scoring_type="ComplEx", seed=0)

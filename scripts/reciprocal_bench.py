@@ -18,7 +18,6 @@ number depends on both.
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -26,37 +25,10 @@ import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import measure  # noqa: E402
 
 E, R, K_USER = 14541, 237, 200  # FB15k-237, ComplEx k = 200
 N_TRAIN, N_TEST = 272115, 20466
-
-
-def gpu_info():
-    name = torch.cuda.get_device_name(0)
-    try:
-        pl = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                            stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True).stdout.strip()
-    except OSError:
-        pl = "unknown"
-    return "%s, power limit / max SM clock: %s" % (name, pl)
-
-
-def timed_pair(a, b, iters, warmup=3):
-    """Median ms of a() and b() over iters calls each, alternated, CUDA events around each call."""
-    for _ in range(warmup):
-        a()
-        b()
-    torch.cuda.synchronize()
-    ms = ([], [])
-    for _ in range(iters):
-        for fn, out in ((a, ms[0]), (b, ms[1])):
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            fn()
-            e1.record()
-            torch.cuda.synchronize()
-            out.append(e0.elapsed_time(e1))
-    return float(np.median(ms[0])), float(np.median(ms[1]))
 
 
 def triples(rng, n):
@@ -77,8 +49,9 @@ def step_run(B, iters):
     plain.set_embeddings(ent, rel[:R])
     recip = KGEEngine("ComplEx", K_USER, 1, E, 2 * R, loss="multiclass_nll", optimizer="sgd")
     recip.set_embeddings(ent, rel)
-    ms_recip, ms_plain = timed_pair(lambda: recip.one_vs_all_backward(recip_rows, "o"),
-                                    lambda: plain.one_vs_all_backward(plain_rows, "s,o"), iters)
+    ms = measure.alternated({"reciprocal": lambda: recip.one_vs_all_backward(recip_rows, "o"),
+                             "plain": lambda: plain.one_vs_all_backward(plain_rows, "s,o")}, iters, 1, 3)
+    ms_recip, ms_plain = float(np.median(ms["reciprocal"])), float(np.median(ms["plain"]))
     plain.close()
     recip.close()
     res = {"B": B, "reciprocal_ms": ms_recip, "plain_ms": ms_plain, "ratio": ms_recip / ms_plain}
@@ -132,7 +105,7 @@ def main():
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("reciprocal_bench.py needs a GPU: times are measured on the device, never estimated")
-    info = gpu_info()
+    info = measure.card()
     print(info, flush=True)
     results = {"gpu": info, "steps": [step_run(B, args.iters) for B in (256, 1000, 4096)],
                "evaluate": eval_run(args.eval_iters)}

@@ -14,7 +14,6 @@ number depends on both.
 """
 import argparse
 import os
-import subprocess
 import sys
 import time
 
@@ -22,19 +21,10 @@ import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import measure  # noqa: E402
 
 # (name, entities, relations, test triples)
 SHAPES = [("FB15k-237", 14505, 237, 20466), ("FB15k", 14951, 1345, 59071), ("YAGO3-10", 123182, 37, 5000)]
-
-
-def gpu_info():
-    name = torch.cuda.get_device_name(0)
-    try:
-        pl = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                            stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True).stdout.strip()
-    except OSError:
-        pl = "unknown"
-    return "%s, power limit / max SM clock: %s" % (name, pl)
 
 
 def pair_flops(model, k):
@@ -43,20 +33,6 @@ def pair_flops(model, k):
     halves of mul + fma + fma (10); RotatE the rotation (2 mul + 2 fma = 6), two differences, the squared modulus
     (mul + fma = 3), sqrt and the sum (13)."""
     return k * {"TransE": 3, "DistMult": 3, "ComplEx": 10, "HolE": 10, "RotatE": 13}[model]
-
-
-def events(fn, iters):
-    fn()
-    torch.cuda.synchronize()
-    ms = []
-    for _ in range(iters):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        fn()
-        e1.record()
-        torch.cuda.synchronize()
-        ms.append(e0.elapsed_time(e1))
-    return float(np.median(ms))
 
 
 def wall(fn, iters):
@@ -104,9 +80,9 @@ def run(model, k, name, E, R, b, iters):
     eng = m.engine
     X = np.stack([rng.integers(0, E, b), rng.integers(0, R, b), rng.integers(0, E, b)], 1).astype(np.int32)
     t = torch.as_tensor(X).cuda()
-    rank_ms = events(lambda: eng.rank(t, "p", "worst"), iters)
-    topk_ms = events(lambda: eng.topk(t, "p", 10), iters)
-    base_ms = events(lambda: baseline_ranks(eng, t, R), iters)
+    rank_ms = float(np.median(measure.per_call_ms(lambda: eng.rank(t, "p", "worst"), iters, 1)))
+    topk_ms = float(np.median(measure.per_call_ms(lambda: eng.topk(t, "p", 10), iters, 1)))
+    base_ms = float(np.median(measure.per_call_ms(lambda: baseline_ranks(eng, t, R), iters, 1)))
     ev_ms = wall(lambda: m.evaluate(X, corrupt_side="p", verbose=False), iters)
     evf_ms = wall(lambda: m.evaluate(X, corrupt_side="p", use_filter={"test": X}, verbose=False), iters)
     q_ms = wall(lambda: query_topn_batch(m, X, side="p", top_n=10), max(1, iters // 2))
@@ -130,7 +106,7 @@ def main():
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("relation_bench.py needs a GPU: times are measured on the device, never estimated")
-    print(gpu_info(), flush=True)
+    print(measure.card(), flush=True)
     for model in args.models.split(","):
         for name, E, R, b in SHAPES:
             run(model, 200, name, E, R, b, args.iters)

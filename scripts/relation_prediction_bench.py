@@ -31,34 +31,10 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+import measure  # noqa: E402
 
 E, R, K_USER = 14541, 237, 200  # FB15k-237, ComplEx k = 200
 BATCHES = (256, 1000, 4096)
-
-
-def gpu_info():
-    name = torch.cuda.get_device_name(0)
-    try:
-        pl = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                            stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True).stdout.strip()
-    except OSError:
-        pl = "unknown"
-    return "%s, power limit / max SM clock: %s" % (name, pl)
-
-
-def events(fn, iters, warmup=3):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    ms = []
-    for _ in range(iters):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        fn()
-        e1.record()
-        torch.cuda.synchronize()
-        ms.append(e0.elapsed_time(e1))
-    return float(np.median(ms))
 
 
 def tables(n_ent, n_rel, seed=0):
@@ -112,8 +88,8 @@ def run(B, iters):
     X = np.stack([rng.integers(0, E, B), rng.integers(0, R, B), rng.integers(0, E, B)], 1).astype(np.int32)
     t = torch.as_tensor(X).cuda()
     eng = engine(ent, rel)
-    ms_ent = events(lambda: eng.one_vs_all_backward(t, "s,o"), iters)
-    ms_rel = events(lambda: eng.one_vs_all_relation_backward(t, 1.0), iters)
+    ms_ent = float(np.median(measure.per_call_ms(lambda: eng.one_vs_all_backward(t, "s,o"), iters, 3)))
+    ms_rel = float(np.median(measure.per_call_ms(lambda: eng.one_vs_all_relation_backward(t, 1.0), iters, 3)))
     # agreement with the baseline on one relation step from zeroed accumulators
     eng.g_ent.zero_()
     eng.g_rel.zero_()
@@ -127,7 +103,7 @@ def run(B, iters):
     tl = torch.as_tensor(X).long().cuda()
     base_loss = float(torch_relation_term(te, tr, tl).detach())
     base_g_rel = tr.grad.cpu().numpy()
-    ms_torch = events(lambda: torch_relation_term(te, tr, tl), iters)
+    ms_torch = float(np.median(measure.per_call_ms(lambda: torch_relation_term(te, tr, tl), iters, 3)))
     kernels = profile_kernels(lambda: eng.one_vs_all_relation_backward(t, 1.0))
     ld = eng.ld
     eng.close()
@@ -167,7 +143,7 @@ def worker(out_dir, iters):
     for B in BATCHES:
         t = torch.as_tensor(np.stack([rng.integers(0, E, B), rng.integers(0, R, B), rng.integers(0, E, B)],
                                      1).astype(np.int32)).cuda()
-        times[B] = events(lambda: eng.one_vs_all_backward(t, "s,o"), iters)
+        times[B] = float(np.median(measure.per_call_ms(lambda: eng.one_vs_all_backward(t, "s,o"), iters, 3)))
     eng.close()
     outs = {}
 
@@ -256,7 +232,7 @@ def main():
     torch.backends.cudnn.allow_tf32 = False
     if args.worker:
         return worker(args.worker, args.iters)
-    info = gpu_info()
+    info = measure.card()
     print(info, flush=True)
     results = {"gpu": info, "runs": [run(B, args.iters) for B in BATCHES]}
     if args.parent_lib:

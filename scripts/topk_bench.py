@@ -4,40 +4,14 @@ alone and kge_corruption_scores + torch.topk on the same queries.  torch.topk is
 reference (it does not promise the tie order).  CUDA events, L2 flushed between iterations; prints the GPU and its power
 limit, because every number depends on both."""
 import os
-import subprocess
 import sys
 
 import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import measure  # noqa: E402
 from ampligraph_b200.engine import KGEEngine  # noqa: E402
-
-
-def gpu_info():
-    name = torch.cuda.get_device_name(0)
-    try:
-        pl = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                            stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True).stdout.strip()
-    except OSError:
-        pl = "unknown"
-    return "%s, power limit / max SM clock: %s" % (name, pl)
-
-
-def timed(fn, flush, iters):
-    for _ in range(2):
-        fn()
-    torch.cuda.synchronize()
-    ms = []
-    for i in range(iters):
-        flush.fill_(i)
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        fn()
-        e1.record()
-        torch.cuda.synchronize()
-        ms.append(e0.elapsed_time(e1))
-    return float(np.median(ms))
 
 
 def run(model, k, E, b, top, sides=("o", "s"), iters=10, R=237):
@@ -48,10 +22,11 @@ def run(model, k, E, b, top, sides=("o", "s"), iters=10, R=237):
                         .astype(np.int32)).cuda()
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
     ws = eng.lib.kge_topk_workspace_bytes(eng.h, b, E, top)
+    median_ms = lambda fn: float(np.median(measure.per_call_ms(fn, iters, 2, before=flush.zero_)))
     for side in sides:
-        t_topk = timed(lambda: eng.topk(t, side, top), flush, iters)
-        t_cs = timed(lambda: eng.corruption_scores(t, side), flush, iters)
-        t_cst = timed(lambda: torch.topk(eng.corruption_scores(t, side), top, dim=1), flush, iters)
+        t_topk = median_ms(lambda: eng.topk(t, side, top))
+        t_cs = median_ms(lambda: eng.corruption_scores(t, side))
+        t_cst = median_ms(lambda: torch.topk(eng.corruption_scores(t, side), top, dim=1))
         print("%-8s k=%-4d E=%-8d b=%-5d top=%-4d side=%s  topk %9.1f us  scores %9.1f us  scores+torch.topk %9.1f us  "
               "topk/scores %.3f  workspace %.1f MB (score matrix %.1f MB)"
               % (model, k, E, b, top, side, t_topk * 1e3, t_cs * 1e3, t_cst * 1e3, t_topk / t_cs, ws / 2**20,
@@ -72,7 +47,7 @@ def chunk_sweep():
 
 
 if __name__ == "__main__":
-    print(gpu_info(), flush=True)
+    print(measure.card(), flush=True)
     if "--chunk-sweep" in sys.argv:
         chunk_sweep()
         sys.exit(0)

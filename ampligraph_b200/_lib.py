@@ -57,6 +57,14 @@ class KgeNegativeSampler(C.Structure):
                 ("obj_filter_vals", C.c_void_p)]
 
 
+class KgeNSCaching(C.Structure):
+    _fields_ = [("struct_size", C.c_int32), ("cache_size", C.c_int32), ("random_size", C.c_int32), ("pad_", C.c_int32),
+                ("sub_n_keys", C.c_int64), ("sub_ids", C.c_void_p), ("sub_count", C.c_void_p),
+                ("obj_n_keys", C.c_int64), ("obj_ids", C.c_void_p), ("obj_count", C.c_void_p),
+                ("sub_filter_n", C.c_int64), ("sub_filter_keys", C.c_void_p), ("sub_filter_vals", C.c_void_p),
+                ("obj_filter_n", C.c_int64), ("obj_filter_keys", C.c_void_p), ("obj_filter_vals", C.c_void_p)]
+
+
 _P = C.c_void_p
 # name -> (restype, argtypes); kept in one table so tests can check it against the header
 PROTOTYPES = {
@@ -77,6 +85,8 @@ PROTOTYPES = {
     "kge_host_corruptions": (C.c_int, [_P, C.c_int64, C.c_int32, C.c_int64, C.c_uint64, C.c_uint64, _P]),
     "kge_sample_negatives": (C.c_int, [_P, C.POINTER(KgeNegativeSampler), _P, C.c_int64, C.c_uint64, C.c_uint64, _P, _P,
                                        _P, _P]),
+    "kge_nscaching_step": (C.c_int, [_P, C.POINTER(KgeNSCaching), _P, _P, _P, _P, _P, C.c_int64, C.c_uint64, C.c_uint64,
+                                     _P, _P, _P, _P]),
     "kge_train_step": (C.c_int, [_P, C.c_int32, _P, _P, _P, _P, _P, C.c_int64, _P, _P, C.c_uint64, C.c_uint64,
                                  _P, _P, _P, _P, _P, _P]),
     "kge_train_step_sharded": (C.c_int, [_P, C.c_int32, C.POINTER(KgeShardMap), _P, _P, _P, C.c_int64, _P, _P,

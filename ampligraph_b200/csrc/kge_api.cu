@@ -521,6 +521,75 @@ extern "C" int kge_set_train_workspace(kge_handle *h, void *ws_dev, int64_t byte
     return KGE_OK;
 }
 
+// NSCaching: refresh the batch's cache rows, then draw the step's corruptions from them (kge_nscaching.cu)
+extern "C" int kge_nscaching_step(kge_handle *h, const kge_nscaching *cache, const float *ent_dev, const float *rel_dev,
+                                  const int32_t *triples_dev, const int32_t *key_rows_dev, const uint8_t *update_dev,
+                                  int64_t B, uint64_t seed, uint64_t step, int32_t *neg_ent_dev,
+                                  uint8_t *neg_keep_subj_dev, uint64_t *misses_dev, void *stream)
+{
+    KGE_CHECK_HANDLE(h, "kge_nscaching_step");
+    const kge_nscaching *q = cache;
+    if (!q || q->struct_size != (int32_t)sizeof(kge_nscaching))
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_nscaching_step: bad kge_nscaching (ABI mismatch)");
+    if (q->cache_size < 1 || q->random_size < 1 || q->cache_size > 512 - q->random_size)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_nscaching_step: need cache_size >= 1, random_size >= 1 and their sum "
+                                              "<= 512, got %d and %d", q->cache_size, q->random_size);
+    if (q->sub_n_keys < 1 || q->obj_n_keys < 1 || !q->sub_ids_dev || !q->sub_count_dev || !q->obj_ids_dev || !q->obj_count_dev)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_nscaching_step: a side without cache rows or with null cache arrays");
+    if (q->sub_filter_n < 0 || q->obj_filter_n < 0 ||
+        (q->sub_filter_n > 0 && (!q->sub_filter_keys_dev || !q->sub_filter_vals_dev)) ||
+        (q->obj_filter_n > 0 && (!q->obj_filter_keys_dev || !q->obj_filter_vals_dev)))
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_nscaching_step: a filter count < 0, or > 0 without its arrays");
+    if (B < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_nscaching_step: B < 0");
+    if (B > ((1ll << 56) - 1) / h->cfg.eta) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_nscaching_step: eta*B >= 2^56");
+    if (B == 0) return KGE_OK;
+    if (!ent_dev || !rel_dev || !triples_dev || !key_rows_dev || !update_dev || !neg_ent_dev || !neg_keep_subj_dev)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_nscaching_step: null table, triples, key rows, flags or output pointer");
+    if (int rc = check_no_pending(h, "kge_nscaching_step")) return rc;
+    if (h->stash)
+        return fail(KGE_ERR_UNSUPPORTED, "kge_nscaching_step: a row stash is set (row-sharded tables): NSCaching reads one "
+                                         "whole entity table");
+    const size_t smem = nscaching_smem_bytes(h->L.ld, q->cache_size, q->random_size);
+    if ((long long)smem > h->max_smem)
+        return fail(KGE_ERR_UNSUPPORTED, "kge_nscaching_step: rows of %d floats and %d candidates exceed the shared memory "
+                                         "of the refresh kernel (%d B)", h->L.ld, q->cache_size + q->random_size, h->max_smem);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (int rc = refresh_rotation(h, rel_dev, st)) return rc;
+    NSCacheParams p;
+    memset(&p, 0, sizeof(p));
+    p.ent = ent_dev;
+    p.rel = h->cfg.scoring == KGE_ROTATE ? h->rot : rel_dev;  // the table refresh_rotation has just written
+    p.triples = triples_dev;
+    p.key_rows = key_rows_dev;
+    p.update = update_dev;
+    p.B = B;
+    p.model = h->cfg.scoring;
+    p.kp = h->L.kp;
+    p.ld = h->L.ld;
+    p.eta = h->cfg.eta;
+    p.n1 = q->cache_size;
+    p.n2 = q->random_size;
+    p.n_ent = (unsigned)h->cfg.n_ent;
+    p.scale = h->score_scale;
+    p.seed = seed;
+    p.step = step;
+    p.ids[0] = q->sub_ids_dev;
+    p.count[0] = q->sub_count_dev;
+    p.ids[1] = q->obj_ids_dev;
+    p.count[1] = q->obj_count_dev;
+    p.filt_n[0] = q->sub_filter_n;
+    p.filt_keys[0] = reinterpret_cast<const long long *>(q->sub_filter_keys_dev);
+    p.filt_vals[0] = q->sub_filter_vals_dev;
+    p.filt_n[1] = q->obj_filter_n;
+    p.filt_keys[1] = reinterpret_cast<const long long *>(q->obj_filter_keys_dev);
+    p.filt_vals[1] = q->obj_filter_vals_dev;
+    p.neg_ent = neg_ent_dev;
+    p.neg_keep = neg_keep_subj_dev;
+    p.misses = reinterpret_cast<unsigned long long *>(misses_dev);
+    KGE_CUDA(launch_nscaching(p, h->sm_count, st), "kge_nscaching_step");
+    return KGE_OK;
+}
+
 static bool dropout_set(const kge_handle *h) { return h->drop_p_ent != 0.f || h->drop_p_rel != 0.f; }
 
 // The sampled steps' fused kernels read the raw rows: they refuse while embedding dropout is set

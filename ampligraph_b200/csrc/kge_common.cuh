@@ -196,6 +196,21 @@ __host__ __device__ inline void draw_corruption(uint64_t seed, uint64_t step, ui
     *repl = (int)(((uint64_t)v.y * (uint64_t)n_ent) >> 32);
 }
 
+// (key, val) is one of the n lexsorted pairs (keys[], vals[]): a lower-bound binary search over the pairs.  The filter
+// of the negative samplers (kge_negatives.cu, kge_nscaching.cu): keys p * n_ent + kept entity, values the replaced one.
+__device__ __forceinline__ bool known_pair(const long long *__restrict__ keys, const int32_t *__restrict__ vals, long long n,
+                                           long long key, int val)
+{
+    long long lo = 0, hi = n;
+    while (lo < hi) {
+        const long long mid = (lo + hi) >> 1;
+        const long long k = keys[mid];
+        if (k < key || (k == key && vals[mid] < val)) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo < n && keys[lo] == key && vals[lo] == val;
+}
+
 // ---------------------------------------------------------------------------
 // canonical arithmetic shared with the ranking oracle (oracle/kge_oracle.c states
 // the same operation sequence independently): explicit _rn intrinsics so that

@@ -107,6 +107,31 @@ struct NegativeParams {
 };
 cudaError_t launch_negatives(const NegativeParams &p, int sm_count, cudaStream_t st);
 
+// kge_nscaching.cu: NSCaching (kge_nscaching_step), the refresh of the batch's cache rows, then the draw.  [side] as in
+// NegativeParams: [0] the subject-replaced caches (one row per (p, o)), [1] the object-replaced ones (one per (s, p)).
+struct NSCacheParams {
+    const float *ent, *rel;    // rel: the rotation table for RotatE
+    const int32_t *triples;    // [B, 3]
+    const int32_t *key_rows;   // [B, 2] cache row of positive i on each side
+    const uint8_t *update;     // [B, 2] 1: positive i refreshes that row this step
+    long long B;
+    int model, kp, ld, eta;
+    int n1, n2;                // cache size and random candidates per refresh (n1, n2 >= 1, n1 + n2 <= 512)
+    unsigned n_ent;
+    float scale;               // HolE's score scale
+    unsigned long long seed, step;
+    int32_t *ids[2];           // [n_keys, n1]
+    int32_t *count[2];         // [n_keys]
+    long long filt_n[2];       // known (key, value) pairs of each side, as NegativeParams (0: not filtered)
+    const long long *filt_keys[2];
+    const int32_t *filt_vals[2];
+    int32_t *neg_ent;          // [eta * B]
+    uint8_t *neg_keep;         // [eta * B]
+    unsigned long long *misses;  // += corruptions drawn from an empty row, or nullptr
+};
+size_t nscaching_smem_bytes(int ld, int n1, int n2);
+cudaError_t launch_nscaching(const NSCacheParams &p, int sm_count, cudaStream_t st);
+
 // kge_train_1vsall.cu: one side of a 1vsAll multiclass-NLL step of the trilinear models (kge_one_vs_all_step)
 struct OneVsAllSide {
     const float *q;          // [B, ld] query vectors of the side (launch_rank_prepare: qvec_s for side s, qvec_o for o;

@@ -23,20 +23,6 @@ __device__ __forceinline__ u32x4 negative_block(const NegativeParams &p, unsigne
                          (uint32_t)p.seed, (uint32_t)(p.seed >> 32));
 }
 
-// (key, val) is one of the n lexsorted pairs (keys[], vals[]): a lower-bound binary search over the pairs
-__device__ __forceinline__ bool known_pair(const long long *__restrict__ keys, const int32_t *__restrict__ vals, long long n,
-                                           long long key, int val)
-{
-    long long lo = 0, hi = n;
-    while (lo < hi) {
-        const long long mid = (lo + hi) >> 1;
-        const long long k = keys[mid];
-        if (k < key || (k == key && vals[mid] < val)) lo = mid + 1;
-        else hi = mid;
-    }
-    return lo < n && keys[lo] == key && vals[lo] == val;
-}
-
 __global__ void __launch_bounds__(256) kge_negatives_kernel(const NegativeParams p)
 {
     const unsigned long long n = (unsigned long long)p.B * (unsigned long long)p.eta;

@@ -165,6 +165,47 @@ def negative_sampler_tables(triples, n_ent, n_rel, sampler="uniform", filtered=F
     return out
 
 
+def query_rows(triples, n_ent, side):
+    """The distinct queries of one side of `triples`, (s, p) for side 'o' and (p, o) for side 's', numbered in order of
+    first appearance -> (first int64 [n_queries]: the triple where each query first appears, ascending; rows int64
+    [len(triples)]: the query number of every triple).  KvsAll's training rows and NSCaching's cache rows."""
+    t = np.asarray(triples, dtype=np.int64).reshape(-1, 3)
+    keys = t[:, 1] * int(n_ent) + t[:, 0 if side == "o" else 2]
+    _, first, inverse = np.unique(keys, return_index=True, return_inverse=True)
+    order = np.argsort(first, kind="stable")  # sorted-key number -> first-appearance number
+    number = np.empty(len(first), dtype=np.int64)
+    number[order] = np.arange(len(first))
+    return first[order], number[inverse.reshape(-1)]
+
+
+def nscaching_tables(triples, n_ent, n_rel, batch_size, filtered=False):
+    """The per-fit tables of NSCaching (kge_nscaching_step, DESIGN.md 3.20) for fit's sequential batches of batch_size
+    triples -> dict:
+      key_rows  int32 [n, 2]: column 0 the subject-replaced cache row of each triple (its (p, o) in order of first
+                appearance, query_rows(.., 's')), column 1 the object-replaced one (its (s, p), query_rows(.., 'o'))
+      update    uint8 [n, 2]: 1 iff the triple is the first of its batch with that row, the one that refreshes it
+      n_keys    (subject-side rows, object-side rows)
+      filter    {'s': (keys int64, values int32), 'o': ...} as negative_sampler_tables' (filtered), else None
+    n_rel is accepted for symmetry with negative_sampler_tables; the rows only depend on the triples."""
+    t = np.asarray(triples, dtype=np.int64).reshape(-1, 3)
+    n, batch_size = len(t), int(batch_size)
+    key_rows = np.zeros((n, 2), dtype=np.int32)
+    update = np.zeros((n, 2), dtype=np.uint8)
+    n_keys = []
+    batch = np.arange(n, dtype=np.int64) // max(batch_size, 1)
+    for col, side in ((0, "s"), (1, "o")):
+        first, rows = query_rows(t, n_ent, side)
+        key_rows[:, col] = rows
+        n_keys.append(len(first))
+        _, lead = np.unique(batch * max(len(first), 1) + rows, return_index=True)  # first of each (batch, row)
+        update[lead, col] = 1
+    out = {"key_rows": key_rows, "update": update, "n_keys": tuple(n_keys), "filter": None}
+    if filtered:
+        f = FilterIndex(t, n_ent)
+        out["filter"] = {"s": f._sub, "o": f._obj}
+    return out
+
+
 def k_vs_all_queries(findex, triples, side):
     """The KvsAll training rows of one side (DESIGN.md 3.13): every distinct (s, p) of `triples` for side 'o', every
     distinct (p, o) for side 's', in order of first appearance, each labelled with its known objects (subjects) in
@@ -173,9 +214,8 @@ def k_vs_all_queries(findex, triples, side):
     holds its first label, so that every column is a valid entity id."""
     t = np.asarray(triples, dtype=np.int64).reshape(-1, 3)
     col = 2 if side == "o" else 0
-    keys = t[:, 1] * findex.n_ent + t[:, 2 - col]
-    _, first = np.unique(keys, return_index=True)
-    queries = np.ascontiguousarray(t[np.sort(first)], dtype=np.int32)
+    first, _ = query_rows(t, findex.n_ent, side)
+    queries = np.ascontiguousarray(t[first], dtype=np.int32)
     off, ids = findex.lookup(queries, side)
     queries[:, col] = ids[off[:-1]]
     return queries, off, ids

@@ -248,6 +248,40 @@ class NegativeSamplerTables:
         self.struct = q
 
 
+class NSCache:
+    """The NSCaching state of one fit (kge_nscaching_step, DESIGN.md 3.20): both sides' device caches, zero (empty) at
+    construction, the key rows and update flags of every training triple (datasets.nscaching_tables), uploaded once and
+    sliced per batch like the triples, the optional filter, and the kge_nscaching that points at them."""
+
+    def __init__(self, tables, cache_size, random_size, device):
+        up = lambda a: torch.as_tensor(np.ascontiguousarray(a)).to(device)
+        self.key_rows = up(tables["key_rows"])
+        self.update = up(tables["update"])
+        self.n_keys = tuple(int(n) for n in tables["n_keys"])
+        n1, n2 = int(cache_size), int(random_size)
+        self.ids = [torch.zeros((max(n, 1), n1), dtype=torch.int32, device=device) for n in self.n_keys]
+        self.count = [torch.zeros(max(n, 1), dtype=torch.int32, device=device) for n in self.n_keys]
+        q = _lib.KgeNSCaching(C.sizeof(_lib.KgeNSCaching), n1, n2)
+        self._keep = []
+        for side, name in ((0, "sub"), (1, "obj")):
+            setattr(q, name + "_n_keys", max(self.n_keys[side], 1))
+            setattr(q, name + "_ids", self.ids[side].data_ptr())
+            setattr(q, name + "_count", self.count[side].data_ptr())
+        filt = tables.get("filter") or {}
+        for side, name in (("s", "sub"), ("o", "obj")):
+            if side in filt and len(filt[side][0]):
+                keys, vals = (up(a) for a in filt[side])
+                self._keep += [keys, vals]
+                setattr(q, name + "_filter_n", keys.numel())
+                setattr(q, name + "_filter_keys", keys.data_ptr())
+                setattr(q, name + "_filter_vals", vals.data_ptr())
+        self.struct = q
+
+    def batch(self, start, size):
+        """The key rows and update flags of the batch of `size` triples from triple `start`."""
+        return self.key_rows[start:start + size], self.update[start:start + size]
+
+
 _NVTX = os.environ.get("KGE_B200_NVTX", "0") == "1"
 
 
@@ -786,6 +820,35 @@ class KGEEngine:
                                                  _ptr(self._neg_misses), self._stream()))
         if n:
             self.launches += 1
+        return self._neg_ent[:n], self._neg_keep[:n]
+
+    def _negative_buffers(self, n):
+        if getattr(self, "_neg_ent", None) is None or self._neg_ent.numel() < n:
+            self._neg_ent = torch.empty(max(n, 1), dtype=torch.int32, device=self.device)
+            self._neg_keep = torch.empty(max(n, 1), dtype=torch.uint8, device=self.device)
+        if getattr(self, "_neg_misses", None) is None:
+            self._neg_misses = torch.zeros(1, dtype=torch.int64, device=self.device)
+
+    @_traced("kge.nscaching_negatives")
+    def nscaching_negatives(self, triples, key_rows, update, cache, seed=0, step=0):
+        """The step's corruptions under NSCaching (kge_nscaching_step, DESIGN.md 3.20): refresh the cache rows whose
+        update flag is set, then draw every corruption from its positive's row.  key_rows int32 [B, 2] and update uint8
+        [B, 2] are the batch's (NSCache.batch); cache an NSCache, whose device caches the call updates.  -> the same
+        persistent (repl, keep) views as sample_negatives; a corruption of an empty row (only the filter empties one)
+        is drawn uniformly and counted by read_negative_misses.  Nothing synchronises."""
+        assert triples.dtype == torch.int32 and triples.is_cuda and triples.is_contiguous()
+        assert key_rows.dtype == torch.int32 and update.dtype == torch.uint8
+        assert key_rows.is_contiguous() and update.is_contiguous()
+        B = triples.shape[0]
+        assert key_rows.shape == (B, 2) and update.shape == (B, 2)
+        n = B * self.eta
+        self._negative_buffers(n)
+        _lib.check(self.lib.kge_nscaching_step(self.h, C.byref(cache.struct), _ptr(self.ent), _ptr(self.rel),
+                                               _ptr(triples), _ptr(key_rows), _ptr(update), B, int(seed), int(step),
+                                               _ptr(self._neg_ent), _ptr(self._neg_keep), _ptr(self._neg_misses),
+                                               self._stream()))
+        if n:
+            self.launches += 2
         return self._neg_ent[:n], self._neg_keep[:n]
 
     def read_negative_misses(self, reset=True):

@@ -12,13 +12,16 @@ import torch
 
 from .. import _lib
 from ..datasets import (NEGATIVE_SAMPLERS, DataIndexer, FilterIndex, as_triple_array, k_vs_all_queries, k_vs_all_steps,
-                        negative_sampler_tables, reciprocal_triples)
-from ..engine import KGEEngine, NegativeSamplerTables
+                        negative_sampler_tables, nscaching_tables, reciprocal_triples)
+from ..engine import KGEEngine, NegativeSamplerTables, NSCache
 from ..evaluation import hits_at_n_score, mr_score, mrr_score, train_test_split_no_unseen
 from . import initializers, loss_functions, optimizers, regularizers
 from .layers.scoring import SCORING_LAYER_REGISTRY
 
 NEGATIVE_FILTER_ATTEMPTS = 10  # draws of a corruption's entity under fit(filter_negatives=True) (DESIGN.md 3.18)
+FIT_NEGATIVE_SAMPLERS = NEGATIVE_SAMPLERS + ("nscaching",)
+NSCACHING_PARAMS = {"cache_size": 50, "random_size": 50}  # N1, N2: the paper's defaults (DESIGN.md 3.20)
+NSCACHING_MAX_CANDIDATES = 512  # N1 + N2: the refresh kernel's candidates per row
 
 
 class History:
@@ -266,7 +269,7 @@ class ScoringBasedEmbeddingModel:
             validation_corrupt_side="s,o", validation_freq=10, validation_burn_in=0, validation_filter=False,
             validation_entities_subset=None, partitioning_k=1, focusE=False, focusE_params={}, one_vs_all=None,
             k_vs_all=None, label_smoothing=0.0, relation_prediction_weight=0.0, negative_sampler="uniform",
-            filter_negatives=False, entity_dropout=0.0, relation_dropout=0.0):
+            filter_negatives=False, entity_dropout=0.0, relation_dropout=0.0, negative_sampler_params=None):
         """fit (:544-883).  `shuffle` is accepted and ignored exactly like the reference
         (batches are the sequential slices of graph_data_loader.py:495-500).  validation_split: carve the validation
         set out of x with train_test_split_no_unseen(x, test_size=validation_split, seed=self.seed), as the reference
@@ -317,6 +320,16 @@ class ScoringBasedEmbeddingModel:
         every single-GPU sampled step of fit (the fused step, user losses, focusE), not to one_vs_all or k_vs_all;
         train_on_batch and train_on_batches stay uniform.  'uniform' without the filter is the path fit always took.
 
+        negative_sampler='nscaching' (extension; DESIGN.md 3.20; Zhang et al., ICDE 2019) keeps a cache of
+        high-scoring entities for every (s, p) and every (p, o) of x and draws each corruption uniformly from the cache
+        of its positive's query, the side on a fair coin.  Every step first refreshes the caches of its batch's queries:
+        the cached entities plus random_size uniform ones, with duplicates (and, with filter_negatives=True, triples of
+        x) dropped, are sampled down to cache_size without replacement with probability proportional to exp(score) of
+        the current embeddings.  negative_sampler_params={"cache_size": N1, "random_size": N2} (ints >= 1,
+        N1 + N2 <= 512; default 50 and 50, the paper's) is accepted with 'nscaching' only.  The caches start empty at
+        every fit and persist across its epochs.  A corruption of a cache the filter left empty is drawn uniformly and
+        counted in self.negative_filter_misses.
+
         entity_dropout, relation_dropout (extension; DESIGN.md 3.19): p in [0, 1), inverted dropout on the entity and
         relation embedding elements every training score of the fit reads (LibKGE's lookup-embedder dropout, tuned by
         Ruffinelli et al., ICLR 2020): each kept element is scaled by 1 / (1 - p), each dropped one is 0.  A step's
@@ -329,7 +342,8 @@ class ScoringBasedEmbeddingModel:
         self._check_dropout(entity_dropout, relation_dropout, one_vs_all, k_vs_all)
         if self.reciprocal_relations:
             self._check_reciprocal("fit", one_vs_all, k_vs_all, focusE, relation_prediction_weight)
-        sampled_option = self._check_negative_sampler(negative_sampler, filter_negatives, one_vs_all, k_vs_all)
+        sampled_option = self._check_negative_sampler(negative_sampler, filter_negatives, one_vs_all, k_vs_all,
+                                                      negative_sampler_params)
         self._check_per_occurrence(k_vs_all)
         if k_vs_all is not None or label_smoothing != 0.0:
             self._check_k_vs_all(k_vs_all, label_smoothing, one_vs_all, focusE)
@@ -374,7 +388,8 @@ class ScoringBasedEmbeddingModel:
             return self._fit_loop(x, triples, batch_size, epochs, verbose, callbacks, validation_data, initial_epoch,
                                   validation_batch_size, validation_corrupt_side, validation_freq, validation_burn_in,
                                   validation_filter, validation_entities_subset, one_vs_all, k_vs_all, label_smoothing,
-                                  relation_prediction_weight, negative_sampler, filter_negatives, sampled_option)
+                                  relation_prediction_weight, negative_sampler, filter_negatives, sampled_option,
+                                  negative_sampler_params)
         finally:
             if any(dropout):
                 eng.set_embedding_dropout(0.0, 0.0)
@@ -382,7 +397,8 @@ class ScoringBasedEmbeddingModel:
     def _fit_loop(self, x, triples, batch_size, epochs, verbose, callbacks, validation_data, initial_epoch,
                   validation_batch_size, validation_corrupt_side, validation_freq, validation_burn_in,
                   validation_filter, validation_entities_subset, one_vs_all, k_vs_all, label_smoothing,
-                  relation_prediction_weight, negative_sampler, filter_negatives, sampled_option):
+                  relation_prediction_weight, negative_sampler, filter_negatives, sampled_option,
+                  negative_sampler_params=None):
         """fit's training loop, on the engine fit has built (with fit's embedding dropout set on it)."""
         eng = self.engine
         eng.set_hot_entities(triples=triples)  # the most frequent entities of the training set: their gradient rows are summed per warp
@@ -426,7 +442,12 @@ class ScoringBasedEmbeddingModel:
             count = lambda side: kva[side][0].shape[0] if side in kva else 0
             kva_steps = k_vs_all_steps(count("o"), count("s"), batch_size)
         sampler = None
-        if sampled_option:
+        if negative_sampler == "nscaching":
+            params = dict(NSCACHING_PARAMS, **(negative_sampler_params or {}))
+            sampler = NSCache(nscaching_tables(triples, self.max_ent_size, self.max_rel_size, batch_size, filter_negatives),
+                              params["cache_size"], params["random_size"], eng.device)
+            eng.read_negative_misses()  # start this fit's count at 0
+        elif sampled_option:
             sampler = NegativeSamplerTables(
                 negative_sampler_tables(triples, self.max_ent_size, self.max_rel_size, negative_sampler, filter_negatives),
                 NEGATIVE_FILTER_ATTEMPTS, eng.device)
@@ -448,15 +469,15 @@ class ScoringBasedEmbeddingModel:
                     self._per_occurrence_backward(batch)
                     eng.apply_gradients()
                 elif self.use_focusE:
-                    self._two_phase_step(batch, weights[start:start + batch_size], sampler)
+                    self._two_phase_step(batch, weights[start:start + batch_size], sampler, start)
                 elif world > 1:  # this rank's slice of the global batch; the step is the global-batch step
                     from ..parallel import row_shard
                     lo, hi = row_shard(batch.shape[0], world, rank)
                     self._dp.train_step(batch[lo:hi], None, seed=self.seed + 7919 * rank, step=self._step)
                 elif user_loss:
-                    self._user_loss_step(batch, sampler)
+                    self._user_loss_step(batch, sampler, start)
                 else:
-                    negatives = None if sampler is None else eng.sample_negatives(batch, sampler, self.seed, self._step)
+                    negatives = self._sampled_negatives(batch, sampler, start)
                     eng.forward_backward(batch, negatives, seed=self.seed, step=self._step, defer=True)
                     self._per_occurrence_backward(batch)
                     eng.apply_gradients()
@@ -552,14 +573,17 @@ class ScoringBasedEmbeddingModel:
         if why is not None:
             raise NotImplementedError("reciprocal relations: %s" % why)
 
-    def _check_negative_sampler(self, negative_sampler, filter_negatives, one_vs_all, k_vs_all):
-        """The refusals of fit(negative_sampler=..., filter_negatives=...), before anything is indexed or trained ->
-        whether the step draws its corruptions with kge_sample_negatives ('uniform' without the filter does not)."""
-        if not isinstance(negative_sampler, str) or negative_sampler not in NEGATIVE_SAMPLERS:
+    def _check_negative_sampler(self, negative_sampler, filter_negatives, one_vs_all, k_vs_all, params=None):
+        """The refusals of fit(negative_sampler=..., filter_negatives=..., negative_sampler_params=...), before anything
+        is indexed or trained -> whether the step draws its corruptions with kge_sample_negatives or
+        kge_nscaching_step ('uniform' without the filter does neither)."""
+        if not isinstance(negative_sampler, str) or negative_sampler not in FIT_NEGATIVE_SAMPLERS:
             raise ValueError("negative_sampler must be one of %s, got %r"
-                             % (", ".join(map(repr, NEGATIVE_SAMPLERS)), negative_sampler))
+                             % (", ".join(map(repr, FIT_NEGATIVE_SAMPLERS)), negative_sampler))
         if not isinstance(filter_negatives, bool):
             raise ValueError("filter_negatives must be a bool, got %r" % (filter_negatives,))
+        if params is not None:
+            self._check_nscaching_params(negative_sampler, params)
         if negative_sampler == "uniform" and not filter_negatives:
             return False
         if one_vs_all is not None or k_vs_all is not None:
@@ -568,6 +592,39 @@ class ScoringBasedEmbeddingModel:
         if self._world() > 1:
             raise NotImplementedError("negative_sampler and filter_negatives are single-GPU only")
         return True
+
+    @staticmethod
+    def _check_nscaching_params(negative_sampler, params):
+        """The refusals of negative_sampler_params: given with another sampler than 'nscaching', not a dict, unknown
+        keys, values that are not ints (bools are refused) or out of bounds (N1, N2 >= 1, N1 + N2 <= 512)."""
+        if negative_sampler != "nscaching":
+            raise ValueError("negative_sampler_params applies to negative_sampler='nscaching' only, got sampler %r"
+                             % (negative_sampler,))
+        if not isinstance(params, dict):
+            raise ValueError("negative_sampler_params must be a dict, got %r" % (params,))
+        unknown = sorted(set(params) - set(NSCACHING_PARAMS), key=repr)
+        if unknown:
+            raise ValueError("unknown negative_sampler_params keys %s (known: %s)"
+                             % (", ".join(map(repr, unknown)), ", ".join(map(repr, NSCACHING_PARAMS))))
+        for key, v in params.items():
+            if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)):
+                raise ValueError("negative_sampler_params[%r] must be an int, got %r" % (key, v))
+        p = dict(NSCACHING_PARAMS, **params)
+        if p["cache_size"] < 1 or p["random_size"] < 1 or p["cache_size"] + p["random_size"] > NSCACHING_MAX_CANDIDATES:
+            raise ValueError("negative_sampler_params needs cache_size >= 1, random_size >= 1 and cache_size + "
+                             "random_size <= %d, got %d and %d"
+                             % (NSCACHING_MAX_CANDIDATES, p["cache_size"], p["random_size"]))
+
+    def _sampled_negatives(self, batch, sampler, start):
+        """The corruptions of the sampled step on `batch` (fit's triples from `start`): None for the uniform draw of the
+        training kernel, else the (repl, keep) views of kge_sample_negatives (a NegativeSamplerTables) or
+        kge_nscaching_step (an NSCache)."""
+        if sampler is None:
+            return None
+        if isinstance(sampler, NSCache):
+            key_rows, update = sampler.batch(start, batch.shape[0])
+            return self.engine.nscaching_negatives(batch, key_rows, update, sampler, self.seed, self._step)
+        return self.engine.sample_negatives(batch, sampler, self.seed, self._step)
 
     def _check_all_candidates(self, training, loss, focusE):
         """The refusals fit's all-candidate training types share: `training` ('1vsAll' or 'KvsAll') needs a trilinear
@@ -760,16 +817,16 @@ class ScoringBasedEmbeddingModel:
         self.is_fitted = True
         return losses
 
-    def _user_loss_step(self, batch, sampler=None):
-        self._two_phase_step(batch, None, sampler)
+    def _user_loss_step(self, batch, sampler=None, start=0):
+        self._two_phase_step(batch, None, sampler, start)
 
-    def _two_phase_step(self, batch, weights, sampler=None):
+    def _two_phase_step(self, batch, weights, sampler=None, start=0):
         """LossFunctionWrapper / FocusE path: scores from the kernel, dL/dscore from torch autograd
-        over a handful of elementwise ops, gradients from the kernel again.  sampler: the fit's NegativeSamplerTables,
-        or None for the uniform corruptions."""
+        over a handful of elementwise ops, gradients from the kernel again.  sampler: the fit's NegativeSamplerTables or
+        NSCache (batch = the fit's triples from `start`), or None for the uniform corruptions."""
         eng, B = self.engine, batch.shape[0]
         if sampler is not None:
-            repl, keep = eng.sample_negatives(batch, sampler, self.seed, self._step)
+            repl, keep = self._sampled_negatives(batch, sampler, start)
         else:
             neg = eng.generate_corruptions(batch, self.seed, self._step)
             tiled = batch.repeat(self.eta, 1)

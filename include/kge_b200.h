@@ -249,6 +249,51 @@ int kge_sample_negatives(kge_handle *h, const kge_negative_sampler *sampler, con
                          uint64_t seed, uint64_t step, int32_t *neg_ent_dev, uint8_t *neg_keep_subj_dev,
                          uint64_t *misses_dev, void *stream);
 
+/* NSCaching negative sampling (extension; Zhang, Yao, Shao and Chen, ICDE 2019; DESIGN.md 3.20): per-query caches of
+ * high-scoring entities, refreshed each step by importance sampling and drawn from uniformly.  Side 0 (subject replaced)
+ * has one cache row per distinct (p, o), side 1 (object replaced) one per distinct (s, p); row r of a side holds
+ * count[r] <= N1 distinct ids at ids[r * N1 ..].  kge_nscaching_step runs two phases:
+ *   refresh  for every positive i and side with update[i][side] = 1, row = key_rows[i][side]: the candidates
+ *            c = 0, 1, ... are the row's count cached ids, then N2 draws e_j = (w * n_ent) >> 32, w word j & 3 of
+ *            Philox4x32-10 with counter (row, (j >> 2) | side << 31, step_lo, step_hi) and key
+ *            (seed_lo, seed_hi ^ 0x4E534341).  A candidate equal to an earlier one, with a NaN score, or (filter) whose
+ *            corrupted triple (s, p, c) / (c, p, o) is a known pair is dropped.  score = kge_corruption_scores' value;
+ *            key = fl(score + G), G = -logf(-logf(u)), u = ((w' >> 9) + 0.5) 2^-23, w' word c & 3 of the block with
+ *            counter (row, (c >> 2) | 1 << 30 | side << 31, step_lo, step_hi).  The min(N1, valid) candidates with the
+ *            largest keys (ties: lower c) are kept, in ascending c, and count is set to their number.
+ *   draw     corruption r = j*B + i: v = the block of kge_generate_corruptions, side = keep_subj = x & 1,
+ *            n = count[key_rows[i][side]]; replacement ids[row][(y * n) >> 32], or (y * n_ent) >> 32 and
+ *            *misses_dev += 1 when n = 0.
+ * The rotation table is refreshed from rel_dev for RotatE.  Deterministic, stream-ordered, allocates nothing. */
+typedef struct kge_nscaching {
+    int32_t struct_size;              /* sizeof(kge_nscaching), ABI guard */
+    int32_t cache_size;               /* N1 >= 1 */
+    int32_t random_size;              /* N2 >= 1, N1 + N2 <= 512 */
+    int32_t pad_;
+    int64_t sub_n_keys;               /* rows of the subject-replaced caches (distinct (p, o)) */
+    int32_t *sub_ids_dev;             /* [sub_n_keys, N1] */
+    int32_t *sub_count_dev;           /* [sub_n_keys] */
+    int64_t obj_n_keys;               /* rows of the object-replaced caches (distinct (s, p)) */
+    int32_t *obj_ids_dev;             /* [obj_n_keys, N1] */
+    int32_t *obj_count_dev;           /* [obj_n_keys] */
+    int64_t sub_filter_n;             /* optional filter, as kge_negative_sampler: key p * n_ent + o, value s */
+    const int64_t *sub_filter_keys_dev;
+    const int32_t *sub_filter_vals_dev;
+    int64_t obj_filter_n;             /* key p * n_ent + s, value o */
+    const int64_t *obj_filter_keys_dev;
+    const int32_t *obj_filter_vals_dev;
+} kge_nscaching;
+/* ent_dev / rel_dev the tables; triples_dev [B,3]; key_rows_dev int32 [B,2] (row of each side, < that side's n_keys);
+ * update_dev uint8 [B,2] (at most one positive per row and step may set it); eta from the handle; neg_ent_dev /
+ * neg_keep_subj_dev [eta*B] outputs as kge_sample_negatives'; misses_dev uint64 counter added to, or NULL.
+ * KGE_ERR_INVALID_ARGUMENT without a launch for a bad struct, N1 / N2 out of bounds, n_keys < 1 or null cache arrays,
+ * a filter count < 0 or > 0 without its arrays, B < 0, eta*B >= 2^56, null pointers when B > 0, or a pending
+ * KGE_STEP_FUSED_DEFER step; KGE_ERR_UNSUPPORTED while a row stash is set (row-sharded tables).  B = 0 is a no-op. */
+int kge_nscaching_step(kge_handle *h, const kge_nscaching *cache, const float *ent_dev, const float *rel_dev,
+                       const int32_t *triples_dev, const int32_t *key_rows_dev, const uint8_t *update_dev, int64_t B,
+                       uint64_t seed, uint64_t step, int32_t *neg_ent_dev, uint8_t *neg_keep_subj_dev,
+                       uint64_t *misses_dev, void *stream);
+
 /* train_step forward+backward (ScoringBasedEmbeddingModel.py:370-429, call :237-269,
  * Loss.__call__ loss_functions.py:185-225, tape.gradient optimizers.py:166).
  *   triples_dev     [B,3] int32 positives

@@ -8,7 +8,7 @@ namespace kge {
 // --------------------------------------------------------------------------
 // predict_step (ScoringBasedEmbeddingModel.py:1694-1699): one warp per triple,
 // rows read straight from HBM with coalesced 4-byte lanes (k values per half),
-// warp-shuffle reduction.  Not the hot path; tolerance vs the oracle 1e-4 rel.
+// warp-shuffle reduction.  Not the hot path; each score's error bound: tests/exact_oracle.py PredictBound.
 // --------------------------------------------------------------------------
 template <int MODEL>
 __global__ void kge_score_kernel(const float *__restrict__ ent, const float *__restrict__ rel,

@@ -20,6 +20,8 @@ docstring from the kernels' split geometry (ova_chains) and the pair's logit err
 
 RotatE's training arithmetic is not exact on any grid (approximate sqrt / rsqrt, fp32 cos / sin): oracle_step(...,
 rot_table=True) evaluates it on the rotation table the kernels read, and RotatEBound gives its per-element bound.
+
+The predict path (kge_score_triples) has its own chain, one warp per triple: PredictBound gives its per-score bound.
 """
 from collections import namedtuple
 
@@ -595,6 +597,134 @@ class TrilinearBound:
 
 
 # --------------------------------------------------------------------------
+# kge_score_triples (the predict path): a per-element bound
+# --------------------------------------------------------------------------
+def predict_chain(model, k):
+    """N: the roundings any one product (TransE and RotatE: column term) of a predict score passes through (PredictBound),
+    L = ceil(k / 32) columns per lane."""
+    L = -(-k // 32)
+    return {"DistMult": 1 + L + 5, "ComplEx": 2 + 2 * L + 5, "HolE": 2 + 2 * L + 5 + 2, "TransE": 2 + L + 5,
+            "RotatE": 5 + L + 5}[model]
+
+
+def predict_abs(model, e_s, e_p, e_o, c=None, sn=None):
+    """Per triple, the magnitude PredictBound's relative term scales: abs_scores on |tables| (HolE's exact 2 / k
+    included); RotatE sum_d S_re + S_im with (c, sn) the rotation-table row, S_re = |s_re c| + |s_im sn| + |o_re|,
+    S_im = |s_re sn| + |s_im c| + |o_im|."""
+    if model != "RotatE":
+        return abs_scores(model, e_s.abs(), e_p.abs(), e_o.abs())
+    h = e_s.shape[1] // 2
+    sr, si, o = e_s[:, :h].abs(), e_s[:, h:].abs(), e_o.abs()
+    c, sn = c.abs(), sn.abs()
+    return (sr * (c + sn) + si * (sn + c)).sum(1) + o.sum(1)
+
+
+def nonfinite_class(x):
+    """0 finite, 1 NaN, 2 +inf, 3 -inf, elementwise (float64 tensor)."""
+    cls = torch.zeros(x.shape, dtype=torch.int8, device=x.device)
+    cls[torch.isnan(x)] = 1
+    cls[x == np.inf] = 2
+    cls[x == -np.inf] = 3
+    return cls
+
+
+class PredictBound:
+    """The per-element error bound of kge_score_triples (kge_misc.cu: kge_score_kernel, the predict path), against
+    scores(..., rot_table=True) in float64 on the fp32 tables: RotatE reads the kernels' fp32 rotation table (c, sn)
+    on both sides (pinned bit for bit elsewhere), so the bound covers the scoring arithmetic only.  u = 2^-24.
+
+    One warp per triple: lane l accumulates columns l, l + 32, ... < k (L = ceil(k / 32) of them) in one fp32 register,
+    warp_sum (an xor butterfly, 5 levels) adds the 32 lanes, lane 0 stores scale * acc (scale = fl(2 / k) for HolE, 1
+    otherwise).  The library is built without fast math (kge_misc.cu's PTX: sqrt.rn.f32, no .ftz, no .approx), and
+    --fmad=true contracts nothing here: every product feeds an explicit fmaf, a store or a multiply.  A sum evaluated in
+    any order rounds each term once per add it passes through (relative to the sum of the terms' magnitudes), so it
+    is enough to count, per product, the roundings on its way to the output:
+      DistMult   acc = fmaf(s * p, o, acc): s * p (1), the lane's L fmas (the first one adds to an exact 0, still at
+                 most L), the butterfly (5)                                                  N = 1 + L + 5.
+      ComplEx    acc = fmaf(sr, fmaf(pi, oi, pr * orr), acc), then fmaf(si, fmaf(-pi, orr, pr * oi), acc): the inner
+                 product and fma (2; 1 for the fma's own product), 2L outer fmas, the butterfly   N = 2 + 2L + 5.
+      HolE       ComplEx's chain, then scale = fl(2 / k) (1, exact when k is a power of two) and the multiply (1):
+                                                                                              N = 2 + 2L + 5 + 2.
+      TransE     acc -= fabsf((s + p) - o): the residual's two adds are within ((1 + u)^2 - 1)(|s| + |p| + |o|) of
+                 the exact one and fabsf is 1-Lipschitz, so |s| + |p| + |o| carries it (no premise on the residual's
+                 sign); L subtractions, the butterfly                                         N = 2 + L + 5.
+      RotatE     re = fmaf(-si, sn, sr * c) - o_re: s_re c passes 3 roundings, s_im sn 2, o_re 1, so |re' - re| <=
+                 ((1 + u)^3 - 1) S_re, and the same for im with S_im; the modulus is 1-Lipschitz in (re, im), so
+                 |m' - m| <= ((1 + u)^3 - 1) S, S = S_re + S_im (predict_abs).  sqrtf(fmaf(im, im, re * re)): the sum
+                 of squares is within (1 + u)^2 of re'^2 + im'^2, its square root within (1 + u) and sqrt.rn another
+                 (1 + u), so 2 more relative to m' <= S (1 + u)^3; then L subtractions and the butterfly.  N = 5 + L + 5.
+    So |got - want| <= ((1 + u)^N - 1) A <= (N + 1) u A with A = predict_abs; the + 1 is the second-order term:
+    (1 + u)^N - 1 - N u <= N^2 u^2 / (1 - N u) <= u for N <= 4,095 (asserted).
+    Underflow.  A rounding to a subnormal result adds at most 2^-150 absolute; adds and subtractions whose result is
+    subnormal are exact.  DistMult has 2 products / fmas per column that can underflow, ComplEx and HolE 6, TransE none;
+    each such error is then scaled by at most scale (1 + u)^(N + 2) < 4 (scale <= 2 at k = 1), and HolE's final multiply
+    adds one more: (n_u + 1) 2^-148 per triple, n_u = 2k, 6k or 0.  RotatE: the products of the residual and the
+    square re' * re' and the fma can underflow, which moves the sum of squares by at most 2^-148.9 absolute; through the
+    square root that is sqrt(2^-148.9) < 2^-74.4, so 2^-74 per column (the residual's own 2^-148 included): h 2^-74.
+    Non-finite entries: where a row holds +-inf or NaN and no finite value overflows, the score is NaN, +inf or -inf
+    exactly where the float64 oracle's is (every non-finite product term meets the same sums in any order: NaN is
+    absorbing and +inf + -inf is NaN); check compares these classes exactly."""
+
+    def __init__(self, model, ent, rel, triples, max_rel_size=None, device="cpu", chunk=1 << 12):
+        u = FP32_EPS
+        self.model, dev = model, torch.device(device)
+        self.device = dev
+        E = torch.as_tensor(np.asarray(ent), dtype=torch.float64, device=dev)
+        R = torch.as_tensor(np.asarray(rel), dtype=torch.float64, device=dev)
+        self.t = t = torch.as_tensor(np.asarray(triples), dtype=torch.long, device=dev).reshape(-1, 3)
+        K = E.shape[1]
+        k = K if model in ("TransE", "DistMult") else K // 2
+        self.mrs = max_rel_size or R.shape[0]
+        N = predict_chain(model, k)
+        assert N <= 4095, "second-order allowance"
+        if model == "RotatE":
+            ct, st = rotation_table(np.asarray(rel, np.float32)[:, :k], rotation_divisor32(K, self.mrs)[0])
+            ct = torch.as_tensor(ct, dtype=torch.float64, device=dev)
+            st = torch.as_tensor(st, dtype=torch.float64, device=dev)
+            absolute = k * 2.0 ** -74
+        else:
+            absolute = ({"DistMult": 2 * k, "ComplEx": 6 * k, "HolE": 6 * k, "TransE": 0}[model] + 1) * 2.0 ** -148
+        want, bound = [], []
+        with np.errstate(all="ignore"):
+            for a in range(0, t.shape[0], chunk):
+                tc = t[a:a + chunk]
+                s, p, o = E[tc[:, 0]], R[tc[:, 1]], E[tc[:, 2]]
+                want.append(scores(model, s, p, o, self.mrs, rot_table=True))
+                rot = dict(c=ct[tc[:, 1]], sn=st[tc[:, 1]]) if model == "RotatE" else {}
+                bound.append((N + 1) * u * predict_abs(model, s, p, o, **rot) + absolute)
+        self.want = torch.cat(want) if want else torch.zeros(0, dtype=torch.float64, device=dev)
+        self.bound = torch.cat(bound) if bound else torch.zeros(0, dtype=torch.float64, device=dev)
+
+    def check(self, got, want=None, rows=None):
+        """got [n] (or [len(rows)] with rows: indices into the triples) against want (default the oracle's scores):
+        the non-finite classes equal and every finite element within the bound.  -> (ok, worst error / bound over
+        the finite elements, index of the worst element (of rows, when given), or of the first class mismatch)."""
+        got = torch.as_tensor(np.asarray(got), dtype=torch.float64).to(self.device)
+        idx = slice(None) if rows is None else torch.as_tensor(np.asarray(rows), dtype=torch.long, device=self.device)
+        want = self.want[idx] if want is None else torch.as_tensor(want, dtype=torch.float64).to(self.device)
+        bound = self.bound[idx]
+        cg, cw = nonfinite_class(got), nonfinite_class(want)
+        if not bool((cg == cw).all()):
+            return False, float("inf"), int(torch.nonzero(cg != cw)[0, 0])
+        fin = cw == 0
+        err = torch.where(fin, (got - want).abs(), torch.zeros_like(got))
+        ratio = err / torch.where(fin, bound, torch.ones_like(bound))
+        if ratio.numel() == 0:
+            return True, 0.0, -1
+        worst = int(ratio.argmax())
+        return bool((err <= torch.where(fin, bound, torch.zeros_like(bound))).all()), float(ratio[worst]), worst
+
+    def assert_within(self, got, where=""):
+        """check, asserted with the worst element's triple, got, want and bound in the message.  -> worst ratio."""
+        ok, ratio, i = self.check(got)
+        if not ok:
+            g = float(np.asarray(got, np.float64).reshape(-1)[i])
+            raise AssertionError("%s: element %d, triple %s: got %r, want %r, bound %r (worst error / bound %.3g)" % (
+                where, i, self.t[i].tolist(), g, float(self.want[i]), float(self.bound[i]), ratio))
+        return ratio
+
+
+# --------------------------------------------------------------------------
 # engine plumbing shared by the GPU tests
 # --------------------------------------------------------------------------
 def dense(eng, table):
@@ -614,6 +744,34 @@ def launched(run):
         run()
         torch.cuda.synchronize()
     return {e.key for e in prof.key_averages() if "kge_" in e.key}
+
+
+def perturbed_term(model, ent, rel, triples, step, eta, factor, entities=None, max_lookups=32, device="cpu", **kw):
+    """The sensitivity checks' perturbation: the gradient tables of one corruption alone, with its dL/dscore times
+    `factor` (oracle_step with an external dL/dscore).  The corruption is the one whose replaced entity (one of
+    `entities`, default any) has the fewest lookups in the step, at most max_lookups (None: any number), then the
+    largest |dL/dscore|.  kw: oracle_step's rot_table / max_rel_size.  -> (corruption index, Step), or None where no
+    corruption qualifies."""
+    t = np.asarray(triples)
+    corr = step.corr.cpu().numpy()
+    lookups = np.bincount(np.concatenate([t[:, 0], t[:, 2], corr[:, 0], corr[:, 2]]), minlength=len(np.asarray(ent)))
+    tiled = np.tile(t, (eta, 1))
+    repl = np.where(corr[:, 0] != tiled[:, 0], corr[:, 0], corr[:, 2])
+    keep = (corr[:, 0] == tiled[:, 0]).astype(np.uint8)
+    g = step.dsn.abs().cpu().numpy()
+    ok = g > 0
+    if max_lookups is not None:
+        ok &= lookups[repl] <= max_lookups
+    if entities is not None:
+        ok &= np.isin(repl, np.asarray(entities))
+    cands = np.nonzero(ok)[0]
+    if not len(cands):
+        return None
+    r = int(min(cands, key=lambda c: (lookups[repl[c]], -g[c])))
+    i = r % len(t)
+    one = oracle_step(model, ent, rel, t[i:i + 1], 1, [repl[r]], [keep[r]], dpos=[0.0],
+                      dneg=[float(step.dsn[r]) * factor], device=device, **kw)
+    return r, one
 
 
 # --------------------------------------------------------------------------

@@ -3,6 +3,8 @@
 Run on an H100 with `pytest -m gpu`.  Tolerances: fp32 scores / gradients /
 losses within 1e-4 relative (BASELINE.json north_star); ranks bit-exact.
 """
+import zlib
+
 import numpy as np
 import pytest
 import torch
@@ -100,20 +102,83 @@ def test_reference_scoring_kats_on_gpu(kats):
         eng.close()
 
 
+def _score_tables(model, E, R, k, kind, rng):
+    """Glorot tables; 'scaled': every row times 2^e, e uniform in [-20, 20] (RotatE: entity rows only, its phases stay
+    in range), so that small scores sit beside large ones; 'subnormal': a tenth of the rows (RotatE: entity rows) with
+    subnormal entries in half their columns; 'nonfinite': +inf, -inf and NaN in a few entity rows (and one relation row
+    but RotatE's), every finite value far from overflow."""
+    ent, rel = _tables(model, E, R, k, rng)
+    K = ent.shape[1]
+    tabs = ((ent, E), (rel, R)) if model != "RotatE" else ((ent, E),)
+    if kind == "scaled":
+        for tab, rows in tabs:
+            tab *= (2.0 ** rng.integers(-20, 21, rows))[:, None].astype(np.float32)
+    elif kind == "subnormal":
+        for tab, rows in tabs:
+            for r in rng.choice(rows, max(1, rows // 10), replace=False):
+                cols = rng.random(K) < 0.5
+                tab[r, cols] = (rng.uniform(-1, 1, int(cols.sum())) * 2.0 ** -126).astype(np.float32)
+    elif kind == "nonfinite":
+        for v, r in zip((np.inf, -np.inf, np.nan) * 4, rng.choice(E, 12, replace=False)):
+            ent[r, rng.integers(0, K)] = v
+        if model != "RotatE":
+            rel[1, rng.integers(0, K)] = np.inf
+    return ent, rel
+
+
 @pytest.mark.parametrize("model", MODELS)
-@pytest.mark.parametrize("k", [5, 50, 200])
+@pytest.mark.parametrize("k", [1, 5, 31, 32, 33, 50, 100, 130, 200, 1000])
 def test_score_triples_vs_oracle(model, k):
-    from oracle import c_oracle
-    rng = np.random.default_rng(1)
-    E, R, n = 300, 7, 1000
-    ent, rel = _tables(model, E, R, k, rng, scale=0.5)
-    t = _triples(E, R, n, rng)
-    eng = _engine(model, k, 2, E, R)
-    eng.set_embeddings(ent, rel)
-    got = eng.score(_dev(t)).cpu().numpy()
-    ref = c_oracle.score_triples(model, ent, rel, t)
-    assert np.allclose(got, ref, rtol=RTOL, atol=1e-5), np.abs(got - ref).max()
-    eng.close()
+    """kge_score_triples (the predict path) against the float64 oracle, every score within exact_oracle.PredictBound:
+    n = 1, 7 and 20,000 triples (more than the grid's 64 warps per SM, so the grid-stride loop wraps) on Glorot,
+    row-scaled and subnormal tables, and RotatE with max_rel_size != n_rel; non-finite entries give NaN / +inf / -inf
+    exactly where the oracle does.  Sensitivity: the check rejects the kernel's scores against an oracle whose one entity
+    element is multiplied by 1 + 2^-10 (an element made dominant in its row, 32 times the Glorot limit, so that it
+    carries a few percent of its triple's |score|_abs even at k = 1,000)."""
+    import exact_oracle as xo
+    E, R = 3000, 11
+    rng = np.random.default_rng(zlib.crc32(repr((model, k)).encode()))
+    sm = torch.cuda.get_device_properties(0).multi_processor_count
+    big = max(20000, 64 * sm + 1000)
+    runs = [("glorot", None), ("scaled", None), ("subnormal", None), ("nonfinite", None)]
+    if model == "RotatE":
+        runs.append(("glorot", 3 * R + 2))
+    ratios = {}
+    for kind, mrs in runs:
+        ent, rel = _score_tables(model, E, R, k, kind, rng)
+        t_big = _triples(E, R, big, rng)
+        if kind == "glorot" and mrs is None:  # the sensitivity probe: triple 0's subject row, its dominant element
+            e = int(t_big[0, 0])
+            x = torch.as_tensor(ent, dtype=torch.float64)
+            s = x[t_big[:1, 0]].clone().requires_grad_(True)
+            xo.scores(model, s, torch.as_tensor(rel, dtype=torch.float64)[t_big[:1, 1]], x[t_big[:1, 2]], R,
+                      rot_table=True).sum().backward()
+            j = int((s.grad[0] * s.detach()[0]).abs().argmax())
+            ent[e, j] = np.float32(32 * np.sqrt(6.0 / (E + ent.shape[1])) * (1 if ent[e, j] >= 0 else -1))
+        eng = _engine(model, k, 2, E, R, max_rel_size=mrs)
+        eng.set_embeddings(ent, rel)
+        for n in (1, 7, big):
+            t = t_big[:n]
+            got = eng.score(_dev(t)).cpu().numpy()
+            bound = xo.PredictBound(model, ent, rel, t, max_rel_size=mrs, device="cuda")
+            where = "%s k=%d %s max_rel_size=%s n=%d" % (model, k, kind, mrs, n)
+            if kind == "nonfinite":
+                ok, ratio, i = bound.check(got)
+                assert ok, (where, i, t[i].tolist(), float(got[i]), float(bound.want[i]))
+                assert n < big or not np.isfinite(got).all(), where
+            else:
+                assert np.isfinite(got).all(), where
+                ratio = bound.assert_within(got, where)
+            ratios["%s%s n=%d" % (kind, "" if mrs is None else " mrs=%d" % mrs, n)] = round(ratio, 4)
+        if kind == "glorot" and mrs is None:  # sensitivity, on the n = 20,000 run
+            ent2 = ent.copy()
+            ent2[e, j] *= np.float32(1 + 2.0 ** -10)
+            rows = np.nonzero((t[:, 0] == e) | (t[:, 2] == e))[0]
+            want2 = xo.PredictBound(model, ent2, rel, t[rows], device="cuda").want
+            assert not bound.check(got[rows], want=want2, rows=rows)[0], "%s k=%d: the check accepts a perturbed " \
+                "entity element" % (model, k)
+        eng.close()
+    print("\n%s k=%d: worst error / bound %s" % (model, k, ratios))
 
 
 # ---------------------------------------------------------------------------

@@ -204,17 +204,9 @@ def run_case(monkeypatch, model, k, eta, *, E=2000, R=11, B=600, loss="nll", lp=
             assert torch.equal(got, (x.float() + s[0].float()).double()), where + ": new table != fl32(x0 + slot0)"
 
     # sensitivity: one corruption's dL/dscore times 1 + 2^-10 (its replaced entity has at most 32 lookups)
-    lookups = np.bincount(np.concatenate([t[:, 0], t[:, 2], corr[:, 0], corr[:, 2]]), minlength=E)
-    tiled = np.tile(t, (eta, 1))
-    repl = np.where(corr[:, 0] != tiled[:, 0], corr[:, 0], corr[:, 2])
-    keep = (corr[:, 0] == tiled[:, 0]).astype(np.uint8)
-    g = ref.dsn.abs().cpu().numpy()
-    cands = np.nonzero((lookups[repl] <= 32) & (g > 0))[0]
-    assert len(cands), where + ": no corruption with a replaced entity of at most 32 lookups"
-    r = int(min(cands, key=lambda c: (lookups[repl[c]], -g[c])))
-    i = r % B
-    one = xo.oracle_step(model, ent, rel, t[i:i + 1], 1, [repl[r]], [keep[r]], dpos=[0.0],
-                         dneg=[float(ref.dsn[r]) * 2.0 ** -10], device=oracle_device)
+    pick = xo.perturbed_term(model, ent, rel, t, ref, eta, 2.0 ** -10, device=oracle_device)
+    assert pick is not None, where + ": no corruption with a replaced entity of at most 32 lookups"
+    one = pick[1]
     res = bound.check(g_ent, g_rel, ref.g_ent + one.g_ent, ref.g_rel + one.g_rel)
     assert not all(ok for _, ok, _ in res), where + ": the check accepts a perturbed dL/dscore"
 

@@ -87,6 +87,9 @@ PROTOTYPES = {
                                        _P, _P]),
     "kge_nscaching_step": (C.c_int, [_P, C.POINTER(KgeNSCaching), _P, _P, _P, _P, _P, C.c_int64, C.c_uint64, C.c_uint64,
                                      _P, _P, _P, _P]),
+    "kge_shared_negatives_workspace_bytes": (C.c_int64, [_P, C.c_int64, C.c_int64]),
+    "kge_shared_negatives_step": (C.c_int, [_P, C.c_int64, _P, _P, _P, _P, _P, C.c_int64, C.POINTER(KgeNegativeSampler),
+                                            C.c_uint64, C.c_uint64, _P, _P, C.c_int64, _P]),
     "kge_train_step": (C.c_int, [_P, C.c_int32, _P, _P, _P, _P, _P, C.c_int64, _P, _P, C.c_uint64, C.c_uint64,
                                  _P, _P, _P, _P, _P, _P]),
     "kge_train_step_sharded": (C.c_int, [_P, C.c_int32, C.POINTER(KgeShardMap), _P, _P, _P, C.c_int64, _P, _P,

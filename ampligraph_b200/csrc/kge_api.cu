@@ -590,6 +590,100 @@ extern "C" int kge_nscaching_step(kge_handle *h, const kge_nscaching *cache, con
     return KGE_OK;
 }
 
+// Carve-up of the shared-negatives workspace for B positives: [B, eta] scores, [B] positive scores, [B, eta] sides
+static void carve_shared_negatives(const kge_handle *h, int64_t B, Carve &c, SharedNegParams *q)
+{
+    const size_t n = (size_t)h->cfg.eta * (size_t)B;
+    float *sc = c.take<float>(4 * n, 16);
+    float *pos = c.take<float>(4 * (size_t)B, 16);
+    uint8_t *keep = c.take<uint8_t>(n, 16);
+    if (q) { q->sc = sc; q->pos = pos; q->keep = keep; }
+}
+
+extern "C" int64_t kge_shared_negatives_workspace_bytes(const kge_handle *h, int64_t B, int64_t chunk)
+{
+    if (!h || B < 0 || chunk < 1) return 0;
+    Carve c(nullptr);
+    carve_shared_negatives(h, B, c, nullptr);
+    return (int64_t)c.at;
+}
+
+static bool dropout_set(const kge_handle *h);
+
+// Shared negatives: the score, loss and gradient passes of kge_train_shared.cu
+extern "C" int kge_shared_negatives_step(kge_handle *h, int64_t chunk, const float *ent_dev, const float *rel_dev,
+                                         float *grad_ent_dev, float *grad_rel_dev, const int32_t *triples_dev, int64_t B,
+                                         const kge_negative_sampler *sampler, uint64_t seed, uint64_t step,
+                                         double *loss_dev, void *workspace_dev, int64_t ws_bytes, void *stream)
+{
+    KGE_CHECK_HANDLE(h, "kge_shared_negatives_step");
+    if (chunk < 1) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_shared_negatives_step: chunk must be >= 1, got %lld", (long long)chunk);
+    if (B < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_shared_negatives_step: B < 0");
+    if (B > ((1ll << 56) - 1) / h->cfg.eta) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_shared_negatives_step: eta*B >= 2^56");
+    const kge_negative_sampler *s = sampler;
+    if (s && (s->struct_size != (int32_t)sizeof(kge_negative_sampler) || s->max_attempts < 1 || s->max_attempts > 256))
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_shared_negatives_step: bad kge_negative_sampler (ABI mismatch or "
+                                              "max_attempts outside 1..256)");
+    if (int rc = check_no_pending(h, "kge_shared_negatives_step")) return rc;
+    if (s && (s->sub_pool_off_dev || s->sub_pool_ids_dev || s->obj_pool_off_dev || s->obj_pool_ids_dev ||
+              s->sub_filter_n != 0 || s->obj_filter_n != 0))
+        return fail(KGE_ERR_UNSUPPORTED, "kge_shared_negatives_step: a sampler with pools or a filter picks entities per "
+                                         "positive, and shared negatives draw one candidate set per chunk");
+    if (h->stash)
+        return fail(KGE_ERR_UNSUPPORTED, "kge_shared_negatives_step: a row stash is set (row-sharded tables): shared "
+                                         "negatives read one whole entity table");
+    if (dropout_set(h))
+        return fail(KGE_ERR_UNSUPPORTED, "kge_shared_negatives_step: embedding dropout is set (kge_set_embedding_dropout), "
+                                         "and the sampled training kernels do not apply it");
+    if (B == 0) return KGE_OK;
+    if (!ent_dev || !rel_dev || !grad_ent_dev || !grad_rel_dev || !triples_dev || !workspace_dev)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_shared_negatives_step: null table, gradient, triples or workspace pointer");
+    const int64_t need = kge_shared_negatives_workspace_bytes(h, B, chunk);
+    if (ws_bytes < need || ((uintptr_t)workspace_dev & 15))
+        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_shared_negatives_step: workspace of %lld bytes (need %lld, 16-byte "
+                                              "aligned)", (long long)ws_bytes, (long long)need);
+    const long long ctas = shared_negatives_grid(B, chunk, h->cfg.eta, nullptr);
+    if (ctas >= (1ll << 31))
+        return fail(KGE_ERR_UNSUPPORTED, "kge_shared_negatives_step: %lld CTAs exceed one launch", ctas);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (int rc = refresh_rotation(h, rel_dev, st)) return rc;
+    SharedNegParams q;
+    memset(&q, 0, sizeof(q));
+    TrainParams &p = q.t;
+    p.ent = ent_dev;
+    p.rel = h->cfg.scoring == KGE_ROTATE ? h->rot : rel_dev;  // the table refresh_rotation has just written
+    p.grad_ent = grad_ent_dev;
+    p.grad_rel = grad_rel_dev;
+    p.triples = triples_dev;
+    p.B = B;
+    p.seed = seed;
+    p.step = step;
+    p.n_ent = (unsigned)h->cfg.n_ent;
+    p.model = h->cfg.scoring;
+    p.eta = h->cfg.eta;
+    p.kp = h->L.kp;
+    p.ld = h->L.ld;
+    p.nch = h->L.kp / 4;
+    p.loss = h->cfg.loss;
+    p.reduction = h->cfg.reduction;
+    p.mode = KGE_STEP_FUSED;
+    p.margin = h->cfg.margin;
+    p.alpha = h->cfg.alpha;
+    p.score_scale = h->score_scale;
+    p.inv_div = 1.f / h->rot_div;
+    p.loss_out = loss_dev;
+    p.stamp = kge_step_stamp(step);
+    p.stamp_ent = h->stamp_ent;
+    p.stamp_rel = h->stamp_ent ? h->stamp_rel : nullptr;
+    q.chunk = chunk;
+    q.thr = s ? s->thresholds_dev : nullptr;
+    Carve c(workspace_dev);
+    carve_shared_negatives(h, B, c, &q);
+    shared_negatives_grid(B, chunk, h->cfg.eta, &q);
+    KGE_CUDA(launch_shared_negatives(q, h->sm_count, st), "kge_shared_negatives_step");
+    return KGE_OK;
+}
+
 static bool dropout_set(const kge_handle *h) { return h->drop_p_ent != 0.f || h->drop_p_rel != 0.f; }
 
 // The sampled steps' fused kernels read the raw rows: they refuse while embedding dropout is set

@@ -132,6 +132,23 @@ struct NSCacheParams {
 size_t nscaching_smem_bytes(int ld, int n1, int n2);
 cudaError_t launch_nscaching(const NSCacheParams &p, int sm_count, cudaStream_t st);
 
+// kge_train_shared.cu: sampled training with shared negatives (kge_shared_negatives_step).  t carries the tables,
+// triples, Philox key, loss and stamps as for the fused step (t.neg_ent and the slot fields are not read).
+struct SharedNegParams {
+    TrainParams t;
+    long long chunk;           // C >= 1 positives per chunk
+    const uint32_t *thr;       // [n_rel] Bernoulli side thresholds, or nullptr: fair coin
+    float *sc;                 // [B, eta] workspace: scores, then dL/dscore
+    uint8_t *keep;             // [B, eta] workspace: side of each corruption (1: object replaced)
+    float *pos;                // [B] workspace: the positive's score, then dL/dP
+    long long n_chunks, n_ps;  // chunks, and positive slices per chunk, of the score and gradient grids
+    int n_jt;                  // candidate tiles
+};
+// CTAs of the score and gradient passes for (B, chunk, eta); fills q's grid fields when q != nullptr
+long long shared_negatives_grid(long long B, long long chunk, int eta, SharedNegParams *q);
+// the score, loss and gradient passes, on st
+cudaError_t launch_shared_negatives(const SharedNegParams &q, int sm_count, cudaStream_t st);
+
 // kge_train_1vsall.cu: one side of a 1vsAll multiclass-NLL step of the trilinear models (kge_one_vs_all_step)
 struct OneVsAllSide {
     const float *q;          // [B, ld] query vectors of the side (launch_rank_prepare: qvec_s for side s, qvec_o for o;

@@ -119,6 +119,14 @@ def k_vs_all_workspace_bytes(B, n_ent, ld, dropout=False):
     return 2 * r16(rows) + r16(4 * B) + r16(ns * rows) + dropout_workspace_bytes(n_ent, ld, dropout)
 
 
+def shared_negatives_workspace_bytes(B, eta):
+    """kge_shared_negatives_workspace_bytes(h, B, chunk) for a handle with eta corruptions per positive (any chunk >= 1):
+    the [B, eta] scores, the [B] positive scores and the [B, eta] side bytes, each region padded to 16 bytes."""
+    r16 = lambda n: (n + 15) // 16 * 16
+    n = int(B) * int(eta)
+    return r16(4 * n) + r16(4 * int(B)) + r16(n)
+
+
 INT32_MAX = 2 ** 31 - 1
 DBSCAN_BATCH = 1024  # queries per kge_radius_* call of KGEEngine.dbscan (discovery.find_duplicates' batch)
 
@@ -636,6 +644,24 @@ class KGEEngine:
         if B:
             n = 2 if sides == "s,o" else 1
             self.launches += 2 + (1 if self.lazy else 0) + 5 * n + self._dropout_launches(n)
+
+    @_traced("kge.shared_negatives_step")
+    def shared_negatives_backward(self, triples, chunk, seed=0, step=0, sampler=None):
+        """Sampled step with shared negatives up to tape.gradient (kge_shared_negatives_step, DESIGN.md 3.21): the
+        batch is cut into chunks of `chunk` consecutive positives, and every positive of a chunk is corrupted against
+        the chunk's eta candidate entities, each corruption on the side the per-positive sampler picks; the engine's
+        loss and reduction apply per positive.  Accumulates into g_ent / g_rel and loss_acc[0] like forward_backward.
+        sampler: a NegativeSamplerTables whose Bernoulli thresholds pick the sides (pools and filters are refused), or
+        None for the fair coin.  step: the Philox counter and the lazy optimizer's row stamp.  apply_gradients() takes
+        its non-deferred path next."""
+        B = triples.shape[0]
+        self._step_call("shared_negatives_backward", self.lib.kge_shared_negatives_step,
+                        self.lib.kge_shared_negatives_workspace_bytes(self.h, B, int(chunk)), triples, step, (int(chunk),),
+                        (C.byref(sampler.struct) if sampler is not None else None, int(seed), int(step),
+                         _ptr(self.loss_acc)))
+        # RotatE: rotation table; score, loss and gradient passes
+        if B:
+            self.launches += 3 + (1 if self.scoring_type == "RotatE" else 0)
 
     @_traced("kge.one_vs_all_relation_step")
     def one_vs_all_relation_backward(self, triples, weight, step=0):

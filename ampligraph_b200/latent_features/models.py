@@ -269,7 +269,8 @@ class ScoringBasedEmbeddingModel:
             validation_corrupt_side="s,o", validation_freq=10, validation_burn_in=0, validation_filter=False,
             validation_entities_subset=None, partitioning_k=1, focusE=False, focusE_params={}, one_vs_all=None,
             k_vs_all=None, label_smoothing=0.0, relation_prediction_weight=0.0, negative_sampler="uniform",
-            filter_negatives=False, entity_dropout=0.0, relation_dropout=0.0, negative_sampler_params=None):
+            filter_negatives=False, entity_dropout=0.0, relation_dropout=0.0, negative_sampler_params=None,
+            shared_negatives=0):
         """fit (:544-883).  `shuffle` is accepted and ignored exactly like the reference
         (batches are the sequential slices of graph_data_loader.py:495-500).  validation_split: carve the validation
         set out of x with train_test_split_no_unseen(x, test_size=validation_split, seed=self.seed), as the reference
@@ -337,7 +338,20 @@ class ScoringBasedEmbeddingModel:
         model's seed and the step.  They apply to one_vs_all and k_vs_all training only (with reciprocal relations,
         relation_prediction_weight, N3, DURA, label smoothing and either reduction); the regularisers, the optimizer,
         validation, evaluate, predict and every later call read the raw embeddings.  The logged loss is that of the
-        dropped-out scores.  0.0 (the default) leaves training unchanged."""
+        dropped-out scores.  0.0 (the default) leaves training unchanged.
+
+        shared_negatives (extension; DESIGN.md 3.21; PyTorch-BigGraph, DGL-KE): an int C >= 1 cuts every batch into
+        chunks of C consecutive positives (the last may be shorter) and corrupts all positives of a chunk against one
+        set of eta candidate entities drawn from (seed, step), each corruption on the side the per-positive sampler
+        picks ('uniform' or 'bernoulli').  The GPU step reads a candidate row once per slice of 16 positives of a
+        chunk instead of once per positive, whatever C is: C > 16 changes which negatives are drawn, not the cost.
+        Measured on an H100 at eta = 256 (DESIGN.md 5), the step is faster than the per-positive one for RotatE and
+        TransE at k = 1,000 (1.25x, 1.14x) and slower for ComplEx k = 200 on an FB15k-237-sized table (0.57x), whose
+        per-positive step reads its rows from L2; it is not a general speed-up.  Every built-in loss,
+        both reductions, N3 / DURA / LP regularisers and every optimizer apply as in the fused step; with C = 1 the
+        corruptions are those of the default draw.  It is refused with one_vs_all or k_vs_all, with 'pseudo_typed',
+        'nscaching' or filter_negatives=True (ValueError: they pick entities per positive), and with a user loss,
+        focusE or several GPUs (NotImplementedError).  0 (the default) trains as before."""
         self._assert_compile_was_called()
         self._check_dropout(entity_dropout, relation_dropout, one_vs_all, k_vs_all)
         if self.reciprocal_relations:
@@ -350,6 +364,7 @@ class ScoringBasedEmbeddingModel:
         if one_vs_all is not None:
             self._check_one_vs_all(one_vs_all, focusE)
         self._check_relation_prediction(relation_prediction_weight, one_vs_all, k_vs_all)
+        self._check_shared_negatives(shared_negatives, one_vs_all, k_vs_all, negative_sampler, filter_negatives, focusE)
         if validation_split:
             assert isinstance(x, np.ndarray), "Validation split supported for numpy arrays only!"
             x, validation_data = train_test_split_no_unseen(x, test_size=validation_split, seed=self.seed,
@@ -389,7 +404,7 @@ class ScoringBasedEmbeddingModel:
                                   validation_batch_size, validation_corrupt_side, validation_freq, validation_burn_in,
                                   validation_filter, validation_entities_subset, one_vs_all, k_vs_all, label_smoothing,
                                   relation_prediction_weight, negative_sampler, filter_negatives, sampled_option,
-                                  negative_sampler_params)
+                                  negative_sampler_params, shared_negatives)
         finally:
             if any(dropout):
                 eng.set_embedding_dropout(0.0, 0.0)
@@ -398,7 +413,7 @@ class ScoringBasedEmbeddingModel:
                   validation_batch_size, validation_corrupt_side, validation_freq, validation_burn_in,
                   validation_filter, validation_entities_subset, one_vs_all, k_vs_all, label_smoothing,
                   relation_prediction_weight, negative_sampler, filter_negatives, sampled_option,
-                  negative_sampler_params=None):
+                  negative_sampler_params=None, shared_negatives=0):
         """fit's training loop, on the engine fit has built (with fit's embedding dropout set on it)."""
         eng = self.engine
         eng.set_hot_entities(triples=triples)  # the most frequent entities of the training set: their gradient rows are summed per warp
@@ -466,6 +481,11 @@ class ScoringBasedEmbeddingModel:
                     eng.one_vs_all_backward(batch, ova_sides, step=self._step)
                     if relation_prediction_weight > 0:
                         eng.one_vs_all_relation_backward(batch, relation_prediction_weight, step=self._step)
+                    self._per_occurrence_backward(batch)
+                    eng.apply_gradients()
+                elif shared_negatives:
+                    eng.shared_negatives_backward(batch, shared_negatives, seed=self.seed, step=self._step,
+                                                  sampler=sampler)
                     self._per_occurrence_backward(batch)
                     eng.apply_gradients()
                 elif self.use_focusE:
@@ -592,6 +612,27 @@ class ScoringBasedEmbeddingModel:
         if self._world() > 1:
             raise NotImplementedError("negative_sampler and filter_negatives are single-GPU only")
         return True
+
+    def _check_shared_negatives(self, chunk, one_vs_all, k_vs_all, negative_sampler, filter_negatives, focusE):
+        """The refusals of fit(shared_negatives=C), before anything is indexed or trained: C an int >= 0 (not a bool);
+        C >= 1 needs sampled training on one GPU with a built-in loss, without focusE, and a sampler that picks only
+        the side ('uniform' or 'bernoulli', unfiltered)."""
+        if isinstance(chunk, (bool, np.bool_)) or not isinstance(chunk, (int, np.integer)) or chunk < 0:
+            raise ValueError("shared_negatives must be an int >= 0 (positives per chunk; 0: off), got %r" % (chunk,))
+        if chunk == 0:
+            return
+        if one_vs_all is not None or k_vs_all is not None:
+            raise ValueError("shared_negatives is a sampled-training option: it cannot be combined with one_vs_all or "
+                             "k_vs_all")
+        if negative_sampler in ("pseudo_typed", "nscaching") or filter_negatives:
+            raise ValueError("shared_negatives draws one candidate set per chunk, and negative_sampler=%r%s picks "
+                             "entities per positive: use 'uniform' or 'bernoulli' without filter_negatives"
+                             % (negative_sampler, " with filter_negatives=True" if filter_negatives else ""))
+        if isinstance(self.compiled_loss, loss_functions.LossFunctionWrapper) or focusE:
+            raise NotImplementedError("shared_negatives applies the compiled built-in loss inside its kernels: user "
+                                      "losses and focusE are not supported")
+        if self.distributed or self._world() > 1:
+            raise NotImplementedError("shared_negatives is single-GPU only")
 
     @staticmethod
     def _check_nscaching_params(negative_sampler, params):

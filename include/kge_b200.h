@@ -314,6 +314,35 @@ int kge_train_step(kge_handle *h, int32_t mode, const float *ent_dev, const floa
                    uint64_t step, double *loss_dev, float *scores_pos_dev, float *scores_neg_dev,
                    const float *dpos_dev, const float *dneg_dev, void *stream);
 
+/* Shared negatives (extension; DESIGN.md 3.21; PyTorch-BigGraph, DGL-KE): a sampled training step whose B positives
+ * are cut into chunks of C consecutive positives, chunk k = positives [k C, min((k + 1) C, B)), each chunk corrupted
+ * against one set of eta candidate entities:
+ *   candidate  c_{k,j} = (y * n_ent) >> 32, (x, y, ..) the Philox4x32-10 block of kge_generate_corruptions for
+ *              corruption r = j*B + k*C (the chunk's first positive), j = 0..eta-1
+ *   side       corruption j of positive i replaces the side the per-positive sampler picks for r = j*B + i:
+ *              keep_subj = x & 1 without thresholds, with them the subject is replaced iff x < thresholds[p]
+ *   corruption (c_{k,j}, p, o) or (s, p, c_{k,j}); candidates equal to a positive's own entity or to each other are
+ *              ordinary corruptions (no filtering)
+ * With C = 1 the corruptions are kge_generate_corruptions' (kge_sample_negatives' with thresholds only).  The handle's
+ * loss and reduction apply per positive to its eta corruption scores, as in kge_train_step; the gradient of every row
+ * the step read (s, p, o of each positive, every candidate) is ADDED to grad_*_dev, the loss to *loss_dev (may be
+ * NULL), and the lazy optimizer's stamps are written for those rows.  The rotation table is refreshed from rel_dev for
+ * RotatE.
+ *   chunk       C >= 1 (C >= B: one chunk)
+ *   sampler     only its thresholds_dev is used (max_attempts must be valid); NULL: fair coin
+ *   workspace   caller-owned, 16-byte aligned, at least kge_shared_negatives_workspace_bytes(h, B, chunk) bytes
+ * KGE_ERR_INVALID_ARGUMENT without a launch for chunk < 1, B < 0, eta*B >= 2^56, null pointers when B > 0, a short
+ * or not 16-byte aligned workspace, a bad sampler struct or a pending KGE_STEP_FUSED_DEFER step; KGE_ERR_UNSUPPORTED
+ * for a sampler with pools or a filter, while a row stash is set (row-sharded tables) or embedding dropout is set, or
+ * when the score and gradient passes would need 2^31 or more CTAs (chunks x ceil(min(C, B) / 16) x ceil(eta / 32)).
+ * B = 0 is a no-op.
+ * Stream-ordered, allocates nothing. */
+int64_t kge_shared_negatives_workspace_bytes(const kge_handle *h, int64_t B, int64_t chunk);
+int kge_shared_negatives_step(kge_handle *h, int64_t chunk, const float *ent_dev, const float *rel_dev,
+                              float *grad_ent_dev, float *grad_rel_dev, const int32_t *triples_dev, int64_t B,
+                              const kge_negative_sampler *sampler, uint64_t seed, uint64_t step, double *loss_dev,
+                              void *workspace_dev, int64_t ws_bytes, void *stream);
+
 /* Row-sharded entity table (SURVEY.md 8e, BASELINE configs[3],[4]: |E|*k too large for one GPU).
  * Entity id e lives on rank e / rows_per_shard at local row e % rows_per_shard; every rank's shard
  * [rows_per_shard, ld] and its gradient shard are peer-mapped (torch symmetric memory / cudaIpc /

@@ -301,6 +301,12 @@ static int refresh_rotation(kge_handle *h, const float *rel_dev, cudaStream_t st
     return KGE_OK;
 }
 
+// The relation rows a step or query reads: for RotatE the rotation table refresh_rotation writes, else the relation table
+static const float *relation_rows(const kge_handle *h, const float *rel_dev)
+{
+    return h->cfg.scoring == KGE_ROTATE ? h->rot : rel_dev;
+}
+
 extern "C" int kge_score_triples(kge_handle *h, const float *ent_dev, const float *rel_dev,
                                  const int32_t *triples_dev, int64_t n, float *scores_dev, void *stream)
 {
@@ -311,9 +317,8 @@ extern "C" int kge_score_triples(kge_handle *h, const float *ent_dev, const floa
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_score_triples: null pointer");
     cudaStream_t st = (cudaStream_t)stream;
     if (int rc = refresh_rotation(h, rel_dev, st)) return rc;
-    const float *rel = h->cfg.scoring == KGE_ROTATE ? h->rot : rel_dev;
-    KGE_CUDA(launch_score_triples(h->L, h->nit, ent_dev, rel, triples_dev, n, h->score_scale, scores_dev,
-                                  h->sm_count, st),
+    KGE_CUDA(launch_score_triples(h->L, h->nit, ent_dev, relation_rows(h, rel_dev), triples_dev, n, h->score_scale,
+                                  scores_dev, h->sm_count, st),
              "kge_score_triples");
     return KGE_OK;
 }
@@ -331,31 +336,118 @@ extern "C" int kge_generate_corruptions(kge_handle *h, const int32_t *triples_de
     return KGE_OK;
 }
 
+// ---- the sampled steps' shared checks and set-up: the negative sampler, NSCaching, shared negatives, the fused step ----
+
+// A kge_negative_sampler's header: its struct_size, and max_attempts 1..256 (the attempt is the top byte of the Philox
+// counter's second word)
+static int check_sampler(const kge_negative_sampler *q, const char *fn)
+{
+    if (!q || q->struct_size != (int32_t)sizeof(kge_negative_sampler) || q->max_attempts < 1 || q->max_attempts > 256)
+        return fail(KGE_ERR_INVALID_ARGUMENT, "%s: bad kge_negative_sampler (ABI mismatch or max_attempts outside 1..256)",
+                    fn);
+    return KGE_OK;
+}
+
+// The known-pair filter of both sides of a sampler struct (kge_negative_sampler, kge_nscaching): refuses a count < 0,
+// or > 0 without its arrays, and copies them into the filt_* arrays of the launch parameters p (NegativeParams,
+// NSCacheParams; [0] a replaced subject, [1] a replaced object).  The kernels keep three arrays rather than one struct per
+// side: indexing a struct by side costs the NSCaching refresh kernels up to 10 registers.
+template <class Sampler, class Params> static int side_filters(const Sampler *q, const char *fn, Params &p)
+{
+    p.filt_n[0] = q->sub_filter_n;
+    p.filt_keys[0] = reinterpret_cast<const long long *>(q->sub_filter_keys_dev);
+    p.filt_vals[0] = q->sub_filter_vals_dev;
+    p.filt_n[1] = q->obj_filter_n;
+    p.filt_keys[1] = reinterpret_cast<const long long *>(q->obj_filter_keys_dev);
+    p.filt_vals[1] = q->obj_filter_vals_dev;
+    for (int side = 0; side < 2; ++side)
+        if (p.filt_n[side] < 0 || (p.filt_n[side] > 0 && (!p.filt_keys[side] || !p.filt_vals[side])))
+            return fail(KGE_ERR_INVALID_ARGUMENT, "%s: a filter count < 0, or > 0 without its arrays", fn);
+    return KGE_OK;
+}
+
+// A sampled batch of B positives: B >= 0 and eta*B < 2^56 (corruption r = j*B + i shares a Philox counter word with
+// the sampler's attempt byte)
+static int check_sampled_batch(const kge_handle *h, int64_t B, const char *fn)
+{
+    if (B < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: B < 0", fn);
+    if (B > ((1ll << 56) - 1) / h->cfg.eta) return fail(KGE_ERR_INVALID_ARGUMENT, "%s: eta*B >= 2^56", fn);
+    return KGE_OK;
+}
+
+// The steps that read one whole entity table (NSCaching, shared negatives) refuse while a row stash is set
+static int check_no_stash(const kge_handle *h, const char *fn)
+{
+    if (h->stash)
+        return fail(KGE_ERR_UNSUPPORTED, "%s: a row stash is set (row-sharded tables), and this step reads one whole "
+                                         "entity table", fn);
+    return KGE_OK;
+}
+
+static bool dropout_set(const kge_handle *h) { return h->drop_p_ent != 0.f || h->drop_p_rel != 0.f; }
+
+// The sampled steps' fused kernels read the raw rows: they refuse while embedding dropout is set
+static int check_no_dropout(const kge_handle *h, const char *fn)
+{
+    if (!dropout_set(h)) return KGE_OK;
+    return fail(KGE_ERR_UNSUPPORTED, "%s: embedding dropout is set (kge_set_embedding_dropout), and the sampled training "
+                                     "kernels do not apply it: it applies to kge_one_vs_all_step, "
+                                     "kge_one_vs_all_relation_step and kge_k_vs_all_step; clear it with (0, 0)", fn);
+}
+
+// The TrainParams of a sampled training step that come from the handle and the call: the tables (rel as relation_rows
+// gives it: refresh_rotation first), the triples, the Philox key, the row shape, the loss and the lazy-optimizer
+// stamps.  Every other field is zero.  The kernels write the relation stamps only while the entity stamps are set.
+static TrainParams sampled_train_params(const kge_handle *h, const float *ent_dev, const float *rel_dev,
+                                        float *grad_ent_dev, float *grad_rel_dev, const int32_t *triples_dev, int64_t B,
+                                        uint64_t seed, uint64_t step, double *loss_dev)
+{
+    TrainParams p;
+    memset(&p, 0, sizeof(p));
+    p.ent = ent_dev;
+    p.rel = relation_rows(h, rel_dev);
+    p.grad_ent = grad_ent_dev;
+    p.grad_rel = grad_rel_dev;
+    p.triples = triples_dev;
+    p.B = B;
+    p.seed = seed;
+    p.step = step;
+    p.n_ent = (unsigned)h->cfg.n_ent;
+    p.model = h->cfg.scoring;
+    p.eta = h->cfg.eta;
+    p.kp = h->L.kp;
+    p.ld = h->L.ld;
+    p.nch = h->L.kp / 4;
+    p.loss = h->cfg.loss;
+    p.reduction = h->cfg.reduction;
+    p.margin = h->cfg.margin;
+    p.alpha = h->cfg.alpha;
+    p.score_scale = h->score_scale;
+    p.inv_div = 1.f / h->rot_div;
+    p.loss_out = loss_dev;
+    p.stamp = kge_step_stamp(step);
+    p.stamp_ent = h->stamp_ent;
+    p.stamp_rel = h->stamp_rel;
+    return p;
+}
+
 extern "C" int kge_sample_negatives(kge_handle *h, const kge_negative_sampler *sampler, const int32_t *triples_dev,
                                     int64_t B, uint64_t seed, uint64_t step, int32_t *neg_ent_dev,
                                     uint8_t *neg_keep_subj_dev, uint64_t *misses_dev, void *stream)
 {
     KGE_CHECK_HANDLE(h, "kge_sample_negatives");
     const kge_negative_sampler *q = sampler;
-    if (!q || q->struct_size != (int32_t)sizeof(kge_negative_sampler))
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_sample_negatives: bad kge_negative_sampler (ABI mismatch)");
-    if (q->max_attempts < 1 || q->max_attempts > 256)  // the attempt is the top byte of the counter's second word
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_sample_negatives: max_attempts must be 1..256, got %d", q->max_attempts);
+    if (int rc = check_sampler(q, "kge_sample_negatives")) return rc;
     if ((q->sub_pool_off_dev == nullptr) != (q->sub_pool_ids_dev == nullptr) ||
         (q->obj_pool_off_dev == nullptr) != (q->obj_pool_ids_dev == nullptr))
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_sample_negatives: a pool needs both its offsets and its ids");
-    if (q->sub_filter_n < 0 || q->obj_filter_n < 0 ||
-        (q->sub_filter_n > 0 && (!q->sub_filter_keys_dev || !q->sub_filter_vals_dev)) ||
-        (q->obj_filter_n > 0 && (!q->obj_filter_keys_dev || !q->obj_filter_vals_dev)))
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_sample_negatives: a filter count < 0, or > 0 without its arrays");
-    if (B < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_sample_negatives: B < 0");
-    if (B > ((1ll << 56) - 1) / h->cfg.eta)  // eta*B >= 2^56 (the corruption index shares a counter word with the attempt)
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_sample_negatives: eta*B >= 2^56");
+    NegativeParams p;
+    memset(&p, 0, sizeof(p));
+    if (int rc = side_filters(q, "kge_sample_negatives", p)) return rc;
+    if (int rc = check_sampled_batch(h, B, "kge_sample_negatives")) return rc;
     if (B == 0) return KGE_OK;
     if (!triples_dev || !neg_ent_dev || !neg_keep_subj_dev)
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_sample_negatives: null triples or output pointer");
-    NegativeParams p;
-    memset(&p, 0, sizeof(p));
     p.triples = triples_dev;
     p.B = B;
     p.eta = h->cfg.eta;
@@ -368,12 +460,6 @@ extern "C" int kge_sample_negatives(kge_handle *h, const kge_negative_sampler *s
     p.pool_ids[0] = q->sub_pool_ids_dev;
     p.pool_off[1] = reinterpret_cast<const long long *>(q->obj_pool_off_dev);
     p.pool_ids[1] = q->obj_pool_ids_dev;
-    p.filt_n[0] = q->sub_filter_n;
-    p.filt_keys[0] = reinterpret_cast<const long long *>(q->sub_filter_keys_dev);
-    p.filt_vals[0] = q->sub_filter_vals_dev;
-    p.filt_n[1] = q->obj_filter_n;
-    p.filt_keys[1] = reinterpret_cast<const long long *>(q->obj_filter_keys_dev);
-    p.filt_vals[1] = q->obj_filter_vals_dev;
     p.neg_ent = neg_ent_dev;
     p.neg_keep = neg_keep_subj_dev;
     p.misses = reinterpret_cast<unsigned long long *>(misses_dev);
@@ -536,29 +622,23 @@ extern "C" int kge_nscaching_step(kge_handle *h, const kge_nscaching *cache, con
                                               "<= 512, got %d and %d", q->cache_size, q->random_size);
     if (q->sub_n_keys < 1 || q->obj_n_keys < 1 || !q->sub_ids_dev || !q->sub_count_dev || !q->obj_ids_dev || !q->obj_count_dev)
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_nscaching_step: a side without cache rows or with null cache arrays");
-    if (q->sub_filter_n < 0 || q->obj_filter_n < 0 ||
-        (q->sub_filter_n > 0 && (!q->sub_filter_keys_dev || !q->sub_filter_vals_dev)) ||
-        (q->obj_filter_n > 0 && (!q->obj_filter_keys_dev || !q->obj_filter_vals_dev)))
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_nscaching_step: a filter count < 0, or > 0 without its arrays");
-    if (B < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_nscaching_step: B < 0");
-    if (B > ((1ll << 56) - 1) / h->cfg.eta) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_nscaching_step: eta*B >= 2^56");
+    NSCacheParams p;
+    memset(&p, 0, sizeof(p));
+    if (int rc = side_filters(q, "kge_nscaching_step", p)) return rc;
+    if (int rc = check_sampled_batch(h, B, "kge_nscaching_step")) return rc;
     if (B == 0) return KGE_OK;
     if (!ent_dev || !rel_dev || !triples_dev || !key_rows_dev || !update_dev || !neg_ent_dev || !neg_keep_subj_dev)
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_nscaching_step: null table, triples, key rows, flags or output pointer");
     if (int rc = check_no_pending(h, "kge_nscaching_step")) return rc;
-    if (h->stash)
-        return fail(KGE_ERR_UNSUPPORTED, "kge_nscaching_step: a row stash is set (row-sharded tables): NSCaching reads one "
-                                         "whole entity table");
+    if (int rc = check_no_stash(h, "kge_nscaching_step")) return rc;
     const size_t smem = nscaching_smem_bytes(h->L.ld, q->cache_size, q->random_size);
     if ((long long)smem > h->max_smem)
         return fail(KGE_ERR_UNSUPPORTED, "kge_nscaching_step: rows of %d floats and %d candidates exceed the shared memory "
                                          "of the refresh kernel (%d B)", h->L.ld, q->cache_size + q->random_size, h->max_smem);
     cudaStream_t st = (cudaStream_t)stream;
     if (int rc = refresh_rotation(h, rel_dev, st)) return rc;
-    NSCacheParams p;
-    memset(&p, 0, sizeof(p));
     p.ent = ent_dev;
-    p.rel = h->cfg.scoring == KGE_ROTATE ? h->rot : rel_dev;  // the table refresh_rotation has just written
+    p.rel = relation_rows(h, rel_dev);
     p.triples = triples_dev;
     p.key_rows = key_rows_dev;
     p.update = update_dev;
@@ -577,12 +657,6 @@ extern "C" int kge_nscaching_step(kge_handle *h, const kge_nscaching *cache, con
     p.count[0] = q->sub_count_dev;
     p.ids[1] = q->obj_ids_dev;
     p.count[1] = q->obj_count_dev;
-    p.filt_n[0] = q->sub_filter_n;
-    p.filt_keys[0] = reinterpret_cast<const long long *>(q->sub_filter_keys_dev);
-    p.filt_vals[0] = q->sub_filter_vals_dev;
-    p.filt_n[1] = q->obj_filter_n;
-    p.filt_keys[1] = reinterpret_cast<const long long *>(q->obj_filter_keys_dev);
-    p.filt_vals[1] = q->obj_filter_vals_dev;
     p.neg_ent = neg_ent_dev;
     p.neg_keep = neg_keep_subj_dev;
     p.misses = reinterpret_cast<unsigned long long *>(misses_dev);
@@ -608,8 +682,6 @@ extern "C" int64_t kge_shared_negatives_workspace_bytes(const kge_handle *h, int
     return (int64_t)c.at;
 }
 
-static bool dropout_set(const kge_handle *h);
-
 // Shared negatives: the score, loss and gradient passes of kge_train_shared.cu
 extern "C" int kge_shared_negatives_step(kge_handle *h, int64_t chunk, const float *ent_dev, const float *rel_dev,
                                          float *grad_ent_dev, float *grad_rel_dev, const int32_t *triples_dev, int64_t B,
@@ -618,23 +690,17 @@ extern "C" int kge_shared_negatives_step(kge_handle *h, int64_t chunk, const flo
 {
     KGE_CHECK_HANDLE(h, "kge_shared_negatives_step");
     if (chunk < 1) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_shared_negatives_step: chunk must be >= 1, got %lld", (long long)chunk);
-    if (B < 0) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_shared_negatives_step: B < 0");
-    if (B > ((1ll << 56) - 1) / h->cfg.eta) return fail(KGE_ERR_INVALID_ARGUMENT, "kge_shared_negatives_step: eta*B >= 2^56");
+    if (int rc = check_sampled_batch(h, B, "kge_shared_negatives_step")) return rc;
     const kge_negative_sampler *s = sampler;
-    if (s && (s->struct_size != (int32_t)sizeof(kge_negative_sampler) || s->max_attempts < 1 || s->max_attempts > 256))
-        return fail(KGE_ERR_INVALID_ARGUMENT, "kge_shared_negatives_step: bad kge_negative_sampler (ABI mismatch or "
-                                              "max_attempts outside 1..256)");
+    if (s)
+        if (int rc = check_sampler(s, "kge_shared_negatives_step")) return rc;
     if (int rc = check_no_pending(h, "kge_shared_negatives_step")) return rc;
     if (s && (s->sub_pool_off_dev || s->sub_pool_ids_dev || s->obj_pool_off_dev || s->obj_pool_ids_dev ||
               s->sub_filter_n != 0 || s->obj_filter_n != 0))
         return fail(KGE_ERR_UNSUPPORTED, "kge_shared_negatives_step: a sampler with pools or a filter picks entities per "
                                          "positive, and shared negatives draw one candidate set per chunk");
-    if (h->stash)
-        return fail(KGE_ERR_UNSUPPORTED, "kge_shared_negatives_step: a row stash is set (row-sharded tables): shared "
-                                         "negatives read one whole entity table");
-    if (dropout_set(h))
-        return fail(KGE_ERR_UNSUPPORTED, "kge_shared_negatives_step: embedding dropout is set (kge_set_embedding_dropout), "
-                                         "and the sampled training kernels do not apply it");
+    if (int rc = check_no_stash(h, "kge_shared_negatives_step")) return rc;
+    if (int rc = check_no_dropout(h, "kge_shared_negatives_step")) return rc;
     if (B == 0) return KGE_OK;
     if (!ent_dev || !rel_dev || !grad_ent_dev || !grad_rel_dev || !triples_dev || !workspace_dev)
         return fail(KGE_ERR_INVALID_ARGUMENT, "kge_shared_negatives_step: null table, gradient, triples or workspace pointer");
@@ -649,32 +715,7 @@ extern "C" int kge_shared_negatives_step(kge_handle *h, int64_t chunk, const flo
     if (int rc = refresh_rotation(h, rel_dev, st)) return rc;
     SharedNegParams q;
     memset(&q, 0, sizeof(q));
-    TrainParams &p = q.t;
-    p.ent = ent_dev;
-    p.rel = h->cfg.scoring == KGE_ROTATE ? h->rot : rel_dev;  // the table refresh_rotation has just written
-    p.grad_ent = grad_ent_dev;
-    p.grad_rel = grad_rel_dev;
-    p.triples = triples_dev;
-    p.B = B;
-    p.seed = seed;
-    p.step = step;
-    p.n_ent = (unsigned)h->cfg.n_ent;
-    p.model = h->cfg.scoring;
-    p.eta = h->cfg.eta;
-    p.kp = h->L.kp;
-    p.ld = h->L.ld;
-    p.nch = h->L.kp / 4;
-    p.loss = h->cfg.loss;
-    p.reduction = h->cfg.reduction;
-    p.mode = KGE_STEP_FUSED;
-    p.margin = h->cfg.margin;
-    p.alpha = h->cfg.alpha;
-    p.score_scale = h->score_scale;
-    p.inv_div = 1.f / h->rot_div;
-    p.loss_out = loss_dev;
-    p.stamp = kge_step_stamp(step);
-    p.stamp_ent = h->stamp_ent;
-    p.stamp_rel = h->stamp_ent ? h->stamp_rel : nullptr;
+    q.t = sampled_train_params(h, ent_dev, rel_dev, grad_ent_dev, grad_rel_dev, triples_dev, B, seed, step, loss_dev);
     q.chunk = chunk;
     q.thr = s ? s->thresholds_dev : nullptr;
     Carve c(workspace_dev);
@@ -682,17 +723,6 @@ extern "C" int kge_shared_negatives_step(kge_handle *h, int64_t chunk, const flo
     shared_negatives_grid(B, chunk, h->cfg.eta, &q);
     KGE_CUDA(launch_shared_negatives(q, h->sm_count, st), "kge_shared_negatives_step");
     return KGE_OK;
-}
-
-static bool dropout_set(const kge_handle *h) { return h->drop_p_ent != 0.f || h->drop_p_rel != 0.f; }
-
-// The sampled steps' fused kernels read the raw rows: they refuse while embedding dropout is set
-static int check_no_dropout(const kge_handle *h, const char *fn)
-{
-    if (!dropout_set(h)) return KGE_OK;
-    return fail(KGE_ERR_UNSUPPORTED, "%s: embedding dropout is set (kge_set_embedding_dropout), and the sampled training "
-                                     "kernels do not apply it: it applies to kge_one_vs_all_step, "
-                                     "kge_one_vs_all_relation_step and kge_k_vs_all_step; clear it with (0, 0)", fn);
 }
 
 static int train_step_impl(kge_handle *h, int32_t mode, const kge_shard_map *map, const float *ent_dev,
@@ -726,45 +756,21 @@ static int train_step_impl(kge_handle *h, int32_t mode, const kge_shard_map *map
     cudaStream_t st = (cudaStream_t)stream;
     if (int rc = refresh_rotation(h, rel_dev, st)) return rc;
 
-    TrainParams p;
-    memset(&p, 0, sizeof(p));
-    p.ent = ent_dev;
-    p.rel = h->cfg.scoring == KGE_ROTATE ? h->rot : rel_dev;
-    p.grad_ent = grad_ent_dev;
-    p.grad_rel = grad_rel_dev;
-    p.triples = triples_dev;
-    p.B = B;
+    TrainParams p = sampled_train_params(h, ent_dev, rel_dev, grad_ent_dev, grad_rel_dev, triples_dev, B, seed, step,
+                                         loss_dev);
+    p.mode = mode;
     p.neg_ent = neg_ent_dev;
     p.neg_keep = neg_keep_subj_dev;
-    p.seed = seed;
-    p.step = step;
-    p.n_ent = (unsigned)h->cfg.n_ent;
-    p.model = h->cfg.scoring;
-    p.eta = h->cfg.eta;
-    p.kp = h->L.kp;
-    p.ld = h->L.ld;
-    p.nch = h->L.kp / 4;
+    p.scores_pos = scores_pos_dev;
+    p.scores_neg = scores_neg_dev;
+    p.dpos = dpos_dev;
+    p.dneg = dneg_dev;
     p.nbuf = h->nbuf;
     p.wk = h->wk;
     p.n_cb = h->n_cb;
     p.slot_floats = h->slot_floats;
     p.resident = h->resident;
     p.eta_pad = h->eta_pad;
-    p.loss = h->cfg.loss;
-    p.reduction = h->cfg.reduction;
-    p.mode = mode;
-    p.margin = h->cfg.margin;
-    p.alpha = h->cfg.alpha;
-    p.score_scale = h->score_scale;
-    p.inv_div = 1.f / h->rot_div;
-    p.loss_out = loss_dev;
-    p.scores_pos = scores_pos_dev;
-    p.scores_neg = scores_neg_dev;
-    p.dpos = dpos_dev;
-    p.dneg = dneg_dev;
-    p.stamp = (int)(step & 0x3fffffffu) + 1;
-    p.stamp_ent = h->stamp_ent;
-    p.stamp_rel = h->stamp_rel;
     p.hot_ent[0] = h->hot_ent[0];
     p.hot_ent[1] = h->hot_ent[1];
     p.stash = row_stash(h, B);
@@ -1238,12 +1244,6 @@ static int check_side_candidates(const kge_handle *h, const char *fn, int32_t si
 {
     if (side == KGE_SIDE_P) return check_candidates(fn, cand_ids, cand_begin, n_cand, h->cfg.n_rel, "n_rel");
     return check_candidates(fn, cand_ids, cand_begin, n_cand, h->cfg.n_ent, "n_ent");
-}
-
-// The relation-side candidate rows: the relation table, or for RotatE the rotation table prepare_queries refreshed
-static const float *relation_rows(const kge_handle *h, const float *rel_dev)
-{
-    return h->cfg.scoring == KGE_ROTATE ? h->rot : rel_dev;
 }
 
 // The query side of a ranking call: refresh the rotation table (RotatE), prepare the b triples' query vectors and

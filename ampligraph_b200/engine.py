@@ -222,6 +222,21 @@ def graph_counts(triples, n_nodes, device=None):
     return {"degree": degree, "d": d, "tri2": tri2, "sq": sq, "pot": pot}
 
 
+def _set_side_filters(q, filt, up):
+    """Upload a sampler's known-pair filter {"s": (keys, vals), "o": ...} (datasets.FilterIndex) with `up` and point the
+    sub_filter_* / obj_filter_* fields of the ctypes struct q at it; an absent or empty side stays NULL / 0.  -> the
+    uploaded tensors, which must live as long as q is used."""
+    keep = []
+    for side, name in (("s", "sub"), ("o", "obj")):
+        if filt and side in filt and len(filt[side][0]):
+            keys, vals = (up(a) for a in filt[side])
+            keep += [keys, vals]
+            setattr(q, name + "_filter_n", keys.numel())
+            setattr(q, name + "_filter_keys", keys.data_ptr())
+            setattr(q, name + "_filter_vals", vals.data_ptr())
+    return keep
+
+
 class NegativeSamplerTables:
     """The device copy of a fit's negative-sampler tables (datasets.negative_sampler_tables) and the
     kge_negative_sampler that points at them; the tensors live as long as this object."""
@@ -246,13 +261,7 @@ class NegativeSamplerTables:
                 if ids_ptr is not None:  # no ids at all: every row is empty, i.e. no pool
                     setattr(q, name + "_pool_off", ptr(off))
                     setattr(q, name + "_pool_ids", ids_ptr)
-        filt = tables.get("filter") or {}
-        for side, name in (("s", "sub"), ("o", "obj")):
-            if side in filt:
-                keys, vals = filt[side]
-                setattr(q, name + "_filter_n", len(keys))
-                setattr(q, name + "_filter_keys", ptr(keys))
-                setattr(q, name + "_filter_vals", ptr(vals))
+        self._keep += _set_side_filters(q, tables.get("filter"), up)
         self.struct = q
 
 
@@ -270,19 +279,11 @@ class NSCache:
         self.ids = [torch.zeros((max(n, 1), n1), dtype=torch.int32, device=device) for n in self.n_keys]
         self.count = [torch.zeros(max(n, 1), dtype=torch.int32, device=device) for n in self.n_keys]
         q = _lib.KgeNSCaching(C.sizeof(_lib.KgeNSCaching), n1, n2)
-        self._keep = []
         for side, name in ((0, "sub"), (1, "obj")):
             setattr(q, name + "_n_keys", max(self.n_keys[side], 1))
             setattr(q, name + "_ids", self.ids[side].data_ptr())
             setattr(q, name + "_count", self.count[side].data_ptr())
-        filt = tables.get("filter") or {}
-        for side, name in (("s", "sub"), ("o", "obj")):
-            if side in filt and len(filt[side][0]):
-                keys, vals = (up(a) for a in filt[side])
-                self._keep += [keys, vals]
-                setattr(q, name + "_filter_n", keys.numel())
-                setattr(q, name + "_filter_keys", keys.data_ptr())
-                setattr(q, name + "_filter_vals", vals.data_ptr())
+        self._keep = _set_side_filters(q, tables.get("filter"), up)
         self.struct = q
 
     def batch(self, start, size):
@@ -836,11 +837,7 @@ class KGEEngine:
         to a device counter (read_negative_misses); nothing synchronises."""
         assert triples.dtype == torch.int32 and triples.is_cuda and triples.is_contiguous()
         n = triples.shape[0] * self.eta
-        if getattr(self, "_neg_ent", None) is None or self._neg_ent.numel() < n:
-            self._neg_ent = torch.empty(max(n, 1), dtype=torch.int32, device=self.device)
-            self._neg_keep = torch.empty(max(n, 1), dtype=torch.uint8, device=self.device)
-        if getattr(self, "_neg_misses", None) is None:
-            self._neg_misses = torch.zeros(1, dtype=torch.int64, device=self.device)
+        self._negative_buffers(n)
         _lib.check(self.lib.kge_sample_negatives(self.h, C.byref(tables.struct), _ptr(triples), triples.shape[0], int(seed),
                                                  int(step), _ptr(self._neg_ent), _ptr(self._neg_keep),
                                                  _ptr(self._neg_misses), self._stream()))

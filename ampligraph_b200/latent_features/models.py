@@ -490,17 +490,12 @@ class ScoringBasedEmbeddingModel:
                     eng.apply_gradients()
                 elif self.use_focusE:
                     self._two_phase_step(batch, weights[start:start + batch_size], sampler, start)
-                elif world > 1:  # this rank's slice of the global batch; the step is the global-batch step
-                    from ..parallel import row_shard
-                    lo, hi = row_shard(batch.shape[0], world, rank)
-                    self._dp.train_step(batch[lo:hi], None, seed=self.seed + 7919 * rank, step=self._step)
-                elif user_loss:
-                    self._user_loss_step(batch, sampler, start)
                 else:
-                    negatives = self._sampled_negatives(batch, sampler, start)
-                    eng.forward_backward(batch, negatives, seed=self.seed, step=self._step, defer=True)
-                    self._per_occurrence_backward(batch)
-                    eng.apply_gradients()
+                    if world > 1:  # this rank's slice of the global batch; the step is the global-batch step
+                        from ..parallel import row_shard
+                        lo, hi = row_shard(batch.shape[0], world, rank)
+                        batch = batch[lo:hi]
+                    self._sampled_step(batch, sampler, start)
                 self._step += 1
                 self._loss_cnt += 1
             # per-batch losses accumulate on the device; one read-back per epoch (the logged value is
@@ -667,6 +662,20 @@ class ScoringBasedEmbeddingModel:
             return self.engine.nscaching_negatives(batch, key_rows, update, sampler, self.seed, self._step)
         return self.engine.sample_negatives(batch, sampler, self.seed, self._step)
 
+    def _sampled_step(self, batch, sampler=None, start=0):
+        """One sampled training step on the device batch `batch`: on several GPUs this rank's share of the global-batch
+        step (DataParallelTrainer), else the user loss's two-phase step, else the fused step, the per-occurrence
+        regularisers and the optimizer.  sampler and start as in _sampled_negatives (None: the uniform draw)."""
+        if self._world() > 1:
+            self._dp.train_step(batch, None, seed=self.seed + 7919 * self._rank(), step=self._step)
+        elif isinstance(self.compiled_loss, loss_functions.LossFunctionWrapper):
+            self._user_loss_step(batch, sampler, start)
+        else:
+            negatives = self._sampled_negatives(batch, sampler, start)
+            self.engine.forward_backward(batch, negatives, seed=self.seed, step=self._step, defer=True)
+            self._per_occurrence_backward(batch)
+            self.engine.apply_gradients()
+
     def _check_all_candidates(self, training, loss, focusE):
         """The refusals fit's all-candidate training types share: `training` ('1vsAll' or 'KvsAll') needs a trilinear
         model, the compiled loss `loss`, no focusE and one GPU."""
@@ -739,15 +748,8 @@ class ScoringBasedEmbeddingModel:
                 self.max_ent_size = self.data_indexer.get_entities_count()
                 self.max_rel_size = self.data_indexer.get_relations_count()
             self._build_engine()
-        batch = host.to(self.engine.device, non_blocking=True)
-        if self._world() > 1:  # this rank's share of the global batch; gradients are exchanged inside the step
-            self._dp.train_step(batch, None, seed=self.seed + 7919 * self._rank(), step=self._step)
-        elif isinstance(self.compiled_loss, loss_functions.LossFunctionWrapper):
-            self._user_loss_step(batch)
-        else:
-            self.engine.forward_backward(batch, None, seed=self.seed, step=self._step, defer=True)
-            self._per_occurrence_backward(batch)
-            self.engine.apply_gradients()
+        # on several GPUs x is this rank's share of the global batch; gradients are exchanged inside the step
+        self._sampled_step(host.to(self.engine.device, non_blocking=True))
         self._step += 1
         if self._world() > 1:
             self._dp.reduce_loss_()  # the loss of the GLOBAL batch, identical on every rank
@@ -782,7 +784,6 @@ class ScoringBasedEmbeddingModel:
             eng.set_hot_entities(triples=self.hot_entities_from)   # [N,3] array may be attached for the hot-entity hint of fit()
             self.hot_entities_from = None
         dev = eng.device
-        user_loss = isinstance(self.compiled_loss, loss_functions.LossFunctionWrapper)
         depth = max(2, int(prefetch))
         cap = first.shape[0]
         main = torch.cuda.current_stream(dev)
@@ -826,15 +827,7 @@ class ScoringBasedEmbeddingModel:
                 queued.append(stage(i + 1, as_host(nxt)))  # overlaps step i
             s, n = queued.pop(0)
             main.wait_event(P["ready"][s])
-            batch = P["dev"][s][:n]
-            if self._world() > 1:
-                self._dp.train_step(batch, None, seed=self.seed + 7919 * self._rank(), step=self._step)
-            elif user_loss:
-                self._user_loss_step(batch)
-            else:
-                eng.forward_backward(batch, None, seed=self.seed, step=self._step, defer=True)
-                self._per_occurrence_backward(batch)
-                eng.apply_gradients()
+            self._sampled_step(P["dev"][s][:n])
             P["free"][s].record(main)
             P["loss_pin"][s].copy_(eng.loss_acc, non_blocking=True)  # D2H of this step's (cumulative) loss record
             P["loss_ev"][s].record(main)
